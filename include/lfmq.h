@@ -1,4 +1,4 @@
-/* lfmq.h -- C ABI of the B200-native training / inference step for the lfm_quant recurrent
+/* lfmq.h -- C ABI of the GPU-native (H100, sm_90a) training / inference step for the lfm_quant recurrent
  * forecaster (RNNPointEstimate, LSTM cell, forecast_steps = 1).
  *
  * The reference (lakshaykc/lfm_quant) defines no FFI: its seam is the Python protocol between the
@@ -29,11 +29,11 @@ extern "C" {
 enum { LFMQ_OK = 0, LFMQ_ERR_ARG = 1, LFMQ_ERR_CUDA = 2, LFMQ_ERR_UNSUPPORTED = 3, LFMQ_ERR_WORKSPACE = 4 };
 enum { LFMQ_OPT_ADADELTA = 0, LFMQ_OPT_ADAM = 1, LFMQ_OPT_RMSPROP = 2, LFMQ_OPT_SGD = 3 };
 /* LFMQ_PREC_FP32:   fp32 SIMT arithmetic everywhere (the parity mode, <=1e-4 rel vs the oracle; any cell / head).
- * LFMQ_PREC_BF16:   gate GEMMs on tcgen05 tensor cores with bf16 operands, fp32 accumulate, fp32 cell state.  LSTM cell,
+ * LFMQ_PREC_BF16:   gate GEMMs on wgmma tensor cores with bf16 operands, fp32 accumulate, fp32 cell state.  LSTM cell,
  *                   point-estimate head, num_hidden a multiple of 64 (<= 1024), any num_layers, dropout and recurrent
  *                   dropout; H = 256 / L = 1 without recurrent dropout runs the persistent cluster kernels.
  * LFMQ_PREC_BF16X3: fp32-tolerance forward on tensor cores (forward_only handles: predict.py:129): every operand split
- *                   into bf16 high + low halves, three tcgen05 products per GEMM (hi*hi + lo*hi + hi*lo), accurate
+ *                   into bf16 high + low halves, three wgmma products per GEMM (hi*hi + lo*hi + hi*lo), accurate
  *                   expf / tanhf gate nonlinearities, fp32 head -- <=1e-4 rel vs the oracle. */
 enum { LFMQ_PREC_FP32 = 0, LFMQ_PREC_BF16 = 1, LFMQ_PREC_BF16X3 = 2 };
 
@@ -132,9 +132,7 @@ int32_t lfmq_mask_count(lfmq_handle h, const float* y, int32_t B, float* out_dev
 /* First half of Train._train_step_point (train.py:181-192): forward, loss, BPTT.  Fills the flat
  * gradient buffer (+ its 4-float tail).  denom_dev = device {B_global, mask_count_global} or NULL to use
  * this call's own batch.  With N ranks the host all-reduces grads[0 : n_trainable+2] (SUM) next.
- * Stream semantics: everything is ordered on `stream`.  A LFMQ_PREC_BF16 handle additionally runs one prefetch-only
- * helper kernel on a library-owned non-blocking stream, forked from and joined back into `stream` with events inside
- * this call (it touches no caller-visible data; environment LFMQ_BWD_PREFETCH=0 disables it). */
+ * Stream semantics: everything is ordered on `stream`. */
 int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, int64_t row0, int64_t step,
                       const float* denom_dev, void* stream);
 

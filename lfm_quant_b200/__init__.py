@@ -1,4 +1,4 @@
-"""lfm_quant_b200: B200-native training / inference step for the lfm_quant recurrent forecaster.
+"""lfm_quant_b200: GPU-native (H100, sm_90a) training / inference step for the lfm_quant recurrent forecaster.
 
 Only what the hot path needs lives here: ``csrc/`` (CUDA kernels + the C-ABI of include/lfmq.h),
 ``_native`` (ctypes binding), ``engine`` (device-memory owner) and ``scripts/`` (the host-side mirror of

@@ -1,4 +1,4 @@
-// Shared helpers for the lfmq CUDA library (sm_100a only).
+// Shared helpers for the lfmq CUDA library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -20,6 +20,18 @@ extern long long g_launches;
       return 2; /* LFMQ_ERR_CUDA */                                                        \
     }                                                                                      \
   } while (0)
+
+// SMs of the current device (grid sizes of the one-wave kernels and of the per-SM partial buffers).
+inline int device_sm_count() {
+  static const int count = [] {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        n < 1)
+      n = 132;
+    return n;
+  }();
+  return count;
+}
 
 // Programmatic dependent launch.  Device side: every kernel launched through launch_pdl() calls pdl_sync() before it
 // touches anything its predecessors wrote -- wait for the previous kernel of the stream, THEN let the next one's CTAs be

@@ -1,5 +1,5 @@
 // fp32 SIMT kernels: the parity path (LFMQ_PREC_FP32) and every HBM-bound piece of the step
-// (batcher gather, BN/dropout, head + loss, clip + optimizer + MaxNorm).  sm_100a.
+// (batcher gather, BN/dropout, head + loss, clip + optimizer + MaxNorm).  sm_90a.
 //
 // Reference call sites are cited per kernel (paths relative to /root/reference/scripts).
 #include "kernels.h"
@@ -978,7 +978,7 @@ __global__ void __launch_bounds__(256) sumsq_norm_kernel(long n, const float* __
 int grad_norm_scale(cudaStream_t s, long n, const float* g, float clip, float* scalars, float* scratch,
                     unsigned int* ticket) {
   double* partial = reinterpret_cast<double*>(scratch);
-  const int nblk = (int)min((long)148, max((long)1, n / 2048));
+  const int nblk = (int)min((long)device_sm_count(), max((long)1, n / 2048));
   if (int rc = launch_pdl(sumsq_norm_kernel, dim3(nblk), dim3(256), 0, s, 1, n, g, partial, clip, scalars, ticket)) return rc;
   return 0;
 }
@@ -1029,7 +1029,7 @@ int opt_update(cudaStream_t s, int opt, long n, float* p, const float* g, float*
 }
 
 // keras.constraints.MaxNorm(max_value, axis=0) on W[I,N]: one warp per column (lanes stride the rows; a thread per
-// column left 2048 threads walking 512 dependent rows each: 115 us at H=512, profiles/r02_summary.md).
+// column left 2048 threads walking 512 dependent rows each).
 __global__ void maxnorm_cols_kernel(int I, int N, float* __restrict__ W, float max_norm) {
   pdl_sync();
   const int n = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;

@@ -1,30 +1,26 @@
-// LFMQ_PREC_BF16: the gate GEMMs on tcgen05 tensor cores (bf16 operands, fp32 accumulation in TMEM, fp32 cell
-// state in registers, bf16 when saved), everything else as fused HBM-streaming kernels.  sm_100a only.
+// LFMQ_PREC_BF16: the gate GEMMs on Hopper tensor cores (wgmma: bf16 operands from shared memory, fp32 accumulation
+// in the registers of the issuing warpgroup, fp32 cell state in registers, bf16 when saved), everything else as fused
+// HBM-streaming kernels.  sm_90a.
 //
 // Data layout in HBM (all carved from the caller's workspace, see tc_layout):
 //   xh    bf16 [maxB][T+1][384]   row (b,t): cols 0..255 = h_{t-1} (zero at t=0), 256..287 = x_t, 288 = 1.0 (t<T),
 //                                 rest 0.  One buffer serves: the A operand of the forward recurrence (K-major
 //                                 tiles via TMA), the head (h_t = row t+1) and the weight-gradient GEMM (MN-major).
-//   gates bf16 [T][tiles][8 blocks of 32 units][4 warps][8 pieces = gate*2+half][32 lanes][16]   post-activation
-//                                 i|f|g|o saved for BPTT.  Writer (forward) and reader (backward) both map one
-//                                 row to one thread, so the state is stored SoA at 32-byte granularity: a warp's
-//                                 256-bit access to `piece` covers 1 KB contiguously instead of 32 scattered sectors
+//   gates bf16 [T][tiles][8 blocks of 32 units][4 row quadrants][8 pieces = gate*2+half][32 rows][16]   post-activation
+//                                 i|f|g|o saved for BPTT, SoA at 32-byte granularity (row-major within a piece)
 //   cst   bf16 [T][tiles][8][4][2 pieces][32][16]   cell states (the recurrence itself keeps them in fp32 registers)
 //   dz    bf16 [maxB][T+1][4H]    gate pre-activation gradients (row T stays zero); columns in the order the
 //                                 backward kernel stages them as its A operand, [16-unit block][gate][16], so that a
 //                                 chunk goes out with one TMA store; only the weight-gradient GEMM reads it
 //   dpb   bf16 [T][tiles][128][32]  dLoss/dpred tiles (cols >= 16 zero): written by the tensor-core head as it stages
 //                                 them, expanded to dLoss/dh by the backward kernel's own MMAs (no dropout)
-//   dhout bf16 [T][tiles][4 ranks][4 warps][4 chunks][32 lanes][16]   dropout > 0 only: dLoss/dh from the SIMT head
-//                                 (after BN/dropout backward), already in the backward kernel's per-thread SoA order
+//   dhout bf16 [T][tiles][4 ranks][4 row quadrants][4 chunks][32 rows][16]   dropout > 0 only: dLoss/dh from the SIMT
+//                                 head (after BN/dropout backward)
 //
 // Forward recurrence = ONE persistent kernel (lstm_fwd_tc_kernel): clusters of 4 CTAs, one 128-row batch tile per
 // cluster, all clusters co-resident.  CTA r keeps the weight slice of hidden units [64r, 64r+64) (all four gates,
 // 256 gate columns) resident in shared memory for the whole unroll.  h_t is exchanged through global memory (it is
-// an output anyway) and comes back as the next step's A operand via TMA multicast -- measured on B200
-// (profiles/r01_tc_probe.txt) that path moves 64 KB into every SM of a cluster in ~1500 cycles while DSMEM stores
-// or bulk copies manage only 9-13 B/cycle/SM.  Clusters of 8 were tried first and dropped: only 15 of them are
-// co-resident.  See DESIGN.md section 5 for the per-step cycle budget of both recurrences.
+// an output anyway) and comes back as the next step's A operand via TMA multicast.  See DESIGN.md section 5.
 #include "lstm_tc.h"
 
 #include <cuda.h>
@@ -32,11 +28,11 @@
 #include <stdlib.h>
 
 #include "kernels.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace lfmq {
 
-using namespace sm100;
+using namespace sm90;
 
 namespace {
 
@@ -129,16 +125,12 @@ struct TcImpl {
   __nv_bfloat16* dpb;                          // [T][tiles][128][32] bf16 dLoss/dpred tiles (cols >= 16 zero)
   CUtensorMap tm_wos, tm_dpb;
   float* bop;
-  CUtensorMap tm_ubk, tm_px;                   // backward recurrence
+  CUtensorMap tm_ubk;                          // backward recurrence
   CUtensorMap tm_xh_mn, tm_dz_mn;              // weight gradient (MN-major)
   int max_clusters = 0, bwd_max_clusters = 0;
   bool bwd_ready = false;
-  // L2 prefetch helper for the backward recurrence (LFMQ_BWD_PREFETCH=1): runs on the SMs the recurrence leaves idle
-  cudaStream_t side = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  unsigned long long* progress = nullptr;      // device: steps completed by the backward kernel, counted across calls
-  unsigned long long epoch = 0;
   int head_ctas = 0, head_wctas = 0;
+  int n_sms = 0;
 };
 
 // =============================================================================================
@@ -203,30 +195,18 @@ __device__ __forceinline__ void pack_weights_body(int bid, int I, const float* _
 // Persistent forward recurrence
 // =============================================================================================
 struct FwdParams {
-  int B, T, n_iters, n_clusters, k16_x, n_tiles_cap;
+  int B, T, n_iters, n_clusters, n_tiles, k16_x, n_tiles_cap;
   __nv_bfloat16* xh;
   __nv_bfloat16* gates;   // null: do not save
   __nv_bfloat16* cst;     // null: do not save
   const float* biasp;
-  long long* trace;       // debug (LFMQ_TRACE_FWD=1): clock64 stamps of CTA 0, every third step
 };
 
-#define FWD_TRACE(role, t, pt)                                                        \
-  do {                                                                                \
-    if (p.trace && blockIdx.x == 0 && (t) % 3 == 0) p.trace[((role) * 16 + (t) / 3) * 8 + (pt)] = clock64(); \
-  } while (0)
-
-constexpr int FWD_EPI_WARPS = 8;                          // 4 TMEM lane quadrants x 2 column halves
-constexpr int FWD_THREADS = 32 * (2 + FWD_EPI_WARPS);     // producer + MMA + epilogue = 320
-#ifndef LFMQ_FWD_TMA_PUBLISH
-#define LFMQ_FWD_TMA_PUBLISH 0
-#endif
-// Publishing h_t: 0 = a 32-byte STG per thread and chunk followed by a release fence over all of them; 1 = the CTA's
-// [128 x 64] slice staged in shared memory (in the A-operand buffer, which no MMA reads any more once the step's last
-// chunk is committed) and sent as ONE TMA store whose completion is awaited before the peers are signalled.  Measured
-// (profiles/r02_time_c31_fwd_tma_publish.txt): the awaited TMA store takes ~2.5 K cycles under the kernel's own store
-// traffic (580 alone, profiles/r02_micro_tma_store_c30.txt): fwd 0.262 -> 0.315 ms, predict 3.67 -> 4.42 ms.  Off.
-constexpr bool TMA_PUBLISH = LFMQ_FWD_TMA_PUBLISH != 0;
+// Warps 0-7: two consumer warpgroups (rows 0-63 / 64-127 of the tile; each issues its own wgmma and runs the cell
+// update on its accumulator fragment); warpgroup 2: warp 8 = TMA producer.  setmaxnreg moves the registers of the
+// producer warpgroup to the consumers (128 accumulators + 32 cell states per thread).
+constexpr int FWD_THREADS = 3 * 128;
+constexpr int FWD_PRODUCER_WARP = 8;
 constexpr uint32_t SM_U = 0;                 // 4 k-blocks x [256 x 128 B]
 constexpr uint32_t SM_W = 131072;            // [256 x 64 B]
 constexpr uint32_t SM_H0 = 147456;           // 4 k-blocks x [128 x 128 B]
@@ -237,19 +217,27 @@ constexpr uint32_t FWD_SMEM = SM_BARS + 256 + 1024;   // + alignment slack
 
 struct FwdBars {
   uint64_t w_full, x_full, x_empty, h_full, h_written;
-  uint64_t acc_full[2][4];   // [accumulator buffer][16-unit chunk]
-  uint64_t acc_free;      // deferred saved-state stores have drained the staging TMEM buffer
-  uint64_t tma_issued;    // producer -> epilogue: the fetch of h for the next step has been issued
-  uint32_t tmem_base;
 };
+
+// Post-activation gates i|f|g|o of units jj, jj + 1 (row half h, pair q) from a 64-column chunk of the accumulator:
+// gate g of unit jj + e is fragment register 4 (2 g + q) + 2 h + e.  The sigmoid gates come pre-scaled by 1/2.
+__device__ __forceinline__ void fwd_gates(const float (&a)[32], const float* bs, int h, int q, int jj, float (&gv)[4][2]) {
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int ri = 2 * h + e;
+    gv[0][e] = fmaf(0.5f, tanh_approx(a[4 * (0 + q) + ri] + bs[jj + e]), 0.5f);
+    gv[1][e] = fmaf(0.5f, tanh_approx(a[4 * (2 + q) + ri] + bs[16 + jj + e]), 0.5f);
+    gv[2][e] = tanh_approx(a[4 * (4 + q) + ri] + bs[32 + jj + e]);
+    gv[3][e] = fmaf(0.5f, tanh_approx(a[4 * (6 + q) + ri] + bs[48 + jj + e]), 0.5f);
+  }
+}
 
 // SAVE: training (gates / cell states kept for BPTT).  A template parameter so that the predict kernel carries none of
 // the saved-state logic.
 template <bool SAVE>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
     lstm_fwd_tc_kernel(FwdParams p, const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_x,
-                       const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w,
-                       const __grid_constant__ CUtensorMap tm_hst) {
+                       const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   FwdBars* bars = reinterpret_cast<FwdBars*>(smem + SM_BARS);
@@ -261,30 +249,23 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
   if (tid == 0) {
     mbar_init(&bars->w_full, 1);
     mbar_init(&bars->x_full, 1);
-    mbar_init(&bars->x_empty, 1);
+    mbar_init(&bars->x_empty, 8);           // one arrive per consumer warp
     mbar_init(&bars->h_full, 1);
     mbar_init(&bars->h_written, TC_NC);
-    for (int i = 0; i < 2; ++i)
-      for (int c = 0; c < 4; ++c) mbar_init(&bars->acc_full[i][c], 1);
-    mbar_init(&bars->acc_free, 32 * FWD_EPI_WARPS);
-    mbar_init(&bars->tma_issued, 1);
     fence_mbar_init();
   }
   if (tid < TC_NSL) bias_s[tid] = p.biasp[rank * TC_NSL + tid];
-  if (warp == 1) tmem_alloc(&bars->tmem_base, 512);
-  tcgen05_fence_before();
   __syncthreads();
   cluster_sync_all();          // peers' barriers are initialised before anyone multicasts / arrives remotely
-  tcgen05_fence_after();
-  const uint32_t tmem = bars->tmem_base;
   const int T = p.T;
   // Programmatic dependent launch: everything above and the weight slice (packed two kernels ago) do not depend on the
   // preceding kernel (xh_fill_x); the 144 KB weight load overlaps its tail.
-  if (!(warp == 0 && lane == 0)) pdl_sync();
+  if (!(warp == FWD_PRODUCER_WARP && lane == 0)) pdl_sync();
 
-  if (warp == 0) {
+  if (warp >= FWD_PRODUCER_WARP) {
+    setmaxnreg_dec<40>();
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (warp == FWD_PRODUCER_WARP && lane == 0) {
       mbar_arrive_expect_tx(&bars->w_full, 131072 + 16384);
       for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + SM_U + kb * 32768, &tm_u, &bars->w_full, kb * 64, rank * TC_NSL);
       tma_load_2d(smem + SM_W, &tm_w, &bars->w_full, 0, rank * TC_NSL);
@@ -293,231 +274,151 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
       uint8_t* xbuf = smem + SM_X0;
       uint32_t n_hw = 0, n_xe = 0;
       for (int it = 0; it < p.n_iters; ++it) {
+        if (it * p.n_clusters + cid >= p.n_tiles) break;   // clusters without a tile in the last round
         const int b0 = (it * p.n_clusters + cid) * 128;
         for (int t = 0; t < T; ++t) {
           if (it > 0 || t > 0) mbar_wait(&bars->x_empty, (n_xe++) & 1);
-          FWD_TRACE(0, t, 0);
           mbar_arrive_expect_tx(&bars->x_full, 8192);
           tma_load_2d(xbuf, &tm_x, &bars->x_full, t * TC_XH_LD + TC_XOFF, b0);
           if (t >= 1) {
             mbar_wait_cluster(&bars->h_written, (n_hw++) & 1);   // all 4 slices of h_{t-1} are in global memory
-            FWD_TRACE(0, t, 1);
             fence_proxy_async_global();
             mbar_arrive_expect_tx(&bars->h_full, 65536);
             for (int kb = 0; kb < 4; ++kb)
               tma_load_2d_mcast(hbuf + kb * 16384 + rank * 4096, &tm_h, &bars->h_full, t * TC_XH_LD + kb * 64,
                                 b0 + 32 * (int)rank, 0xF);
-            FWD_TRACE(0, t, 2);
-            if (SAVE) mbar_arrive(&bars->tma_issued);
           }
         }
         mbar_wait_cluster(&bars->h_written, (n_hw++) & 1);       // phase of step T-1 (keeps parities aligned)
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(128, 64, false, false);      // one 16-unit chunk = 64 gate columns
-      mbar_wait(&bars->w_full, 0);
-      uint32_t n_xf = 0, n_hf = 0;
-      for (int it = 0; it < p.n_iters; ++it) {
-        for (int t = 0; t < T; ++t) {
-          const uint32_t g = (uint32_t)(it * T + t);
-          const uint32_t acc = tmem + (g & 1) * 256;
-          mbar_wait(&bars->x_full, (n_xf++) & 1);
-          // training: acc[g&1] doubled as the staging buffer of step g-1's saved gates / cell states
-          if (SAVE && g > 0) mbar_wait(&bars->acc_free, (g - 1) & 1);
-          FWD_TRACE(1, t, 0);
-          tcgen05_fence_after();
-          // x part of all four chunks first (it does not wait for h), then the h part chunk by chunk, each chunk
-          // committed on its own barrier: the epilogue of chunk c overlaps the MMAs of chunks c+1..
-          for (int c = 0; c < 4; ++c)
-            for (int k16 = 0; k16 < p.k16_x; ++k16) {
-              const uint64_t da = make_smem_desc(smem_u32(smem + SM_X0) + k16 * 32, 0, 512, LAYOUT_SW64);
-              const uint64_t db = make_smem_desc(smem_u32(smem + SM_W + c * 4096) + k16 * 32, 0, 512, LAYOUT_SW64);
-              umma_f16(acc + c * 64, da, db, idesc, k16 > 0);
-            }
-          umma_commit(&bars->x_empty);
-          if (t == 0) {
-            for (int c = 0; c < 4; ++c) umma_commit(&bars->acc_full[g & 1][c]);
-          } else {
-            mbar_wait(&bars->h_full, (n_hf++) & 1);
-            FWD_TRACE(1, t, 1);
-            tcgen05_fence_after();
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-#pragma unroll
-              for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-                for (int k16 = 0; k16 < 4; ++k16) {
-                  const uint64_t da = make_smem_desc(smem_u32(smem + SM_H0 + kb * 16384) + k16 * 32, 0, 1024, LAYOUT_SW128);
-                  const uint64_t db = make_smem_desc(smem_u32(smem + SM_U + kb * 32768 + c * 8192) + k16 * 32, 0, 1024,
-                                                     LAYOUT_SW128);
-                  umma_f16(acc + c * 64, da, db, idesc, 1);
-                }
-              umma_commit(&bars->acc_full[g & 1][c]);
-            }
-            FWD_TRACE(1, t, 2);
-          }
-        }
-      }
-    }
   } else {
-    // ===================== epilogue: gates, cell update, h exchange =====================
-    const int half = (warp - 2) / 4;        // this warp takes the 16-unit chunks half and half + 2 of the CTA's 64 units
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may touch
-    const int m = q * 32 + lane;            // row of the 128-row tile
-    const bool leader = (warp == 2) && lane == 0;
-    uint32_t n_ti = 0;                      // phases of tma_issued consumed (one per step that has a successor)
-    float cstate[32];
+    setmaxnreg_inc<232>();
+    // ===================== consumers: gate GEMMs, gates, cell update, h exchange =====================
+    // Accumulator of warpgroup wg: rows 64 wg .. 64 wg + 63, four 64-column chunks (one per 16 hidden units).  In chunk
+    // c the thread holds, for rows r0 and r0 + 8, the four gates of units jj = 8 p + 2 cq + e (p, e in {0, 1}):
+    // gate g of unit jj is fragment register 4 (2 g + p) + 2 h + e.  The cell state of those 2 x 16 values stays in
+    // fp32 registers for the whole unroll.
+    const int wg = warp >> 2, w = warp & 3, cq = lane & 3;
+    const int r0 = 64 * wg + 16 * w + (lane >> 2);
+    mbar_wait(&bars->w_full, 0);
+    uint32_t n_xf = 0, n_hf = 0;
+    float acc[4][32];
+    float cstate[4][2][2][2];               // [chunk][row half h][pair p][e]
     for (int it = 0; it < p.n_iters; ++it) {
       const int tile_c = it * p.n_clusters + cid;
-      const long b = (long)tile_c * 128 + m;
-      const bool valid = b < p.B;
+      if (tile_c >= p.n_tiles) break;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) cstate[j] = 0.f;
+      for (int c = 0; c < 4; ++c)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int q = 0; q < 2; ++q) cstate[c][h][q][0] = cstate[c][h][q][1] = 0.f;
       for (int t = 0; t < T; ++t) {
-        const uint32_t g = (uint32_t)(it * T + t);
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        const uint32_t taddr_other = tmem + lane_addr + ((g + 1) & 1) * 256 + half * 80;
-        // saved state, SoA at 32-byte granularity: [(t, tile, 32-unit block fr, quadrant)][piece = gate*2 + h16][lane],
-        // unit = 32 fr + 16 h16 + e.  Chunk c = half + 2 jb of this CTA is fr = 2 rank + jb, h16 = half.
-        const long wblk0 = (((long)t * p.n_tiles_cap + tile_c) * 8 + 2 * (int)rank) * 4 + q;      // jb = 0; jb = 1: + 4
-        __nv_bfloat16* grow = SAVE ? p.gates + (wblk0 * 8 * 32 + lane) * 16 + half * 512 : nullptr;   // + gate*1024 (+ jb*4*8*512)
-        __nv_bfloat16* crow = SAVE ? p.cst + (wblk0 * 2 * 32 + lane) * 16 + half * 512 : nullptr;     // (+ jb*4*2*512)
-        uint32_t phs[2][8];
+        // x part of all four chunks first (it does not wait for h), then the h part chunk by chunk, each chunk its own
+        // commit group: the cell update of chunk c overlaps the MMAs of chunks c+1..
+        mbar_wait(&bars->x_full, (n_xf++) & 1);
+        wgmma_fence();
 #pragma unroll
-        for (int jb = 0; jb < 2; ++jb) {
-          const int c = half + 2 * jb;            // 16-unit chunk of this CTA's 64 hidden units
-          mbar_wait(&bars->acc_full[g & 1][c], (g >> 1) & 1);
-          if (leader && jb == 0) FWD_TRACE(2, t, 0);
-          tcgen05_fence_after();
-          const uint32_t taddr = tmem + lane_addr + (g & 1) * 256 + c * 64;
-          __nv_bfloat16* hrow = p.xh + (b * (T + 1) + (t + 1)) * TC_XH_LD + rank * TC_HS + c * 16;
-          uint32_t vi[16], vf[16], vg[16], vo[16];
-          tmem_ld_32x32b_x16(taddr + 0, vi);
-          tmem_ld_32x32b_x16(taddr + 16, vf);
-          tmem_ld_32x32b_x16(taddr + 32, vg);
-          tmem_ld_32x32b_x16(taddr + 48, vo);
-          tmem_ld_wait();
-          uint32_t ph[8], pi[8], pf[8], pg[8], po[8];
-          float cn[16];
+        for (int c = 0; c < 4; ++c)
+          for (int k16 = 0; k16 < p.k16_x; ++k16) {
+            const uint64_t da = make_smem_desc(smem_u32(smem + SM_X0 + wg * 4096) + k16 * 32, 0, 512, LAYOUT_SW64);
+            const uint64_t db = make_smem_desc(smem_u32(smem + SM_W + c * 4096) + k16 * 32, 0, 512, LAYOUT_SW64);
+            wgmma_m64n64k16<0, 0>(acc[c], da, db, k16 > 0);
+          }
+        wgmma_commit();
+        if (t > 0) {
+          mbar_wait(&bars->h_full, (n_hf++) & 1);
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+#pragma unroll
+            for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+              for (int k16 = 0; k16 < 4; ++k16) {
+                const uint64_t da = make_smem_desc(smem_u32(smem + SM_H0 + kb * 16384 + wg * 8192) + k16 * 32, 0, 1024,
+                                                   LAYOUT_SW128);
+                const uint64_t db = make_smem_desc(smem_u32(smem + SM_U + kb * 32768 + c * 8192) + k16 * 32, 0, 1024,
+                                                   LAYOUT_SW128);
+                wgmma_m64n64k16<0, 0>(acc[c], da, db, 1);
+              }
+            wgmma_commit();
+          }
+          wgmma_wait<4>();
+        } else {
+          wgmma_wait<0>();
+        }
+        if (lane == 0) mbar_arrive(&bars->x_empty);      // the x tile has been read
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          if (t > 0) {
+            if (c == 0) wgmma_wait<3>();
+            if (c == 1) wgmma_wait<2>();
+            if (c == 2) wgmma_wait<1>();
+            if (c == 3) wgmma_wait<0>();
+          }
+          fence_regs(acc[c]);
           const float* bs = bias_s + c * 64;
 #pragma unroll
-          for (int jj = 0; jj < 16; jj += 2) {
-            float hv[2], iv[2], fv[2], gv[2], ov[2];
+          for (int h = 0; h < 2; ++h) {
+            const int m = r0 + 8 * h;               // row of the 128-row tile
+            const long b = (long)tile_c * 128 + m;
 #pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const int j = jb * 16 + jj + u;
-              const float gi = fmaf(0.5f, tanh_approx(__uint_as_float(vi[jj + u]) + bs[jj + u]), 0.5f);
-              const float gf = fmaf(0.5f, tanh_approx(__uint_as_float(vf[jj + u]) + bs[16 + jj + u]), 0.5f);
-              const float gg = tanh_approx(__uint_as_float(vg[jj + u]) + bs[32 + jj + u]);
-              const float go = fmaf(0.5f, tanh_approx(__uint_as_float(vo[jj + u]) + bs[48 + jj + u]), 0.5f);
-              const float cc = fmaf(gf, cstate[j], gi * gg);
-              cstate[j] = cc;
-              cn[jj + u] = cc;
-              hv[u] = go * tanh_approx(cc);
-              iv[u] = gi; fv[u] = gf; gv[u] = gg; ov[u] = go;
+            for (int q = 0; q < 2; ++q) {
+              const int jj = 8 * q + 2 * cq;          // first of the two units of this pair
+              float gv[4][2], hv[2];
+              fwd_gates(acc[c], bs, h, q, jj, gv);
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float cc = fmaf(gv[1][e], cstate[c][h][q][e], gv[0][e] * gv[2][e]);
+                cstate[c][h][q][e] = cc;
+                hv[e] = gv[3][e] * tanh_approx(cc);
+              }
+              if (b < p.B)
+                *reinterpret_cast<uint32_t*>(p.xh + (b * (T + 1) + (t + 1)) * TC_XH_LD + rank * TC_HS + c * 16 + jj) =
+                    pack_bf16x2(hv[0], hv[1]);
             }
-            ph[jj / 2] = pack_bf16x2(hv[0], hv[1]);
-            pi[jj / 2] = pack_bf16x2(iv[0], iv[1]);
-            pf[jj / 2] = pack_bf16x2(fv[0], fv[1]);
-            pg[jj / 2] = pack_bf16x2(gv[0], gv[1]);
-            po[jj / 2] = pack_bf16x2(ov[0], ov[1]);
-          }
-          if (TMA_PUBLISH) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) phs[jb][e] = ph[e];
-          } else if (valid) {
-            st_global_v8(hrow, ph);   // one full 32-byte sector per store (STG.256)
-          }
-          if (SAVE) {
-            // Saved gates / cell states are not needed by the h exchange: park them in the idle accumulator
-            // buffer (TMEM) and write them to HBM after the publish, off the per-step critical path.
-            const uint32_t tst = taddr_other + jb * 40;
-            uint32_t cu[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) cu[e] = pack_bf16x2(cn[2 * e], cn[2 * e + 1]);
-            tmem_st_32x32b_x8(tst, pi);
-            tmem_st_32x32b_x8(tst + 8, pf);
-            tmem_st_32x32b_x8(tst + 16, pg);
-            tmem_st_32x32b_x8(tst + 24, po);
-            tmem_st_32x32b_x8(tst + 32, cu);
           }
         }
-        if (TMA_PUBLISH) {
-          // all MMAs of the step are complete once chunk 3 is committed: the A-operand buffer is free to stage h_t in
-          // (the peers' multicast of h_t lands there only after every CTA, this one included, has signalled)
-          if (half == 0) mbar_wait(&bars->acc_full[g & 1][3], (g >> 1) & 1);
-          uint8_t* srow = smem + SM_H0 + m * 128;
-#pragma unroll
-          for (int jb = 0; jb < 2; ++jb) {
-            const int ch = (half + 2 * jb) * 2;            // 16-byte chunk of the 128-byte row, 128B-swizzled by row
-            *reinterpret_cast<uint4*>(srow + (((ch) ^ (m & 7)) << 4)) = make_uint4(phs[jb][0], phs[jb][1], phs[jb][2], phs[jb][3]);
-            *reinterpret_cast<uint4*>(srow + (((ch + 1) ^ (m & 7)) << 4)) = make_uint4(phs[jb][4], phs[jb][5], phs[jb][6], phs[jb][7]);
-          }
-          fence_proxy_async_smem();
-        }
-        if (SAVE) tmem_st_wait();
-        tcgen05_fence_before();
-        if (leader) FWD_TRACE(2, t, 1);
-        // Publish this CTA's h slice: CTA-level barrier over the 256 epilogue threads, then 4 lanes of the leader
-        // warp arrive (release.cluster, cumulative over the barrier) on the 4 CTAs' h_written barriers in parallel.
-        // Readers acquire at cluster scope and cross into the async proxy before their TMA loads.
-        named_bar_sync(1, 32 * FWD_EPI_WARPS);
-        if (leader) FWD_TRACE(2, t, 4);
-        if (TMA_PUBLISH && warp == 2) {
-          if (lane == 0) {
-            tma_store_2d(&tm_hst, smem + SM_H0, (t + 1) * TC_XH_LD + (int)rank * TC_HS, tile_c * 128);   // rows >= B clipped
-            bulk_commit_group();
-            bulk_wait_group0();                 // the slice is in global memory before anybody is told
-          }
-          __syncwarp();
-        }
-        if (warp == 2 && lane < TC_NC)
-          mbar_arrive_cluster(mapa_u32(smem_u32(&bars->h_written), (uint32_t)lane));
+        // Publish this CTA's h slice: barrier over the 256 consumer threads, then 4 lanes of warp 0 arrive
+        // (release.cluster, cumulative over the barrier) on the 4 CTAs' h_written barriers in parallel.  Readers acquire
+        // at cluster scope and cross into the async proxy before their TMA loads.  All MMAs of the step are complete
+        // here, so the h buffer may be overwritten by the multicast of the next step.
+        named_bar_sync(1, 256);
+        if (warp == 0 && lane < TC_NC) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->h_written), (uint32_t)lane));
         if (SAVE) {
-          // Saved state of this step, parked in the idle accumulator buffer.  All CTAs reach this point together, so
-          // writing the whole 80 KB per CTA at once is a ~3 K-cycle burst at full HBM write bandwidth: it outlasts the
-          // publish, and the producer's proxy fence + TMA issue for the next step then queue behind it (clock64 trace:
-          // 1.5 K cycles instead of 0.3 K without saved state).  So: first half now (over before the producer needs to
-          // fence), second half out of TMEM into registers -- the MMA may have the staging buffer back -- and to global
-          // only once the producer has issued the next step's h fetch.
-          tcgen05_fence_after();
-          uint32_t sg[32], sc[8];
-          tmem_ld_32x32b_x32(taddr_other, sg);
-          tmem_ld_32x32b_x8(taddr_other + 32, sc);
-          tmem_ld_wait();
-          if (valid) {      // chunk jb = 0 (32-unit block fr = 2 rank)
-            st_global_v8(grow + 0 * 1024, sg);
-            st_global_v8(grow + 1 * 1024, sg + 8);
-            st_global_v8(grow + 2 * 1024, sg + 16);
-            st_global_v8(grow + 3 * 1024, sg + 24);
-            st_global_v8(crow, sc);
-          }
-          tmem_ld_32x32b_x32(taddr_other + 40, sg);
-          tmem_ld_32x32b_x8(taddr_other + 40 + 32, sc);
-          tmem_ld_wait();
-          tcgen05_fence_before();
-          mbar_arrive(&bars->acc_free);
-          if (t < T - 1) mbar_wait(&bars->tma_issued, (n_ti++) & 1);
-          if (valid) {      // chunk jb = 1 (32-unit block fr = 2 rank + 1: 4 quadrant blocks further)
-            __nv_bfloat16* grow1 = grow + 4L * 8 * 512;
-            st_global_v8(grow1 + 0 * 1024, sg);
-            st_global_v8(grow1 + 1 * 1024, sg + 8);
-            st_global_v8(grow1 + 2 * 1024, sg + 16);
-            st_global_v8(grow1 + 3 * 1024, sg + 24);
-            st_global_v8(crow + 4L * 2 * 512, sc);
+          // Saved gates / cell states are not needed by the h exchange: they go out after the publish, so that the
+          // release above does not wait for them.  The gates are evaluated again from the accumulators (still intact
+          // until the next step's MMAs) -- cheaper than holding 80 packed values per thread across the publish.
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const float* bs = bias_s + c * 64;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int m = r0 + 8 * h;
+              if ((long)tile_c * 128 + m >= p.B) continue;
+              // saved state, SoA at 32-byte granularity: [(t, tile, 32-unit block fr, row quadrant)][piece = gate*2 +
+              // h16][row & 31][16], unit = 32 fr + 16 h16 + e; this chunk is fr = 2 rank + c / 2, h16 = c % 2
+              const long blk = (((long)t * p.n_tiles_cap + tile_c) * 8 + 2 * (int)rank + (c >> 1)) * 4 + (m >> 5);
+#pragma unroll
+              for (int q = 0; q < 2; ++q) {
+                const int jj = 8 * q + 2 * cq;
+                float gv[4][2];
+                fwd_gates(acc[c], bs, h, q, jj, gv);
+                __nv_bfloat16* gp = p.gates + (blk * 8 + (c & 1)) * 512 + (m & 31) * 16 + jj;
+#pragma unroll
+                for (int g = 0; g < 4; ++g)
+                  *reinterpret_cast<uint32_t*>(gp + g * 1024) = pack_bf16x2(gv[g][0], gv[g][1]);
+                *reinterpret_cast<uint32_t*>(p.cst + (blk * 2 + (c & 1)) * 512 + (m & 31) * 16 + jj) =
+                    pack_bf16x2(cstate[c][h][q][0], cstate[c][h][q][1]);
+              }
+            }
           }
         }
-        if (leader) FWD_TRACE(2, t, 5);
       }
     }
   }
   __syncwarp();
-  tcgen05_fence_before();
   cluster_sync_all();          // nobody leaves while peers may still multicast into / arrive on this CTA
-  if (warp == 1) tmem_dealloc(tmem, 512);
 }
 
 // =============================================================================================
@@ -541,16 +442,9 @@ struct HeadParams {
   __nv_bfloat16* dhout;
   float* dpred;         // [B*T][16] dLoss/dpred (training), consumed by head_wgrad_kernel
   float* partial;       // [gridDim.x][HEAD_PART]
-  long long* trace;     // debug (LFMQ_TRACE_HEAD=1): clock64 stamps of CTA 0, first 8 tiles
 };
 
-#define HEAD_TRACE(role, n, pt)                                                                       \
-  do {                                                                                                \
-    if (p.trace && blockIdx.x == 0 && (n) < 8) p.trace[((role) * 8 + (n)) * 8 + (pt)] = clock64();    \
-  } while (0)
-
 constexpr int HEAD_PART = 2 * TC_H + TC_OPAD + 16;   // dgamma | dbeta | dbo | s0 s1 s2 (per CTA of the fused pass)
-constexpr int HEAD_THREADS = 256;
 constexpr int HWG_PART = TC_H * TC_OPAD;              // dWo partial per CTA of the weight-gradient pass
 constexpr int HWG_ROWS = 32;                          // rows staged per tile
 
@@ -780,9 +674,9 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
 
 // Tensor-core head (dropout off): with y = a*h + b (BN inference affine) the Dense layer folds to
 //   pred = h * (diag(a) Wo) + (bo + b Wo)
-// a tcgen05 MMA on the TMA-staged h tile (K-major SW128, exactly the layout the recurrence uses): 16 x (M128 N16 K16).
+// a wgmma on the TMA-staged h tile (K-major SW128, exactly the layout the recurrence uses): 2 x 16 x (M64 N16 K16).
 // Threads own one row each for the loss terms and dpred, staged as a 128 x 32 bf16 tile (SW64).  Training: that tile
-// feeds h^T dpred (MN-major MMAs, accumulated in TMEM across tiles -> dWo, dgamma) and goes to HBM by TMA store for the
+// feeds h^T dpred (MN-major MMAs, accumulated in registers across tiles -> dWo, dgamma) and goes to HBM by TMA store for the
 // backward recurrence, which forms dLoss/dh = dpred (Wo a)^T on its own tensor cores; colsum(dpred) -> dbo, dbeta.
 struct HeadTcWeights {
   const __nv_bfloat16* WoTp;   // [16][256]  a_j * Wo[j][n]
@@ -859,15 +753,15 @@ __global__ void __launch_bounds__(256) pack_all_kernel(PackArgs a) {
 
 constexpr uint32_t HT_TILE = 0;            // 4 k-blocks x [128 x 128 B]
 constexpr uint32_t HT_WOT = 65536;         // 4 k-blocks x [16 x 128 B]
-// (73728 .. 90111: unused since dLoss/dh moved to the backward kernel; kept so the tile offsets stay 1024-aligned)
+constexpr uint32_t HT_PRED = 73728;        // [128][17] fp32: pred rows, fragment -> one row per thread
 constexpr uint32_t HT_DP = 90112;          // [128 x 64 B]
 constexpr uint32_t HT_BARS = 98304;
 constexpr int HT_SMEM = HT_BARS + 128 + 1024;
-constexpr int HT_THREADS = 160;            // warp 0: TMA + MMA issue, warps 1-4: one row per thread
+constexpr int HT_THREADS = 160;            // warps 0-3: MMA warpgroup, one row per thread; warp 4: TMA
+constexpr int HT_PRED_LD = 17;
 
 struct HtBars {
-  uint64_t wt_full, tile_full, pred_full, dp_full, dp_free, tile_free, w_done;
-  uint32_t tmem_base;
+  uint64_t wt_full, tile_full, tile_free;
 };
 
 template <bool TRAIN>
@@ -879,6 +773,7 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   HtBars* bars = reinterpret_cast<HtBars*>(smem + HT_BARS);
+  float* pred_s = reinterpret_cast<float*>(smem + HT_PRED);
   __shared__ __align__(16) float bn_s[3][TC_H];      // gamma*inv | mean | inv
   __shared__ float red_s[HEAD_PART];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -894,87 +789,29 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
   if (tid == 0) {
     mbar_init(&bars->wt_full, 1);
     mbar_init(&bars->tile_full, 1);
-    mbar_init(&bars->pred_full, 1);
-    mbar_init(&bars->dp_full, 128);
-    mbar_init(&bars->dp_free, 1);
-    mbar_init(&bars->tile_free, 128);
-    mbar_init(&bars->w_done, 1);
+    mbar_init(&bars->tile_free, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc(&bars->tmem_base, 256);
   fence_proxy_async_smem();
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = bars->tmem_base;
-  const uint32_t acc_p = tmem;             // 16 columns
-  const uint32_t acc_w = tmem + 160;       // 2 x 16 columns: sum over this CTA's tiles of h^T dpred (rows = hidden unit)
   const int n_tiles = p.T * n_btiles;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       mbar_arrive_expect_tx(&bars->wt_full, 8192);
       for (int kb = 0; kb < 4; ++kb) tma_load_2d(smem + HT_WOT + kb * 2048, &tm_wot, &bars->wt_full, kb * 64, 0);
-      mbar_wait(&bars->wt_full, 0);
-      const uint32_t idesc_p = make_idesc_bf16(128, 16, false, false);
       uint32_t n = 0;
       for (int ti = blockIdx.x; ti < n_tiles; ti += gridDim.x, ++n) {
         const int t = ti / n_btiles, bt = ti % n_btiles;
-        if (n > 0) mbar_wait(TRAIN ? &bars->dp_free : &bars->tile_free, (n - 1) & 1);
-        HEAD_TRACE(0, n, 0);
+        if (n > 0) mbar_wait(&bars->tile_free, (n - 1) & 1);
         mbar_arrive_expect_tx(&bars->tile_full, 65536);
         for (int kb = 0; kb < 4; ++kb)
           tma_load_2d(smem + HT_TILE + kb * 16384, &tm_h, &bars->tile_full, (t + 1) * TC_XH_LD + kb * 64, bt * 128);
-        mbar_wait(&bars->tile_full, n & 1);
-        HEAD_TRACE(0, n, 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            const uint64_t da = make_smem_desc(smem_u32(smem + HT_TILE + kb * 16384) + k16 * 32, 0, 1024, LAYOUT_SW128);
-            const uint64_t db = make_smem_desc(smem_u32(smem + HT_WOT + kb * 2048) + k16 * 32, 0, 1024, LAYOUT_SW128);
-            umma_f16(acc_p, da, db, idesc_p, (kb | k16) != 0);
-          }
-        umma_commit(&bars->pred_full);
-        if (TRAIN) {
-          mbar_wait(&bars->dp_full, n & 1);
-          HEAD_TRACE(0, n, 2);
-          tcgen05_fence_after();
-          // the staged dLoss/dpred tile also goes to HBM as it is (128 x 64 B, SW64): the backward recurrence adds
-          // dpred (Wo gamma inv)^T for its own hidden units on its tensor cores
-          tma_store_2d(&tm_dpb, smem + HT_DP, 0, (t * n_tiles_cap + bt) * 128);
-          bulk_commit_group();
-          // dWo' += h^T dpred: A = the h tile read MN-major (hidden unit = M), B = the dpred tile read MN-major,
-          // K = the 128 rows.
-          {
-            const uint32_t idesc_w = make_idesc_bf16(128, 16, true, true);
-#pragma unroll
-            for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-              for (int k16 = 0; k16 < 8; ++k16) {
-                const uint64_t wa = make_smem_desc(smem_u32(smem + HT_TILE + 2 * mb * 16384) + k16 * 2048, 16384, 1024,
-                                                   LAYOUT_SW128);
-                const uint64_t wb = make_smem_desc(smem_u32(smem + HT_DP) + k16 * 1024, 0, 512, LAYOUT_SW64);
-                umma_f16(acc_w + mb * 16, wa, wb, idesc_w, (n > 0 || k16 > 0) ? 1u : 0u);
-              }
-          }
-          bulk_wait_group_read0();          // the store has read the dpred tile
-          umma_commit(&bars->dp_free);      // ... and the h^T dpred MMAs are done with it and with the h tile
-          HEAD_TRACE(0, n, 3);
-        }
-      }
-      if (TRAIN) {
-        umma_commit(&bars->w_done);
-        bulk_wait_group0();
       }
     }
   } else {
-    const int m = tid - 32;                 // row of the tile
-    const int wq = warp & 3;                // TMEM lane quadrant of this warp
-    const int mrow = wq * 32 + lane;        // row this thread can reach in TMEM == row it owns
-    (void)m;
-    const uint32_t lane_addr = (uint32_t)(wq * 32) << 16;
+    const int mrow = tid;                   // row of the tile this thread owns
+    const int fw = warp, cq = lane & 3;     // accumulator fragment: rows 16 fw + lane / 4 (+ 8) of each 64-row half
     float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
     if (TRAIN) {
       const float Bg = p.denom[0], Mg = p.denom[1];
@@ -989,6 +826,13 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
     float accbo[TC_OPAD];
 #pragma unroll
     for (int k = 0; k < TC_OPAD; ++k) accbo[k] = 0.f;
+    // this CTA's sum over its tiles of h^T dpred: hidden units 64 mq .. 64 mq + 63 (M) x 16 outputs (N)
+    float accw[4][8];
+#pragma unroll
+    for (int mq = 0; mq < 4; ++mq)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) accw[mq][i] = 0.f;
+    mbar_wait(&bars->wt_full, 0);
     uint32_t n = 0;
     for (int ti = blockIdx.x; ti < n_tiles; ti += gridDim.x, ++n) {
       const int t = ti / n_btiles, bt = ti % n_btiles;
@@ -1003,15 +847,35 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
         for (int k = 0; k < TC_OPAD; ++k)
           if (k < p.O) yt[k] = p.y[r * p.O + k];
       }
-      mbar_wait(&bars->pred_full, n & 1);
-      if (tid == 32) HEAD_TRACE(1, n, 0);
-      tcgen05_fence_after();
-      uint32_t pv[16];
-      tmem_ld_32x32b_x16(acc_p + lane_addr, pv);
-      tmem_ld_wait();
+      mbar_wait(&bars->tile_full, n & 1);
+      // pred = h (diag(a) Wo): two m64 x n16 halves, K = 256
+      float ap[2][8];
+      wgmma_fence();
+#pragma unroll
+      for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+        for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+          for (int k16 = 0; k16 < 4; ++k16) {
+            const uint64_t da = make_smem_desc(smem_u32(smem + HT_TILE + kb * 16384 + mh * 8192) + k16 * 32, 0, 1024,
+                                               LAYOUT_SW128);
+            const uint64_t db = make_smem_desc(smem_u32(smem + HT_WOT + kb * 2048) + k16 * 32, 0, 1024, LAYOUT_SW128);
+            wgmma_m64n16k16<0, 0>(ap[mh], da, db, (kb | k16) != 0);
+          }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(ap[0]);
+      fence_regs(ap[1]);
+#pragma unroll
+      for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          pred_s[(64 * mh + 16 * fw + (lane >> 2) + 8 * ((i >> 1) & 1)) * HT_PRED_LD + 8 * (i >> 2) + 2 * cq + (i & 1)] =
+              ap[mh][i];
+      named_bar_sync(1, 128);
       float pr[TC_OPAD];
 #pragma unroll
-      for (int k = 0; k < TC_OPAD; ++k) pr[k] = __uint_as_float(pv[k]) + bop[k];
+      for (int k = 0; k < TC_OPAD; ++k) pr[k] = pred_s[mrow * HT_PRED_LD + k] + bop[k];
       if (p.preds && valid) {
 #pragma unroll
         for (int k = 0; k < TC_OPAD; ++k)
@@ -1047,8 +911,10 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
             for (int k4 = 0; k4 < TC_OPAD; k4 += 4)
               *reinterpret_cast<float4*>(p.dpred + r * TC_OPAD + k4) = make_float4(dp[k4], dp[k4 + 1], dp[k4 + 2], dp[k4 + 3]);
           }
-          // dpred row -> A operand tile [128 x 64 B], SWIZZLE_64B: chunk c of row m at m*64 + ((c ^ ((m>>1)&3)) << 4)
-          if (n > 0) mbar_wait(&bars->dp_free, (n - 1) & 1);     // MMAs and the TMA store are done with the previous tile
+          // the TMA store of the previous tile's dpred has read the staging tile (the MMAs that read it are complete)
+          if (n > 0 && tid == 0) bulk_wait_group_read0();
+          named_bar_sync(1, 128);
+          // dpred row -> [128 x 64 B] tile, SWIZZLE_64B: chunk c of row m at m*64 + ((c ^ ((m>>1)&3)) << 4)
           uint8_t* drow = smem + HT_DP + mrow * 64;
           const int s64 = (mrow >> 1) & 3;
           *reinterpret_cast<uint4*>(drow + ((0 ^ s64) << 4)) =
@@ -1056,14 +922,35 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
           *reinterpret_cast<uint4*>(drow + ((1 ^ s64) << 4)) =
               make_uint4(pack_bf16x2(dp[8], dp[9]), pack_bf16x2(dp[10], dp[11]), pack_bf16x2(dp[12], dp[13]), pack_bf16x2(dp[14], dp[15]));
           fence_proxy_async_smem();
-          mbar_arrive(&bars->dp_full);
-          if (tid == 32) HEAD_TRACE(1, n, 1);
+          named_bar_sync(1, 128);
+          // the staged dLoss/dpred tile also goes to HBM as it is (128 x 64 B, SW64): the backward recurrence adds
+          // dpred (Wo gamma inv)^T for its own hidden units on its tensor cores
+          if (tid == 0) {
+            tma_store_2d(&tm_dpb, smem + HT_DP, 0, (t * n_tiles_cap + bt) * 128);
+            bulk_commit_group();
+          }
+          // dWo' += h^T dpred: A = the h tile read MN-major (hidden unit = M), B = the dpred tile read MN-major,
+          // K = the 128 rows
+          wgmma_fence();
+#pragma unroll
+          for (int mq = 0; mq < 4; ++mq)
+#pragma unroll
+            for (int k16 = 0; k16 < 8; ++k16) {
+              const uint64_t wa = make_smem_desc(smem_u32(smem + HT_TILE + mq * 16384) + k16 * 2048, 16384, 1024,
+                                                 LAYOUT_SW128);
+              const uint64_t wb = make_smem_desc(smem_u32(smem + HT_DP) + k16 * 1024, 0, 512, LAYOUT_SW64);
+              wgmma_m64n16k16<1, 1>(accw[mq], wa, wb, 1);
+            }
+          wgmma_commit();
+          wgmma_wait<0>();
+#pragma unroll
+          for (int mq = 0; mq < 4; ++mq) fence_regs(accw[mq]);
           // nothing else per tile: dLoss/dh is formed by the backward recurrence from the dpred tile (lstm_bwd_tc_kernel
           // <FUSED>), dgamma / dbeta by head_fold_kernel from h^T dpred and colsum(dpred)
         }
       }
-      tcgen05_fence_before();
-      if (!TRAIN) mbar_arrive(&bars->tile_free);
+      named_bar_sync(1, 128);               // the tile and the pred rows have been read by everybody
+      if (tid == 0) mbar_arrive(&bars->tile_free);
     }
     if (p.y) {
       s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
@@ -1078,34 +965,21 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
       }
     }
     if (TRAIN) {
-      // this CTA's h^T dpred: TMEM lane = hidden unit (mod 128), 16 columns per 128-unit block
+      // this CTA's h^T dpred, [hidden unit][16]
       float* wp = wpartial + (long)blockIdx.x * HWG_PART;
-      if (n > 0) {
-        mbar_wait(&bars->w_done, 0);
-        tcgen05_fence_after();
 #pragma unroll
-        for (int mb = 0; mb < 2; ++mb) {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(acc_w + lane_addr + mb * 16, v);
-          tmem_ld_wait();
-          float* o = wp + (mb * 128 + mrow) * TC_OPAD;
+      for (int mq = 0; mq < 4; ++mq)
 #pragma unroll
-          for (int k4 = 0; k4 < 16; k4 += 4)
-            *reinterpret_cast<float4*>(o + k4) = make_float4(__uint_as_float(v[k4]), __uint_as_float(v[k4 + 1]),
-                                                             __uint_as_float(v[k4 + 2]), __uint_as_float(v[k4 + 3]));
+        for (int i = 0; i < 8; i += 2) {
+          const int j = 64 * mq + 16 * fw + (lane >> 2) + 8 * ((i >> 1) & 1);
+          *reinterpret_cast<float2*>(wp + j * TC_OPAD + 8 * (i >> 2) + 2 * cq) = make_float2(accw[mq][i], accw[mq][i + 1]);
         }
-      } else {
-        for (int mb = 0; mb < 2; ++mb)
-          for (int k = 0; k < TC_OPAD; ++k) wp[(mb * 128 + mrow) * TC_OPAD + k] = 0.f;
-      }
+      if (tid == 0) bulk_wait_group0();
     }
   }
-  __syncwarp();
-  tcgen05_fence_before();
   __syncthreads();
   if (p.y)
     for (int i = tid; i < HEAD_PART; i += HT_THREADS) p.partial[(long)i * gridDim.x + blockIdx.x] = red_s[i];
-  if (warp == 0) tmem_dealloc(tmem, 256);
 }
 
 // dWo[j][k] = sum_r y[r][j] * dpred[r][k] with y = Dropout(BN(h)) recomputed from h: CTA tiles of 32 rows staged in
@@ -1302,8 +1176,9 @@ void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, char* ba
   m.WoTp = reinterpret_cast<__nv_bfloat16*>(take(TC_OPAD * H * 2));
   m.WoSp = reinterpret_cast<__nv_bfloat16*>(take(H * 32 * 2));
   m.bop = reinterpret_cast<float*>(take(TC_OPAD * 4));
-  m.head_ctas = 148 * 2;
-  m.head_wctas = 148 * 2;
+  m.n_sms = device_sm_count();
+  m.head_ctas = m.n_sms * 2;
+  m.head_wctas = m.n_sms * 2;
   m.head_part_elems = (size_t)m.head_ctas * HEAD_PART;
   m.head_part = reinterpret_cast<float*>(take(m.head_part_elems * 4));
   if (!c.forward_only) {
@@ -1359,9 +1234,9 @@ int tc_init(TcState& st, const lfmq_config& c) {
   if ((rc = make_map_2d(&m.tm_w, m.Wp, 32, 4 * TC_H, 64, 32, 256, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-  // how many 8-CTA clusters can be co-resident (one CTA per SM because of shared memory)
+  // how many 4-CTA clusters can be co-resident (one CTA per SM because of shared memory)
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(TC_NC * 37);
+  cfg.gridDim = dim3(TC_NC * (m.n_sms / TC_NC));
   cfg.blockDim = dim3(FWD_THREADS);
   cfg.dynamicSmemBytes = FWD_SMEM;
   cudaLaunchAttribute attr[1];
@@ -1384,13 +1259,6 @@ int tc_init(TcState& st, const lfmq_config& c) {
 }
 
 void tc_destroy(TcState& st) {
-  if (st.impl && st.impl->side) {
-    cudaStreamSynchronize(st.impl->side);
-    cudaEventDestroy(st.impl->ev_fork);
-    cudaEventDestroy(st.impl->ev_join);
-    cudaStreamDestroy(st.impl->side);
-    cudaFree(st.impl->progress);
-  }
   delete st.impl;
   st.impl = nullptr;
 }
@@ -1422,45 +1290,21 @@ static int tc_run_recurrence(TcState& st, const float* x, int B, bool save, cuda
   p.B = B; p.T = m.T;
   p.n_clusters = n_tiles < m.max_clusters ? n_tiles : m.max_clusters;
   p.n_iters = (n_tiles + p.n_clusters - 1) / p.n_clusters;
+  p.n_tiles = n_tiles;
   p.k16_x = (m.I + 15) / 16;
   p.n_tiles_cap = (m.maxB + 127) / 128;
   p.xh = m.xh;
   p.gates = save ? m.gates : nullptr;
   p.cst = save ? m.cst : nullptr;
   p.biasp = m.biasp;
-  static long long* trace_dev = nullptr;
-  static const bool want_trace = getenv("LFMQ_TRACE_FWD") != nullptr;
-  if (want_trace && !trace_dev) {
-    LFMQ_CUDA_CHECK(cudaMalloc(&trace_dev, 3 * 16 * 8 * sizeof(long long)));
-  }
-  if (want_trace) LFMQ_CUDA_CHECK(cudaMemsetAsync(trace_dev, 0, 3 * 16 * 8 * sizeof(long long), s));
-  p.trace = want_trace ? trace_dev : nullptr;
   if (save) {
     if (int rc = launch_pdl(lstm_fwd_tc_kernel<true>, dim3(TC_NC * p.n_clusters), dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, p,
-                            m.tm_h, m.tm_x, m.tm_u, m.tm_w, m.tm_h128))
+                            m.tm_h, m.tm_x, m.tm_u, m.tm_w))
       return rc;
   } else {
     if (int rc = launch_pdl(lstm_fwd_tc_kernel<false>, dim3(TC_NC * p.n_clusters), dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, p,
-                            m.tm_h, m.tm_x, m.tm_u, m.tm_w, m.tm_h128))
+                            m.tm_h, m.tm_x, m.tm_u, m.tm_w))
       return rc;
-  }
-  if (want_trace) {
-    long long h[3 * 16 * 8];
-    LFMQ_CUDA_CHECK(cudaStreamSynchronize(s));
-    LFMQ_CUDA_CHECK(cudaMemcpy(h, trace_dev, sizeof(h), cudaMemcpyDeviceToHost));
-    const long long t0 = h[(1 * 16 + 0) * 8 + 0];
-    const char* names[3] = {"producer", "mma", "epilogue"};
-    for (int t = 0; t < 16; ++t) {
-      fprintf(stderr, "[trace t=%2d]", 3 * t);
-      for (int r = 0; r < 3; ++r) {
-        fprintf(stderr, "  %s:", names[r]);
-        for (int k = 0; k < 6; ++k) {
-          const long long v = h[(r * 16 + t) * 8 + k];
-          fprintf(stderr, " %lld", v ? v - t0 : -1LL);
-        }
-      }
-      fprintf(stderr, "\n");
-    }
   }
   return 0;
 }
@@ -1477,11 +1321,6 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, f
   h.Wo = params + m.oWo; h.bo = params + m.obo;
   h.y = y; h.denom = denom; h.p1 = c.target_lambda; h.p2 = c.rnn_lambda;
   h.use_dropout = (c.train && c.dropout > 0.f) ? 1 : 0;
-  static long long* htrace = nullptr;
-  static const bool want_htrace = getenv("LFMQ_TRACE_HEAD") != nullptr;
-  if (want_htrace && !htrace) LFMQ_CUDA_CHECK(cudaMalloc(&htrace, 2 * 8 * 8 * sizeof(long long)));
-  if (want_htrace) LFMQ_CUDA_CHECK(cudaMemsetAsync(htrace, 0, 2 * 8 * 8 * sizeof(long long), s));
-  h.trace = want_htrace ? htrace : nullptr;
   h.key.k0 = (uint32_t)(c.seed & 0xffffffffu);
   h.key.k1 = (uint32_t)(c.seed >> 32);
   h.key.stream = 0;
@@ -1510,19 +1349,6 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, f
                               m.tm_dpb, n_btiles, n_tiles_cap, m.head_wpart))
         return rc;
       n_wcta = grid;
-      if (want_htrace) {
-        long long hh[2 * 8 * 8];
-        LFMQ_CUDA_CHECK(cudaStreamSynchronize(s));
-        LFMQ_CUDA_CHECK(cudaMemcpy(hh, htrace, sizeof(hh), cudaMemcpyDeviceToHost));
-        const long long t0 = hh[0];
-        for (int k = 0; k < 8; ++k) {
-          fprintf(stderr, "[htrace tile %d]  ctl:", k);
-          for (int q = 0; q < 4; ++q) fprintf(stderr, " %lld", hh[(0 * 8 + k) * 8 + q] ? hh[(0 * 8 + k) * 8 + q] - t0 : -1LL);
-          fprintf(stderr, "  row:");
-          for (int q = 0; q < 6; ++q) fprintf(stderr, " %lld", hh[(1 * 8 + k) * 8 + q] ? hh[(1 * 8 + k) * 8 + q] - t0 : -1LL);
-          fprintf(stderr, "\n");
-        }
-      }
     } else {
       head_rows_kernel<true><<<grid, 128, HROWS_SMEM, s>>>(h, m.tm_h128, n_btiles, n_tiles_cap);
       LFMQ_LAUNCH_CHECK();
@@ -1602,94 +1428,53 @@ int tc_backward(TcState& st, const lfmq_config& c, const float* params, float* g
 // =============================================================================================
 // Persistent backward recurrence (reverse t inside the kernel), clusters of 4 CTAs per 128-row tile.
 //   CTA r owns hidden units [64r, 64r+64): it computes dz_t for its 256 gate columns (pointwise, SURVEY App. A.4),
-//   keeps them as the A operand in shared memory and multiplies by ITS K-slice of U (resident for the whole unroll):
-//       partial_r[128 x 256] = dz_t[:, own 256 gate cols] * U[all 256 hidden, own gate cols]^T       (tcgen05)
+//   stages them as the A operand in shared memory and multiplies by ITS K-slice of U (resident for the whole unroll):
+//       partial_r[128 x 256] = dz_t[:, own 256 gate cols] * U[all 256 hidden, own gate cols]^T       (wgmma)
 //   dh_{t-1}[:, slice q] = sum_r partial_r[:, slice q]: the three foreign 128x64 slices travel as bf16 through a
-//   global scratch (written with STG.256, fetched with TMA) -- a reduce-scatter whose volume (48 KB in per CTA and
-//   step) is 5x smaller than all-gathering dz; DSMEM would cost ~3700 cycles for it (profiles/r01_tc_probe.txt).
+//   global scratch (written by the owners, fetched with 1-D bulk copies) -- a reduce-scatter whose volume (48 KB in
+//   per CTA and step) is 5x smaller than all-gathering dz.
 //   K order inside the slice: k' = 64*jb + 16*g + jj  <->  gate column g*H + 64r + 16*jb + jj, so hidden chunk jb
 //   (16 units x 4 gates) is one 64-wide k-block and its MMAs overlap the pointwise work of chunk jb+1.
+//   The N order of the resident U slice is rotated per CTA: accumulator columns 64d .. 64d+63 are hidden slice
+//   (r + d) mod 4, so the CTA's own slice is always columns 0..63.
 // =============================================================================================
 namespace lfmq {
 
 struct BwdParams {
-  int B, T, n_iters, n_clusters, n_tiles_cap;
+  int B, T, n_iters, n_clusters, n_tiles, n_tiles_cap;
   const __nv_bfloat16* gates;
   const __nv_bfloat16* cst;
   const __nv_bfloat16* dhout;
-  __nv_bfloat16* dz;
-  __nv_bfloat16* pexch;      // [tile][parity][src][dst][128][64]
-  long long* trace;          // debug (LFMQ_TRACE_BWD=1)
-  unsigned long long* progress;   // null, or where CTA 0 publishes base + (steps it has completed)
-  unsigned long long base;
+  __nv_bfloat16* pexch;      // [tile][parity][src][dst][16-column block][128 rows][16]
 };
 
-#define BWD_TRACE(role, k, pt)                                                                            \
-  do {                                                                                                    \
-    if (p.trace && blockIdx.x == 0 && (k) % 3 == 0) p.trace[((role) * 16 + (k) / 3) * 8 + (pt)] = clock64();      \
-  } while (0)
-
 constexpr int BWD_NC = 4;
-#ifndef LFMQ_BWD_LATE_C1
-#define LFMQ_BWD_LATE_C1 1
-#endif
-constexpr bool LATE_C1 = LFMQ_BWD_LATE_C1 == 1;     // at the top of the step
-constexpr bool POST_C1 = LFMQ_BWD_LATE_C1 == 2;     // experiment: right after the export stores of the previous step
-#ifndef LFMQ_BWD_LATE_C0
-#define LFMQ_BWD_LATE_C0 0
-#endif
-#ifndef LFMQ_BWD_DSMEM
-#define LFMQ_BWD_DSMEM 0
-#endif
-// Partial exchange: 0 = through L2 (st.global, cluster arrive, TMA load by the peer's producer); 1 = every pointwise
-// thread pushes its piece of the foreign slices straight into the peers' shared memory (st.async completing tx-bytes on
-// the peer's recv_full).  Measured (profiles/r02_time_c19_dsmem_exchange.txt): the push makes the export itself shorter
-// (3.4 K -> 1.9 K cycles) but the 48 KB per CTA and step take ~4 K cycles to land (DSMEM moves ~12 B/clk/SM), against
-// 2.6 K for signal + TMA load from L2: bwd 0.304 -> 0.341 ms.  Kept as a build option, off.
-constexpr bool DSMEM_X = LFMQ_BWD_DSMEM != 0;
-#ifndef LFMQ_BWD_WARP_SIGNAL
-#define LFMQ_BWD_WARP_SIGNAL 0
-#endif
-// 1 = every pointwise warp signals the peers itself after its own export stores (no CTA-wide named barrier first)
-constexpr bool WARP_SIG = LFMQ_BWD_WARP_SIGNAL != 0 && !DSMEM_X;
-#ifndef LFMQ_BWD_EXPORT_BATCH
-#define LFMQ_BWD_EXPORT_BATCH 1
-#endif
-constexpr bool EXPORT_BATCH = LFMQ_BWD_EXPORT_BATCH != 0;
-#ifndef LFMQ_BWD_PX_BLOCKED
-#define LFMQ_BWD_PX_BLOCKED 1
-#endif
-// exchange scratch as [16-column block][row][16]: a warp's 256-bit export store is 1 KB contiguous (it was 32 separate
-// 32-byte pieces, one per 128-byte row), the receiver fetches its 16 KB slice with one 1-D bulk copy and reads it as is
-constexpr bool PX_BLOCKED = LFMQ_BWD_PX_BLOCKED != 0 && !DSMEM_X;
-constexpr bool LATE_C0 = LFMQ_BWD_LATE_C0 != 0;     // experiment: the first chunk's operands at the top of the step as well
-// Warp roles, by warpgroup (setmaxnreg moves registers between warpgroups): warps 0-3 pointwise set 0, warps 4-7 pointwise
-// set 1, warps 8-11 = producer, MMA issuer, dz store, idle.  The role warpgroup gives its registers up (72 each), the
-// pointwise warps take 216 (2 x 216 + 72 = the 504 of the 168 x 3 pool): the 168 of an even split left ~100 spilled values on the pointwise warps' path, with next to
-// no L1 to catch them (226 KB of shared memory in use).
+// Warpgroups 0 and 1: pointwise gate gradients, A-operand staging, MMAs and partial exchange for rows 0-63 / 64-127 of
+// the tile (the accumulator lives in their registers); warpgroup 2: warp 8 = TMA producer.  setmaxnreg moves the
+// registers of the producer warpgroup to the two that hold 128 accumulators each.
 constexpr int BWD_THREADS = 384;
-constexpr int BWD_W_PROD = 8, BWD_W_MMA = 9, BWD_W_STORE = 10;
+constexpr int BWD_W_PROD = 8;
 constexpr uint32_t SB_U = 0;                    // 4 k-blocks x [256 x 128 B]
 constexpr uint32_t SB_A = 131072;               // 2 stages x [128 x 128 B]
-constexpr uint32_t SB_R = 163840;               // 3 foreign slices x [128 x 128 B]
+constexpr uint32_t SB_R = 163840;               // 3 foreign slices x [16-column block][128 rows][16] bf16
 constexpr uint32_t SB_DPB = 212992;             // FUSED: dLoss/dpred tile of one step [128 x 64 B], SW64
 constexpr uint32_t SB_WOS = 221184;             // FUSED: (Wo gamma inv) rows of this CTA's 64 hidden units [64 x 64 B], SW64
 constexpr uint32_t SB_BARS = 225280;
 constexpr uint32_t BWD_SMEM = SB_BARS + 256 + 1024;
 
 struct BwdBars {
-  uint64_t w_full, a_full[2], a_empty[2], acc_full[2], recv_full, recv_free, exp_ready;
-  uint64_t dpb_full, dpb_free;   // FUSED: the dpred tile has landed / the MMA reading it has completed
-  uint32_t tmem_base;
+  uint64_t w_full, recv_full, recv_free, exp_ready;
+  uint64_t dpb_full, dpb_free;   // FUSED: the dpred tile has landed / the MMAs reading it have completed
 };
 
+__device__ __forceinline__ uint32_t ld_b32(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
+
 // FUSED (no dropout in the head): dLoss/dh of the head is not read from HBM.  With dy = dpred Wo^T it equals
-// dpred (Wo gamma inv)^T; the MMA warp adds that product for this CTA's 64 hidden units (two M128 x N64 x K16 MMAs per
-// step on the 8 KB dpred tile) into the accumulator whose own slice the pointwise warps read anyway.
+// dpred (Wo gamma inv)^T; each warpgroup adds that product for this CTA's 64 hidden units (M64 x N64 x K32 on the 8 KB
+// dpred tile) into the own-slice columns of its accumulator.
 template <bool FUSED>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
-    lstm_bwd_tc_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk,
-                       const __grid_constant__ CUtensorMap tm_px, const __grid_constant__ CUtensorMap tm_dzst,
+    lstm_bwd_tc_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
                        const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -1701,415 +1486,239 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
 
   if (tid == 0) {
     mbar_init(&bars->w_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bars->a_full[i], 128);
-      mbar_init(&bars->a_empty[i], 2);      // the MMAs that read the stage have completed + the dz store has read it
-      mbar_init(&bars->acc_full[i], 1);
-    }
     mbar_init(&bars->recv_full, 1);
-    mbar_init(&bars->recv_free, WARP_SIG ? 8 : 1);
-    mbar_init(&bars->exp_ready, (DSMEM_X || WARP_SIG) ? (BWD_NC - 1) * 8 : BWD_NC - 1);   // DSMEM_X: 'peers have read my last export'
+    mbar_init(&bars->recv_free, 1);
+    mbar_init(&bars->exp_ready, BWD_NC - 1);
     mbar_init(&bars->dpb_full, 1);
-    mbar_init(&bars->dpb_free, 1);
+    mbar_init(&bars->dpb_free, 8);          // one arrive per consumer warp
     fence_mbar_init();
   }
-  if (warp == BWD_W_MMA) tmem_alloc(&bars->tmem_base, 512);
-  tcgen05_fence_before();
   __syncthreads();
   cluster_sync_all();
-  tcgen05_fence_after();
-  const uint32_t tmem = bars->tmem_base;
   // programmatic dependent launch: the weight slices (packed at the start of the step) load under the predecessor's tail
   if (!(warp == BWD_W_PROD && lane == 0)) pdl_sync();
 
   if (warp >= 8) {
-  // one setmaxnreg for the whole role warpgroup (it is warpgroup-collective), then the roles; not re-indented
-  setmaxnreg_dec<72>();
-  if (warp == BWD_W_PROD) {
-    // ===================== TMA producer: weights once, then the foreign partial slices of every step =========
-    // (an L2 prefetch of the saved activations two steps ahead was tried here and made the kernel 25 % slower)
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == BWD_W_PROD && lane == 0) {
+      // ===================== TMA producer: weights once, then the foreign partial slices of every step =========
       mbar_arrive_expect_tx(&bars->w_full, 131072 + (FUSED ? 4096 : 0));
-      for (int jb = 0; jb < 4; ++jb) tma_load_2d(smem + SB_U + jb * 32768, &tm_ubk, &bars->w_full, jb * 64, rank * 256);
+      for (int jb = 0; jb < 4; ++jb)
+        for (int d = 0; d < 4; ++d)
+          tma_load_2d(smem + SB_U + jb * 32768 + d * 8192, &tm_ubk, &bars->w_full, jb * 64,
+                      (int)rank * 256 + (int)((rank + d) & 3) * 64);
       if (FUSED) tma_load_2d(smem + SB_WOS, &tm_wos, &bars->w_full, 0, rank * 64);
       pdl_sync();
-    }
-    uint32_t n_er = 0, n_dp = 0;
-    // dpred tile of time step td into the single staging buffer, once the MMA that read the previous one is done
-    auto load_dpred = [&](int tile, int td) {
-      if (n_dp > 0) mbar_wait(&bars->dpb_free, (n_dp - 1) & 1);
-      ++n_dp;
-      mbar_arrive_expect_tx(&bars->dpb_full, 8192);
-      tma_load_2d(smem + SB_DPB, &tm_dpb, &bars->dpb_full, 0, (td * p.n_tiles_cap + min(tile, p.n_tiles_cap - 1)) * 128);
-    };
-    for (int it = 0; it < p.n_iters; ++it) {
-      const int tile = it * p.n_clusters + cid;
-      if (FUSED && lane == 0) load_dpred(tile, T - 1);
-      for (int t = T - 1; t >= 0; --t) {
-        if (FUSED && lane == 0 && t > 0) load_dpred(tile, t - 1);      // for the MMA appended to this step
-        if (DSMEM_X && lane == 0 && t <= T - 2) {    // peers push the slices themselves: only arm the barrier, one phase
-          if (n_er > 0) mbar_wait(&bars->recv_full, (n_er - 1) & 1);    // at a time
-          ++n_er;
-          BWD_TRACE(0, T - 1 - t, 0);
-          mbar_arrive_expect_tx(&bars->recv_full, 3 * 16384);
-        }
-        if (!DSMEM_X && lane == 0 && t <= T - 2) {   // step t consumes the partials exported after step t+1
-          mbar_wait_cluster(&bars->exp_ready, (n_er) & 1);
-          mbar_wait(&bars->recv_free, (n_er++) & 1);    // own epilogue is done reading the previous slices
-          BWD_TRACE(0, T - 1 - t, 0);
-          fence_proxy_async_global();
-          mbar_arrive_expect_tx(&bars->recv_full, 3 * 16384);
-          const int par = (t + 1) & 1;
-          for (uint32_t d = 1; d < BWD_NC; ++d) {
-            const uint32_t src = (rank + d) & 3;
-            if (PX_BLOCKED)
+      uint32_t n_er = 0, n_dp = 0;
+      // dpred tile of time step td into the single staging buffer, once the MMAs that read the previous one are done
+      auto load_dpred = [&](int tile, int td) {
+        if (n_dp > 0) mbar_wait(&bars->dpb_free, (n_dp - 1) & 1);
+        ++n_dp;
+        mbar_arrive_expect_tx(&bars->dpb_full, 8192);
+        tma_load_2d(smem + SB_DPB, &tm_dpb, &bars->dpb_full, 0, (td * p.n_tiles_cap + tile) * 128);
+      };
+      for (int it = 0; it < p.n_iters; ++it) {
+        const int tile = it * p.n_clusters + cid;
+        if (tile >= p.n_tiles) break;                     // clusters without a tile in the last round
+        if (FUSED) load_dpred(tile, T - 1);
+        for (int t = T - 1; t >= 0; --t) {
+          if (FUSED && t > 0) load_dpred(tile, t - 1);      // for the MMA at the end of this step
+          if (t <= T - 2) {                                 // step t consumes the partials exported after step t+1
+            mbar_wait_cluster(&bars->exp_ready, n_er & 1);
+            mbar_wait(&bars->recv_free, (n_er++) & 1);      // own consumers are done reading the previous slices
+            fence_proxy_async_global();
+            mbar_arrive_expect_tx(&bars->recv_full, 3 * 16384);
+            const int par = (t + 1) & 1;
+            for (uint32_t d = 1; d < BWD_NC; ++d) {
+              const uint32_t src = (rank + d) & 3;
               bulk_load_1d(smem + SB_R + (d - 1) * 16384,
                            p.pexch + ((((long)(tile * 2 + par) * 4 + (int)src) * 4 + (int)rank)) * 128 * 64, 16384,
                            &bars->recv_full);
-            else
-              tma_load_2d(smem + SB_R + (d - 1) * 16384, &tm_px, &bars->recv_full, 0,
-                          ((((tile * 2 + par) * 4 + (int)src) * 4 + (int)rank)) * 128);
-          }
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == BWD_W_MMA) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(128, 256, false, false);
-      const uint32_t idesc_dy = make_idesc_bf16(128, 64, false, false);
-      mbar_wait(&bars->w_full, 0);
-      uint32_t gs = 0;      // global step counter
-      uint32_t n_dpu = 0;   // dpred tiles consumed
-      // dpred(td) (Wo gamma inv)^T for this CTA's 64 hidden units into `dst` (own columns of an accumulator buffer)
-      auto dy_mma = [&](uint32_t dst, bool accumulate) {
-        mbar_wait(&bars->dpb_full, (n_dpu++) & 1);
-        tcgen05_fence_after();
-#pragma unroll
-        for (int k16 = 0; k16 < 2; ++k16) {
-          const uint64_t da = make_smem_desc(smem_u32(smem + SB_DPB) + k16 * 32, 0, 512, LAYOUT_SW64);
-          const uint64_t db = make_smem_desc(smem_u32(smem + SB_WOS) + k16 * 32, 0, 512, LAYOUT_SW64);
-          umma_f16(dst, da, db, idesc_dy, (accumulate || k16 > 0) ? 1u : 0u);
-        }
-        umma_commit(&bars->dpb_free);
-      };
-      for (int it = 0; it < p.n_iters; ++it) {
-        if (FUSED) {        // dLoss/dh of the head for the tile's first step (t = T-1): nothing recurrent to add to yet
-          const uint32_t pb = (gs + 1) & 1;
-          dy_mma(tmem + pb * 256 + rank * 64, false);
-          umma_commit(&bars->acc_full[pb]);
-        }
-        for (int t = T - 1; t >= 0; --t, ++gs) {
-          const uint32_t acc = tmem + (gs & 1) * 256;
-          for (int jb = 0; jb < 4; ++jb) {
-            const uint32_t st = jb & 1;                      // stage = producing warp-set
-            const uint32_t n_use = gs * 2 + (jb >> 1);
-            mbar_wait(&bars->a_full[st], n_use & 1);
-            if (jb == 0) BWD_TRACE(1, T - 1 - t, 0);
-            if (jb == 3) BWD_TRACE(1, T - 1 - t, 1);
-            tcgen05_fence_after();
-#pragma unroll
-            for (int k16 = 0; k16 < 4; ++k16) {
-              const uint64_t da = make_smem_desc(smem_u32(smem + SB_A + st * 16384) + k16 * 32, 0, 1024, LAYOUT_SW128);
-              const uint64_t db = make_smem_desc(smem_u32(smem + SB_U + jb * 32768) + k16 * 32, 0, 1024, LAYOUT_SW128);
-              umma_f16(acc, da, db, idesc, (jb | k16) != 0);
             }
-            umma_commit(&bars->a_empty[st]);
-          }
-          if (FUSED && t > 0) dy_mma(acc + rank * 64, true);      // head part of dLoss/dh_{t-1}, read as `rec` next step
-          umma_commit(&bars->acc_full[gs & 1]);
-          BWD_TRACE(1, T - 1 - t, 2);
-        }
-      }
-    }
-  } else if (warp == BWD_W_STORE) {
-    // ===================== dz store warp =====================
-    // dz_t of every staged chunk leaves for HBM straight from the A operand: one TMA store (128 rows x 128 B, rows >= B
-    // clipped) instead of four STG.256 per pointwise thread.  dz keeps the operand's column order [16-unit block][gate][16]
-    // (see tc_layout); wgrad_reduce_kernel puts the gate columns back in order.  A warp of its own: the wait for the
-    // store's shared-memory read (~1.5 K cycles per chunk, profiles/r01_btrace_v6) used to sit on the MMA thread, between
-    // the last chunk's MMAs and the commit the exchange waits for.
-    // (Keeping two stores in flight -- issuing chunk i before waiting for chunk i-1's read -- was measured and lost:
-    // 0.397 ms against 0.384 ms with the prefetch helper, 0.451 against 0.43 without, profiles/r02_summary.md.)
-    if (lane == 0) {
-      uint32_t gs = 0;
-      for (int it = 0; it < p.n_iters; ++it) {
-        for (int t = T - 1; t >= 0; --t, ++gs) {
-          for (int jb = 0; jb < 4; ++jb) {
-            const uint32_t st = jb & 1;
-            const uint32_t n_use = gs * 2 + (jb >> 1);
-            mbar_wait(&bars->a_full[st], n_use & 1);
-            tma_store_3d(&tm_dzst, smem + SB_A + st * 16384, (4 * (int)rank + jb) * 64, t,
-                         (it * p.n_clusters + cid) * 128);
-            bulk_commit_group();
-            bulk_wait_group_read0();
-            mbar_arrive(&bars->a_empty[st]);
           }
         }
       }
-      bulk_wait_group0();                        // all dz stores complete before the kernel ends
     }
-  }
   } else {
-    setmaxnreg_inc<216>();
-    // ===================== pointwise gate gradients, A-operand staging, partial exchange =====================
-    // Two warp-sets (A: warps 2-5, B: warps 6-9) split the four 16-unit chunks of a step: set s handles chunks
-    // s and s+2 and owns A-operand stage s, so two chunks' global loads are always in flight together, and each
-    // set issues the loads of its first chunk of step t-1 before the exchange of step t (they do not depend on it).
-    const int set = warp >> 2;               // 0 / 1
-    const int wq = warp & 3;                 // TMEM lane quadrant
-    const int m = wq * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(wq * 32) << 16;
-    const int sw = m & 7;
-    float dc[32];
-    uint32_t gs = 0, n_rf = 0;
-    uint32_t n_exp = 0;                      // exports done (DSMEM_X)
-    uint32_t caf[2] = {0, 0};                // completed phases of acc_full[b] (mirrors the MMA warp's commit sequence)
-    // inputs of this set's two chunks of one step (slot ci): loaded ahead of the exchange they do not depend on
-    uint32_t gi[2][8], gf[2][8], gg[2][8], go[2][8], dhp[2][8], ct[2][8], cp[2][8];
+    setmaxnreg_inc<232>();
+    // ===================== consumers =====================
+    // Warpgroup wg owns rows 64 wg .. 64 wg + 63.  Accumulator fragment (m64 x n256): register i holds row
+    // r0 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 cq + (i & 1).  Own slice = registers 0..31: unit 16 jb + jj of this
+    // CTA's 64, jj = 8 q + 2 cq + e, is register 4 (2 jb + q) + 2 h + e.
+    const int wg = warp >> 2, w = warp & 3, cq = lane & 3;
+    const int r0 = 64 * wg + 16 * w + (lane >> 2);
+    const bool elected = (tid & 127) == 0;
+    const uint32_t wg_bar = 2 + wg;
     const long tstride = (long)p.n_tiles_cap * 8 * 4 * 2 * 32 * 16;   // cst elements per time step
+    float acc[128];
+    float rown[32];                          // dLoss/dh (recurrent + head part) of the own slice for the current step
+    float dc[32];                            // carried dLoss/dc, same indexing as rown
+    uint32_t n_rf = 0, n_dpf = 0;
+    mbar_wait(&bars->w_full, 0);
 
-    auto load_chunk = [&](int ci, int tile, bool valid, int t) {
-      const int jb = 2 * ci + set;
-      if (valid) {
-        const long wblk = (((long)t * p.n_tiles_cap + tile) * 8 + 2 * rank + (jb >> 1)) * 4 + wq;
-        const int hb = jb & 1;
-        const __nv_bfloat16* grow = p.gates + (wblk * 8 * 32 + lane) * 16;
-        const __nv_bfloat16* crow = p.cst + ((wblk * 2 + hb) * 32 + lane) * 16;
-        ld_global_v8(grow + (0 * 2 + hb) * 512, gi[ci]);
-        ld_global_v8(grow + (1 * 2 + hb) * 512, gf[ci]);
-        ld_global_v8(grow + (2 * 2 + hb) * 512, gg[ci]);
-        ld_global_v8(grow + (3 * 2 + hb) * 512, go[ci]);
-        if (!FUSED)
-          ld_global_v8(p.dhout + ((((((long)t * p.n_tiles_cap + tile) * 4 + rank) * 4 + wq) * 4 + jb) * 32 + lane) * 16,
-                       dhp[ci]);
-        // c_t was this slot's c_{t-1} one step ago (the unroll runs backwards): only the first step of a tile loads it
-        if (t == T - 1) {
-          ld_global_v8(crow, ct[ci]);
-        } else {
+    // head part of dLoss/dh (dpred (Wo gamma inv)^T) into the own-slice registers: accumulate = 0 at a tile's first step
+    auto dy_mma = [&](uint32_t accumulate) {
+      mbar_wait(&bars->dpb_full, (n_dpf++) & 1);
+      wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 8; ++j) ct[ci][j] = cp[ci][j];
-        }
-        if (t > 0) {
-          ld_global_v8(crow - tstride, cp[ci]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) cp[ci][j] = 0u;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          gi[ci][j] = gf[ci][j] = gg[ci][j] = go[ci][j] = dhp[ci][j] = ct[ci][j] = cp[ci][j] = 0u;
+      for (int k16 = 0; k16 < 2; ++k16) {
+        const uint64_t da = make_smem_desc(smem_u32(smem + SB_DPB + wg * 4096) + k16 * 32, 0, 512, LAYOUT_SW64);
+        const uint64_t db = make_smem_desc(smem_u32(smem + SB_WOS) + k16 * 32, 0, 512, LAYOUT_SW64);
+        wgmma_m64n64k16<0, 0>(*reinterpret_cast<float(*)[32]>(acc), da, db, (accumulate || k16 > 0) ? 1u : 0u);
       }
+      wgmma_commit();
     };
 
     for (int it = 0; it < p.n_iters; ++it) {
       const int tile = it * p.n_clusters + cid;
-      const long b = (long)tile * 128 + m;
-      const bool valid = b < p.B;
+      if (tile >= p.n_tiles) break;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) dc[j] = 0.f;
-      if (!LATE_C0) load_chunk(0, tile, valid, T - 1);
-      if (!LATE_C1) load_chunk(1, tile, valid, T - 1);     // (also POST_C1: nothing precedes the first step)
-      if (FUSED) {                             // the head's dLoss/dh_{T-1} for the own slice is in the accumulator
-        const uint32_t pb = (gs + 1) & 1;
-        mbar_wait(&bars->acc_full[pb], caf[pb] & 1);
-        ++caf[pb];
+      for (int i = 0; i < 32; ++i) dc[i] = 0.f;
+      if (FUSED) {                             // the head's dLoss/dh_{T-1}: nothing recurrent to add to yet
+        dy_mma(0);
+        wgmma_wait<0>();
+        fence_regs(acc);
+        if (lane == 0) mbar_arrive(&bars->dpb_free);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) rown[i] = acc[i];
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) rown[i] = 0.f;
       }
-      for (int t = T - 1; t >= 0; --t, ++gs) {
+      for (int t = T - 1; t >= 0; --t) {
         const bool has_rec = t < T - 1;
-        const uint32_t acc_prev = tmem + ((gs + 1) & 1) * 256;     // partial of step t+1 (own slice still there)
-        // LATE_C1: the second chunk's operands are requested only now and land under the first chunk's arithmetic, so
-        // that only one chunk's operands (48 registers, not 96) are live across the export section below
-        if (LATE_C0) load_chunk(0, tile, valid, t);
-        if (LATE_C1) load_chunk(1, tile, valid, t);
         if (has_rec) mbar_wait(&bars->recv_full, (n_rf++) & 1);
-        if (tid == 64) BWD_TRACE(2, T - 1 - t, 0);
 #pragma unroll
-        for (int ci = 0; ci < 2; ++ci) {
-          const int jb = 2 * ci + set;
-          float rec[16];
-          if (has_rec || FUSED) {
-            uint32_t vr[16];
-            if (!has_rec) tcgen05_fence_after();
-            tmem_ld_32x32b_x16(acc_prev + lane_addr + rank * 64 + jb * 16, vr);
-            tmem_ld_wait();
+        for (int jb = 0; jb < 4; ++jb) {
+          const int st = jb & 1;
+          uint8_t* stage = smem + SB_A + st * 16384;
+          // all operands of the chunk requested before the first is used: one memory latency per chunk
+          uint32_t gi[2][2], gf[2][2], gg[2][2], go[2][2], ct[2][2], cp[2][2], dhp[2][2];     // [h][q]
 #pragma unroll
-            for (int j = 0; j < 16; ++j) rec[j] = __uint_as_float(vr[j]);
+          for (int h = 0; h < 2; ++h) {
+            const int m = r0 + 8 * h;
+            const bool valid = (long)tile * 128 + m < p.B;
+            const long blk = (((long)t * p.n_tiles_cap + tile) * 8 + 2 * rank + (jb >> 1)) * 4 + (m >> 5);
 #pragma unroll
-            for (int d = 0; d < 3 && has_rec; ++d) {
-              const uint8_t* rs = smem + SB_R + d * 16384 + (PX_BLOCKED ? (jb * 128 + m) * 32 : m * 128);
+            for (int q = 0; q < 2; ++q) {
+              const int jj = 8 * q + 2 * cq;
+              if (valid) {
+                const __nv_bfloat16* gp = p.gates + (blk * 8 + (jb & 1)) * 512 + (m & 31) * 16 + jj;
+                const __nv_bfloat16* cp_ = p.cst + (blk * 2 + (jb & 1)) * 512 + (m & 31) * 16 + jj;
+                gi[h][q] = ld_b32(gp);
+                gf[h][q] = ld_b32(gp + 1024);
+                gg[h][q] = ld_b32(gp + 2048);
+                go[h][q] = ld_b32(gp + 3072);
+                ct[h][q] = ld_b32(cp_);
+                cp[h][q] = t > 0 ? ld_b32(cp_ - tstride) : 0u;
+                dhp[h][q] = FUSED ? 0u
+                               : ld_b32(p.dhout + ((((((long)t * p.n_tiles_cap + tile) * 4 + rank) * 4 + (m >> 5)) * 4 + jb) * 32 +
+                                                   (m & 31)) * 16 + jj);
+              } else {
+                gi[h][q] = gf[h][q] = gg[h][q] = go[h][q] = ct[h][q] = cp[h][q] = dhp[h][q] = 0u;
+              }
+            }
+          }
+          // the stage is free: the MMAs of its previous use (two chunks ago) and the dz store that read it are done
+          wgmma_wait<1>();
+          if (elected) bulk_wait_group_read1();
+          named_bar_sync(wg_bar, 128);
 #pragma unroll
-              for (int h2 = 0; h2 < 2; ++h2) {
-                const uint4 v = *reinterpret_cast<const uint4*>(rs + (PX_BLOCKED ? h2 << 4 : ((2 * jb + h2) ^ sw) << 4));
-                const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+          for (int h = 0; h < 2; ++h) {
+            const int m = r0 + 8 * h;
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  rec[8 * h2 + 2 * e] += bf16_lo(w[e]);
-                  rec[8 * h2 + 2 * e + 1] += bf16_hi(w[e]);
+            for (int q = 0; q < 2; ++q) {
+              const int jj = 8 * q + 2 * cq;
+              const int ri = 4 * (2 * jb + q) + 2 * h;       // register of (unit jj, e = 0) in rown / dc
+              float rec0 = rown[ri], rec1 = rown[ri + 1];
+              if (has_rec) {
+#pragma unroll
+                for (int d = 0; d < 3; ++d) {
+                  const uint32_t v = *reinterpret_cast<const uint32_t*>(smem + SB_R + d * 16384 + ((jb * 128 + m) * 16 + jj) * 2);
+                  rec0 += bf16_lo(v);
+                  rec1 += bf16_hi(v);
                 }
               }
+              // gate-gradient algebra in packed bf16x2 (two units per word); only the carried dLoss/dc stays in fp32
+              // registers.  SURVEY App. A.4.
+              const uint32_t i2 = gi[h][q], f2 = gf[h][q], g2 = gg[h][q], o2 = go[h][q];
+              const uint32_t dh2 = FUSED ? pack_bf16x2(rec0, rec1) : add_bf16x2(dhp[h][q], pack_bf16x2(rec0, rec1));
+              const uint32_t tc2 = tanh_bf16x2(ct[h][q]);
+              const uint32_t omtc2 = fma_bf16x2(neg_bf16x2(tc2), tc2, BF16X2_ONE);        // 1 - tanh(c)^2
+              const uint32_t t1 = mul_bf16x2(mul_bf16x2(dh2, o2), omtc2);                 // dh * o * (1 - tc^2)
+              const float dcn0 = dc[ri] + bf16_lo(t1);
+              const float dcn1 = dc[ri + 1] + bf16_hi(t1);
+              dc[ri] = dcn0 * bf16_lo(f2);
+              dc[ri + 1] = dcn1 * bf16_hi(f2);
+              const uint32_t dcn2 = pack_bf16x2(dcn0, dcn1);
+              const uint32_t omi = fma_bf16x2(neg_bf16x2(i2), i2, i2);                    // i (1 - i)
+              const uint32_t omf = fma_bf16x2(neg_bf16x2(f2), f2, f2);                    // f (1 - f)
+              const uint32_t omg = fma_bf16x2(neg_bf16x2(g2), g2, BF16X2_ONE);            // 1 - g^2
+              const uint32_t omo = fma_bf16x2(neg_bf16x2(o2), o2, o2);                    // o (1 - o)
+              const uint32_t z[4] = {mul_bf16x2(dcn2, mul_bf16x2(g2, omi)), mul_bf16x2(dcn2, mul_bf16x2(cp[h][q], omf)),
+                                     mul_bf16x2(dcn2, mul_bf16x2(i2, omg)), mul_bf16x2(mul_bf16x2(dh2, tc2), omo)};
+              // A operand k-block jb: row m, 16-byte chunk 2g+q holds gate g, units 8q..8q+7 (SW128 K-major)
+#pragma unroll
+              for (int g = 0; g < 4; ++g)
+                *reinterpret_cast<uint32_t*>(stage + m * 128 + (((2 * g + q) ^ (m & 7)) << 4) + 4 * cq) = z[g];
             }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) rec[j] = 0.f;
           }
-          // gate-gradient algebra in packed bf16x2 (all operands arrive packed; dz leaves packed); only the carried
-          // dLoss/dc stays in fp32 registers.  SURVEY App. A.4.
-          uint32_t zi[8], zf[8], zg[8], zo[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const uint32_t i2 = gi[ci][e], f2 = gf[ci][e], g2 = gg[ci][e], o2 = go[ci][e];
-            const uint32_t dh2 = FUSED ? pack_bf16x2(rec[2 * e], rec[2 * e + 1])
-                                       : add_bf16x2(dhp[ci][e], pack_bf16x2(rec[2 * e], rec[2 * e + 1]));
-            const uint32_t tc2 = tanh_bf16x2(ct[ci][e]);
-            const uint32_t omtc2 = fma_bf16x2(neg_bf16x2(tc2), tc2, BF16X2_ONE);        // 1 - tanh(c)^2
-            const uint32_t t1 = mul_bf16x2(mul_bf16x2(dh2, o2), omtc2);                 // dh * o * (1 - tc^2)
-            const float dcn0 = dc[ci * 16 + 2 * e] + bf16_lo(t1);
-            const float dcn1 = dc[ci * 16 + 2 * e + 1] + bf16_hi(t1);
-            dc[ci * 16 + 2 * e] = dcn0 * bf16_lo(f2);
-            dc[ci * 16 + 2 * e + 1] = dcn1 * bf16_hi(f2);
-            const uint32_t dcn2 = pack_bf16x2(dcn0, dcn1);
-            const uint32_t omi = fma_bf16x2(neg_bf16x2(i2), i2, i2);                    // i (1 - i)
-            const uint32_t omf = fma_bf16x2(neg_bf16x2(f2), f2, f2);                    // f (1 - f)
-            const uint32_t omg = fma_bf16x2(neg_bf16x2(g2), g2, BF16X2_ONE);            // 1 - g^2
-            const uint32_t omo = fma_bf16x2(neg_bf16x2(o2), o2, o2);                    // o (1 - o)
-            zi[e] = mul_bf16x2(dcn2, mul_bf16x2(g2, omi));
-            zf[e] = mul_bf16x2(dcn2, mul_bf16x2(cp[ci][e], omf));
-            zg[e] = mul_bf16x2(dcn2, mul_bf16x2(i2, omg));
-            zo[e] = mul_bf16x2(mul_bf16x2(dh2, tc2), omo);
-          }
-          // A operand k-block jb in stage `set`: row m, chunk 2g+h holds gate g, units 8h..8h+7 (SW128 K-major)
-          const uint32_t n_use = gs * 2 + ci;                 // use index of this stage
-          if (n_use >= 1) mbar_wait(&bars->a_empty[set], (n_use - 1) & 1);
-          uint8_t* arow = smem + SB_A + set * 16384 + m * 128;
-          *reinterpret_cast<uint4*>(arow + ((0 ^ sw) << 4)) = make_uint4(zi[0], zi[1], zi[2], zi[3]);
-          *reinterpret_cast<uint4*>(arow + ((1 ^ sw) << 4)) = make_uint4(zi[4], zi[5], zi[6], zi[7]);
-          *reinterpret_cast<uint4*>(arow + ((2 ^ sw) << 4)) = make_uint4(zf[0], zf[1], zf[2], zf[3]);
-          *reinterpret_cast<uint4*>(arow + ((3 ^ sw) << 4)) = make_uint4(zf[4], zf[5], zf[6], zf[7]);
-          *reinterpret_cast<uint4*>(arow + ((4 ^ sw) << 4)) = make_uint4(zg[0], zg[1], zg[2], zg[3]);
-          *reinterpret_cast<uint4*>(arow + ((5 ^ sw) << 4)) = make_uint4(zg[4], zg[5], zg[6], zg[7]);
-          *reinterpret_cast<uint4*>(arow + ((6 ^ sw) << 4)) = make_uint4(zo[0], zo[1], zo[2], zo[3]);
-          *reinterpret_cast<uint4*>(arow + ((7 ^ sw) << 4)) = make_uint4(zo[4], zo[5], zo[6], zo[7]);
           fence_proxy_async_smem();
-          mbar_arrive(&bars->a_full[set]);
-          if (tid == 64 && ci == 0) BWD_TRACE(2, T - 1 - t, 1);
-          if (tid == 64 && ci == 1) BWD_TRACE(2, T - 1 - t, 2);
-          if (tid == 192 && ci == 0) BWD_TRACE(0, T - 1 - t, 1);     // warp-set 1 in the producer row's free slots
-          if (tid == 192 && ci == 1) BWD_TRACE(0, T - 1 - t, 2);
+          named_bar_sync(wg_bar, 128);
+          wgmma_fence();
+#pragma unroll
+          for (int k16 = 0; k16 < 4; ++k16) {
+            const uint64_t da = make_smem_desc(smem_u32(stage + wg * 8192) + k16 * 32, 0, 1024, LAYOUT_SW128);
+            const uint64_t db = make_smem_desc(smem_u32(smem + SB_U + jb * 32768) + k16 * 32, 0, 1024, LAYOUT_SW128);
+            wgmma_m64n256k16<0, 0>(acc, da, db, (jb | k16) != 0);
+          }
+          wgmma_commit();
+          // dz_t of the chunk leaves for HBM straight from the A operand: one TMA store per warpgroup (64 rows x 128 B,
+          // rows >= B clipped).  dz keeps the operand's column order [16-unit block][gate][16] (see tc_layout);
+          // wgrad_reduce_kernel puts the gate columns back in order.
+          if (elected) {
+            tma_store_3d(&tm_dzst, stage + wg * 8192, (4 * (int)rank + jb) * 64, t, tile * 128 + 64 * wg);
+            bulk_commit_group();
+          }
         }
-        if (DSMEM_X && has_rec) {                    // this warp is done with the received slices: tell the three senders
-          __syncwarp();
-          if (lane >= 1 && lane < BWD_NC)
-            mbar_arrive_cluster(mapa_u32(smem_u32(&bars->exp_ready), (rank + (uint32_t)lane) & 3));
-        }
-        // inputs of both chunks of the next step: independent of the exchange below.  Placement matters because the
-        // SM's memory pipe is a FIFO: issued here they delay the export slightly but land before the next step
-        // starts; issued after the export they arrive too late (+9 % kernel time), issued inside the chunk loop they
-        // hold up the chunk's own dz / A-operand stores (+17 %).
+        if (FUSED && t > 0) dy_mma(1);         // head part of dLoss/dh_{t-1}, read as `rown` next step
+        wgmma_wait<0>();
+        fence_regs(acc);
+        if (FUSED && t > 0 && lane == 0) mbar_arrive(&bars->dpb_free);
         if (t > 0) {
-          if (!LATE_C0) load_chunk(0, tile, valid, t - 1);
-          if (!LATE_C1 && !POST_C1) load_chunk(1, tile, valid, t - 1);
-        }
-        // ---- export the foreign slices of partial_t (needed by the peers for step t-1) ----
-        if (t > 0) {
-          mbar_wait(&bars->acc_full[gs & 1], caf[gs & 1] & 1);
-          if (tid == 64) BWD_TRACE(2, T - 1 - t, 3);
-          tcgen05_fence_after();
-          const uint32_t acc = tmem + (gs & 1) * 256 + lane_addr;
+          // ---- export the foreign slices of partial_t (needed by the peers for step t-1) ----
           const int par = t & 1;
-          if (DSMEM_X) {
-            // all 24 reader warps of the three peers have released the slices of the previous export
-            if (n_exp > 0) mbar_wait_cluster(&bars->exp_ready, (n_exp - 1) & 1);
-            ++n_exp;
 #pragma unroll
-            for (uint32_t d = 1; d < BWD_NC; ++d) {
-              const uint32_t dst = (rank + d) & 3;
-              // at the receiver, slot (d' - 1) holds the slice of source (dst + d') & 3: d' = 4 - d
-              const uint32_t rrow = mapa_u32(smem_u32(smem + SB_R + (3 - d) * 16384 + m * 128), dst);
-              const uint32_t rbar = mapa_u32(smem_u32(&bars->recv_full), dst);
-#pragma unroll
-              for (int hh = 0; hh < 2; ++hh) {
-                uint32_t v[16];
-                tmem_ld_32x32b_x16(acc + dst * 64 + set * 32 + hh * 16, v);
-                tmem_ld_wait();
-                uint32_t pk[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) pk[e] = pack_bf16x2(__uint_as_float(v[2 * e]), __uint_as_float(v[2 * e + 1]));
-                const int c0 = set * 4 + hh * 2;           // 16-byte chunk of the 64-column slice, 128B-swizzled by row
-                st_async_v4(rrow + (((c0) ^ sw) << 4), rbar, pk[0], pk[1], pk[2], pk[3]);
-                st_async_v4(rrow + (((c0 + 1) ^ sw) << 4), rbar, pk[4], pk[5], pk[6], pk[7]);
-              }
-            }
-          }
-#pragma unroll
-          if (!DSMEM_X && EXPORT_BATCH) {
-            // all six 16-column pieces requested from TMEM before the first is waited for: one tcgen05.ld latency
-            // instead of six (the 216-register budget of the pointwise warpgroups has room for the 96 values)
-            uint32_t v[6][16];
-#pragma unroll
-            for (uint32_t d = 1; d < BWD_NC; ++d)
-#pragma unroll
-              for (int hh = 0; hh < 2; ++hh)
-                tmem_ld_32x32b_x16(acc + ((rank + d) & 3) * 64 + set * 32 + hh * 16, v[(d - 1) * 2 + hh]);
-            tmem_ld_wait();
-#pragma unroll
-            for (uint32_t d = 1; d < BWD_NC; ++d) {
-              const uint32_t dst = (rank + d) & 3;
-              __nv_bfloat16* slice = p.pexch + (((long)(tile * 2 + par) * 4 + rank) * 4 + dst) * 128 * 64;
-              __nv_bfloat16* out = PX_BLOCKED ? slice + ((long)(set * 2) * 128 + m) * 16 : slice + m * 64 + set * 32;
-#pragma unroll
-              for (int hh = 0; hh < 2; ++hh) {
-                const uint32_t* vv = v[(d - 1) * 2 + hh];
-                uint32_t pk[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) pk[e] = pack_bf16x2(__uint_as_float(vv[2 * e]), __uint_as_float(vv[2 * e + 1]));
-                st_global_v8(out + hh * (PX_BLOCKED ? 128 * 16 : 16), pk);
-              }
-            }
-          }
-#pragma unroll
-          for (uint32_t d = 1; d < BWD_NC && !DSMEM_X && !EXPORT_BATCH; ++d) {
-            const uint32_t dst = (rank + d) & 3;
+          for (int d = 1; d < BWD_NC; ++d) {
+            const uint32_t dst = (rank + (uint32_t)d) & 3;
             __nv_bfloat16* slice = p.pexch + (((long)(tile * 2 + par) * 4 + rank) * 4 + dst) * 128 * 64;
-            __nv_bfloat16* out = PX_BLOCKED ? slice + ((long)(set * 2) * 128 + m) * 16 : slice + m * 64 + set * 32;
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              uint32_t v[16];
-              tmem_ld_32x32b_x16(acc + dst * 64 + set * 32 + hh * 16, v);
-              tmem_ld_wait();
-              uint32_t pk[8];
+            for (int jl = 0; jl < 8; ++jl)
 #pragma unroll
-              for (int e = 0; e < 8; ++e) pk[e] = pack_bf16x2(__uint_as_float(v[2 * e]), __uint_as_float(v[2 * e + 1]));
-              st_global_v8(out + hh * (PX_BLOCKED ? 128 * 16 : 16), pk);
-            }
+              for (int h = 0; h < 2; ++h) {
+                const int i = 4 * (8 * d + jl) + 2 * h;
+                *reinterpret_cast<uint32_t*>(slice + ((jl >> 1) * 128 + r0 + 8 * h) * 16 + 8 * (jl & 1) + 2 * cq) =
+                    pack_bf16x2(acc[i], acc[i + 1]);
+              }
           }
-          tcgen05_fence_before();
-          if (POST_C1) load_chunk(1, tile, valid, t - 1);
-          if (tid == 64) BWD_TRACE(2, T - 1 - t, 4);
-          if (!DSMEM_X && !WARP_SIG) named_bar_sync(1, 256);
-          if (WARP_SIG) __syncwarp();
-          if (tid == 64) BWD_TRACE(2, T - 1 - t, 5);
-          if (!DSMEM_X && (warp == 0 || WARP_SIG) && lane == 0) mbar_arrive(&bars->recv_free);
-          if (!DSMEM_X && (warp == 0 || WARP_SIG) && lane >= 1 && lane < BWD_NC) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) rown[i] = acc[i];
+          // both warpgroups have exported and have read the received slices of this step
+          named_bar_sync(1, 256);
+          if (warp == 0 && lane == 0) mbar_arrive(&bars->recv_free);
+          if (warp == 0 && lane >= 1 && lane < BWD_NC)
             mbar_arrive_cluster(mapa_u32(smem_u32(&bars->exp_ready), (rank + (uint32_t)lane) & 3));
-          }
         }
-        ++caf[gs & 1];                         // the MMA warp commits acc_full[gs & 1] every step, also at t = 0
-        if (p.progress && blockIdx.x == 0 && tid == 64)
-          *reinterpret_cast<volatile unsigned long long*>(p.progress) = p.base + (unsigned long long)(it * T + (T - t));
       }
     }
+    if (elected) bulk_wait_group0();            // all dz stores complete before the kernel ends
   }
   __syncwarp();
-  tcgen05_fence_before();
   cluster_sync_all();
-  if (warp == BWD_W_MMA) tmem_dealloc(tmem, 512);
 }
 
 // =============================================================================================
-// Weight gradients as ONE tcgen05 GEMM over all B*(T+1) rows:  D[384 x 1024] = xh^T * dz   (both MN-major)
+// Weight gradients as ONE wgmma GEMM over all B*(T+1) rows:  D[384 x 1024] = xh^T * dz   (both MN-major)
 //   rows 0..255 -> dU, rows 256..256+I-1 -> dW, row 288 (the constant-one column) -> db.
 // grid = (3 M-tiles, 4 N-tiles, S K-splits); deterministic split-K through fp32 partials.
 // =============================================================================================
@@ -2119,7 +1728,7 @@ struct WgradParams {
   float* partial;       // [S][384][1024]
 };
 
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = 2 * 128 + 32;     // two consumer warpgroups (M rows 0-63 / 64-127) + TMA producer warp
 constexpr int WG_STAGES = 4;
 constexpr uint32_t WG_STAGE_BYTES = 16384 + 32768;
 constexpr uint32_t WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
@@ -2131,8 +1740,6 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES);
   uint64_t* empty = full + WG_STAGES;
-  uint64_t* acc_full = empty + WG_STAGES;
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.x * 128, n0 = blockIdx.y * 256;
   const int kb_beg = blockIdx.z * p.kb_per_split;
@@ -2142,18 +1749,13 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
   if (tid == 0) {
     for (int s = 0; s < WG_STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);              // one arrive per consumer warp
     }
-    mbar_init(acc_full, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_s, 256);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tmem_base_s;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       for (int i = 0; i < nkb; ++i) {
         const int s = i % WG_STAGES;
@@ -2165,49 +1767,34 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
         for (int nb = 0; nb < 4; ++nb) tma_load_2d(st + 16384 + nb * 8192, &tm_b, &full[s], n0 + nb * 64, krow);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && nkb > 0) {
-      const uint32_t idesc = make_idesc_bf16(128, 256, true, true);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % WG_STAGES;
-        mbar_wait(&full[s], (i / WG_STAGES) & 1);
-        tcgen05_fence_after();
-        uint8_t* st = smem + s * WG_STAGE_BYTES;
-#pragma unroll
-        for (int k16 = 0; k16 < 4; ++k16) {
-          const uint64_t da = make_smem_desc(smem_u32(st) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-          const uint64_t db = make_smem_desc(smem_u32(st + 16384) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-          umma_f16(tmem, da, db, idesc, (i | k16) != 0);
-        }
-        umma_commit(&empty[s]);
-      }
-      umma_commit(acc_full);
-    }
   } else {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    float* out = p.partial + ((long)blockIdx.z * 384 + m0 + m) * 1024 + n0;
-    if (nkb > 0) {
-      mbar_wait(acc_full, 0);
-      tcgen05_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < 256; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem + ((uint32_t)(q * 32) << 16) + c0, v);
-        tmem_ld_wait();
+    const int wg = warp >> 2, w = warp & 3, cq = lane & 3;
+    float acc[128];
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(out + c0 + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                 __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % WG_STAGES;
+      mbar_wait(&full[s], (i / WG_STAGES) & 1);
+      uint8_t* st = smem + s * WG_STAGE_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k16 = 0; k16 < 4; ++k16) {
+        const uint64_t da = make_smem_desc(smem_u32(st + wg * 8192) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
+        const uint64_t db = make_smem_desc(smem_u32(st + 16384) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
+        wgmma_m64n256k16<1, 1>(acc, da, db, 1);
       }
-    } else {
-      for (int c0 = 0; c0 < 256; c0 += 4) *reinterpret_cast<float4*>(out + c0) = make_float4(0.f, 0.f, 0.f, 0.f);
+      wgmma_commit();
+      wgmma_wait<1>();                      // the previous stage's MMAs are complete: release it
+      if (i > 0 && lane == 0) mbar_arrive(&empty[(i - 1) % WG_STAGES]);
     }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    const int row = m0 + 64 * wg + 16 * w + (lane >> 2);
+    float* out = p.partial + ((long)blockIdx.z * 384 + row) * 1024 + n0 + 2 * cq;
+#pragma unroll
+    for (int i = 0; i < 128; i += 2)
+      *reinterpret_cast<float2*>(out + (long)8 * ((i >> 1) & 1) * 1024 + 8 * (i >> 2)) = make_float2(acc[i], acc[i + 1]);
   }
-  __syncwarp();
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 256);
 }
 
 // Sums the K-split partials and scatters D rows into dU / dW / db of the flat gradient vector.  D's columns are in
@@ -2229,46 +1816,6 @@ __global__ void wgrad_reduce_kernel(int S, int I, const float* __restrict__ part
   *dst = s;
 }
 
-// Runs beside lstm_bwd_tc_kernel on the SMs it leaves idle: pulls the saved gates / cell states of the time step that
-// is `lead` steps ahead of the recurrence into L2 (per step and tile iteration they are one contiguous range), paced by
-// the step counter CTA 0 of the recurrence publishes.  All 128 CTAs of the recurrence issue their preloads at the same
-// moment -- 12 MB at full HBM bandwidth, on the critical path; from L2 the same burst is ~2x shorter.  Measured
-// (B=4096, T=48): lead 1 0.405 ms, lead 2 0.390 ms, lead 3 0.418 ms, lead 4 / none 0.43 ms (prefetched lines do not
-// survive longer than ~2 steps of the kernel's own write traffic).  It only prefetches: no effect on results.  Waits
-// are bounded (1 ms, then it gives up for good), e.g. when a profiler serialises the two kernels.
-__global__ void __launch_bounds__(128) bwd_prefetch_kernel(const __nv_bfloat16* gates, const __nv_bfloat16* cst, int T,
-                                                          int n_iters, int n_clusters, int n_tiles, int n_tiles_cap,
-                                                          int lead, const unsigned long long* progress,
-                                                          unsigned long long base) {
-  const int nthr = gridDim.x * blockDim.x, gt = blockIdx.x * blockDim.x + threadIdx.x;
-  const long gates_tile = 8L * 4 * 8 * 32 * 16 * 2, cst_tile = 8L * 4 * 2 * 32 * 16 * 2;   // bytes per (step, tile)
-  __shared__ int give_up;
-  if (threadIdx.x == 0) give_up = 0;
-  __syncthreads();
-  for (int it = 0; it < n_iters; ++it) {
-    const int tile0 = it * n_clusters;
-    const int ntile = min(n_clusters, n_tiles - tile0);
-    if (ntile <= 0) break;
-    for (int t = T - 1; t >= 0; --t) {
-      const unsigned long long need = base + (unsigned long long)max(0, it * T + (T - 1 - t) - lead);
-      if (threadIdx.x == 0) {
-        int spins = 0;
-        while (*reinterpret_cast<const volatile unsigned long long*>(progress) < need && spins < 10000) {
-          __nanosleep(100);
-          ++spins;
-        }
-        if (spins >= 10000) give_up = 1;
-      }
-      __syncthreads();
-      if (give_up) return;
-      const char* g = reinterpret_cast<const char*>(gates) + ((long)t * n_tiles_cap + tile0) * gates_tile;
-      const char* c = reinterpret_cast<const char*>(cst) + ((long)t * n_tiles_cap + tile0) * cst_tile;
-      for (long off = (long)gt * 4096; off < ntile * gates_tile; off += (long)nthr * 4096) prefetch_l2_bulk(g + off, 4096);
-      for (long off = (long)gt * 4096; off < ntile * cst_tile; off += (long)nthr * 4096) prefetch_l2_bulk(c + off, 4096);
-    }
-  }
-}
-
 int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, float* grads, int B, bool fused,
                      cudaStream_t s) {
   TcImpl& m = *st.impl;
@@ -2277,11 +1824,10 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
     LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
     LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
     LFMQ_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
-    if ((rc = make_map_2d(&m.tm_ubk, m.Ubk, 256, 4 * TC_H, 512, 64, 256, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-    const uint64_t px_rows = (uint64_t)((m.maxB + 127) / 128) * 2 * 16 * 128;
-    if ((rc = make_map_2d(&m.tm_px, m.pexch, 64, px_rows, 128, 64, 128, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    // boxes of 64 hidden units: the kernel loads its K-slice of U in rotated N order (own hidden slice first)
+    if ((rc = make_map_2d(&m.tm_ubk, m.Ubk, 256, 4 * TC_H, 512, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
     cudaLaunchConfig_t qc = {};
-    qc.gridDim = dim3(BWD_NC * 37);
+    qc.gridDim = dim3(BWD_NC * (m.n_sms / BWD_NC));
     qc.blockDim = dim3(BWD_THREADS);
     qc.dynamicSmemBytes = BWD_SMEM;
     cudaLaunchAttribute qa[1];
@@ -2309,70 +1855,25 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
     bp.n_tiles_cap = (m.maxB + 127) / 128;
     bp.n_clusters = n_tiles < m.bwd_max_clusters ? n_tiles : m.bwd_max_clusters;
     bp.n_iters = (n_tiles + bp.n_clusters - 1) / bp.n_clusters;
-    bp.gates = m.gates; bp.cst = m.cst; bp.dhout = m.dhout; bp.dz = m.dz; bp.pexch = m.pexch;
-    static long long* btrace = nullptr;
-    static const bool want_btrace = getenv("LFMQ_TRACE_BWD") != nullptr;
-    if (want_btrace && !btrace) LFMQ_CUDA_CHECK(cudaMalloc(&btrace, 3 * 16 * 8 * sizeof(long long)));
-    if (want_btrace) LFMQ_CUDA_CHECK(cudaMemsetAsync(btrace, 0, 3 * 16 * 8 * sizeof(long long), s));
-    bp.trace = want_btrace ? btrace : nullptr;
-    static const int pf_lead = getenv("LFMQ_BWD_PREFETCH") ? atoi(getenv("LFMQ_BWD_PREFETCH")) : 2;   // 0 = off
-    bp.progress = nullptr;
-    bp.base = 0;
-    if (pf_lead > 0) {
-      if (!m.side) {
-        LFMQ_CUDA_CHECK(cudaStreamCreateWithFlags(&m.side, cudaStreamNonBlocking));
-        LFMQ_CUDA_CHECK(cudaEventCreateWithFlags(&m.ev_fork, cudaEventDisableTiming));
-        LFMQ_CUDA_CHECK(cudaEventCreateWithFlags(&m.ev_join, cudaEventDisableTiming));
-        LFMQ_CUDA_CHECK(cudaMalloc(&m.progress, sizeof(unsigned long long)));
-        LFMQ_CUDA_CHECK(cudaMemset(m.progress, 0, sizeof(unsigned long long)));
-      }
-      bp.progress = m.progress;
-      bp.base = m.epoch;
-      m.epoch += (unsigned long long)T * bp.n_iters;
-    }
-    // dz as [b][t][1024] with columns ordered [16-unit block][gate][16]: one staged chunk = 128 rows x 64 columns
+    bp.n_tiles = n_tiles;
+    bp.gates = m.gates; bp.cst = m.cst; bp.dhout = m.dhout; bp.pexch = m.pexch;
+    // dz as [b][t][1024] with columns ordered [16-unit block][gate][16]: one warpgroup's part of a staged chunk =
+    // 64 rows x 64 columns
     CUtensorMap tm_dzst;
     {
       const uint64_t dims[3] = {1024, (uint64_t)(T + 1), (uint64_t)B};
       const uint64_t strides[2] = {2048, (uint64_t)2048 * (T + 1)};
-      const uint32_t box[3] = {64, 1, 128};
+      const uint32_t box[3] = {64, 1, 64};
       if ((rc = make_map_nd(&tm_dzst, m.dz, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-    }
-    if (pf_lead > 0) {
-      LFMQ_CUDA_CHECK(cudaEventRecord(m.ev_fork, s));
-      LFMQ_CUDA_CHECK(cudaStreamWaitEvent(m.side, m.ev_fork, 0));
-      bwd_prefetch_kernel<<<20, 128, 0, m.side>>>(m.gates, m.cst, T, bp.n_iters, bp.n_clusters, n_tiles, bp.n_tiles_cap,
-                                                  pf_lead, m.progress, bp.base);
-      g_launches++;
-      LFMQ_CUDA_CHECK(cudaEventRecord(m.ev_join, m.side));
     }
     if (fused) {
       if ((rc = launch_pdl(lstm_bwd_tc_kernel<true>, dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, bp,
-                           m.tm_ubk, m.tm_px, tm_dzst, m.tm_dpb, m.tm_wos)))
+                           m.tm_ubk, tm_dzst, m.tm_dpb, m.tm_wos)))
         return rc;
     } else {
       if ((rc = launch_pdl(lstm_bwd_tc_kernel<false>, dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, bp,
-                           m.tm_ubk, m.tm_px, tm_dzst, m.tm_dpb, m.tm_wos)))
+                           m.tm_ubk, tm_dzst, m.tm_dpb, m.tm_wos)))
         return rc;
-    }
-    if (pf_lead > 0) LFMQ_CUDA_CHECK(cudaStreamWaitEvent(s, m.ev_join, 0));
-    if (want_btrace) {
-      long long h[3 * 16 * 8];
-      LFMQ_CUDA_CHECK(cudaStreamSynchronize(s));
-      LFMQ_CUDA_CHECK(cudaMemcpy(h, btrace, sizeof(h), cudaMemcpyDeviceToHost));
-      const long long t0 = h[(2 * 16 + 0) * 8 + 0];
-      const char* names[3] = {"producer", "mma", "epilogue"};
-      for (int k = 0; k < 16; ++k) {
-        fprintf(stderr, "[btrace k=%2d]", 3 * k);
-        for (int r = 0; r < 3; ++r) {
-          fprintf(stderr, "  %s:", names[r]);
-          for (int q = 0; q < 6; ++q) {
-            const long long v = h[(r * 16 + k) * 8 + q];
-            fprintf(stderr, " %lld", v ? v - t0 : -1LL);
-          }
-        }
-        fprintf(stderr, "\n");
-      }
     }
   }
   st.prof->end(LFMQ_REGION_BWD, s);
@@ -2385,7 +1886,8 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
   if ((rc = make_map_2d(&tm_b, m.dz, 4 * TC_H, rows, 4 * TC_H * 2, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   WgradParams wp;
   wp.n_kblocks = (int)((rows + 63) / 64);
-  int S = 12;
+  int S = m.n_sms / 12;                    // 3 x 4 output tiles per split: one wave of CTAs
+  if (S < 1) S = 1;
   if (wp.n_kblocks < S) S = wp.n_kblocks;
   wp.kb_per_split = (wp.n_kblocks + S - 1) / S;
   S = (wp.n_kblocks + wp.kb_per_split - 1) / wp.kb_per_split;

@@ -1,4 +1,4 @@
-// bf16 tensor-core path (LFMQ_PREC_BF16): persistent tcgen05 LSTM forward, per-step tcgen05 backward, tcgen05
+// bf16 tensor-core path (LFMQ_PREC_BF16): persistent wgmma LSTM forward and backward recurrences, wgmma
 // weight-gradient GEMM and the fused HBM-bound head.  See lstm_tc.cu / DESIGN.md.
 #pragma once
 #include "../../include/lfmq.h"

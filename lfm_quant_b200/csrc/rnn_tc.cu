@@ -2,7 +2,8 @@
 // cluster kernels of lstm_tc.cu do not cover -- H a multiple of 64 up to 512, stacked layers, dropout and recurrent
 // dropout (BASELINE configs[2]: H=512, L=2, dropout) -- and the fp32-tolerance mode LFMQ_PREC_BF16X3.
 //
-// One tcgen05 tile-GEMM skeleton (TMA ring -> tcgen05.mma -> TMEM -> epilogue warps) with three epilogues:
+// One wgmma tile-GEMM skeleton (TMA ring -> wgmma -> register accumulators -> epilogue in the same warpgroups) with
+// these epilogues:
 //   EPI_FWD    z_t = [h_{t-1} (*rec mask) | in_t] [U; W]   (one launch per time step and layer)
 //              epilogue = bias, gate nonlinearities, c_t / h_t update, h_t -> next step's A operand, saved state
 //   EPI_BWD    rec = dz_{t+1} U^T                           (one launch per time step and layer, reverse time)
@@ -30,11 +31,11 @@
 #include <vector>
 
 #include "kernels.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace lfmq {
 
-using namespace sm100;
+using namespace sm90;
 
 namespace {
 
@@ -77,7 +78,7 @@ inline long cdivl(long a, long b) { return (a + b - 1) / b; }
 // =============================================================================================
 // Tile GEMM skeleton
 // =============================================================================================
-// warp 0: TMA producer, warp 1: MMA issuer, then 4 epilogue warps (one TMEM lane quadrant each) per 128-row M tile
+// warps 0-7: two consumer warpgroups (MMAs + epilogue) per 128-row M tile, warp 8: TMA producer
 constexpr int G_MAXSEG = 6;
 constexpr int GBAR_N = 4096;       // step-barrier counters per handle: one per (persistent launch, row-tile group)
 
@@ -88,14 +89,14 @@ struct GSeg {
 struct GArgs {
   int n_seg;
   GSeg seg[G_MAXSEG];
-  int a_row_base;      // A row coordinate = a_row_base + 128 * (MT * blockIdx.x + rt_off)
+  int a_row_base;      // A row coordinate = a_row_base + 128 * (blockIdx.x + rt_off)
   int b_row_base;      // B row coordinate = b_row_base + BN * blockIdx.y
   int rt_off;          // first 128-row tile of this launch (the batch can be split over two concurrent launches)
   // Persistent mode (n_steps > 1): one launch runs n_steps consecutive time steps of a layer; step i works on A rows
   // a_row_base + i * row_step with EpiParams::t + i * t_step.  The A operand of a CTA's next step is written by the
   // gridDim.y CTAs of its own row-tile group (same blockIdx.x, all column tiles), so the steps are separated by one
   // barrier PER ROW-TILE GROUP (a counter in global memory; every CTA of the launch resident at once), not by a launch
-  // boundary: CTA dispatch, barrier init, TMEM allocation and the wait for the whole previous grid to retire are paid
+  // boundary: CTA dispatch, barrier init and the wait for the whole previous grid to retire are paid
   // once, and the row-tile groups drift apart instead of hitting HBM in lockstep.
   int n_steps, row_step, t_step;
   int lin_cols;        // > 0: 1-D grid, CTA i = (row tile i / lin_cols, column tile i % lin_cols): the column tiles of a row
@@ -103,9 +104,6 @@ struct GArgs {
   unsigned int* gbar;  // [gridDim.x], zeroed before the launch; counts the group's CTAs that have finished a step
 };
 
-#ifndef LFMQ_GEN_BWD_EW
-#define LFMQ_GEN_BWD_EW 2
-#endif
 enum { EPI_FWD = 0, EPI_BWD = 1, EPI_STORE = 2, EPI_FWD_ACC = 3, EPI_HEAD = 4 };   // _ACC: expf / tanhf (bf16x3)
 
 struct EpiParams {
@@ -140,150 +138,119 @@ struct EpiParams {
   float* hpartial;              // [GH_PART][gridDim.x]
   float hp1, hp2;
   int hO, htarget, htrain;
-  long long* trace;             // debug (LFMQ_TRACE_GEN=1): clock64 stamps of CTA (0,0): start, first stage landed, last MMA
-                                // issued, accumulator complete, epilogue done
 };
 
-// MT = 128-row M tiles per CTA: 1 (two CTAs per SM overlap one tile's epilogue with the other's loads) or 2 (a 256-row
-// CTA tile: each B stage feeds two MMAs, which cuts the L2 -> SM operand traffic per FLOP by a third; the stepped GEMMs
-// are bound by exactly that traffic, profiles/r02_summary.md).  The ring takes whatever shared memory one / two resident
-// CTAs leave: the loads are latency-bound (~5 K cycles per stage under load), bytes in flight are what buys bandwidth.
-template <int BN, int MT, int EPI = 0>
+// Two consumer warpgroups per CTA (rows 0-63 / 64-127 of the 128-row M tile, each with an m64 x BN accumulator in
+// registers) and one TMA producer warp.  The forward (N = 256: 128 accumulator registers per thread) and backward
+// steps run one CTA per SM; the multi-wave GEMMs (EPI_STORE, EPI_HEAD) keep two CTAs per SM.  The ring takes whatever
+// shared memory one / two resident CTAs leave: the loads are latency-bound, bytes in flight are what buys bandwidth.
+template <int BN, int EPI>
 struct GSmem {
-  static constexpr int EW = (EPI == 1) ? LFMQ_GEN_BWD_EW : 1;   // warps per TMEM lane quadrant and M tile (EPI_BWD)
-  static constexpr uint32_t A_BYTES = MT * 128 * 128;     // MT x (128 rows x 64 bf16)
+  static constexpr uint32_t A_BYTES = 128 * 128;          // 128 rows x 64 bf16
   static constexpr uint32_t B_BYTES = BN * 128;
   static constexpr uint32_t STAGE = A_BYTES + B_BYTES;
-  // one launch = one wave for the recurrence steps (<= 148 tiles: one CTA per SM, deep ring); the multi-wave GEMMs keep
-  // two CTAs per SM
-#ifndef LFMQ_GEN_BWD_2CTA
-#define LFMQ_GEN_BWD_2CTA 0
-#endif
-  // (LFMQ_GEN_BWD_2CTA: experiment -- two 64-unit backward CTAs per SM so that one's epilogue can overlap the other's mainloop)
-  static constexpr int CTAS_PER_SM =
-      (MT == 1 && (BN >= 256 || EPI == 2 || EPI == 4 || (LFMQ_GEN_BWD_2CTA && EPI == 1 && BN == 64))) ? 2 : 1;      // (2 = EPI_STORE, 4 = EPI_HEAD)
+  static constexpr int CTAS_PER_SM = (EPI == 2 || EPI == 4) ? 2 : 1;      // (2 = EPI_STORE, 4 = EPI_HEAD)
   static constexpr int NS = (int)((CTAS_PER_SM == 2 ? 98304u : 196608u) / STAGE);
   static constexpr uint32_t BARS = NS * STAGE;
-  static constexpr uint32_t TOTAL = BARS + 256 + 1024;    // + alignment slack
-  static constexpr int THREADS = 64 + 128 * MT * EW;      // producer + MMA + 4 * EW epilogue warps per M tile
+  static constexpr uint32_t HEAD_ROWS = BARS + 256;        // EPI_HEAD: [128][17] fp32 pred rows
+  static constexpr uint32_t TOTAL = HEAD_ROWS + (EPI == 4 ? 128 * 17 * 4 : 0) + 1024;   // + alignment slack
+  static constexpr int THREADS = 2 * 128 + 32;
 };
 
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-__device__ __forceinline__ void rec_mask16(const DropoutKey& k, int64_t grow, int H, int j0, float m[16]) {
-  const uint64_t qb = (uint64_t)grow * (uint64_t)(H / 4) + (uint64_t)(j0 / 4);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) dropout_quad(k, qb + i, m + 4 * i);
+// recurrent-dropout mask of the four units of quad j / 4 (the quad numbering of the SIMT path)
+__device__ __forceinline__ void rec_mask4(const DropoutKey& k, int64_t grow, int H, int j, float m[4]) {
+  dropout_quad(k, (uint64_t)grow * (uint64_t)(H / 4) + (uint64_t)(j / 4), m);
 }
 
-__device__ __forceinline__ void unpack16(const uint32_t w[8], float v[16]) {
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    v[2 * e] = bf16_lo(w[e]);
-    v[2 * e + 1] = bf16_hi(w[e]);
-  }
-}
+__device__ __forceinline__ uint32_t ld_b32(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
+__device__ __forceinline__ void st_b32(__nv_bfloat16* p, uint32_t v) { *reinterpret_cast<uint32_t*>(p) = v; }
+
 __device__ __forceinline__ void pack16(const float v[16], uint32_t w[8]) {
 #pragma unroll
   for (int e = 0; e < 8; ++e) w[e] = pack_bf16x2(v[2 * e], v[2 * e + 1]);
 }
 
+template <int BN>
+__device__ __forceinline__ void wgmma_bn(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (BN == 256) wgmma_m64n256k16<0, 0>(acc, da, db, accumulate);
+  if constexpr (BN == 128) wgmma_m64n128k16<0, 0>(acc, da, db, accumulate);
+  if constexpr (BN == 64) wgmma_m64n64k16<0, 0>(acc, da, db, accumulate);
+  if constexpr (BN == 16) wgmma_m64n16k16<0, 0>(acc, da, db, accumulate);
+}
+
+// Fragment coordinates of a consumer thread: rows m0 and m0 + 8 of the 128-row tile (register bit 1), columns
+// 8 (i >> 2) + 2 cq + (i & 1).
+struct Frag {
+  int m0, cq;
+};
+
 // ---- EPI_FWD: gates, cell update, h_t (SURVEY App. A.1; rnn_point_estimate.py:80-87) ----------------------------
-// Accumulator columns of a tile: [16-unit block][gate i|f|g|o][16] (the packed order of the B operand rows).
-template <int BN, bool ACC>
-__device__ __forceinline__ void epi_fwd(const EpiParams& p, uint32_t tmem, int q, int lane, int rt, const float* bias_s) {
-  const int m = q * 32 + lane;
-  const long b = (long)rt * 128 + m;
-  const bool valid = b < p.B;
-  const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-  constexpr int U = BN / 4;                         // hidden units of this tile
-  const int unit0 = blockIdx.y * U;
-  // c_{t-1} of the NEXT block is kept in flight while the current one is worked on (an L2 round trip per block otherwise)
-  float cnext[16];
-  const long cs_blk = 4L * 32 * 16;                 // cstate elements per 16-unit block
-  float* cs0 = p.cstate + ((((long)rt * p.NB16 + (unit0 >> 4)) * 4 + q) * 32 + lane) * 16;
-  if (p.t > 0) {
-    ld_global_v8f(cs0, cnext);
-    ld_global_v8f(cs0 + 8, cnext + 8);
-  } else {
+// Accumulator columns of a tile: [16-unit block][gate i|f|g|o][16] (the packed order of the B operand rows).  Gate g of
+// unit jj = 8 q + 2 cq + e of block blk is register 32 blk + 4 (2 g + q) + 2 h + e.
+template <bool ACC>
+__device__ __forceinline__ void epi_fwd(const EpiParams& p, const float (&acc)[128], Frag f, int rt, int by,
+                                        const float* bias_s) {
+  constexpr int U = 64;                             // hidden units of this tile
+  const int unit0 = by * U;
 #pragma unroll
-    for (int j = 0; j < 16; ++j) cnext[j] = 0.f;
-  }
-#pragma unroll 1
-  for (int blk = 0; blk < U / 16; ++blk) {
-    const int j0 = unit0 + blk * 16;
-    const int gblk = j0 >> 4;
-    uint32_t vi[16], vf[16], vg[16], vo[16];
-    const uint32_t ta = tmem + lane_addr + blk * 64;
-    tmem_ld_32x32b_x16(ta + 0, vi);
-    tmem_ld_32x32b_x16(ta + 16, vf);
-    tmem_ld_32x32b_x16(ta + 32, vg);
-    tmem_ld_32x32b_x16(ta + 48, vo);
-    float cprev[16];
-    float* cs = cs0 + blk * cs_blk;
+  for (int h = 0; h < 2; ++h) {
+    const int m = f.m0 + 8 * h;
+    const long b = (long)rt * 128 + m;
+    const bool valid = b < p.B;
 #pragma unroll
-    for (int j = 0; j < 16; ++j) cprev[j] = cnext[j];
-    if (p.t > 0 && blk + 1 < U / 16) {
-      ld_global_v8f(cs + cs_blk, cnext);
-      ld_global_v8f(cs + cs_blk + 8, cnext + 8);
-    }
-    tmem_ld_wait();
-    const float* bs = bias_s + blk * 64;          // this tile's packed bias, staged in shared memory (broadcast reads)
-    float gi[16], gf[16], gg[16], go[16], cn[16], hv[16];
+    for (int blk = 0; blk < U / 16; ++blk) {
+      const int gblk = (unit0 >> 4) + blk;
+      float* cs = p.cstate + ((((long)rt * p.NB16 + gblk) * 4 + (m >> 5)) * 32 + (m & 31)) * 16;
+      const float* bs = bias_s + blk * 64;        // this tile's packed bias, staged in shared memory (broadcast reads)
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const float zi = __uint_as_float(vi[j]) + bs[j];
-      const float zf = __uint_as_float(vf[j]) + bs[16 + j];
-      const float zg = __uint_as_float(vg[j]) + bs[32 + j];
-      const float zo = __uint_as_float(vo[j]) + bs[48 + j];
-      if (ACC) {
-        gi[j] = sigmoid_acc(zi); gf[j] = sigmoid_acc(zf); gg[j] = tanhf(zg); go[j] = sigmoid_acc(zo);
-      } else {      // sigmoid(z) = 0.5 tanh(z/2) + 0.5; the 1/2 is folded into the packed weights and bias
-        gi[j] = fmaf(0.5f, tanh_approx(zi), 0.5f);
-        gf[j] = fmaf(0.5f, tanh_approx(zf), 0.5f);
-        gg[j] = tanh_approx(zg);
-        go[j] = fmaf(0.5f, tanh_approx(zo), 0.5f);
-      }
-      cn[j] = fmaf(gf[j], cprev[j], gi[j] * gg[j]);
-      hv[j] = go[j] * (ACC ? tanhf(cn[j]) : tanh_approx(cn[j]));
-    }
-    st_global_v8f(cs, cn);
-    st_global_v8f(cs + 8, cn + 8);
-    if (valid) {
-      const long hoff = ((long)(p.t + 1) * p.Bp + b) * p.H + j0;
-      uint32_t w[8];
-      pack16(hv, w);
-      st_global_v8(p.hseq + hoff, w);
-      if (p.hseq_lo) {        // bf16x3: h = hi + lo with |lo| <= 2^-9 |h|
-        float lo[16];
+      for (int q = 0; q < 2; ++q) {
+        const int jj = 8 * q + 2 * f.cq;
+        const int j = unit0 + blk * 16 + jj;
+        const float2 cprev = p.t > 0 ? *reinterpret_cast<const float2*>(cs + jj) : make_float2(0.f, 0.f);
+        float gv[4][2], cn[2], hv[2];
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          lo[2 * e] = hv[2 * e] - bf16_lo(w[e]);
-          lo[2 * e + 1] = hv[2 * e + 1] - bf16_hi(w[e]);
+        for (int e = 0; e < 2; ++e) {
+          const int ri = 32 * blk + 4 * q + 2 * h + e;
+          const float zi = acc[ri] + bs[jj + e];
+          const float zf = acc[ri + 8] + bs[16 + jj + e];
+          const float zg = acc[ri + 16] + bs[32 + jj + e];
+          const float zo = acc[ri + 24] + bs[48 + jj + e];
+          float gi, gf, gg, go;
+          if (ACC) {
+            gi = sigmoid_acc(zi); gf = sigmoid_acc(zf); gg = tanhf(zg); go = sigmoid_acc(zo);
+          } else {      // sigmoid(z) = 0.5 tanh(z/2) + 0.5; the 1/2 is folded into the packed weights and bias
+            gi = fmaf(0.5f, tanh_approx(zi), 0.5f);
+            gf = fmaf(0.5f, tanh_approx(zf), 0.5f);
+            gg = tanh_approx(zg);
+            go = fmaf(0.5f, tanh_approx(zo), 0.5f);
+          }
+          cn[e] = fmaf(gf, e ? cprev.y : cprev.x, gi * gg);
+          hv[e] = go * (ACC ? tanhf(cn[e]) : tanh_approx(cn[e]));
+          gv[0][e] = gi; gv[1][e] = gf; gv[2][e] = gg; gv[3][e] = go;
         }
-        uint32_t wl[8];
-        pack16(lo, wl);
-        st_global_v8(p.hseq_lo + hoff, wl);
-      }
-      if (p.hmseq) {
-        float mk[16];
-        rec_mask16(p.rkey, p.row0 + b, p.H, j0, mk);
+        *reinterpret_cast<float2*>(cs + jj) = make_float2(cn[0], cn[1]);
+        if (valid) {
+          const long hoff = ((long)(p.t + 1) * p.Bp + b) * p.H + j;
+          const uint32_t w = pack_bf16x2(hv[0], hv[1]);
+          st_b32(p.hseq + hoff, w);
+          if (p.hseq_lo)        // bf16x3: h = hi + lo with |lo| <= 2^-9 |h|
+            st_b32(p.hseq_lo + hoff, pack_bf16x2(hv[0] - bf16_lo(w), hv[1] - bf16_hi(w)));
+          if (p.hmseq) {
+            float mk[4];
+            rec_mask4(p.rkey, p.row0 + b, p.H, j, mk);
+            st_b32(p.hmseq + hoff, pack_bf16x2(mk[j & 3] * hv[0], mk[(j & 3) + 1] * hv[1]));
+          }
+          if (p.gates) {
+            const long sb = (((long)p.t * p.NRT + rt) * p.NB16 + gblk);
+            __nv_bfloat16* gp = p.gates + (((sb * 4 + 0) * 4 + (m >> 5)) * 32 + (m & 31)) * 16 + jj;
+            const long gstride = 4L * 32 * 16;           // between gates
 #pragma unroll
-        for (int j = 0; j < 16; ++j) mk[j] *= hv[j];
-        uint32_t wm[8];
-        pack16(mk, wm);
-        st_global_v8(p.hmseq + hoff, wm);
-      }
-      if (p.gates) {
-        const long sb = (((long)p.t * p.NRT + rt) * p.NB16 + gblk);
-        __nv_bfloat16* gp = p.gates + (((sb * 4 + 0) * 4 + q) * 32 + lane) * 16;
-        const long gstride = 4L * 32 * 16;           // between gates
-        pack16(gi, w); st_global_v8(gp, w);
-        pack16(gf, w); st_global_v8(gp + gstride, w);
-        pack16(gg, w); st_global_v8(gp + 2 * gstride, w);
-        pack16(go, w); st_global_v8(gp + 3 * gstride, w);
-        pack16(cn, w);
-        st_global_v8(p.cst + ((sb * 4 + q) * 32 + lane) * 16, w);
+            for (int g = 0; g < 4; ++g) st_b32(gp + g * gstride, pack_bf16x2(gv[g][0], gv[g][1]));
+            st_b32(p.cst + ((sb * 4 + (m >> 5)) * 32 + (m & 31)) * 16 + jj, pack_bf16x2(cn[0], cn[1]));
+          }
+        }
       }
     }
   }
@@ -291,177 +258,117 @@ __device__ __forceinline__ void epi_fwd(const EpiParams& p, uint32_t tmem, int q
 
 // ---- EPI_BWD: BPTT pointwise algebra of step t (SURVEY App. A.4) ----------------------------------------------
 // Accumulator columns: hidden units unit0 .. unit0+BN-1 in order (rec = dz_{t+1} U^T, before the recurrent mask).
-// The saved gates / cell states come from HBM (~1.5 K cycles per dependent load): each warp keeps the operands of its
-// NEXT 16-unit block in flight while it works on the current one, and `ew` warps per lane quadrant split the blocks
-// (profiles/r02_summary.md: the serial version spent 22 K of a step's 40 K cycles here).
-struct BwdOps {
-  uint32_t wi[8], wf[8], wg[8], wo[8], wc[8], wcp[8], wd[8];
-};
-
-__device__ __forceinline__ void bwd_load_ops(const EpiParams& p, int rt, int q, int lane, long b, bool valid, int j0,
-                                             BwdOps& o) {
-  if (!valid) {        // rows beyond the batch take part in the warp-collective TMEM loads but touch no memory
-#pragma unroll
-    for (int e = 0; e < 8; ++e) o.wi[e] = o.wf[e] = o.wg[e] = o.wo[e] = o.wc[e] = o.wcp[e] = o.wd[e] = 0u;
-    return;
-  }
-  const int gblk = j0 >> 4;
+// Every thread handles its fragment's pairs of adjacent units: two per packed bf16x2 word of the saved state.
+template <int BN>
+__device__ __forceinline__ void epi_bwd(const EpiParams& p, const float (&acc)[BN / 2], Frag f, int rt, int by) {
+  const int unit0 = by * BN;
   const long gstride = 4L * 32 * 16;
   const long tstride_c = (long)p.NRT * p.NB16 * 4 * 32 * 16;     // cst elements per time step
-  const long sb = (((long)p.t * p.NRT + rt) * p.NB16 + gblk);
-  const __nv_bfloat16* gp = p.gates + (((sb * 4 + 0) * 4 + q) * 32 + lane) * 16;
-  const __nv_bfloat16* cp_ = p.cst + ((sb * 4 + q) * 32 + lane) * 16;
-  ld_global_v8(gp, o.wi);
-  ld_global_v8(gp + gstride, o.wf);
-  ld_global_v8(gp + 2 * gstride, o.wg);
-  ld_global_v8(gp + 3 * gstride, o.wo);
-  ld_global_v8(cp_, o.wc);
-  if (p.t > 0) {
-    ld_global_v8(cp_ - tstride_c, o.wcp);
-  } else {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) o.wcp[e] = 0u;
-  }
-  ld_global_v8(p.dhout + ((long)p.t * p.Bp + b) * p.H + j0, o.wd);
-}
-
-// (A prefetch.global.L2 of the next block's operands one block ahead was measured too: 2.635 -> 2.652 ms, dropped.)
-__device__ __forceinline__ void bwd_block(const EpiParams& p, uint32_t tmem_blk, int rt, int q, int lane, long b, bool valid,
-                                          int j0, const BwdOps& o) {
-  const int gblk = j0 >> 4;
-  float* dcs = p.dcstate + ((((long)rt * p.NB16 + gblk) * 4 + q) * 32 + lane) * 16;
-  float dcc[16];
-  if (p.t < p.T - 1 && valid) {
-    ld_global_v8f(dcs, dcc);
-    ld_global_v8f(dcs + 8, dcc + 8);
-  } else {
+  for (int h = 0; h < 2; ++h) {
+    const int m = f.m0 + 8 * h;
+    const long b = (long)rt * 128 + m;
+    const bool valid = b < p.B;
+    const int q = m >> 5, ln = m & 31;
+    __nv_bfloat16* dzr = p.dz + ((long)p.t * p.Bp + b) * 4 * p.H;
 #pragma unroll
-    for (int j = 0; j < 16; ++j) dcc[j] = 0.f;
-  }
-  float rec[16];
-  if (p.has_rec) {
-    uint32_t vr[16];
-    tmem_ld_32x32b_x16(tmem_blk, vr);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) rec[j] = __uint_as_float(vr[j]);
-    if (p.use_rec) {
-      float mk[16];
-      rec_mask16(p.rkey, p.row0 + b, p.H, j0, mk);
-#pragma unroll
-      for (int j = 0; j < 16; ++j) rec[j] *= mk[j];
+    for (int J = 0; J < BN / 8; ++J) {
+      const int j = unit0 + 8 * J + 2 * f.cq;
+      const int gblk = j >> 4, jj = j & 15;
+      float* dcs = p.dcstate + ((((long)rt * p.NB16 + gblk) * 4 + q) * 32 + ln) * 16 + jj;
+      uint32_t i2 = 0, f2 = 0, g2 = 0, o2 = 0, c2 = 0, cp2 = 0, d2 = 0;
+      float2 dcc = make_float2(0.f, 0.f);
+      if (valid) {        // rows beyond the batch load nothing and store zero dz
+        const long sb = (((long)p.t * p.NRT + rt) * p.NB16 + gblk);
+        const __nv_bfloat16* gp = p.gates + (((sb * 4 + 0) * 4 + q) * 32 + ln) * 16 + jj;
+        const __nv_bfloat16* cp_ = p.cst + ((sb * 4 + q) * 32 + ln) * 16 + jj;
+        i2 = ld_b32(gp);
+        f2 = ld_b32(gp + gstride);
+        g2 = ld_b32(gp + 2 * gstride);
+        o2 = ld_b32(gp + 3 * gstride);
+        c2 = ld_b32(cp_);
+        cp2 = p.t > 0 ? ld_b32(cp_ - tstride_c) : 0u;
+        d2 = ld_b32(p.dhout + ((long)p.t * p.Bp + b) * p.H + j);
+        if (p.t < p.T - 1) dcc = *reinterpret_cast<const float2*>(dcs);
+      }
+      float rec0 = 0.f, rec1 = 0.f;
+      if (p.has_rec) {
+        rec0 = acc[4 * J + 2 * h];
+        rec1 = acc[4 * J + 2 * h + 1];
+        if (p.use_rec) {
+          float mk[4];
+          rec_mask4(p.rkey, p.row0 + b, p.H, j, mk);
+          rec0 *= mk[j & 3];
+          rec1 *= mk[(j & 3) + 1];
+        }
+      }
+      // Gate-gradient algebra in packed bf16x2 (all operands arrive packed, dz leaves packed); only the carried
+      // dLoss/dc stays in fp32.  SURVEY App. A.4.
+      const uint32_t dh2 = add_bf16x2(d2, pack_bf16x2(rec0, rec1));
+      const uint32_t tc2 = tanh_bf16x2(c2);
+      const uint32_t omtc2 = fma_bf16x2(neg_bf16x2(tc2), tc2, BF16X2_ONE);        // 1 - tanh(c)^2
+      const uint32_t t1 = mul_bf16x2(mul_bf16x2(dh2, o2), omtc2);                 // dh * o * (1 - tc^2)
+      const float dcn0 = dcc.x + bf16_lo(t1);
+      const float dcn1 = dcc.y + bf16_hi(t1);
+      const uint32_t dcn2 = pack_bf16x2(dcn0, dcn1);
+      const uint32_t omi = fma_bf16x2(neg_bf16x2(i2), i2, i2);                    // i (1 - i)
+      const uint32_t omf = fma_bf16x2(neg_bf16x2(f2), f2, f2);                    // f (1 - f)
+      const uint32_t omg = fma_bf16x2(neg_bf16x2(g2), g2, BF16X2_ONE);            // 1 - g^2
+      const uint32_t omo = fma_bf16x2(neg_bf16x2(o2), o2, o2);                    // o (1 - o)
+      uint32_t zi = mul_bf16x2(dcn2, mul_bf16x2(g2, omi));
+      uint32_t zf = mul_bf16x2(dcn2, mul_bf16x2(cp2, omf));
+      uint32_t zg = mul_bf16x2(dcn2, mul_bf16x2(i2, omg));
+      uint32_t zo = mul_bf16x2(mul_bf16x2(dh2, tc2), omo);
+      if (valid) {
+        *reinterpret_cast<float2*>(dcs) = make_float2(dcn0 * bf16_lo(f2), dcn1 * bf16_hi(f2));
+      } else {          // rows beyond the batch: dz exactly zero (the weight-gradient GEMM sums over all rows)
+        zi = zf = zg = zo = 0u;
+      }
+      st_b32(dzr + j, zi);
+      st_b32(dzr + p.H + j, zf);
+      st_b32(dzr + 2L * p.H + j, zg);
+      st_b32(dzr + 3L * p.H + j, zo);
     }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) rec[j] = 0.f;
-  }
-  __nv_bfloat16* dzr = p.dz + ((long)p.t * p.Bp + b) * 4 * p.H + j0;
-  // Gate-gradient algebra in packed bf16x2 (all operands arrive packed, dz leaves packed; a third of the instructions of
-  // the fp32 form, which made this epilogue issue-bound); only the carried dLoss/dc stays in fp32.  SURVEY App. A.4.
-  uint32_t zi[8], zf[8], zg[8], zo[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {          // two units per packed word
-    const uint32_t i2 = o.wi[e], f2 = o.wf[e], g2 = o.wg[e], o2 = o.wo[e];
-    const uint32_t dh2 = add_bf16x2(o.wd[e], pack_bf16x2(rec[2 * e], rec[2 * e + 1]));
-    const uint32_t tc2 = tanh_bf16x2(o.wc[e]);
-    const uint32_t omtc2 = fma_bf16x2(neg_bf16x2(tc2), tc2, BF16X2_ONE);        // 1 - tanh(c)^2
-    const uint32_t t1 = mul_bf16x2(mul_bf16x2(dh2, o2), omtc2);                 // dh * o * (1 - tc^2)
-    const float dcn0 = dcc[2 * e] + bf16_lo(t1);
-    const float dcn1 = dcc[2 * e + 1] + bf16_hi(t1);
-    dcc[2 * e] = dcn0 * bf16_lo(f2);
-    dcc[2 * e + 1] = dcn1 * bf16_hi(f2);
-    const uint32_t dcn2 = pack_bf16x2(dcn0, dcn1);
-    const uint32_t omi = fma_bf16x2(neg_bf16x2(i2), i2, i2);                    // i (1 - i)
-    const uint32_t omf = fma_bf16x2(neg_bf16x2(f2), f2, f2);                    // f (1 - f)
-    const uint32_t omg = fma_bf16x2(neg_bf16x2(g2), g2, BF16X2_ONE);            // 1 - g^2
-    const uint32_t omo = fma_bf16x2(neg_bf16x2(o2), o2, o2);                    // o (1 - o)
-    zi[e] = mul_bf16x2(dcn2, mul_bf16x2(g2, omi));
-    zf[e] = mul_bf16x2(dcn2, mul_bf16x2(o.wcp[e], omf));
-    zg[e] = mul_bf16x2(dcn2, mul_bf16x2(i2, omg));
-    zo[e] = mul_bf16x2(mul_bf16x2(dh2, tc2), omo);
-  }
-  if (valid) {
-    st_global_v8f(dcs, dcc);
-    st_global_v8f(dcs + 8, dcc + 8);
-  } else {             // rows beyond the batch: dz exactly zero (the weight-gradient GEMM sums over all rows)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) zi[e] = zf[e] = zg[e] = zo[e] = 0u;
-  }
-  // (row-major 32-byte pieces, one line per lane: a store-free timing run put their cost at up to 0.44 ms per train step of
-  //  BASELINE configs[2], profiles/r02_summary.md c27; they stay row-major because dz is a TMA-loaded GEMM operand)
-  st_global_v8(dzr, zi);
-  st_global_v8(dzr + (long)p.H, zf);
-  st_global_v8(dzr + 2L * p.H, zg);
-  st_global_v8(dzr + 3L * p.H, zo);
-}
-
-// `part` of `nparts` warps of this lane quadrant: blocks part, part + nparts, ...
-template <int BN>
-__device__ __forceinline__ void epi_bwd(const EpiParams& p, uint32_t tmem, int q, int lane, int rt, int part, int nparts) {
-  const int m = q * 32 + lane;
-  const long b = (long)rt * 128 + m;
-  const bool valid = b < p.B;
-  const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-  const int unit0 = blockIdx.y * BN;
-  constexpr int NB = BN / 16;
-  // tcgen05.ld is warp-collective (.sync.aligned): every lane of the warp runs the block loop, also those whose row lies
-  // beyond the batch (a ragged last tile) -- they load nothing and store zeros.  (An early return of those lanes hung
-  // the kernel, profiles/r02_summary.md.)
-  // One block at a time, all of its nine loads issued together.  (Keeping the next block's operands in flight as well
-  // needs 2 x 56 registers: at the 168-register cap of a 320-thread CTA that spilled ~100 values per block, and with
-  // 198 KB of shared memory in use the L1 that would catch the spills is ~30 KB -- the epilogue took 25 K cycles whatever
-  // the arithmetic looked like, profiles/r02_summary.md.)
-  BwdOps A;
-#pragma unroll 1
-  for (int blk = part; blk < NB; blk += nparts) {
-    bwd_load_ops(p, rt, q, lane, b, valid, unit0 + blk * 16, A);
-    bwd_block(p, tmem + lane_addr + blk * 16, rt, q, lane, b, valid, unit0 + blk * 16, A);
   }
 }
 
 // ---- EPI_STORE: accumulator -> bf16 row-major ---------------------------------------------------------------------
 template <int BN>
-__device__ __forceinline__ void epi_store(const EpiParams& p, uint32_t tmem, int q, int lane, long row, int by) {
-  const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-  __nv_bfloat16* o = p.out + row * p.ldc + (long)by * BN;
-#pragma unroll 1
-  for (int c0 = 0; c0 < BN; c0 += 32) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(tmem + lane_addr + c0, v);
-    tmem_ld_wait();
-    uint32_t w[16];
+__device__ __forceinline__ void epi_store(const EpiParams& p, const float (&acc)[BN / 2], Frag f, long row0, int by) {
 #pragma unroll
-    for (int e = 0; e < 16; ++e) w[e] = pack_bf16x2(__uint_as_float(v[2 * e]), __uint_as_float(v[2 * e + 1]));
-    st_global_v8(o + c0, w);
-    st_global_v8(o + c0 + 16, w + 8);
+  for (int h = 0; h < 2; ++h) {
+    __nv_bfloat16* o = p.out + (row0 + f.m0 + 8 * h) * p.ldc + (long)by * BN + 2 * f.cq;
+#pragma unroll
+    for (int J = 0; J < BN / 8; ++J) st_b32(o + 8 * J, pack_bf16x2(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]));
   }
 }
 
 // ---- EPI_HEAD: Dense + weighted MSE + dLoss/dpred on the accumulator of pred = y Wo (N = 16) ---------------------------
-// One CTA = one 128-row tile (t, rt) of the time-major head input; thread = row.  (rnn_point_estimate.py:105;
-// model_utils/losses.py:55-135; SURVEY App. A.3)
+// One CTA = one 128-row tile (t, rt) of the time-major head input; the accumulator is staged in shared memory so that
+// threads 0..127 own one row each.  (rnn_point_estimate.py:105; model_utils/losses.py:55-135; SURVEY App. A.3)
 constexpr int GH_O = 16;
 constexpr int GH_PART = GH_O + 4;      // dbo | s0 s1 s2
-__device__ __forceinline__ void epi_head(const EpiParams& p, uint32_t tmem, int q, int lane, float* red_s) {
+__device__ __forceinline__ void epi_head(const EpiParams& p, const float (&acc)[8], Frag f, float* rows_s, float* red_s) {
+  const int tid = threadIdx.x, lane = tid & 31;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) rows_s[(f.m0 + 8 * ((i >> 1) & 1)) * 17 + 8 * (i >> 2) + 2 * f.cq + (i & 1)] = acc[i];
+  if (tid < GH_PART) red_s[tid] = 0.f;
+  named_bar_sync(1, 256);
+  if (tid >= 128) return;
   const int tile = blockIdx.x;
   const int t = tile / p.NRT, rt = tile % p.NRT;
-  const int m = q * 32 + lane;
+  const int m = tid;
   const long b = (long)rt * 128 + m;
   const bool valid = b < p.B;
-  if (m < GH_PART) red_s[m] = 0.f;
-  named_bar_sync(1, 128);
-  uint32_t v[16];
-  tmem_ld_32x32b_x16(tmem + ((uint32_t)(q * 32) << 16), v);
   const long r = b * p.T + t;          // row of the caller's [B][T][O] tensors
   float yt[GH_O];
 #pragma unroll
   for (int k = 0; k < GH_O; ++k) yt[k] = 0.f;
   if (p.hy && valid)
     for (int k = 0; k < p.hO; ++k) yt[k] = p.hy[r * p.hO + k];
-  tmem_ld_wait();
   float pr[GH_O];
 #pragma unroll
-  for (int k = 0; k < GH_O; ++k) pr[k] = (k < p.hO) ? __uint_as_float(v[k]) + __ldg(p.hbo + k) : 0.f;
+  for (int k = 0; k < GH_O; ++k) pr[k] = (k < p.hO) ? rows_s[m * 17 + k] + __ldg(p.hbo + k) : 0.f;
   if (p.hpreds && valid)
     for (int k = 0; k < p.hO; ++k) p.hpreds[r * p.hO + k] = pr[k];
   if (!p.hy) return;
@@ -497,7 +404,8 @@ __device__ __forceinline__ void epi_head(const EpiParams& p, uint32_t tmem, int 
   }
   if (p.htrain) {       // every row of the tile is written (zeros beyond the batch): the dy / dWo GEMMs run over all rows
     uint32_t w[8];
-    pack16(dp, w);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) w[e] = pack_bf16x2(dp[2 * e], dp[2 * e + 1]);
     st_global_v8(p.hdpb + ((long)t * p.Bp + b) * 64, w);
   }
   s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
@@ -510,26 +418,22 @@ __device__ __forceinline__ void epi_head(const EpiParams& p, uint32_t tmem, int 
     if (p.htrain)
       for (int k = 0; k < GH_O; ++k) atomicAdd(&red_s[k], dp[k]);
   }
-  named_bar_sync(1, 128);
+  named_bar_sync(2, 128);
   if (m < GH_PART) p.hpartial[(long)m * gridDim.x + blockIdx.x] = red_s[m];
 }
 
-template <int BN, int EPI, int MT>
-__global__ void __launch_bounds__(GSmem<BN, MT, EPI>::THREADS, GSmem<BN, MT, EPI>::CTAS_PER_SM)
+template <int BN, int EPI>
+__global__ void __launch_bounds__(GSmem<BN, EPI>::THREADS, GSmem<BN, EPI>::CTAS_PER_SM)
     tile_gemm_kernel(GArgs g, EpiParams ep, const __grid_constant__ CUtensorMap tmA0,
                      const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
                      const __grid_constant__ CUtensorMap tmA3, const __grid_constant__ CUtensorMap tmB0,
                      const __grid_constant__ CUtensorMap tmB1) {
-  using S = GSmem<BN, MT, EPI>;
+  using S = GSmem<BN, EPI>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::BARS);
   uint64_t* empty = full + S::NS;
-  uint64_t* acc_full = empty + S::NS;
-  uint64_t* tmem_free = acc_full + 1;               // persistent mode: the epilogue has drained the accumulator
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(tmem_free + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  constexpr uint32_t TMEM_COLS = (BN * MT < 32) ? 32 : BN * MT;
   __shared__ float red_s[EPI == EPI_HEAD ? GH_PART : 1];
   __shared__ float bias_s[(EPI == EPI_FWD || EPI == EPI_FWD_ACC) ? BN : 1];
   if constexpr (EPI == EPI_FWD || EPI == EPI_FWD_ACC)
@@ -541,35 +445,27 @@ __global__ void __launch_bounds__(GSmem<BN, MT, EPI>::THREADS, GSmem<BN, MT, EPI
   if (tid == 0) {
     for (int s = 0; s < S::NS; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);               // one arrive per consumer warp
     }
-    mbar_init(acc_full, 1);
-    mbar_init(tmem_free, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_s, TMEM_COLS);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tmem_base_s;
   const int bx = g.lin_cols > 0 ? (int)blockIdx.x / g.lin_cols : (int)blockIdx.x;      // row-tile / column-tile coordinates
   const int by = g.lin_cols > 0 ? (int)blockIdx.x % g.lin_cols : (int)blockIdx.y;
-  const bool tr = ep.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0;
-  if (tr && tid == 0) ep.trace[0] = clock64();
 
   // Programmatic dependent launch (the recurrence steps are launched with the stream-serialization attribute): this
-  // kernel's CTAs are dispatched while the previous step's grid drains.  Everything above (barriers, TMEM) and the B
+  // kernel's CTAs are dispatched while the previous step's grid drains.  Everything above (barriers) and the B
   // operand (weights: packed long before the previous step) of the first ring stages is independent of it; the A
   // operand and every state the epilogue reads were written by the previous step, so all threads wait here first.
   // launch_dependents comes AFTER the wait: when the next grid starts, this one has seen its predecessor complete, so
   // by induction only the immediate predecessor can still be running.
   const int n_steps = g.n_steps > 1 ? g.n_steps : 1;
   const unsigned int n_cta = gridDim.y;             // CTAs of this row-tile group
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       const int brow = g.b_row_base + BN * by;
       for (int it = 0; it < n_steps; ++it) {
-        const int arow = g.a_row_base + it * g.row_step + 128 * (MT * bx + g.rt_off);
+        const int arow = g.a_row_base + it * g.row_step + 128 * (bx + g.rt_off);
         const int gi0 = it * total_kb;               // ring position of this step's first k-block
         {   // B operand (weights) of the first NS stages of the step, before the dependency wait
           int i = 0;
@@ -584,12 +480,9 @@ __global__ void __launch_bounds__(GSmem<BN, MT, EPI>::THREADS, GSmem<BN, MT, EPI
             }
           }
         }
-        long long* trc = tr ? ep.trace + (long)it * g.t_step * 8 : nullptr;     // trace entries are [t][8]
-        if (trc && it > 0) trc[0] = clock64();
         if (it == 0) {
           griddep_wait();
           griddep_launch_dependents();
-          if (trc) trc[1] = clock64();
         } else {
           // every CTA of the row-tile group has published step it-1 (generic-proxy stores, fenced before the count went up)
           const long long spin0 = clock64();
@@ -599,7 +492,6 @@ __global__ void __launch_bounds__(GSmem<BN, MT, EPI>::THREADS, GSmem<BN, MT, EPI
             if (clock64() - spin0 > 4000000000LL) __trap();
           }
           fence_proxy_async_global();
-          if (trc) trc[1] = clock64();
         }
         int i = 0;
         for (int sg = 0; sg < g.n_seg; ++sg) {
@@ -614,9 +506,7 @@ __global__ void __launch_bounds__(GSmem<BN, MT, EPI>::THREADS, GSmem<BN, MT, EPI
               mbar_arrive_expect_tx(&full[s], S::STAGE);
               tma_load_2d(st + S::A_BYTES, mb, &full[s], sgm.b_col0 + kb * 64, brow);
             }
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt)
-              tma_load_2d(st + mt * 16384, ma, &full[s], sgm.a_col0 + kb * 64, arow + 128 * mt);
+            tma_load_2d(st, ma, &full[s], sgm.a_col0 + kb * 64, arow);
           }
         }
       }
@@ -624,84 +514,53 @@ __global__ void __launch_bounds__(GSmem<BN, MT, EPI>::THREADS, GSmem<BN, MT, EPI
       griddep_wait();
       griddep_launch_dependents();
     }
-  } else if (warp == 1) {
+  } else if (warp < 8) {
     griddep_wait();
     griddep_launch_dependents();
-    if (lane == 0 && total_kb > 0) {
-      const uint32_t idesc = make_idesc_bf16(128, BN, false, false);
-      for (int it = 0; it < n_steps; ++it) {
-        if (it > 0) {                          // the epilogue of the previous step has read the accumulator
-          mbar_wait(tmem_free, (it - 1) & 1);
-          tcgen05_fence_after();
-        }
-        for (int i = 0; i < total_kb; ++i) {
-          const int gi = it * total_kb + i, s = gi % S::NS;
-          mbar_wait(&full[s], (gi / S::NS) & 1);
-          if (tr && i == 0) ep.trace[(long)it * g.t_step * 8 + 2] = clock64();
-          tcgen05_fence_after();
-          uint8_t* st = smem + s * S::STAGE;
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            const uint64_t db = make_smem_desc(smem_u32(st + S::A_BYTES) + k16 * 32, 0, 1024, LAYOUT_SW128);
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt) {
-              const uint64_t da = make_smem_desc(smem_u32(st + mt * 16384) + k16 * 32, 0, 1024, LAYOUT_SW128);
-              umma_f16(tmem + mt * BN, da, db, idesc, (i | k16) != 0);
-            }
-          }
-          umma_commit(&empty[s]);
-        }
-        umma_commit(acc_full);
-        if (tr) ep.trace[(long)it * g.t_step * 8 + 3] = clock64();
-      }
-    }
-  } else {
-    griddep_wait();
-    griddep_launch_dependents();
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;                 // group of four warps = one pass over the four TMEM lane quadrants
-    const int mt = grp / S::EW;                      // which 128-row M tile of the CTA this group works on
-    const int part = grp % S::EW;                    // ... and which share of its column blocks
-    const int rt = MT * bx + mt + g.rt_off;        // 128-row tile index
-    // (An L2 prefetch of the epilogue's saved-state operands issued here, during the mainloop, was measured and lost:
-    //  it delays the operand ring -- first stage 1.5 K -> 3 K cycles -- and the epilogue, which is issue-bound, not
-    //  HBM-bound, got no shorter: 2.97 -> 3.25 ms for the backward steps of BASELINE configs[2].)
-    const uint32_t tacc = tmem + mt * BN;
+    const int wg = warp >> 2;
+    const Frag f{64 * wg + 16 * (warp & 3) + (lane >> 2), lane & 3};
+    const int rt = bx + g.rt_off;                    // 128-row tile index
     const int t_first = ep.t;
+    float acc[BN / 2];
     for (int it = 0; it < n_steps; ++it) {
       ep.t = t_first + it * g.t_step;
-      if (total_kb > 0) {
-        mbar_wait(acc_full, it & 1);
-        tcgen05_fence_after();
+      for (int i = 0; i < total_kb; ++i) {
+        const int gi = it * total_kb + i, s = gi % S::NS;
+        mbar_wait(&full[s], (gi / S::NS) & 1);
+        uint8_t* st = smem + s * S::STAGE;
+        wgmma_fence();
+#pragma unroll
+        for (int k16 = 0; k16 < 4; ++k16) {
+          const uint64_t db = make_smem_desc(smem_u32(st + S::A_BYTES) + k16 * 32, 0, 1024, LAYOUT_SW128);
+          const uint64_t da = make_smem_desc(smem_u32(st + wg * 8192) + k16 * 32, 0, 1024, LAYOUT_SW128);
+          wgmma_bn<BN>(acc, da, db, (i | k16) != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                             // the previous stage's MMAs are complete: release it
+        if (i > 0 && lane == 0) mbar_arrive(&empty[(gi - 1) % S::NS]);
       }
-      if (tr && warp == 2 && lane == 0) ep.trace[(long)it * g.t_step * 8 + 4] = clock64();
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (total_kb > 0 && lane == 0) mbar_arrive(&empty[(it * total_kb + total_kb - 1) % S::NS]);
       if constexpr (EPI == EPI_HEAD) {
-        epi_head(ep, tacc, q, lane, red_s);
-      } else if ((long)rt * 128 < ep.Bp || EPI == EPI_STORE) {      // (a 256-row CTA tile may hang over the last row tile)
-        if constexpr (EPI == EPI_FWD) epi_fwd<BN, false>(ep, tacc, q, lane, rt, bias_s);
-        if constexpr (EPI == EPI_FWD_ACC) epi_fwd<BN, true>(ep, tacc, q, lane, rt, bias_s);
-        if constexpr (EPI == EPI_BWD) epi_bwd<BN>(ep, tacc, q, lane, rt, part, S::EW);
-        if constexpr (EPI == EPI_STORE) epi_store<BN>(ep, tacc, q, lane, (long)g.a_row_base + 128L * rt + q * 32 + lane, by);
+        epi_head(ep, acc, f, reinterpret_cast<float*>(smem + S::HEAD_ROWS), red_s);
+      } else if ((long)rt * 128 < ep.Bp || EPI == EPI_STORE) {
+        if constexpr (EPI == EPI_FWD) epi_fwd<false>(ep, acc, f, rt, by, bias_s);
+        if constexpr (EPI == EPI_FWD_ACC) epi_fwd<true>(ep, acc, f, rt, by, bias_s);
+        if constexpr (EPI == EPI_BWD) epi_bwd<BN>(ep, acc, f, rt, by);
+        if constexpr (EPI == EPI_STORE) epi_store<BN>(ep, acc, f, (long)g.a_row_base + 128L * rt, by);
       }
-      if (tr && warp == 2 && lane == 0) ep.trace[(long)it * g.t_step * 8 + 5] = clock64();
       if (n_steps > 1) {
-        // end of a step: all epilogue warps of the CTA are done with the accumulator and have issued their stores; one
+        // end of a step: both consumer warpgroups are done with the accumulator and have issued their stores; one
         // thread makes them visible device-wide and counts the CTA in (the pattern of a cooperative grid sync)
-        tcgen05_fence_before();
-        named_bar_sync(2, S::THREADS - 64);
-        if (warp == 2 && lane == 0) {
-          mbar_arrive(tmem_free);
+        named_bar_sync(2, 256);
+        if (tid == 0) {
           __threadfence();
           atomicAdd(g.gbar + blockIdx.x, 1u);
         }
       }
     }
-    (void)part;
   }
-  __syncwarp();
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 // =============================================================================================
@@ -713,46 +572,35 @@ struct GWgradParams {
   int n_kblocks, kb_per_split, Mpad, Ntot;
   float* partial;       // [S][Mpad][Ntot]
 };
-// MT = 128-row M tiles per CTA (2: a 256 x 256 CTA tile, each B stage feeds two MMAs -- a third less operand traffic
-// per FLOP, see GSmem)
-template <int MT>
 struct GWCfg {
-  static constexpr int THREADS = 64 + 128 * MT;
-  static constexpr uint32_t A_BYTES = MT * 16384;
+  static constexpr int THREADS = 2 * 128 + 32;      // two consumer warpgroups (M rows 0-63 / 64-127) + TMA producer warp
+  static constexpr uint32_t A_BYTES = 16384;
   static constexpr uint32_t STAGE_BYTES = A_BYTES + 32768;
-  static constexpr int STAGES = (int)(196608u / STAGE_BYTES);       // 4 (MT = 1) or 3 (MT = 2)
+  static constexpr int STAGES = (int)(196608u / STAGE_BYTES);
   static constexpr uint32_t SMEM = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
-template <int MT>
-__global__ void __launch_bounds__(GWCfg<MT>::THREADS, 1)
+__global__ void __launch_bounds__(GWCfg::THREADS, 1)
     gwgrad_kernel(GWgradParams p, const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b) {
-  using C = GWCfg<MT>;
+  using C = GWCfg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
   uint64_t* empty = full + C::STAGES;
-  uint64_t* acc_full = empty + C::STAGES;
-  uint32_t* tmem_base_s = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m0 = blockIdx.x * 128 * MT, n0 = blockIdx.y * 256;
+  const int m0 = blockIdx.x * 128, n0 = blockIdx.y * 256;
   const int kb_beg = blockIdx.z * p.kb_per_split;
   const int kb_end = min(p.n_kblocks, kb_beg + p.kb_per_split);
   const int nkb = max(0, kb_end - kb_beg);
   if (tid == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);              // one arrive per consumer warp
     }
-    mbar_init(acc_full, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_s, 256 * MT);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tmem_base_s;
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       for (int i = 0; i < nkb; ++i) {
         const int s = i % C::STAGES;
@@ -760,57 +608,38 @@ __global__ void __launch_bounds__(GWCfg<MT>::THREADS, 1)
         mbar_arrive_expect_tx(&full[s], C::STAGE_BYTES);
         uint8_t* st = smem + s * C::STAGE_BYTES;
         const int krow = (kb_beg + i) * 64;
-        for (int mb = 0; mb < 2 * MT; ++mb) tma_load_2d(st + mb * 8192, &tm_a, &full[s], m0 + mb * 64, krow);
+        for (int mb = 0; mb < 2; ++mb) tma_load_2d(st + mb * 8192, &tm_a, &full[s], m0 + mb * 64, krow);
         for (int nb = 0; nb < 4; ++nb) tma_load_2d(st + C::A_BYTES + nb * 8192, &tm_b, &full[s], n0 + nb * 64, krow);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && nkb > 0) {
-      const uint32_t idesc = make_idesc_bf16(128, 256, true, true);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % C::STAGES;
-        mbar_wait(&full[s], (i / C::STAGES) & 1);
-        tcgen05_fence_after();
-        uint8_t* st = smem + s * C::STAGE_BYTES;
-#pragma unroll
-        for (int k16 = 0; k16 < 4; ++k16) {
-          const uint64_t db = make_smem_desc(smem_u32(st + C::A_BYTES) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-#pragma unroll
-          for (int mt = 0; mt < MT; ++mt) {
-            const uint64_t da = make_smem_desc(smem_u32(st + mt * 16384) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-            umma_f16(tmem + mt * 256, da, db, idesc, (i | k16) != 0);
-          }
-        }
-        umma_commit(&empty[s]);
-      }
-      umma_commit(acc_full);
-    }
   } else {
-    const int q = warp & 3;
-    const int mt = (warp - 2) >> 2;
-    const int m = mt * 128 + q * 32 + lane;
-    float* out = p.partial + ((long)blockIdx.z * p.Mpad + m0 + m) * p.Ntot + n0;
-    if (nkb > 0) {
-      mbar_wait(acc_full, 0);
-      tcgen05_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < 256; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem + ((uint32_t)(q * 32) << 16) + mt * 256 + c0, v);
-        tmem_ld_wait();
+    const int wg = warp >> 2, cq = lane & 3;
+    float acc[128];
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(out + c0 + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                 __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % C::STAGES;
+      mbar_wait(&full[s], (i / C::STAGES) & 1);
+      uint8_t* st = smem + s * C::STAGE_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k16 = 0; k16 < 4; ++k16) {
+        const uint64_t db = make_smem_desc(smem_u32(st + C::A_BYTES) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
+        const uint64_t da = make_smem_desc(smem_u32(st + wg * 8192) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
+        wgmma_m64n256k16<1, 1>(acc, da, db, 1);
       }
-    } else {
-      for (int c0 = 0; c0 < 256; c0 += 4) *reinterpret_cast<float4*>(out + c0) = make_float4(0.f, 0.f, 0.f, 0.f);
+      wgmma_commit();
+      wgmma_wait<1>();                      // the previous stage's MMAs are complete: release it
+      if (i > 0 && lane == 0) mbar_arrive(&empty[(i - 1) % C::STAGES]);
     }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    const int row = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    float* out = p.partial + ((long)blockIdx.z * p.Mpad + row) * p.Ntot + n0 + 2 * cq;
+#pragma unroll
+    for (int i = 0; i < 128; i += 2)
+      *reinterpret_cast<float2*>(out + (long)8 * ((i >> 1) & 1) * p.Ntot + 8 * (i >> 2)) = make_float2(acc[i], acc[i + 1]);
   }
-  __syncwarp();
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 256 * MT);
 }
 
 // dst[row][n] = sum_z partial[z][row][n] for row < Mvalid (dst row-major [Mvalid][Ntot])
@@ -1372,7 +1201,6 @@ struct GenImpl {
   int n_sms = 0;
   cudaStream_t side = nullptr;          // second half of the batch in the backward recurrence (see gen_backward)
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  long long* trace = nullptr;      // LFMQ_TRACE_GEN=1: [phase 0 fwd / 1 bwd][layer][t][8] clock64 stamps of CTA (0,0)
   int maxB = 0, Bp = 0, NRT = 0, T = 0, F = 0, O = 0, H = 0, L = 0, NB16 = 0;
   bool x3 = false, train_ws = false;
   int64_t oWo = 0, obo = 0;
@@ -1464,7 +1292,7 @@ void gen_layout(GenState& st, const lfmq_config& c, const GenLayerOff* lo, int64
   m.head_tc_part = reinterpret_cast<float*>(take((size_t)GH_PART * T * m.NRT * 4));
   m.dpb = m.train_ws ? reinterpret_cast<__nv_bfloat16*>(take(T * Bp * 64 * 2)) : nullptr;
   m.cstate = reinterpret_cast<float*>(take(Bp * H * 4));
-  m.head_ctas = 148;
+  m.head_ctas = device_sm_count();
   m.head_part = reinterpret_cast<float*>(take((size_t)GH_PART * m.head_ctas * 4));
   if (m.train_ws) {
     m.dcstate = reinterpret_cast<float*>(take(Bp * H * 4));
@@ -1472,7 +1300,7 @@ void gen_layout(GenState& st, const lfmq_config& c, const GenLayerOff* lo, int64
     m.dy = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * H * 2));
     m.dhout = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * H * 2));
     m.dpred = reinterpret_cast<float*>(take(T * Bp * GH_O * 4));
-    m.head_wctas = 148;
+    m.head_wctas = device_sm_count();
     m.head_wpart = reinterpret_cast<float*>(take((size_t)H * GH_O * m.head_wctas * 4));
     m.bn_ctas_max = (int)cdivl((long)T * m.maxB, GBN_ROWS);
     m.bn_part = reinterpret_cast<float*>(take((size_t)2 * H * m.bn_ctas_max * 4));
@@ -1541,31 +1369,24 @@ int gen_init(GenState& st, const lfmq_config& c) {
     if ((rc = gmap_2d(&m.tm_dz, m.dz, 4 * H, T * Bp, 64, 128))) return rc;
     if ((rc = gmap_2d(&m.tm_dz_mn, m.dz, 4 * H, T * Bp, 64, 64))) return rc;
   }
-#define LFMQ_GEMM_ATTR(BN_, EPI_, MT_)                                                                         \
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(tile_gemm_kernel<BN_, EPI_, MT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                       GSmem<BN_, MT_, EPI_>::TOTAL))
-  LFMQ_GEMM_ATTR(256, EPI_FWD, 1);
-  LFMQ_GEMM_ATTR(256, EPI_FWD, 2);
-  LFMQ_GEMM_ATTR(256, EPI_FWD_ACC, 1);
-  LFMQ_GEMM_ATTR(256, EPI_FWD_ACC, 2);
-  LFMQ_GEMM_ATTR(128, EPI_BWD, 1);
-  LFMQ_GEMM_ATTR(64, EPI_BWD, 1);
-  LFMQ_GEMM_ATTR(16, EPI_HEAD, 1);
-  LFMQ_GEMM_ATTR(128, EPI_STORE, 1);
-  LFMQ_GEMM_ATTR(64, EPI_STORE, 1);
+#define LFMQ_GEMM_ATTR(BN_, EPI_)                                                                              \
+  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(tile_gemm_kernel<BN_, EPI_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                       GSmem<BN_, EPI_>::TOTAL))
+  LFMQ_GEMM_ATTR(256, EPI_FWD);
+  LFMQ_GEMM_ATTR(256, EPI_FWD_ACC);
+  LFMQ_GEMM_ATTR(128, EPI_BWD);
+  LFMQ_GEMM_ATTR(64, EPI_BWD);
+  LFMQ_GEMM_ATTR(16, EPI_HEAD);
+  LFMQ_GEMM_ATTR(128, EPI_STORE);
+  LFMQ_GEMM_ATTR(64, EPI_STORE);
 #undef LFMQ_GEMM_ATTR
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(gwgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GWCfg<1>::SMEM));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(gwgrad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GWCfg<2>::SMEM));
+  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(gwgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GWCfg::SMEM));
   const int hsmem = (int)((H / 64) * 16384 + H * GH_O * 4 + 64 + 1024);
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(ghead_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem));
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(ghead_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem));
   if (m.train_ws) {
     const int bsm = (256 / ((int)H / 8) > 0 ? 256 / ((int)H / 8) : 1) * 2 * (int)H * 4;
     LFMQ_CUDA_CHECK(cudaFuncSetAttribute(gbn_drop_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bsm));
-  }
-  if (getenv("LFMQ_TRACE_GEN")) {
-    LFMQ_CUDA_CHECK(cudaMalloc(&m.trace, (size_t)2 * m.L * T * 8 * sizeof(long long)));
-    LFMQ_CUDA_CHECK(cudaMemset(m.trace, 0, (size_t)2 * m.L * T * 8 * sizeof(long long)));
   }
   LFMQ_CUDA_CHECK(cudaMalloc(&m.gbar, GBAR_N * sizeof(unsigned int)));
   LFMQ_CUDA_CHECK(cudaMemset(m.gbar, 0, GBAR_N * sizeof(unsigned int)));
@@ -1588,22 +1409,6 @@ static bool gen_can_persist(const GenImpl& m, long ctas, int n_concurrent, int p
          m.gbar_next + ctas * n_concurrent <= GBAR_N;
 }
 
-static void gen_print_trace(GenImpl& m, cudaStream_t s) {
-  if (!m.trace) return;
-  const size_t n = (size_t)2 * m.L * m.T * 8;
-  std::vector<long long> h(n);
-  cudaStreamSynchronize(s);
-  cudaMemcpy(h.data(), m.trace, n * sizeof(long long), cudaMemcpyDeviceToHost);
-  for (int ph = 0; ph < 2; ++ph)
-    for (int l = 0; l < m.L; ++l)
-      for (int t = 0; t < m.T; t += 8) {
-        const long long* r = h.data() + (((size_t)ph * m.L + l) * m.T + t) * 8;
-        if (!r[0]) continue;
-        fprintf(stderr, "[gtrace %s l=%d t=%2d] wait-passed %lld first-stage %lld mma-issued %lld acc-full %lld epi-done %lld\n",
-                ph ? "bwd" : "fwd", l, t, r[1] - r[0], r[2] - r[0], r[3] - r[0], r[4] - r[0], r[5] - r[0]);
-      }
-}
-
 void gen_destroy(GenState& st) {
   if (st.impl && st.impl->side) {
     cudaStreamSynchronize(st.impl->side);
@@ -1611,7 +1416,6 @@ void gen_destroy(GenState& st) {
     cudaEventDestroy(st.impl->ev_join);
     cudaStreamDestroy(st.impl->side);
   }
-  if (st.impl && st.impl->trace) cudaFree(st.impl->trace);
   if (st.impl && st.impl->gbar) cudaFree(st.impl->gbar);
   delete st.impl;
   st.impl = nullptr;
@@ -1619,25 +1423,25 @@ void gen_destroy(GenState& st) {
 
 // Launch of one tile_gemm_kernel instantiation; `pdl`: with the programmatic-stream-serialization attribute (the
 // kernel waits for its predecessor itself, see the kernel).  LFMQ_GEN_PDL=0 turns the attribute off.
-template <int BN, int EPI, int MT>
+template <int BN, int EPI>
 static int launch_tile_gemm(dim3 grid, cudaStream_t s, bool pdl, const GArgs& g, const EpiParams& ep, const CUtensorMap& a0,
                             const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& a3, const CUtensorMap& b0,
                             const CUtensorMap& b1) {
   static const bool pdl_on = !(getenv("LFMQ_GEN_PDL") && atoi(getenv("LFMQ_GEN_PDL")) == 0);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
-  cfg.blockDim = dim3(GSmem<BN, MT, EPI>::THREADS);
-  cfg.dynamicSmemBytes = GSmem<BN, MT, EPI>::TOTAL;
+  cfg.blockDim = dim3(GSmem<BN, EPI>::THREADS);
+  cfg.dynamicSmemBytes = GSmem<BN, EPI>::TOTAL;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = (pdl && pdl_on) ? 1 : 0;
-  LFMQ_CUDA_CHECK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<BN, EPI, MT>, g, ep, a0, a1, a2, a3, b0, b1));
+  LFMQ_CUDA_CHECK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<BN, EPI>, g, ep, a0, a1, a2, a3, b0, b1));
   g_launches++;
   if (debug_sync_on()) {
-    fprintf(stderr, "[lfmq launch] tile_gemm<%d,%d,%d> grid %u x %u t=%d ...", BN, EPI, MT, grid.x, grid.y, ep.t);
+    fprintf(stderr, "[lfmq launch] tile_gemm<%d,%d> grid %u x %u t=%d ...", BN, EPI, grid.x, grid.y, ep.t);
     fflush(stderr);
     cudaError_t e = cudaDeviceSynchronize();
     fprintf(stderr, " %s\n", cudaGetErrorString(e));
@@ -1687,8 +1491,6 @@ static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params
   const int nrt = (B + 127) / 128;
   const bool rec = c.train && c.recurrent_dropout > 0.f;
   const bool drop = c.train && c.dropout > 0.f;
-  static const char* dual_env = getenv("LFMQ_GEN_DUAL");      // 0 / 1 force, unset: by tile count
-  const bool dual = dual_env ? atoi(dual_env) != 0 : ((long)((nrt + 1) / 2) * (4 * H / 256) >= 96);
   LFMQ_CUDA_CHECK(cudaMemsetAsync(m.gbar, 0, GBAR_N * sizeof(unsigned int), s));
   m.gbar_next = 0;
   {
@@ -1711,11 +1513,10 @@ static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params
     ep.rkey = gkey(c, 2 * l + 1, step, c.recurrent_dropout);
     const CUtensorMap& th = rec ? ly.tm_hm : ly.tm_h;
     // steps 1 .. T-1 as ONE persistent launch when all its CTAs fit on the machine at once (see GArgs::n_steps)
-    const long fwd_ctas = dual ? (long)((nrt + 1) / 2) * (4 * H / 256) : (long)nrt * (4 * H / 256);
-    const bool persist = gen_can_persist(m, fwd_ctas, 1, dual ? 1 : 2, T - 1);
+    const long fwd_ctas = (long)nrt * (4 * H / 256);
+    const bool persist = gen_can_persist(m, fwd_ctas, 1, GSmem<256, EPI_FWD>::CTAS_PER_SM, T - 1);
     for (int t = 0; t < T; ++t) {
       ep.t = t;
-      ep.trace = m.trace ? m.trace + (((size_t)0 * m.L + l) * T + t) * 8 : nullptr;
       GArgs g = {};
       g.a_row_base = t * Bp;
       g.b_row_base = 0;
@@ -1724,7 +1525,7 @@ static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params
         g.row_step = Bp;
         g.t_step = 1;
         g.gbar = m.gbar + m.gbar_next;
-        m.gbar_next += dual ? (nrt + 1) / 2 : nrt;
+        m.gbar_next += nrt;
       }
       const int nkb_h = (t > 0) ? H / 64 : 0, nkb_x = ly.Ipad / 64;
       int ns = 0;
@@ -1738,20 +1539,15 @@ static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params
         g.seg[ns++] = GSeg{1, 1, nkb_x, 0, H};
       }
       g.n_seg = ns;
-      // 256-row CTA tiles when there are enough of them to fill the machine (a third less operand traffic per FLOP),
-      // else 128-row tiles, two CTAs per SM.  Steps after the first of a layer follow another step kernel: PDL.
+      // Steps after the first of a layer follow another step kernel: PDL.
       int rc;
-#define LFMQ_FWD_LAUNCH(EPI_, MT_, GRID_)                                                                          \
-  rc = launch_tile_gemm<256, EPI_, MT_>(GRID_, s, t > 0, g, ep, th, ly.tm_in, m.x3 ? ly.tm_h_lo : th,               \
-                                        m.x3 ? ly.tm_in_lo : ly.tm_in, ly.tm_wf, m.x3 ? ly.tm_wf_lo : ly.tm_wf)
-      const dim3 grid2((nrt + 1) / 2, 4 * H / 256), grid1(nrt, 4 * H / 256);
-      if (m.x3) {
-        if (dual) LFMQ_FWD_LAUNCH(EPI_FWD_ACC, 2, grid2);
-        else LFMQ_FWD_LAUNCH(EPI_FWD_ACC, 1, grid1);
-      } else {
-        if (dual) LFMQ_FWD_LAUNCH(EPI_FWD, 2, grid2);
-        else LFMQ_FWD_LAUNCH(EPI_FWD, 1, grid1);
-      }
+#define LFMQ_FWD_LAUNCH(EPI_)                                                                                     \
+  rc = launch_tile_gemm<256, EPI_>(dim3(nrt, 4 * H / 256), s, t > 0, g, ep, th, ly.tm_in, m.x3 ? ly.tm_h_lo : th,  \
+                                   m.x3 ? ly.tm_in_lo : ly.tm_in, ly.tm_wf, m.x3 ? ly.tm_wf_lo : ly.tm_wf)
+      if (m.x3)
+        LFMQ_FWD_LAUNCH(EPI_FWD_ACC);
+      else
+        LFMQ_FWD_LAUNCH(EPI_FWD);
 #undef LFMQ_FWD_LAUNCH
       if (rc) return rc;
       if (persist && t == 1) break;              // that launch ran steps 1 .. T-1
@@ -1770,16 +1566,14 @@ static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params
 // D[Mvalid x Ntot] = A^T B over the T*Bp time-major rows (split-K partials in wg_part, [S][Mpad][Ntot]); the caller reduces
 static int gen_wgrad_gemm(GenImpl& m, const CUtensorMap& tm_a, const CUtensorMap& tm_b, int Mvalid, int Ntot, int* S_out,
                           int* Mpad_out, cudaStream_t s) {
-  const bool dual = Mvalid > 128;                    // 256 x 256 CTA tiles when there are at least two 128-row M tiles
-  const int mrows = dual ? 256 : 128;
-  const int mt = (Mvalid + mrows - 1) / mrows;
-  const int Mpad = mt * mrows;
+  const int mt = (Mvalid + 127) / 128;
+  const int Mpad = mt * 128;
   const long rows = (long)m.T * m.Bp;
   GWgradParams wp;
   wp.n_kblocks = (int)cdivl(rows, 64);
   // K splits: fill the machine, within what the partial buffer holds (the head's [H x 16] product has one N tile and
   // wants many splits; the gate products have 8-16 output tiles and get 8)
-  int S = 148 / (mt * (Ntot / 256));
+  int S = m.n_sms / (mt * (Ntot / 256));
   const size_t smax = m.wg_part_elems / ((size_t)Mpad * Ntot);
   if ((size_t)S > smax) S = (int)smax;
   if (S > 64) S = 64;
@@ -1794,10 +1588,7 @@ static int gen_wgrad_gemm(GenImpl& m, const CUtensorMap& tm_a, const CUtensorMap
     LFMQ_SET_ERR("weight-gradient partial buffer too small");
     return LFMQ_ERR_WORKSPACE;
   }
-  if (dual)
-    gwgrad_kernel<2><<<dim3(mt, Ntot / 256, S), GWCfg<2>::THREADS, GWCfg<2>::SMEM, s>>>(wp, tm_a, tm_b);
-  else
-    gwgrad_kernel<1><<<dim3(mt, Ntot / 256, S), GWCfg<1>::THREADS, GWCfg<1>::SMEM, s>>>(wp, tm_a, tm_b);
+  gwgrad_kernel<<<dim3(mt, Ntot / 256, S), GWCfg::THREADS, GWCfg::SMEM, s>>>(wp, tm_a, tm_b);
   LFMQ_LAUNCH_CHECK();
   *S_out = S;
   *Mpad_out = Mpad;
@@ -1833,7 +1624,7 @@ static int gen_run_head(GenState& st, const lfmq_config& c, const float* params,
   h.dpred = train ? m.dpred : nullptr;
   h.partial = m.head_part;
   if (!m.x3) {
-    // Tensor-core head: pred = y Wo as a tcgen05 GEMM (N = 16) with the loss in its epilogue; training adds
+    // Tensor-core head: pred = y Wo as a wgmma GEMM (N = 16) with the loss in its epilogue; training adds
     // dy = dpred Wo^T (K = 16 padded to one k-block) and dWo = y^T dpred (the weight-gradient GEMM, N padded to 256).
     // The fp32-accumulating SIMT head below stays for LFMQ_PREC_BF16X3 (1e-4 tolerance).
     const int ntile = m.T * m.NRT;                  // every row tile of the time-major buffers (zeros beyond the batch)
@@ -1846,7 +1637,7 @@ static int gen_run_head(GenState& st, const lfmq_config& c, const float* params,
     g.n_seg = 1;
     g.seg[0] = GSeg{0, 0, m.H / 64, 0, 0};
     int rc;
-    if ((rc = launch_tile_gemm<16, EPI_HEAD, 1>(dim3(ntile, 1), s, false, g, ep, m.tm_head_in, m.tm_head_in, m.tm_head_in,
+    if ((rc = launch_tile_gemm<16, EPI_HEAD>(dim3(ntile, 1), s, false, g, ep, m.tm_head_in, m.tm_head_in, m.tm_head_in,
                                                 m.tm_head_in, m.tm_wot, m.tm_wot)))
       return rc;
     if (train) {
@@ -1860,10 +1651,10 @@ static int gen_run_head(GenState& st, const lfmq_config& c, const float* params,
       const int row_tiles = m.T * m.Bp / 128;
       gd.lin_cols = (m.H % 128 == 0) ? m.H / 128 : m.H / 64;
       if (m.H % 128 == 0)
-        rc = launch_tile_gemm<128, EPI_STORE, 1>(dim3(row_tiles * (m.H / 128)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
+        rc = launch_tile_gemm<128, EPI_STORE>(dim3(row_tiles * (m.H / 128)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
                                                  m.tm_dpb, m.tm_wos, m.tm_wos);
       else
-        rc = launch_tile_gemm<64, EPI_STORE, 1>(dim3(row_tiles * (m.H / 64)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
+        rc = launch_tile_gemm<64, EPI_STORE>(dim3(row_tiles * (m.H / 64)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
                                                 m.tm_dpb, m.tm_wos, m.tm_wos);
       if (rc) return rc;
       int S = 0, Mpad = 0;
@@ -1991,7 +1782,6 @@ int gen_backward(GenState& st, const lfmq_config& c, const float* params, float*
         cudaStream_t hs = half ? m.side : s;
         const int rt_off = half ? n_a : 0, n_rt = half ? n_b : n_a;
         ep.t = t;
-        ep.trace = (m.trace && half == 0) ? m.trace + (((size_t)1 * m.L + l) * T + t) * 8 : nullptr;
         ep.has_rec = (t < T - 1) ? 1 : 0;
         GArgs g = {};
         g.a_row_base = (t + 1) * Bp;      // dz_{t+1}
@@ -2007,10 +1797,10 @@ int gen_backward(GenState& st, const lfmq_config& c, const float* params, float*
           m.gbar_next += n_rt;
         }
         if (m.BNU == 128)
-          rc = launch_tile_gemm<128, EPI_BWD, 1>(dim3(n_rt, H / 128), hs, t < T - 1, g, ep, m.tm_dz, m.tm_dz, m.tm_dz,
+          rc = launch_tile_gemm<128, EPI_BWD>(dim3(n_rt, H / 128), hs, t < T - 1, g, ep, m.tm_dz, m.tm_dz, m.tm_dz,
                                                  m.tm_dz, ly.tm_ub, ly.tm_ub);
         else
-          rc = launch_tile_gemm<64, EPI_BWD, 1>(dim3(n_rt, H / 64), hs, t < T - 1, g, ep, m.tm_dz, m.tm_dz, m.tm_dz,
+          rc = launch_tile_gemm<64, EPI_BWD>(dim3(n_rt, H / 64), hs, t < T - 1, g, ep, m.tm_dz, m.tm_dz, m.tm_dz,
                                                 m.tm_dz, ly.tm_ub, ly.tm_ub);
         if (rc) return rc;
       }
@@ -2047,17 +1837,16 @@ int gen_backward(GenState& st, const lfmq_config& c, const float* params, float*
       const int row_tiles = T * Bp / 128;
       g.lin_cols = (H % 128 == 0) ? H / 128 : H / 64;
       if (H % 128 == 0)
-        rc = launch_tile_gemm<128, EPI_STORE, 1>(dim3(row_tiles * (H / 128)), s, false, g, es, m.tm_dz, m.tm_dz, m.tm_dz,
+        rc = launch_tile_gemm<128, EPI_STORE>(dim3(row_tiles * (H / 128)), s, false, g, es, m.tm_dz, m.tm_dz, m.tm_dz,
                                                  m.tm_dz, ly.tm_wb, ly.tm_wb);
       else
-        rc = launch_tile_gemm<64, EPI_STORE, 1>(dim3(row_tiles * (H / 64)), s, false, g, es, m.tm_dz, m.tm_dz, m.tm_dz,
+        rc = launch_tile_gemm<64, EPI_STORE>(dim3(row_tiles * (H / 64)), s, false, g, es, m.tm_dz, m.tm_dz, m.tm_dz,
                                                 m.tm_dz, ly.tm_wb, ly.tm_wb);
       if (rc) return rc;
     }
     st.prof->end(LFMQ_REGION_WGRAD, s);
   }
   (void)x;
-  gen_print_trace(m, s);
   return 0;
 }
 

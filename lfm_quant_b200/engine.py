@@ -22,7 +22,7 @@ def _stream():
 
 
 class ForecasterEngine(object):
-    """fwd / loss / BPTT / clip / optimizer / MaxNorm for RNNPointEstimate on one B200.
+    """fwd / loss / BPTT / clip / optimizer / MaxNorm for RNNPointEstimate on one GPU.
 
     Mirrors what the reference builds in RNNPointEstimate._build_model
     (scripts/models/point_estimate/rnn_point_estimate.py:40-107) plus the step body of

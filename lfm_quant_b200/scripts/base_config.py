@@ -1,5 +1,5 @@
 """Flag schema of the forecaster -- every flag of scripts/lfm_quant.py:23-106 and scripts/base_config.py:12-96,
-same names, types and defaults -- plus the B200 extensions at the bottom.
+same names, types and defaults -- plus the native-path extensions at the bottom.
 
 ``get_configs(argv=None, list_sep='-')`` reproduces the post-processing of scripts/lfm_quant.py:108-129
 (unrollings from years, '-'-separated lists); scripts/base_config.py:115 splits forecast_steps_weights on ','
@@ -101,8 +101,8 @@ SCHEMA = [
     ('model_ranking_fname', _STRING, './model-ranking.dat', 'Model Ranking File Name'),
     ('model_ranking_factor', _STRING, 'pred_var_entval', 'Model ranking factor'),
     ('cdrs_inference_date', _STRING, None, "CDRS Inference date. Format: '%Y-%m-%d' "),
-    # ---- B200 extensions (not in the reference) --------------------------------------------------------
-    ('precision', _STRING, 'fp32', "'fp32' (parity mode) or 'bf16' (tcgen05 tensor-core gate GEMMs)"),
+    # ---- native-path extensions (not in the reference) -------------------------------------------------
+    ('precision', _STRING, 'fp32', "'fp32' (parity mode) or 'bf16' (tensor-core gate GEMMs)"),
 ]
 
 _DEFINERS = {_STRING: configs.DEFINE_string, _INT: configs.DEFINE_integer, _FLOAT: configs.DEFINE_float,

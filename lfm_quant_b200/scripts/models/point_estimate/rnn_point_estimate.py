@@ -2,7 +2,7 @@
 
 Same constructor ``RNNPointEstimate(config, dataset)`` and ``.model`` attribute; the Keras functional graph is
 replaced by ``NativeForecaster``: n_layers x [LSTM -> BatchNormalization(inference affine) -> Dropout] -> Dense,
-executed by hand-written sm_100a CUDA behind the C-ABI of include/lfmq.h.
+executed by hand-written sm_90a CUDA behind the C-ABI of include/lfmq.h.
 """
 from __future__ import absolute_import, division, print_function
 
@@ -87,7 +87,7 @@ class NativeChainForecaster(object):
         return self.engine.n_total
 
     def summary(self):
-        lines = ['Model: "RNNPointEstimate" (native sm_100a, forecast_steps=%d, precision=%s)' % (self.engine.S,
+        lines = ['Model: "RNNPointEstimate" (native sm_90a, forecast_steps=%d, precision=%s)' % (self.engine.S,
                                                                                                 self.engine.precision),
                  '%-44s %-16s %10s' % ('Variable', 'Shape', 'Param #'), '=' * 72]
         for _, name, shape, _, tr in self.engine.specs:
@@ -198,7 +198,7 @@ class NativeForecaster(object):
         return self.engine.n_total
 
     def summary(self):
-        lines = ['Model: "%s" (native sm_100a, precision=%s)' % ('RNNUqRangeEstimate' if self.uq else 'RNNPointEstimate',
+        lines = ['Model: "%s" (native sm_90a, precision=%s)' % ('RNNUqRangeEstimate' if self.uq else 'RNNPointEstimate',
                                                                    self.engine.precision),
                  '%-44s %-16s %10s' % ('Variable', 'Shape', 'Param #'), '=' * 72]
         for name, shape, _, tr in self.engine.specs:

@@ -90,8 +90,10 @@ def test_shard_rows_partition():
 def _cli_worker(rank, world, port, out_dir):
     """What scripts/train.py does under torchrun: dp.init_from_env() from the launcher's environment, then each rank
     takes its rows of every global batch of window indices."""
+    # CPU processes (gloo), as in the rest of this module: with CUDA visible init_from_env would pick NCCL and
+    # LOCAL_RANK's GPU, which a machine with fewer GPUs than ranks does not have
     os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
+                      LOCAL_RANK=str(rank), CUDA_VISIBLE_DEVICES='')
     r, w = dp.init_from_env()
     assert (r, w) == (rank, world) and dist.is_initialized()
     rows = []

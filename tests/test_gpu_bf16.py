@@ -1,4 +1,4 @@
-"""GPU tests of the bf16 tensor-core path (LFMQ_PREC_BF16): tcgen05 gate GEMMs with bf16 operands, fp32 accumulate.
+"""GPU tests of the bf16 tensor-core path (LFMQ_PREC_BF16): wgmma gate GEMMs with bf16 operands, fp32 accumulate.
 
 bf16 operands carry 8 mantissa bits, so these tests use a bf16-level tolerance against the fp64 oracle (the fp32
 parity mode is held to 1e-4 in test_gpu_parity.py) and additionally check the tensor-core path against the fp32
@@ -156,7 +156,8 @@ def test_bf16_matches_fp32_path_at_baseline_shape():
 
 def test_bf16_training_with_more_tiles_than_resident_clusters():
     """B = 4500 is 36 batch tiles (the last one ragged): the persistent recurrences run a second iteration per cluster,
-    which exercises the barrier phases carried across tiles (forward tma_issued / acc_free, backward exp_ready) and the
+    while clusters left without a tile in that round sit it out; this exercises the barrier phases carried across tiles
+    (forward x_empty / h_written, backward exp_ready / recv_free / dpb_free) and the
     dz TMA-store coordinates of later tiles.  Gradients and loss vs the fp32 CUDA path."""
     B, T, F, O, H, L = 4500, 5, 32, 16, 256, 1
     params, x, y = make_problem(B, T, F, O, H, L, seed=31, init_scale=0.5)
