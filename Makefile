@@ -3,7 +3,7 @@ NVCC      ?= nvcc
 ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := -O3 -Xptxas -v -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC -Xcompiler -Wall -Xcompiler -Wno-unknown-pragmas --expt-relaxed-constexpr
 CSRC      := lfm_quant_b200/csrc
-SRCS      := $(CSRC)/lfmq_api.cu $(CSRC)/kernels_simt.cu $(CSRC)/lstm_tc.cu $(CSRC)/rnn_tc.cu
+SRCS      := $(CSRC)/lfmq_api.cu $(CSRC)/kernels_simt.cu $(CSRC)/lstm_tc.cu $(CSRC)/rnn_tc.cu $(CSRC)/tc_shared.cu
 OBJS      := $(SRCS:.cu=.o)
 LIB       := lfm_quant_b200/_lfmq.so
 
@@ -21,5 +21,5 @@ clean:
 # A/B builds of kernel variants: `make alt ALT_FLAGS="-D..."` -> lfm_quant_b200/_lfmq_alt.so (LFMQ_LIB_PATH selects it)
 alt:
 	mkdir -p build/alt
-	for f in lfmq_api kernels_simt lstm_tc rnn_tc; do $(NVCC) $(NVCCFLAGS) $(ALT_FLAGS) -c $(CSRC)/$$f.cu -o build/alt/$$f.o || exit 1; done
-	$(NVCC) $(ARCH) -shared -o lfm_quant_b200/_lfmq_alt.so build/alt/lfmq_api.o build/alt/kernels_simt.o build/alt/lstm_tc.o build/alt/rnn_tc.o -lcudart
+	for f in lfmq_api kernels_simt lstm_tc rnn_tc tc_shared; do $(NVCC) $(NVCCFLAGS) $(ALT_FLAGS) -c $(CSRC)/$$f.cu -o build/alt/$$f.o || exit 1; done
+	$(NVCC) $(ARCH) -shared -o lfm_quant_b200/_lfmq_alt.so $(patsubst $(CSRC)/%.cu,build/alt/%.o,$(SRCS)) -lcudart

@@ -68,11 +68,12 @@ inline bool debug_sync_on() {
     LFMQ_DEBUG_SYNC();                                        \
   } while (0)
 
-// Host side: launch with the programmatic-stream-serialization attribute (LFMQ_PDL=0 turns it off).  `attrs_extra` lets
-// the cluster kernels add their cluster dimension.
+// Host side: launch with the programmatic-stream-serialization attribute when `pdl` is set (LFMQ_PDL=0 turns it off for
+// every launch).  `pdl` is per call because a kernel that reads anything before its pdl_wait() must not overlap a
+// predecessor that writes it.  `cluster_x` > 1 adds the cluster dimension of the cluster kernels.
 template <typename... KArgs, typename... Args>
 inline int launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, int cluster_x,
-                      Args&&... args) {
+                      bool pdl, Args&&... args) {
   static const bool on = !(getenv("LFMQ_PDL") && atoi(getenv("LFMQ_PDL")) == 0);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
@@ -88,7 +89,7 @@ inline int launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sm
     attr[n].val.clusterDim.z = 1;
     ++n;
   }
-  if (on) {
+  if (on && pdl) {
     attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[n].val.programmaticStreamSerializationAllowed = 1;
     ++n;
@@ -130,12 +131,37 @@ struct DropoutKey {
   float scale;         // 1 / (1 - rate)
 };
 
+inline DropoutKey dropout_key(uint64_t seed, int stream, int64_t step, float rate) {
+  DropoutKey k;
+  k.k0 = (uint32_t)(seed & 0xffffffffu);
+  k.k1 = (uint32_t)(seed >> 32);
+  k.stream = (uint32_t)stream;
+  k.step = (uint32_t)(step & 0xffffffff);
+  k.thr = (uint32_t)((double)rate * 16777216.0);
+  k.scale = 1.0f / (1.0f - rate);
+  return k;
+}
+
 __device__ __forceinline__ void dropout_quad(const DropoutKey& k, uint64_t q, float m[4]) {
   uint32_t r[4];
   philox4x32_10((uint32_t)q, (uint32_t)(q >> 32), k.stream, k.step, k.k0, k.k1, r);
 #pragma unroll
   for (int i = 0; i < 4; ++i) m[i] = ((r[i] >> 8) >= k.thr) ? k.scale : 0.0f;
 }
+
+// Carves the caller's workspace into buffers on 1024-byte boundaries; with base == nullptr it only sizes.
+constexpr size_t WS_ALIGN = 1024;
+inline size_t ws_align_up(size_t v) { return (v + WS_ALIGN - 1) / WS_ALIGN * WS_ALIGN; }
+struct Carver {
+  char* base;
+  size_t off;
+  template <typename T>
+  T* take(size_t n) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off = ws_align_up(off + n * sizeof(T));
+    return p;
+  }
+};
 
 // Event brackets around the regions of a step (include/lfmq.h LFMQ_REGION_*).
 struct Profiler {

@@ -925,7 +925,7 @@ __global__ void __launch_bounds__(256) mask_rows_kernel(long rows, int O, int B,
 
 int mask_count(cudaStream_t s, int B, int T, int O, const float* y, float* out2, unsigned int* tickets) {
   const long rows = (long)B * T;
-  if (int rc = launch_pdl(mask_rows_kernel, dim3(cdiv(rows, 256)), dim3(256), 0, s, 1, rows, O, B, y, tickets, out2)) return rc;
+  if (int rc = launch_pdl(mask_rows_kernel, dim3(cdiv(rows, 256)), dim3(256), 0, s, 1, true, rows, O, B, y, tickets, out2)) return rc;
   return 0;
 }
 
@@ -979,7 +979,7 @@ int grad_norm_scale(cudaStream_t s, long n, const float* g, float clip, float* s
                     unsigned int* ticket) {
   double* partial = reinterpret_cast<double*>(scratch);
   const int nblk = (int)min((long)device_sm_count(), max((long)1, n / 2048));
-  if (int rc = launch_pdl(sumsq_norm_kernel, dim3(nblk), dim3(256), 0, s, 1, n, g, partial, clip, scalars, ticket)) return rc;
+  if (int rc = launch_pdl(sumsq_norm_kernel, dim3(nblk), dim3(256), 0, s, 1, true, n, g, partial, clip, scalars, ticket)) return rc;
   return 0;
 }
 
@@ -1024,7 +1024,7 @@ __global__ void opt_update_kernel(int opt, long n, float* __restrict__ p, const 
 
 int opt_update(cudaStream_t s, int opt, long n, float* p, const float* g, float* slot0, float* slot1,
                const float* scalars, float lr, float, float, float momentum) {
-  if (int rc = launch_pdl(opt_update_kernel, dim3(cdiv(n, 256)), dim3(256), 0, s, 1, opt, n, p, g, slot0, slot1, scalars, lr, momentum)) return rc;
+  if (int rc = launch_pdl(opt_update_kernel, dim3(cdiv(n, 256)), dim3(256), 0, s, 1, true, opt, n, p, g, slot0, slot1, scalars, lr, momentum)) return rc;
   return 0;
 }
 
@@ -1047,7 +1047,7 @@ __global__ void maxnorm_cols_kernel(int I, int N, float* __restrict__ W, float m
 }
 
 int maxnorm_cols(cudaStream_t s, int I, int N, float* W, float max_norm) {
-  if (int rc = launch_pdl(maxnorm_cols_kernel, dim3(cdiv((long)N * 32, 256)), dim3(256), 0, s, 1, I, N, W, max_norm)) return rc;
+  if (int rc = launch_pdl(maxnorm_cols_kernel, dim3(cdiv((long)N * 32, 256)), dim3(256), 0, s, 1, true, I, N, W, max_norm)) return rc;
   return 0;
 }
 

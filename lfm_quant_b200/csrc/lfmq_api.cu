@@ -49,27 +49,14 @@ struct lfmq_handle_s {
   float *zh, *dz2;   // GRU only: recurrent projection of one step, gradient w.r.t. the recurrent projection
   size_t scratch_elems;
   lfmq::TcState tc;
-  lfmq::GenState gen;
+  int64_t last_step = 0;     // step and row0 of the last forward: the fp32 backward regenerates that call's dropout masks
+  int64_t last_row0 = 0;
   int stream_base = 0;       // first Philox stream index of this handle's layers (stage s of a forecast chain: 2 (L0+s-1))
   int use_gen;               // 1: the general tensor-core path (rnn_tc.cu) runs this handle's bf16 / bf16x3 work
   lfmq::Profiler prof;
 };
 
 namespace {
-
-constexpr size_t ALIGN = 1024;
-size_t align_up(size_t v) { return (v + ALIGN - 1) / ALIGN * ALIGN; }
-
-struct Carver {
-  char* base;
-  size_t off;
-  template <typename T>
-  T* take(size_t n) {
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off = align_up(off + n * sizeof(T));
-    return p;
-  }
-};
 
 int validate(const lfmq_config* c) {
   if (!c || c->struct_size != (int32_t)sizeof(lfmq_config)) {
@@ -165,35 +152,41 @@ size_t layout(lfmq_handle_s* h, char* base) {
   h->tickets = reinterpret_cast<unsigned int*>(h->scalars);   // [0] mask count, [1] mask ticket, [2] norm ticket;
                                                               // zeroed at create, every user resets what it used
   const size_t BT = B * T;
-  for (int l = 0; l < L; ++l) {
-    LayerBuf& lb = h->layers[l];
-    lb.h = cv.take<float>(BT * H);
-    lb.c = cv.take<float>(BT * H);
-    lb.y = cv.take<float>(BT * H);
-    lb.gates = c.forward_only ? nullptr : cv.take<float>(BT * 4 * H);
-    lb.rmask = cv.take<float>(B * H);
+  // The fp32 path's activations.  The tensor-core paths carve their own (tc_layout / gen_layout) and never touch these.
+  h->z = h->zh = h->hm = h->preds = h->var = h->apre = nullptr;
+  h->dz = h->dz2 = h->dy = h->dh_out = h->hp = h->dh_rec = h->dc = h->dpred = h->da = nullptr;
+  if (c.precision == LFMQ_PREC_FP32) {
+    for (int l = 0; l < L; ++l) {
+      LayerBuf& lb = h->layers[l];
+      lb.h = cv.take<float>(BT * H);
+      lb.c = cv.take<float>(BT * H);
+      lb.y = cv.take<float>(BT * H);
+      lb.gates = c.forward_only ? nullptr : cv.take<float>(BT * 4 * H);
+      lb.rmask = cv.take<float>(B * H);
+    }
+    h->z = cv.take<float>(B * 4 * H);
+    h->zh = (c.rnn_cell == LFMQ_CELL_GRU) ? cv.take<float>(B * 3 * H) : nullptr;
+    h->hm = cv.take<float>(B * H);
+    h->preds = cv.take<float>(BT * O);
+    h->var = c.uq ? cv.take<float>(BT * O) : nullptr;
+    h->apre = (c.uq && !c.forward_only) ? cv.take<float>(BT * O) : nullptr;
+    if (!c.forward_only) {
+      h->dz = cv.take<float>(BT * 4 * H);
+      h->dz2 = (c.rnn_cell == LFMQ_CELL_GRU) ? cv.take<float>(BT * 3 * H) : nullptr;
+      h->dy = cv.take<float>(BT * H);
+      h->dh_out = cv.take<float>(BT * H);
+      h->hp = cv.take<float>(BT * H);
+      h->dh_rec = cv.take<float>(B * H);
+      h->dc = cv.take<float>(B * H);
+      h->dpred = cv.take<float>(BT * O);
+      h->da = c.uq ? cv.take<float>(BT * O) : nullptr;
+    }
   }
-  h->z = cv.take<float>(B * 4 * H);
-  h->zh = (c.rnn_cell == LFMQ_CELL_GRU) ? cv.take<float>(B * 3 * H) : nullptr;
-  h->hm = cv.take<float>(B * H);
-  h->preds = cv.take<float>(BT * O);
-  h->var = c.uq ? cv.take<float>(BT * O) : nullptr;
-  h->apre = (c.uq && !c.forward_only) ? cv.take<float>(BT * O) : nullptr;
+  // scratch serves every precision (lfmq_loss, grad_norm_scale)
   size_t scratch = (size_t)4 << 20;
   if (!c.forward_only) {
-    h->dz = cv.take<float>(BT * 4 * H);
-    h->dz2 = (c.rnn_cell == LFMQ_CELL_GRU) ? cv.take<float>(BT * 3 * H) : nullptr;
-    h->dy = cv.take<float>(BT * H);
-    h->dh_out = cv.take<float>(BT * H);
-    h->hp = cv.take<float>(BT * H);
-    h->dh_rec = cv.take<float>(B * H);
-    h->dc = cv.take<float>(B * H);
-    h->dpred = cv.take<float>(BT * O);
-    h->da = c.uq ? cv.take<float>(BT * O) : nullptr;
     const size_t bn_need = ((BT + 127) / 128) * 2 * H + (size_t)1024 * 2 * H;
     if (bn_need > scratch) scratch = bn_need;
-  } else {
-    h->dz = h->dz2 = h->dy = h->dh_out = h->hp = h->dh_rec = h->dc = h->dpred = h->da = nullptr;
   }
   h->scratch_elems = scratch;
   h->scratch = cv.take<float>(scratch);
@@ -214,25 +207,14 @@ size_t layout(lfmq_handle_s* h, char* base) {
       }
       char why[160];
       if (lfmq::gen_supported(c, why, sizeof(why)))      // lfmq_create reports unsupported configurations (gen_init)
-        lfmq::gen_layout(h->gen, c, lo.data(), h->oWo, h->obo, cv.base, cv.off);
+        lfmq::gen_layout(h->tc, c, lo.data(), h->oWo, h->obo, cv);
     } else {
       const LayerBuf& lb = h->layers[0];
       lfmq::tc_layout(h->tc, c, lfmq::TcParamOff{lb.oW, lb.oU, lb.ob, lb.ogamma, lb.obeta, lb.omean, lb.ovar, h->oWo, h->obo},
-                      cv.base, cv.off);
+                      cv);
     }
   }
   return cv.off;
-}
-
-DropoutKey make_key(const lfmq_config& c, int stream, int64_t step, float rate) {
-  DropoutKey k;
-  k.k0 = (uint32_t)(c.seed & 0xffffffffu);
-  k.k1 = (uint32_t)(c.seed >> 32);
-  k.stream = (uint32_t)stream;
-  k.step = (uint32_t)(step & 0xffffffff);
-  k.thr = (uint32_t)((double)rate * 16777216.0);
-  k.scale = 1.0f / (1.0f - rate);
-  return k;
 }
 
 #define RUN(expr)                 \
@@ -268,7 +250,8 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
     const float* rmask = nullptr;
     const bool stochastic = c.train || c.uq;       // rnn_uq_range_estimate.py:86,88: training=True is a literal there
     if (stochastic && c.recurrent_dropout > 0.f) {
-      RUN(gen_row_mask(s, B, H, make_key(c, h->stream_base + 2 * l + 1, step, c.recurrent_dropout), row0, lb.rmask));
+      RUN(gen_row_mask(s, B, H, dropout_key(c.seed, h->stream_base + 2 * l + 1, step, c.recurrent_dropout), row0,
+                       lb.rmask));
       rmask = lb.rmask;
     }
     for (int t = 0; t < T && c.rnn_cell == LFMQ_CELL_GRU; ++t) {
@@ -292,7 +275,7 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
     }
     const bool drop = stochastic && c.dropout > 0.f;
     RUN(bn_dropout_fwd(s, B, T, H, lb.h, P + lb.ogamma, P + lb.obeta, P + lb.omean, P + lb.ovar, c.bn_epsilon, drop,
-                       make_key(c, h->stream_base + 2 * l, step, c.dropout), row0, lb.y));
+                       dropout_key(c.seed, h->stream_base + 2 * l, step, c.dropout), row0, lb.y));
   }
   h->prof.end(LFMQ_REGION_FWD, s);
   h->prof.begin(LFMQ_REGION_HEAD, s);
@@ -335,8 +318,8 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
     const bool drop = (c.train || c.uq) && c.dropout > 0.f;
     h->prof.begin(LFMQ_REGION_BWD, s);
     RUN(bn_dropout_bwd(s, B, T, H, h->dy, lb.h, P + lb.ogamma, P + lb.omean, P + lb.ovar, c.bn_epsilon, drop,
-                       make_key(c, h->stream_base + 2 * l, h->tc.last_step, c.dropout), h->tc.last_row0, h->dh_out, G + lb.ogamma,
-                       G + lb.obeta, h->scratch, h->scratch_elems));
+                       dropout_key(c.seed, h->stream_base + 2 * l, h->last_step, c.dropout), h->last_row0, h->dh_out,
+                       G + lb.ogamma, G + lb.obeta, h->scratch, h->scratch_elems));
     const bool gru = c.rnn_cell == LFMQ_CELL_GRU;
     const int NG = gru ? 3 : 4;
     for (int t = T - 1; t >= 0 && gru; --t) {
@@ -387,7 +370,6 @@ int apply_update(lfmq_handle h, float lr, int64_t iteration, cudaStream_t s) {
     RUN(maxnorm_cols(s, h->layers[l].I, (c.rnn_cell == LFMQ_CELL_GRU ? 3 : 4) * c.num_hidden, h->params + h->layers[l].oW,
                      c.max_norm));
   h->tc.weights_dirty = 1;
-  h->gen.weights_dirty = 1;
   return 0;
 }
 
@@ -408,9 +390,9 @@ int32_t lfmq_workspace_bytes(const lfmq_config* cfg, uint64_t* bytes) {
   }
   lfmq_handle_s tmp;
   tmp.cfg = *cfg;
-  *bytes = layout(&tmp, nullptr) + ALIGN;
+  *bytes = layout(&tmp, nullptr) + WS_ALIGN;
   lfmq::tc_destroy(tmp.tc);
-  lfmq::gen_destroy(tmp.gen);
+  lfmq::gen_destroy(tmp.tc);
   return LFMQ_OK;
 }
 
@@ -422,7 +404,7 @@ int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_
   }
   lfmq_handle_s* h = new lfmq_handle_s;
   h->cfg = *cfg;
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(workspace)));
+  char* base = reinterpret_cast<char*>(ws_align_up(reinterpret_cast<size_t>(workspace)));
   const size_t need = layout(h, nullptr) + (base - reinterpret_cast<char*>(workspace));
   if (need > workspace_bytes) {
     LFMQ_SET_ERR("workspace too small: need %zu bytes, got %llu", need, (unsigned long long)workspace_bytes);
@@ -431,7 +413,6 @@ int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_
   }
   layout(h, base);
   h->tc.prof = &h->prof;
-  h->gen.prof = &h->prof;
   int rc = 0;
   if (h->use_gen) {
     char why[160];
@@ -439,7 +420,7 @@ int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_
       LFMQ_SET_ERR("tensor-core precision unsupported for this configuration: %s; use LFMQ_PREC_FP32", why);
       rc = LFMQ_ERR_UNSUPPORTED;
     } else {
-      rc = lfmq::gen_init(h->gen, h->cfg);
+      rc = lfmq::gen_init(h->tc, h->cfg);
     }
   } else {
     rc = lfmq::tc_init(h->tc, h->cfg);
@@ -478,7 +459,7 @@ int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_
 int32_t lfmq_destroy(lfmq_handle h) {
   if (h) {
     lfmq::tc_destroy(h->tc);
-    lfmq::gen_destroy(h->gen);
+    lfmq::gen_destroy(h->tc);
     if (h->prof.created)
       for (int r = 0; r < Profiler::kRegions; ++r)
         for (int i = 0; i < Profiler::kCap; ++i) {
@@ -547,7 +528,6 @@ int32_t lfmq_set_params(lfmq_handle h, const float* host, int64_t n, void* strea
   LFMQ_CUDA_CHECK(cudaMemcpyAsync(h->params, host, sizeof(float) * n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
   LFMQ_CUDA_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
   h->tc.weights_dirty = 1;
-  h->gen.weights_dirty = 1;
   return LFMQ_OK;
 }
 
@@ -568,13 +548,13 @@ int32_t lfmq_forward(lfmq_handle h, const float* x, int32_t B, int64_t row0, int
     return LFMQ_ERR_ARG;
   }
   cudaStream_t s = (cudaStream_t)stream;
-  h->tc.last_step = step;
-  h->tc.last_row0 = row0;
+  h->last_step = step;
+  h->last_row0 = row0;
   if (h->cfg.uq) {
     LFMQ_SET_ERR("lfmq_forward: uq handle, call lfmq_forward_uq");
     return LFMQ_ERR_ARG;
   }
-  if (h->use_gen) return lfmq::gen_forward(h->gen, h->cfg, h->params, x, B, row0, step, preds, s);
+  if (h->use_gen) return lfmq::gen_forward(h->tc, h->cfg, h->params, x, B, row0, step, preds, s);
   if (h->cfg.precision == LFMQ_PREC_BF16)
     return lfmq::tc_forward(h->tc, h->cfg, h->params, x, B, row0, step, preds, /*save=*/false, s);
   return forward_fp32(h, x, B, row0, step, preds, nullptr, s);
@@ -591,8 +571,8 @@ int32_t lfmq_forward_uq(lfmq_handle h, const float* x, int32_t B, int64_t row0, 
     LFMQ_SET_ERR("lfmq_forward_uq: handle was created with uq = 0");
     return LFMQ_ERR_ARG;
   }
-  h->tc.last_step = step;
-  h->tc.last_row0 = row0;
+  h->last_step = step;
+  h->last_row0 = row0;
   return forward_fp32(h, x, B, row0, step, preds, var, (cudaStream_t)stream);
 }
 
@@ -645,8 +625,8 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
   }
   cudaStream_t s = (cudaStream_t)stream;
   const lfmq_config& c = h->cfg;
-  h->tc.last_step = step;
-  h->tc.last_row0 = row0;
+  h->last_step = step;
+  h->last_row0 = row0;
   if (c.uq) {
     if (denom_dev) {
       LFMQ_SET_ERR("lfmq_backward: data-parallel denominators are not built for uq handles");
@@ -666,7 +646,7 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
     denom = h->denom;
   }
   float* tail = h->grads + h->n_train;
-  if (h->use_gen) return lfmq::gen_backward(h->gen, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
+  if (h->use_gen) return lfmq::gen_backward(h->tc, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
   if (c.precision == LFMQ_PREC_BF16)
     return lfmq::tc_backward(h->tc, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
   RUN(forward_fp32(h, x, B, row0, step, h->preds, nullptr, s));
@@ -811,8 +791,8 @@ int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const f
       LFMQ_SET_ERR("lfmq_chain_backward: y[%d] == NULL", i);
       return LFMQ_ERR_ARG;
     }
-    h->tc.last_step = step;
-    h->tc.last_row0 = row0;
+    h->last_step = step;
+    h->last_row0 = row0;
     if (i > 0) {
       float* next = work + (size_t)(i - 1) * slot;
       RUN(chain_next_input(s, B, T, F, O, in, stages[i - 1]->preds, x, next));

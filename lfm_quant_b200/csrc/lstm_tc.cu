@@ -45,66 +45,6 @@ constexpr int TC_XOFF = 256;       // first x column inside an xh row
 constexpr int TC_ONE = 288;        // the constant-one column (db falls out of the weight-gradient GEMM)
 constexpr int TC_OPAD = 16;        // head handles n_outputs <= 16
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int make_map_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
-                uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle sw) {
-  static PFN_encodeTiled enc = nullptr;
-  if (!enc) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    LFMQ_CUDA_CHECK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-    enc = reinterpret_cast<PFN_encodeTiled>(fn);
-    if (!enc) {
-      LFMQ_SET_ERR("cuTensorMapEncodeTiled not available");
-      return LFMQ_ERR_CUDA;
-    }
-  }
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {row_stride_bytes};
-  cuuint32_t box[2] = {box_inner, box_outer};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    LFMQ_SET_ERR("cuTensorMapEncodeTiled failed with %d (inner %llu outer %llu box %u x %u)", (int)r,
-                 (unsigned long long)inner, (unsigned long long)outer, box_inner, box_outer);
-    return LFMQ_ERR_CUDA;
-  }
-  return 0;
-}
-
-// General tiled map (bf16): dims / box innermost first, strides in bytes for dims 1..rank-1.
-int make_map_nd(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                const uint32_t* box, CUtensorMapSwizzle sw) {
-  static PFN_encodeTiled enc = nullptr;
-  if (!enc) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    LFMQ_CUDA_CHECK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-    enc = reinterpret_cast<PFN_encodeTiled>(fn);
-    if (!enc) {
-      LFMQ_SET_ERR("cuTensorMapEncodeTiled not available");
-      return LFMQ_ERR_CUDA;
-    }
-  }
-  cuuint64_t d[5], st[4];
-  cuuint32_t bx[5], es[5];
-  for (int i = 0; i < rank; ++i) { d[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
-  for (int i = 0; i + 1 < rank; ++i) st[i] = strides_bytes[i];
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), d, st, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    LFMQ_SET_ERR("cuTensorMapEncodeTiled (rank %d) failed with %d", rank, (int)r);
-    return LFMQ_ERR_CUDA;
-  }
-  return 0;
-}
-
 }  // namespace
 
 struct TcImpl {
@@ -116,7 +56,7 @@ struct TcImpl {
   // workspace
   __nv_bfloat16 *xh, *gates, *dz, *dhout, *Up, *Wp, *Ubk, *pexch;
   __nv_bfloat16* cst;
-  float *biasp, *head_part, *head_wpart, *dpred, *wg_part, *dc;
+  float *biasp, *head_part, *head_wpart, *dpred, *wg_part;
   size_t head_part_elems, wg_part_elems;
   CUtensorMap tm_h, tm_x, tm_u, tm_w;          // forward
   CUtensorMap tm_h128, tm_wot;                 // head: 128-row h tiles, folded head weights
@@ -1154,48 +1094,42 @@ bool tc_shape_supported(const lfmq_config& c) {
   return tc_supported(c, why, sizeof(why));
 }
 
-void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, char* base, size_t& off) {
+void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& cv) {
   if (c.precision != LFMQ_PREC_BF16) return;
   char why[128];
   if (!tc_supported(c, why, sizeof(why))) return;   // tc_init reports the error
   if (!st.impl) st.impl = new TcImpl;
   TcImpl& m = *st.impl;
-  auto take = [&](size_t bytes) -> char* {
-    char* p = base ? base + off : nullptr;
-    off = (off + bytes + 1023) / 1024 * 1024;
-    return p;
-  };
   const size_t B = (size_t)c.max_batch, T = (size_t)c.seq_len, H = TC_H;
   m.maxB = c.max_batch; m.T = c.seq_len; m.I = c.n_inputs; m.O = c.n_outputs;
   m.eps = c.bn_epsilon;
-  m.xh = reinterpret_cast<__nv_bfloat16*>(take(B * (T + 1) * TC_XH_LD * 2));
-  m.Up = reinterpret_cast<__nv_bfloat16*>(take(4 * H * H * 2));
-  m.Wp = reinterpret_cast<__nv_bfloat16*>(take(4 * H * 32 * 2));
-  m.Ubk = reinterpret_cast<__nv_bfloat16*>(take(4 * H * H * 2));
-  m.biasp = reinterpret_cast<float*>(take(4 * H * 4));
-  m.WoTp = reinterpret_cast<__nv_bfloat16*>(take(TC_OPAD * H * 2));
-  m.WoSp = reinterpret_cast<__nv_bfloat16*>(take(H * 32 * 2));
-  m.bop = reinterpret_cast<float*>(take(TC_OPAD * 4));
+  m.xh = cv.take<__nv_bfloat16>(B * (T + 1) * TC_XH_LD);
+  m.Up = cv.take<__nv_bfloat16>(4 * H * H);
+  m.Wp = cv.take<__nv_bfloat16>(4 * H * 32);
+  m.Ubk = cv.take<__nv_bfloat16>(4 * H * H);
+  m.biasp = cv.take<float>(4 * H);
+  m.WoTp = cv.take<__nv_bfloat16>(TC_OPAD * H);
+  m.WoSp = cv.take<__nv_bfloat16>(H * 32);
+  m.bop = cv.take<float>(TC_OPAD);
   m.n_sms = device_sm_count();
   m.head_ctas = m.n_sms * 2;
   m.head_wctas = m.n_sms * 2;
   m.head_part_elems = (size_t)m.head_ctas * HEAD_PART;
-  m.head_part = reinterpret_cast<float*>(take(m.head_part_elems * 4));
+  m.head_part = cv.take<float>(m.head_part_elems);
   if (!c.forward_only) {
     const size_t Bt = (B + 127) / 128 * 128;      // saved state is blocked by 128-row tiles
-    m.gates = reinterpret_cast<__nv_bfloat16*>(take(Bt * T * 4 * H * 2));
-    m.cst = reinterpret_cast<__nv_bfloat16*>(take(Bt * T * H * 2));
-    m.dz = reinterpret_cast<__nv_bfloat16*>(take(B * (T + 1) * 4 * H * 2));
-    m.dhout = reinterpret_cast<__nv_bfloat16*>(take(((B + 127) / 128 * 128) * T * H * 2));
-    m.dc = nullptr;
-    m.pexch = reinterpret_cast<__nv_bfloat16*>(take(((B + 127) / 128) * 2 * 16 * 128 * 64 * 2));
-    m.dpred = reinterpret_cast<float*>(take(B * T * TC_OPAD * 4));
-    m.dpb = reinterpret_cast<__nv_bfloat16*>(take(T * ((B + 127) / 128) * 128 * 32 * 2));
-    m.head_wpart = reinterpret_cast<float*>(take((size_t)m.head_wctas * HWG_PART * 4));
+    m.gates = cv.take<__nv_bfloat16>(Bt * T * 4 * H);
+    m.cst = cv.take<__nv_bfloat16>(Bt * T * H);
+    m.dz = cv.take<__nv_bfloat16>(B * (T + 1) * 4 * H);
+    m.dhout = cv.take<__nv_bfloat16>(((B + 127) / 128 * 128) * T * H);
+    m.pexch = cv.take<__nv_bfloat16>(((B + 127) / 128) * 2 * 16 * 128 * 64);
+    m.dpred = cv.take<float>(B * T * TC_OPAD);
+    m.dpb = cv.take<__nv_bfloat16>(T * ((B + 127) / 128) * 128 * 32);
+    m.head_wpart = cv.take<float>((size_t)m.head_wctas * HWG_PART);
     m.wg_part_elems = (size_t)64 * 384 * 1024;
-    m.wg_part = reinterpret_cast<float*>(take(m.wg_part_elems * 4));
+    m.wg_part = cv.take<float>(m.wg_part_elems);
   } else {
-    m.gates = nullptr; m.cst = nullptr; m.dz = nullptr; m.dhout = nullptr; m.dc = nullptr; m.wg_part = nullptr;
+    m.gates = nullptr; m.cst = nullptr; m.dz = nullptr; m.dhout = nullptr; m.wg_part = nullptr;
     m.dpred = nullptr; m.head_wpart = nullptr; m.pexch = nullptr; m.dpb = nullptr;
     m.wg_part_elems = 0;
   }
@@ -1217,21 +1151,21 @@ int tc_init(TcState& st, const lfmq_config& c) {
   if (m.dz) LFMQ_CUDA_CHECK(cudaMemset(m.dz, 0, B * (T + 1) * 4 * TC_H * 2));
   const uint64_t xh_row = (uint64_t)(T + 1) * TC_XH_LD;     // elements per batch row of the 2-D view
   int rc;
-  if ((rc = make_map_2d(&m.tm_h, m.xh, xh_row, B, xh_row * 2, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = make_map_2d(&m.tm_x, m.xh, xh_row, B, xh_row * 2, 32, 128, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
-  if ((rc = make_map_2d(&m.tm_h128, m.xh, xh_row, B, xh_row * 2, 64, 128, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = make_map_2d(&m.tm_wot, m.WoTp, TC_H, TC_OPAD, TC_H * 2, 64, 16, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = make_map_2d(&m.tm_wos, m.WoSp, 32, TC_H, 64, 32, 64, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_h, m.xh, xh_row, B, xh_row * 2, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_x, m.xh, xh_row, B, xh_row * 2, 32, 128, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_h128, m.xh, xh_row, B, xh_row * 2, 64, 128, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_wot, m.WoTp, TC_H, TC_OPAD, TC_H * 2, 64, 16, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_wos, m.WoSp, 32, TC_H, 64, 32, 64, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
   if (m.dpb &&
-      (rc = make_map_2d(&m.tm_dpb, m.dpb, 32, (uint64_t)m.T * ((m.maxB + 127) / 128) * 128, 64, 32, 128,
+      (rc = encode_map_2d(&m.tm_dpb, m.dpb, 32, (uint64_t)m.T * ((m.maxB + 127) / 128) * 128, 64, 32, 128,
                         CU_TENSOR_MAP_SWIZZLE_64B)))
     return rc;
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HT_SMEM));
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, HT_SMEM));
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HROWS_SMEM));
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, HROWS_SMEM));
-  if ((rc = make_map_2d(&m.tm_u, m.Up, TC_H, 4 * TC_H, TC_H * 2, 64, 256, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = make_map_2d(&m.tm_w, m.Wp, 32, 4 * TC_H, 64, 32, 256, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_u, m.Up, TC_H, 4 * TC_H, TC_H * 2, 64, 256, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_w, m.Wp, 32, 4 * TC_H, 64, 32, 256, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
   // how many 4-CTA clusters can be co-resident (one CTA per SM because of shared memory)
@@ -1276,7 +1210,7 @@ static int tc_pack_weights(TcState& st, const float* params, cudaStream_t s) {
   a.Wo = params + m.oWo; a.bo = params + m.obo; a.gamma = params + m.ogamma; a.beta = params + m.obeta;
   a.mean = params + m.omean; a.var = params + m.ovar;
   a.Up = m.Up; a.Wp = m.Wp; a.Ubk = m.Ubk; a.WoTp = m.WoTp; a.WoSp = m.WoSp; a.biasp = m.biasp; a.bop = m.bop;
-  if (int rc = launch_pdl(pack_all_kernel, dim3(a.nb_w + a.nb_h + a.nb_u), dim3(256), 0, s, 1, a)) return rc;
+  if (int rc = launch_pdl(pack_all_kernel, dim3(a.nb_w + a.nb_h + a.nb_u), dim3(256), 0, s, 1, true, a)) return rc;
   st.weights_dirty = 0;
   return 0;
 }
@@ -1284,7 +1218,7 @@ static int tc_pack_weights(TcState& st, const float* params, cudaStream_t s) {
 static int tc_run_recurrence(TcState& st, const float* x, int B, bool save, cudaStream_t s) {
   TcImpl& m = *st.impl;
   const long bt = (long)B * m.T * 5;
-  if (int rc = launch_pdl(xh_fill_x_kernel, dim3((int)((bt + 255) / 256)), dim3(256), 0, s, 1, B, m.T, m.I, x, m.xh)) return rc;
+  if (int rc = launch_pdl(xh_fill_x_kernel, dim3((int)((bt + 255) / 256)), dim3(256), 0, s, 1, true, B, m.T, m.I, x, m.xh)) return rc;
   const int n_tiles = (B + 127) / 128;
   FwdParams p;
   p.B = B; p.T = m.T;
@@ -1298,11 +1232,11 @@ static int tc_run_recurrence(TcState& st, const float* x, int B, bool save, cuda
   p.cst = save ? m.cst : nullptr;
   p.biasp = m.biasp;
   if (save) {
-    if (int rc = launch_pdl(lstm_fwd_tc_kernel<true>, dim3(TC_NC * p.n_clusters), dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, p,
+    if (int rc = launch_pdl(lstm_fwd_tc_kernel<true>, dim3(TC_NC * p.n_clusters), dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, true, p,
                             m.tm_h, m.tm_x, m.tm_u, m.tm_w))
       return rc;
   } else {
-    if (int rc = launch_pdl(lstm_fwd_tc_kernel<false>, dim3(TC_NC * p.n_clusters), dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, p,
+    if (int rc = launch_pdl(lstm_fwd_tc_kernel<false>, dim3(TC_NC * p.n_clusters), dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, true, p,
                             m.tm_h, m.tm_x, m.tm_u, m.tm_w))
       return rc;
   }
@@ -1321,12 +1255,7 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, f
   h.Wo = params + m.oWo; h.bo = params + m.obo;
   h.y = y; h.denom = denom; h.p1 = c.target_lambda; h.p2 = c.rnn_lambda;
   h.use_dropout = (c.train && c.dropout > 0.f) ? 1 : 0;
-  h.key.k0 = (uint32_t)(c.seed & 0xffffffffu);
-  h.key.k1 = (uint32_t)(c.seed >> 32);
-  h.key.stream = 0;
-  h.key.step = (uint32_t)(step & 0xffffffff);
-  h.key.thr = (uint32_t)((double)c.dropout * 16777216.0);
-  h.key.scale = 1.0f / (1.0f - c.dropout);
+  h.key = dropout_key(c.seed, 0, step, c.dropout);
   h.row0 = row0;
   h.preds = preds;
   // dhout / fp32 dpred are only produced on the dropout (SIMT) path; the tensor-core head leaves bf16 dpred tiles (dpb)
@@ -1345,7 +1274,7 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, f
   int n_wcta = m.head_wctas;
   if (train) {
     if (use_tc) {
-      if (int rc = launch_pdl(head_tc_kernel<true>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, h, hw, m.tm_h128, m.tm_wot,
+      if (int rc = launch_pdl(head_tc_kernel<true>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, true, h, hw, m.tm_h128, m.tm_wot,
                               m.tm_dpb, n_btiles, n_tiles_cap, m.head_wpart))
         return rc;
       n_wcta = grid;
@@ -1357,7 +1286,7 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, f
     }
   } else {
     if (use_tc) {
-      if (int rc = launch_pdl(head_tc_kernel<false>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, h, hw, m.tm_h128,
+      if (int rc = launch_pdl(head_tc_kernel<false>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, true, h, hw, m.tm_h128,
                               m.tm_wot, m.tm_wot, n_btiles, n_tiles_cap, (float*)nullptr))
         return rc;
     } else {
@@ -1367,14 +1296,14 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, f
   }
   if (y) {
     const int n_out = HWG_PART + HEAD_PART;
-    if (int rc = launch_pdl(head_reduce_kernel, dim3((n_out * 32 + 255) / 256), dim3(256), 0, s, 1, grid,
+    if (int rc = launch_pdl(head_reduce_kernel, dim3((n_out * 32 + 255) / 256), dim3(256), 0, s, 1, true, grid,
                             (const float*)m.head_part, n_wcta, (const float*)m.head_wpart, m.O, B, denom, c.target_lambda,
                             c.rnn_lambda, train ? 1 : 0, grads ? grads + m.oWo : (float*)nullptr,
                             grads ? grads + m.obo : (float*)nullptr, grads ? grads + m.ogamma : (float*)nullptr,
                             grads ? grads + m.obeta : (float*)nullptr, out2))
       return rc;
     if (train && use_tc) {
-      if (int rc = launch_pdl(head_fold_kernel, dim3((TC_H + 127) / 128), dim3(128), 0, s, 1, m.O, grads + m.oWo,
+      if (int rc = launch_pdl(head_fold_kernel, dim3((TC_H + 127) / 128), dim3(128), 0, s, 1, true, m.O, grads + m.oWo,
                               (const float*)(grads + m.obo), grads + m.ogamma, grads + m.obeta, params + m.oWo,
                               params + m.ogamma, params + m.obeta, params + m.omean, params + m.ovar, c.bn_epsilon))
         return rc;
@@ -1718,85 +1647,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
 }
 
 // =============================================================================================
-// Weight gradients as ONE wgmma GEMM over all B*(T+1) rows:  D[384 x 1024] = xh^T * dz   (both MN-major)
+// Weight gradients as ONE wgmma GEMM over all B*(T+1) rows (wgrad_gemm):  D[384 x 1024] = xh^T * dz   (both MN-major)
 //   rows 0..255 -> dU, rows 256..256+I-1 -> dW, row 288 (the constant-one column) -> db.
-// grid = (3 M-tiles, 4 N-tiles, S K-splits); deterministic split-K through fp32 partials.
 // =============================================================================================
-struct WgradParams {
-  int n_kblocks;        // ceil(rows / 64)
-  int kb_per_split;
-  float* partial;       // [S][384][1024]
-};
-
-constexpr int WG_THREADS = 2 * 128 + 32;     // two consumer warpgroups (M rows 0-63 / 64-127) + TMA producer warp
-constexpr int WG_STAGES = 4;
-constexpr uint32_t WG_STAGE_BYTES = 16384 + 32768;
-constexpr uint32_t WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
-
-__global__ void __launch_bounds__(WG_THREADS, 1)
-    wgrad_tc_kernel(WgradParams p, const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b) {
-  pdl_sync();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES);
-  uint64_t* empty = full + WG_STAGES;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m0 = blockIdx.x * 128, n0 = blockIdx.y * 256;
-  const int kb_beg = blockIdx.z * p.kb_per_split;
-  const int kb_end = min(p.n_kblocks, kb_beg + p.kb_per_split);
-  const int nkb = max(0, kb_end - kb_beg);
-
-  if (tid == 0) {
-    for (int s = 0; s < WG_STAGES; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);              // one arrive per consumer warp
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (warp == 8) {
-    if (lane == 0) {
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % WG_STAGES;
-        if (i >= WG_STAGES) mbar_wait(&empty[s], ((i / WG_STAGES) - 1) & 1);
-        mbar_arrive_expect_tx(&full[s], WG_STAGE_BYTES);
-        uint8_t* st = smem + s * WG_STAGE_BYTES;
-        const int krow = (kb_beg + i) * 64;
-        for (int mb = 0; mb < 2; ++mb) tma_load_2d(st + mb * 8192, &tm_a, &full[s], m0 + mb * 64, krow);
-        for (int nb = 0; nb < 4; ++nb) tma_load_2d(st + 16384 + nb * 8192, &tm_b, &full[s], n0 + nb * 64, krow);
-      }
-    }
-  } else {
-    const int wg = warp >> 2, w = warp & 3, cq = lane & 3;
-    float acc[128];
-#pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % WG_STAGES;
-      mbar_wait(&full[s], (i / WG_STAGES) & 1);
-      uint8_t* st = smem + s * WG_STAGE_BYTES;
-      wgmma_fence();
-#pragma unroll
-      for (int k16 = 0; k16 < 4; ++k16) {
-        const uint64_t da = make_smem_desc(smem_u32(st + wg * 8192) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-        const uint64_t db = make_smem_desc(smem_u32(st + 16384) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-        wgmma_m64n256k16<1, 1>(acc, da, db, 1);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                      // the previous stage's MMAs are complete: release it
-      if (i > 0 && lane == 0) mbar_arrive(&empty[(i - 1) % WG_STAGES]);
-    }
-    wgmma_wait<0>();
-    fence_regs(acc);
-    const int row = m0 + 64 * wg + 16 * w + (lane >> 2);
-    float* out = p.partial + ((long)blockIdx.z * 384 + row) * 1024 + n0 + 2 * cq;
-#pragma unroll
-    for (int i = 0; i < 128; i += 2)
-      *reinterpret_cast<float2*>(out + (long)8 * ((i >> 1) & 1) * 1024 + 8 * (i >> 2)) = make_float2(acc[i], acc[i + 1]);
-  }
-}
-
 // Sums the K-split partials and scatters D rows into dU / dW / db of the flat gradient vector.  D's columns are in
 // dz's order [16-unit block][gate][16]; the gradients want gate-major columns g*H + unit.
 __global__ void wgrad_reduce_kernel(int S, int I, const float* __restrict__ partial, float* __restrict__ gU,
@@ -1823,9 +1676,9 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
   if (!m.bwd_ready) {
     LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
     LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    LFMQ_CUDA_CHECK(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+    if ((rc = wgrad_gemm_init())) return rc;
     // boxes of 64 hidden units: the kernel loads its K-slice of U in rotated N order (own hidden slice first)
-    if ((rc = make_map_2d(&m.tm_ubk, m.Ubk, 256, 4 * TC_H, 512, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if ((rc = encode_map_2d(&m.tm_ubk, m.Ubk, 256, 4 * TC_H, 512, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
     cudaLaunchConfig_t qc = {};
     qc.gridDim = dim3(BWD_NC * (m.n_sms / BWD_NC));
     qc.blockDim = dim3(BWD_THREADS);
@@ -1864,14 +1717,14 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
       const uint64_t dims[3] = {1024, (uint64_t)(T + 1), (uint64_t)B};
       const uint64_t strides[2] = {2048, (uint64_t)2048 * (T + 1)};
       const uint32_t box[3] = {64, 1, 64};
-      if ((rc = make_map_nd(&tm_dzst, m.dz, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+      if ((rc = encode_map_bf16(&tm_dzst, m.dz, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
     }
     if (fused) {
-      if ((rc = launch_pdl(lstm_bwd_tc_kernel<true>, dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, bp,
+      if ((rc = launch_pdl(lstm_bwd_tc_kernel<true>, dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, true, bp,
                            m.tm_ubk, tm_dzst, m.tm_dpb, m.tm_wos)))
         return rc;
     } else {
-      if ((rc = launch_pdl(lstm_bwd_tc_kernel<false>, dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, bp,
+      if ((rc = launch_pdl(lstm_bwd_tc_kernel<false>, dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, true, bp,
                            m.tm_ubk, tm_dzst, m.tm_dpb, m.tm_wos)))
         return rc;
     }
@@ -1882,18 +1735,12 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
   // MN-major maps over exactly the B*(T+1) rows of this call (rows beyond are zero-filled by TMA)
   const uint64_t rows = (uint64_t)B * (T + 1);
   CUtensorMap tm_a, tm_b;
-  if ((rc = make_map_2d(&tm_a, m.xh, TC_XH_LD, rows, TC_XH_LD * 2, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = make_map_2d(&tm_b, m.dz, 4 * TC_H, rows, 4 * TC_H * 2, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  WgradParams wp;
-  wp.n_kblocks = (int)((rows + 63) / 64);
-  int S = m.n_sms / 12;                    // 3 x 4 output tiles per split: one wave of CTAs
-  if (S < 1) S = 1;
-  if (wp.n_kblocks < S) S = wp.n_kblocks;
-  wp.kb_per_split = (wp.n_kblocks + S - 1) / S;
-  S = (wp.n_kblocks + wp.kb_per_split - 1) / wp.kb_per_split;
-  wp.partial = m.wg_part;
-  if ((rc = launch_pdl(wgrad_tc_kernel, dim3(3, 4, S), dim3(WG_THREADS), WG_SMEM, s, 1, wp, tm_a, tm_b))) return rc;
-  if ((rc = launch_pdl(wgrad_reduce_kernel, dim3((384 * 1024 + 255) / 256), dim3(256), 0, s, 1, S, m.I,
+  if ((rc = encode_map_2d(&tm_a, m.xh, TC_XH_LD, rows, TC_XH_LD * 2, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&tm_b, m.dz, 4 * TC_H, rows, 4 * TC_H * 2, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  int S = 0, Mpad = 0;
+  if ((rc = wgrad_gemm(tm_a, tm_b, (long)rows, TC_XH_LD, 4 * TC_H, m.wg_part, m.wg_part_elems, true, s, &S, &Mpad)))
+    return rc;
+  if ((rc = launch_pdl(wgrad_reduce_kernel, dim3((384 * 1024 + 255) / 256), dim3(256), 0, s, 1, true, S, m.I,
                        (const float*)m.wg_part, grads + m.oU, grads + m.oW, grads + m.ob)))
     return rc;
   st.prof->end(LFMQ_REGION_WGRAD, s);

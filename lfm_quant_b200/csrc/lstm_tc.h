@@ -1,29 +1,17 @@
 // bf16 tensor-core path (LFMQ_PREC_BF16): persistent wgmma LSTM forward and backward recurrences, wgmma
 // weight-gradient GEMM and the fused HBM-bound head.  See lstm_tc.cu / DESIGN.md.
 #pragma once
-#include "../../include/lfmq.h"
-#include "common.cuh"
+#include "tc_shared.h"
 
 namespace lfmq {
-
-struct TcImpl;
-
-struct TcState {
-  // bookkeeping shared with the fp32 path
-  int64_t last_step = 0;
-  int64_t last_row0 = 0;
-  int weights_dirty = 1;
-  Profiler* prof = nullptr;
-  TcImpl* impl = nullptr;
-};
 
 // The shape family of the persistent cluster kernels: LSTM, point estimate, H = 256, L = 1, F <= 32, O <= 16, no
 // recurrent dropout.
 bool tc_shape_supported(const lfmq_config& cfg);
-// Extends the workspace carve (base may be null when only sizing); `off` is advanced.
 // offsets (in floats) of the single layer's tensors and the head in the flat parameter vector, from lfmq_api.cu:layout()
 struct TcParamOff { int64_t oW, oU, ob, ogamma, obeta, omean, ovar, oWo, obo; };
-void tc_layout(TcState& st, const lfmq_config& cfg, const TcParamOff& po, char* base, size_t& off);
+// Carves the cluster path's buffers from the workspace (only sizes them when the carver has no base).
+void tc_layout(TcState& st, const lfmq_config& cfg, const TcParamOff& po, Carver& cv);
 int tc_init(TcState& st, const lfmq_config& cfg);
 void tc_destroy(TcState& st);
 // preds may be null (training: the head is fused with the loss in tc_backward)

@@ -39,36 +39,9 @@ using namespace sm90;
 
 namespace {
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 // bf16 2-D map over a row-major [outer][inner] buffer, SWIZZLE_128B boxes of box_inner (= 64) x box_outer elements.
 int gmap_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer, uint32_t box_inner, uint32_t box_outer) {
-  static PFN_encodeTiled enc = nullptr;
-  if (!enc) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    LFMQ_CUDA_CHECK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-    enc = reinterpret_cast<PFN_encodeTiled>(fn);
-    if (!enc) {
-      LFMQ_SET_ERR("cuTensorMapEncodeTiled not available");
-      return LFMQ_ERR_CUDA;
-    }
-  }
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {inner * 2};
-  cuuint32_t box[2] = {box_inner, box_outer};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    LFMQ_SET_ERR("cuTensorMapEncodeTiled failed with %d (inner %llu outer %llu box %u x %u)", (int)r,
-                 (unsigned long long)inner, (unsigned long long)outer, box_inner, box_outer);
-    return LFMQ_ERR_CUDA;
-  }
-  return 0;
+  return encode_map_2d(m, base, inner, outer, inner * 2, box_inner, box_outer, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 inline long cdivl(long a, long b) { return (a + b - 1) / b; }
@@ -166,11 +139,6 @@ __device__ __forceinline__ void rec_mask4(const DropoutKey& k, int64_t grow, int
 
 __device__ __forceinline__ uint32_t ld_b32(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
 __device__ __forceinline__ void st_b32(__nv_bfloat16* p, uint32_t v) { *reinterpret_cast<uint32_t*>(p) = v; }
-
-__device__ __forceinline__ void pack16(const float v[16], uint32_t w[8]) {
-#pragma unroll
-  for (int e = 0; e < 8; ++e) w[e] = pack_bf16x2(v[2 * e], v[2 * e + 1]);
-}
 
 template <int BN>
 __device__ __forceinline__ void wgmma_bn(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -481,8 +449,7 @@ __global__ void __launch_bounds__(GSmem<BN, EPI>::THREADS, GSmem<BN, EPI>::CTAS_
           }
         }
         if (it == 0) {
-          griddep_wait();
-          griddep_launch_dependents();
+          pdl_sync();
         } else {
           // every CTA of the row-tile group has published step it-1 (generic-proxy stores, fenced before the count went up)
           const long long spin0 = clock64();
@@ -511,12 +478,10 @@ __global__ void __launch_bounds__(GSmem<BN, EPI>::THREADS, GSmem<BN, EPI>::CTAS_
         }
       }
     } else {
-      griddep_wait();
-      griddep_launch_dependents();
+      pdl_sync();
     }
   } else if (warp < 8) {
-    griddep_wait();
-    griddep_launch_dependents();
+    pdl_sync();
     const int wg = warp >> 2;
     const Frag f{64 * wg + 16 * (warp & 3) + (lane >> 2), lane & 3};
     const int rt = bx + g.rt_off;                    // 128-row tile index
@@ -564,84 +529,8 @@ __global__ void __launch_bounds__(GSmem<BN, EPI>::THREADS, GSmem<BN, EPI>::CTAS_
 }
 
 // =============================================================================================
-// Weight gradients: D[M x N] = A^T B over the T*Bp time-major rows, both operands MN-major straight from their
-// row-major buffers (the scheme of wgrad_tc_kernel in lstm_tc.cu, for any M, N).  grid = (M tiles of 128, N tiles of
-// 256, K splits); deterministic split-K through fp32 partials.
+// Weight gradients D = A^T B over the T*Bp time-major rows: wgrad_gemm (tc_shared.h) and the reductions of its partials
 // =============================================================================================
-struct GWgradParams {
-  int n_kblocks, kb_per_split, Mpad, Ntot;
-  float* partial;       // [S][Mpad][Ntot]
-};
-struct GWCfg {
-  static constexpr int THREADS = 2 * 128 + 32;      // two consumer warpgroups (M rows 0-63 / 64-127) + TMA producer warp
-  static constexpr uint32_t A_BYTES = 16384;
-  static constexpr uint32_t STAGE_BYTES = A_BYTES + 32768;
-  static constexpr int STAGES = (int)(196608u / STAGE_BYTES);
-  static constexpr uint32_t SMEM = STAGES * STAGE_BYTES + 1024 + 256;
-};
-
-__global__ void __launch_bounds__(GWCfg::THREADS, 1)
-    gwgrad_kernel(GWgradParams p, const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b) {
-  using C = GWCfg;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-  uint64_t* empty = full + C::STAGES;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m0 = blockIdx.x * 128, n0 = blockIdx.y * 256;
-  const int kb_beg = blockIdx.z * p.kb_per_split;
-  const int kb_end = min(p.n_kblocks, kb_beg + p.kb_per_split);
-  const int nkb = max(0, kb_end - kb_beg);
-  if (tid == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);              // one arrive per consumer warp
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (warp == 8) {
-    if (lane == 0) {
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % C::STAGES;
-        if (i >= C::STAGES) mbar_wait(&empty[s], ((i / C::STAGES) - 1) & 1);
-        mbar_arrive_expect_tx(&full[s], C::STAGE_BYTES);
-        uint8_t* st = smem + s * C::STAGE_BYTES;
-        const int krow = (kb_beg + i) * 64;
-        for (int mb = 0; mb < 2; ++mb) tma_load_2d(st + mb * 8192, &tm_a, &full[s], m0 + mb * 64, krow);
-        for (int nb = 0; nb < 4; ++nb) tma_load_2d(st + C::A_BYTES + nb * 8192, &tm_b, &full[s], n0 + nb * 64, krow);
-      }
-    }
-  } else {
-    const int wg = warp >> 2, cq = lane & 3;
-    float acc[128];
-#pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % C::STAGES;
-      mbar_wait(&full[s], (i / C::STAGES) & 1);
-      uint8_t* st = smem + s * C::STAGE_BYTES;
-      wgmma_fence();
-#pragma unroll
-      for (int k16 = 0; k16 < 4; ++k16) {
-        const uint64_t db = make_smem_desc(smem_u32(st + C::A_BYTES) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-        const uint64_t da = make_smem_desc(smem_u32(st + wg * 8192) + k16 * 2048, 8192, 1024, LAYOUT_SW128);
-        wgmma_m64n256k16<1, 1>(acc, da, db, 1);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                      // the previous stage's MMAs are complete: release it
-      if (i > 0 && lane == 0) mbar_arrive(&empty[(i - 1) % C::STAGES]);
-    }
-    wgmma_wait<0>();
-    fence_regs(acc);
-    const int row = m0 + 64 * wg + 16 * (warp & 3) + (lane >> 2);
-    float* out = p.partial + ((long)blockIdx.z * p.Mpad + row) * p.Ntot + n0 + 2 * cq;
-#pragma unroll
-    for (int i = 0; i < 128; i += 2)
-      *reinterpret_cast<float2*>(out + (long)8 * ((i >> 1) & 1) * p.Ntot + 8 * (i >> 2)) = make_float2(acc[i], acc[i + 1]);
-  }
-}
-
 // dst[row][n] = sum_z partial[z][row][n] for row < Mvalid (dst row-major [Mvalid][Ntot])
 // (rows row_first .. row_first + Mvalid - 1 of the partials)
 __global__ void gwgrad_reduce_kernel(int S, int Mvalid, int Mpad, int Ntot, const float* __restrict__ partial,
@@ -928,52 +817,32 @@ __global__ void __launch_bounds__(128) gcolsum_kernel(long rows, int N, long row
 }
 
 // =============================================================================================
-// Head on y = in[L] (bf16 [T][Bp][H], BN / Dropout already applied): Dense -> weighted MSE -> dpred, dy, loss sums.
-// One thread per row of a 128-row tile (TMA-staged, SW128), Wo broadcast from shared memory.
-// (rnn_point_estimate.py:105; model_utils/losses.py:55-135; SURVEY App. A.2-A.4)
+// bf16x3 head on y = in[L] (bf16 [T][Bp][H] + low halves, BN / Dropout already applied): pred = y Wo + bo accumulated in
+// fp32.  bf16x3 handles are forward-only (gen_supported), so this head only predicts.  One thread per row of a 128-row
+// tile (TMA-staged, SW128), Wo broadcast from shared memory.  (rnn_point_estimate.py:105)
 // =============================================================================================
 struct GHeadParams {
-  int B, T, O, H, Bp, NRT, target_idx, train;
+  int B, T, O, H, Bp, NRT;
   const float *Wo, *bo;
-  const float* y;            // targets [B][T][O] fp32 (null: predict)
-  const float* denom;
-  float p1, p2;
-  float* preds;              // [B][T][O] fp32 or null
-  const __nv_bfloat16* yin_lo;   // bf16x3: low halves of the head input (row-major, same layout), else null
-  __nv_bfloat16* dy;         // [T][Bp][H] (train)
-  float* dpred;              // [T*Bp][16] fp32 (train)
-  float* partial;            // [GH_PART][grid]
+  float* preds;              // [B][T][O] fp32
+  const __nv_bfloat16* yin_lo;   // low halves of the head input (row-major, same layout)
 };
-template <bool TRAIN>
 __global__ void __launch_bounds__(128, 1) ghead_rows_kernel(GHeadParams p, const __grid_constant__ CUtensorMap tm_y) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* tile = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nkb = p.H / 64;
   float* Wo_s = reinterpret_cast<float*>(tile + (size_t)nkb * 16384);          // [H][16]
   uint64_t* bar = reinterpret_cast<uint64_t*>(Wo_s + (size_t)p.H * GH_O);
-  __shared__ float red_s[GH_PART];
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x;
   for (int i = tid; i < p.H * GH_O; i += 128) {
     const int j = i / GH_O, k = i % GH_O;
     Wo_s[i] = (k < p.O) ? p.Wo[j * p.O + k] : 0.f;
   }
-  for (int i = tid; i < GH_PART; i += 128) red_s[i] = 0.f;
   if (tid == 0) {
     mbar_init(bar, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
-  if (TRAIN) {
-    const float Bg = p.denom[0], Mg = p.denom[1];
-    c_all = (1.f - p.p1) * (1.f - p.p2) / ((float)p.O * Mg);
-    c_last = (1.f - p.p1) * p.p2 / (Bg * (float)p.O);
-    c_tar = p.p1 / Bg;
-  }
-  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
-  float accbo[GH_O];
-#pragma unroll
-  for (int k = 0; k < GH_O; ++k) accbo[k] = 0.f;
   const int sw = tid & 7;
   uint32_t phase = 0;
   const int n_tiles = p.T * p.NRT;
@@ -986,11 +855,6 @@ __global__ void __launch_bounds__(128, 1) ghead_rows_kernel(GHeadParams p, const
       for (int kb = 0; kb < nkb; ++kb) tma_load_2d(tile + kb * 16384, &tm_y, bar, kb * 64, t * p.Bp + rt * 128);
     }
     const long r = b * p.T + t;          // row of the caller's [B][T][O] tensors
-    float yt[GH_O];
-#pragma unroll
-    for (int k = 0; k < GH_O; ++k) yt[k] = 0.f;
-    if (p.y && valid)
-      for (int k = 0; k < p.O; ++k) yt[k] = p.y[r * p.O + k];
     mbar_wait(bar, phase);
     phase ^= 1;
     const uint8_t* hrow = tile + tid * 128;
@@ -1025,139 +889,15 @@ __global__ void __launch_bounds__(128, 1) ghead_rows_kernel(GHeadParams p, const
     }
     if (p.preds && valid)
       for (int k = 0; k < p.O; ++k) p.preds[r * p.O + k] = pr[k];
-    if (p.y) {
-      bool any = false;
-#pragma unroll
-      for (int k = 0; k < GH_O; ++k) any |= (yt[k] != 0.0f);          // losses.py:72
-      const float mk = (any && valid) ? 1.f : 0.f;
-      const bool last = (t == p.T - 1);
-      float dp[GH_O];
-#pragma unroll
-      for (int k = 0; k < GH_O; ++k) {
-        const float d = (k < p.O && valid) ? (pr[k] * mk - yt[k]) : 0.f;  // losses.py:75
-        const float d2 = d * d;
-        s2 += d2;
-        float coef = c_all;
-        if (last) {
-          s1 += d2;
-          coef += c_last;
-          if (k == p.target_idx) {
-            s0 += d2;
-            coef += c_tar;
-          }
-        }
-        dp[k] = TRAIN ? 2.f * d * coef * mk : 0.f;
-        if (TRAIN) accbo[k] += dp[k];
-      }
-      if (TRAIN) {
-        const long rr = (long)t * p.Bp + b;       // time-major row (all 128 rows of the tile are written)
-#pragma unroll
-        for (int k4 = 0; k4 < GH_O; k4 += 4)
-          *reinterpret_cast<float4*>(p.dpred + rr * GH_O + k4) = make_float4(dp[k4], dp[k4 + 1], dp[k4 + 2], dp[k4 + 3]);
-        __nv_bfloat16* dyr = p.dy + rr * p.H;
-#pragma unroll 1
-        for (int c = 0; c < p.H / 16; ++c) {
-          float dv[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float4* w4 = reinterpret_cast<const float4*>(Wo_s + (c * 16 + e) * GH_O);
-            float sacc = 0.f;
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              const float4 w = w4[kk];
-              sacc = fmaf(dp[4 * kk + 0], w.x, sacc);
-              sacc = fmaf(dp[4 * kk + 1], w.y, sacc);
-              sacc = fmaf(dp[4 * kk + 2], w.z, sacc);
-              sacc = fmaf(dp[4 * kk + 3], w.w, sacc);
-            }
-            dv[e] = sacc;
-          }
-          uint32_t w[8];
-          pack16(dv, w);
-          st_global_v8(dyr + c * 16, w);
-        }
-      }
-    }
     __syncthreads();        // everyone is done with the tile before it is overwritten
   }
-  if (p.y) {
-    s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
-#pragma unroll
-    for (int k = 0; k < GH_O; ++k) accbo[k] = warp_sum(accbo[k]);
-    if (lane == 0) {
-      atomicAdd(&red_s[GH_O + 0], s0);
-      atomicAdd(&red_s[GH_O + 1], s1);
-      atomicAdd(&red_s[GH_O + 2], s2);
-      if (TRAIN)
-        for (int k = 0; k < GH_O; ++k) atomicAdd(&red_s[k], accbo[k]);
-    }
-    __syncthreads();
-    for (int i = tid; i < GH_PART; i += 128) p.partial[(long)i * gridDim.x + blockIdx.x] = red_s[i];
-  }
 }
 
-// dWo[j][k] = sum_rows y[row][j] dpred[row][k]: grid (row chunks, H/64); 256 threads = 64 units x 4 groups of 4 outputs.
-constexpr int GHW_ROWS = 32;
-__global__ void __launch_bounds__(256) ghead_wgrad_kernel(long rows, int H, const __nv_bfloat16* __restrict__ yin,
-                                                         const float* __restrict__ dpred, float* __restrict__ wpartial) {
-  __shared__ __align__(16) float y_s[GHW_ROWS][64];
-  __shared__ __align__(16) float dp_s[GHW_ROWS][GH_O];
-  const int tid = threadIdx.x;
-  const int j0 = blockIdx.y * 64;
-  const int jl = tid >> 2, kg = tid & 3;
-  float acc[4] = {0.f, 0.f, 0.f, 0.f};
-  for (long r0 = (long)blockIdx.x * GHW_ROWS; r0 < rows; r0 += (long)gridDim.x * GHW_ROWS) {
-    {   // 32 rows x 64 units = 256 chunks of 8
-      const int rr = tid >> 3, ch = tid & 7;
-      const long r = r0 + rr;
-      float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      if (r < rows) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(yin + r * H + j0 + ch * 8);
-        v[0] = bf16_lo(raw.x); v[1] = bf16_hi(raw.x); v[2] = bf16_lo(raw.y); v[3] = bf16_hi(raw.y);
-        v[4] = bf16_lo(raw.z); v[5] = bf16_hi(raw.z); v[6] = bf16_lo(raw.w); v[7] = bf16_hi(raw.w);
-      }
-      *reinterpret_cast<float4*>(&y_s[rr][ch * 8]) = make_float4(v[0], v[1], v[2], v[3]);
-      *reinterpret_cast<float4*>(&y_s[rr][ch * 8 + 4]) = make_float4(v[4], v[5], v[6], v[7]);
-    }
-    for (int idx = tid; idx < GHW_ROWS * GH_O; idx += 256) {
-      const long r = r0 + idx / GH_O;
-      dp_s[idx / GH_O][idx % GH_O] = (r < rows) ? dpred[r * GH_O + idx % GH_O] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int rr = 0; rr < GHW_ROWS; ++rr) {
-      const float yv = y_s[rr][jl];
-      const float4 dv = *reinterpret_cast<const float4*>(&dp_s[rr][kg * 4]);
-      acc[0] = fmaf(yv, dv.x, acc[0]);
-      acc[1] = fmaf(yv, dv.y, acc[1]);
-      acc[2] = fmaf(yv, dv.z, acc[2]);
-      acc[3] = fmaf(yv, dv.w, acc[3]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    wpartial[((long)(j0 + jl) * GH_O + kg * 4 + i) * gridDim.x + blockIdx.x] = acc[i];     // [value][cta]
-}
-
-// Sums the head partials: loss terms -> {loss, mse_0}, dbo, dWo.
-__global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial, int n_wcta,
-                                    const float* __restrict__ wpartial, int H, int O, const float* denom, float p1,
-                                    float p2, int train, float* __restrict__ gWo, float* __restrict__ gbo,
-                                    float* __restrict__ out2) {
-  const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // one warp per output value
+// Sums the tensor-core head's per-tile partials: loss terms -> {loss, mse_0}, dbo.
+__global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial, int O, const float* denom, float p1,
+                                    float p2, int train, float* __restrict__ gbo, float* __restrict__ out2) {
+  const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // one warp per output value
   const int lane = threadIdx.x & 31;
-  const int nW = H * GH_O;
-  if (i < nW) {
-    if (!train || !gWo) return;
-    const int j = i / GH_O, k = i % GH_O;
-    double s = 0.0;
-    for (int c = lane; c < n_wcta; c += 32) s += wpartial[(long)i * n_wcta + c];
-    s = warp_sum(s);
-    if (lane == 0 && k < O && gWo) gWo[j * O + k] = (float)s;
-    return;
-  }
-  const int q = i - nW;
   if (q >= GH_PART) return;
   double s = 0.0;
   for (int c = lane; c < n_cta; c += 32) s += partial[(long)q * n_cta + c];
@@ -1198,7 +938,6 @@ struct GenImpl {
   bool enabled = false;
   unsigned int* gbar = nullptr;         // grid-barrier counters of the persistent step launches (GBAR_N, zeroed per call)
   int gbar_next = 0;
-  int n_sms = 0;
   cudaStream_t side = nullptr;          // second half of the batch in the backward recurrence (see gen_backward)
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   int maxB = 0, Bp = 0, NRT = 0, T = 0, F = 0, O = 0, H = 0, L = 0, NB16 = 0;
@@ -1214,10 +953,10 @@ struct GenImpl {
   float *cstate = nullptr, *dcstate = nullptr;
   __nv_bfloat16 *dz = nullptr, *dy = nullptr, *dhout = nullptr;
   CUtensorMap tm_dz, tm_dz_mn;
-  float *dpred = nullptr, *head_part = nullptr, *head_wpart = nullptr, *bn_part = nullptr, *cs_part = nullptr;
+  float *bn_part = nullptr, *cs_part = nullptr;
   float* wg_part = nullptr;
   size_t wg_part_elems = 0;
-  int head_ctas = 0, head_wctas = 0, bn_ctas_max = 0, cs_chunks = 0;
+  int head_ctas = 0, bn_ctas_max = 0, cs_chunks = 0;
   int BNU = 128;      // hidden units per backward tile
 };
 
@@ -1237,15 +976,9 @@ bool gen_supported(const lfmq_config& c, char* why, size_t n) {
   return true;
 }
 
-void gen_layout(GenState& st, const lfmq_config& c, const GenLayerOff* lo, int64_t oWo, int64_t obo, char* base,
-                size_t& off) {
-  if (!st.impl) st.impl = new GenImpl;
-  GenImpl& m = *st.impl;
-  auto take = [&](size_t bytes) -> char* {
-    char* p = base ? base + off : nullptr;
-    off = (off + bytes + 1023) / 1024 * 1024;
-    return p;
-  };
+void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_t oWo, int64_t obo, Carver& cv) {
+  if (!st.gen) st.gen = new GenImpl;
+  GenImpl& m = *st.gen;
   m.maxB = c.max_batch; m.T = c.seq_len; m.F = c.n_inputs; m.O = c.n_outputs; m.H = c.num_hidden; m.L = c.num_layers;
   m.Bp = (c.max_batch + 127) / 128 * 128;
   m.NRT = m.Bp / 128;
@@ -1254,10 +987,6 @@ void gen_layout(GenState& st, const lfmq_config& c, const GenLayerOff* lo, int64
   m.train_ws = !c.forward_only;
   m.oWo = oWo; m.obo = obo;
   m.BNU = (m.H % 128 == 0) ? 128 : 64;
-  {   // experiment (LFMQ_GEN_BWD_BN64=1): 64-unit backward tiles also when H % 128 == 0 -> twice the CTAs per step
-    static const char* e = getenv("LFMQ_GEN_BWD_BN64");
-    if (e && atoi(e)) m.BNU = 64;
-  }
   const size_t T = m.T, Bp = m.Bp, H = m.H;
   const bool rec = (c.train && c.recurrent_dropout > 0.f);
   m.layers.assign(m.L, GenLayer{});
@@ -1267,45 +996,41 @@ void gen_layout(GenState& st, const lfmq_config& c, const GenLayerOff* lo, int64
     ly.I = lo[l].I;
     ly.Ipad = (ly.I + 63) / 64 * 64;
     ly.Kp = (int)H + ly.Ipad;
-    ly.hseq = reinterpret_cast<__nv_bfloat16*>(take((T + 1) * Bp * H * 2));
-    ly.hseq_lo = m.x3 ? reinterpret_cast<__nv_bfloat16*>(take((T + 1) * Bp * H * 2)) : nullptr;
-    ly.hmseq = rec ? reinterpret_cast<__nv_bfloat16*>(take((T + 1) * Bp * H * 2)) : nullptr;
-    ly.in = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * ly.Ipad * 2));
-    ly.in_lo = m.x3 ? reinterpret_cast<__nv_bfloat16*>(take(T * Bp * ly.Ipad * 2)) : nullptr;
-    ly.Wf = reinterpret_cast<__nv_bfloat16*>(take((size_t)4 * H * ly.Kp * 2));
-    ly.Wf_lo = m.x3 ? reinterpret_cast<__nv_bfloat16*>(take((size_t)4 * H * ly.Kp * 2)) : nullptr;
-    ly.biasp = reinterpret_cast<float*>(take(4 * H * 4));
-    ly.bn = reinterpret_cast<float*>(take(4 * H * 4));
+    ly.hseq = cv.take<__nv_bfloat16>((T + 1) * Bp * H);
+    ly.hseq_lo = m.x3 ? cv.take<__nv_bfloat16>((T + 1) * Bp * H) : nullptr;
+    ly.hmseq = rec ? cv.take<__nv_bfloat16>((T + 1) * Bp * H) : nullptr;
+    ly.in = cv.take<__nv_bfloat16>(T * Bp * ly.Ipad);
+    ly.in_lo = m.x3 ? cv.take<__nv_bfloat16>(T * Bp * ly.Ipad) : nullptr;
+    ly.Wf = cv.take<__nv_bfloat16>((size_t)4 * H * ly.Kp);
+    ly.Wf_lo = m.x3 ? cv.take<__nv_bfloat16>((size_t)4 * H * ly.Kp) : nullptr;
+    ly.biasp = cv.take<float>(4 * H);
+    ly.bn = cv.take<float>(4 * H);
     if (m.train_ws) {
-      ly.gates = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * 4 * H * 2));
-      ly.cst = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * H * 2));
-      ly.Ub = reinterpret_cast<__nv_bfloat16*>(take(H * 4 * H * 2));
-      ly.Wb = (l > 0) ? reinterpret_cast<__nv_bfloat16*>(take((size_t)ly.I * 4 * H * 2)) : nullptr;
+      ly.gates = cv.take<__nv_bfloat16>(T * Bp * 4 * H);
+      ly.cst = cv.take<__nv_bfloat16>(T * Bp * H);
+      ly.Ub = cv.take<__nv_bfloat16>(H * 4 * H);
+      ly.Wb = (l > 0) ? cv.take<__nv_bfloat16>((size_t)ly.I * 4 * H) : nullptr;
     } else {
       ly.gates = ly.cst = ly.Ub = ly.Wb = nullptr;
     }
   }
-  m.head_in = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * H * 2));
-  m.head_in_lo = m.x3 ? reinterpret_cast<__nv_bfloat16*>(take(T * Bp * H * 2)) : nullptr;
-  m.WoT = reinterpret_cast<__nv_bfloat16*>(take(16 * H * 2));
-  m.WoS = reinterpret_cast<__nv_bfloat16*>(take(H * 64 * 2));
-  m.head_tc_part = reinterpret_cast<float*>(take((size_t)GH_PART * T * m.NRT * 4));
-  m.dpb = m.train_ws ? reinterpret_cast<__nv_bfloat16*>(take(T * Bp * 64 * 2)) : nullptr;
-  m.cstate = reinterpret_cast<float*>(take(Bp * H * 4));
+  m.head_in = cv.take<__nv_bfloat16>(T * Bp * H);
+  m.head_in_lo = m.x3 ? cv.take<__nv_bfloat16>(T * Bp * H) : nullptr;
+  m.WoT = cv.take<__nv_bfloat16>(16 * H);
+  m.WoS = cv.take<__nv_bfloat16>(H * 64);
+  m.head_tc_part = cv.take<float>((size_t)GH_PART * T * m.NRT);
+  m.dpb = m.train_ws ? cv.take<__nv_bfloat16>(T * Bp * 64) : nullptr;
+  m.cstate = cv.take<float>(Bp * H);
   m.head_ctas = device_sm_count();
-  m.head_part = reinterpret_cast<float*>(take((size_t)GH_PART * m.head_ctas * 4));
   if (m.train_ws) {
-    m.dcstate = reinterpret_cast<float*>(take(Bp * H * 4));
-    m.dz = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * 4 * H * 2));
-    m.dy = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * H * 2));
-    m.dhout = reinterpret_cast<__nv_bfloat16*>(take(T * Bp * H * 2));
-    m.dpred = reinterpret_cast<float*>(take(T * Bp * GH_O * 4));
-    m.head_wctas = device_sm_count();
-    m.head_wpart = reinterpret_cast<float*>(take((size_t)H * GH_O * m.head_wctas * 4));
+    m.dcstate = cv.take<float>(Bp * H);
+    m.dz = cv.take<__nv_bfloat16>(T * Bp * 4 * H);
+    m.dy = cv.take<__nv_bfloat16>(T * Bp * H);
+    m.dhout = cv.take<__nv_bfloat16>(T * Bp * H);
     m.bn_ctas_max = (int)cdivl((long)T * m.maxB, GBN_ROWS);
-    m.bn_part = reinterpret_cast<float*>(take((size_t)2 * H * m.bn_ctas_max * 4));
+    m.bn_part = cv.take<float>((size_t)2 * H * m.bn_ctas_max);
     m.cs_chunks = 1024;
-    m.cs_part = reinterpret_cast<float*>(take((size_t)4 * H * m.cs_chunks * 4));
+    m.cs_part = cv.take<float>((size_t)4 * H * m.cs_chunks);
     const size_t Mmax = (H > 64 ? H : 128);               // dU: H rows; dW: Ipad rows (<= max(H, 64..1024))
     size_t mp = (Mmax + 255) / 256 * 256;
     for (int l = 0; l < m.L; ++l) {
@@ -1313,17 +1038,17 @@ void gen_layout(GenState& st, const lfmq_config& c, const GenLayerOff* lo, int64
       if (ip > mp) mp = ip;
     }
     m.wg_part_elems = (size_t)8 * mp * 4 * H;             // up to 8 K-splits
-    m.wg_part = reinterpret_cast<float*>(take(m.wg_part_elems * 4));
+    m.wg_part = cv.take<float>(m.wg_part_elems);
   }
 }
 
-int gen_init(GenState& st, const lfmq_config& c) {
+int gen_init(TcState& st, const lfmq_config& c) {
   char why[160];
   if (!gen_supported(c, why, sizeof(why))) {
     LFMQ_SET_ERR("tensor-core precision unsupported for this configuration: %s; use LFMQ_PREC_FP32", why);
     return LFMQ_ERR_UNSUPPORTED;
   }
-  GenImpl& m = *st.impl;
+  GenImpl& m = *st.gen;
   const size_t T = m.T, Bp = m.Bp, H = m.H;
   int rc;
   for (int l = 0; l < m.L; ++l) {
@@ -1365,7 +1090,6 @@ int gen_init(GenState& st, const lfmq_config& c) {
     LFMQ_CUDA_CHECK(cudaMemset(m.dz, 0, T * Bp * 4 * H * 2));
     LFMQ_CUDA_CHECK(cudaMemset(m.dy, 0, T * Bp * H * 2));
     LFMQ_CUDA_CHECK(cudaMemset(m.dhout, 0, T * Bp * H * 2));
-    LFMQ_CUDA_CHECK(cudaMemset(m.dpred, 0, T * Bp * GH_O * 4));
     if ((rc = gmap_2d(&m.tm_dz, m.dz, 4 * H, T * Bp, 64, 128))) return rc;
     if ((rc = gmap_2d(&m.tm_dz_mn, m.dz, 4 * H, T * Bp, 64, 64))) return rc;
   }
@@ -1380,21 +1104,15 @@ int gen_init(GenState& st, const lfmq_config& c) {
   LFMQ_GEMM_ATTR(128, EPI_STORE);
   LFMQ_GEMM_ATTR(64, EPI_STORE);
 #undef LFMQ_GEMM_ATTR
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(gwgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GWCfg::SMEM));
+  if ((rc = wgrad_gemm_init())) return rc;
   const int hsmem = (int)((H / 64) * 16384 + H * GH_O * 4 + 64 + 1024);
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(ghead_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(ghead_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem));
+  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(ghead_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hsmem));
   if (m.train_ws) {
     const int bsm = (256 / ((int)H / 8) > 0 ? 256 / ((int)H / 8) : 1) * 2 * (int)H * 4;
     LFMQ_CUDA_CHECK(cudaFuncSetAttribute(gbn_drop_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bsm));
   }
   LFMQ_CUDA_CHECK(cudaMalloc(&m.gbar, GBAR_N * sizeof(unsigned int)));
   LFMQ_CUDA_CHECK(cudaMemset(m.gbar, 0, GBAR_N * sizeof(unsigned int)));
-  {
-    int dev = 0;
-    LFMQ_CUDA_CHECK(cudaGetDevice(&dev));
-    LFMQ_CUDA_CHECK(cudaDeviceGetAttribute(&m.n_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
   m.enabled = true;
   st.weights_dirty = 1;
   return 0;
@@ -1405,64 +1123,34 @@ int gen_init(GenState& st, const lfmq_config& c) {
 // turns the mode off (one launch per time step, chained with programmatic dependent launch).
 static bool gen_can_persist(const GenImpl& m, long ctas, int n_concurrent, int per_sm, int n_steps) {
   static const bool on = !(getenv("LFMQ_GEN_PERSIST") && atoi(getenv("LFMQ_GEN_PERSIST")) == 0);
-  return on && n_steps > 1 && m.gbar != nullptr && ctas * n_concurrent <= (long)m.n_sms * per_sm &&
+  return on && n_steps > 1 && m.gbar != nullptr && ctas * n_concurrent <= (long)device_sm_count() * per_sm &&
          m.gbar_next + ctas * n_concurrent <= GBAR_N;
 }
 
-void gen_destroy(GenState& st) {
-  if (st.impl && st.impl->side) {
-    cudaStreamSynchronize(st.impl->side);
-    cudaEventDestroy(st.impl->ev_fork);
-    cudaEventDestroy(st.impl->ev_join);
-    cudaStreamDestroy(st.impl->side);
+void gen_destroy(TcState& st) {
+  if (st.gen && st.gen->side) {
+    cudaStreamSynchronize(st.gen->side);
+    cudaEventDestroy(st.gen->ev_fork);
+    cudaEventDestroy(st.gen->ev_join);
+    cudaStreamDestroy(st.gen->side);
   }
-  if (st.impl && st.impl->gbar) cudaFree(st.impl->gbar);
-  delete st.impl;
-  st.impl = nullptr;
+  if (st.gen && st.gen->gbar) cudaFree(st.gen->gbar);
+  delete st.gen;
+  st.gen = nullptr;
 }
 
-// Launch of one tile_gemm_kernel instantiation; `pdl`: with the programmatic-stream-serialization attribute (the
-// kernel waits for its predecessor itself, see the kernel).  LFMQ_GEN_PDL=0 turns the attribute off.
+// Launch of one tile_gemm_kernel instantiation; `pdl`: with the programmatic-stream-serialization attribute.  The kernel
+// loads weight tiles before its pdl_sync(), so a step may only overlap a predecessor that does not write them.
 template <int BN, int EPI>
 static int launch_tile_gemm(dim3 grid, cudaStream_t s, bool pdl, const GArgs& g, const EpiParams& ep, const CUtensorMap& a0,
                             const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& a3, const CUtensorMap& b0,
                             const CUtensorMap& b1) {
-  static const bool pdl_on = !(getenv("LFMQ_GEN_PDL") && atoi(getenv("LFMQ_GEN_PDL")) == 0);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = dim3(GSmem<BN, EPI>::THREADS);
-  cfg.dynamicSmemBytes = GSmem<BN, EPI>::TOTAL;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (pdl && pdl_on) ? 1 : 0;
-  LFMQ_CUDA_CHECK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<BN, EPI>, g, ep, a0, a1, a2, a3, b0, b1));
-  g_launches++;
-  if (debug_sync_on()) {
-    fprintf(stderr, "[lfmq launch] tile_gemm<%d,%d> grid %u x %u t=%d ...", BN, EPI, grid.x, grid.y, ep.t);
-    fflush(stderr);
-    cudaError_t e = cudaDeviceSynchronize();
-    fprintf(stderr, " %s\n", cudaGetErrorString(e));
-    fflush(stderr);
-  }
-  return 0;
+  return launch_pdl(tile_gemm_kernel<BN, EPI>, grid, dim3(GSmem<BN, EPI>::THREADS), GSmem<BN, EPI>::TOTAL, s, 1, pdl, g, ep,
+                    a0, a1, a2, a3, b0, b1);
 }
 
-static DropoutKey gkey(const lfmq_config& c, int stream, int64_t step, float rate) {
-  DropoutKey k;
-  k.k0 = (uint32_t)(c.seed & 0xffffffffu);
-  k.k1 = (uint32_t)(c.seed >> 32);
-  k.stream = (uint32_t)stream;
-  k.step = (uint32_t)(step & 0xffffffff);
-  k.thr = (uint32_t)((double)rate * 16777216.0);
-  k.scale = 1.0f / (1.0f - rate);
-  return k;
-}
-
-static int gen_pack(GenState& st, const float* params, float eps, cudaStream_t s) {
-  GenImpl& m = *st.impl;
+static int gen_pack(TcState& st, const float* params, float eps, cudaStream_t s) {
+  GenImpl& m = *st.gen;
   if (!st.weights_dirty) return 0;
   for (int l = 0; l < m.L; ++l) {
     GenLayer& ly = m.layers[l];
@@ -1484,9 +1172,9 @@ static int gen_pack(GenState& st, const float* params, float eps, cudaStream_t s
 }
 
 // all layers' recurrences + BN/Dropout; leaves in[L] (the head input)
-static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
+static int gen_run_trunk(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
                          int64_t step, bool save, cudaStream_t s) {
-  GenImpl& m = *st.impl;
+  GenImpl& m = *st.gen;
   const int T = m.T, H = m.H, Bp = m.Bp;
   const int nrt = (B + 127) / 128;
   const bool rec = c.train && c.recurrent_dropout > 0.f;
@@ -1510,7 +1198,7 @@ static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params
     ep.cst = save ? ly.cst : nullptr;
     ep.accurate = m.x3 ? 1 : 0;
     ep.use_rec = rec ? 1 : 0;
-    ep.rkey = gkey(c, 2 * l + 1, step, c.recurrent_dropout);
+    ep.rkey = dropout_key(c.seed, 2 * l + 1, step, c.recurrent_dropout);
     const CUtensorMap& th = rec ? ly.tm_hm : ly.tm_h;
     // steps 1 .. T-1 as ONE persistent launch when all its CTAs fit on the machine at once (see GArgs::n_steps)
     const long fwd_ctas = (long)nrt * (4 * H / 256);
@@ -1557,41 +1245,9 @@ static int gen_run_trunk(GenState& st, const lfmq_config& c, const float* params
     __nv_bfloat16* yo_lo = last ? m.head_in_lo : m.layers[l + 1].in_lo;
     const long n = (long)T * B * (H / 8);
     gbn_drop_fwd_kernel<<<(int)cdivl(n, 256), 256, 0, s>>>(B, T, H, Bp, ly.hseq, ly.hseq_lo, ly.bn, drop ? 1 : 0,
-                                                           gkey(c, 2 * l, step, c.dropout), row0, yo, yo_lo);
+                                                           dropout_key(c.seed, 2 * l, step, c.dropout), row0, yo, yo_lo);
     LFMQ_LAUNCH_CHECK();
   }
-  return 0;
-}
-
-// D[Mvalid x Ntot] = A^T B over the T*Bp time-major rows (split-K partials in wg_part, [S][Mpad][Ntot]); the caller reduces
-static int gen_wgrad_gemm(GenImpl& m, const CUtensorMap& tm_a, const CUtensorMap& tm_b, int Mvalid, int Ntot, int* S_out,
-                          int* Mpad_out, cudaStream_t s) {
-  const int mt = (Mvalid + 127) / 128;
-  const int Mpad = mt * 128;
-  const long rows = (long)m.T * m.Bp;
-  GWgradParams wp;
-  wp.n_kblocks = (int)cdivl(rows, 64);
-  // K splits: fill the machine, within what the partial buffer holds (the head's [H x 16] product has one N tile and
-  // wants many splits; the gate products have 8-16 output tiles and get 8)
-  int S = m.n_sms / (mt * (Ntot / 256));
-  const size_t smax = m.wg_part_elems / ((size_t)Mpad * Ntot);
-  if ((size_t)S > smax) S = (int)smax;
-  if (S > 64) S = 64;
-  if (S < 1) S = 1;
-  if (S > wp.n_kblocks) S = wp.n_kblocks;
-  wp.kb_per_split = (wp.n_kblocks + S - 1) / S;
-  S = (wp.n_kblocks + wp.kb_per_split - 1) / wp.kb_per_split;
-  wp.Mpad = Mpad;
-  wp.Ntot = Ntot;
-  wp.partial = m.wg_part;
-  if ((size_t)S * Mpad * Ntot > m.wg_part_elems) {
-    LFMQ_SET_ERR("weight-gradient partial buffer too small");
-    return LFMQ_ERR_WORKSPACE;
-  }
-  gwgrad_kernel<<<dim3(mt, Ntot / 256, S), GWCfg::THREADS, GWCfg::SMEM, s>>>(wp, tm_a, tm_b);
-  LFMQ_LAUNCH_CHECK();
-  *S_out = S;
-  *Mpad_out = Mpad;
   return 0;
 }
 
@@ -1599,7 +1255,9 @@ static int gen_wgrad_gemm(GenImpl& m, const CUtensorMap& tm_a, const CUtensorMap
 static int gen_wgrad(GenImpl& m, const CUtensorMap& tm_a, int Mvalid, float* dst, cudaStream_t s, float* db = nullptr) {
   const int Ntot = 4 * m.H;
   int S = 0, Mpad = 0, rc;
-  if ((rc = gen_wgrad_gemm(m, tm_a, m.tm_dz_mn, db ? Mvalid + 1 : Mvalid, Ntot, &S, &Mpad, s))) return rc;
+  if ((rc = wgrad_gemm(tm_a, m.tm_dz_mn, (long)m.T * m.Bp, db ? Mvalid + 1 : Mvalid, Ntot, m.wg_part, m.wg_part_elems,
+                       false, s, &S, &Mpad)))
+    return rc;
   const long n4 = (long)Mvalid * Ntot / 4;
   gwgrad_reduce_kernel<<<(int)cdivl(n4, 256), 256, 0, s>>>(S, Mvalid, Mpad, Ntot, m.wg_part, dst, 0);
   LFMQ_LAUNCH_CHECK();
@@ -1610,97 +1268,74 @@ static int gen_wgrad(GenImpl& m, const CUtensorMap& tm_a, int Mvalid, float* dst
   return 0;
 }
 
-static int gen_run_head(GenState& st, const lfmq_config& c, const float* params, float* grads, const float* y, int B,
+static int gen_run_head(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* y, int B,
                         const float* denom, float* preds, float* out2, bool train, cudaStream_t s) {
-  GenImpl& m = *st.impl;
-  GHeadParams h = {};
-  h.B = B; h.T = m.T; h.O = m.O; h.H = m.H; h.Bp = m.Bp; h.NRT = (B + 127) / 128; h.target_idx = c.target_idx;
-  h.train = train ? 1 : 0;
-  h.Wo = params + m.oWo; h.bo = params + m.obo;
-  h.y = y; h.denom = denom; h.p1 = c.target_lambda; h.p2 = c.rnn_lambda;
-  h.preds = preds;
-  h.yin_lo = m.head_in_lo;
-  h.dy = train ? m.dy : nullptr;
-  h.dpred = train ? m.dpred : nullptr;
-  h.partial = m.head_part;
-  if (!m.x3) {
-    // Tensor-core head: pred = y Wo as a wgmma GEMM (N = 16) with the loss in its epilogue; training adds
-    // dy = dpred Wo^T (K = 16 padded to one k-block) and dWo = y^T dpred (the weight-gradient GEMM, N padded to 256).
-    // The fp32-accumulating SIMT head below stays for LFMQ_PREC_BF16X3 (1e-4 tolerance).
-    const int ntile = m.T * m.NRT;                  // every row tile of the time-major buffers (zeros beyond the batch)
-    EpiParams ep = {};
-    ep.T = m.T; ep.B = B; ep.Bp = m.Bp; ep.H = m.H; ep.NRT = m.NRT; ep.NB16 = m.NB16;
-    ep.hy = y; ep.hdenom = denom; ep.hbo = params + m.obo; ep.hpreds = preds; ep.hdpb = m.dpb;
-    ep.hpartial = m.head_tc_part; ep.hp1 = c.target_lambda; ep.hp2 = c.rnn_lambda; ep.hO = m.O;
-    ep.htarget = c.target_idx; ep.htrain = train ? 1 : 0;
-    GArgs g = {};
-    g.n_seg = 1;
-    g.seg[0] = GSeg{0, 0, m.H / 64, 0, 0};
-    int rc;
-    if ((rc = launch_tile_gemm<16, EPI_HEAD>(dim3(ntile, 1), s, false, g, ep, m.tm_head_in, m.tm_head_in, m.tm_head_in,
-                                                m.tm_head_in, m.tm_wot, m.tm_wot)))
-      return rc;
-    if (train) {
-      EpiParams es = {};
-      es.out = m.dy;
-      es.ldc = m.H;
-      es.Bp = m.Bp;
-      GArgs gd = {};
-      gd.n_seg = 1;
-      gd.seg[0] = GSeg{0, 0, 1, 0, 0};
-      const int row_tiles = m.T * m.Bp / 128;
-      gd.lin_cols = (m.H % 128 == 0) ? m.H / 128 : m.H / 64;
-      if (m.H % 128 == 0)
-        rc = launch_tile_gemm<128, EPI_STORE>(dim3(row_tiles * (m.H / 128)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
-                                                 m.tm_dpb, m.tm_wos, m.tm_wos);
-      else
-        rc = launch_tile_gemm<64, EPI_STORE>(dim3(row_tiles * (m.H / 64)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
-                                                m.tm_dpb, m.tm_wos, m.tm_wos);
-      if (rc) return rc;
-      int S = 0, Mpad = 0;
-      if ((rc = gen_wgrad_gemm(m, m.tm_head_in_mn, m.tm_dpb_mn, m.H, 256, &S, &Mpad, s))) return rc;
-      ghead_wo_reduce_kernel<<<(m.H * m.O + 255) / 256, 256, 0, s>>>(S, m.H, m.O, Mpad, m.wg_part, grads + m.oWo);
-      LFMQ_LAUNCH_CHECK();
-    }
-    if (y) {
-      const int n_out = m.H * GH_O + GH_PART;
-      ghead_reduce_kernel<<<(n_out * 32 + 255) / 256, 256, 0, s>>>(ntile, m.head_tc_part, 0, nullptr, m.H, m.O, denom,
-                                                                 c.target_lambda, c.rnn_lambda, train ? 1 : 0, nullptr,
-                                                                 grads ? grads + m.obo : nullptr, out2);
-      LFMQ_LAUNCH_CHECK();
-    }
+  GenImpl& m = *st.gen;
+  if (m.x3) {
+    // LFMQ_PREC_BF16X3 (1e-4 tolerance): the fp32-accumulating SIMT head.  Its handles are forward-only, so it predicts.
+    GHeadParams h = {};
+    h.B = B; h.T = m.T; h.O = m.O; h.H = m.H; h.Bp = m.Bp; h.NRT = (B + 127) / 128;
+    h.Wo = params + m.oWo; h.bo = params + m.obo;
+    h.preds = preds;
+    h.yin_lo = m.head_in_lo;
+    int grid = m.T * h.NRT;
+    if (grid > m.head_ctas) grid = m.head_ctas;
+    const int hsmem = (m.H / 64) * 16384 + m.H * GH_O * 4 + 64 + 1024;
+    ghead_rows_kernel<<<grid, 128, hsmem, s>>>(h, m.tm_head_in);
+    LFMQ_LAUNCH_CHECK();
     return 0;
   }
-  int grid = m.T * h.NRT;
-  if (grid > m.head_ctas) grid = m.head_ctas;
-  const int hsmem = (m.H / 64) * 16384 + m.H * GH_O * 4 + 64 + 1024;
-  if (train)
-    ghead_rows_kernel<true><<<grid, 128, hsmem, s>>>(h, m.tm_head_in);
-  else
-    ghead_rows_kernel<false><<<grid, 128, hsmem, s>>>(h, m.tm_head_in);
-  LFMQ_LAUNCH_CHECK();
-  int n_wcta = 0;
+  // Tensor-core head: pred = y Wo as a wgmma GEMM (N = 16) with the loss in its epilogue; training adds
+  // dy = dpred Wo^T (K = 16 padded to one k-block) and dWo = y^T dpred (the weight-gradient GEMM, N padded to 256).
+  const int ntile = m.T * m.NRT;                  // every row tile of the time-major buffers (zeros beyond the batch)
+  EpiParams ep = {};
+  ep.T = m.T; ep.B = B; ep.Bp = m.Bp; ep.H = m.H; ep.NRT = m.NRT; ep.NB16 = m.NB16;
+  ep.hy = y; ep.hdenom = denom; ep.hbo = params + m.obo; ep.hpreds = preds; ep.hdpb = m.dpb;
+  ep.hpartial = m.head_tc_part; ep.hp1 = c.target_lambda; ep.hp2 = c.rnn_lambda; ep.hO = m.O;
+  ep.htarget = c.target_idx; ep.htrain = train ? 1 : 0;
+  GArgs g = {};
+  g.n_seg = 1;
+  g.seg[0] = GSeg{0, 0, m.H / 64, 0, 0};
+  int rc;
+  if ((rc = launch_tile_gemm<16, EPI_HEAD>(dim3(ntile, 1), s, false, g, ep, m.tm_head_in, m.tm_head_in, m.tm_head_in,
+                                              m.tm_head_in, m.tm_wot, m.tm_wot)))
+    return rc;
   if (train) {
-    // rows of the time-major buffers: T * Bp (rows >= B of a tile carry dpred = 0)
-    const long rows = (long)m.T * m.Bp;
-    n_wcta = m.head_wctas;
-    ghead_wgrad_kernel<<<dim3(n_wcta, m.H / 64), 256, 0, s>>>(rows, m.H, m.head_in, m.dpred, m.head_wpart);
+    EpiParams es = {};
+    es.out = m.dy;
+    es.ldc = m.H;
+    es.Bp = m.Bp;
+    GArgs gd = {};
+    gd.n_seg = 1;
+    gd.seg[0] = GSeg{0, 0, 1, 0, 0};
+    const int row_tiles = m.T * m.Bp / 128;
+    gd.lin_cols = (m.H % 128 == 0) ? m.H / 128 : m.H / 64;
+    if (m.H % 128 == 0)
+      rc = launch_tile_gemm<128, EPI_STORE>(dim3(row_tiles * (m.H / 128)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
+                                               m.tm_dpb, m.tm_wos, m.tm_wos);
+    else
+      rc = launch_tile_gemm<64, EPI_STORE>(dim3(row_tiles * (m.H / 64)), s, false, gd, es, m.tm_dpb, m.tm_dpb, m.tm_dpb,
+                                              m.tm_dpb, m.tm_wos, m.tm_wos);
+    if (rc) return rc;
+    int S = 0, Mpad = 0;
+    if ((rc = wgrad_gemm(m.tm_head_in_mn, m.tm_dpb_mn, (long)m.T * m.Bp, m.H, 256, m.wg_part, m.wg_part_elems, false, s,
+                         &S, &Mpad)))
+      return rc;
+    ghead_wo_reduce_kernel<<<(m.H * m.O + 255) / 256, 256, 0, s>>>(S, m.H, m.O, Mpad, m.wg_part, grads + m.oWo);
     LFMQ_LAUNCH_CHECK();
   }
   if (y) {
-    const int n_out = m.H * GH_O + GH_PART;
-    ghead_reduce_kernel<<<(n_out * 32 + 255) / 256, 256, 0, s>>>(grid, m.head_part, n_wcta, m.head_wpart, m.H, m.O, denom,
-                                                               c.target_lambda, c.rnn_lambda, train ? 1 : 0,
-                                                               grads ? grads + m.oWo : nullptr,
-                                                               grads ? grads + m.obo : nullptr, out2);
+    ghead_reduce_kernel<<<(GH_PART * 32 + 255) / 256, 256, 0, s>>>(ntile, m.head_tc_part, m.O, denom, c.target_lambda,
+                                                                  c.rnn_lambda, train ? 1 : 0,
+                                                                  grads ? grads + m.obo : nullptr, out2);
     LFMQ_LAUNCH_CHECK();
   }
   return 0;
 }
 
-int gen_forward(GenState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
+int gen_forward(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
                 int64_t step, float* preds, cudaStream_t s) {
-  if (!st.impl || !st.impl->enabled) {
+  if (!st.gen || !st.gen->enabled) {
     LFMQ_SET_ERR("general tensor-core path not initialised");
     return LFMQ_ERR_UNSUPPORTED;
   }
@@ -1715,13 +1350,13 @@ int gen_forward(GenState& st, const lfmq_config& c, const float* params, const f
   return 0;
 }
 
-int gen_backward(GenState& st, const lfmq_config& c, const float* params, float* grads, const float* x, const float* y,
+int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* x, const float* y,
                  int B, int64_t row0, int64_t step, const float* denom, float* tail, cudaStream_t s) {
-  if (!st.impl || !st.impl->enabled || !st.impl->train_ws) {
+  if (!st.gen || !st.gen->enabled || !st.gen->train_ws) {
     LFMQ_SET_ERR("general tensor-core path not initialised for training");
     return LFMQ_ERR_UNSUPPORTED;
   }
-  GenImpl& m = *st.impl;
+  GenImpl& m = *st.gen;
   const int T = m.T, H = m.H, Bp = m.Bp;
   const int nrt = (B + 127) / 128;
   const bool rec = c.train && c.recurrent_dropout > 0.f;
@@ -1736,7 +1371,6 @@ int gen_backward(GenState& st, const lfmq_config& c, const float* params, float*
     // so the rows of the row tiles that are not launched now must be zero (they may hold an earlier call's values)
     const size_t tail_rows = (size_t)(Bp - nrt * 128);
     LFMQ_CUDA_CHECK(cudaMemset2DAsync(m.dz + (size_t)nrt * 128 * 4 * H, (size_t)Bp * 4 * H * 2, 0, tail_rows * 4 * H * 2, T, s));
-    LFMQ_CUDA_CHECK(cudaMemset2DAsync(m.dpred + (size_t)nrt * 128 * GH_O, (size_t)Bp * GH_O * 4, 0, tail_rows * GH_O * 4, T, s));
   }
   st.prof->begin(LFMQ_REGION_HEAD, s);
   if ((rc = gen_run_head(st, c, params, grads, y, B, denom, nullptr, tail, true, s))) return rc;
@@ -1748,7 +1382,7 @@ int gen_backward(GenState& st, const lfmq_config& c, const float* params, float*
       const int ctas = (int)cdivl((long)T * B, GBN_ROWS);
       const int RL = 256 / (H / 8) > 0 ? 256 / (H / 8) : 1;
       gbn_drop_bwd_kernel<<<ctas, 256, RL * 2 * H * 4, s>>>(B, T, H, Bp, m.dy, ly.hseq, ly.bn, drop ? 1 : 0,
-                                                           gkey(c, 2 * l, step, c.dropout), row0, m.dhout, m.bn_part);
+                                                           dropout_key(c.seed, 2 * l, step, c.dropout), row0, m.dhout, m.bn_part);
       LFMQ_LAUNCH_CHECK();
       gpartial_reduce_kernel<<<(2 * H * 32 + 255) / 256, 256, 0, s>>>(ctas, H, H, m.bn_part, grads + ly.off.ogamma,
                                                                     grads + ly.off.obeta);
@@ -1758,12 +1392,11 @@ int gen_backward(GenState& st, const lfmq_config& c, const float* params, float*
     ep.T = T; ep.B = B; ep.Bp = Bp; ep.H = H; ep.NRT = m.NRT; ep.NB16 = m.NB16; ep.row0 = row0;
     ep.gates = ly.gates; ep.cst = ly.cst; ep.dhout = m.dhout; ep.dcstate = m.dcstate; ep.dz = m.dz;
     ep.use_rec = rec ? 1 : 0;
-    ep.rkey = gkey(c, 2 * l + 1, step, c.recurrent_dropout);
+    ep.rkey = dropout_key(c.seed, 2 * l + 1, step, c.recurrent_dropout);
     // The step's epilogue is HBM-bound (saved gates / cell states in, dz out: ~46 MB per step at H = 512) and its
     // mainloop L2-bound, and one launch puts every CTA into the same phase at the same time.  Two half-batches on two
     // streams (each its own PDL chain) drift apart, so one half's epilogue runs beside the other's mainloop.
-    static const char* split_env = getenv("LFMQ_GEN_SPLIT");      // 0 / 1 force, unset: by tile count
-    const bool split = split_env ? (atoi(split_env) != 0 && nrt >= 2) : (nrt >= 16);
+    const bool split = nrt >= 16;
     const int n_a = split ? (nrt + 1) / 2 : nrt, n_b = nrt - n_a;
     if (split) {
       if (!m.side) {

@@ -138,13 +138,6 @@ __device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const CUtensor
       : "memory");
 }
 
-// ---- programmatic dependent launch ----------------------------------------------------------------
-// wait: returns once the preceding kernel of the stream has completed and its writes are visible (a no-op when the
-// kernel was not launched with the programmatic-stream-serialization attribute); launch_dependents: the next kernel's
-// CTAs may be dispatched as soon as every CTA of this grid has executed it (or exited).
-__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // ---- register re-allocation between warpgroups (4 aligned consecutive warps execute it together) ---------
 template <int N>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }

@@ -63,6 +63,21 @@ def test_workspace_bytes_and_validation_without_gpu():
         N.check(lib.lfmq_workspace_bytes(C.byref(_cfg(num_layers=0)), C.byref(n)))
 
 
+def test_tensor_core_workspace_leaves_out_fp32_activations():
+    """A bf16 handle carves only its own path's buffers, not the fp32 path's per-layer h, c, y (at B=65536, T=48, H=256
+    those alone are 3*B*T*H*4 bytes = 9.7 GB)."""
+    lib = N.load()
+
+    def ws(precision, max_batch=4096, forward_only=0):
+        n = C.c_uint64(0)
+        cfg = _cfg(max_batch=max_batch, seq_len=48, num_hidden=256, precision=precision, forward_only=forward_only)
+        N.check(lib.lfmq_workspace_bytes(C.byref(cfg), C.byref(n)))
+        return n.value
+
+    assert ws(N.PREC_BF16) < ws(N.PREC_FP32)
+    assert ws(N.PREC_BF16, 65536, 1) < ws(N.PREC_FP32, 65536, 1)
+
+
 def test_engine_refuses_to_run_without_cuda():
     import torch
     if torch.cuda.is_available():
