@@ -100,8 +100,8 @@ __global__ void xh_fill_x_kernel(int B, int T, int F, const float* __restrict__ 
 }
 
 // Weight slices in the order the forward kernel consumes them.  Gate g of hidden unit 64r + 16c + jj is row
-// n = 64c + 16g + jj of slice r (four 16-unit chunks of 64 gate columns each: the MMAs are issued and committed chunk by
-// chunk, so the epilogue of chunk c runs under the MMAs of chunk c+1); the three sigmoid gates are pre-scaled by 0.5
+// n = 64c + 16g + jj of slice r (four 16-unit chunks of 64 gate columns each: the MMAs are issued and committed two
+// chunks at a time, so the epilogue of chunks 0-1 runs under the MMAs of chunks 2-3); the three sigmoid gates are pre-scaled by 0.5
 // (sigmoid(z) = 0.5*tanh(z/2) + 0.5).
 __device__ __forceinline__ void pack_weights_body(int bid, int I, const float* __restrict__ W, const float* __restrict__ U,
                                     const float* __restrict__ bias, __nv_bfloat16* __restrict__ Up,
@@ -161,7 +161,7 @@ struct FwdBars {
 
 // Post-activation gates i|f|g|o of units jj, jj + 1 (row half h, pair q) from a 64-column chunk of the accumulator:
 // gate g of unit jj + e is fragment register 4 (2 g + q) + 2 h + e.  The sigmoid gates come pre-scaled by 1/2.
-__device__ __forceinline__ void fwd_gates(const float (&a)[32], const float* bs, int h, int q, int jj, float (&gv)[4][2]) {
+__device__ __forceinline__ void fwd_gates(const float* a, const float* bs, int h, int q, int jj, float (&gv)[4][2]) {
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     const int ri = 2 * h + e;
@@ -243,7 +243,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
     const int r0 = 64 * wg + 16 * w + (lane >> 2);
     mbar_wait(&bars->w_full, 0);
     uint32_t n_xf = 0, n_hf = 0;
-    float acc[4][32];
+    float acc[2][64];                       // [half g]: chunks 2 g (registers 0-31) and 2 g + 1 (32-63)
     float cstate[4][2][2][2];               // [chunk][row half h][pair p][e]
     for (int it = 0; it < p.n_iters; ++it) {
       const int tile_c = it * p.n_clusters + cid;
@@ -255,48 +255,49 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
 #pragma unroll
           for (int q = 0; q < 2; ++q) cstate[c][h][q][0] = cstate[c][h][q][1] = 0.f;
       for (int t = 0; t < T; ++t) {
-        // x part of all four chunks first (it does not wait for h), then the h part chunk by chunk, each chunk its own
-        // commit group: the cell update of chunk c overlaps the MMAs of chunks c+1..
+        // Two 128-column halves (chunks 2 g, 2 g + 1: an m64n128 fragment is the two m64n64 fragments side by side), each
+        // its own commit group for the h part: the cell update of chunks 0-1 overlaps the MMAs of chunks 2-3.  Against
+        // one group per 64-column chunk, each k-step re-reads the h tile's A operand from shared memory half as often.
+        // The x part of both halves goes first: it does not wait for h.
         mbar_wait(&bars->x_full, (n_xf++) & 1);
         wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 4; ++c)
+        for (int g = 0; g < 2; ++g)
           for (int k16 = 0; k16 < p.k16_x; ++k16) {
             const uint64_t da = make_smem_desc(smem_u32(smem + SM_X0 + wg * 4096) + k16 * 32, 0, 512, LAYOUT_SW64);
-            const uint64_t db = make_smem_desc(smem_u32(smem + SM_W + c * 4096) + k16 * 32, 0, 512, LAYOUT_SW64);
-            wgmma_m64n64k16<0, 0>(acc[c], da, db, k16 > 0);
+            const uint64_t db = make_smem_desc(smem_u32(smem + SM_W + g * 8192) + k16 * 32, 0, 512, LAYOUT_SW64);
+            wgmma_m64n128k16<0, 0>(acc[g], da, db, k16 > 0);
           }
         wgmma_commit();
         if (t > 0) {
           mbar_wait(&bars->h_full, (n_hf++) & 1);
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
+          for (int g = 0; g < 2; ++g) {
 #pragma unroll
             for (int kb = 0; kb < 4; ++kb)
 #pragma unroll
               for (int k16 = 0; k16 < 4; ++k16) {
                 const uint64_t da = make_smem_desc(smem_u32(smem + SM_H0 + kb * 16384 + wg * 8192) + k16 * 32, 0, 1024,
                                                    LAYOUT_SW128);
-                const uint64_t db = make_smem_desc(smem_u32(smem + SM_U + kb * 32768 + c * 8192) + k16 * 32, 0, 1024,
+                const uint64_t db = make_smem_desc(smem_u32(smem + SM_U + kb * 32768 + g * 16384) + k16 * 32, 0, 1024,
                                                    LAYOUT_SW128);
-                wgmma_m64n64k16<0, 0>(acc[c], da, db, 1);
+                wgmma_m64n128k16<0, 0>(acc[g], da, db, 1);
               }
             wgmma_commit();
           }
-          wgmma_wait<4>();
+          wgmma_wait<2>();
         } else {
           wgmma_wait<0>();
         }
         if (lane == 0) mbar_arrive(&bars->x_empty);      // the x tile has been read
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
-          if (t > 0) {
-            if (c == 0) wgmma_wait<3>();
-            if (c == 1) wgmma_wait<2>();
-            if (c == 2) wgmma_wait<1>();
-            if (c == 3) wgmma_wait<0>();
-          }
-          fence_regs(acc[c]);
+          // Unconditional although nothing is in flight at t = 0: behind a branch on t, ptxas cannot follow the commit
+          // groups and serialises every wgmma of the kernel (C7514).
+          if (c == 0) wgmma_wait<1>();
+          if (c == 2) wgmma_wait<0>();
+          if ((c & 1) == 0) fence_regs(acc[c >> 1]);
+          const float* ac = acc[c >> 1] + 32 * (c & 1);
           const float* bs = bias_s + c * 64;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -306,7 +307,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
             for (int q = 0; q < 2; ++q) {
               const int jj = 8 * q + 2 * cq;          // first of the two units of this pair
               float gv[4][2], hv[2];
-              fwd_gates(acc[c], bs, h, q, jj, gv);
+              fwd_gates(ac, bs, h, q, jj, gv);
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const float cc = fmaf(gv[1][e], cstate[c][h][q][e], gv[0][e] * gv[2][e]);
@@ -343,7 +344,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
               for (int q = 0; q < 2; ++q) {
                 const int jj = 8 * q + 2 * cq;
                 float gv[4][2];
-                fwd_gates(acc[c], bs, h, q, jj, gv);
+                fwd_gates(acc[c >> 1] + 32 * (c & 1), bs, h, q, jj, gv);
                 __nv_bfloat16* gp = p.gates + (blk * 8 + (c & 1)) * 512 + (m & 31) * 16 + jj;
 #pragma unroll
                 for (int g = 0; g < 4; ++g)
@@ -1406,7 +1407,10 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
     lstm_bwd_tc_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
                        const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // Aligned by an offset from smem_raw rather than by masking a generic address, so that the compiler still knows the
+  // pointer is shared: the staging stores and slice reads below then take 32-bit shared addresses (STS / LDS), not
+  // 64-bit generic ones, which would be hoisted out of the step loop and held in registers.
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   BwdBars* bars = reinterpret_cast<BwdBars*>(smem + SB_BARS);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t rank = cluster_ctarank();
@@ -1428,7 +1432,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
   if (!(warp == BWD_W_PROD && lane == 0)) pdl_sync();
 
   if (warp >= 8) {
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<24>();
     if (warp == BWD_W_PROD && lane == 0) {
       // ===================== TMA producer: weights once, then the foreign partial slices of every step =========
       mbar_arrive_expect_tx(&bars->w_full, 131072 + (FUSED ? 4096 : 0));
@@ -1469,19 +1473,28 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
       }
     }
   } else {
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<240>();
     // ===================== consumers =====================
     // Warpgroup wg owns rows 64 wg .. 64 wg + 63.  Accumulator fragment (m64 x n256): register i holds row
     // r0 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 cq + (i & 1).  Own slice = registers 0..31: unit 16 jb + jj of this
     // CTA's 64, jj = 8 q + 2 cq + e, is register 4 (2 jb + q) + 2 h + e.
-    const int wg = warp >> 2, w = warp & 3, cq = lane & 3;
+    // Register budget: 128 accumulators, 32 dc, 24 rown and 24 operand words per thread leave about 30 of the 240
+    // registers for everything else.  So wg comes through a shuffle from lane 0, which ptxas knows to be warp-uniform:
+    // the MMAs are issued from one branch per warpgroup (uniform, so the wgmma pipeline is not serialised) with
+    // descriptors formed in uniform registers from the shared-memory base, not held per thread across the step loop.
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), w = warp & 3, cq = lane & 3;
     const int r0 = 64 * wg + 16 * w + (lane >> 2);
     const bool elected = (tid & 127) == 0;
     const uint32_t wg_bar = 2 + wg;
+    // this thread's word of row r0 in a staged A operand, 16-byte chunk 0 of the SW128 pattern: chunk k lies at
+    // st_off ^ (k << 4), since the stage is 1024-byte aligned and row r0 (and r0 + 8) swizzles by r0 & 7
+    const uint32_t st_off = r0 * 128 + ((r0 & 7) << 4) + 4 * cq;
     const long tstride = (long)p.n_tiles_cap * 8 * 4 * 2 * 32 * 16;   // cst elements per time step
     float acc[128];
-    float rown[32];                          // dLoss/dh (recurrent + head part) of the own slice for the current step
-    float dc[32];                            // carried dLoss/dc, same indexing as rown
+    // dLoss/dh (recurrent + head part) of the own slice for the current step: chunk 0's eight values are read straight
+    // from acc[0..7] (nothing overwrites them before chunk 0's MMAs), chunks 1-3 are copied out, rown[i] = acc[8 + i]
+    float rown[24];
+    float dc[32];                            // carried dLoss/dc, indexed like acc[0..31]
     uint32_t n_rf = 0, n_dpf = 0;
     mbar_wait(&bars->w_full, 0);
 
@@ -1489,12 +1502,16 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
     auto dy_mma = [&](uint32_t accumulate) {
       mbar_wait(&bars->dpb_full, (n_dpf++) & 1);
       wgmma_fence();
+      auto mma = [&](const uint8_t* a_tile) {
 #pragma unroll
-      for (int k16 = 0; k16 < 2; ++k16) {
-        const uint64_t da = make_smem_desc(smem_u32(smem + SB_DPB + wg * 4096) + k16 * 32, 0, 512, LAYOUT_SW64);
-        const uint64_t db = make_smem_desc(smem_u32(smem + SB_WOS) + k16 * 32, 0, 512, LAYOUT_SW64);
-        wgmma_m64n64k16<0, 0>(*reinterpret_cast<float(*)[32]>(acc), da, db, (accumulate || k16 > 0) ? 1u : 0u);
-      }
+        for (int k16 = 0; k16 < 2; ++k16) {
+          const uint64_t da = make_smem_desc(smem_u32(a_tile) + k16 * 32, 0, 512, LAYOUT_SW64);
+          const uint64_t db = make_smem_desc(smem_u32(smem + SB_WOS) + k16 * 32, 0, 512, LAYOUT_SW64);
+          wgmma_m64n64k16<0, 0>(*reinterpret_cast<float(*)[32]>(acc), da, db, (accumulate || k16 > 0) ? 1u : 0u);
+        }
+      };
+      if (wg == 0) mma(smem + SB_DPB);
+      else mma(smem + SB_DPB + 4096);
       wgmma_commit();
     };
 
@@ -1509,14 +1526,24 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
         fence_regs(acc);
         if (lane == 0) mbar_arrive(&bars->dpb_free);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) rown[i] = acc[i];
+        for (int i = 0; i < 24; ++i) rown[i] = acc[8 + i];
       } else {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) rown[i] = 0.f;
+        for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 24; ++i) rown[i] = 0.f;
       }
       for (int t = T - 1; t >= 0; --t) {
         const bool has_rec = t < T - 1;
         if (has_rec) mbar_wait(&bars->recv_full, (n_rf++) & 1);
+        // This thread's first element of the step's saved state and head dLoss/dh (row r0, units 2 cq, 2 cq + 1 of
+        // chunk 0).  Rows r0 and r0 + 8 lie in the same 32-row quadrant, so every (chunk, h, q, gate) operand is a
+        // constant offset from these three pointers: no per-operand address arithmetic is live across the chunk loop.
+        const long sblk = (((long)t * p.n_tiles_cap + tile) * 8 + 2 * rank) * 4 + (r0 >> 5);
+        const __nv_bfloat16* gbase = p.gates + sblk * 4096 + (r0 & 31) * 16 + 2 * cq;
+        const __nv_bfloat16* cbase = p.cst + sblk * 1024 + (r0 & 31) * 16 + 2 * cq;
+        const __nv_bfloat16* dbase =
+            p.dhout + ((((long)t * p.n_tiles_cap + tile) * 4 + rank) * 4 + (r0 >> 5)) * 2048 + (r0 & 31) * 16 + 2 * cq;
 #pragma unroll
         for (int jb = 0; jb < 4; ++jb) {
           const int st = jb & 1;
@@ -1525,24 +1552,19 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
           uint32_t gi[2][2], gf[2][2], gg[2][2], go[2][2], ct[2][2], cp[2][2], dhp[2][2];     // [h][q]
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int m = r0 + 8 * h;
-            const bool valid = (long)tile * 128 + m < p.B;
-            const long blk = (((long)t * p.n_tiles_cap + tile) * 8 + 2 * rank + (jb >> 1)) * 4 + (m >> 5);
+            const bool valid = (long)tile * 128 + r0 + 8 * h < p.B;
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
-              const int jj = 8 * q + 2 * cq;
               if (valid) {
-                const __nv_bfloat16* gp = p.gates + (blk * 8 + (jb & 1)) * 512 + (m & 31) * 16 + jj;
-                const __nv_bfloat16* cp_ = p.cst + (blk * 2 + (jb & 1)) * 512 + (m & 31) * 16 + jj;
-                gi[h][q] = ld_b32(gp);
-                gf[h][q] = ld_b32(gp + 1024);
-                gg[h][q] = ld_b32(gp + 2048);
-                go[h][q] = ld_b32(gp + 3072);
-                ct[h][q] = ld_b32(cp_);
-                cp[h][q] = t > 0 ? ld_b32(cp_ - tstride) : 0u;
-                dhp[h][q] = FUSED ? 0u
-                               : ld_b32(p.dhout + ((((((long)t * p.n_tiles_cap + tile) * 4 + rank) * 4 + (m >> 5)) * 4 + jb) * 32 +
-                                                   (m & 31)) * 16 + jj);
+                const int so = (jb >> 1) * 4 * 4096 + (jb & 1) * 512 + 128 * h + 8 * q;   // gates; cst: the same / 4
+                const int co = (jb >> 1) * 4 * 1024 + (jb & 1) * 512 + 128 * h + 8 * q;
+                gi[h][q] = ld_b32(gbase + so);
+                gf[h][q] = ld_b32(gbase + so + 1024);
+                gg[h][q] = ld_b32(gbase + so + 2048);
+                go[h][q] = ld_b32(gbase + so + 3072);
+                ct[h][q] = ld_b32(cbase + co);
+                cp[h][q] = t > 0 ? ld_b32(cbase + co - tstride) : 0u;
+                dhp[h][q] = FUSED ? 0u : ld_b32(dbase + jb * 512 + 128 * h + 8 * q);
               } else {
                 gi[h][q] = gf[h][q] = gg[h][q] = go[h][q] = ct[h][q] = cp[h][q] = dhp[h][q] = 0u;
               }
@@ -1558,8 +1580,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
               const int jj = 8 * q + 2 * cq;
-              const int ri = 4 * (2 * jb + q) + 2 * h;       // register of (unit jj, e = 0) in rown / dc
-              float rec0 = rown[ri], rec1 = rown[ri + 1];
+              const int ri = 4 * (2 * jb + q) + 2 * h;       // register of (unit jj, e = 0) in acc[0..31] / dc
+              float rec0 = jb == 0 ? acc[ri] : rown[ri - 8], rec1 = jb == 0 ? acc[ri + 1] : rown[ri - 7];
               if (has_rec) {
 #pragma unroll
                 for (int d = 0; d < 3; ++d) {
@@ -1589,18 +1611,22 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
               // A operand k-block jb: row m, 16-byte chunk 2g+q holds gate g, units 8q..8q+7 (SW128 K-major)
 #pragma unroll
               for (int g = 0; g < 4; ++g)
-                *reinterpret_cast<uint32_t*>(stage + m * 128 + (((2 * g + q) ^ (m & 7)) << 4) + 4 * cq) = z[g];
+                *reinterpret_cast<uint32_t*>(stage + 1024 * h + (st_off ^ ((2 * g + q) << 4))) = z[g];
             }
           }
           fence_proxy_async_smem();
           named_bar_sync(wg_bar, 128);
           wgmma_fence();
+          auto chunk_mma = [&](const uint8_t* a_tile) {     // one branch per warpgroup, see wg above
 #pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            const uint64_t da = make_smem_desc(smem_u32(stage + wg * 8192) + k16 * 32, 0, 1024, LAYOUT_SW128);
-            const uint64_t db = make_smem_desc(smem_u32(smem + SB_U + jb * 32768) + k16 * 32, 0, 1024, LAYOUT_SW128);
-            wgmma_m64n256k16<0, 0>(acc, da, db, (jb | k16) != 0);
-          }
+            for (int k16 = 0; k16 < 4; ++k16) {
+              const uint64_t da = make_smem_desc(smem_u32(a_tile) + k16 * 32, 0, 1024, LAYOUT_SW128);
+              const uint64_t db = make_smem_desc(smem_u32(smem + SB_U + jb * 32768) + k16 * 32, 0, 1024, LAYOUT_SW128);
+              wgmma_m64n256k16<0, 0>(acc, da, db, (jb | k16) != 0);
+            }
+          };
+          if (wg == 0) chunk_mma(stage);
+          else chunk_mma(stage + 8192);
           wgmma_commit();
           // dz_t of the chunk leaves for HBM straight from the A operand: one TMA store per warpgroup (64 rows x 128 B,
           // rows >= B clipped).  dz keeps the operand's column order [16-unit block][gate][16] (see tc_layout);
@@ -1610,28 +1636,29 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
             bulk_commit_group();
           }
         }
-        if (FUSED && t > 0) dy_mma(1);         // head part of dLoss/dh_{t-1}, read as `rown` next step
+        if (FUSED && t > 0) dy_mma(1);         // head part of dLoss/dh_{t-1}, read (acc[0..7], rown) next step
         wgmma_wait<0>();
         fence_regs(acc);
         if (FUSED && t > 0 && lane == 0) mbar_arrive(&bars->dpb_free);
         if (t > 0) {
           // ---- export the foreign slices of partial_t (needed by the peers for step t-1) ----
+          // one pointer per peer, formed here: every store is a constant offset from it
           const int par = t & 1;
+          __nv_bfloat16* ex = p.pexch + ((long)(tile * 2 + par) * 4 + rank) * 4 * 8192 + r0 * 16 + 2 * cq;
 #pragma unroll
           for (int d = 1; d < BWD_NC; ++d) {
-            const uint32_t dst = (rank + (uint32_t)d) & 3;
-            __nv_bfloat16* slice = p.pexch + (((long)(tile * 2 + par) * 4 + rank) * 4 + dst) * 128 * 64;
+            __nv_bfloat16* slice = ex + ((rank + (uint32_t)d) & 3) * 8192;
 #pragma unroll
             for (int jl = 0; jl < 8; ++jl)
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const int i = 4 * (8 * d + jl) + 2 * h;
-                *reinterpret_cast<uint32_t*>(slice + ((jl >> 1) * 128 + r0 + 8 * h) * 16 + 8 * (jl & 1) + 2 * cq) =
+                *reinterpret_cast<uint32_t*>(slice + (jl >> 1) * 2048 + 128 * h + 8 * (jl & 1)) =
                     pack_bf16x2(acc[i], acc[i + 1]);
               }
           }
 #pragma unroll
-          for (int i = 0; i < 32; ++i) rown[i] = acc[i];
+          for (int i = 0; i < 24; ++i) rown[i] = acc[8 + i];
           // both warpgroups have exported and have read the received slices of this step
           named_bar_sync(1, 256);
           if (warp == 0 && lane == 0) mbar_arrive(&bars->recv_free);
