@@ -54,7 +54,8 @@ struct TcImpl {
   // parameter offsets in the flat fp32 vector (L = 1)
   int64_t oW, oU, ob, ogamma, obeta, oWo, obo, omean, ovar;
   // workspace
-  __nv_bfloat16 *xh, *gates, *dz, *dhout, *Up, *Wp, *Ubk, *pexch;
+  bool train = false;                          // training handle: saved state and the backward recurrence exist
+  __nv_bfloat16 *xh, *gates, *dz, *dhout, *Up, *Wp, *Ubk;
   __nv_bfloat16* cst;
   float *biasp, *head_part, *head_wpart, *dpred, *wg_part;
   size_t head_part_elems, wg_part_elems;
@@ -1104,6 +1105,7 @@ void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& 
   const size_t B = (size_t)c.max_batch, T = (size_t)c.seq_len, H = TC_H;
   m.maxB = c.max_batch; m.T = c.seq_len; m.I = c.n_inputs; m.O = c.n_outputs;
   m.eps = c.bn_epsilon;
+  m.train = !c.forward_only;
   m.xh = cv.take<__nv_bfloat16>(B * (T + 1) * TC_XH_LD);
   m.Up = cv.take<__nv_bfloat16>(4 * H * H);
   m.Wp = cv.take<__nv_bfloat16>(4 * H * 32);
@@ -1117,13 +1119,12 @@ void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& 
   m.head_wctas = m.n_sms * 2;
   m.head_part_elems = (size_t)m.head_ctas * HEAD_PART;
   m.head_part = cv.take<float>(m.head_part_elems);
-  if (!c.forward_only) {
+  if (m.train) {
     const size_t Bt = (B + 127) / 128 * 128;      // saved state is blocked by 128-row tiles
     m.gates = cv.take<__nv_bfloat16>(Bt * T * 4 * H);
     m.cst = cv.take<__nv_bfloat16>(Bt * T * H);
     m.dz = cv.take<__nv_bfloat16>(B * (T + 1) * 4 * H);
     m.dhout = cv.take<__nv_bfloat16>(((B + 127) / 128 * 128) * T * H);
-    m.pexch = cv.take<__nv_bfloat16>(((B + 127) / 128) * 2 * 16 * 128 * 64);
     m.dpred = cv.take<float>(B * T * TC_OPAD);
     m.dpb = cv.take<__nv_bfloat16>(T * ((B + 127) / 128) * 128 * 32);
     m.head_wpart = cv.take<float>((size_t)m.head_wctas * HWG_PART);
@@ -1131,7 +1132,7 @@ void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& 
     m.wg_part = cv.take<float>(m.wg_part_elems);
   } else {
     m.gates = nullptr; m.cst = nullptr; m.dz = nullptr; m.dhout = nullptr; m.wg_part = nullptr;
-    m.dpred = nullptr; m.head_wpart = nullptr; m.pexch = nullptr; m.dpb = nullptr;
+    m.dpred = nullptr; m.head_wpart = nullptr; m.dpb = nullptr;
     m.wg_part_elems = 0;
   }
   // offsets of the tensors in the flat parameter vector: the API layer's layout() is the one place that defines them
@@ -1206,7 +1207,7 @@ static int tc_pack_weights(TcState& st, const float* params, cudaStream_t s) {
   a.I = m.I; a.O = m.O; a.eps = m.eps;
   a.nb_w = nblk;
   a.nb_h = (TC_H * 32 + 255) / 256;
-  a.nb_u = m.pexch ? nblk : 0;      // training handle: K-slices of U for the backward recurrence
+  a.nb_u = m.train ? nblk : 0;      // K-slices of U for the backward recurrence
   a.W = params + m.oW; a.U = params + m.oU; a.bias = params + m.ob;
   a.Wo = params + m.oWo; a.bo = params + m.obo; a.gamma = params + m.ogamma; a.beta = params + m.obeta;
   a.mean = params + m.omean; a.var = params + m.ovar;
@@ -1360,9 +1361,9 @@ int tc_backward(TcState& st, const lfmq_config& c, const float* params, float* g
 //   CTA r owns hidden units [64r, 64r+64): it computes dz_t for its 256 gate columns (pointwise, SURVEY App. A.4),
 //   stages them as the A operand in shared memory and multiplies by ITS K-slice of U (resident for the whole unroll):
 //       partial_r[128 x 256] = dz_t[:, own 256 gate cols] * U[all 256 hidden, own gate cols]^T       (wgmma)
-//   dh_{t-1}[:, slice q] = sum_r partial_r[:, slice q]: the three foreign 128x64 slices travel as bf16 through a
-//   global scratch (written by the owners, fetched with 1-D bulk copies) -- a reduce-scatter whose volume (48 KB in
-//   per CTA and step) is 5x smaller than all-gathering dz.
+//   dh_{t-1}[:, slice q] = sum_r partial_r[:, slice q]: each CTA writes the three foreign 128x64 slices, as bf16,
+//   straight into the owners' shared memory (st.async through distributed shared memory) -- a reduce-scatter whose
+//   volume (48 KB in per CTA and step) is 5x smaller than all-gathering dz.
 //   K order inside the slice: k' = 64*jb + 16*g + jj  <->  gate column g*H + 64r + 16*jb + jj, so hidden chunk jb
 //   (16 units x 4 gates) is one 64-wide k-block and its MMAs overlap the pointwise work of chunk jb+1.
 //   The N order of the resident U slice is rotated per CTA: accumulator columns 64d .. 64d+63 are hidden slice
@@ -1375,7 +1376,6 @@ struct BwdParams {
   const __nv_bfloat16* gates;
   const __nv_bfloat16* cst;
   const __nv_bfloat16* dhout;
-  __nv_bfloat16* pexch;      // [tile][parity][src][dst][16-column block][128 rows][16]
 };
 
 constexpr int BWD_NC = 4;
@@ -1386,14 +1386,16 @@ constexpr int BWD_THREADS = 384;
 constexpr int BWD_W_PROD = 8;
 constexpr uint32_t SB_U = 0;                    // 4 k-blocks x [256 x 128 B]
 constexpr uint32_t SB_A = 131072;               // 2 stages x [128 x 128 B]
-constexpr uint32_t SB_R = 163840;               // 3 foreign slices x [16-column block][128 rows][16] bf16
+constexpr uint32_t SB_R = 163840;               // received partial slices [slot d-1][chunk jb][consumer thread][16 B]
 constexpr uint32_t SB_DPB = 212992;             // FUSED: dLoss/dpred tile of one step [128 x 64 B], SW64
 constexpr uint32_t SB_WOS = 221184;             // FUSED: (Wo gamma inv) rows of this CTA's 64 hidden units [64 x 64 B], SW64
 constexpr uint32_t SB_BARS = 225280;
 constexpr uint32_t BWD_SMEM = SB_BARS + 256 + 1024;
 
 struct BwdBars {
-  uint64_t w_full, recv_full, recv_free, exp_ready;
+  uint64_t w_full;
+  uint64_t recv_full[2];         // per consumer warpgroup: the peers' partial slices for its 64 rows have landed
+  uint64_t slot_free[2];         // per consumer warpgroup: the peers have read the slices this CTA last sent them
   uint64_t dpb_full, dpb_free;   // FUSED: the dpred tile has landed / the MMAs reading it have completed
 };
 
@@ -1419,9 +1421,10 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
 
   if (tid == 0) {
     mbar_init(&bars->w_full, 1);
-    mbar_init(&bars->recv_full, 1);
-    mbar_init(&bars->recv_free, 1);
-    mbar_init(&bars->exp_ready, BWD_NC - 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&bars->recv_full[i], 1);
+      mbar_init(&bars->slot_free[i], BWD_NC - 1);   // one arrive per peer
+    }
     mbar_init(&bars->dpb_full, 1);
     mbar_init(&bars->dpb_free, 8);          // one arrive per consumer warp
     fence_mbar_init();
@@ -1434,7 +1437,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
   if (warp >= 8) {
     setmaxnreg_dec<24>();
     if (warp == BWD_W_PROD && lane == 0) {
-      // ===================== TMA producer: weights once, then the foreign partial slices of every step =========
+      // ===================== TMA producer: weights once, then (FUSED) the dpred tile of every step =========
       mbar_arrive_expect_tx(&bars->w_full, 131072 + (FUSED ? 4096 : 0));
       for (int jb = 0; jb < 4; ++jb)
         for (int d = 0; d < 4; ++d)
@@ -1442,32 +1445,17 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
                       (int)rank * 256 + (int)((rank + d) & 3) * 64);
       if (FUSED) tma_load_2d(smem + SB_WOS, &tm_wos, &bars->w_full, 0, rank * 64);
       pdl_sync();
-      uint32_t n_er = 0, n_dp = 0;
-      // dpred tile of time step td into the single staging buffer, once the MMAs that read the previous one are done
-      auto load_dpred = [&](int tile, int td) {
-        if (n_dp > 0) mbar_wait(&bars->dpb_free, (n_dp - 1) & 1);
-        ++n_dp;
-        mbar_arrive_expect_tx(&bars->dpb_full, 8192);
-        tma_load_2d(smem + SB_DPB, &tm_dpb, &bars->dpb_full, 0, (td * p.n_tiles_cap + tile) * 128);
-      };
-      for (int it = 0; it < p.n_iters; ++it) {
-        const int tile = it * p.n_clusters + cid;
-        if (tile >= p.n_tiles) break;                     // clusters without a tile in the last round
-        if (FUSED) load_dpred(tile, T - 1);
-        for (int t = T - 1; t >= 0; --t) {
-          if (FUSED && t > 0) load_dpred(tile, t - 1);      // for the MMA at the end of this step
-          if (t <= T - 2) {                                 // step t consumes the partials exported after step t+1
-            mbar_wait_cluster(&bars->exp_ready, n_er & 1);
-            mbar_wait(&bars->recv_free, (n_er++) & 1);      // own consumers are done reading the previous slices
-            fence_proxy_async_global();
-            mbar_arrive_expect_tx(&bars->recv_full, 3 * 16384);
-            const int par = (t + 1) & 1;
-            for (uint32_t d = 1; d < BWD_NC; ++d) {
-              const uint32_t src = (rank + d) & 3;
-              bulk_load_1d(smem + SB_R + (d - 1) * 16384,
-                           p.pexch + ((((long)(tile * 2 + par) * 4 + (int)src) * 4 + (int)rank)) * 128 * 64, 16384,
-                           &bars->recv_full);
-            }
+      if (FUSED) {
+        uint32_t n_dp = 0;
+        for (int it = 0; it < p.n_iters; ++it) {
+          const int tile = it * p.n_clusters + cid;
+          if (tile >= p.n_tiles) break;                   // clusters without a tile in the last round
+          // dpred tile of time step td into the single staging buffer, once the MMAs that read the previous one are done
+          for (int td = T - 1; td >= 0; --td) {
+            if (n_dp > 0) mbar_wait(&bars->dpb_free, (n_dp - 1) & 1);
+            ++n_dp;
+            mbar_arrive_expect_tx(&bars->dpb_full, 8192);
+            tma_load_2d(smem + SB_DPB, &tm_dpb, &bars->dpb_full, 0, (td * p.n_tiles_cap + tile) * 128);
           }
         }
       }
@@ -1489,13 +1477,22 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
     // this thread's word of row r0 in a staged A operand, 16-byte chunk 0 of the SW128 pattern: chunk k lies at
     // st_off ^ (k << 4), since the stage is 1024-byte aligned and row r0 (and r0 + 8) swizzles by r0 & 7
     const uint32_t st_off = r0 * 128 + ((r0 & 7) << 4) + 4 * cq;
+    // Received partials, in fragment order: thread i of the sending CTA holds in acc[32 d .. 32 d + 31] (d = (dst - src)
+    // mod 4) exactly the rows and columns that thread i here adds to acc[0..31].  Slot d - 1 holds the slice of peer
+    // (rank + d) mod 4 as [chunk jb][consumer thread][4 words]: vector jb of a thread is the four packed bf16x2 words
+    // of chunk jb, word 2 h + q (registers 8 jb + 2 h + 4 q).  The sender writes it with one 16-byte st.async, a warp
+    // covering 512 contiguous bytes; it is read back as two 8-byte halves, one per row half h (three live 16-byte
+    // vectors would spill).
+    const uint32_t recv_off = SB_R + tid * 16;
     const long tstride = (long)p.n_tiles_cap * 8 * 4 * 2 * 32 * 16;   // cst elements per time step
     float acc[128];
     // dLoss/dh (recurrent + head part) of the own slice for the current step: chunk 0's eight values are read straight
     // from acc[0..7] (nothing overwrites them before chunk 0's MMAs), chunks 1-3 are copied out, rown[i] = acc[8 + i]
     float rown[24];
     float dc[32];                            // carried dLoss/dc, indexed like acc[0..31]
-    uint32_t n_rf = 0, n_dpf = 0;
+    // exchanges sent so far: step t sends the partials that the peers' step t - 1 receives, so the receive waited for at
+    // step t is the (n_ex - 1)-th phase of recv_full, and the send waits for the n_ex-th phase of slot_free
+    uint32_t n_ex = 0, n_dpf = 0;
     mbar_wait(&bars->w_full, 0);
 
     // head part of dLoss/dh (dpred (Wo gamma inv)^T) into the own-slice registers: accumulate = 0 at a tile's first step
@@ -1535,7 +1532,6 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
       }
       for (int t = T - 1; t >= 0; --t) {
         const bool has_rec = t < T - 1;
-        if (has_rec) mbar_wait(&bars->recv_full, (n_rf++) & 1);
         // This thread's first element of the step's saved state and head dLoss/dh (row r0, units 2 cq, 2 cq + 1 of
         // chunk 0).  Rows r0 and r0 + 8 lie in the same 32-row quadrant, so every (chunk, h, q, gate) operand is a
         // constant offset from these three pointers: no per-operand address arithmetic is live across the chunk loop.
@@ -1544,12 +1540,11 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
         const __nv_bfloat16* cbase = p.cst + sblk * 1024 + (r0 & 31) * 16 + 2 * cq;
         const __nv_bfloat16* dbase =
             p.dhout + ((((long)t * p.n_tiles_cap + tile) * 4 + rank) * 4 + (r0 >> 5)) * 2048 + (r0 & 31) * 16 + 2 * cq;
-#pragma unroll
-        for (int jb = 0; jb < 4; ++jb) {
-          const int st = jb & 1;
-          uint8_t* stage = smem + SB_A + st * 16384;
-          // all operands of the chunk requested before the first is used: one memory latency per chunk
-          uint32_t gi[2][2], gf[2][2], gg[2][2], go[2][2], ct[2][2], cp[2][2], dhp[2][2];     // [h][q]
+        // Saved-state operands of one chunk, all requested before the first is used: one memory latency per chunk.
+        // They do not depend on the exchange, so chunk 0's go out before the wait for the peers' partials, and chunk
+        // jb + 1's right after chunk jb's staging stores, into the registers chunk jb no longer needs.
+        uint32_t gi[2][2], gf[2][2], gg[2][2], go[2][2], ct[2][2], cp[2][2], dhp[2][2];     // [h][q]
+        auto load_chunk = [&](int jb) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const bool valid = (long)tile * 128 + r0 + 8 * h < p.B;
@@ -1570,26 +1565,37 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
               }
             }
           }
+        };
+        load_chunk(0);
+        if (has_rec) mbar_wait_cluster(&bars->recv_full[wg], (n_ex + 1) & 1);
+#pragma unroll
+        for (int jb = 0; jb < 4; ++jb) {
+          const int st = jb & 1;
+          uint8_t* stage = smem + SB_A + st * 16384;
           // the stage is free: the MMAs of its previous use (two chunks ago) and the dz store that read it are done
           wgmma_wait<1>();
           if (elected) bulk_wait_group_read1();
           named_bar_sync(wg_bar, 128);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int m = r0 + 8 * h;
+            // dLoss/dh of the own slice: own part, plus the peers' slices d = 1, 2, 3 in that order, summed in place
+            // (acc[0..7] are rewritten by chunk 0's MMAs, rown[] by the next step)
+            auto own = [&](int ri) -> float& { return jb == 0 ? acc[ri] : rown[ri - 8]; };
+            if (has_rec) {
+#pragma unroll
+              for (int d = 0; d < 3; ++d) {
+                const uint2 v = *reinterpret_cast<const uint2*>(smem + recv_off + d * 16384 + jb * 4096 + 8 * h);
+                const int ri = 8 * jb + 2 * h;
+                own(ri) += bf16_lo(v.x);
+                own(ri + 1) += bf16_hi(v.x);
+                own(ri + 4) += bf16_lo(v.y);
+                own(ri + 5) += bf16_hi(v.y);
+              }
+            }
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
-              const int jj = 8 * q + 2 * cq;
               const int ri = 4 * (2 * jb + q) + 2 * h;       // register of (unit jj, e = 0) in acc[0..31] / dc
-              float rec0 = jb == 0 ? acc[ri] : rown[ri - 8], rec1 = jb == 0 ? acc[ri + 1] : rown[ri - 7];
-              if (has_rec) {
-#pragma unroll
-                for (int d = 0; d < 3; ++d) {
-                  const uint32_t v = *reinterpret_cast<const uint32_t*>(smem + SB_R + d * 16384 + ((jb * 128 + m) * 16 + jj) * 2);
-                  rec0 += bf16_lo(v);
-                  rec1 += bf16_hi(v);
-                }
-              }
+              const float rec0 = own(ri), rec1 = own(ri + 1);
               // gate-gradient algebra in packed bf16x2 (two units per word); only the carried dLoss/dc stays in fp32
               // registers.  SURVEY App. A.4.
               const uint32_t i2 = gi[h][q], f2 = gf[h][q], g2 = gg[h][q], o2 = go[h][q];
@@ -1614,6 +1620,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
                 *reinterpret_cast<uint32_t*>(stage + 1024 * h + (st_off ^ ((2 * g + q) << 4))) = z[g];
             }
           }
+          if (jb < 3) load_chunk(jb + 1);
           fence_proxy_async_smem();
           named_bar_sync(wg_bar, 128);
           wgmma_fence();
@@ -1636,41 +1643,46 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
             bulk_commit_group();
           }
         }
+        // The warpgroup has read its received slices of this step (chunk 3's second barrier follows the last reads):
+        // arm recv_full for step t - 1, then tell the peers their slots are free.  The arm precedes the arrive that
+        // lets any peer send, so no tx completes on a phase before it is armed.
+        if (elected && t > 0) {
+          mbar_arrive_expect_tx(&bars->recv_full[wg], (BWD_NC - 1) * 8192);
+#pragma unroll
+          for (uint32_t d = 1; d < BWD_NC; ++d) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->slot_free[wg]), (rank + d) & 3));
+        }
         if (FUSED && t > 0) dy_mma(1);         // head part of dLoss/dh_{t-1}, read (acc[0..7], rown) next step
         wgmma_wait<0>();
         fence_regs(acc);
         if (FUSED && t > 0 && lane == 0) mbar_arrive(&bars->dpb_free);
         if (t > 0) {
-          // ---- export the foreign slices of partial_t (needed by the peers for step t-1) ----
-          // one pointer per peer, formed here: every store is a constant offset from it
-          const int par = t & 1;
-          __nv_bfloat16* ex = p.pexch + ((long)(tile * 2 + par) * 4 + rank) * 4 * 8192 + r0 * 16 + 2 * cq;
+          // ---- export the foreign slices of partial_t (needed by the peers for step t-1) into their shared memory ----
+          // Peer (rank + d) mod 4 files this CTA's slice in its slot 3 - d.  Its warpgroup wg has read what this CTA
+          // sent last step once slot_free[wg] completes; the stores complete tx on its recv_full[wg].
+          mbar_wait_cluster(&bars->slot_free[wg], (n_ex++) & 1);
 #pragma unroll
           for (int d = 1; d < BWD_NC; ++d) {
-            __nv_bfloat16* slice = ex + ((rank + (uint32_t)d) & 3) * 8192;
+            const uint32_t peer = (rank + (uint32_t)d) & 3;
+            const uint32_t dst = mapa_u32(smem_u32(smem + recv_off + (3 - d) * 16384), peer);
+            const uint32_t bar = mapa_u32(smem_u32(&bars->recv_full[wg]), peer);
 #pragma unroll
-            for (int jl = 0; jl < 8; ++jl)
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const int i = 4 * (8 * d + jl) + 2 * h;
-                *reinterpret_cast<uint32_t*>(slice + (jl >> 1) * 2048 + 128 * h + 8 * (jl & 1)) =
-                    pack_bf16x2(acc[i], acc[i + 1]);
-              }
+            for (int jb = 0; jb < 4; ++jb) {
+              const int i = 32 * d + 8 * jb;
+              st_async_v4(dst + jb * 4096,
+                          make_uint4(pack_bf16x2(acc[i], acc[i + 1]), pack_bf16x2(acc[i + 4], acc[i + 5]),
+                                     pack_bf16x2(acc[i + 2], acc[i + 3]), pack_bf16x2(acc[i + 6], acc[i + 7])),
+                          bar);
+            }
           }
 #pragma unroll
           for (int i = 0; i < 24; ++i) rown[i] = acc[8 + i];
-          // both warpgroups have exported and have read the received slices of this step
-          named_bar_sync(1, 256);
-          if (warp == 0 && lane == 0) mbar_arrive(&bars->recv_free);
-          if (warp == 0 && lane >= 1 && lane < BWD_NC)
-            mbar_arrive_cluster(mapa_u32(smem_u32(&bars->exp_ready), (rank + (uint32_t)lane) & 3));
         }
       }
     }
     if (elected) bulk_wait_group0();            // all dz stores complete before the kernel ends
   }
   __syncwarp();
-  cluster_sync_all();
+  cluster_sync_all();          // nobody leaves while peers may still store into / arrive on this CTA
 }
 
 // =============================================================================================
@@ -1736,7 +1748,7 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
     bp.n_clusters = n_tiles < m.bwd_max_clusters ? n_tiles : m.bwd_max_clusters;
     bp.n_iters = (n_tiles + bp.n_clusters - 1) / bp.n_clusters;
     bp.n_tiles = n_tiles;
-    bp.gates = m.gates; bp.cst = m.cst; bp.dhout = m.dhout; bp.pexch = m.pexch;
+    bp.gates = m.gates; bp.cst = m.cst; bp.dhout = m.dhout;
     // dz as [b][t][1024] with columns ordered [16-unit block][gate][16]: one warpgroup's part of a staged chunk =
     // 64 rows x 64 columns
     CUtensorMap tm_dzst;

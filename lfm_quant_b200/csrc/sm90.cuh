@@ -112,11 +112,11 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* s
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
-// 1-D bulk copy global -> shared::cta (size a multiple of 16 B), completing tx-bytes on a local mbarrier
-__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
+// 16-byte store into a cluster peer's shared memory, completing 16 tx-bytes on the peer's mbarrier (both mapa
+// addresses).  The complete_tx has release semantics at cluster scope: the reader waits with mbar_wait_cluster.
+__device__ __forceinline__ void st_async_v4(uint32_t dst, uint4 v, uint32_t bar) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
+               ::"r"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(bar)
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
