@@ -14,18 +14,23 @@
 //                                 chunk goes out with one TMA store; only the weight-gradient GEMM reads it
 //   dpb   bf16 [T][tiles][128][32]  dLoss/dpred tiles (cols >= 16 zero): written by the tensor-core head as it stages
 //                                 them, expanded to dLoss/dh by the backward kernel's own MMAs (no dropout)
-//   dhout bf16 [T][tiles][4 ranks][4 row quadrants][4 chunks][32 rows][16]   dropout > 0 only: dLoss/dh from the SIMT
-//                                 head (after BN/dropout backward)
+//   dhout bf16 [T][tiles][4 ranks][4 row quadrants][4 chunks][32 rows][16]   training with dropout > 0 only: dLoss/dh
+//                                 from the SIMT head (after BN/dropout backward); with it the fp32 dpred [B*T][16]
 //
-// Forward recurrence = ONE persistent kernel (lstm_fwd_tc_kernel): clusters of 4 CTAs, one 128-row batch tile per
-// cluster, all clusters co-resident (a last round that fits as 64-row half tiles is a second launch, see tc_rounds).  CTA r keeps the weight slice of hidden units [64r, 64r+64) (all four gates,
-// 256 gate columns) resident in shared memory for the whole unroll.  h_t is exchanged through global memory (it is
-// an output anyway) and comes back as the next step's A operand via TMA multicast.  See DESIGN.md section 5.
+// Forward recurrence = ONE persistent kernel (lstm_fwd_tc_kernel<SAVE, 128>): clusters of 4 CTAs, one 128-row batch
+// tile per cluster, all clusters co-resident (a last round that fits as 64-row half tiles is a second launch, of
+// lstm_fwd_tc_kernel<SAVE, 64>, see tc_rounds).  CTA r keeps the weight slice of hidden units [64r, 64r+64) (all four
+// gates, 256 gate columns) resident in shared memory for the whole unroll.  h_t is exchanged through global memory (it
+// is an output anyway) and comes back as the next step's A operand via TMA multicast.  The backward recurrence
+// (lstm_bwd_tc_kernel<FUSED, ROWS>) runs the same rounds.  tc_init sets both up when a handle is created,
+// tc_run_rounds launches them.  See DESIGN.md section 5.
 #include "lstm_tc.h"
 
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "kernels.h"
 #include "sm90.cuh"
@@ -55,23 +60,24 @@ struct TcImpl {
   int64_t oW, oU, ob, ogamma, obeta, oWo, obo, omean, ovar;
   // workspace
   bool train = false;                          // training handle: saved state and the backward recurrence exist
+  // c.train && dropout > 0: the head runs as the SIMT dropout head (head_rows_kernel, head_wgrad_kernel), which hands
+  // dLoss/dh to the backward through dhout; otherwise as head_tc_kernel, fused with lstm_bwd_tc_kernel<true, ROWS>
+  bool dropout_head = false;
   __nv_bfloat16 *xh, *gates, *dz, *dhout, *Up, *Wp, *Ubk;
   __nv_bfloat16* cst;
   float *biasp, *head_part, *head_wpart, *dpred, *wg_part;
   size_t head_part_elems, wg_part_elems;
-  CUtensorMap tm_h, tm_x, tm_u, tm_w;          // forward
-  CUtensorMap tm_h16, tm_x64;                  // forward over half tiles: the boxes of tm_h, tm_x with half the rows
+  // Maps whose boxes carry batch rows come in pairs: [0] for 128-row tiles, [1] for 64-row half tiles (tc_run_rounds)
+  CUtensorMap tm_h[2], tm_x[2], tm_u, tm_w;    // forward
   CUtensorMap tm_h128, tm_wot;                 // head: 128-row h tiles, folded head weights
   __nv_bfloat16* WoTp;
   __nv_bfloat16* WoSp;                         // [256][32]  Wo[j][k] * gamma_j * inv_j (k < 16), zero padded
   __nv_bfloat16* dpb;                          // [T][tiles][128][32] bf16 dLoss/dpred tiles (cols >= 16 zero)
-  CUtensorMap tm_wos, tm_dpb, tm_dpb64;        // tm_dpb64: 64-row boxes, for the backward over half tiles
+  CUtensorMap tm_wos, tm_dpb[2];               // tm_dpb[0]: also the head's dpred tile stores
   float* bop;
   CUtensorMap tm_ubk;                          // backward recurrence
-  CUtensorMap tm_xh_mn, tm_dz_mn;              // weight gradient (MN-major)
   int max_clusters = 0, bwd_max_clusters = 0;
   bool half_tiles = true;                      // a last round that fits as 64-row half tiles runs as such (tc_rounds)
-  bool bwd_ready = false;
   int head_ctas = 0, head_wctas = 0;
   int n_sms = 0;
 };
@@ -182,11 +188,11 @@ __device__ __forceinline__ void fwd_gates(const float* a, const float* bs, int h
 // ROWS: rows per cluster and round, 128 (a tile) or 64 (half a tile: row quadrants {0,1} or {2,3} of tile u / 2, for a
 // last round that would otherwise leave most clusters idle).  At 64 rows both consumer warpgroups take the same rows
 // and split the gate columns: warpgroup wg issues and updates only its 128-column half (chunks 2 wg, 2 wg + 1).  The
-// maps tm_h and tm_x come with boxes of ROWS / 4 and ROWS rows.  The body of lstm_fwd_tc_kernel (128 rows) and
-// lstm_fwd_tc_half_kernel (64 rows); the maps are those kernels' __grid_constant__ parameters.
+// maps tm_h and tm_x come with boxes of ROWS / 4 and ROWS rows.
 template <bool SAVE, int ROWS>
-__device__ __forceinline__ void lstm_fwd_tc(const FwdParams& p, const CUtensorMap& tm_h, const CUtensorMap& tm_x,
-                                            const CUtensorMap& tm_u, const CUtensorMap& tm_w) {
+__global__ void __launch_bounds__(FWD_THREADS, 1)
+    lstm_fwd_tc_kernel(FwdParams p, const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_x,
+                       const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   FwdBars* bars = reinterpret_cast<FwdBars*>(smem + SM_BARS);
@@ -378,27 +384,13 @@ __device__ __forceinline__ void lstm_fwd_tc(const FwdParams& p, const CUtensorMa
   cluster_sync_all();          // nobody leaves while peers may still multicast into / arrive on this CTA
 }
 
-template <bool SAVE>
-__global__ void __launch_bounds__(FWD_THREADS, 1)
-    lstm_fwd_tc_kernel(FwdParams p, const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_x,
-                       const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w) {
-  lstm_fwd_tc<SAVE, 128>(p, tm_h, tm_x, tm_u, tm_w);
-}
-
-template <bool SAVE>
-__global__ void __launch_bounds__(FWD_THREADS, 1)
-    lstm_fwd_tc_half_kernel(FwdParams p, const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_x,
-                            const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w) {
-  lstm_fwd_tc<SAVE, 64>(p, tm_h, tm_x, tm_u, tm_w);
-}
-
 // =============================================================================================
 // Fused head: BN(inference affine) -> Dropout -> Dense -> weighted-MSE loss -> (training) all head gradients
 // and dLoss/dh.  One warp per [b,t] row, H = 256 (8 hidden units per lane), n_outputs <= 16.
 // (models/point_estimate/rnn_point_estimate.py:88-89,105; model_utils/losses.py:55-135; SURVEY App. A.2-A.4)
 // =============================================================================================
 struct HeadParams {
-  int B, T, O, target_idx, train;
+  int B, T, O, target_idx;
   const __nv_bfloat16* xh;
   const float *gamma, *beta, *mean, *var;
   float eps;
@@ -1107,325 +1099,6 @@ __global__ void head_fold_kernel(int O, float* __restrict__ gWo, const float* __
 }
 
 // =============================================================================================
-// Host side
-// =============================================================================================
-static bool tc_supported(const lfmq_config& c, char* why, size_t n) {
-  if (c.rnn_cell != LFMQ_CELL_LSTM) { snprintf(why, n, "the bf16 tensor-core path is built for the LSTM cell only"); return false; }
-  if (c.uq) { snprintf(why, n, "the bf16 tensor-core path is built for the point-estimate head only"); return false; }
-  if (c.num_hidden != TC_H) { snprintf(why, n, "num_hidden must be 256 (got %d)", c.num_hidden); return false; }
-  if (c.num_layers != 1) { snprintf(why, n, "num_layers must be 1 (got %d)", c.num_layers); return false; }
-  if (c.n_inputs > 32) { snprintf(why, n, "n_inputs must be <= 32 (got %d)", c.n_inputs); return false; }
-  if (c.n_outputs > TC_OPAD) { snprintf(why, n, "n_outputs must be <= 16 (got %d)", c.n_outputs); return false; }
-  if (c.recurrent_dropout > 0.f) { snprintf(why, n, "recurrent_dropout is not built on the bf16 path"); return false; }
-  return true;
-}
-
-bool tc_shape_supported(const lfmq_config& c) {
-  char why[128];
-  return tc_supported(c, why, sizeof(why));
-}
-
-void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& cv) {
-  if (c.precision != LFMQ_PREC_BF16) return;
-  char why[128];
-  if (!tc_supported(c, why, sizeof(why))) return;   // tc_init reports the error
-  if (!st.impl) st.impl = new TcImpl;
-  TcImpl& m = *st.impl;
-  const size_t B = (size_t)c.max_batch, T = (size_t)c.seq_len, H = TC_H;
-  m.maxB = c.max_batch; m.T = c.seq_len; m.I = c.n_inputs; m.O = c.n_outputs;
-  m.eps = c.bn_epsilon;
-  m.train = !c.forward_only;
-  m.xh = cv.take<__nv_bfloat16>(B * (T + 1) * TC_XH_LD);
-  m.Up = cv.take<__nv_bfloat16>(4 * H * H);
-  m.Wp = cv.take<__nv_bfloat16>(4 * H * 32);
-  m.Ubk = cv.take<__nv_bfloat16>(4 * H * H);
-  m.biasp = cv.take<float>(4 * H);
-  m.WoTp = cv.take<__nv_bfloat16>(TC_OPAD * H);
-  m.WoSp = cv.take<__nv_bfloat16>(H * 32);
-  m.bop = cv.take<float>(TC_OPAD);
-  m.n_sms = device_sm_count();
-  m.head_ctas = m.n_sms * 2;
-  m.head_wctas = m.n_sms * 2;
-  m.head_part_elems = (size_t)m.head_ctas * HEAD_PART;
-  m.head_part = cv.take<float>(m.head_part_elems);
-  if (m.train) {
-    const size_t Bt = (B + 127) / 128 * 128;      // saved state is blocked by 128-row tiles
-    m.gates = cv.take<__nv_bfloat16>(Bt * T * 4 * H);
-    m.cst = cv.take<__nv_bfloat16>(Bt * T * H);
-    m.dz = cv.take<__nv_bfloat16>(B * (T + 1) * 4 * H);
-    m.dhout = cv.take<__nv_bfloat16>(((B + 127) / 128 * 128) * T * H);
-    m.dpred = cv.take<float>(B * T * TC_OPAD);
-    m.dpb = cv.take<__nv_bfloat16>(T * ((B + 127) / 128) * 128 * 32);
-    m.head_wpart = cv.take<float>((size_t)m.head_wctas * HWG_PART);
-    m.wg_part_elems = (size_t)64 * 384 * 1024;
-    m.wg_part = cv.take<float>(m.wg_part_elems);
-  } else {
-    m.gates = nullptr; m.cst = nullptr; m.dz = nullptr; m.dhout = nullptr; m.wg_part = nullptr;
-    m.dpred = nullptr; m.head_wpart = nullptr; m.dpb = nullptr;
-    m.wg_part_elems = 0;
-  }
-  // offsets of the tensors in the flat parameter vector: the API layer's layout() is the one place that defines them
-  m.oW = po.oW; m.oU = po.oU; m.ob = po.ob; m.ogamma = po.ogamma; m.obeta = po.obeta;
-  m.oWo = po.oWo; m.obo = po.obo; m.omean = po.omean; m.ovar = po.ovar;
-}
-
-int tc_init(TcState& st, const lfmq_config& c) {
-  if (c.precision != LFMQ_PREC_BF16) return 0;
-  char why[128];
-  if (!tc_supported(c, why, sizeof(why))) {
-    LFMQ_SET_ERR("LFMQ_PREC_BF16 supports the H=256 single-layer forecaster only: %s; use LFMQ_PREC_FP32", why);
-    return LFMQ_ERR_UNSUPPORTED;
-  }
-  TcImpl& m = *st.impl;
-  const size_t B = (size_t)m.maxB, T = (size_t)m.T;
-  LFMQ_CUDA_CHECK(cudaMemset(m.xh, 0, B * (T + 1) * TC_XH_LD * 2));
-  if (m.dz) LFMQ_CUDA_CHECK(cudaMemset(m.dz, 0, B * (T + 1) * 4 * TC_H * 2));
-  const uint64_t xh_row = (uint64_t)(T + 1) * TC_XH_LD;     // elements per batch row of the 2-D view
-  int rc;
-  if ((rc = encode_map_2d(&m.tm_h, m.xh, xh_row, B, xh_row * 2, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = encode_map_2d(&m.tm_x, m.xh, xh_row, B, xh_row * 2, 32, 128, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
-  if ((rc = encode_map_2d(&m.tm_h16, m.xh, xh_row, B, xh_row * 2, 64, 16, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = encode_map_2d(&m.tm_x64, m.xh, xh_row, B, xh_row * 2, 32, 64, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
-  if ((rc = encode_map_2d(&m.tm_h128, m.xh, xh_row, B, xh_row * 2, 64, 128, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = encode_map_2d(&m.tm_wot, m.WoTp, TC_H, TC_OPAD, TC_H * 2, 64, 16, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = encode_map_2d(&m.tm_wos, m.WoSp, 32, TC_H, 64, 32, 64, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
-  if (m.dpb &&
-      (rc = encode_map_2d(&m.tm_dpb, m.dpb, 32, (uint64_t)m.T * ((m.maxB + 127) / 128) * 128, 64, 32, 128,
-                        CU_TENSOR_MAP_SWIZZLE_64B)))
-    return rc;
-  if (m.dpb &&
-      (rc = encode_map_2d(&m.tm_dpb64, m.dpb, 32, (uint64_t)m.T * ((m.maxB + 127) / 128) * 128, 64, 32, 64,
-                        CU_TENSOR_MAP_SWIZZLE_64B)))
-    return rc;
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HT_SMEM));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, HT_SMEM));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HROWS_SMEM));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, HROWS_SMEM));
-  if ((rc = encode_map_2d(&m.tm_u, m.Up, TC_H, 4 * TC_H, TC_H * 2, 64, 256, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  if ((rc = encode_map_2d(&m.tm_w, m.Wp, 32, 4 * TC_H, 64, 32, 256, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_half_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_fwd_tc_half_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM));
-  // LFMQ_TC_HALF_TILES=0 keeps every round at 128-row tiles (A/B measurements, tests comparing the two schedules)
-  const char* ht = getenv("LFMQ_TC_HALF_TILES");
-  m.half_tiles = !(ht != nullptr && atoi(ht) == 0);
-  // how many 4-CTA clusters can be co-resident (one CTA per SM because of shared memory)
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(TC_NC * (m.n_sms / TC_NC));
-  cfg.blockDim = dim3(FWD_THREADS);
-  cfg.dynamicSmemBytes = FWD_SMEM;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = TC_NC;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  int nclusters = 0;
-  LFMQ_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&nclusters, lstm_fwd_tc_kernel<true>, &cfg));
-  if (nclusters < 1) {
-    LFMQ_SET_ERR("no 4-CTA cluster of the forward kernel fits on this device");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
-  m.max_clusters = nclusters;
-  m.enabled = true;
-  st.weights_dirty = 1;
-  return 0;
-}
-
-void tc_destroy(TcState& st) {
-  delete st.impl;
-  st.impl = nullptr;
-}
-
-static int tc_pack_weights(TcState& st, const float* params, cudaStream_t s) {
-  TcImpl& m = *st.impl;
-  if (!st.weights_dirty) return 0;
-  const int nblk = (int)(((long)4 * TC_H * TC_H + 255) / 256);
-  PackArgs a;
-  a.I = m.I; a.O = m.O; a.eps = m.eps;
-  a.nb_w = nblk;
-  a.nb_h = (TC_H * 32 + 255) / 256;
-  a.nb_u = m.train ? nblk : 0;      // K-slices of U for the backward recurrence
-  a.W = params + m.oW; a.U = params + m.oU; a.bias = params + m.ob;
-  a.Wo = params + m.oWo; a.bo = params + m.obo; a.gamma = params + m.ogamma; a.beta = params + m.obeta;
-  a.mean = params + m.omean; a.var = params + m.ovar;
-  a.Up = m.Up; a.Wp = m.Wp; a.Ubk = m.Ubk; a.WoTp = m.WoTp; a.WoSp = m.WoSp; a.biasp = m.biasp; a.bop = m.bop;
-  if (int rc = launch_pdl(pack_all_kernel, dim3(a.nb_w + a.nb_h + a.nb_u), dim3(256), 0, s, 1, true, a)) return rc;
-  st.weights_dirty = 0;
-  return 0;
-}
-
-// The rounds of a persistent recurrence over B rows with at most max_clusters co-resident clusters: n_full 128-row tiles
-// (units 0 .. n_full - 1 of 128 rows), then n_half 64-row half tiles (units 2 n_full .. of 64 rows) in one more round.
-// Rounds are independent (each unit starts from zero state), so the two kinds are two launches in stream order.  The
-// last round runs as half tiles whenever they fit on the co-resident clusters: a round of a few whole tiles leaves
-// most clusters idle for all T steps while the busy ones carry 128 rows through every step's dependency chain.
-struct TcRounds {
-  int n_full, n_half;
-};
-
-static TcRounds tc_rounds(int B, int max_clusters, bool half_tiles) {
-  const int n_tiles = (B + 127) / 128;
-  const int n_cl = n_tiles < max_clusters ? n_tiles : max_clusters;
-  const int full_rounds = (n_tiles + n_cl - 1) / n_cl - 1;
-  const int rows_last = B - full_rounds * n_cl * 128;
-  if (half_tiles && (rows_last + 63) / 64 <= max_clusters) return {full_rounds * n_cl, (rows_last + 63) / 64};
-  return {n_tiles, 0};
-}
-
-// n_units units of ROWS rows from unit0 on, in rounds of at most max_clusters clusters
-template <class Params>
-static void tc_set_rounds(Params& p, int unit0, int n_units, int max_clusters) {
-  p.unit0 = unit0;
-  p.n_units = n_units;
-  p.n_clusters = n_units < max_clusters ? n_units : max_clusters;
-  p.n_iters = (n_units + p.n_clusters - 1) / p.n_clusters;
-}
-
-template <int ROWS>
-static int tc_launch_fwd(const TcImpl& m, FwdParams p, bool save, int unit0, int n_units, cudaStream_t s) {
-  tc_set_rounds(p, unit0, n_units, m.max_clusters);
-  auto* kernel = ROWS == 128 ? (save ? lstm_fwd_tc_kernel<true> : lstm_fwd_tc_kernel<false>)
-                             : (save ? lstm_fwd_tc_half_kernel<true> : lstm_fwd_tc_half_kernel<false>);
-  return launch_pdl(kernel, dim3(TC_NC * p.n_clusters),
-                    dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, true, p, ROWS == 128 ? m.tm_h : m.tm_h16,
-                    ROWS == 128 ? m.tm_x : m.tm_x64, m.tm_u, m.tm_w);
-}
-
-static int tc_run_recurrence(TcState& st, const float* x, int B, bool save, cudaStream_t s) {
-  TcImpl& m = *st.impl;
-  const long bt = (long)B * m.T * 5;
-  if (int rc = launch_pdl(xh_fill_x_kernel, dim3((int)((bt + 255) / 256)), dim3(256), 0, s, 1, true, B, m.T, m.I, x, m.xh)) return rc;
-  FwdParams p;
-  p.B = B; p.T = m.T;
-  p.k16_x = (m.I + 15) / 16;
-  p.n_tiles_cap = (m.maxB + 127) / 128;
-  p.xh = m.xh;
-  p.gates = save ? m.gates : nullptr;
-  p.cst = save ? m.cst : nullptr;
-  p.biasp = m.biasp;
-  const TcRounds r = tc_rounds(B, m.max_clusters, m.half_tiles);
-  if (r.n_full > 0)
-    if (int rc = tc_launch_fwd<128>(m, p, save, 0, r.n_full, s)) return rc;
-  if (r.n_half > 0)
-    if (int rc = tc_launch_fwd<64>(m, p, save, 2 * r.n_full, r.n_half, s)) return rc;
-  return 0;
-}
-
-static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* y, int B,
-                       int64_t row0, int64_t step, const float* denom, float* preds, float* out2, bool train,
-                       cudaStream_t s) {
-  TcImpl& m = *st.impl;
-  HeadParams h;
-  h.B = B; h.T = m.T; h.O = m.O; h.target_idx = c.target_idx; h.train = train ? 1 : 0;
-  h.xh = m.xh;
-  h.gamma = params + m.ogamma; h.beta = params + m.obeta; h.mean = params + m.omean; h.var = params + m.ovar;
-  h.eps = c.bn_epsilon;
-  h.Wo = params + m.oWo; h.bo = params + m.obo;
-  h.y = y; h.denom = denom; h.p1 = c.target_lambda; h.p2 = c.rnn_lambda;
-  h.use_dropout = (c.train && c.dropout > 0.f) ? 1 : 0;
-  h.key = dropout_key(c.seed, 0, step, c.dropout);
-  h.row0 = row0;
-  h.preds = preds;
-  // dhout / fp32 dpred are only produced on the dropout (SIMT) path; the tensor-core head leaves bf16 dpred tiles (dpb)
-  const bool simt_train = train && c.train && c.dropout > 0.f;
-  h.dhout = simt_train ? m.dhout : nullptr;
-  h.dpred = simt_train ? m.dpred : nullptr;
-  h.partial = m.head_part;
-  const int n_btiles = (B + 127) / 128;
-  const int n_tiles_cap = (m.maxB + 127) / 128;
-  int grid = m.T * n_btiles;
-  if (grid > m.head_ctas) grid = m.head_ctas;
-  h.partial = m.head_part;
-  HeadTcWeights hw;
-  hw.WoTp = m.WoTp; hw.bop = m.bop;
-  const bool use_tc = !h.use_dropout;       // the BN fold into the head weights needs y = a*h + b
-  int n_wcta = m.head_wctas;
-  if (train) {
-    if (use_tc) {
-      if (int rc = launch_pdl(head_tc_kernel<true>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, true, h, hw, m.tm_h128, m.tm_wot,
-                              m.tm_dpb, n_btiles, n_tiles_cap, m.head_wpart))
-        return rc;
-      n_wcta = grid;
-    } else {
-      head_rows_kernel<true><<<grid, 128, HROWS_SMEM, s>>>(h, m.tm_h128, n_btiles, n_tiles_cap);
-      LFMQ_LAUNCH_CHECK();
-      head_wgrad_kernel<<<m.head_wctas, 256, 0, s>>>(h, m.head_wpart);
-      LFMQ_LAUNCH_CHECK();
-    }
-  } else {
-    if (use_tc) {
-      if (int rc = launch_pdl(head_tc_kernel<false>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, true, h, hw, m.tm_h128,
-                              m.tm_wot, m.tm_wot, n_btiles, n_tiles_cap, (float*)nullptr))
-        return rc;
-    } else {
-      head_rows_kernel<false><<<grid, 128, HROWS_SMEM, s>>>(h, m.tm_h128, n_btiles, n_tiles_cap);
-      LFMQ_LAUNCH_CHECK();
-    }
-  }
-  if (y) {
-    const int n_out = HWG_PART + HEAD_PART;
-    if (int rc = launch_pdl(head_reduce_kernel, dim3((n_out * 32 + 255) / 256), dim3(256), 0, s, 1, true, grid,
-                            (const float*)m.head_part, n_wcta, (const float*)m.head_wpart, m.O, B, denom, c.target_lambda,
-                            c.rnn_lambda, train ? 1 : 0, grads ? grads + m.oWo : (float*)nullptr,
-                            grads ? grads + m.obo : (float*)nullptr, grads ? grads + m.ogamma : (float*)nullptr,
-                            grads ? grads + m.obeta : (float*)nullptr, out2))
-      return rc;
-    if (train && use_tc) {
-      if (int rc = launch_pdl(head_fold_kernel, dim3((TC_H + 127) / 128), dim3(128), 0, s, 1, true, m.O, grads + m.oWo,
-                              (const float*)(grads + m.obo), grads + m.ogamma, grads + m.obeta, params + m.oWo,
-                              params + m.ogamma, params + m.obeta, params + m.omean, params + m.ovar, c.bn_epsilon))
-        return rc;
-    }
-  }
-  return 0;
-}
-
-int tc_forward(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
-               int64_t step, float* preds, bool save, cudaStream_t s) {
-  if (!st.impl || !st.impl->enabled) {
-    LFMQ_SET_ERR("bf16 path not initialised");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
-  int rc;
-  if ((rc = tc_pack_weights(st, params, s))) return rc;
-  st.prof->begin(LFMQ_REGION_FWD, s);
-  if ((rc = tc_run_recurrence(st, x, B, save, s))) return rc;
-  st.prof->end(LFMQ_REGION_FWD, s);
-  if (preds) {
-    st.prof->begin(LFMQ_REGION_HEAD, s);
-    if ((rc = tc_run_head(st, c, params, nullptr, nullptr, B, row0, step, nullptr, preds, nullptr, false, s))) return rc;
-    st.prof->end(LFMQ_REGION_HEAD, s);
-  }
-  return 0;
-}
-
-int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, float* grads, int B, bool fused,
-                     cudaStream_t s);
-
-int tc_backward(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* x, const float* y,
-                int B, int64_t row0, int64_t step, const float* denom, float* tail, cudaStream_t s) {
-  if (!st.impl || !st.impl->enabled) {
-    LFMQ_SET_ERR("bf16 path not initialised");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
-  int rc;
-  if ((rc = tc_pack_weights(st, params, s))) return rc;
-  st.prof->begin(LFMQ_REGION_FWD, s);
-  if ((rc = tc_run_recurrence(st, x, B, true, s))) return rc;
-  st.prof->end(LFMQ_REGION_FWD, s);
-  st.prof->begin(LFMQ_REGION_HEAD, s);
-  if ((rc = tc_run_head(st, c, params, grads, y, B, row0, step, denom, nullptr, tail, true, s))) return rc;
-  st.prof->end(LFMQ_REGION_HEAD, s);
-  // the tensor-core head (no dropout) leaves dLoss/dpred tiles for the backward kernel to expand on its own MMAs
-  return tc_backward_impl(st, c, params, grads, B, /*fused=*/!(c.train && c.dropout > 0.f), s);
-}
-
-}  // namespace lfmq
-
-// =============================================================================================
 // Persistent backward recurrence (reverse t inside the kernel), clusters of 4 CTAs per 128-row tile.
 //   CTA r owns hidden units [64r, 64r+64): it computes dz_t for its 256 gate columns (pointwise, SURVEY App. A.4),
 //   stages them as the A operand in shared memory and multiplies by ITS K-slice of U (resident for the whole unroll):
@@ -1438,8 +1111,6 @@ int tc_backward(TcState& st, const lfmq_config& c, const float* params, float* g
 //   The N order of the resident U slice is rotated per CTA: accumulator columns 64d .. 64d+63 are hidden slice
 //   (r + d) mod 4, so the CTA's own slice is always columns 0..63.
 // =============================================================================================
-namespace lfmq {
-
 // Row units as in FwdParams: unit0 .. unit0 + n_units - 1, ROWS rows each.
 struct BwdParams {
   int B, T, n_iters, n_clusters, unit0, n_units, n_tiles_cap;
@@ -1476,10 +1147,10 @@ __device__ __forceinline__ uint32_t ld_b32(const __nv_bfloat16* p) { return *rei
 // dpred tile) into the own-slice columns of its accumulator.
 // ROWS: rows per cluster and round, 128 (a tile) or 64 (half a tile, see lstm_fwd_tc_kernel).  At 64 rows warpgroup 0
 // carries them exactly as it carries rows 0-63 of a tile, and warpgroup 1 has no rows; tm_dpb comes with 64-row boxes.
-// The body of lstm_bwd_tc_kernel (128 rows) and lstm_bwd_tc_half_kernel (64 rows), as lstm_fwd_tc.
 template <bool FUSED, int ROWS>
-__device__ __forceinline__ void lstm_bwd_tc(const BwdParams& p, const CUtensorMap& tm_ubk, const CUtensorMap& tm_dzst,
-                                            const CUtensorMap& tm_dpb, const CUtensorMap& tm_wos) {
+__global__ void __launch_bounds__(BWD_THREADS, 1)
+    lstm_bwd_tc_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
+                       const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
   extern __shared__ uint8_t smem_raw[];
   // Aligned by an offset from smem_raw rather than by masking a generic address, so that the compiler still knows the
   // pointer is shared: the staging stores and slice reads below then take 32-bit shared addresses (STS / LDS), not
@@ -1759,20 +1430,6 @@ __device__ __forceinline__ void lstm_bwd_tc(const BwdParams& p, const CUtensorMa
   cluster_sync_all();          // nobody leaves while peers may still store into / arrive on this CTA
 }
 
-template <bool FUSED>
-__global__ void __launch_bounds__(BWD_THREADS, 1)
-    lstm_bwd_tc_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
-                       const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
-  lstm_bwd_tc<FUSED, 128>(p, tm_ubk, tm_dzst, tm_dpb, tm_wos);
-}
-
-template <bool FUSED>
-__global__ void __launch_bounds__(BWD_THREADS, 1)
-    lstm_bwd_tc_half_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
-                            const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
-  lstm_bwd_tc<FUSED, 64>(p, tm_ubk, tm_dzst, tm_dpb, tm_wos);
-}
-
 // =============================================================================================
 // Weight gradients as ONE wgmma GEMM over all B*(T+1) rows (wgrad_gemm):  D[384 x 1024] = xh^T * dz   (both MN-major)
 //   rows 0..255 -> dU, rows 256..256+I-1 -> dW, row 288 (the constant-one column) -> db.
@@ -1796,70 +1453,359 @@ __global__ void wgrad_reduce_kernel(int S, int I, const float* __restrict__ part
   *dst = s;
 }
 
-int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, float* grads, int B, bool fused,
-                     cudaStream_t s) {
+// =============================================================================================
+// Host side
+// =============================================================================================
+static bool tc_supported(const lfmq_config& c, char* why, size_t n) {
+  if (c.rnn_cell != LFMQ_CELL_LSTM) { snprintf(why, n, "the bf16 tensor-core path is built for the LSTM cell only"); return false; }
+  if (c.uq) { snprintf(why, n, "the bf16 tensor-core path is built for the point-estimate head only"); return false; }
+  if (c.num_hidden != TC_H) { snprintf(why, n, "num_hidden must be 256 (got %d)", c.num_hidden); return false; }
+  if (c.num_layers != 1) { snprintf(why, n, "num_layers must be 1 (got %d)", c.num_layers); return false; }
+  if (c.n_inputs > 32) { snprintf(why, n, "n_inputs must be <= 32 (got %d)", c.n_inputs); return false; }
+  if (c.n_outputs > TC_OPAD) { snprintf(why, n, "n_outputs must be <= 16 (got %d)", c.n_outputs); return false; }
+  if (c.recurrent_dropout > 0.f) { snprintf(why, n, "recurrent_dropout is not built on the bf16 path"); return false; }
+  return true;
+}
+
+bool tc_shape_supported(const lfmq_config& c) {
+  char why[128];
+  return tc_supported(c, why, sizeof(why));
+}
+
+void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& cv) {
+  if (c.precision != LFMQ_PREC_BF16) return;
+  char why[128];
+  if (!tc_supported(c, why, sizeof(why))) return;   // tc_init reports the error
+  if (!st.impl) st.impl = new TcImpl;
   TcImpl& m = *st.impl;
+  const size_t B = (size_t)c.max_batch, T = (size_t)c.seq_len, H = TC_H;
+  m.maxB = c.max_batch; m.T = c.seq_len; m.I = c.n_inputs; m.O = c.n_outputs;
+  m.eps = c.bn_epsilon;
+  m.train = !c.forward_only;
+  m.dropout_head = c.train && c.dropout > 0.f;
+  m.xh = cv.take<__nv_bfloat16>(B * (T + 1) * TC_XH_LD);
+  m.Up = cv.take<__nv_bfloat16>(4 * H * H);
+  m.Wp = cv.take<__nv_bfloat16>(4 * H * 32);
+  m.Ubk = cv.take<__nv_bfloat16>(4 * H * H);
+  m.biasp = cv.take<float>(4 * H);
+  m.WoTp = cv.take<__nv_bfloat16>(TC_OPAD * H);
+  m.WoSp = cv.take<__nv_bfloat16>(H * 32);
+  m.bop = cv.take<float>(TC_OPAD);
+  m.n_sms = device_sm_count();
+  m.head_ctas = m.n_sms * 2;
+  m.head_wctas = m.n_sms * 2;
+  m.head_part_elems = (size_t)m.head_ctas * HEAD_PART;
+  m.head_part = cv.take<float>(m.head_part_elems);
+  if (m.train) {
+    const size_t Bt = (B + 127) / 128 * 128;      // saved state is blocked by 128-row tiles
+    m.gates = cv.take<__nv_bfloat16>(Bt * T * 4 * H);
+    m.cst = cv.take<__nv_bfloat16>(Bt * T * H);
+    m.dz = cv.take<__nv_bfloat16>(B * (T + 1) * 4 * H);
+    m.dhout = m.dropout_head ? cv.take<__nv_bfloat16>(Bt * T * H) : nullptr;   // only the dropout head uses these two
+    m.dpred = m.dropout_head ? cv.take<float>(B * T * TC_OPAD) : nullptr;
+    m.dpb = cv.take<__nv_bfloat16>(T * ((B + 127) / 128) * 128 * 32);
+    m.head_wpart = cv.take<float>((size_t)m.head_wctas * HWG_PART);
+    m.wg_part_elems = (size_t)64 * 384 * 1024;
+    m.wg_part = cv.take<float>(m.wg_part_elems);
+  } else {
+    m.gates = nullptr; m.cst = nullptr; m.dz = nullptr; m.dhout = nullptr; m.wg_part = nullptr;
+    m.dpred = nullptr; m.head_wpart = nullptr; m.dpb = nullptr;
+    m.wg_part_elems = 0;
+  }
+  // offsets of the tensors in the flat parameter vector: the API layer's layout() is the one place that defines them
+  m.oW = po.oW; m.oU = po.oU; m.ob = po.ob; m.ogamma = po.ogamma; m.obeta = po.obeta;
+  m.oWo = po.oWo; m.obo = po.obo; m.omean = po.omean; m.ovar = po.ovar;
+}
+
+// The instantiations of the two recurrences, [flag][i]: flag = SAVE / FUSED, i = 0 for 128-row tiles and 1 for 64-row
+// half tiles, as the pairs of maps in TcImpl.
+using FwdKernel = void (*)(FwdParams, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap);
+using BwdKernel = void (*)(BwdParams, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap);
+static const FwdKernel fwd_kernels[2][2] = {{lstm_fwd_tc_kernel<false, 128>, lstm_fwd_tc_kernel<false, 64>},
+                                            {lstm_fwd_tc_kernel<true, 128>, lstm_fwd_tc_kernel<true, 64>}};
+static const BwdKernel bwd_kernels[2][2] = {{lstm_bwd_tc_kernel<false, 128>, lstm_bwd_tc_kernel<false, 64>},
+                                            {lstm_bwd_tc_kernel<true, 128>, lstm_bwd_tc_kernel<true, 64>}};
+static_assert(BWD_NC == TC_NC, "both recurrences run on 4-CTA clusters");
+
+// Sets the dynamic shared memory of the four instantiations of a recurrence, and how many of its 4-CTA clusters can be
+// co-resident (one CTA per SM because of shared memory); fails if not even one fits.
+template <class Kernel>
+static int tc_cluster_setup(Kernel const (&kernels)[2][2], int threads, int smem, const char* what, int* max_clusters) {
+  for (const auto& by_rows : kernels)
+    for (Kernel k : by_rows) LFMQ_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(TC_NC * (device_sm_count() / TC_NC));
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = TC_NC;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  LFMQ_CUDA_CHECK(cudaOccupancyMaxActiveClusters(max_clusters, kernels[1][0], &cfg));
+  if (*max_clusters < 1) {
+    LFMQ_SET_ERR("no 4-CTA cluster of the %s kernel fits on this device", what);
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  return 0;
+}
+
+int tc_init(TcState& st, const lfmq_config& c) {
+  if (c.precision != LFMQ_PREC_BF16) return 0;
+  char why[128];
+  if (!tc_supported(c, why, sizeof(why))) {
+    LFMQ_SET_ERR("LFMQ_PREC_BF16 supports the H=256 single-layer forecaster only: %s; use LFMQ_PREC_FP32", why);
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  TcImpl& m = *st.impl;
+  const size_t B = (size_t)m.maxB, T = (size_t)m.T;
+  LFMQ_CUDA_CHECK(cudaMemset(m.xh, 0, B * (T + 1) * TC_XH_LD * 2));
+  if (m.dz) LFMQ_CUDA_CHECK(cudaMemset(m.dz, 0, B * (T + 1) * 4 * TC_H * 2));
+  const uint64_t xh_row = (uint64_t)(T + 1) * TC_XH_LD;     // elements per batch row of the 2-D view
+  const uint64_t dpb_rows = (uint64_t)m.T * ((m.maxB + 127) / 128) * 128;
   int rc;
-  if (!m.bwd_ready) {
-    LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_half_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    LFMQ_CUDA_CHECK(cudaFuncSetAttribute(lstm_bwd_tc_half_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
+  for (int i = 0; i < 2; ++i) {
+    const uint32_t rows = 128 >> i;          // rows of a tile (i = 0) or half tile (i = 1)
+    if ((rc = encode_map_2d(&m.tm_h[i], m.xh, xh_row, B, xh_row * 2, 64, rows / 4, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if ((rc = encode_map_2d(&m.tm_x[i], m.xh, xh_row, B, xh_row * 2, 32, rows, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
+    if (m.dpb && (rc = encode_map_2d(&m.tm_dpb[i], m.dpb, 32, dpb_rows, 64, 32, rows, CU_TENSOR_MAP_SWIZZLE_64B)))
+      return rc;
+  }
+  if ((rc = encode_map_2d(&m.tm_h128, m.xh, xh_row, B, xh_row * 2, 64, 128, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_wot, m.WoTp, TC_H, TC_OPAD, TC_H * 2, 64, 16, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_wos, m.WoSp, 32, TC_H, 64, 32, 64, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
+  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HT_SMEM));
+  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, HT_SMEM));
+  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HROWS_SMEM));
+  LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, HROWS_SMEM));
+  if ((rc = encode_map_2d(&m.tm_u, m.Up, TC_H, 4 * TC_H, TC_H * 2, 64, 256, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if ((rc = encode_map_2d(&m.tm_w, m.Wp, 32, 4 * TC_H, 64, 32, 256, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
+  if ((rc = tc_cluster_setup(fwd_kernels, FWD_THREADS, FWD_SMEM, "forward", &m.max_clusters))) return rc;
+  if (m.train) {
     if ((rc = wgrad_gemm_init())) return rc;
     // boxes of 64 hidden units: the kernel loads its K-slice of U in rotated N order (own hidden slice first)
     if ((rc = encode_map_2d(&m.tm_ubk, m.Ubk, 256, 4 * TC_H, 512, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-    cudaLaunchConfig_t qc = {};
-    qc.gridDim = dim3(BWD_NC * (m.n_sms / BWD_NC));
-    qc.blockDim = dim3(BWD_THREADS);
-    qc.dynamicSmemBytes = BWD_SMEM;
-    cudaLaunchAttribute qa[1];
-    qa[0].id = cudaLaunchAttributeClusterDimension;
-    qa[0].val.clusterDim.x = BWD_NC;
-    qa[0].val.clusterDim.y = 1;
-    qa[0].val.clusterDim.z = 1;
-    qc.attrs = qa;
-    qc.numAttrs = 1;
-    int ncl = 0;
-    LFMQ_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&ncl, lstm_bwd_tc_kernel<true>, &qc));
-    if (ncl < 1) {
-      LFMQ_SET_ERR("no 4-CTA cluster of the backward kernel fits on this device");
-      return LFMQ_ERR_UNSUPPORTED;
-    }
-    m.bwd_max_clusters = ncl;
-    m.bwd_ready = true;
+    if ((rc = tc_cluster_setup(bwd_kernels, BWD_THREADS, BWD_SMEM, "backward", &m.bwd_max_clusters))) return rc;
   }
+  // LFMQ_TC_HALF_TILES=0 keeps every round at 128-row tiles (A/B measurements, tests comparing the two schedules)
+  const char* ht = getenv("LFMQ_TC_HALF_TILES");
+  m.half_tiles = !(ht != nullptr && atoi(ht) == 0);
+  m.enabled = true;
+  st.weights_dirty = 1;
+  return 0;
+}
+
+void tc_destroy(TcState& st) {
+  delete st.impl;
+  st.impl = nullptr;
+}
+
+static int tc_pack_weights(TcState& st, const float* params, cudaStream_t s) {
+  TcImpl& m = *st.impl;
+  if (!st.weights_dirty) return 0;
+  const int nblk = (int)(((long)4 * TC_H * TC_H + 255) / 256);
+  PackArgs a;
+  a.I = m.I; a.O = m.O; a.eps = m.eps;
+  a.nb_w = nblk;
+  a.nb_h = (TC_H * 32 + 255) / 256;
+  a.nb_u = m.train ? nblk : 0;      // K-slices of U for the backward recurrence
+  a.W = params + m.oW; a.U = params + m.oU; a.bias = params + m.ob;
+  a.Wo = params + m.oWo; a.bo = params + m.obo; a.gamma = params + m.ogamma; a.beta = params + m.obeta;
+  a.mean = params + m.omean; a.var = params + m.ovar;
+  a.Up = m.Up; a.Wp = m.Wp; a.Ubk = m.Ubk; a.WoTp = m.WoTp; a.WoSp = m.WoSp; a.biasp = m.biasp; a.bop = m.bop;
+  if (int rc = launch_pdl(pack_all_kernel, dim3(a.nb_w + a.nb_h + a.nb_u), dim3(256), 0, s, 1, true, a)) return rc;
+  st.weights_dirty = 0;
+  return 0;
+}
+
+// The rounds of a persistent recurrence over B rows with at most max_clusters co-resident clusters: n_full 128-row tiles
+// (units 0 .. n_full - 1 of 128 rows), then n_half 64-row half tiles (units 2 n_full .. of 64 rows) in one more round.
+// Rounds are independent (each unit starts from zero state), so the two kinds are two launches in stream order.  The
+// last round runs as half tiles whenever they fit on the co-resident clusters: a round of a few whole tiles leaves
+// most clusters idle for all T steps while the busy ones carry 128 rows through every step's dependency chain.
+struct TcRounds {
+  int n_full, n_half;
+};
+
+static TcRounds tc_rounds(int B, int max_clusters, bool half_tiles) {
+  const int n_tiles = (B + 127) / 128;
+  const int n_cl = n_tiles < max_clusters ? n_tiles : max_clusters;
+  const int full_rounds = (n_tiles + n_cl - 1) / n_cl - 1;
+  const int rows_last = B - full_rounds * n_cl * 128;
+  if (half_tiles && (rows_last + 63) / 64 <= max_clusters) return {full_rounds * n_cl, (rows_last + 63) / 64};
+  return {n_tiles, 0};
+}
+
+// n_units units of ROWS rows from unit0 on, in rounds of at most max_clusters clusters
+template <class Params>
+static void tc_set_rounds(Params& p, int unit0, int n_units, int max_clusters) {
+  p.unit0 = unit0;
+  p.n_units = n_units;
+  p.n_clusters = n_units < max_clusters ? n_units : max_clusters;
+  p.n_iters = (n_units + p.n_clusters - 1) / p.n_clusters;
+}
+
+// Runs a recurrence over the rounds of its p.B rows (tc_rounds): the 128-row instantiation over the n_full tiles, then
+// the 64-row one over the n_half half tiles.  FwdParams runs lstm_fwd_tc_kernel<flag = SAVE, ·>, BwdParams
+// lstm_bwd_tc_kernel<flag = FUSED, ·>, whose dz stores go through tm_dzst.
+template <class Params>
+static int tc_run_rounds(const TcImpl& m, Params p, bool flag, cudaStream_t s, const CUtensorMap* tm_dzst = nullptr) {
+  constexpr bool fwd = std::is_same<Params, FwdParams>::value;
+  const int max_clusters = fwd ? m.max_clusters : m.bwd_max_clusters;
+  const TcRounds r = tc_rounds(p.B, max_clusters, m.half_tiles);
+  for (int i = 0; i < 2; ++i) {
+    const int n_units = i == 0 ? r.n_full : r.n_half;
+    if (n_units == 0) continue;
+    tc_set_rounds(p, i == 0 ? 0 : 2 * r.n_full, n_units, max_clusters);
+    const dim3 grid(TC_NC * p.n_clusters);
+    int rc;
+    if constexpr (fwd)
+      rc = launch_pdl(fwd_kernels[flag][i], grid, dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, true, p, m.tm_h[i], m.tm_x[i],
+                      m.tm_u, m.tm_w);
+    else
+      rc = launch_pdl(bwd_kernels[flag][i], grid, dim3(BWD_THREADS), BWD_SMEM, s, TC_NC, true, p, m.tm_ubk, *tm_dzst,
+                      m.tm_dpb[i], m.tm_wos);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+static int tc_run_recurrence(TcState& st, const float* x, int B, bool save, cudaStream_t s) {
+  TcImpl& m = *st.impl;
+  const long bt = (long)B * m.T * 5;
+  if (int rc = launch_pdl(xh_fill_x_kernel, dim3((int)((bt + 255) / 256)), dim3(256), 0, s, 1, true, B, m.T, m.I, x, m.xh)) return rc;
+  FwdParams p;
+  p.B = B; p.T = m.T;
+  p.k16_x = (m.I + 15) / 16;
+  p.n_tiles_cap = (m.maxB + 127) / 128;
+  p.xh = m.xh;
+  p.gates = save ? m.gates : nullptr;
+  p.cst = save ? m.cst : nullptr;
+  p.biasp = m.biasp;
+  return tc_run_rounds(m, p, save, s);
+}
+
+static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* y, int B,
+                       int64_t row0, int64_t step, const float* denom, float* preds, float* out2, bool train,
+                       cudaStream_t s) {
+  TcImpl& m = *st.impl;
+  HeadParams h;
+  h.B = B; h.T = m.T; h.O = m.O; h.target_idx = c.target_idx;
+  h.xh = m.xh;
+  h.gamma = params + m.ogamma; h.beta = params + m.obeta; h.mean = params + m.omean; h.var = params + m.ovar;
+  h.eps = c.bn_epsilon;
+  h.Wo = params + m.oWo; h.bo = params + m.obo;
+  h.y = y; h.denom = denom; h.p1 = c.target_lambda; h.p2 = c.rnn_lambda;
+  h.use_dropout = m.dropout_head ? 1 : 0;
+  h.key = dropout_key(c.seed, 0, step, c.dropout);
+  h.row0 = row0;
+  h.preds = preds;
+  // dhout / fp32 dpred exist only for the dropout head in training; the tensor-core head leaves bf16 dpred tiles (dpb)
+  h.dhout = train ? m.dhout : nullptr;
+  h.dpred = train ? m.dpred : nullptr;
+  h.partial = m.head_part;
+  const int n_btiles = (B + 127) / 128;
+  const int n_tiles_cap = (m.maxB + 127) / 128;
+  int grid = m.T * n_btiles;
+  if (grid > m.head_ctas) grid = m.head_ctas;
+  HeadTcWeights hw;
+  hw.WoTp = m.WoTp; hw.bop = m.bop;
+  const bool use_tc = !m.dropout_head;      // the BN fold into the head weights needs y = a*h + b
+  int n_wcta = m.head_wctas;
+  if (train) {
+    if (use_tc) {
+      if (int rc = launch_pdl(head_tc_kernel<true>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, true, h, hw, m.tm_h128, m.tm_wot,
+                              m.tm_dpb[0], n_btiles, n_tiles_cap, m.head_wpart))
+        return rc;
+      n_wcta = grid;
+    } else {
+      head_rows_kernel<true><<<grid, 128, HROWS_SMEM, s>>>(h, m.tm_h128, n_btiles, n_tiles_cap);
+      LFMQ_LAUNCH_CHECK();
+      head_wgrad_kernel<<<m.head_wctas, 256, 0, s>>>(h, m.head_wpart);
+      LFMQ_LAUNCH_CHECK();
+    }
+  } else {
+    if (use_tc) {
+      if (int rc = launch_pdl(head_tc_kernel<false>, dim3(grid), dim3(HT_THREADS), HT_SMEM, s, 1, true, h, hw, m.tm_h128,
+                              m.tm_wot, m.tm_wot, n_btiles, n_tiles_cap, (float*)nullptr))
+        return rc;
+    } else {
+      head_rows_kernel<false><<<grid, 128, HROWS_SMEM, s>>>(h, m.tm_h128, n_btiles, n_tiles_cap);
+      LFMQ_LAUNCH_CHECK();
+    }
+  }
+  if (y) {
+    const int n_out = HWG_PART + HEAD_PART;
+    if (int rc = launch_pdl(head_reduce_kernel, dim3((n_out * 32 + 255) / 256), dim3(256), 0, s, 1, true, grid,
+                            (const float*)m.head_part, n_wcta, (const float*)m.head_wpart, m.O, B, denom, c.target_lambda,
+                            c.rnn_lambda, train ? 1 : 0, grads ? grads + m.oWo : (float*)nullptr,
+                            grads ? grads + m.obo : (float*)nullptr, grads ? grads + m.ogamma : (float*)nullptr,
+                            grads ? grads + m.obeta : (float*)nullptr, out2))
+      return rc;
+    if (train && use_tc) {
+      if (int rc = launch_pdl(head_fold_kernel, dim3((TC_H + 127) / 128), dim3(128), 0, s, 1, true, m.O, grads + m.oWo,
+                              (const float*)(grads + m.obo), grads + m.ogamma, grads + m.obeta, params + m.oWo,
+                              params + m.ogamma, params + m.obeta, params + m.omean, params + m.ovar, c.bn_epsilon))
+        return rc;
+    }
+  }
+  return 0;
+}
+
+int tc_forward(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
+               int64_t step, float* preds, bool save, cudaStream_t s) {
+  if (!st.impl || !st.impl->enabled) {
+    LFMQ_SET_ERR("bf16 path not initialised");
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  int rc;
+  if ((rc = tc_pack_weights(st, params, s))) return rc;
+  st.prof->begin(LFMQ_REGION_FWD, s);
+  if ((rc = tc_run_recurrence(st, x, B, save, s))) return rc;
+  st.prof->end(LFMQ_REGION_FWD, s);
+  if (preds) {
+    st.prof->begin(LFMQ_REGION_HEAD, s);
+    if ((rc = tc_run_head(st, c, params, nullptr, nullptr, B, row0, step, nullptr, preds, nullptr, false, s))) return rc;
+    st.prof->end(LFMQ_REGION_HEAD, s);
+  }
+  return 0;
+}
+
+int tc_backward(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* x, const float* y,
+                int B, int64_t row0, int64_t step, const float* denom, float* tail, cudaStream_t s) {
+  if (!st.impl || !st.impl->enabled) {
+    LFMQ_SET_ERR("bf16 path not initialised");
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  TcImpl& m = *st.impl;
   const size_t T = (size_t)m.T;
+  int rc;
+  if ((rc = tc_pack_weights(st, params, s))) return rc;
+  st.prof->begin(LFMQ_REGION_FWD, s);
+  if ((rc = tc_run_recurrence(st, x, B, true, s))) return rc;
+  st.prof->end(LFMQ_REGION_FWD, s);
+  st.prof->begin(LFMQ_REGION_HEAD, s);
+  if ((rc = tc_run_head(st, c, params, grads, y, B, row0, step, denom, nullptr, tail, true, s))) return rc;
+  st.prof->end(LFMQ_REGION_HEAD, s);
+
   st.prof->begin(LFMQ_REGION_BWD, s);
+  BwdParams bp;
+  bp.B = B; bp.T = m.T;
+  bp.n_tiles_cap = (m.maxB + 127) / 128;
+  bp.gates = m.gates; bp.cst = m.cst; bp.dhout = m.dhout;
+  // dz as [b][t][1024] with columns ordered [16-unit block][gate][16]: one warpgroup's part of a staged chunk =
+  // 64 rows x 64 columns
+  CUtensorMap tm_dzst;
   {
-    BwdParams bp;
-    bp.B = B; bp.T = m.T;
-    bp.n_tiles_cap = (m.maxB + 127) / 128;
-    bp.gates = m.gates; bp.cst = m.cst; bp.dhout = m.dhout;
-    // dz as [b][t][1024] with columns ordered [16-unit block][gate][16]: one warpgroup's part of a staged chunk =
-    // 64 rows x 64 columns
-    CUtensorMap tm_dzst;
-    {
-      const uint64_t dims[3] = {1024, (uint64_t)(T + 1), (uint64_t)B};
-      const uint64_t strides[2] = {2048, (uint64_t)2048 * (T + 1)};
-      const uint32_t box[3] = {64, 1, 64};
-      if ((rc = encode_map_bf16(&tm_dzst, m.dz, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-    }
-    const TcRounds r = tc_rounds(B, m.bwd_max_clusters, m.half_tiles);
-    if (r.n_full > 0) {
-      tc_set_rounds(bp, 0, r.n_full, m.bwd_max_clusters);
-      if ((rc = launch_pdl(fused ? lstm_bwd_tc_kernel<true> : lstm_bwd_tc_kernel<false>,
-                           dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, true, bp, m.tm_ubk,
-                           tm_dzst, m.tm_dpb, m.tm_wos)))
-        return rc;
-    }
-    if (r.n_half > 0) {
-      tc_set_rounds(bp, 2 * r.n_full, r.n_half, m.bwd_max_clusters);
-      if ((rc = launch_pdl(fused ? lstm_bwd_tc_half_kernel<true> : lstm_bwd_tc_half_kernel<false>,
-                           dim3(BWD_NC * bp.n_clusters), dim3(BWD_THREADS), BWD_SMEM, s, BWD_NC, true, bp, m.tm_ubk,
-                           tm_dzst, m.tm_dpb64, m.tm_wos)))
-        return rc;
-    }
+    const uint64_t dims[3] = {1024, (uint64_t)(T + 1), (uint64_t)B};
+    const uint64_t strides[2] = {2048, (uint64_t)2048 * (T + 1)};
+    const uint32_t box[3] = {64, 1, 64};
+    if ((rc = encode_map_bf16(&tm_dzst, m.dz, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   }
+  // the tensor-core head (no dropout) leaves dLoss/dpred tiles for the backward kernel to expand on its own MMAs
+  if ((rc = tc_run_rounds(m, bp, /*fused=*/!m.dropout_head, s, &tm_dzst))) return rc;
   st.prof->end(LFMQ_REGION_BWD, s);
 
   st.prof->begin(LFMQ_REGION_WGRAD, s);
@@ -1875,8 +1821,6 @@ int tc_backward_impl(TcState& st, const lfmq_config& c, const float* params, flo
                        (const float*)m.wg_part, grads + m.oU, grads + m.oW, grads + m.ob)))
     return rc;
   st.prof->end(LFMQ_REGION_WGRAD, s);
-  (void)params;
-  (void)c;
   return 0;
 }
 

@@ -78,6 +78,24 @@ def test_tensor_core_workspace_leaves_out_fp32_activations():
     assert ws(N.PREC_BF16, 65536, 1) < ws(N.PREC_FP32, 65536, 1)
 
 
+def test_cluster_path_carves_dropout_head_buffers_only_with_dropout():
+    """A bf16 training handle without dropout runs the tensor-core head, fused with the backward recurrence: it carves
+    neither the dropout head's dLoss/dh (bf16 [tiles*128][T][H]) nor its fp32 dLoss/dpred ([B*T][16])."""
+    lib = N.load()
+    B, T, F, O, H = 4096, 48, 32, 16, 256
+
+    def ws(dropout):
+        n = C.c_uint64(0)
+        cfg = _cfg(max_batch=B, seq_len=T, n_inputs=F, n_outputs=O, num_hidden=H, target_idx=O - 1,
+                   precision=N.PREC_BF16, train=1, dropout=dropout)
+        N.check(lib.lfmq_workspace_bytes(C.byref(cfg), C.byref(n)))
+        return n.value
+
+    dhout = (B + 127) // 128 * 128 * T * H * 2
+    dpred = B * T * 16 * 4
+    assert ws(0.0) + dhout + dpred <= ws(0.2)
+
+
 def test_engine_refuses_to_run_without_cuda():
     import torch
     if torch.cuda.is_available():

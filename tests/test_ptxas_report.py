@@ -5,8 +5,9 @@ step loop, costs time on every one of the T steps without changing any result, s
 compiles every library source with exactly the commands the Makefile runs (`make -n -B`, objects redirected to a
 temporary directory) and reads `-Xptxas -v`:
   - no kernel may have its wgmma serialised (C7510-C7520 "Potential Performance Loss ... serialized");
-  - lstm_fwd_tc_kernel and lstm_bwd_tc_kernel, both instantiations each, must not spill: 0 bytes of spill stores and
-    loads, and no local-memory load or store (LDL / STL) anywhere in their SASS.
+  - lstm_fwd_tc_kernel<SAVE, ROWS> and lstm_bwd_tc_kernel<FUSED, ROWS>, all four instantiations each (128-row tiles
+    and 64-row half tiles), must not spill: 0 bytes of spill stores and loads, and no local-memory load or store
+    (LDL / STL) anywhere in their SASS.
 """
 import os
 import re
@@ -20,6 +21,7 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 RECURRENCES = ('lstm_fwd_tc_kernel', 'lstm_bwd_tc_kernel')
+ROWS = (128, 64)                   # tiles, half tiles
 
 
 def _nvcc():
@@ -86,11 +88,12 @@ def _spills(log):
     return out
 
 
-def _instantiations(names, name):
-    """The mangled names of the <false> and <true> instantiations of a bool-templated kernel."""
-    found = [k for k in names if re.match(r'_ZN4lfmq%d%sILb[01]E' % (len(name), name), k)]
-    assert len(found) == 2, (name, sorted(names))
-    return found
+def _instantiations(names, name, rows):
+    """The mangled names of the <false, rows> and <true, rows> instantiations of a recurrence, after checking that all
+    four <flag, ROWS> instantiations (flag false / true, ROWS 128 / 64) are there."""
+    found = [k for k in names if re.match(r'_ZN4lfmq%d%sILb[01]ELi(128|64)EEEv' % (len(name), name), k)]
+    assert len(found) == 4, (name, sorted(names))
+    return [k for k in found if 'ELi%dEE' % rows in k]
 
 
 def test_no_serialised_wgmma(build):
@@ -99,16 +102,18 @@ def test_no_serialised_wgmma(build):
     assert not bad, '\n'.join(bad)
 
 
+@pytest.mark.parametrize('rows', ROWS)
 @pytest.mark.parametrize('kernel', RECURRENCES)
-def test_recurrence_does_not_spill(build, kernel):
+def test_recurrence_does_not_spill(build, kernel, rows):
     log, _ = build
     spills = _spills(log)
-    for k in _instantiations(spills, kernel):
+    for k in _instantiations(spills, kernel, rows):
         assert spills[k] == (0, 0), '%s: %d B spill stores, %d B spill loads' % ((k,) + spills[k])
 
 
+@pytest.mark.parametrize('rows', ROWS)
 @pytest.mark.parametrize('kernel', RECURRENCES)
-def test_recurrence_sass_has_no_local_memory_access(build, kernel):
+def test_recurrence_sass_has_no_local_memory_access(build, kernel, rows):
     _, sass = build
     if sass is None:
         pytest.skip('cuobjdump not found')
@@ -121,6 +126,6 @@ def test_recurrence_sass_has_no_local_memory_access(build, kernel):
             funcs[cur] = []
         elif cur:
             funcs[cur].append(line)
-    for k in _instantiations(funcs, kernel):
+    for k in _instantiations(funcs, kernel, rows):
         local = [l.strip() for l in funcs[k] if re.search(r'\b(LDL|STL)\b', l)]
         assert not local, '%s: %d local-memory instructions, e.g. %s' % (k, len(local), local[:3])
