@@ -29,16 +29,20 @@ extern "C" {
 enum { LFMQ_OK = 0, LFMQ_ERR_ARG = 1, LFMQ_ERR_CUDA = 2, LFMQ_ERR_UNSUPPORTED = 3, LFMQ_ERR_WORKSPACE = 4 };
 enum { LFMQ_OPT_ADADELTA = 0, LFMQ_OPT_ADAM = 1, LFMQ_OPT_RMSPROP = 2, LFMQ_OPT_SGD = 3 };
 /* LFMQ_PREC_FP32:   fp32 SIMT arithmetic everywhere (the parity mode, <=1e-4 rel vs the oracle; any cell / head).
- * LFMQ_PREC_BF16:   gate GEMMs on wgmma tensor cores with bf16 operands, fp32 accumulate, fp32 cell state.  LSTM cell,
- *                   point-estimate head, num_hidden a multiple of 64 (<= 1024), any num_layers, dropout and recurrent
- *                   dropout; H = 256 / L = 1 without recurrent dropout runs the persistent cluster kernels.
- * LFMQ_PREC_BF16X3: fp32-tolerance forward on tensor cores (forward_only handles: predict.py:129): every operand split
- *                   into bf16 high + low halves, three wgmma products per GEMM (hi*hi + lo*hi + hi*lo), accurate
- *                   expf / tanhf gate nonlinearities, fp32 head -- <=1e-4 rel vs the oracle. */
+ * LFMQ_PREC_BF16:   gate GEMMs on wgmma tensor cores with bf16 operands, fp32 accumulate, fp32 cell state.
+ *                   num_hidden a multiple of 64 (<= 512), any num_layers, dropout and recurrent dropout.  Training: LSTM
+ *                   cell, point-estimate head.  forward_only handles: LSTM or GRU cell, point-estimate or uq head (uq:
+ *                   Dropout / recurrent dropout stay active, as on the fp32 path).  The LSTM point estimate at H = 256 /
+ *                   L = 1 without recurrent dropout runs the persistent cluster kernels.
+ * LFMQ_PREC_BF16X3: fp32-tolerance forward on tensor cores (forward_only handles: predict.py:129), same cells and heads
+ *                   as forward_only LFMQ_PREC_BF16: every operand split into bf16 high + low halves, three wgmma products
+ *                   per GEMM (hi*hi + lo*hi + hi*lo), accurate expf / tanhf gate nonlinearities, fp32 head -- <=1e-4 rel
+ *                   vs the oracle. */
 enum { LFMQ_PREC_FP32 = 0, LFMQ_PREC_BF16 = 1, LFMQ_PREC_BF16X3 = 2 };
 
 /* config.rnn_cell (lfm_quant.py:39; rnn_point_estimate.py:80-102).  GRU is Keras' default reset_after=True cell:
- * 3 gate blocks z|r|h, bias [2][3H] (input row, recurrent row).  LFMQ_PREC_BF16 supports the LSTM cell only. */
+ * 3 gate blocks z|r|h, bias [2][3H] (input row, recurrent row).  The tensor-core precisions train the LSTM cell only;
+ * they run the GRU cell on forward_only handles. */
 enum { LFMQ_CELL_LSTM = 0, LFMQ_CELL_GRU = 1 };
 
 typedef struct lfmq_handle_s* lfmq_handle;

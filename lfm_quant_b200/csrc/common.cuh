@@ -149,6 +149,9 @@ __device__ __forceinline__ void dropout_quad(const DropoutKey& k, uint64_t q, fl
   for (int i = 0; i < 4; ++i) m[i] = ((r[i] >> 8) >= k.thr) ? k.scale : 0.0f;
 }
 
+// softplus of the variance head (custom_layers.py:12-13), shared by the SIMT and tensor-core heads
+__device__ __forceinline__ float softplus_f(float a) { return fmaxf(a, 0.f) + log1pf(expf(-fabsf(a))); }
+
 // Carves the caller's workspace into buffers on 1024-byte boundaries; with base == nullptr it only sizes.
 constexpr size_t WS_ALIGN = 1024;
 inline size_t ws_align_up(size_t v) { return (v + WS_ALIGN - 1) / WS_ALIGN * WS_ALIGN; }

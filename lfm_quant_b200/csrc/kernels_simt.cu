@@ -781,8 +781,6 @@ __global__ void loss_final_kernel(int nblk, const double* __restrict__ partial, 
 // RNNUqRangeEstimate head and loss (rnn_uq_range_estimate.py:104-108, model_utils/custom_layers.py:12-13,
 // model_utils/losses.py:180-284).
 // =============================================================================================
-__device__ __forceinline__ float softplus_f(float a) { return fmaxf(a, 0.f) + log1pf(expf(-fabsf(a))); }
-
 // var = max(softplus(a), 1e-6); in place when var == a
 __global__ void softplus_floor_kernel(long n, const float* __restrict__ a, float* __restrict__ var) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;

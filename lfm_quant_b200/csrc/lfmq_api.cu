@@ -207,7 +207,7 @@ size_t layout(lfmq_handle_s* h, char* base) {
       }
       char why[160];
       if (lfmq::gen_supported(c, why, sizeof(why)))      // lfmq_create reports unsupported configurations (gen_init)
-        lfmq::gen_layout(h->tc, c, lo.data(), h->oWo, h->obo, cv);
+        lfmq::gen_layout(h->tc, c, lo.data(), h->oWo, h->obo, h->oWv, h->obv, cv);
     } else {
       const LayerBuf& lb = h->layers[0];
       lfmq::tc_layout(h->tc, c, lfmq::TcParamOff{lb.oW, lb.oU, lb.ob, lb.ogamma, lb.obeta, lb.omean, lb.ovar, h->oWo, h->obo},
@@ -573,6 +573,7 @@ int32_t lfmq_forward_uq(lfmq_handle h, const float* x, int32_t B, int64_t row0, 
   }
   h->last_step = step;
   h->last_row0 = row0;
+  if (h->use_gen) return lfmq::gen_forward_uq(h->tc, h->cfg, h->params, x, B, row0, step, preds, var, (cudaStream_t)stream);
   return forward_fp32(h, x, B, row0, step, preds, var, (cudaStream_t)stream);
 }
 

@@ -1,11 +1,15 @@
-// General tensor-core path of the recurrent forecaster (LSTM cell, point-estimate head): every shape the H=256 / L=1
-// cluster kernels of lstm_tc.cu do not cover -- H a multiple of 64 up to 512, stacked layers, dropout and recurrent
-// dropout (BASELINE configs[2]: H=512, L=2, dropout) -- and the fp32-tolerance mode LFMQ_PREC_BF16X3.
+// General tensor-core path of the recurrent forecaster: every shape the H=256 / L=1 LSTM cluster kernels of lstm_tc.cu
+// do not cover -- H a multiple of 64 up to 512, stacked layers, dropout and recurrent dropout (BASELINE configs[2]:
+// H=512, L=2, dropout) -- and the fp32-tolerance mode LFMQ_PREC_BF16X3.  Training runs the LSTM point estimate;
+// forward-only handles also run the GRU cell and the RNNUqRangeEstimate heads (MC dropout included).
 //
 // One wgmma tile-GEMM skeleton (TMA ring -> wgmma -> register accumulators -> epilogue in the same warpgroups) with
 // these epilogues:
 //   EPI_FWD    z_t = [h_{t-1} (*rec mask) | in_t] [U; W]   (one launch per time step and layer)
 //              epilogue = bias, gate nonlinearities, c_t / h_t update, h_t -> next step's A operand, saved state
+//   EPI_GRU_FWD  the same GEMM on the GRU's packed [U; W] (gate slots z | r | n_x | n_h, see gpack_kernel)
+//              epilogue = Keras reset-after GRU update of h_t (carried in fp32), forward-only: nothing saved
+//   EPI_HEAD_UQ  [pred | var pre-activation] = y [Wo | Wv] (N = 32), epilogue = biases, softplus floor
 //   EPI_BWD    rec = dz_{t+1} U^T                           (one launch per time step and layer, reverse time)
 //              epilogue = BPTT pointwise algebra of step t (SURVEY App. A.4) -> dz_t, carried dLoss/dc
 //   EPI_STORE  C = A B^T as bf16 (dLoss/d(input) of layers above the first: dz W^T)
@@ -17,7 +21,8 @@
 // Data layout (time-major, Bp = maxB rounded up to 128 rows, "blocked" = [..][row tile][16-unit block][piece][4 warps]
 // [32 lanes][16] so that a warp's 32-byte-per-thread access is 1 KB contiguous):
 //   hseq[l]  bf16 [T+1][Bp][H]    slot t = h_{t-1} (slot 0 zero): A operand of step t, input of BN/Dropout, A^T of dU
-//   hmseq[l] bf16 [T+1][Bp][H]    recurrent dropout only: h_{t-1} * mask (what the recurrence and dU actually consume)
+//   hmseq[l] bf16 [T+1][Bp][H]    recurrent dropout only: h_{t-1} * mask (what the recurrence and dU actually consume);
+//                                 hmseq_lo[l] its low halves (bf16x3)
 //   in[l]    bf16 [T][Bp][Ipad]   layer input (l = 0: x cast to bf16; l > 0: Dropout(BN(h_{l-1}))); in[L] feeds the head
 //   gates[l] bf16 blocked [T][row tile][H/16][4 gates]   post-activation i, f, g, o;  cst[l] blocked [T][row tile][H/16]
 //   dz       bf16 [T][Bp][4H]     gate pre-activation gradients, standard column order i|f|g|o (shared by the layers)
@@ -77,7 +82,12 @@ struct GArgs {
   unsigned int* gbar;  // [gridDim.x], zeroed before the launch; counts the group's CTAs that have finished a step
 };
 
-enum { EPI_FWD = 0, EPI_BWD = 1, EPI_STORE = 2, EPI_FWD_ACC = 3, EPI_HEAD = 4 };   // _ACC: expf / tanhf (bf16x3)
+enum {   // _ACC: expf / tanhf (bf16x3)
+  EPI_FWD = 0, EPI_BWD = 1, EPI_STORE = 2, EPI_FWD_ACC = 3, EPI_HEAD = 4, EPI_GRU_FWD = 5, EPI_GRU_FWD_ACC = 6,
+  EPI_HEAD_UQ = 7
+};
+constexpr bool epi_is_fwd(int e) { return e == EPI_FWD || e == EPI_FWD_ACC || e == EPI_GRU_FWD || e == EPI_GRU_FWD_ACC; }
+constexpr bool epi_is_head(int e) { return e == EPI_HEAD || e == EPI_HEAD_UQ; }
 
 struct EpiParams {
   // common
@@ -85,7 +95,7 @@ struct EpiParams {
   int64_t row0;
   // forward
   const float* bias;            // [4H] in the packed column order (sigmoid gates pre-scaled by 1/2 unless accurate)
-  float* cstate;                // fp32 blocked [row tile][H/16][4][32][16]: c_{t-1} in, c_t out
+  float* cstate;                // fp32 blocked [row tile][H/16][4][32][16]: c_{t-1} in, c_t out (GRU: h_{t-1} in, h_t out)
   __nv_bfloat16* hseq;          // [T+1][Bp][H]
   __nv_bfloat16* hseq_lo;       // bf16x3: low halves of h
   __nv_bfloat16* hmseq;         // recurrent dropout: masked copy (null otherwise)
@@ -111,22 +121,27 @@ struct EpiParams {
   float* hpartial;              // [GH_PART][gridDim.x]
   float hp1, hp2;
   int hO, htarget, htrain;
+  // forward, bf16x3 with recurrent dropout: low halves of the masked h
+  __nv_bfloat16* hmseq_lo;
+  // variance head (EPI_HEAD_UQ): var = max(softplus(y Wv + bv), 1e-6)
+  const float* hbv;             // [O]
+  float* hvar;                  // [B][T][O] fp32
 };
 
 // Two consumer warpgroups per CTA (rows 0-63 / 64-127 of the 128-row M tile, each with an m64 x BN accumulator in
 // registers) and one TMA producer warp.  The forward (N = 256: 128 accumulator registers per thread) and backward
-// steps run one CTA per SM; the multi-wave GEMMs (EPI_STORE, EPI_HEAD) keep two CTAs per SM.  The ring takes whatever
+// steps run one CTA per SM; the multi-wave GEMMs (EPI_STORE, the heads) keep two CTAs per SM.  The ring takes whatever
 // shared memory one / two resident CTAs leave: the loads are latency-bound, bytes in flight are what buys bandwidth.
 template <int BN, int EPI>
 struct GSmem {
   static constexpr uint32_t A_BYTES = 128 * 128;          // 128 rows x 64 bf16
   static constexpr uint32_t B_BYTES = BN * 128;
   static constexpr uint32_t STAGE = A_BYTES + B_BYTES;
-  static constexpr int CTAS_PER_SM = (EPI == 2 || EPI == 4) ? 2 : 1;      // (2 = EPI_STORE, 4 = EPI_HEAD)
+  static constexpr int CTAS_PER_SM = (EPI == 2 || epi_is_head(EPI)) ? 2 : 1;      // (2 = EPI_STORE)
   static constexpr int NS = (int)((CTAS_PER_SM == 2 ? 98304u : 196608u) / STAGE);
   static constexpr uint32_t BARS = NS * STAGE;
-  static constexpr uint32_t HEAD_ROWS = BARS + 256;        // EPI_HEAD: [128][17] fp32 pred rows
-  static constexpr uint32_t TOTAL = HEAD_ROWS + (EPI == 4 ? 128 * 17 * 4 : 0) + 1024;   // + alignment slack
+  static constexpr uint32_t HEAD_ROWS = BARS + 256;        // heads: [128][BN + 1] fp32 accumulator rows
+  static constexpr uint32_t TOTAL = HEAD_ROWS + (epi_is_head(EPI) ? 128 * (BN + 1) * 4 : 0) + 1024;   // + alignment slack
   static constexpr int THREADS = 2 * 128 + 32;
 };
 
@@ -145,6 +160,7 @@ __device__ __forceinline__ void wgmma_bn(float (&acc)[BN / 2], uint64_t da, uint
   if constexpr (BN == 256) wgmma_m64n256k16<0, 0>(acc, da, db, accumulate);
   if constexpr (BN == 128) wgmma_m64n128k16<0, 0>(acc, da, db, accumulate);
   if constexpr (BN == 64) wgmma_m64n64k16<0, 0>(acc, da, db, accumulate);
+  if constexpr (BN == 32) wgmma_m64n32k16<0, 0>(acc, da, db, accumulate);
   if constexpr (BN == 16) wgmma_m64n16k16<0, 0>(acc, da, db, accumulate);
 }
 
@@ -208,7 +224,12 @@ __device__ __forceinline__ void epi_fwd(const EpiParams& p, const float (&acc)[1
           if (p.hmseq) {
             float mk[4];
             rec_mask4(p.rkey, p.row0 + b, p.H, j, mk);
-            st_b32(p.hmseq + hoff, pack_bf16x2(mk[j & 3] * hv[0], mk[(j & 3) + 1] * hv[1]));
+            const float m0 = mk[j & 3] * hv[0], m1 = mk[(j & 3) + 1] * hv[1];
+            const uint32_t wm = pack_bf16x2(m0, m1);
+            st_b32(p.hmseq + hoff, wm);
+            if constexpr (ACC) {      // bf16x3: the masked h is the A operand of the lo(h) hi(W) pass
+              if (p.hmseq_lo) st_b32(p.hmseq_lo + hoff, pack_bf16x2(m0 - bf16_lo(wm), m1 - bf16_hi(wm)));
+            }
           }
           if (p.gates) {
             const long sb = (((long)p.t * p.NRT + rt) * p.NB16 + gblk);
@@ -217,6 +238,75 @@ __device__ __forceinline__ void epi_fwd(const EpiParams& p, const float (&acc)[1
 #pragma unroll
             for (int g = 0; g < 4; ++g) st_b32(gp + g * gstride, pack_bf16x2(gv[g][0], gv[g][1]));
             st_b32(p.cst + ((sb * 4 + (m >> 5)) * 32 + (m & 31)) * 16 + jj, pack_bf16x2(cn[0], cn[1]));
+          }
+        }
+      }
+    }
+  }
+}
+
+// ---- EPI_GRU_FWD: Keras reset-after GRU (rnn_point_estimate.py:89-98; the SIMT gru_pointwise_fwd_kernel) -----------
+// Accumulator columns of a tile: [16-unit block][slot z|r|n_x|n_h][16], slot registers as in epi_fwd.  n_x holds only
+// x_t W_h and n_h only h_{t-1} U_h (gpack_kernel zeroes the other half of their K range), so that
+//   z = sig(acc_z + b_z), r = sig(acc_r + b_r), n = tanh(acc_nx + b_nx + r (acc_nh + b_nh)), h_t = z h_{t-1} + (1 - z) n
+// with h_{t-1} the unmasked state carried in fp32 in cstate.  Forward-only: no gate state is saved.
+template <bool ACC>
+__device__ __forceinline__ void epi_gru_fwd(const EpiParams& p, const float (&acc)[128], Frag f, int rt, int by,
+                                            const float* bias_s) {
+  constexpr int U = 64;                             // hidden units of this tile
+  // The bias values and Philox quad indices of a thread do not change between the steps of a persistent launch.  Hoisted
+  // out of the step loop, they stay live next to the 128 accumulators and spill (about 0.9 KB of spill stores per thread
+  // at CUDA 12.9).  The empty asm statements make them opaque to the compiler, so they are re-read and recomputed per step.
+  const int unit0 = by * U, mm0 = f.m0;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = mm0 + 8 * h;
+    const long b = (long)rt * 128 + m;
+    const bool valid = b < p.B;
+#pragma unroll
+    for (int blk = 0; blk < U / 16; ++blk) {
+      const int gblk = (unit0 >> 4) + blk;
+      float* cs = p.cstate + ((((long)rt * p.NB16 + gblk) * 4 + (m >> 5)) * 32 + (m & 31)) * 16;
+      const float* bs = bias_s + blk * 64;
+      asm volatile("" : "+l"(bs));
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int jj = 8 * q + 2 * f.cq;
+        const int j = unit0 + blk * 16 + jj;
+        const float2 hprev = p.t > 0 ? *reinterpret_cast<const float2*>(cs + jj) : make_float2(0.f, 0.f);
+        float hv[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int ri = 32 * blk + 4 * q + 2 * h + e;
+          const float az = acc[ri] + bs[jj + e];
+          const float ar = acc[ri + 8] + bs[16 + jj + e];
+          const float anx = acc[ri + 16] + bs[32 + jj + e];
+          const float anh = acc[ri + 24] + bs[48 + jj + e];
+          float gz, gr, gn;
+          if (ACC) {
+            gz = sigmoid_acc(az); gr = sigmoid_acc(ar); gn = tanhf(fmaf(gr, anh, anx));
+          } else {      // z and r pre-scaled by 1/2 in the packed weights and bias, as the LSTM's sigmoid gates
+            gz = fmaf(0.5f, tanh_approx(az), 0.5f);
+            gr = fmaf(0.5f, tanh_approx(ar), 0.5f);
+            gn = tanh_approx(fmaf(gr, anh, anx));
+          }
+          hv[e] = fmaf(gz, (e ? hprev.y : hprev.x) - gn, gn);
+        }
+        *reinterpret_cast<float2*>(cs + jj) = make_float2(hv[0], hv[1]);
+        if (valid) {
+          const long hoff = ((long)(p.t + 1) * p.Bp + b) * p.H + j;
+          const uint32_t w = pack_bf16x2(hv[0], hv[1]);
+          st_b32(p.hseq + hoff, w);
+          if (ACC && p.hseq_lo) st_b32(p.hseq_lo + hoff, pack_bf16x2(hv[0] - bf16_lo(w), hv[1] - bf16_hi(w)));
+          if (p.hmseq) {
+            float mk[4];
+            uint64_t quad = (uint64_t)(p.row0 + b) * (uint64_t)(p.H / 4) + (uint64_t)(j / 4);    // rec_mask4
+            asm volatile("" : "+l"(quad));
+            dropout_quad(p.rkey, quad, mk);
+            const float hm0 = mk[j & 3] * hv[0], hm1 = mk[(j & 3) + 1] * hv[1];
+            const uint32_t wm = pack_bf16x2(hm0, hm1);
+            st_b32(p.hmseq + hoff, wm);
+            if (ACC && p.hmseq_lo) st_b32(p.hmseq_lo + hoff, pack_bf16x2(hm0 - bf16_lo(wm), hm1 - bf16_hi(wm)));
           }
         }
       }
@@ -390,6 +480,26 @@ __device__ __forceinline__ void epi_head(const EpiParams& p, const float (&acc)[
   if (m < GH_PART) p.hpartial[(long)m * gridDim.x + blockIdx.x] = red_s[m];
 }
 
+// ---- EPI_HEAD_UQ: the two heads of RNNUqRangeEstimate on the accumulator of y [Wo | Wv] (N = 32), forward only -------
+// pred = y Wo + bo, var = max(softplus(y Wv + bv), 1e-6) (rnn_uq_range_estimate.py:104-108, custom_layers.py:12-13).
+// Staged in shared memory like epi_head so that threads 0..127 own one row each and write its O outputs contiguously.
+__device__ __forceinline__ void epi_head_uq(const EpiParams& p, const float (&acc)[16], Frag f, float* rows_s) {
+  constexpr int LD = 2 * GH_O + 1;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) rows_s[(f.m0 + 8 * ((i >> 1) & 1)) * LD + 8 * (i >> 2) + 2 * f.cq + (i & 1)] = acc[i];
+  named_bar_sync(1, 256);
+  const int m = threadIdx.x;
+  if (m >= 128) return;
+  const int t = (int)blockIdx.x / p.NRT, rt = (int)blockIdx.x % p.NRT;
+  const long b = (long)rt * 128 + m;
+  if (b >= p.B) return;
+  const long r = b * p.T + t;          // row of the caller's [B][T][O] tensors
+  for (int k = 0; k < p.hO; ++k) {
+    p.hpreds[r * p.hO + k] = rows_s[m * LD + k] + __ldg(p.hbo + k);
+    p.hvar[r * p.hO + k] = fmaxf(softplus_f(rows_s[m * LD + GH_O + k] + __ldg(p.hbv + k)), 1e-6f);
+  }
+}
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GSmem<BN, EPI>::THREADS, GSmem<BN, EPI>::CTAS_PER_SM)
     tile_gemm_kernel(GArgs g, EpiParams ep, const __grid_constant__ CUtensorMap tmA0,
@@ -403,8 +513,8 @@ __global__ void __launch_bounds__(GSmem<BN, EPI>::THREADS, GSmem<BN, EPI>::CTAS_
   uint64_t* empty = full + S::NS;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   __shared__ float red_s[EPI == EPI_HEAD ? GH_PART : 1];
-  __shared__ float bias_s[(EPI == EPI_FWD || EPI == EPI_FWD_ACC) ? BN : 1];
-  if constexpr (EPI == EPI_FWD || EPI == EPI_FWD_ACC)
+  __shared__ float bias_s[epi_is_fwd(EPI) ? BN : 1];
+  if constexpr (epi_is_fwd(EPI))
     for (int i = tid; i < BN; i += S::THREADS) bias_s[i] = ep.bias[blockIdx.y * BN + i];    // weights: not the predecessor's
 
   int total_kb = 0;
@@ -509,9 +619,13 @@ __global__ void __launch_bounds__(GSmem<BN, EPI>::THREADS, GSmem<BN, EPI>::CTAS_
       if (total_kb > 0 && lane == 0) mbar_arrive(&empty[(it * total_kb + total_kb - 1) % S::NS]);
       if constexpr (EPI == EPI_HEAD) {
         epi_head(ep, acc, f, reinterpret_cast<float*>(smem + S::HEAD_ROWS), red_s);
+      } else if constexpr (EPI == EPI_HEAD_UQ) {
+        epi_head_uq(ep, acc, f, reinterpret_cast<float*>(smem + S::HEAD_ROWS));
       } else if ((long)rt * 128 < ep.Bp || EPI == EPI_STORE) {
         if constexpr (EPI == EPI_FWD) epi_fwd<false>(ep, acc, f, rt, by, bias_s);
         if constexpr (EPI == EPI_FWD_ACC) epi_fwd<true>(ep, acc, f, rt, by, bias_s);
+        if constexpr (EPI == EPI_GRU_FWD) epi_gru_fwd<false>(ep, acc, f, rt, by, bias_s);
+        if constexpr (EPI == EPI_GRU_FWD_ACC) epi_gru_fwd<true>(ep, acc, f, rt, by, bias_s);
         if constexpr (EPI == EPI_BWD) epi_bwd<BN>(ep, acc, f, rt, by);
         if constexpr (EPI == EPI_STORE) epi_store<BN>(ep, acc, f, (long)g.a_row_base + 128L * rt, by);
       }
@@ -586,8 +700,13 @@ __global__ void gcast_x_kernel(int B, int T, int F, int Bp, int Ipad, const floa
 //   Ub  [H][4H]   backward B operand = recurrent_kernel as it is (rec = dz U^T)
 //   Wb  [I][4H]   dLoss/d(input) B operand = kernel as it is (layers above the first)
 //   biasp [4H]    bias in Wf's row order, same pre-scale
+// GRU (forward only): the four gate slots of a 16-unit block are z | r | n_x | n_h (Keras blocks z | r | h of W, U [I|H][3H]
+// and bias [2][3H]).  n_x takes only W_h (zero rows for K < H) and n_h only U_h (zero rows for K >= H), so that the reset
+// gate can scale h_{t-1} U_h + b_rh alone; z and r take the pre-scale `hs`, their bias is the sum of both bias rows,
+// n_x takes b[0]_h and n_h b[1]_h.  The zero blocks cost (H + I) H of the (H + Ipad) 4H MACs; the GEMM keeps the LSTM's
+// shape.
 struct GPackArgs {
-  int H, I, Ipad, Kp;
+  int H, I, Ipad, Kp, gru;
   float hs, eps;
   const float *W, *U, *bias, *gamma, *beta, *mean, *var;
   __nv_bfloat16 *Wf, *Wf_lo, *Ub, *Wb;
@@ -602,11 +721,22 @@ __global__ void gpack_kernel(GPackArgs a) {
     const int k = (int)(idx % a.Kp);
     const int n = (int)(idx / a.Kp);
     const int tile = n / 256, blk = (n % 256) / 64, gate = (n % 64) / 16, jj = n % 16;
-    const int col = gate * H + tile * 64 + blk * 16 + jj;
-    const float sc = (gate == 2) ? 1.0f : a.hs;
+    const int u = tile * 64 + blk * 16 + jj;
     float v = 0.f;
-    if (k < H) v = sc * a.U[(long)k * 4 * H + col];
-    else if (k - H < a.I) v = sc * a.W[(long)(k - H) * 4 * H + col];
+    if (a.gru) {
+      const int col = (gate < 2 ? gate : 2) * H + u;
+      const float sc = (gate < 2) ? a.hs : 1.0f;
+      if (k < H) {
+        if (gate != 2) v = sc * a.U[(long)k * 3 * H + col];
+      } else if (k - H < a.I) {
+        if (gate != 3) v = sc * a.W[(long)(k - H) * 3 * H + col];
+      }
+    } else {
+      const int col = gate * H + u;
+      const float sc = (gate == 2) ? 1.0f : a.hs;
+      if (k < H) v = sc * a.U[(long)k * 4 * H + col];
+      else if (k - H < a.I) v = sc * a.W[(long)(k - H) * 4 * H + col];
+    }
     const __nv_bfloat16 hi = __float2bfloat16(v);
     a.Wf[idx] = hi;
     if (a.Wf_lo) a.Wf_lo[idx] = __float2bfloat16(v - __bfloat162float(hi));
@@ -616,7 +746,12 @@ __global__ void gpack_kernel(GPackArgs a) {
   if (idx < 4 * H) {
     const int n = (int)idx;
     const int tile = n / 256, blk = (n % 256) / 64, gate = (n % 64) / 16, jj = n % 16;
-    a.biasp[n] = ((gate == 2) ? 1.0f : a.hs) * a.bias[gate * H + tile * 64 + blk * 16 + jj];
+    const int u = tile * 64 + blk * 16 + jj;
+    if (a.gru)
+      a.biasp[n] = gate < 2 ? a.hs * (a.bias[gate * H + u] + a.bias[3 * H + gate * H + u])
+                            : a.bias[(gate == 2 ? 0 : 3 * H) + 2 * H + u];
+    else
+      a.biasp[n] = ((gate == 2) ? 1.0f : a.hs) * a.bias[gate * H + u];
   }
   if (idx < H) {
     const int j = (int)idx;
@@ -630,7 +765,8 @@ __global__ void gpack_kernel(GPackArgs a) {
 }
 
 // Head operands: WoT [16][H] (B operand of pred = y Wo: row = output k, K = hidden) and WoS [H][64] (B operand of
-// dy = dpred Wo^T: row = hidden unit, K = output k, zero beyond O).
+// dy = dpred Wo^T: row = hidden unit, K = output k, zero beyond O; null: not packed).  uq handles pack the variance
+// head's Wv into rows 16..31 of WoT with a second call.
 __global__ void gpack_head_kernel(int H, int O, const float* __restrict__ Wo, __nv_bfloat16* __restrict__ WoT,
                                   __nv_bfloat16* __restrict__ WoS) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -638,7 +774,7 @@ __global__ void gpack_head_kernel(int H, int O, const float* __restrict__ Wo, __
     const int k = idx / H, j = idx % H;
     WoT[idx] = __float2bfloat16(k < O ? Wo[j * O + k] : 0.f);
   }
-  if (idx < H * 64) {
+  if (WoS && idx < H * 64) {
     const int j = idx / 64, k = idx % 64;
     WoS[idx] = __float2bfloat16(k < O ? Wo[j * O + k] : 0.f);
   }
@@ -819,13 +955,15 @@ __global__ void __launch_bounds__(128) gcolsum_kernel(long rows, int N, long row
 // =============================================================================================
 // bf16x3 head on y = in[L] (bf16 [T][Bp][H] + low halves, BN / Dropout already applied): pred = y Wo + bo accumulated in
 // fp32.  bf16x3 handles are forward-only (gen_supported), so this head only predicts.  One thread per row of a 128-row
-// tile (TMA-staged, SW128), Wo broadcast from shared memory.  (rnn_point_estimate.py:105)
+// tile (TMA-staged, SW128), Wo broadcast from shared memory.  (rnn_point_estimate.py:105)  uq handles run it a second
+// time on the variance head (Wv, bv, softplus_floor = 1: var = max(softplus(y Wv + bv), 1e-6)).
 // =============================================================================================
 struct GHeadParams {
   int B, T, O, H, Bp, NRT;
   const float *Wo, *bo;
   float* preds;              // [B][T][O] fp32
   const __nv_bfloat16* yin_lo;   // low halves of the head input (row-major, same layout)
+  int softplus_floor;
 };
 __global__ void __launch_bounds__(128, 1) ghead_rows_kernel(GHeadParams p, const __grid_constant__ CUtensorMap tm_y) {
   extern __shared__ uint8_t smem_raw[];
@@ -888,7 +1026,7 @@ __global__ void __launch_bounds__(128, 1) ghead_rows_kernel(GHeadParams p, const
       }
     }
     if (p.preds && valid)
-      for (int k = 0; k < p.O; ++k) p.preds[r * p.O + k] = pr[k];
+      for (int k = 0; k < p.O; ++k) p.preds[r * p.O + k] = p.softplus_floor ? fmaxf(softplus_f(pr[k]), 1e-6f) : pr[k];
     __syncthreads();        // everyone is done with the tile before it is overwritten
   }
 }
@@ -927,10 +1065,10 @@ __global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial
 struct GenLayer {
   GenLayerOff off;
   int I, Ipad, Kp;
-  __nv_bfloat16 *hseq, *hseq_lo, *hmseq, *in, *in_lo, *gates, *cst;
+  __nv_bfloat16 *hseq, *hseq_lo, *hmseq, *hmseq_lo, *in, *in_lo, *gates, *cst;
   __nv_bfloat16 *Wf, *Wf_lo, *Ub, *Wb;
   float *biasp, *bn;
-  CUtensorMap tm_h, tm_h_lo, tm_hm, tm_in, tm_in_lo, tm_wf, tm_wf_lo, tm_ub, tm_wb;    // K-major (recurrence, dx)
+  CUtensorMap tm_h, tm_h_lo, tm_hm, tm_hm_lo, tm_in, tm_in_lo, tm_wf, tm_wf_lo, tm_ub, tm_wb;   // K-major (recurrence, dx)
   CUtensorMap tm_hA_mn, tm_in_mn;                                                       // MN-major (weight gradients)
 };
 
@@ -941,12 +1079,12 @@ struct GenImpl {
   cudaStream_t side = nullptr;          // second half of the batch in the backward recurrence (see gen_backward)
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   int maxB = 0, Bp = 0, NRT = 0, T = 0, F = 0, O = 0, H = 0, L = 0, NB16 = 0;
-  bool x3 = false, train_ws = false;
-  int64_t oWo = 0, obo = 0;
+  bool x3 = false, train_ws = false, gru = false, uq = false;
+  int64_t oWo = 0, obo = 0, oWv = -1, obv = -1;
   std::vector<GenLayer> layers;
   __nv_bfloat16 *head_in = nullptr, *head_in_lo = nullptr;      // in[L]
   CUtensorMap tm_head_in;
-  // tensor-core head (bf16): packed Wo, bf16 dLoss/dpred rows, per-tile loss partials
+  // tensor-core head (bf16): packed Wo (uq: [Wo | Wv], 32 rows), bf16 dLoss/dpred rows, per-tile loss partials
   __nv_bfloat16 *WoT = nullptr, *WoS = nullptr, *dpb = nullptr;
   float* head_tc_part = nullptr;
   CUtensorMap tm_wot, tm_wos, tm_dpb, tm_dpb_mn, tm_head_in_mn;
@@ -961,8 +1099,15 @@ struct GenImpl {
 };
 
 bool gen_supported(const lfmq_config& c, char* why, size_t n) {
-  if (c.rnn_cell != LFMQ_CELL_LSTM) { snprintf(why, n, "the tensor-core paths are built for the LSTM cell only"); return false; }
-  if (c.uq) { snprintf(why, n, "the tensor-core paths are built for the point-estimate head only"); return false; }
+  if (c.rnn_cell != LFMQ_CELL_LSTM && !c.forward_only) {
+    snprintf(why, n, "training on the tensor-core paths is built for the LSTM cell only (GRU handles must be forward_only)");
+    return false;
+  }
+  if (c.uq && !c.forward_only) {
+    snprintf(why, n,
+             "training on the tensor-core paths is built for the point-estimate head only (uq handles must be forward_only)");
+    return false;
+  }
   if (c.num_hidden % 64 != 0 || c.num_hidden > 512) {
     snprintf(why, n, "num_hidden must be a multiple of 64 and <= 512 (got %d)", c.num_hidden);
     return false;
@@ -976,7 +1121,12 @@ bool gen_supported(const lfmq_config& c, char* why, size_t n) {
   return true;
 }
 
-void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_t oWo, int64_t obo, Carver& cv) {
+// Dropout and recurrent dropout are active in training and, on uq handles, always (MC dropout: `training=True` is a
+// literal in rnn_uq_range_estimate.py:86,88), as on the fp32 path.
+static bool gen_stochastic(const lfmq_config& c) { return c.train || c.uq; }
+
+void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_t oWo, int64_t obo, int64_t oWv,
+                int64_t obv, Carver& cv) {
   if (!st.gen) st.gen = new GenImpl;
   GenImpl& m = *st.gen;
   m.maxB = c.max_batch; m.T = c.seq_len; m.F = c.n_inputs; m.O = c.n_outputs; m.H = c.num_hidden; m.L = c.num_layers;
@@ -985,10 +1135,12 @@ void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_
   m.NB16 = m.H / 16;
   m.x3 = c.precision == LFMQ_PREC_BF16X3;
   m.train_ws = !c.forward_only;
-  m.oWo = oWo; m.obo = obo;
+  m.gru = c.rnn_cell == LFMQ_CELL_GRU;
+  m.uq = c.uq != 0;
+  m.oWo = oWo; m.obo = obo; m.oWv = oWv; m.obv = obv;
   m.BNU = (m.H % 128 == 0) ? 128 : 64;
   const size_t T = m.T, Bp = m.Bp, H = m.H;
-  const bool rec = (c.train && c.recurrent_dropout > 0.f);
+  const bool rec = (gen_stochastic(c) && c.recurrent_dropout > 0.f);
   m.layers.assign(m.L, GenLayer{});
   for (int l = 0; l < m.L; ++l) {
     GenLayer& ly = m.layers[l];
@@ -999,6 +1151,7 @@ void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_
     ly.hseq = cv.take<__nv_bfloat16>((T + 1) * Bp * H);
     ly.hseq_lo = m.x3 ? cv.take<__nv_bfloat16>((T + 1) * Bp * H) : nullptr;
     ly.hmseq = rec ? cv.take<__nv_bfloat16>((T + 1) * Bp * H) : nullptr;
+    ly.hmseq_lo = (rec && m.x3) ? cv.take<__nv_bfloat16>((T + 1) * Bp * H) : nullptr;
     ly.in = cv.take<__nv_bfloat16>(T * Bp * ly.Ipad);
     ly.in_lo = m.x3 ? cv.take<__nv_bfloat16>(T * Bp * ly.Ipad) : nullptr;
     ly.Wf = cv.take<__nv_bfloat16>((size_t)4 * H * ly.Kp);
@@ -1016,7 +1169,7 @@ void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_
   }
   m.head_in = cv.take<__nv_bfloat16>(T * Bp * H);
   m.head_in_lo = m.x3 ? cv.take<__nv_bfloat16>(T * Bp * H) : nullptr;
-  m.WoT = cv.take<__nv_bfloat16>(16 * H);
+  m.WoT = cv.take<__nv_bfloat16>((m.uq ? 32 : 16) * H);
   m.WoS = cv.take<__nv_bfloat16>(H * 64);
   m.head_tc_part = cv.take<float>((size_t)GH_PART * T * m.NRT);
   m.dpb = m.train_ws ? cv.take<__nv_bfloat16>(T * Bp * 64) : nullptr;
@@ -1057,12 +1210,14 @@ int gen_init(TcState& st, const lfmq_config& c) {
     LFMQ_CUDA_CHECK(cudaMemset(ly.hseq, 0, (T + 1) * Bp * H * 2));
     if (ly.hseq_lo) LFMQ_CUDA_CHECK(cudaMemset(ly.hseq_lo, 0, (T + 1) * Bp * H * 2));
     if (ly.hmseq) LFMQ_CUDA_CHECK(cudaMemset(ly.hmseq, 0, (T + 1) * Bp * H * 2));
+    if (ly.hmseq_lo) LFMQ_CUDA_CHECK(cudaMemset(ly.hmseq_lo, 0, (T + 1) * Bp * H * 2));
     LFMQ_CUDA_CHECK(cudaMemset(ly.in, 0, T * Bp * ly.Ipad * 2));
     if (ly.in_lo) LFMQ_CUDA_CHECK(cudaMemset(ly.in_lo, 0, T * Bp * ly.Ipad * 2));
     const uint64_t hrows = (T + 1) * Bp;
     if ((rc = gmap_2d(&ly.tm_h, ly.hseq, H, hrows, 64, 128))) return rc;
     if (ly.hseq_lo && (rc = gmap_2d(&ly.tm_h_lo, ly.hseq_lo, H, hrows, 64, 128))) return rc;
     if (ly.hmseq && (rc = gmap_2d(&ly.tm_hm, ly.hmseq, H, hrows, 64, 128))) return rc;
+    if (ly.hmseq_lo && (rc = gmap_2d(&ly.tm_hm_lo, ly.hmseq_lo, H, hrows, 64, 128))) return rc;
     if ((rc = gmap_2d(&ly.tm_in, ly.in, ly.Ipad, T * Bp, 64, 128))) return rc;
     if (ly.in_lo && (rc = gmap_2d(&ly.tm_in_lo, ly.in_lo, ly.Ipad, T * Bp, 64, 128))) return rc;
     if ((rc = gmap_2d(&ly.tm_wf, ly.Wf, ly.Kp, 4 * H, 64, 256))) return rc;
@@ -1078,7 +1233,7 @@ int gen_init(TcState& st, const lfmq_config& c) {
   LFMQ_CUDA_CHECK(cudaMemset(m.head_in, 0, T * Bp * H * 2));
   if (m.head_in_lo) LFMQ_CUDA_CHECK(cudaMemset(m.head_in_lo, 0, T * Bp * H * 2));
   if ((rc = gmap_2d(&m.tm_head_in, m.head_in, H, T * Bp, 64, 128))) return rc;
-  if ((rc = gmap_2d(&m.tm_wot, m.WoT, H, 16, 64, 16))) return rc;
+  if ((rc = gmap_2d(&m.tm_wot, m.WoT, H, m.uq ? 32 : 16, 64, m.uq ? 32 : 16))) return rc;
   if (m.train_ws) {
     LFMQ_CUDA_CHECK(cudaMemset(m.dpb, 0, T * Bp * 64 * 2));       // columns >= 16 stay zero for good
     if ((rc = gmap_2d(&m.tm_wos, m.WoS, 64, H, 64, (H % 128 == 0) ? 128 : 64))) return rc;
@@ -1100,7 +1255,10 @@ int gen_init(TcState& st, const lfmq_config& c) {
   LFMQ_GEMM_ATTR(256, EPI_FWD_ACC);
   LFMQ_GEMM_ATTR(128, EPI_BWD);
   LFMQ_GEMM_ATTR(64, EPI_BWD);
+  LFMQ_GEMM_ATTR(256, EPI_GRU_FWD);
+  LFMQ_GEMM_ATTR(256, EPI_GRU_FWD_ACC);
   LFMQ_GEMM_ATTR(16, EPI_HEAD);
+  LFMQ_GEMM_ATTR(32, EPI_HEAD_UQ);
   LFMQ_GEMM_ATTR(128, EPI_STORE);
   LFMQ_GEMM_ATTR(64, EPI_STORE);
 #undef LFMQ_GEMM_ATTR
@@ -1155,7 +1313,7 @@ static int gen_pack(TcState& st, const float* params, float eps, cudaStream_t s)
   for (int l = 0; l < m.L; ++l) {
     GenLayer& ly = m.layers[l];
     GPackArgs a;
-    a.H = m.H; a.I = ly.I; a.Ipad = ly.Ipad; a.Kp = ly.Kp;
+    a.H = m.H; a.I = ly.I; a.Ipad = ly.Ipad; a.Kp = ly.Kp; a.gru = m.gru ? 1 : 0;
     a.hs = m.x3 ? 1.0f : 0.5f;
     a.eps = eps;
     a.W = params + ly.off.oW; a.U = params + ly.off.oU; a.bias = params + ly.off.ob;
@@ -1167,6 +1325,10 @@ static int gen_pack(TcState& st, const float* params, float eps, cudaStream_t s)
   }
   gpack_head_kernel<<<(int)cdivl((long)m.H * 64, 256), 256, 0, s>>>(m.H, m.O, params + m.oWo, m.WoT, m.WoS);
   LFMQ_LAUNCH_CHECK();
+  if (m.uq) {
+    gpack_head_kernel<<<(int)cdivl((long)m.H * 16, 256), 256, 0, s>>>(m.H, m.O, params + m.oWv, m.WoT + 16 * m.H, nullptr);
+    LFMQ_LAUNCH_CHECK();
+  }
   st.weights_dirty = 0;
   return 0;
 }
@@ -1177,8 +1339,8 @@ static int gen_run_trunk(TcState& st, const lfmq_config& c, const float* params,
   GenImpl& m = *st.gen;
   const int T = m.T, H = m.H, Bp = m.Bp;
   const int nrt = (B + 127) / 128;
-  const bool rec = c.train && c.recurrent_dropout > 0.f;
-  const bool drop = c.train && c.dropout > 0.f;
+  const bool rec = gen_stochastic(c) && c.recurrent_dropout > 0.f;
+  const bool drop = gen_stochastic(c) && c.dropout > 0.f;
   LFMQ_CUDA_CHECK(cudaMemsetAsync(m.gbar, 0, GBAR_N * sizeof(unsigned int), s));
   m.gbar_next = 0;
   {
@@ -1194,12 +1356,14 @@ static int gen_run_trunk(TcState& st, const lfmq_config& c, const float* params,
     ep.T = T; ep.B = B; ep.Bp = Bp; ep.H = H; ep.NRT = m.NRT; ep.NB16 = m.NB16; ep.row0 = row0;
     ep.bias = ly.biasp; ep.cstate = m.cstate; ep.hseq = ly.hseq; ep.hseq_lo = ly.hseq_lo;
     ep.hmseq = rec ? ly.hmseq : nullptr;
+    ep.hmseq_lo = rec ? ly.hmseq_lo : nullptr;
     ep.gates = save ? ly.gates : nullptr;
     ep.cst = save ? ly.cst : nullptr;
     ep.accurate = m.x3 ? 1 : 0;
     ep.use_rec = rec ? 1 : 0;
     ep.rkey = dropout_key(c.seed, 2 * l + 1, step, c.recurrent_dropout);
     const CUtensorMap& th = rec ? ly.tm_hm : ly.tm_h;
+    const CUtensorMap& th_lo = rec ? ly.tm_hm_lo : ly.tm_h_lo;     // bf16x3
     // steps 1 .. T-1 as ONE persistent launch when all its CTAs fit on the machine at once (see GArgs::n_steps)
     const long fwd_ctas = (long)nrt * (4 * H / 256);
     const bool persist = gen_can_persist(m, fwd_ctas, 1, GSmem<256, EPI_FWD>::CTAS_PER_SM, T - 1);
@@ -1230,9 +1394,13 @@ static int gen_run_trunk(TcState& st, const lfmq_config& c, const float* params,
       // Steps after the first of a layer follow another step kernel: PDL.
       int rc;
 #define LFMQ_FWD_LAUNCH(EPI_)                                                                                     \
-  rc = launch_tile_gemm<256, EPI_>(dim3(nrt, 4 * H / 256), s, t > 0, g, ep, th, ly.tm_in, m.x3 ? ly.tm_h_lo : th,  \
+  rc = launch_tile_gemm<256, EPI_>(dim3(nrt, 4 * H / 256), s, t > 0, g, ep, th, ly.tm_in, m.x3 ? th_lo : th,  \
                                    m.x3 ? ly.tm_in_lo : ly.tm_in, ly.tm_wf, m.x3 ? ly.tm_wf_lo : ly.tm_wf)
-      if (m.x3)
+      if (m.gru && m.x3)
+        LFMQ_FWD_LAUNCH(EPI_GRU_FWD_ACC);
+      else if (m.gru)
+        LFMQ_FWD_LAUNCH(EPI_GRU_FWD);
+      else if (m.x3)
         LFMQ_FWD_LAUNCH(EPI_FWD_ACC);
       else
         LFMQ_FWD_LAUNCH(EPI_FWD);
@@ -1346,6 +1514,54 @@ int gen_forward(TcState& st, const lfmq_config& c, const float* params, const fl
   st.prof->end(LFMQ_REGION_FWD, s);
   st.prof->begin(LFMQ_REGION_HEAD, s);
   if ((rc = gen_run_head(st, c, params, nullptr, nullptr, B, nullptr, preds, nullptr, false, s))) return rc;
+  st.prof->end(LFMQ_REGION_HEAD, s);
+  return 0;
+}
+
+// The two heads of a uq handle on y = in[L]: bf16, one N = 32 GEMM over [Wo | Wv]; bf16x3, the fp32-accumulating SIMT
+// head once per head.
+static int gen_run_head_uq(GenImpl& m, const float* params, int B, float* preds, float* var, cudaStream_t s) {
+  if (m.x3) {
+    GHeadParams h = {};
+    h.B = B; h.T = m.T; h.O = m.O; h.H = m.H; h.Bp = m.Bp; h.NRT = (B + 127) / 128;
+    h.yin_lo = m.head_in_lo;
+    int grid = m.T * h.NRT;
+    if (grid > m.head_ctas) grid = m.head_ctas;
+    const int hsmem = (m.H / 64) * 16384 + m.H * GH_O * 4 + 64 + 1024;
+    for (int v = 0; v < 2; ++v) {
+      h.Wo = params + (v ? m.oWv : m.oWo);
+      h.bo = params + (v ? m.obv : m.obo);
+      h.preds = v ? var : preds;
+      h.softplus_floor = v;
+      ghead_rows_kernel<<<grid, 128, hsmem, s>>>(h, m.tm_head_in);
+      LFMQ_LAUNCH_CHECK();
+    }
+    return 0;
+  }
+  EpiParams ep = {};
+  ep.T = m.T; ep.B = B; ep.Bp = m.Bp; ep.H = m.H; ep.NRT = m.NRT; ep.NB16 = m.NB16;
+  ep.hbo = params + m.obo; ep.hpreds = preds; ep.hO = m.O;
+  ep.hbv = params + m.obv; ep.hvar = var;
+  GArgs g = {};
+  g.n_seg = 1;
+  g.seg[0] = GSeg{0, 0, m.H / 64, 0, 0};
+  return launch_tile_gemm<32, EPI_HEAD_UQ>(dim3(m.T * m.NRT, 1), s, false, g, ep, m.tm_head_in, m.tm_head_in,
+                                           m.tm_head_in, m.tm_head_in, m.tm_wot, m.tm_wot);
+}
+
+int gen_forward_uq(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
+                   int64_t step, float* preds, float* var, cudaStream_t s) {
+  if (!st.gen || !st.gen->enabled || !st.gen->uq) {
+    LFMQ_SET_ERR("general tensor-core path not initialised for a uq handle");
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  int rc;
+  if ((rc = gen_pack(st, params, c.bn_epsilon, s))) return rc;
+  st.prof->begin(LFMQ_REGION_FWD, s);
+  if ((rc = gen_run_trunk(st, c, params, x, B, row0, step, false, s))) return rc;
+  st.prof->end(LFMQ_REGION_FWD, s);
+  st.prof->begin(LFMQ_REGION_HEAD, s);
+  if ((rc = gen_run_head_uq(*st.gen, params, B, preds, var, s))) return rc;
   st.prof->end(LFMQ_REGION_HEAD, s);
   return 0;
 }
