@@ -6,9 +6,11 @@
 //   xh    bf16 [maxB][T+1][384]   row (b,t): cols 0..255 = h_{t-1} (zero at t=0), 256..287 = x_t, 288 = 1.0 (t<T),
 //                                 rest 0.  One buffer serves: the A operand of the forward recurrence (K-major
 //                                 tiles via TMA), the head (h_t = row t+1) and the weight-gradient GEMM (MN-major).
-//   gates bf16 [T][tiles][8 blocks of 32 units][4 row quadrants][8 pieces = gate*2+half][32 rows][16]   post-activation
-//                                 i|f|g|o saved for BPTT, SoA at 32-byte granularity (row-major within a piece)
-//   cst   bf16 [T][tiles][8][4][2 pieces][32][16]   cell states (the recurrence itself keeps them in fp32 registers)
+//   gates bf16 [T][tiles][4 ranks][4 chunks][128 rows][2 q][4 cq][4 gates][2 e]   post-activation i|f|g|o saved for
+//                                 BPTT, in accumulator-fragment order: unit 64 rank + 16 chunk + 8 q + 2 cq + e, so the
+//                                 thread (row, cq) that holds a pair q in both recurrences owns one 16-byte vector
+//   cst   bf16 [T][tiles][4 ranks][4 chunks][128 rows][4 cq][2 q][2 e]   cell states, same order, one 8-byte vector per
+//                                 thread and row (the recurrence itself keeps them in fp32 registers)
 //   dz    bf16 [maxB][T+1][4H]    gate pre-activation gradients (row T stays zero); columns in the order the
 //                                 backward kernel stages them as its A operand, [16-unit block][gate][16], so that a
 //                                 chunk goes out with one TMA store; only the weight-gradient GEMM reads it
@@ -264,6 +266,13 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
     uint32_t n_xf = 0, n_hf = 0;
     float acc[NG][64];                      // [half g0 + g]: chunks 2 g (registers 0-31) and 2 g + 1 (32-63)
     float cstate[2 * NG][2][2][2];          // [chunk cc][row half h][pair p][e]
+    // SAVE: the cell update leaves the post-activation gates for the saved state in the accumulator registers they came
+    // from, which are dead until the next step's first MMA (scale-d 0).  Except for chunks 0-1 of a 128-row tile: they
+    // are updated while the MMAs of chunks 2-3 are in flight, and writing accumulator registers then makes ptxas
+    // serialise every wgmma of the kernel (C7515), so their gates are packed into bf16x2 words and stored right after
+    // their update (holding those 32 words across the publish instead spills).
+    uint32_t held[2][2][2][4];              // [chunk cc][row half h][pair q][gate]
+    auto held_chunk = [](int cc) { return NG == 2 && cc < 2; };
     for (int it = 0; it < p.n_iters; ++it) {
       if (it * p.n_clusters + cid >= p.n_units) break;
       const int b0 = (p.unit0 + it * p.n_clusters + cid) * ROWS;          // first row of the unit
@@ -275,6 +284,31 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
 #pragma unroll
           for (int q = 0; q < 2; ++q) cstate[c][h][q][0] = cstate[c][h][q][1] = 0.f;
       for (int t = 0; t < T; ++t) {
+        // Saved state of chunk cc (post-activation gates as the cell update left them, cell states c_t), in fragment
+        // order (see tc_layout): per row half, two 16-byte gate vectors and one 8-byte cell-state vector, the 4 lanes
+        // of a row covering 64 and 32 contiguous bytes.
+        auto save_chunk = [&](int cc) {
+          const int c = 2 * g0 + cc;
+          const float* ac = acc[cc >> 1] + 32 * (cc & 1);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int m = mo + r0 + 8 * h;          // row of the 128-row tile
+            if ((long)tile * 128 + m >= p.B) continue;
+            const long row = ((((long)t * p.n_tiles_cap + tile) * TC_NC + rank) * 4 + c) * 128 + m;
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+              const int ri = 4 * q + 2 * h;         // register of gate 0, e = 0; gate g is 8 g further
+              st_global_v4(p.gates + row * 64 + 32 * q + 8 * cq,
+                           held_chunk(cc) ? make_uint4(held[cc & 1][h][q][0], held[cc & 1][h][q][1],
+                                                       held[cc & 1][h][q][2], held[cc & 1][h][q][3])
+                                          : make_uint4(pack_bf16x2(ac[ri], ac[ri + 1]), pack_bf16x2(ac[ri + 8], ac[ri + 9]),
+                                                       pack_bf16x2(ac[ri + 16], ac[ri + 17]),
+                                                       pack_bf16x2(ac[ri + 24], ac[ri + 25])));
+            }
+            st_global_v2(p.cst + row * 16 + 4 * cq, make_uint2(pack_bf16x2(cstate[cc][h][0][0], cstate[cc][h][0][1]),
+                                                              pack_bf16x2(cstate[cc][h][1][0], cstate[cc][h][1][1])));
+          }
+        };
         // Two 128-column halves (chunks 2 g, 2 g + 1: an m64n128 fragment is the two m64n64 fragments side by side), each
         // its own commit group for the h part: the cell update of chunks 0-1 overlaps the MMAs of chunks 2-3.  Against
         // one group per 64-column chunk, each k-step re-reads the h tile's A operand from shared memory half as often.
@@ -319,7 +353,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
           if (cc == 2) wgmma_wait<0>();
           if ((cc & 1) == 0) fence_regs(acc[cc >> 1]);
           const int c = 2 * g0 + cc;                // 64-column chunk of the CTA's slice
-          const float* ac = acc[cc >> 1] + 32 * (cc & 1);
+          float* ac = acc[cc >> 1] + 32 * (cc & 1);
           const float* bs = bias_s + c * 64;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -334,12 +368,21 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
                 const float cs = fmaf(gv[1][e], cstate[cc][h][q][e], gv[0][e] * gv[2][e]);
                 cstate[cc][h][q][e] = cs;
                 hv[e] = gv[3][e] * tanh_approx(cs);
+                if (SAVE && !held_chunk(cc))
+#pragma unroll
+                  for (int g = 0; g < 4; ++g) ac[4 * (2 * g + q) + 2 * h + e] = gv[g][e];
               }
+              if (SAVE && held_chunk(cc))
+#pragma unroll
+                for (int g = 0; g < 4; ++g) held[cc & 1][h][q][g] = pack_bf16x2(gv[g][0], gv[g][1]);
               if (b < p.B)
                 *reinterpret_cast<uint32_t*>(p.xh + (b * (T + 1) + (t + 1)) * TC_XH_LD + rank * TC_HS + c * 16 + jj) =
                     pack_bf16x2(hv[0], hv[1]);
             }
           }
+          // Chunks 0-1 of a 128-row tile go out here, under the MMAs of chunks 2-3 (DESIGN.md section 5a measures
+          // this against storing them after the publish).
+          if (SAVE && held_chunk(cc)) save_chunk(cc);
         }
         // Publish this CTA's h slice: barrier over the 256 consumer threads, then 4 lanes of warp 0 arrive
         // (release.cluster, cumulative over the barrier) on the 4 CTAs' h_written barriers in parallel.  Readers acquire
@@ -348,34 +391,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
         named_bar_sync(1, 256);
         if (warp == 0 && lane < TC_NC) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->h_written), (uint32_t)lane));
         if (SAVE) {
-          // Saved gates / cell states are not needed by the h exchange: they go out after the publish, so that the
-          // release above does not wait for them.  The gates are evaluated again from the accumulators (still intact
-          // until the next step's MMAs) -- cheaper than holding 80 packed values per thread across the publish.
+          // The other chunks' saved state is not needed by the h exchange: it goes out after the publish, so that the
+          // release above does not wait for it.
 #pragma unroll
-          for (int cc = 0; cc < 2 * NG; ++cc) {
-            const int c = 2 * g0 + cc;
-            const float* bs = bias_s + c * 64;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int m = mo + r0 + 8 * h;        // row of the 128-row tile
-              if ((long)tile * 128 + m >= p.B) continue;
-              // saved state, SoA at 32-byte granularity: [(t, tile, 32-unit block fr, row quadrant)][piece = gate*2 +
-              // h16][row & 31][16], unit = 32 fr + 16 h16 + e; this chunk is fr = 2 rank + c / 2, h16 = c % 2
-              const long blk = (((long)t * p.n_tiles_cap + tile) * 8 + 2 * (int)rank + (c >> 1)) * 4 + (m >> 5);
-#pragma unroll
-              for (int q = 0; q < 2; ++q) {
-                const int jj = 8 * q + 2 * cq;
-                float gv[4][2];
-                fwd_gates(acc[cc >> 1] + 32 * (cc & 1), bs, h, q, jj, gv);
-                __nv_bfloat16* gp = p.gates + (blk * 8 + (c & 1)) * 512 + (m & 31) * 16 + jj;
-#pragma unroll
-                for (int g = 0; g < 4; ++g)
-                  *reinterpret_cast<uint32_t*>(gp + g * 1024) = pack_bf16x2(gv[g][0], gv[g][1]);
-                *reinterpret_cast<uint32_t*>(p.cst + (blk * 2 + (c & 1)) * 512 + (m & 31) * 16 + jj) =
-                    pack_bf16x2(cstate[cc][h][q][0], cstate[cc][h][q][1]);
-              }
-            }
-          }
+          for (int cc = 0; cc < 2 * NG; ++cc)
+            if (!held_chunk(cc)) save_chunk(cc);
         }
       }
     }
@@ -1227,7 +1247,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
     // covering 512 contiguous bytes; it is read back as two 8-byte halves, one per row half h (three live 16-byte
     // vectors would spill).
     const uint32_t recv_off = SB_R + tid * 16;
-    const long tstride = (long)p.n_tiles_cap * 8 * 4 * 2 * 32 * 16;   // cst elements per time step
+    const long tstride = (long)p.n_tiles_cap * 128 * TC_H;            // cst elements per time step
     float acc[128];
     // dLoss/dh (recurrent + head part) of the own slice for the current step: chunk 0's eight values are read straight
     // from acc[0..7] (nothing overwrites them before chunk 0's MMAs), chunks 1-3 are copied out, rown[i] = acc[8 + i]
@@ -1278,11 +1298,11 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
       for (int t = T - 1; t >= 0; --t) {
         const bool has_rec = t < T - 1;
         // This thread's first element of the step's saved state and head dLoss/dh (row r0, units 2 cq, 2 cq + 1 of
-        // chunk 0).  Rows r0 and r0 + 8 lie in the same 32-row quadrant, so every (chunk, h, q, gate) operand is a
-        // constant offset from these three pointers: no per-operand address arithmetic is live across the chunk loop.
-        const long sblk = (((long)t * p.n_tiles_cap + tile) * 8 + 2 * rank) * 4 + (mq >> 5);
-        const __nv_bfloat16* gbase = p.gates + sblk * 4096 + (mq & 31) * 16 + 2 * cq;
-        const __nv_bfloat16* cbase = p.cst + sblk * 1024 + (mq & 31) * 16 + 2 * cq;
+        // chunk 0).  Every (chunk, h, q) operand is a constant offset from these three pointers (for dhout because rows
+        // r0 and r0 + 8 lie in the same 32-row quadrant): no per-operand address arithmetic is live across the chunk loop.
+        const long srow = (((long)t * p.n_tiles_cap + tile) * BWD_NC + rank) * 4 * 128 + mq;   // saved-state row, chunk 0
+        const __nv_bfloat16* gbase = p.gates + srow * 64 + 8 * cq;
+        const __nv_bfloat16* cbase = p.cst + srow * 16 + 4 * cq;
         const __nv_bfloat16* dbase =
             p.dhout + ((((long)t * p.n_tiles_cap + tile) * 4 + rank) * 4 + (mq >> 5)) * 2048 + (mq & 31) * 16 + 2 * cq;
         // Saved-state operands of one chunk, all requested before the first is used: one memory latency per chunk.
@@ -1293,21 +1313,25 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const bool valid = (long)b0 + r0 + 8 * h < p.B;
+            const int so = 128 * jb + 8 * h;          // saved-state rows from srow
+            if (valid) {
+              // gate vector q holds i|f|g|o of pair q, cell-state word q pair q: the order the forward stores them in
+              const uint2 c = *reinterpret_cast<const uint2*>(cbase + so * 16);
+              const uint2 cprev = t > 0 ? *reinterpret_cast<const uint2*>(cbase + so * 16 - tstride) : make_uint2(0u, 0u);
 #pragma unroll
-            for (int q = 0; q < 2; ++q) {
-              if (valid) {
-                const int so = (jb >> 1) * 4 * 4096 + (jb & 1) * 512 + 128 * h + 8 * q;   // gates; cst: the same / 4
-                const int co = (jb >> 1) * 4 * 1024 + (jb & 1) * 512 + 128 * h + 8 * q;
-                gi[h][q] = ld_b32(gbase + so);
-                gf[h][q] = ld_b32(gbase + so + 1024);
-                gg[h][q] = ld_b32(gbase + so + 2048);
-                go[h][q] = ld_b32(gbase + so + 3072);
-                ct[h][q] = ld_b32(cbase + co);
-                cp[h][q] = t > 0 ? ld_b32(cbase + co - tstride) : 0u;
+              for (int q = 0; q < 2; ++q) {
+                const uint4 v = *reinterpret_cast<const uint4*>(gbase + so * 64 + 32 * q);
+                gi[h][q] = v.x;
+                gf[h][q] = v.y;
+                gg[h][q] = v.z;
+                go[h][q] = v.w;
+                ct[h][q] = q ? c.y : c.x;
+                cp[h][q] = q ? cprev.y : cprev.x;
                 dhp[h][q] = FUSED ? 0u : ld_b32(dbase + jb * 512 + 128 * h + 8 * q);
-              } else {
-                gi[h][q] = gf[h][q] = gg[h][q] = go[h][q] = ct[h][q] = cp[h][q] = dhp[h][q] = 0u;
               }
+            } else {
+#pragma unroll
+              for (int q = 0; q < 2; ++q) gi[h][q] = gf[h][q] = gg[h][q] = go[h][q] = ct[h][q] = cp[h][q] = dhp[h][q] = 0u;
             }
           }
         };
@@ -1497,7 +1521,10 @@ void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& 
   m.head_part_elems = (size_t)m.head_ctas * HEAD_PART;
   m.head_part = cv.take<float>(m.head_part_elems);
   if (m.train) {
-    const size_t Bt = (B + 127) / 128 * 128;      // saved state is blocked by 128-row tiles
+    // Saved state is blocked by 128-row tiles; both recurrences move it in 16- and 8-byte vectors, which the carver's
+    // 1024-byte alignment of every buffer keeps aligned.
+    static_assert(WS_ALIGN % 16 == 0, "gates / cst are accessed as 16-byte vectors");
+    const size_t Bt = (B + 127) / 128 * 128;
     m.gates = cv.take<__nv_bfloat16>(Bt * T * 4 * H);
     m.cst = cv.take<__nv_bfloat16>(Bt * T * H);
     m.dz = cv.take<__nv_bfloat16>(B * (T + 1) * 4 * H);

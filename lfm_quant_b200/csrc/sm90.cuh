@@ -251,6 +251,14 @@ __device__ __forceinline__ void st_global_v8(void* p, const uint32_t v[8]) {
   q[1] = make_uint4(v[4], v[5], v[6], v[7]);
 }
 
+// ---- 16- and 8-byte global stores that stay vectors (a uint4 / uint2 assignment may be split into 32-bit stores) ----
+__device__ __forceinline__ void st_global_v4(void* p, uint4 v) {
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ void st_global_v2(void* p, uint2 v) {
+  asm volatile("st.global.v2.b32 [%0], {%1, %2};" ::"l"(p), "r"(v.x), "r"(v.y) : "memory");
+}
+
 // ---- math ---------------------------------------------------------------------------------------
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
