@@ -13,7 +13,7 @@ import pytest
 import torch
 
 import lfm_oracle as orc
-from util import make_engine, make_problem, rel_err
+from util import make_engine, make_problem, make_uq_problem, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -60,18 +60,6 @@ def test_gru_bf16x3_long_sequence_meets_the_fp32_tolerance():
     eng.close()
 
 
-def _uq_problem(B, T, F, O, H, L, seed, cell):
-    rng = np.random.RandomState(seed)
-    params = orc.init_params(L, F, O, H, init_scale=0.5, seed=seed + 1, dtype=np.float64, rnn_cell=cell, uq=True)
-    for l in range(L):
-        params[5 * l + 2] = params[5 * l + 2] + rng.normal(size=params[5 * l + 2].shape) * 0.1
-    params[-1] = rng.normal(size=O) * 0.5
-    params[-3] = rng.normal(size=O) * 0.5
-    params = [p.astype(np.float32).astype(np.float64) for p in params]
-    x = rng.normal(size=(B, T, F)).astype(np.float32)
-    return params, x
-
-
 UQ_KW = dict(dropout=0.2, recurrent_dropout=0.1, seed=521)
 
 
@@ -80,7 +68,7 @@ UQ_KW = dict(dropout=0.2, recurrent_dropout=0.1, seed=521)
                                         ((150, 6, 33, 5, 64, 1), 'gru'), ((130, 4, 32, 16, 256, 2), 'gru')])
 def test_uq_forward_only_matches_oracle_with_mc_dropout(shape, cell, precision):
     B, T, F, O, H, L = shape
-    params, x = _uq_problem(B, T, F, O, H, L, seed=13, cell=cell)
+    params, x = make_uq_problem(B, T, F, O, H, L, seed=13, cell=cell)
     eng = make_engine(B, T, F, O, H, L, target_idx=O - 1, uq=True, rnn_cell=cell, train=False, forward_only=True,
                       precision=precision, **UQ_KW)
     eng.set_weights(params)
@@ -106,7 +94,7 @@ def test_uq_bf16x3_draws_the_masks_of_the_fp32_path(cell):
     """bf16x3 and fp32 handles agree to the fp32 tolerance at the same (step, row0): the Dropout and recurrent-dropout
     masks are the same sample on both paths."""
     B, T, F, O, H, L = 160, 8, 32, 16, 128, 2
-    params, x = _uq_problem(B, T, F, O, H, L, seed=17, cell=cell)
+    params, x = make_uq_problem(B, T, F, O, H, L, seed=17, cell=cell)
     outs = {}
     for precision in ('fp32', 'bf16x3'):
         eng = make_engine(B, T, F, O, H, L, target_idx=1, uq=True, rnn_cell=cell, train=False, forward_only=True,

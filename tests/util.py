@@ -21,10 +21,29 @@ def make_problem(B, T, F, O, H, L, seed=0, zero_rows=True, init_scale=0.5, rnn_c
     return params, x, y
 
 
+def make_uq_problem(B, T, F, O, H, L, seed, cell):
+    """Weights of RNNUqRangeEstimate (target and variance heads) and inputs."""
+    rng = np.random.RandomState(seed)
+    params = orc.init_params(L, F, O, H, init_scale=0.5, seed=seed + 1, dtype=np.float64, rnn_cell=cell, uq=True)
+    for l in range(L):
+        params[5 * l + 2] = params[5 * l + 2] + rng.normal(size=params[5 * l + 2].shape) * 0.1
+    params[-1] = rng.normal(size=O) * 0.5
+    params[-3] = rng.normal(size=O) * 0.5
+    params = [p.astype(np.float32).astype(np.float64) for p in params]
+    x = rng.normal(size=(B, T, F)).astype(np.float32)
+    return params, x
+
+
 def rel_err(a, b):
     a = np.asarray(a, dtype=np.float64)
     b = np.asarray(b, dtype=np.float64)
     return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-30))
+
+
+def cosine(a, b):
+    a = np.asarray(a, dtype=np.float64).ravel()
+    b = np.asarray(b, dtype=np.float64).ravel()
+    return float(np.dot(a, b) / (np.linalg.norm(a) * np.linalg.norm(b) + 1e-30))
 
 
 def make_engine(B, T, F, O, H, L, **kw):
