@@ -158,16 +158,31 @@ int32_t lfmq_train_step(lfmq_handle h, const float* x, const float* y, int32_t B
  * `stages`, `preds`, `y` are host arrays of n_stages (<= 8) entries; `weights` = config.forecast_steps_weights (host).
  * `work`: device floats, n_stages * B * seq_len * n_inputs (stage inputs + one input-gradient buffer).
  * Dropout streams of stage s continue the trunk's layer numbering (layer num_layers + s - 1).
- * Training-mode stages (cfg.train) run on the LFMQ_PREC_FP32 kernels; forward_only stages may use any precision. */
+ * Training-mode stages (cfg.train) run on the LFMQ_PREC_FP32 kernels; forward_only stages may use any precision.
+ * Every stage of one chain has the same cfg.uq.  A uq chain (models/uq_range_estimate/rnn_uq_range_estimate.py:114-157)
+ * gives every stage the heads OUTPUT_TARGET_{s+1} and OUTPUT_VARIANCE_{s+1}, keeps Dropout / recurrent dropout on in
+ * every stage and builds each next window from the previous stage's TARGET predictions (variances never feed forward).
+ * It runs lfmq_chain_forward_uq and lfmq_chain_loss_uq; lfmq_chain_backward and lfmq_chain_apply serve both kinds. */
 /* model(inp) -> [pred_1 .. pred_S], each [B,T,O] (train.py:182, predict.py:129) */
 int32_t lfmq_chain_forward(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
                            int64_t step, float* const* preds, float* work, void* stream);
 /* Losses.weight_adjusted_mse(y_true list, y_pred list) (losses.py:19-53): out_dev = {sum_s w_s loss_s, sum_s w_s mse_s} */
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,
                         const float* weights, int32_t B, float* out_dev, void* stream);
+/* uq chain: model(inp) -> [tar_1, var_1, .., tar_S, var_S] (train.py:204-206, predict.py:135-138): preds[s] and vars[s],
+ * each [B,T,O], Dropout masks drawn for (step, row0) on every call */
+int32_t lfmq_chain_forward_uq(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
+                              int64_t step, float* const* preds, float* const* vars, float* work, void* stream);
+/* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
+ * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
+ * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */
+int32_t lfmq_chain_loss_uq(const lfmq_handle* stages, int32_t n_stages, const float* const* preds,
+                           const float* const* vars, const float* const* y, const float* weights, int32_t B,
+                           float* out_dev, void* stream);
 /* forward of all stages, the weighted loss, and BPTT through the whole graph: the input gradient of stage s flows into
  * the last time step of the earlier predictions it was built from.  Fills every stage's gradient buffer;
- * loss_out_dev (nullable) = {loss, mse} as lfmq_chain_loss. */
+ * loss_out_dev (nullable) = {loss, mse} as lfmq_chain_loss; on a uq chain (3 floats) {uq_loss, uq_loss_last_tar, mse}
+ * as lfmq_chain_loss_uq, the gradient of sum_s w_s uq_loss_s (train.py:201-218). */
 int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
                             const float* weights, int32_t B, int64_t row0, int64_t step, float* work,
                             float* loss_out_dev, void* stream);

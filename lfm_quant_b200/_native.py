@@ -70,7 +70,9 @@ SYMBOLS = {
     'lfmq_apply': (C.c_int32, [_P, C.c_float, C.c_int64, _P]),
     'lfmq_train_step': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int64, C.c_int64, C.c_float, _P, _P]),
     'lfmq_chain_forward': (C.c_int32, [_P, C.c_int32, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),
+    'lfmq_chain_forward_uq': (C.c_int32, [_P, C.c_int32, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P, _P]),
     'lfmq_chain_loss': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P]),
+    'lfmq_chain_loss_uq': (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_backward': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),
     'lfmq_chain_apply': (C.c_int32, [_P, C.c_int32, C.c_float, C.c_int64, _P]),
     'lfmq_window_index': (C.c_int32, [C.POINTER(LfmqWindowIndexArgs), _P]),

@@ -56,6 +56,17 @@ int scale_inplace(cudaStream_t s, long n, float* p, float w);
 int chain_scatter_dx(cudaStream_t s, int B, int T, int F, int O, int stage, const float* dx, const ChainPtrs& dpred);
 int chain_combine(cudaStream_t s, int S, const ChainPtrs& scalars, float clip, const ChainPtrs& loss2,
                   const ChainWeights& w, float* out2);
+// forecast_steps > 1 of RNNUqRangeEstimate: every stage's uq loss rows in one launch, then one reduction launch.
+// pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and
+// out3 (nullable) = the weighted sums {uq_loss, uq_loss_last_tar, mse}; counts_in = 1 takes the counts from counts.p[s]
+// (required with dpred), else the pass counts its own rows.  dpred / da (nullable) = w_s * dLoss_s / d(pred, apre).
+struct ChainUqArgs {
+  ChainPtrs pred, var, apre, y, dpred, da, counts, loss, uq0, mse0;
+  ChainWeights w;
+  int counts_in;
+};
+int chain_uq_loss_grad(cudaStream_t s, int S, int B, int T, int O, const ChainUqArgs& a, int target_idx, float p1,
+                       float p2, float* out3, float* scratch);
 
 struct GatherArgs {
   int n_rows, n_cols, B, T, F, O, stride, seq_norm_col, log_squasher, aux_masking;

@@ -797,14 +797,12 @@ int softplus_floor(cudaStream_t s, long n, const float* a, float* var) {
 // log(vm) in fp32 exactly as written there -- a masked row gives 0*inf + log 0 = NaN, as in the reference; sums are
 // carried in fp64.  pred == nullptr: only the two mask counts.  dpred != nullptr: gradients w.r.t. pred and w.r.t. the
 // variance head's pre-activation `apre` (tf.maximum passes the gradient to softplus above the floor), using the counts
-// of a previous pass.
-__global__ void __launch_bounds__(256) uq_loss_rows_kernel(int B, int T, int O, const float* __restrict__ pred,
-                                                           const float* __restrict__ var,
-                                                           const float* __restrict__ apre,
-                                                           const float* __restrict__ y,
-                                                           const float* __restrict__ counts, int target_idx, float p1,
-                                                           float p2, float* __restrict__ dpred,
-                                                           float* __restrict__ da, double* __restrict__ partial) {
+// of a previous pass, both multiplied by the forecast step's weight w (exactly 1 for forecast_steps = 1).
+__device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* __restrict__ pred,
+                                             const float* __restrict__ var, const float* __restrict__ apre,
+                                             const float* __restrict__ y, const float* __restrict__ counts,
+                                             int target_idx, float p1, float p2, float w, float* __restrict__ dpred,
+                                             float* __restrict__ da, double* __restrict__ partial) {
   double acc[4] = {0, 0, 0, 0};   // uq_0, uq_1, uq_2 numerators, mse_0 numerator
   double cnt[4] = {0, 0, 0, 0};   // unmasked rows, unmasked last-step rows
   float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
@@ -837,38 +835,102 @@ __global__ void __launch_bounds__(256) uq_loss_rows_kernel(int B, int T, int O, 
         if (k == target_idx) { acc[0] += term; acc[3] += diff; coef += c_tar; }
       }
       if (dpred) {
-        dpred[r * O + k] = coef * (2.f * d / vm) * m;
+        dpred[r * O + k] = coef * (2.f * d / vm) * m * w;
         const float dv = coef * (-diff / (vm * vm) + 1.f / vm) * m;
         const float a = apre[r * O + k];
-        da[r * O + k] = dv * ((softplus_f(a) > 1e-6f) ? sigmoid_f(a) : 0.f);
+        da[r * O + k] = dv * ((softplus_f(a) > 1e-6f) ? sigmoid_f(a) : 0.f) * w;
       }
     }
   }
-  block_reduce4(acc, partial + (long)blockIdx.x * 8);
+  block_reduce4(acc, partial);
   __syncthreads();
-  block_reduce4(cnt, partial + (long)blockIdx.x * 8 + 4);
+  block_reduce4(cnt, partial + 4);
+}
+
+__global__ void __launch_bounds__(256) uq_loss_rows_kernel(int B, int T, int O, const float* __restrict__ pred,
+                                                           const float* __restrict__ var,
+                                                           const float* __restrict__ apre,
+                                                           const float* __restrict__ y,
+                                                           const float* __restrict__ counts, int target_idx, float p1,
+                                                           float p2, float* __restrict__ dpred,
+                                                           float* __restrict__ da, double* __restrict__ partial) {
+  uq_loss_rows(B, T, O, pred, var, apre, y, counts, target_idx, p1, p2, 1.0f, dpred, da, partial + (long)blockIdx.x * 8);
+}
+
+// One warp reduces the nblk partial rows of one loss pass.  Lane 0 writes the counts and / or the three scalars
+// {uq_loss, uq_loss_last_tar, mse_0} (any output may be null) and returns them in vals3.
+__device__ __forceinline__ void uq_loss_final(int nblk, const double* __restrict__ partial,
+                                              const float* __restrict__ counts_in, int B, int O, float p1, float p2,
+                                              float* out_loss, float* out_uq0, float* out_mse0, float* counts_out,
+                                              float* vals3) {
+  const int lane = threadIdx.x & 31;
+  double s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int b = lane; b < nblk; b += 32)
+    for (int i = 0; i < 8; ++i) s[i] += partial[(long)b * 8 + i];
+  for (int i = 0; i < 8; ++i) s[i] = warp_sum(s[i]);
+  if (lane != 0) return;
+  if (counts_out) {
+    counts_out[0] = (float)s[4];
+    counts_out[1] = (float)s[5];
+  }
+  const double ms_all = counts_in ? (double)counts_in[0] : s[4];
+  const double ms_last = counts_in ? (double)counts_in[1] : s[5];
+  const double uq0 = s[0] / ms_last, uq1 = s[1] / (ms_last * O), uq2 = s[2] / (ms_all * O);
+  vals3[0] = (float)(p1 * uq0 + (1.0 - p1) * (p2 * uq1 + (1.0 - p2) * uq2));
+  vals3[1] = (float)uq0;
+  vals3[2] = (float)(s[3] / (double)B);
+  if (out_loss) *out_loss = vals3[0];
+  if (out_uq0) *out_uq0 = vals3[1];
+  if (out_mse0) *out_mse0 = vals3[2];
 }
 
 __global__ void uq_loss_final_kernel(int nblk, const double* __restrict__ partial, const float* __restrict__ counts_in,
                                      int B, int O, float p1, float p2, float* __restrict__ out_loss,
                                      float* __restrict__ out_uq0, float* __restrict__ out_mse0,
                                      float* __restrict__ counts_out) {
-  double s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (int b = threadIdx.x; b < nblk; b += 32)
-    for (int i = 0; i < 8; ++i) s[i] += partial[(long)b * 8 + i];
-  for (int i = 0; i < 8; ++i) s[i] = warp_sum(s[i]);
-  if (threadIdx.x != 0) return;
-  if (counts_out) {
-    counts_out[0] = (float)s[4];
-    counts_out[1] = (float)s[5];
+  float v[3];
+  uq_loss_final(nblk, partial, counts_in, B, O, p1, p2, out_loss, out_uq0, out_mse0, counts_out, v);
+}
+
+// forecast_steps > 1 of RNNUqRangeEstimate (losses.py:137-178): blockIdx.y = forecast stage.  Each stage runs the rows
+// above on its own tensors and counts, its gradients scaled by its weight w_s.
+__global__ void __launch_bounds__(256) chain_uq_rows_kernel(int B, int T, int O, ChainUqArgs a, int target_idx, float p1,
+                                                            float p2, double* __restrict__ partial) {
+  const int s = blockIdx.y;
+  uq_loss_rows(B, T, O, a.pred.p[s], a.var.p[s], a.apre.p[s], a.y.p[s], a.counts_in ? a.counts.p[s] : nullptr,
+               target_idx, p1, p2, a.w.w[s], a.dpred.p[s], a.da.p[s],
+               partial + ((long)s * gridDim.x + blockIdx.x) * 8);
+}
+
+// Warp s reduces stage s; then the weighted sums over the stages (losses.py:170-177):
+// out3 = {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}.
+__global__ void chain_uq_final_kernel(int S, int nblk, ChainUqArgs a, int B, int O, float p1, float p2,
+                                      const double* __restrict__ partial, float* __restrict__ out3) {
+  __shared__ float vals[LFMQ_MAX_STAGES][3];
+  const int s = threadIdx.x >> 5;
+  uq_loss_final(nblk, partial + (long)s * nblk * 8, a.counts_in ? a.counts.p[s] : nullptr, B, O, p1, p2,
+                a.loss.p[s], a.uq0.p[s], a.mse0.p[s], a.counts_in ? nullptr : a.counts.p[s], vals[s]);
+  __syncthreads();
+  if (threadIdx.x != 0 || !out3) return;
+  float l = 0.f, u = 0.f, m = 0.f;
+  for (int k = 0; k < S; ++k) {
+    l += a.w.w[k] * vals[k][0];
+    u += a.w.w[k] * vals[k][1];
+    m += a.w.w[k] * vals[k][2];
   }
-  if (!out_loss) return;
-  const double ms_all = counts_in ? (double)counts_in[0] : s[4];
-  const double ms_last = counts_in ? (double)counts_in[1] : s[5];
-  const double uq0 = s[0] / ms_last, uq1 = s[1] / (ms_last * O), uq2 = s[2] / (ms_all * O);
-  *out_loss = (float)(p1 * uq0 + (1.0 - p1) * (p2 * uq1 + (1.0 - p2) * uq2));
-  *out_uq0 = (float)uq0;
-  *out_mse0 = (float)(s[3] / (double)B);
+  out3[0] = l;
+  out3[1] = u;
+  out3[2] = m;
+}
+
+int chain_uq_loss_grad(cudaStream_t s, int S, int B, int T, int O, const ChainUqArgs& a, int target_idx, float p1,
+                       float p2, float* out3, float* scratch) {
+  double* partial = reinterpret_cast<double*>(scratch);
+  chain_uq_rows_kernel<<<dim3(LOSS_BLOCKS, S), 256, 0, s>>>(B, T, O, a, target_idx, p1, p2, partial);
+  LFMQ_LAUNCH_CHECK();
+  chain_uq_final_kernel<<<1, 32 * S, 0, s>>>(S, LOSS_BLOCKS, a, B, O, p1, p2, partial, out3);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
 }
 
 // pred == nullptr: counts only -> counts_out.  Otherwise the three scalars; with dpred also the gradients (counts_in

@@ -51,7 +51,6 @@ struct lfmq_handle_s {
   lfmq::TcState tc;
   int64_t last_step = 0;     // step and row0 of the last forward: the fp32 backward regenerates that call's dropout masks
   int64_t last_row0 = 0;
-  int stream_base = 0;       // first Philox stream index of this handle's layers (stage s of a forecast chain: 2 (L0+s-1))
   int use_gen;               // 1: the general tensor-core path (rnn_tc.cu) runs this handle's bf16 / bf16x3 work
   lfmq::Profiler prof;
 };
@@ -250,7 +249,7 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
     const float* rmask = nullptr;
     const bool stochastic = c.train || c.uq;       // rnn_uq_range_estimate.py:86,88: training=True is a literal there
     if (stochastic && c.recurrent_dropout > 0.f) {
-      RUN(gen_row_mask(s, B, H, dropout_key(c.seed, h->stream_base + 2 * l + 1, step, c.recurrent_dropout), row0,
+      RUN(gen_row_mask(s, B, H, dropout_key(c.seed, h->tc.stream_base + 2 * l + 1, step, c.recurrent_dropout), row0,
                        lb.rmask));
       rmask = lb.rmask;
     }
@@ -275,7 +274,7 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
     }
     const bool drop = stochastic && c.dropout > 0.f;
     RUN(bn_dropout_fwd(s, B, T, H, lb.h, P + lb.ogamma, P + lb.obeta, P + lb.omean, P + lb.ovar, c.bn_epsilon, drop,
-                       dropout_key(c.seed, h->stream_base + 2 * l, step, c.dropout), row0, lb.y));
+                       dropout_key(c.seed, h->tc.stream_base + 2 * l, step, c.dropout), row0, lb.y));
   }
   h->prof.end(LFMQ_REGION_FWD, s);
   h->prof.begin(LFMQ_REGION_HEAD, s);
@@ -318,7 +317,7 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
     const bool drop = (c.train || c.uq) && c.dropout > 0.f;
     h->prof.begin(LFMQ_REGION_BWD, s);
     RUN(bn_dropout_bwd(s, B, T, H, h->dy, lb.h, P + lb.ogamma, P + lb.omean, P + lb.ovar, c.bn_epsilon, drop,
-                       dropout_key(c.seed, h->stream_base + 2 * l, h->last_step, c.dropout), h->last_row0, h->dh_out,
+                       dropout_key(c.seed, h->tc.stream_base + 2 * l, h->last_step, c.dropout), h->last_row0, h->dh_out,
                        G + lb.ogamma, G + lb.obeta, h->scratch, h->scratch_elems));
     const bool gru = c.rnn_cell == LFMQ_CELL_GRU;
     const int NG = gru ? 3 : 4;
@@ -690,7 +689,8 @@ int32_t lfmq_train_step(lfmq_handle h, const float* x, const float* y, int32_t B
 // ---- forecast_steps > 1 (rnn_point_estimate.py:109-150) -------------------------------------------------------
 namespace {
 // Stage 0 is the trunk (num_layers layers + OUTPUT_1); stage s >= 1 one more recurrent layer + BatchNormalization +
-// Dropout + OUTPUT_{s+1} on the raw feature width.  All stages share T, F, O.
+// Dropout + OUTPUT_{s+1} on the raw feature width.  All stages share T, F, O and the head: point estimate in every stage,
+// or in every stage the uq heads OUTPUT_TARGET_{s+1} / OUTPUT_VARIANCE_{s+1} (rnn_uq_range_estimate.py:114-157).
 int chain_check(const lfmq_handle* st, int32_t S, int32_t B, bool training) {
   if (!st || S < 1 || S > lfmq::LFMQ_MAX_STAGES) {
     LFMQ_SET_ERR("lfmq_chain: n_stages %d outside [1, %d]", S, lfmq::LFMQ_MAX_STAGES);
@@ -700,9 +700,9 @@ int chain_check(const lfmq_handle* st, int32_t S, int32_t B, bool training) {
     RUN(check_batch(st[i], B));
     const lfmq_config& c = st[i]->cfg;
     const lfmq_config& c0 = st[0]->cfg;
-    if (c.seq_len != c0.seq_len || c.n_inputs != c0.n_inputs || c.n_outputs != c0.n_outputs || c.uq ||
+    if (c.seq_len != c0.seq_len || c.n_inputs != c0.n_inputs || c.n_outputs != c0.n_outputs || c.uq != c0.uq ||
         (i > 0 && c.num_layers != 1)) {
-      LFMQ_SET_ERR("lfmq_chain: stage %d does not continue stage 0 (same T/F/O, one layer, point estimate)", i);
+      LFMQ_SET_ERR("lfmq_chain: stage %d does not continue stage 0 (same T/F/O, one layer, same uq flag)", i);
       return LFMQ_ERR_ARG;
     }
     if ((training || c.train) && c.precision != LFMQ_PREC_FP32) {
@@ -714,7 +714,7 @@ int chain_check(const lfmq_handle* st, int32_t S, int32_t B, bool training) {
       return LFMQ_ERR_UNSUPPORTED;
     }
     // the Philox stream index continues after the trunk's layers: the extra layer of stage i is layer L0 + i - 1
-    st[i]->stream_base = (i == 0) ? 0 : 2 * (c0.num_layers + i - 1);
+    st[i]->tc.stream_base = (i == 0) ? 0 : 2 * (c0.num_layers + i - 1);
   }
   return 0;
 }
@@ -725,6 +725,10 @@ int32_t lfmq_chain_forward(const lfmq_handle* stages, int32_t n_stages, const fl
   RUN(chain_check(stages, n_stages, B, false));
   if (!x || !preds || (n_stages > 1 && !work)) {
     LFMQ_SET_ERR("lfmq_chain_forward: null pointer");
+    return LFMQ_ERR_ARG;
+  }
+  if (stages[0]->cfg.uq) {
+    LFMQ_SET_ERR("lfmq_chain_forward: uq chain, call lfmq_chain_forward_uq");
     return LFMQ_ERR_ARG;
   }
   cudaStream_t s = (cudaStream_t)stream;
@@ -742,6 +746,36 @@ int32_t lfmq_chain_forward(const lfmq_handle* stages, int32_t n_stages, const fl
       in = next;
     }
     RUN(lfmq_forward(stages[i], in, B, row0, step, preds[i], stream));
+  }
+  return LFMQ_OK;
+}
+
+int32_t lfmq_chain_forward_uq(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
+                              int64_t step, float* const* preds, float* const* vars, float* work, void* stream) {
+  RUN(chain_check(stages, n_stages, B, false));
+  if (!x || !preds || !vars || (n_stages > 1 && !work)) {
+    LFMQ_SET_ERR("lfmq_chain_forward_uq: null pointer");
+    return LFMQ_ERR_ARG;
+  }
+  if (!stages[0]->cfg.uq) {
+    LFMQ_SET_ERR("lfmq_chain_forward_uq: point-estimate chain, call lfmq_chain_forward");
+    return LFMQ_ERR_ARG;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const lfmq_config& c = stages[0]->cfg;
+  const size_t slot = (size_t)B * c.seq_len * c.n_inputs;
+  const float* in = x;
+  for (int i = 0; i < n_stages; ++i) {
+    if (!preds[i] || !vars[i]) {
+      LFMQ_SET_ERR("lfmq_chain_forward_uq: preds[%d] or vars[%d] == NULL", i, i);
+      return LFMQ_ERR_ARG;
+    }
+    if (i > 0) {      // the next window is built from the target predictions (outputs[-2], :118); variances stay put
+      float* next = work + (size_t)(i - 1) * slot;
+      RUN(chain_next_input(s, B, c.seq_len, c.n_inputs, c.n_outputs, in, preds[i - 1], x, next));
+      in = next;
+    }
+    RUN(lfmq_forward_uq(stages[i], in, B, row0, step, preds[i], vars[i], stream));
   }
   return LFMQ_OK;
 }
@@ -767,6 +801,72 @@ int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float
   return chain_combine(s, n_stages, none, 0.f, l2, w, out_dev);
 }
 
+int32_t lfmq_chain_loss_uq(const lfmq_handle* stages, int32_t n_stages, const float* const* preds,
+                           const float* const* vars, const float* const* y, const float* weights, int32_t B,
+                           float* out_dev, void* stream) {
+  if (!stages || n_stages < 1 || n_stages > lfmq::LFMQ_MAX_STAGES || !preds || !vars || !y || !weights || !out_dev ||
+      B <= 0) {
+    LFMQ_SET_ERR("lfmq_chain_loss_uq: bad argument");
+    return LFMQ_ERR_ARG;
+  }
+  lfmq::ChainUqArgs a{};
+  for (int i = 0; i < n_stages; ++i) {
+    if (!stages[i] || !stages[i]->cfg.uq || !preds[i] || !vars[i] || !y[i]) {
+      LFMQ_SET_ERR("lfmq_chain_loss_uq: stage %d: null pointer or a point-estimate handle", i);
+      return LFMQ_ERR_ARG;
+    }
+    a.pred.p[i] = const_cast<float*>(preds[i]);
+    a.var.p[i] = const_cast<float*>(vars[i]);
+    a.y.p[i] = const_cast<float*>(y[i]);
+    a.w.w[i] = weights[i];
+  }
+  const lfmq_config& c = stages[0]->cfg;
+  return chain_uq_loss_grad((cudaStream_t)stream, n_stages, B, c.seq_len, c.n_outputs, a, c.target_idx, c.target_lambda,
+                            c.rnn_lambda, out_dev, stages[0]->scratch);
+}
+
+namespace {
+// lfmq_chain_backward of a uq chain (train.py:201-218): every stage's forward, then one loss pass over all stages for
+// the mask counts and one for the losses and w_s * dLoss_s / d(pred_s, variance pre-activation_s).
+int chain_forward_loss_uq(const lfmq_handle* st, int S, const float* x, const float* const* y, const float* weights,
+                          int B, int64_t row0, int64_t step, float* work, float* loss_out_dev, cudaStream_t s) {
+  const lfmq_config& c0 = st[0]->cfg;
+  const int T = c0.seq_len, F = c0.n_inputs, O = c0.n_outputs;
+  const size_t slot = (size_t)B * T * F;
+  lfmq::ChainUqArgs a{};
+  const float* in = x;
+  for (int i = 0; i < S; ++i) {
+    lfmq_handle h = st[i];
+    h->last_step = step;
+    h->last_row0 = row0;
+    if (i > 0) {
+      float* next = work + (size_t)(i - 1) * slot;
+      RUN(chain_next_input(s, B, T, F, O, in, st[i - 1]->preds, x, next));
+      in = next;
+    }
+    RUN(forward_fp32(h, in, B, row0, step, h->preds, h->var, s));
+    a.y.p[i] = const_cast<float*>(y[i]);
+    a.counts.p[i] = h->denom;
+    a.w.w[i] = weights[i];
+  }
+  float* scratch = st[0]->scratch;
+  RUN(chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, nullptr, scratch));
+  for (int i = 0; i < S; ++i) {
+    a.pred.p[i] = st[i]->preds;
+    a.var.p[i] = st[i]->var;
+    a.apre.p[i] = st[i]->apre;
+    a.dpred.p[i] = st[i]->dpred;
+    a.da.p[i] = st[i]->da;
+    float* tail = st[i]->grads + st[i]->n_train;     // the stage's own {uq_loss, mse_0, .., .., uq_loss_last_tar}
+    a.loss.p[i] = tail;
+    a.mse0.p[i] = tail + 1;
+    a.uq0.p[i] = tail + 4;
+  }
+  a.counts_in = 1;
+  return chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, loss_out_dev, scratch);
+}
+}  // namespace
+
 int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
                             const float* weights, int32_t B, int64_t row0, int64_t step, float* work,
                             float* loss_out_dev, void* stream) {
@@ -784,14 +884,19 @@ int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const f
   // forward of every stage (each keeps its own saved state), then each stage's loss and dLoss/dpred_s, weighted
   lfmq::ChainPtrs dpred{}, l2{}, none{};
   lfmq::ChainWeights w{};
-  const float* in = x;
-  for (int i = 0; i < S; ++i) {
-    lfmq_handle h = stages[i];
-    const lfmq_config& c = h->cfg;
+  for (int i = 0; i < S; ++i)
     if (!y[i]) {
       LFMQ_SET_ERR("lfmq_chain_backward: y[%d] == NULL", i);
       return LFMQ_ERR_ARG;
     }
+  if (c0.uq) {
+    RUN(chain_forward_loss_uq(stages, S, x, y, weights, B, row0, step, work, loss_out_dev, s));
+    for (int i = 0; i < S; ++i) dpred.p[i] = stages[i]->dpred;      // variances never feed forward: no dvar feedback
+  }
+  const float* in = x;
+  for (int i = 0; i < S && !c0.uq; ++i) {
+    lfmq_handle h = stages[i];
+    const lfmq_config& c = h->cfg;
     h->last_step = step;
     h->last_row0 = row0;
     if (i > 0) {
@@ -809,7 +914,7 @@ int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const f
     l2.p[i] = tail;
     w.w[i] = weights[i];
   }
-  if (loss_out_dev) RUN(chain_combine(s, S, none, 0.f, l2, w, loss_out_dev));
+  if (loss_out_dev && !c0.uq) RUN(chain_combine(s, S, none, 0.f, l2, w, loss_out_dev));
   // BPTT from the last stage down; the input gradient of stage i lands on the last time step of earlier predictions
   for (int i = S - 1; i >= 1; --i) {
     const float* in_i = work + (size_t)(i - 1) * slot;

@@ -1361,7 +1361,7 @@ static int gen_run_trunk(TcState& st, const lfmq_config& c, const float* params,
     ep.cst = save ? ly.cst : nullptr;
     ep.accurate = m.x3 ? 1 : 0;
     ep.use_rec = rec ? 1 : 0;
-    ep.rkey = dropout_key(c.seed, 2 * l + 1, step, c.recurrent_dropout);
+    ep.rkey = dropout_key(c.seed, st.stream_base + 2 * l + 1, step, c.recurrent_dropout);
     const CUtensorMap& th = rec ? ly.tm_hm : ly.tm_h;
     const CUtensorMap& th_lo = rec ? ly.tm_hm_lo : ly.tm_h_lo;     // bf16x3
     // steps 1 .. T-1 as ONE persistent launch when all its CTAs fit on the machine at once (see GArgs::n_steps)
@@ -1413,7 +1413,7 @@ static int gen_run_trunk(TcState& st, const lfmq_config& c, const float* params,
     __nv_bfloat16* yo_lo = last ? m.head_in_lo : m.layers[l + 1].in_lo;
     const long n = (long)T * B * (H / 8);
     gbn_drop_fwd_kernel<<<(int)cdivl(n, 256), 256, 0, s>>>(B, T, H, Bp, ly.hseq, ly.hseq_lo, ly.bn, drop ? 1 : 0,
-                                                           dropout_key(c.seed, 2 * l, step, c.dropout), row0, yo, yo_lo);
+                                                           dropout_key(c.seed, st.stream_base + 2 * l, step, c.dropout), row0, yo, yo_lo);
     LFMQ_LAUNCH_CHECK();
   }
   return 0;
@@ -1598,7 +1598,7 @@ int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* 
       const int ctas = (int)cdivl((long)T * B, GBN_ROWS);
       const int RL = 256 / (H / 8) > 0 ? 256 / (H / 8) : 1;
       gbn_drop_bwd_kernel<<<ctas, 256, RL * 2 * H * 4, s>>>(B, T, H, Bp, m.dy, ly.hseq, ly.bn, drop ? 1 : 0,
-                                                           dropout_key(c.seed, 2 * l, step, c.dropout), row0, m.dhout, m.bn_part);
+                                                           dropout_key(c.seed, st.stream_base + 2 * l, step, c.dropout), row0, m.dhout, m.bn_part);
       LFMQ_LAUNCH_CHECK();
       gpartial_reduce_kernel<<<(2 * H * 32 + 255) / 256, 256, 0, s>>>(ctas, H, H, m.bn_part, grads + ly.off.ogamma,
                                                                     grads + ly.off.obeta);
@@ -1608,7 +1608,7 @@ int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* 
     ep.T = T; ep.B = B; ep.Bp = Bp; ep.H = H; ep.NRT = m.NRT; ep.NB16 = m.NB16; ep.row0 = row0;
     ep.gates = ly.gates; ep.cst = ly.cst; ep.dhout = m.dhout; ep.dcstate = m.dcstate; ep.dz = m.dz;
     ep.use_rec = rec ? 1 : 0;
-    ep.rkey = dropout_key(c.seed, 2 * l + 1, step, c.recurrent_dropout);
+    ep.rkey = dropout_key(c.seed, st.stream_base + 2 * l + 1, step, c.recurrent_dropout);
     // The step's epilogue is HBM-bound (saved gates / cell states in, dz out: ~46 MB per step at H = 512) and its
     // mainloop L2-bound, and one launch puts every CTA into the same phase at the same time.  Two half-batches on two
     // streams (each its own PDL chain) drift apart, so one half's epilogue runs beside the other's mainloop.

@@ -14,6 +14,7 @@ struct GenImpl;
 // Tensor-core state of a handle.  layout() in lfmq_api.cu sets up at most one of the two paths.
 struct TcState {
   int weights_dirty = 1;        // the parameters changed since the path last packed its bf16 copies of them
+  int stream_base = 0;          // first Philox stream index of the handle's layers (stage s of a forecast chain: 2 (L0+s-1))
   Profiler* prof = nullptr;
   TcImpl* impl = nullptr;       // cluster path
   GenImpl* gen = nullptr;       // general path

@@ -237,12 +237,15 @@ class ForecasterEngine(object):
 class ForecastChainEngine(object):
     """forecast_steps > 1 (scripts/models/point_estimate/rnn_point_estimate.py:109-150): stage 0 is the trunk, every
     further stage one more recurrent layer + BatchNormalization + Dropout + Dense on the shifted input window.  One
-    ForecasterEngine (one C-ABI handle) per stage; the lfmq_chain_* entry points run the whole graph."""
+    ForecasterEngine (one C-ABI handle) per stage; the lfmq_chain_* entry points run the whole graph.
+    uq=True: RNNUqRangeEstimate's graph (models/uq_range_estimate/rnn_uq_range_estimate.py:114-157), every stage with a
+    target and a variance head and dropout always on; the next window is built from the target predictions."""
 
-    def __init__(self, *, forecast_steps, weights, num_layers, **kw):
+    def __init__(self, *, forecast_steps, weights, num_layers, uq=False, **kw):
         assert forecast_steps >= 1
         self.S = int(forecast_steps)
-        self.stages = [ForecasterEngine(num_layers=num_layers if s == 0 else 1, **kw) for s in range(self.S)]
+        self.uq = bool(uq)
+        self.stages = [ForecasterEngine(num_layers=num_layers if s == 0 else 1, uq=self.uq, **kw) for s in range(self.S)]
         e0 = self.stages[0]
         self.lib, self.device, self.cfg, self.precision = e0.lib, e0.device, e0.cfg, e0.precision
         self.T, self.F, self.O, self.H, self.L = e0.T, e0.F, e0.O, e0.H, e0.L
@@ -260,6 +263,8 @@ class ForecastChainEngine(object):
                     name = name.replace('%s_1/' % cell, '%s_%d/' % (cell, self.L + s))
                     name = name.replace('batch_normalization/', 'batch_normalization_%d/' % (self.L + s - 1))
                     name = name.replace('OUTPUT_1/', 'OUTPUT_%d/' % (s + 1))
+                    name = name.replace('OUTPUT_TARGET_1/', 'OUTPUT_TARGET_%d/' % (s + 1))
+                    name = name.replace('OUTPUT_VARIANCE_1/', 'OUTPUT_VARIANCE_%d/' % (s + 1))
                 self.specs.append((s, name, shp, off, tr))
         self.n_total = sum(e.n_total for e in self.stages)
         self.n_trainable = sum(e.n_trainable for e in self.stages)
@@ -274,9 +279,15 @@ class ForecastChainEngine(object):
         return self._work
 
     def forward(self, x, step=0, row0=0):
-        """model(inp) -> [pred_1 .. pred_S], device tensors [B,T,O]."""
+        """model(inp) -> [pred_1 .. pred_S], device tensors [B,T,O]; a uq chain returns the Keras output list
+        [tar_1, var_1, .., tar_S, var_S] (rnn_uq_range_estimate.py:107-108,152-155)."""
         B = self.stages[0]._check_x(x)
         preds = [torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device) for _ in range(self.S)]
+        if self.uq:
+            var = [torch.empty_like(p) for p in preds]
+            N.check(self.lib.lfmq_chain_forward_uq(self._handles, self.S, _ptr(x), B, row0, step, self._ptrs(preds),
+                                                   self._ptrs(var), _ptr(self._workbuf(B)), _stream()))
+            return [t for pv in zip(preds, var) for t in pv]
         N.check(self.lib.lfmq_chain_forward(self._handles, self.S, _ptr(x), B, row0, step, self._ptrs(preds),
                                             _ptr(self._workbuf(B)), _stream()))
         return preds
@@ -290,13 +301,22 @@ class ForecastChainEngine(object):
                                          preds[0].shape[0], _ptr(out), _stream()))
         return out
 
+    def loss_uq(self, preds, var, ys):
+        """Losses.weight_adjusted_uq_loss(ys, preds, var) (losses.py:137-178): device tensor
+        {uq_loss, uq_loss_last_tar, mse}, each summed over the steps with forecast_steps_weights."""
+        out = torch.empty(3, dtype=torch.float32, device=preds[0].device)
+        preds, var, ys = ([t.contiguous() for t in a] for a in (preds, var, ys))
+        N.check(self.lib.lfmq_chain_loss_uq(self._handles, self.S, self._ptrs(preds), self._ptrs(var), self._ptrs(ys),
+                                            self._w, preds[0].shape[0], _ptr(out), _stream()))
+        return out
+
     def backward(self, x, ys, step=0, row0=0, out=None):
         B = self.stages[0]._check_x(x)
         assert len(ys) == self.S
         for y in ys:
             assert y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and tuple(y.shape) == (B, self.T, self.O)
         if out is None:
-            out = torch.empty(2, dtype=torch.float32, device=x.device)
+            out = torch.empty(3 if self.uq else 2, dtype=torch.float32, device=x.device)
         N.check(self.lib.lfmq_chain_backward(self._handles, self.S, _ptr(x), self._ptrs(ys), self._w, B, row0, step,
                                              _ptr(self._workbuf(B)), _ptr(out), _stream()))
         return out
@@ -305,10 +325,11 @@ class ForecastChainEngine(object):
         N.check(self.lib.lfmq_chain_apply(self._handles, self.S, float(lr), int(iteration), _stream()))
 
     def train_step(self, x, ys, step, lr):
-        """One Train._train_step_point over the S-output model; device tensor {loss, mse}."""
+        """One Train._train_step_point over the S-output model; device tensor {loss, mse}.  uq chain: one
+        Train._train_step_uq_range, {uq_loss_last_tar, mse} (train.py:225), both weighted over the steps."""
         out = self.backward(x, ys, step=step)
         self.apply(lr, step)
-        return out
+        return out[1:] if self.uq else out
 
     def unscale(self, arr, scale, center, log_squasher):
         return self.stages[0].unscale(arr, scale, center, log_squasher)
@@ -324,7 +345,7 @@ class ForecastChainEngine(object):
         return [w for e in self.stages for w in e.get_weights(trainable_only)]
 
     def set_weights(self, weights):
-        """weights in trainable_variables order: the trunk's, then 7 per extra stage."""
+        """weights in trainable_variables order: the trunk's, then 7 per extra stage (9 on a uq chain)."""
         i = 0
         for e in self.stages:
             n = len(e.trainable_specs)

@@ -1,6 +1,6 @@
 """Losses(config, target_idx).weight_adjusted_mse (reference: scripts/model_utils/losses.py:19-135), evaluated by
 the native loss kernel (lfmq_loss; lfmq_chain_loss for forecast_steps > 1), and Losses.weight_adjusted_uq_loss
-(:137-284) by lfmq_loss_uq (forecast_steps == 1).  Only the RNN branches are built; the MLP / Huber branches belong to
+(:137-284) by lfmq_loss_uq (lfmq_chain_loss_uq for forecast_steps > 1).  Only the RNN branches are built; the MLP / Huber branches belong to
 other model families."""
 from __future__ import absolute_import, division, print_function
 
@@ -66,21 +66,32 @@ class Losses(object):
         return _Scalar(out[0]), _Scalar(out[1])
 
     def weight_adjusted_uq_loss(self, y_true, y_pred, y_var):
-        """losses.py:137-178: (uq_loss, uq_loss_last_tar, mse), each with ``.numpy()``."""
+        """losses.py:137-178: (uq_loss, uq_loss_last_tar, mse), each with ``.numpy()``, each summed over the forecast
+        steps with config.forecast_steps_weights."""
         assert self.config.UQ, "weight_adjusted_mse is only available for uq range estimate models. UQ should be True"
         assert self.config.forecast_steps > 0, 'forecasts_steps should be a positive integer. %i was provided' % \
             self.config.forecast_steps
         for name, v in (('y_true', y_true), ('y_pred', y_pred), ('y_var', y_var)):
             assert isinstance(v, (list, tuple)), \
                 'arguments to loss function need to be a list [%s], [%s1, %s2, ..]' % (name, name, name)
-        if self.config.forecast_steps != 1 or 'RNN' not in self.config.nn_type:
-            raise NotImplementedError('only RNN uq range estimates with forecast_steps=1 are built on this path')
-        if len(self.config.forecast_steps_weights) == 1:
-            self.config.forecast_steps_weights = [1.0]
+        if 'RNN' not in self.config.nn_type:
+            raise NotImplementedError('only RNN uq range estimates are built on this path')
+        S = self.config.forecast_steps
+        for name, v in (('y_true', y_true), ('y_pred', y_pred), ('y_var', y_var)):
+            assert len(v) >= S, '%s holds %d forecast steps, forecast_steps is %d' % (name, len(v), S)
+        if S == 1:
+            if len(self.config.forecast_steps_weights) == 1:
+                self.config.forecast_steps_weights = [1.0]
+        else:
+            assert len(self.config.forecast_steps_weights) == S     # losses.py:164-166
         import torch
         assert self.engine is not None, 'Losses is not bound to a native engine'
         dev = self.engine.device
         to = lambda a: (a if isinstance(a, torch.Tensor) else
                         torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))).to(dev, torch.float32).contiguous()
-        out = self.engine.loss_uq(to(y_pred[0]), to(y_var[0]), to(y_true[0]))
+        if S == 1:
+            out = self.engine.loss_uq(to(y_pred[0]), to(y_var[0]), to(y_true[0]))
+        else:                       # losses.py:159-177: per-step losses with their own masks, linearly weighted
+            out = self.engine.loss_uq([to(p) for p in y_pred[:S]], [to(v) for v in y_var[:S]],
+                                      [to(y) for y in y_true[:S]])
         return _Scalar(out[0]), _Scalar(out[1]), _Scalar(out[2])

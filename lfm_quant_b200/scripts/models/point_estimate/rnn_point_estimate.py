@@ -30,13 +30,14 @@ class NativeChainForecaster(object):
     the list [pred_1 .. pred_S]; ``train_step`` takes the list of S targets.  Every extra forecast step is one more
     recurrent layer + BatchNormalization + Dropout + Dense over the input window shifted by one, with
     [latest prediction's last time step, last available aux features] appended (models/model_base_class.py:18-51).
-    Training-mode graphs run on the fp32 kernels; a forward-only graph (predict.py) may use any precision."""
+    Training-mode graphs run on the fp32 kernels; a forward-only graph (predict.py) may use any precision.
+    uq=True: RNNUqRangeEstimate's graph (rnn_uq_range_estimate.py:114-157); ``model(inp)`` / ``model.predict(inp)`` return
+    the interleaved list [tar_1, var_1, .., tar_S, var_S] and ``train_step`` returns {uq_loss_last_tar, mse}."""
 
-    uq = False
-
-    def __init__(self, config, seq_len, n_inputs, n_outputs, target_idx):
+    def __init__(self, config, seq_len, n_inputs, n_outputs, target_idx, uq=False):
         from ....engine import ForecastChainEngine
         self.config = config
+        self.uq = bool(uq)
         if config.rnn_cell not in ('lstm', 'gru'):
             raise NotImplementedError                    # rnn_point_estimate.py:148-149
         precision = getattr(config, 'precision', 'fp32')
@@ -52,7 +53,7 @@ class NativeChainForecaster(object):
             dropout=config.dropout, recurrent_dropout=config.recurrent_dropout, target_lambda=config.target_lambda,
             rnn_lambda=config.rnn_lambda, max_grad_norm=config.max_grad_norm, max_norm=float(config.max_norm),
             sgd_momentum=config.sgd_momentum, seed=config.seed, forward_only=not config.train,
-            rnn_cell=config.rnn_cell)
+            rnn_cell=config.rnn_cell, uq=self.uq)
         specs = [(n, s) for (_, n, s, _, tr) in self.engine.specs if tr]
         self.engine.set_weights(Initializer(config).initial_weights(specs))
         self.trainable_variables = [_Variable(self, i, n, s) for i, (n, s) in enumerate(specs)]
@@ -68,15 +69,15 @@ class NativeChainForecaster(object):
         B, mb = x.shape[0], self.engine.cfg.max_batch
         self._calls += 1
         outs = [self.engine.forward(x[s:s + mb].contiguous(), step=self._calls, row0=s) for s in range(0, B, mb)]
-        S = self.engine.S
-        return [outs[0][k] if len(outs) == 1 else torch.cat([o[k] for o in outs], dim=0) for k in range(S)]
+        return [outs[0][k] if len(outs) == 1 else torch.cat([o[k] for o in outs], dim=0) for k in range(len(outs[0]))]
 
     def predict(self, inp, batch_size=None):
-        """model.predict(inp) (train.py:289, predict.py:129): list of S ndarrays [B,T,O]."""
+        """model.predict(inp) (train.py:289, predict.py:129): list of S ndarrays [B,T,O] (uq: 2S, interleaved)."""
         return [p.cpu().numpy() for p in self.predict_device(inp)]
 
     def train_step(self, inp, targets, lr, iteration):
-        """Train._train_step_point (train.py:178-199) over the S-output graph; device tensor {loss, mse}."""
+        """Train._train_step_point (train.py:178-199) over the S-output graph; device tensor {loss, mse}.  uq graph:
+        Train._train_step_uq_range (train.py:201-225), {uq_loss_last_tar, mse}."""
         assert isinstance(targets, (list, tuple)), 'targets must be the list of forecast_steps targets (train.py:188)'
         return self.engine.train_step(self._to_device(inp), [self._to_device(t) for t in targets], iteration, lr)
 
@@ -87,8 +88,8 @@ class NativeChainForecaster(object):
         return self.engine.n_total
 
     def summary(self):
-        lines = ['Model: "RNNPointEstimate" (native sm_90a, forecast_steps=%d, precision=%s)' % (self.engine.S,
-                                                                                                self.engine.precision),
+        lines = ['Model: "%s" (native sm_90a, forecast_steps=%d, precision=%s)' % (
+                     'RNNUqRangeEstimate' if self.uq else 'RNNPointEstimate', self.engine.S, self.engine.precision),
                  '%-44s %-16s %10s' % ('Variable', 'Shape', 'Param #'), '=' * 72]
         for _, name, shape, _, tr in self.engine.specs:
             lines.append('%-44s %-16s %10d%s' % (name, str(tuple(shape)), int(np.prod(shape)), '' if tr else '  (non-trainable)'))
@@ -130,7 +131,7 @@ class NativeForecaster(object):
         if config.rnn_cell not in ('lstm', 'gru'):
             raise NotImplementedError                    # rnn_point_estimate.py:101-102
         if config.forecast_steps != 1:
-            raise NotImplementedError('forecast_steps > 1 is built by NativeChainForecaster (point estimates only)')
+            raise NotImplementedError('forecast_steps > 1 is built by NativeChainForecaster')
         self.engine = ForecasterEngine(
             max_batch=config.batch_size, seq_len=seq_len, n_inputs=n_inputs, n_outputs=n_outputs,
             num_hidden=config.num_hidden, num_layers=config.num_layers, target_idx=target_idx,

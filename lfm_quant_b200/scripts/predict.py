@@ -42,7 +42,8 @@ class Predict(object):
         self.model.load_weights(os.path.join(self.chkpts_dir, "chkpt"))
         outputs = defaultdict(list)
         for (inp_dev, target_dev, metadata) in self._batches:
-            inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()]
+            # one target window per input window: every forecast step is compared with it (Train._step_targets)
+            inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()] * self.config.forecast_steps
             outputs['date'].append(np.expand_dims(metadata[:, 0].astype('int32'), -1))
             outputs['gvkey'].append(np.expand_dims(metadata[:, 1], -1))
             outputs['seq_norm'].append(np.expand_dims(metadata[:, 2].astype('float32'), -1))
@@ -53,7 +54,7 @@ class Predict(object):
             if not self.config.UQ:
                 preds = [self.model.predict(inp_dev)]
                 variance = [np.zeros(x.shape) for x in preds]   # predict.py:133
-            else:                                               # predict.py:135-138
+            else:                       # predict.py:135-138: [tar_1, var_1, .., tar_S, var_S]
                 model_preds = self.model.predict(inp_dev)
                 preds, variance = model_preds[0::2], model_preds[1::2]
             outputs['norm_preds'].append(self._extract_preds(preds))

@@ -180,11 +180,19 @@ class Train(object):
         self.optimizer.iterations += 1
         return out[1]
 
+    def _step_targets(self, targets):
+        """The list of forecast_steps targets of one batch.  The dataset materialises one target window per input window
+        (forecast_n ahead); every forecast step of a multi-step graph is scored against it."""
+        if self.config.forecast_steps == 1 or isinstance(targets, (list, tuple)):
+            return targets
+        return [targets] * self.config.forecast_steps
+
     def _train_step_uq_range(self, inp, targets):
-        """train.py:201-225 as one fused native step; returns device scalars (uq_loss_last_tar, mse_0)."""
+        """train.py:201-225 as one fused native step; returns device scalars (uq_loss_last_tar, mse_0), weighted over
+        the forecast steps when forecast_steps > 1."""
         assert self.config.UQ
         lr = self.optimizer.current_lr()
-        out = self.model.train_step(inp, targets, lr, self.optimizer.iterations)
+        out = self.model.train_step(inp, self._step_targets(targets), lr, self.optimizer.iterations)
         self.optimizer.iterations += 1
         return out[0], out[1]
 
@@ -249,20 +257,24 @@ class Train(object):
 
     def _validation_metrics_uq_range_estimate(self):
         """train.py:338-416: predict every validation batch (dropout stays on), uq loss over the stacked arrays, MSE of
-        the un-scaled target predictions."""
+        the un-scaled target predictions.  forecast_steps > 1: every step's arrays, the losses weighted over the steps
+        (train.py:387-416)."""
+        S = self.config.forecast_steps
         preds, var, targets = [], [], []
         for cur_batch in self._valid_batches:
             batch_pred = self.model.predict(cur_batch[0])
-            preds.append(batch_pred[0::2][0])
-            var.append(batch_pred[1::2][0])
-            targets.append(cur_batch[1].cpu().numpy())
+            preds.append(batch_pred[0::2])
+            var.append(batch_pred[1::2])
+            tar = self._step_targets(cur_batch[1])
+            targets.append([t.cpu().numpy() for t in (tar if S > 1 else [tar])])
         if not preds:
             return float('nan'), float('nan'), float('nan')
-        pred_all, var_all, target_all = (np.vstack(a).astype('float32') for a in (preds, var, targets))
-        pred_unscaled = self._unscale_preds(copy.deepcopy(pred_all))
-        target_unscaled = self._unscale_preds(copy.deepcopy(target_all))
-        _, valid_uq_loss, valid_mse = self.losses.weight_adjusted_uq_loss([target_all], [pred_all], [var_all])
-        _, valid_mse_fcst = self.losses.weight_adjusted_mse([target_unscaled], [pred_unscaled])
+        pred_all, var_all, target_all = ([np.vstack([b[i] for b in a]).astype('float32') for i in range(S)]
+                                         for a in (preds, var, targets))
+        pred_unscaled = [self._unscale_preds(copy.deepcopy(p)) for p in pred_all]
+        target_unscaled = [self._unscale_preds(copy.deepcopy(t)) for t in target_all]
+        _, valid_uq_loss, valid_mse = self.losses.weight_adjusted_uq_loss(target_all, pred_all, var_all)
+        _, valid_mse_fcst = self.losses.weight_adjusted_mse(target_unscaled, pred_unscaled)
         return valid_uq_loss.numpy(), valid_mse.numpy(), valid_mse_fcst.numpy()
 
     def _unscale_preds(self, arr):
