@@ -132,10 +132,17 @@ int32_t lfmq_loss_uq(lfmq_handle h, const float* preds, const float* var, const 
  * Under data parallelism the host all-reduces these two floats once per batch and passes the result
  * as `denom_dev` below. */
 int32_t lfmq_mask_count(lfmq_handle h, const float* y, int32_t B, float* out_dev, void* stream);
+/* The counts behind the uq loss (losses.py:179-284): out_dev = {B, sum(mask), sum(mask[:, T-1])}, the denominators of
+ * mse_0, of the mean over the mask and of the means over the last step.  Under data parallelism the host all-reduces
+ * these three floats once per batch and passes the result as `denom_dev` of lfmq_backward on a uq handle. */
+int32_t lfmq_mask_count_uq(lfmq_handle h, const float* y, int32_t B, float* out_dev, void* stream);
 
 /* First half of Train._train_step_point (train.py:181-192): forward, loss, BPTT.  Fills the flat
  * gradient buffer (+ its 4-float tail).  denom_dev = device {B_global, mask_count_global} or NULL to use
  * this call's own batch.  With N ranks the host all-reduces grads[0 : n_trainable+2] (SUM) next.
+ * On a uq handle (train.py:201-218) denom_dev = the three counts of lfmq_mask_count_uq summed over the ranks; the tail
+ * entries {uq_loss, mse_0, uq_loss_last_tar} are then this shard's contributions, and the host reduces the gradient
+ * and them through lfmq_chain_grad_pack / lfmq_chain_grad_unpack with n_stages = 1.
  * Stream semantics: everything is ordered on `stream`. */
 int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, int64_t row0, int64_t step,
                       const float* denom_dev, void* stream);
@@ -189,6 +196,33 @@ int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const f
 /* tf.clip_by_global_norm over the variables of ALL stages (train.py:195-196, stage 0's max_grad_norm), then each
  * stage's optimizer update and MaxNorm constraint. */
 int32_t lfmq_chain_apply(const lfmq_handle* stages, int32_t n_stages, float lr, int64_t iteration, void* stream);
+
+/* ---- data parallelism over the company-batch axis for chains and uq handles ----
+ * Each rank runs the chain's backward on its rows with the loss denominators of the whole global batch, packs every
+ * stage's gradients and loss tail into one contiguous vector, all-reduces it (SUM, the only collective of the step),
+ * unpacks it and runs lfmq_chain_apply (or lfmq_apply on a single handle), which clips, updates and constrains the
+ * same reduced gradients on every rank.  A rank without rows packs nothing: it zeroes the vector and joins the
+ * all-reduce, the unpack and the apply. */
+/* Every stage's counts for one batch: out_dev[3 s .. 3 s + 2] = {B, sum(mask), sum(mask[:, T-1])} of y[s], as
+ * lfmq_mask_count_uq.  The host all-reduces the 3 * n_stages floats once per batch.  Point and uq chains alike. */
+int32_t lfmq_chain_mask_count(const lfmq_handle* stages, int32_t n_stages, const float* const* y, int32_t B,
+                              float* out_dev, void* stream);
+/* lfmq_chain_backward with the stages' counts of the global batch (lfmq_chain_mask_count summed over the ranks,
+ * device, 3 floats per stage) as every loss denominator.  row0 = global index of this shard's first row (keys the
+ * dropout masks).  Each stage's tail and loss_out_dev then hold this shard's contributions to the global values. */
+int32_t lfmq_chain_backward_dp(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
+                               const float* weights, int32_t B, int64_t row0, int64_t step, const float* denom_dev,
+                               float* work, float* loss_out_dev, void* stream);
+/* Length of the packed vector: sum_s (n_trainable_s + k), k = 2 tail entries {loss, mse_0} on a point-estimate chain,
+ * k = 3 {uq_loss, mse_0, uq_loss_last_tar} on a uq chain.  grad_norm and clip_scale are not carried: the apply computes
+ * them from the reduced gradients. */
+int32_t lfmq_chain_grad_pack_size(const lfmq_handle* stages, int32_t n_stages, int64_t* n_elems);
+/* flat (device, 16-byte aligned) = [grads_0[0:n_0], tail_0, grads_1[0:n_1], tail_1, ...]: one launch for all stages */
+int32_t lfmq_chain_grad_pack(const lfmq_handle* stages, int32_t n_stages, float* flat, void* stream);
+/* The inverse scatter into the stages' gradient buffers.  loss_out_dev (nullable; needs the host `weights`) = the
+ * weighted sums over the stages of the unpacked tails, as lfmq_chain_backward's loss_out_dev. */
+int32_t lfmq_chain_grad_unpack(const lfmq_handle* stages, int32_t n_stages, const float* flat, const float* weights,
+                               float* loss_out_dev, void* stream);
 
 /* Dataset.get_batch (data_processing.py:307-368) with _get_train_seq/_get_pred_seq (:370-449) and
  * log_squasher (:600-609) over a device-resident float64 copy of Dataset.data_values' numeric columns.

@@ -75,6 +75,13 @@ SYMBOLS = {
     'lfmq_chain_loss_uq': (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_backward': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),
     'lfmq_chain_apply': (C.c_int32, [_P, C.c_int32, C.c_float, C.c_int64, _P]),
+    'lfmq_mask_count_uq': (C.c_int32, [_P, _P, C.c_int32, _P, _P]),
+    'lfmq_chain_mask_count': (C.c_int32, [_P, C.c_int32, _P, C.c_int32, _P, _P]),
+    'lfmq_chain_backward_dp': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P,
+                                           _P]),
+    'lfmq_chain_grad_pack_size': (C.c_int32, [_P, C.c_int32, C.POINTER(C.c_int64)]),
+    'lfmq_chain_grad_pack': (C.c_int32, [_P, C.c_int32, _P, _P]),
+    'lfmq_chain_grad_unpack': (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P]),
     'lfmq_window_index': (C.c_int32, [C.POINTER(LfmqWindowIndexArgs), _P]),
     'lfmq_gather_batch': (C.c_int32, [C.POINTER(LfmqGatherArgs), _P]),
     'lfmq_unscale': (C.c_int32, [_P, _P, C.c_int64, C.c_int32, _P, _P, C.c_int32, _P]),

@@ -67,6 +67,18 @@ struct ChainUqArgs {
 };
 int chain_uq_loss_grad(cudaStream_t s, int S, int B, int T, int O, const ChainUqArgs& a, int target_idx, float p1,
                        float p2, float* out3, float* scratch);
+// Data parallelism: every stage's gradient buffer g[s] (16-byte aligned) holds n[s] gradients and then its tail; the
+// flat vector holds, from off[s], the n[s] gradients and the ntail reduced tail entries: {loss, mse_0} (ntail = 2) or
+// {uq_loss, mse_0, uq_loss_last_tar} (ntail = 3, tail indices 0, 1, 4).  One launch copies all stages (unpack: flat ->
+// buffers).  On unpack, loss_out (nullable) = sum_s w_s of the tails: {loss, mse} or {uq_loss, uq_loss_last_tar, mse}.
+struct GradPack {
+  float* g[LFMQ_MAX_STAGES];
+  long n[LFMQ_MAX_STAGES];
+  long off[LFMQ_MAX_STAGES];
+  int ntail;
+};
+int grad_pack(cudaStream_t s, int S, const GradPack& p, float* flat, bool unpack, const ChainWeights& w,
+              float* loss_out);
 
 struct GatherArgs {
   int n_rows, n_cols, B, T, F, O, stride, seq_norm_col, log_squasher, aux_masking;

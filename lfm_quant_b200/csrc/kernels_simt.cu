@@ -683,6 +683,65 @@ int chain_combine(cudaStream_t s, int S, const ChainPtrs& scalars, float clip, c
   return 0;
 }
 
+// Data parallelism over a chain (or one handle): blockIdx.y = stage.  Stage s's gradients grads_s[0:n_s] and its
+// reduced tail entries (kGradPackTail) occupy flat[off_s : off_s + n_s + ntail].  The gradient buffers are 16-byte
+// aligned; the flat side is accessed as float4 where off_s is a multiple of 4, else element by element.
+__constant__ int kGradPackTail[3] = {0, 1, 4};      // {loss, mse_0} or {uq_loss, mse_0, uq_loss_last_tar}
+
+__global__ void __launch_bounds__(256) grad_pack_kernel(GradPack p, float* __restrict__ flat, int unpack,
+                                                        ChainWeights w, float* __restrict__ loss_out) {
+  const int s = blockIdx.y;
+  float* __restrict__ g = p.g[s];
+  float* __restrict__ f = flat + p.off[s];
+  const long n = p.n[s], n4 = n >> 2;
+  const bool vec = (p.off[s] & 3) == 0;
+  float4* g4 = reinterpret_cast<float4*>(g);
+  float4* f4 = reinterpret_cast<float4*>(f);
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
+    if (unpack) {
+      g4[i] = vec ? f4[i] : make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
+    } else {
+      const float4 v = g4[i];
+      if (vec) {
+        f4[i] = v;
+      } else {
+        f[4 * i] = v.x;
+        f[4 * i + 1] = v.y;
+        f[4 * i + 2] = v.z;
+        f[4 * i + 3] = v.w;
+      }
+    }
+  }
+  if (blockIdx.x != 0) return;
+  const int rem = (int)(n - 4 * n4);
+  if ((int)threadIdx.x < rem + p.ntail) {      // the last n % 4 gradients, then the tail entries
+    const int j = (int)threadIdx.x - rem;
+    const long gi = j < 0 ? 4 * n4 + threadIdx.x : n + kGradPackTail[j];
+    const long fi = j < 0 ? gi : n + j;
+    if (unpack) g[gi] = f[fi];
+    else f[fi] = g[gi];
+  }
+  // the weighted sums over the stages of lfmq_chain_loss / lfmq_chain_loss_uq, from the reduced tails
+  if (unpack && loss_out && s == 0 && threadIdx.x == 32) {
+    for (int j = 0; j < p.ntail; ++j) {
+      const int k = (p.ntail == 3 && j > 0) ? 3 - j : j;     // uq: {uq_loss, uq_loss_last_tar, mse}
+      float acc = 0.f;
+      for (int t = 0; t < (int)gridDim.y; ++t) acc += w.w[t] * flat[p.off[t] + p.n[t] + k];
+      loss_out[j] = acc;
+    }
+  }
+}
+
+int grad_pack(cudaStream_t s, int S, const GradPack& p, float* flat, bool unpack, const ChainWeights& w,
+              float* loss_out) {
+  long n4 = 1;
+  for (int i = 0; i < S; ++i) n4 = n4 > (p.n[i] >> 2) ? n4 : (p.n[i] >> 2);
+  const int gx = (int)(cdiv(n4, 256) < 264 ? cdiv(n4, 256) : 264);
+  grad_pack_kernel<<<dim3(gx, S), 256, 0, s>>>(p, flat, unpack ? 1 : 0, w, loss_out);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
 __global__ void fill_kernel(float* p, long n, float v) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -795,9 +854,11 @@ int softplus_floor(cudaStream_t s, long n, const float* a, float* var) {
 
 // One thread per [b,t] row.  Per element (losses.py:197-201,268-273): pm = p*m, vm = v*m, term = (pm-y)^2 * (1/vm) +
 // log(vm) in fp32 exactly as written there -- a masked row gives 0*inf + log 0 = NaN, as in the reference; sums are
-// carried in fp64.  pred == nullptr: only the two mask counts.  dpred != nullptr: gradients w.r.t. pred and w.r.t. the
+// carried in fp64.  pred == nullptr: only the mask counts.  dpred != nullptr: gradients w.r.t. pred and w.r.t. the
 // variance head's pre-activation `apre` (tf.maximum passes the gradient to softplus above the floor), using the counts
-// of a previous pass, both multiplied by the forecast step's weight w (exactly 1 for forecast_steps = 1).
+// of a previous pass (or their sums over the data-parallel ranks), both multiplied by the forecast step's weight w
+// (exactly 1 for forecast_steps = 1).  Counts are {B, unmasked rows, unmasked last-step rows}: the denominators of
+// mse_0, of the mean over the mask and of the means over the last step.
 __device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* __restrict__ pred,
                                              const float* __restrict__ var, const float* __restrict__ apre,
                                              const float* __restrict__ y, const float* __restrict__ counts,
@@ -807,7 +868,7 @@ __device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* _
   double cnt[4] = {0, 0, 0, 0};   // unmasked rows, unmasked last-step rows
   float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
   if (dpred) {
-    const float ms_all = counts[0], ms_last = counts[1];
+    const float ms_all = counts[1], ms_last = counts[2];
     c_all = (1.f - p1) * (1.f - p2) / (ms_all * (float)O);
     c_last = (1.f - p1) * p2 / (ms_last * (float)O);
     c_tar = p1 / ms_last;
@@ -870,15 +931,17 @@ __device__ __forceinline__ void uq_loss_final(int nblk, const double* __restrict
   for (int i = 0; i < 8; ++i) s[i] = warp_sum(s[i]);
   if (lane != 0) return;
   if (counts_out) {
-    counts_out[0] = (float)s[4];
-    counts_out[1] = (float)s[5];
+    counts_out[0] = (float)B;
+    counts_out[1] = (float)s[4];
+    counts_out[2] = (float)s[5];
   }
-  const double ms_all = counts_in ? (double)counts_in[0] : s[4];
-  const double ms_last = counts_in ? (double)counts_in[1] : s[5];
+  const double Bd = counts_in ? (double)counts_in[0] : (double)B;
+  const double ms_all = counts_in ? (double)counts_in[1] : s[4];
+  const double ms_last = counts_in ? (double)counts_in[2] : s[5];
   const double uq0 = s[0] / ms_last, uq1 = s[1] / (ms_last * O), uq2 = s[2] / (ms_all * O);
   vals3[0] = (float)(p1 * uq0 + (1.0 - p1) * (p2 * uq1 + (1.0 - p2) * uq2));
   vals3[1] = (float)uq0;
-  vals3[2] = (float)(s[3] / (double)B);
+  vals3[2] = (float)(s[3] / Bd);
   if (out_loss) *out_loss = vals3[0];
   if (out_uq0) *out_uq0 = vals3[1];
   if (out_mse0) *out_mse0 = vals3[2];

@@ -612,6 +612,18 @@ int32_t lfmq_mask_count(lfmq_handle h, const float* y, int32_t B, float* out_dev
   return mask_count((cudaStream_t)stream, B, h->cfg.seq_len, h->cfg.n_outputs, y, out_dev, h->tickets);
 }
 
+int32_t lfmq_mask_count_uq(lfmq_handle h, const float* y, int32_t B, float* out_dev, void* stream) {
+  RUN(check_batch(h, B));
+  if (!y || !out_dev) {
+    LFMQ_SET_ERR("lfmq_mask_count_uq: null pointer");
+    return LFMQ_ERR_ARG;
+  }
+  const lfmq_config& c = h->cfg;
+  return uq_loss_grad((cudaStream_t)stream, B, c.seq_len, c.n_outputs, nullptr, nullptr, nullptr, y, nullptr,
+                      c.target_idx, c.target_lambda, c.rnn_lambda, nullptr, nullptr, nullptr, nullptr, nullptr, out_dev,
+                      h->scratch);
+}
+
 int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, int64_t row0, int64_t step,
                       const float* denom_dev, void* stream) {
   RUN(check_batch(h, B));
@@ -627,16 +639,16 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
   const lfmq_config& c = h->cfg;
   h->last_step = step;
   h->last_row0 = row0;
-  if (c.uq) {
-    if (denom_dev) {
-      LFMQ_SET_ERR("lfmq_backward: data-parallel denominators are not built for uq handles");
-      return LFMQ_ERR_UNSUPPORTED;
-    }
+  if (c.uq) {      // denom_dev: the three counts of lfmq_mask_count_uq, summed over the ranks
     float* t = h->grads + h->n_train;
     RUN(forward_fp32(h, x, B, row0, step, h->preds, h->var, s));
-    RUN(uq_loss_grad(s, B, c.seq_len, c.n_outputs, nullptr, nullptr, nullptr, y, nullptr, c.target_idx, c.target_lambda,
-                     c.rnn_lambda, nullptr, nullptr, nullptr, nullptr, nullptr, h->denom, h->scratch));
-    RUN(uq_loss_grad(s, B, c.seq_len, c.n_outputs, h->preds, h->var, h->apre, y, h->denom, c.target_idx, c.target_lambda,
+    const float* counts = denom_dev;
+    if (!counts) {
+      RUN(uq_loss_grad(s, B, c.seq_len, c.n_outputs, nullptr, nullptr, nullptr, y, nullptr, c.target_idx,
+                       c.target_lambda, c.rnn_lambda, nullptr, nullptr, nullptr, nullptr, nullptr, h->denom, h->scratch));
+      counts = h->denom;
+    }
+    RUN(uq_loss_grad(s, B, c.seq_len, c.n_outputs, h->preds, h->var, h->apre, y, counts, c.target_idx, c.target_lambda,
                      c.rnn_lambda, h->dpred, h->da, t, t + 4, t + 1, nullptr, h->scratch));
     return backward_fp32(h, x, B, s);
   }
@@ -794,7 +806,7 @@ int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float
       LFMQ_SET_ERR("lfmq_chain_loss: null handle");
       return LFMQ_ERR_ARG;
     }
-    l2.p[i] = stages[i]->scalars + 10;      // two spare floats of the handle's scalar block
+    l2.p[i] = stages[i]->scalars + 12;      // two spare floats of the handle's scalar block (denom uses 8..10)
     RUN(lfmq_loss(stages[i], preds[i], y[i], B, l2.p[i], stream));
     w.w[i] = weights[i];
   }
@@ -828,8 +840,10 @@ int32_t lfmq_chain_loss_uq(const lfmq_handle* stages, int32_t n_stages, const fl
 namespace {
 // lfmq_chain_backward of a uq chain (train.py:201-218): every stage's forward, then one loss pass over all stages for
 // the mask counts and one for the losses and w_s * dLoss_s / d(pred_s, variance pre-activation_s).
+// denom (nullable): every stage's three counts (lfmq_chain_mask_count), summed over the data-parallel ranks.
 int chain_forward_loss_uq(const lfmq_handle* st, int S, const float* x, const float* const* y, const float* weights,
-                          int B, int64_t row0, int64_t step, float* work, float* loss_out_dev, cudaStream_t s) {
+                          int B, int64_t row0, int64_t step, const float* denom, float* work, float* loss_out_dev,
+                          cudaStream_t s) {
   const lfmq_config& c0 = st[0]->cfg;
   const int T = c0.seq_len, F = c0.n_inputs, O = c0.n_outputs;
   const size_t slot = (size_t)B * T * F;
@@ -846,11 +860,11 @@ int chain_forward_loss_uq(const lfmq_handle* st, int S, const float* x, const fl
     }
     RUN(forward_fp32(h, in, B, row0, step, h->preds, h->var, s));
     a.y.p[i] = const_cast<float*>(y[i]);
-    a.counts.p[i] = h->denom;
+    a.counts.p[i] = denom ? const_cast<float*>(denom) + 3 * i : h->denom;
     a.w.w[i] = weights[i];
   }
   float* scratch = st[0]->scratch;
-  RUN(chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, nullptr, scratch));
+  if (!denom) RUN(chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, nullptr, scratch));
   for (int i = 0; i < S; ++i) {
     a.pred.p[i] = st[i]->preds;
     a.var.p[i] = st[i]->var;
@@ -867,9 +881,10 @@ int chain_forward_loss_uq(const lfmq_handle* st, int S, const float* x, const fl
 }
 }  // namespace
 
-int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
-                            const float* weights, int32_t B, int64_t row0, int64_t step, float* work,
-                            float* loss_out_dev, void* stream) {
+namespace {
+int chain_backward(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
+                   const float* weights, int32_t B, int64_t row0, int64_t step, const float* denom, float* work,
+                   float* loss_out_dev, void* stream) {
   RUN(chain_check(stages, n_stages, B, true));
   if (!x || !y || !weights || !work) {
     LFMQ_SET_ERR("lfmq_chain_backward: null pointer");
@@ -890,7 +905,7 @@ int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const f
       return LFMQ_ERR_ARG;
     }
   if (c0.uq) {
-    RUN(chain_forward_loss_uq(stages, S, x, y, weights, B, row0, step, work, loss_out_dev, s));
+    RUN(chain_forward_loss_uq(stages, S, x, y, weights, B, row0, step, denom, work, loss_out_dev, s));
     for (int i = 0; i < S; ++i) dpred.p[i] = stages[i]->dpred;      // variances never feed forward: no dvar feedback
   }
   const float* in = x;
@@ -905,10 +920,11 @@ int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const f
       in = next;
     }
     RUN(forward_fp32(h, in, B, row0, step, h->preds, nullptr, s));
-    RUN(mask_count(s, B, T, O, y[i], h->denom, h->tickets));
+    const float* d = denom ? denom + 3 * i : h->denom;      // {B, mask_count} lead the stage's three counts
+    if (!denom) RUN(mask_count(s, B, T, O, y[i], h->denom, h->tickets));
     float* tail = h->grads + h->n_train;
-    RUN(loss_grad(s, B, T, O, h->preds, y[i], h->denom, c.target_idx, c.target_lambda, c.rnn_lambda, h->dpred, tail,
-                  nullptr, h->scratch));
+    RUN(loss_grad(s, B, T, O, h->preds, y[i], d, c.target_idx, c.target_lambda, c.rnn_lambda, h->dpred, tail, nullptr,
+                  h->scratch));
     if (weights[i] != 1.0f) RUN(scale_inplace(s, (long)B * T * O, h->dpred, weights[i]));
     dpred.p[i] = h->dpred;
     l2.p[i] = tail;
@@ -922,6 +938,103 @@ int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const f
     RUN(chain_scatter_dx(s, B, T, F, O, i, dx, dpred));
   }
   return backward_fp32(stages[0], x, B, s);
+}
+
+// the handles whose gradients one flat vector carries: all trainable, all of one kind (uq or point estimate)
+int pack_check(const lfmq_handle* st, int32_t S, const char* fn, lfmq::GradPack* p, int64_t* total) {
+  if (!st || S < 1 || S > lfmq::LFMQ_MAX_STAGES) {
+    LFMQ_SET_ERR("%s: n_stages %d outside [1, %d]", fn, S, lfmq::LFMQ_MAX_STAGES);
+    return LFMQ_ERR_ARG;
+  }
+  int64_t off = 0;
+  for (int i = 0; i < S; ++i) {
+    if (!st[i] || st[i]->cfg.forward_only || st[i]->cfg.uq != st[0]->cfg.uq) {
+      LFMQ_SET_ERR("%s: stage %d is null, forward_only or of another kind than stage 0", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+    p->g[i] = st[i]->grads;
+    p->n[i] = st[i]->n_train;
+    p->off[i] = off;
+    off += st[i]->n_train + (st[0]->cfg.uq ? 3 : 2);
+  }
+  p->ntail = st[0]->cfg.uq ? 3 : 2;
+  *total = off;
+  return 0;
+}
+}  // namespace
+
+int32_t lfmq_chain_backward(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
+                            const float* weights, int32_t B, int64_t row0, int64_t step, float* work,
+                            float* loss_out_dev, void* stream) {
+  return chain_backward(stages, n_stages, x, y, weights, B, row0, step, nullptr, work, loss_out_dev, stream);
+}
+
+int32_t lfmq_chain_backward_dp(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
+                               const float* weights, int32_t B, int64_t row0, int64_t step, const float* denom_dev,
+                               float* work, float* loss_out_dev, void* stream) {
+  if (!denom_dev) {
+    LFMQ_SET_ERR("lfmq_chain_backward_dp: denom_dev == NULL (lfmq_chain_backward takes this batch's own counts)");
+    return LFMQ_ERR_ARG;
+  }
+  return chain_backward(stages, n_stages, x, y, weights, B, row0, step, denom_dev, work, loss_out_dev, stream);
+}
+
+int32_t lfmq_chain_mask_count(const lfmq_handle* stages, int32_t n_stages, const float* const* y, int32_t B,
+                              float* out_dev, void* stream) {
+  RUN(chain_check(stages, n_stages, B, false));
+  if (!y || !out_dev) {
+    LFMQ_SET_ERR("lfmq_chain_mask_count: null pointer");
+    return LFMQ_ERR_ARG;
+  }
+  lfmq::ChainUqArgs a{};
+  for (int i = 0; i < n_stages; ++i) {
+    if (!y[i]) {
+      LFMQ_SET_ERR("lfmq_chain_mask_count: y[%d] == NULL", i);
+      return LFMQ_ERR_ARG;
+    }
+    a.y.p[i] = const_cast<float*>(y[i]);
+    a.counts.p[i] = out_dev + 3 * i;
+  }
+  const lfmq_config& c = stages[0]->cfg;
+  return chain_uq_loss_grad((cudaStream_t)stream, n_stages, B, c.seq_len, c.n_outputs, a, c.target_idx, c.target_lambda,
+                            c.rnn_lambda, nullptr, stages[0]->scratch);
+}
+
+int32_t lfmq_chain_grad_pack_size(const lfmq_handle* stages, int32_t n_stages, int64_t* n_elems) {
+  lfmq::GradPack p{};
+  int64_t n = 0;
+  RUN(pack_check(stages, n_stages, "lfmq_chain_grad_pack_size", &p, &n));
+  if (!n_elems) {
+    LFMQ_SET_ERR("lfmq_chain_grad_pack_size: n_elems == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  *n_elems = n;
+  return LFMQ_OK;
+}
+
+int32_t lfmq_chain_grad_pack(const lfmq_handle* stages, int32_t n_stages, float* flat, void* stream) {
+  lfmq::GradPack p{};
+  int64_t n = 0;
+  RUN(pack_check(stages, n_stages, "lfmq_chain_grad_pack", &p, &n));
+  if (!flat || (reinterpret_cast<uintptr_t>(flat) & 15) != 0) {
+    LFMQ_SET_ERR("lfmq_chain_grad_pack: flat must be a 16-byte aligned device pointer");
+    return LFMQ_ERR_ARG;
+  }
+  return grad_pack((cudaStream_t)stream, n_stages, p, flat, false, lfmq::ChainWeights{}, nullptr);
+}
+
+int32_t lfmq_chain_grad_unpack(const lfmq_handle* stages, int32_t n_stages, const float* flat, const float* weights,
+                               float* loss_out_dev, void* stream) {
+  lfmq::GradPack p{};
+  int64_t n = 0;
+  RUN(pack_check(stages, n_stages, "lfmq_chain_grad_unpack", &p, &n));
+  if (!flat || (reinterpret_cast<uintptr_t>(flat) & 15) != 0 || (loss_out_dev && !weights)) {
+    LFMQ_SET_ERR("lfmq_chain_grad_unpack: flat must be a 16-byte aligned device pointer; loss_out_dev needs weights");
+    return LFMQ_ERR_ARG;
+  }
+  lfmq::ChainWeights w{};
+  for (int i = 0; i < n_stages && weights; ++i) w.w[i] = weights[i];
+  return grad_pack((cudaStream_t)stream, n_stages, p, const_cast<float*>(flat), true, w, loss_out_dev);
 }
 
 int32_t lfmq_chain_apply(const lfmq_handle* stages, int32_t n_stages, float lr, int64_t iteration, void* stream) {

@@ -1,6 +1,7 @@
 """Data parallelism over the company-batch axis (SURVEY section 8e): host-side plumbing shared by
-ForecasterEngine.train_step_dp, bench.py and the gloo tests.  One process per GPU; exactly ONE collective on the
-data path per step -- the SUM all-reduce of the flat gradient (+ its loss / mse tail) over NCCL."""
+ForecasterEngine.train_step_dp, ForecastChainEngine.train_step_dp, bench.py and the gloo tests.  One process per GPU;
+exactly ONE collective on the data path per step -- the SUM all-reduce of the flat gradient (+ its loss / mse tail)
+over NCCL; for chains and uq handles, of the packed vector of every stage's gradients and loss tail."""
 from __future__ import absolute_import, division, print_function
 
 
@@ -26,6 +27,22 @@ def allreduce_flat_gradient(flat_grads, n_trainable, dist):
     clip_by_global_norm, the optimizer and MaxNorm then run redundantly on every rank on the reduced gradient."""
     dist.all_reduce(flat_grads[:n_trainable + 2], op=dist.ReduceOp.SUM)
     return flat_grads
+
+
+def global_stage_counts(local_counts, dist):
+    """Multi-step forecasts and RNNUqRangeEstimate: every forecast stage's {B, unmasked rows, unmasked last-step rows}
+    ([S, 3], or the 3 counts of one uq handle) -> their sums over the ranks, in ONE all-reduce of the small vector.
+    Each stage's loss takes its own denominators (losses.py:47-51,159-177); done once per batch when it is built."""
+    assert local_counts.shape[-1] == 3, tuple(local_counts.shape)
+    return global_denominators(local_counts, dist)
+
+
+def allreduce_packed(flat, dist):
+    """The single data-path collective of a chain or uq step: SUM over ranks of the packed vector, every stage's
+    gradients followed by its loss tail -- {loss, mse_0}, or {uq_loss, mse_0, uq_loss_last_tar} on uq handles
+    (ForecastChainEngine.pack).  grad_norm and clip_scale are not in it: the apply computes them afterwards."""
+    dist.all_reduce(flat, op=dist.ReduceOp.SUM)
+    return flat
 
 
 def init_from_env():

@@ -81,6 +81,7 @@ class ForecasterEngine(object):
         self.params = self._view('lfmq_params_ptr', self.n_total)
         self.grads = self._view('lfmq_grads_ptr', self.n_trainable + 8)   # tail: loss, mse_0, grad_norm, clip_scale, uq_loss_last_tar
         self._denom = torch.zeros(2, dtype=torch.float32, device=self.device)
+        self._dp = None
 
     def _view(self, fn, n):
         p = C.c_void_p(0)
@@ -188,6 +189,19 @@ class ForecasterEngine(object):
         N.check(self.lib.lfmq_mask_count(self.handle, _ptr(y), y.shape[0], _ptr(out), _stream()))
         return out
 
+    def mask_count_uq(self, y):
+        """Device {B, unmasked rows, unmasked last-step rows}: the denominators of the uq loss (losses.py:179-284)."""
+        out = torch.empty(3, dtype=torch.float32, device=y.device)
+        N.check(self.lib.lfmq_mask_count_uq(self.handle, _ptr(y), y.shape[0], _ptr(out), _stream()))
+        return out
+
+    def loss_counts(self, y):
+        """The loss denominators of one batch that data parallelism all-reduces: mask_count_uq on a uq engine, else
+        mask_count.  y None (a rank without rows): zeros of the same length."""
+        if y is None:
+            return torch.zeros(3 if self.uq else 2, dtype=torch.float32, device=self.device)
+        return self.mask_count_uq(y) if self.uq else self.mask_count(y)
+
     def backward(self, x, y, step=0, row0=0, denom=None):
         B = self._check_x(x)
         assert y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and tuple(y.shape) == (B, self.T, self.O)
@@ -207,9 +221,19 @@ class ForecasterEngine(object):
 
     def train_step_dp(self, x, y, step, lr, row0, denom_global):
         """Data-parallel step: local BPTT with global denominators, ONE NCCL all-reduce over the flat
-        gradient (+ loss/mse tail), then the replicated clip + optimizer (SURVEY 8e)."""
+        gradient (+ loss/mse tail), then the replicated clip + optimizer (SURVEY 8e).
+        uq engine: the gradient and {uq_loss, mse_0, uq_loss_last_tar} travel as one packed vector (a chain of one
+        stage, lfmq_chain_grad_pack); x None joins the step without rows.  Returns the global
+        {uq_loss_last_tar, mse_0}, as train_step."""
         import torch.distributed as dist
         from .dp import allreduce_flat_gradient
+        if self.uq:
+            if self._dp is None:
+                self._dp = _PackedStep([self], [1.0])
+            self._dp.step(lambda: self.backward(x, y, step=step, row0=row0, denom=denom_global), x is not None, dist)
+            self.apply(lr, step)
+            t = self.grads[self.n_trainable:]
+            return torch.stack([t[4], t[1]])
         self.backward(x, y, step=step, row0=row0, denom=denom_global)
         allreduce_flat_gradient(self.grads, self.n_trainable, dist)
         self.apply(lr, step)
@@ -234,6 +258,32 @@ class ForecasterEngine(object):
         return int(self.lib.lfmq_launch_count())
 
 
+class _PackedStep(object):
+    """The collective of a data-parallel step over the handles of a chain (or one uq handle): the backward fills every
+    stage's gradient buffer, one launch packs them with their reduced loss tails into one contiguous vector, ONE SUM
+    all-reduce, one launch scatters it back (and forms the weighted losses).  The apply then runs on every rank."""
+
+    def __init__(self, engines, weights):
+        e0 = engines[0]
+        self.lib, self.S = e0.lib, len(engines)
+        self.handles = (C.c_void_p * self.S)(*[e.handle.value for e in engines])
+        self.w = (C.c_float * self.S)(*weights)
+        n = C.c_int64(0)
+        N.check(self.lib.lfmq_chain_grad_pack_size(self.handles, self.S, C.byref(n)))
+        self.flat = torch.empty(n.value, dtype=torch.float32, device=e0.device)
+
+    def step(self, backward, has_rows, dist, loss_out=None):
+        from .dp import allreduce_packed
+        if has_rows:
+            backward()
+            N.check(self.lib.lfmq_chain_grad_pack(self.handles, self.S, _ptr(self.flat), _stream()))
+        else:
+            self.flat.zero_()
+        allreduce_packed(self.flat, dist)
+        N.check(self.lib.lfmq_chain_grad_unpack(self.handles, self.S, _ptr(self.flat), self.w, _ptr(loss_out),
+                                                _stream()))
+
+
 class ForecastChainEngine(object):
     """forecast_steps > 1 (scripts/models/point_estimate/rnn_point_estimate.py:109-150): stage 0 is the trunk, every
     further stage one more recurrent layer + BatchNormalization + Dropout + Dense on the shifted input window.  One
@@ -254,6 +304,7 @@ class ForecastChainEngine(object):
         self._handles = (C.c_void_p * self.S)(*[e.handle.value for e in self.stages])
         self._w = (C.c_float * self.S)(*self.weights)
         self._work = None
+        self._dp = None
         # Keras names: the extra layer of stage s is lstm_{L+s} / batch_normalization_{L+s-1} / OUTPUT_{s+1}
         self.specs = []            # (stage, name, shape, offset in the stage's flat vector, trainable)
         cell = kw.get('rnn_cell', 'lstm')
@@ -323,6 +374,68 @@ class ForecastChainEngine(object):
 
     def apply(self, lr, iteration):
         N.check(self.lib.lfmq_chain_apply(self._handles, self.S, float(lr), int(iteration), _stream()))
+
+    # ---- data parallelism over the company-batch axis --------------------------------------------
+    def mask_count(self, ys):
+        """Device [S, 3]: every stage's {B, unmasked rows, unmasked last-step rows} (lfmq_chain_mask_count), the
+        counts one batch all-reduces (dp.global_stage_counts).  ys None (a rank without rows): zeros."""
+        if ys is None:
+            return torch.zeros(self.S, 3, dtype=torch.float32, device=self.device)
+        assert len(ys) == self.S
+        out = torch.empty(self.S, 3, dtype=torch.float32, device=self.device)
+        B = ys[0].shape[0]
+        N.check(self.lib.lfmq_chain_mask_count(self._handles, self.S, self._ptrs([y.contiguous() for y in ys]), B,
+                                               _ptr(out), _stream()))
+        return out
+
+    def backward_dp(self, x, ys, denoms, step=0, row0=0, out=None):
+        """backward with the global batch's stage counts (device [S, 3]) as the loss denominators; every stage's tail
+        and `out` then hold this shard's contributions."""
+        B = self.stages[0]._check_x(x)
+        assert len(ys) == self.S and denoms.is_cuda and denoms.numel() == 3 * self.S
+        for y in ys:
+            assert y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and tuple(y.shape) == (B, self.T, self.O)
+        if out is None:
+            out = torch.empty(3 if self.uq else 2, dtype=torch.float32, device=x.device)
+        N.check(self.lib.lfmq_chain_backward_dp(self._handles, self.S, _ptr(x), self._ptrs(ys), self._w, B, row0, step,
+                                                _ptr(denoms.contiguous()), _ptr(self._workbuf(B)), _ptr(out),
+                                                _stream()))
+        return out
+
+    def _packed(self):
+        if self._dp is None:
+            self._dp = _PackedStep(self.stages, self.weights)
+        return self._dp
+
+    @property
+    def n_packed(self):
+        """Length of the vector the step all-reduces: sum_s (n_trainable_s + 2), + 3 on a uq chain."""
+        return self._packed().flat.numel()
+
+    def pack(self, flat=None):
+        """Every stage's gradients and reduced loss tail as one contiguous device vector (one launch)."""
+        p = self._packed()
+        flat = p.flat if flat is None else flat
+        assert flat.is_cuda and flat.dtype == torch.float32 and flat.numel() == p.flat.numel() and flat.is_contiguous()
+        N.check(self.lib.lfmq_chain_grad_pack(self._handles, self.S, _ptr(flat), _stream()))
+        return flat
+
+    def unpack(self, flat, out=None):
+        """The inverse scatter; `out` (optional) receives the weighted losses, as backward's."""
+        assert flat.is_cuda and flat.dtype == torch.float32 and flat.numel() == self.n_packed and flat.is_contiguous()
+        N.check(self.lib.lfmq_chain_grad_unpack(self._handles, self.S, _ptr(flat), self._w, _ptr(out), _stream()))
+        return out
+
+    def train_step_dp(self, x, ys, step, lr, row0, denoms):
+        """Data-parallel step of the whole graph: local BPTT of this rank's rows with the global stage counts, ONE
+        all-reduce of the packed vector, then the joint clip, optimizer and MaxNorm on every rank.  x None joins the
+        step without rows.  Returns the global {loss, mse}; uq chain {uq_loss_last_tar, mse}, as train_step."""
+        import torch.distributed as dist
+        out = torch.empty(3 if self.uq else 2, dtype=torch.float32, device=self.device)
+        self._packed().step(lambda: self.backward_dp(x, ys, denoms, step=step, row0=row0), x is not None, dist,
+                            loss_out=out)
+        self.apply(lr, step)
+        return out[1:] if self.uq else out
 
     def train_step(self, x, ys, step, lr):
         """One Train._train_step_point over the S-output model; device tensor {loss, mse}.  uq chain: one

@@ -81,6 +81,14 @@ class NativeChainForecaster(object):
         assert isinstance(targets, (list, tuple)), 'targets must be the list of forecast_steps targets (train.py:188)'
         return self.engine.train_step(self._to_device(inp), [self._to_device(t) for t in targets], iteration, lr)
 
+    def train_step_dp(self, x, ys, step, lr, row0, denoms):
+        """train_step under data parallelism: this rank's rows (x None: none) with the global stage counts `denoms`
+        (dp.global_stage_counts), one all-reduce, the replicated apply; returns the global values train_step does."""
+        if x is not None:
+            assert isinstance(ys, (list, tuple)), 'ys must be the list of forecast_steps targets'
+            x, ys = self._to_device(x), [self._to_device(t) for t in ys]
+        return self.engine.train_step_dp(x, ys, step, lr, row0, denoms)
+
     def reset_states(self):
         return None
 

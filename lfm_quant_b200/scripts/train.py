@@ -35,14 +35,13 @@ class Train(object):
         from .. import dp as _dp
         self.rank, self.world = _dp.init_from_env()
         self.model = Model(self.config, self.dataset).get_model()
-        if self.world > 1 and self.config.forecast_steps > 1:
-            raise NotImplementedError('data parallelism is built for forecast_steps = 1')
-        if self.world > 1:                       # one set of initial weights: rank 0's
+        if self.world > 1:                       # one set of initial weights: rank 0's, for every forecast stage
             import torch
             import torch.distributed as dist
-            flat = torch.from_numpy(self.model.engine.get_flat()).to(self.model.engine.device)
-            dist.broadcast(flat, 0)
-            self.model.engine.set_flat(flat.cpu().numpy())
+            for eng in getattr(self.model.engine, 'stages', [self.model.engine]):
+                flat = torch.from_numpy(eng.get_flat()).to(eng.device)
+                dist.broadcast(flat, 0)
+                eng.set_flat(flat.cpu().numpy())
         self.target_index = self.dataset.target_index
         self.optimizer = Optimizers(self.config).get_optimizer()
         self.optimizer.bind(self.model)
@@ -73,19 +72,27 @@ class Train(object):
         self._valid_batches = [self.dataset.get_batch(*items) for items in self.valid_set]
 
     def _build_train_batch(self, items):
-        """(inp, target, metadata[, row0, global denominators]) of one global batch; the shard of this rank under DP."""
+        """(inp, target, metadata[, row0, global denominators]) of one global batch; the shard of this rank under DP.
+        The denominators: {B, mask count} of the point estimate; the uq loss's {B, mask count, last-step mask count};
+        with forecast_steps > 1 those three per forecast stage."""
         if self.world == 1:
             return self.dataset.get_batch(*items)
         import torch.distributed as dist
         from .. import dp as _dp
         inp_idx, tar_idx, meta, row0 = _dp.shard_batch_indices(items[0], items[1], items[2], self.rank, self.world)
         eng = self.model.engine
-        if len(inp_idx) == 0:                    # fewer windows than ranks: this rank only joins the collectives
+        x = y = md = None
+        if len(inp_idx) > 0:                     # else fewer windows than ranks: this rank only joins the collectives
+            x, y, md = self.dataset.get_batch(inp_idx, tar_idx, meta)
+        if self.config.forecast_steps > 1:
+            denom = _dp.global_stage_counts(eng.mask_count(None if y is None else self._step_targets(y)), dist)
+        elif self.config.UQ:
+            denom = _dp.global_stage_counts(eng.loss_counts(y), dist)
+        elif y is None:
             import torch
             denom = _dp.global_denominators(torch.zeros(2, dtype=torch.float32, device=eng.device), dist)
-            return (None, None, None, row0, denom)
-        x, y, md = self.dataset.get_batch(inp_idx, tar_idx, meta)
-        denom = _dp.global_denominators(eng.mask_count(y), dist)     # loss denominators are global (losses.py:87,90,131-135)
+        else:                                    # loss denominators are global (losses.py:87,90,131-135)
+            denom = _dp.global_denominators(eng.mask_count(y), dist)
         return (x, y, md, row0, denom)
 
     def train(self):
@@ -110,8 +117,7 @@ class Train(object):
             for (batch_n, cur_batch) in enumerate(self._batches):
                 inp, target = cur_batch[0], cur_batch[1]
                 if self.world > 1:
-                    mse = self._train_step_point_dp(cur_batch)
-                    uq_loss = None
+                    uq_loss, mse = self._train_step_dp(cur_batch)
                 elif self.config.UQ:
                     uq_loss, mse = self._train_step_uq_range(inp, target)
                 else:
@@ -156,7 +162,7 @@ class Train(object):
         """train.py:178-199 as one fused native step; returns the step's mse_0 as a device scalar."""
         assert not self.config.UQ
         lr = self.optimizer.current_lr()
-        out = self.model.train_step(inp, targets, lr, self.optimizer.iterations)
+        out = self.model.train_step(inp, self._step_targets(targets), lr, self.optimizer.iterations)
         self.optimizer.iterations += 1
         return out[1]
 
@@ -179,6 +185,23 @@ class Train(object):
             out = eng.train_step_dp(inp, targets, it, lr, row0, denom)
         self.optimizer.iterations += 1
         return out[1]
+
+    def _train_step_dp(self, cur_batch):
+        """One data-parallel step of any model: (uq_loss_last_tar or None, mse), both global device scalars.  The point
+        estimate reduces its flat gradient in place; RNNUqRangeEstimate and multi-step forecasts all-reduce the packed
+        vector of every stage's gradients and loss tail (ForecastChainEngine.train_step_dp)."""
+        if self.config.forecast_steps == 1 and not self.config.UQ:
+            return None, self._train_step_point_dp(cur_batch)
+        inp, targets, _, row0, denom = cur_batch
+        lr = self.optimizer.current_lr()
+        it = self.optimizer.iterations
+        if self.config.forecast_steps > 1:
+            out = self.model.train_step_dp(inp, None if inp is None else self._step_targets(targets), it, lr, row0,
+                                           denom)
+        else:
+            out = self.model.engine.train_step_dp(inp, targets, it, lr, row0, denom)
+        self.optimizer.iterations += 1
+        return (out[0] if self.config.UQ else None), out[1]
 
     def _step_targets(self, targets):
         """The list of forecast_steps targets of one batch.  The dataset materialises one target window per input window
@@ -226,7 +249,7 @@ class Train(object):
         if not self._valid_batches:
             return None, float('nan'), float('nan')
         preds = [self.model.predict_device(cur_batch[0]) for cur_batch in self._valid_batches]
-        targets = [cur_batch[1] for cur_batch in self._valid_batches]
+        targets = [self._step_targets(cur_batch[1]) for cur_batch in self._valid_batches]
         if self.config.forecast_steps == 1:              # preds, targets need to be lists (train.py:291-294)
             preds = [[p] for p in preds]
             targets = [[t] for t in targets]
