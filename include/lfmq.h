@@ -13,7 +13,8 @@
  *   - all tensors are dense row-major fp32 unless stated; x is [B, T, F], y/preds are [B, T, O].
  *   - every call that touches the device takes a cudaStream_t (as void*) and is asynchronous.
  *   - return value: 0 on success, else an LFMQ_ERR_* code; lfmq_last_error() gives the message
- *     (thread-local).  One handle per process/GPU; a handle is not thread-safe.
+ *     (thread-local).  A handle is not thread-safe; different handles may run at the same time from different host
+ *     threads on different streams, each with a device share (lfmq_set_device_share) when they share a GPU.
  */
 #ifndef LFMQ_H_
 #define LFMQ_H_
@@ -91,6 +92,17 @@ int32_t lfmq_workspace_bytes(const lfmq_config* cfg, uint64_t* bytes);
  * (model_utils/initializers.py:14-24) uploads weights with lfmq_set_params. */
 int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_bytes, lfmq_handle* out);
 int32_t lfmq_destroy(lfmq_handle h);
+
+/* Handles that run concurrently on one GPU (ensembles: runtime/model_execution.py:154-199 trains and predicts N members).
+ * Some launches of the general tensor-core path are persistent: their CTAs wait for each other at a barrier in global
+ * memory, which needs all of them resident at once.  lfmq_set_device_share(h, num, den) lets such a launch of h count on
+ * num/den of the SMs only (fewer CTAs than that budget, else the steps are launched one by one).  Default 1/1, the whole
+ * device.  Give every handle that may run at the same time as others on the same GPU a share, with the shares summing
+ * to at most 1; launches that do not wait across CTAs need none.  Host-only; takes effect from the next call. */
+int32_t lfmq_set_device_share(lfmq_handle h, int32_t num, int32_t den);
+/* The CTA budget of one persistent launch under a share (host arithmetic, no device): sm_count * ctas_per_sm for the
+ * whole device, else floor(sm_count * num / den), one CTA per SM. */
+int32_t lfmq_persistent_cta_budget(int32_t sm_count, int32_t ctas_per_sm, int32_t num, int32_t den, int64_t* budget);
 
 /* model.trainable_variables / model.weights (train.py:192,198): tensors are listed in Keras order,
  * trainable ones first: per layer lstm_l/{kernel,recurrent_kernel,bias} (gru_l/... with bias [2][3H] for LFMQ_CELL_GRU), batch_normalization[_k]/{gamma,beta};

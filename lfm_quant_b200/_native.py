@@ -53,6 +53,8 @@ SYMBOLS = {
     'lfmq_workspace_bytes': (C.c_int32, [C.POINTER(LfmqConfig), C.POINTER(C.c_uint64)]),
     'lfmq_create': (C.c_int32, [C.POINTER(LfmqConfig), _P, C.c_uint64, C.POINTER(_P)]),
     'lfmq_destroy': (C.c_int32, [_P]),
+    'lfmq_set_device_share': (C.c_int32, [_P, C.c_int32, C.c_int32]),
+    'lfmq_persistent_cta_budget': (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     'lfmq_param_count': (C.c_int32, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     'lfmq_param_spec': (C.c_int32, [_P, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int32),
                                      C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),

@@ -5,10 +5,12 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <atomic>
+
 namespace lfmq {
 
 extern thread_local char g_err[512];
-extern long long g_launches;
+extern std::atomic<long long> g_launches;   // handles may launch from several host threads at once
 
 #define LFMQ_SET_ERR(...) snprintf(::lfmq::g_err, sizeof(::lfmq::g_err), __VA_ARGS__)
 

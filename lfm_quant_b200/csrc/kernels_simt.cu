@@ -9,7 +9,7 @@
 namespace lfmq {
 
 thread_local char g_err[512] = {0};
-long long g_launches = 0;
+std::atomic<long long> g_launches{0};
 
 static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 

@@ -502,6 +502,26 @@ int32_t lfmq_param_spec(lfmq_handle h, int32_t index, char* name, int32_t name_c
   return LFMQ_OK;
 }
 
+int32_t lfmq_set_device_share(lfmq_handle h, int32_t num, int32_t den) {
+  if (!h || num < 1 || den < num) {
+    LFMQ_SET_ERR("lfmq_set_device_share: need a handle and 0 < num <= den (got %d/%d)", num, den);
+    return LFMQ_ERR_ARG;
+  }
+  h->tc.share_num = num;
+  h->tc.share_den = den;
+  return LFMQ_OK;
+}
+
+int32_t lfmq_persistent_cta_budget(int32_t sm_count, int32_t ctas_per_sm, int32_t num, int32_t den, int64_t* budget) {
+  if (sm_count < 1 || ctas_per_sm < 1 || num < 1 || den < num || !budget) {
+    LFMQ_SET_ERR("lfmq_persistent_cta_budget: need sm_count, ctas_per_sm >= 1 and 0 < num <= den (got %d, %d, %d/%d)",
+                 sm_count, ctas_per_sm, num, den);
+    return LFMQ_ERR_ARG;
+  }
+  *budget = lfmq::persistent_cta_budget(sm_count, ctas_per_sm, num, den);
+  return LFMQ_OK;
+}
+
 int32_t lfmq_params_ptr(lfmq_handle h, float** dev) {
   if (!h || !dev) return LFMQ_ERR_ARG;
   *dev = h->params;

@@ -1277,11 +1277,14 @@ int gen_init(TcState& st, const lfmq_config& c) {
 }
 
 // Persistent step launches need every CTA of the launch(es) running at once (they meet at a grid-wide barrier).
-// `n_concurrent` launches of `ctas` CTAs each, `per_sm` resident CTAs of that instantiation per SM.  LFMQ_GEN_PERSIST=0
-// turns the mode off (one launch per time step, chained with programmatic dependent launch).
-static bool gen_can_persist(const GenImpl& m, long ctas, int n_concurrent, int per_sm, int n_steps) {
+// `n_concurrent` launches of `ctas` CTAs each, `per_sm` resident CTAs of that instantiation per SM, within the handle's
+// device share (persistent_cta_budget).  LFMQ_GEN_PERSIST=0 turns the mode off (one launch per time step, chained with
+// programmatic dependent launch).
+static bool gen_can_persist(const TcState& st, long ctas, int n_concurrent, int per_sm, int n_steps) {
   static const bool on = !(getenv("LFMQ_GEN_PERSIST") && atoi(getenv("LFMQ_GEN_PERSIST")) == 0);
-  return on && n_steps > 1 && m.gbar != nullptr && ctas * n_concurrent <= (long)device_sm_count() * per_sm &&
+  const GenImpl& m = *st.gen;
+  return on && n_steps > 1 && m.gbar != nullptr &&
+         ctas * n_concurrent <= persistent_cta_budget(device_sm_count(), per_sm, st.share_num, st.share_den) &&
          m.gbar_next + ctas * n_concurrent <= GBAR_N;
 }
 
@@ -1366,7 +1369,7 @@ static int gen_run_trunk(TcState& st, const lfmq_config& c, const float* params,
     const CUtensorMap& th_lo = rec ? ly.tm_hm_lo : ly.tm_h_lo;     // bf16x3
     // steps 1 .. T-1 as ONE persistent launch when all its CTAs fit on the machine at once (see GArgs::n_steps)
     const long fwd_ctas = (long)nrt * (4 * H / 256);
-    const bool persist = gen_can_persist(m, fwd_ctas, 1, GSmem<256, EPI_FWD>::CTAS_PER_SM, T - 1);
+    const bool persist = gen_can_persist(st, fwd_ctas, 1, GSmem<256, EPI_FWD>::CTAS_PER_SM, T - 1);
     for (int t = 0; t < T; ++t) {
       ep.t = t;
       GArgs g = {};
@@ -1625,7 +1628,7 @@ int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* 
     }
     // steps T-2 .. 0 of each chain as ONE persistent launch when all CTAs of both chains fit on the machine at once
     const long bwd_ctas = (long)n_a * (H / m.BNU);
-    const bool persist = gen_can_persist(m, bwd_ctas, split ? 2 : 1, 1, T - 1);
+    const bool persist = gen_can_persist(st, bwd_ctas, split ? 2 : 1, 1, T - 1);
     for (int t = T - 1; t >= 0; --t) {
       for (int half = 0; half < (split ? 2 : 1); ++half) {       // launches interleaved: neither chain lags the other
         cudaStream_t hs = half ? m.side : s;

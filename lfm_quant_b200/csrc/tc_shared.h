@@ -15,10 +15,22 @@ struct GenImpl;
 struct TcState {
   int weights_dirty = 1;        // the parameters changed since the path last packed its bf16 copies of them
   int stream_base = 0;          // first Philox stream index of the handle's layers (stage s of a forecast chain: 2 (L0+s-1))
+  int share_num = 1;            // lfmq_set_device_share: the fraction of the SMs this handle may count on for the
+  int share_den = 1;            // co-residency of a persistent launch (persistent_cta_budget)
   Profiler* prof = nullptr;
   TcImpl* impl = nullptr;       // cluster path
   GenImpl* gen = nullptr;       // general path
 };
+
+// The most CTAs a persistent launch (CTAs that wait for each other at a barrier in global memory) may have so that all of
+// them are resident at once, given sm_count SMs, ctas_per_sm resident CTAs of its kernel on an otherwise empty SM and a
+// device share num/den (0 < num <= den).  The whole device (num == den): sm_count * ctas_per_sm.  A share below one:
+// floor(sm_count * num / den) CTAs, one per SM -- then every set of concurrent handles whose shares sum to at most one
+// leaves an SM empty while any of their persistent launches still waits for a CTA (DESIGN.md section 6a).
+inline long persistent_cta_budget(int sm_count, int ctas_per_sm, int num, int den) {
+  if (num >= den) return (long)sm_count * ctas_per_sm;
+  return (long)sm_count * num / den;
+}
 
 // bf16 tiled tensor map: dims and box innermost first, byte strides of dims 1 .. rank-1, no interleave, 128-byte L2
 // promotion, no out-of-bounds fill.

@@ -100,6 +100,11 @@ class ForecasterEngine(object):
         except Exception:
             pass
 
+    def set_device_share(self, num, den):
+        """The fraction num/den of the GPU's SMs a persistent launch of this handle may count on (lfmq_set_device_share):
+        handles that run at the same time on one GPU each take a share, the shares summing to at most 1."""
+        N.check(self.lib.lfmq_set_device_share(self.handle, int(num), int(den)))
+
     # ---- weights -------------------------------------------------------------------------------
     @property
     def trainable_specs(self):
@@ -319,6 +324,11 @@ class ForecastChainEngine(object):
                 self.specs.append((s, name, shp, off, tr))
         self.n_total = sum(e.n_total for e in self.stages)
         self.n_trainable = sum(e.n_trainable for e in self.stages)
+
+    def set_device_share(self, num, den):
+        """ForecasterEngine.set_device_share for every stage: the stages of a chain run one after another on one stream."""
+        for e in self.stages:
+            e.set_device_share(num, den)
 
     def _ptrs(self, tensors):
         return (C.c_void_p * self.S)(*[t.data_ptr() for t in tensors])

@@ -326,10 +326,11 @@ class Dataset(object):
 
     @staticmethod
     def train_test_split(keys, validation_size, seed, is_train):
-        """data_processing.py:515-537."""
-        np.random.seed(seed)
+        """data_processing.py:515-537.  The reference seeds the global NumPy generator and draws from it; a generator of
+        its own draws the same keys and lets the members of an ensemble build their datasets on concurrent threads."""
         if is_train:
-            valid_keys = np.random.choice(keys, size=int(len(keys) * validation_size), replace=False)
+            rng = np.random.RandomState(seed)
+            valid_keys = rng.choice(keys, size=int(len(keys) * validation_size), replace=False)
             train_keys = list(set(keys) - set(valid_keys))
             test_keys = []
         else:

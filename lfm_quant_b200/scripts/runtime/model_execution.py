@@ -1,12 +1,88 @@
-"""ModelExecution (reference: scripts/runtime/model_execution.py:19-157): ``fixed_dates`` training / prediction of
-one config in-process.  The ensemble / multi-process fan-out of the reference (:113-146,159-199) spawns whole
-independent trainings through files and is outside the data-parallel hot path; ``num_procs > 1`` is rejected."""
+"""ModelExecution (reference: scripts/runtime/model_execution.py:19-241): ``fixed_dates`` training / prediction of
+one config in-process.  A point-estimate ensemble (num_procs > 1, :154-199) runs its members in this process too: NPE of
+them at a time, each on its own host thread and CUDA stream, side by side on the GPU(s) (DESIGN.md
+section 6a).  The reference starts one ``lfm_quant.py`` process per member instead (:142)."""
 from __future__ import absolute_import, division, print_function
 
+import copy
 import os
+import pathlib
+import random
+from collections import Counter
+from concurrent.futures import FIRST_EXCEPTION, ThreadPoolExecutor, wait
+from itertools import cycle
 
 import numpy as np
 import pandas as pd
+
+
+def member_configs(config):
+    """The N = num_procs members of a point-estimate ensemble (model_execution.py:162-190): member k has member_id k,
+    model_dir <experiments_dir>/<model_dir>/<name>-k (absolute, so that the member's files land there whatever the
+    working directory), default_gpu /gpu:(k mod num_gpu), and num_procs = NPE = 1.  Member 0 keeps config.seed; the
+    others draw theirs from random.Random(config.seed) where the reference draws from the unseeded global generator
+    (:187-188), so an ensemble can be reproduced.  Returns (<experiments_dir>/<model_dir>, [configs])."""
+    assert os.path.isdir(config.experiments_dir), "Experiments dir  %s does not exist" % config.experiments_dir
+    experiment_dir = os.path.join(os.path.abspath(config.experiments_dir), config.model_dir)
+    gpus = cycle(range(config.num_gpu))
+    seeds = random.Random(config.seed)
+    members = []
+    for k in range(config.num_procs):
+        c = copy.deepcopy(config)
+        c.member_id = k
+        c.model_dir = os.path.join(experiment_dir, '%s-%d' % (config.name, k))
+        c.default_gpu = '/gpu:%d' % next(gpus)
+        if k > 0:
+            c.seed = seeds.randint(0, 1000)
+        c.num_procs = 1
+        c.NPE = 1
+        members.append(c)
+    return experiment_dir, members
+
+
+def write_member_conf(config):
+    """<member dir>/model-<member_id>.conf, the file format the reference writes for a member (model_execution.py:130-140):
+    one line per flag that has a value, in order of the flag names.  A scalar is written as ``--name<7 spaces>value``
+    with a trailing space; a list or tuple as its items joined by '-'.  ``lfm_quant.py --config`` on the file runs the
+    member alone."""
+    pathlib.Path(config.model_dir).mkdir(parents=True, exist_ok=True)
+    path = os.path.join(config.model_dir, 'model-%d.conf' % config.member_id)
+    flags = config.as_dict()
+    lines = []
+    for name in sorted(flags):
+        value = flags[name]
+        if isinstance(value, (list, tuple)):
+            lines.append('--%s       %s\n' % (name, '-'.join(str(item) for item in value)))
+        elif isinstance(value, (bool, int, float, str)):
+            lines.append('--%s       %s \n' % (name, value))
+    with open(path, 'w') as fh:
+        fh.writelines(lines)
+    return path
+
+
+def ensemble_point_estimate(frames, forecast_steps):
+    """ensemble_preds.dat of a point-estimate ensemble (the reference's aggregate_point_estimate,
+    utils/post_processing.py:39-81) from the members' preds.dat frames: member 0's frame, every column whose name holds
+    'preds' averaged over the members, and each forecast step's squared scaled error, absolute error, relative error
+    and seq_norm-scaled squared error recomputed from those averages.  The members must hold the same (date, gvkey) rows
+    in the same order, which the reference assumes without checking; here a mismatch raises ValueError."""
+    keys = frames[0][['date', 'gvkey']].reset_index(drop=True)
+    for k, f in enumerate(frames[1:], 1):
+        if len(f) != len(keys) or not f[['date', 'gvkey']].reset_index(drop=True).equals(keys):
+            raise ValueError('ensemble member %d predicted other (date, gvkey) rows than member 0, or in another order; '
+                             'the members cannot be averaged row by row' % k)
+    out = frames[0].copy()
+    averaged = [c for c in out.columns if 'preds' in c]
+    out[averaged] = np.stack([f[averaged].to_numpy(dtype=np.float64) for f in frames]).mean(axis=0)
+    for s in range(1, forecast_steps + 1):
+        target, pred = out['targets_%d' % s], out['preds_%d' % s]
+        err = (target - pred).abs()
+        out['norm_squared_diff_%d' % s] = (out['norm_targets_%d' % s] - out['norm_preds_%d' % s]) ** 2
+        out['abs_err_%d' % s] = err
+        out['fcst_err_%d' % s] = err / target.abs()
+        out['unscaled_squared_err_%d' % s] = (err / out['seq_norm']) ** 2
+        print("Scaled MSE for step %i: %1.4f" % (s, out['norm_squared_diff_%d' % s].mean()))
+    return out
 
 
 class ModelExecution(object):
@@ -55,10 +131,67 @@ class ModelExecution(object):
         print("Prediction")
         return Predict(config, dataset).predict()
 
+    @staticmethod
+    def member_execution(config, share_den):
+        """One member of an ensemble on the calling thread: its GPU (the last character of default_gpu), a stream of
+        its own for every call, and 1/share_den of the GPU for the co-residency of its persistent launches.  Then
+        Train or Predict as a single execution."""
+        import torch
+        from ..data_processing import Dataset
+        from ..predict import Predict
+        from ..train import Train
+        gpu = str(config.default_gpu)[-1]
+        if not (gpu.isdigit() and torch.cuda.is_available() and int(gpu) < torch.cuda.device_count()):
+            raise RuntimeError('ensemble member %d: default_gpu %s is not a CUDA device of this process (%d visible)'
+                               % (config.member_id, config.default_gpu,
+                                  torch.cuda.device_count() if torch.cuda.is_available() else 0))
+        torch.cuda.set_device(int(gpu))
+        stream = torch.cuda.Stream()
+        with torch.cuda.stream(stream):
+            runner = (Train if config.train else Predict)(config, Dataset(config))
+            runner.model.engine.set_device_share(1, share_den)
+            out = runner.train() if config.train else runner.predict()
+        stream.synchronize()
+        return out
+
+    def point_estimate_ensemble(self):
+        """model_execution.py:154-199 in one process.  Training returns every member's best validation MSE, as
+        read_results reads it; prediction writes every member's pred/<preds_fname>, then
+        <experiments_dir>/<model_dir>/ensemble_preds.dat (ensemble_point_estimate), and returns that frame."""
+        cfg = self.config
+        assert cfg.num_procs > 1
+        if int(os.environ.get('WORLD_SIZE', '1')) > 1:
+            raise NotImplementedError('an ensemble (num_procs > 1) runs its members side by side in one process and '
+                                      'cannot be combined with torchrun data parallelism; run it without torchrun')
+        experiment_dir, members = member_configs(cfg)
+        for m in members:
+            write_member_conf(m)
+        npe = max(1, min(int(cfg.NPE), len(members)))
+        # at most min(NPE, members on that GPU) members run on one GPU at a time: their shares sum to at most 1
+        on_gpu = Counter(m.default_gpu for m in members)
+        with ThreadPoolExecutor(max_workers=npe) as pool:
+            futures = [pool.submit(self.member_execution, m, min(npe, on_gpu[m.default_gpu])) for m in members]
+            wait(futures, return_when=FIRST_EXCEPTION)
+            failed = [f for f in futures if f.done() and not f.cancelled() and f.exception() is not None]
+            if failed:
+                # members that have not started never start; the running ones finish before the error is raised
+                pool.shutdown(cancel_futures=True)
+                raise failed[0].exception()
+        results = [self.read_results(m) for m in members]
+        if cfg.train:
+            return [r[0] for r in results]
+        frames = [r[2] for r in results]
+        missing = [m.member_id for m, f in zip(members, frames) if f is None]
+        if missing:
+            raise RuntimeError('ensemble members %s wrote no %s' % (missing, cfg.preds_fname))
+        df = ensemble_point_estimate(frames, cfg.forecast_steps)
+        df.to_csv(os.path.join(experiment_dir, 'ensemble_preds.dat'), sep=' ', index=False)
+        return df
+
     def uq_estimate_execution(self):
         """runtime/model_execution.py:201-241: training, or prediction with one process, is a single execution; the
-        multi-process MC-dropout ensemble (num_procs > 1 at predict time) fans out through files like the other
-        ensembles and is not built."""
+        multi-process MC-dropout ensemble (num_procs > 1 at predict time: many dropout samples of one model) is not
+        built."""
         if self.config.train or self.config.num_procs == 1:
             return self.single_execution(self.config)
         raise NotImplementedError('UQ ensemble prediction (num_procs > 1) fans out whole predictions through files; run '
@@ -67,7 +200,6 @@ class ModelExecution(object):
     def fixed_dates_execution(self):
         if self.config.UQ:
             return self.uq_estimate_execution()
-        if self.config.num_procs != 1:
-            raise NotImplementedError('ensembles (num_procs > 1) fan out whole trainings through files; run one '
-                                      'lfm_quant.py per member')
-        return self.single_execution(self.config)
+        if self.config.num_procs == 1:
+            return self.single_execution(self.config)
+        return self.point_estimate_ensemble()

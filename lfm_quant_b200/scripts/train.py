@@ -110,6 +110,8 @@ class Train(object):
         for epoch in range(epochs):
             self.model.reset_states()
             mse_steps, uq_loss_steps = [], []
+            # The reference's other unseeded draw, the seeds of ensemble members k > 0 (model_execution.py:187-188), comes
+            # from random.Random(config.seed) here (runtime/model_execution.member_configs).
             if self.world == 1 and not os.environ.get('LFMQ_SEEDED_SHUFFLE'):
                 random.shuffle(self._batches)                   # train.py:115 (unseeded in the reference)
             else:                                               # every rank must walk the same batch order
