@@ -28,7 +28,7 @@ import pytest
 import torch
 
 import lfm_oracle as orc
-from util import cosine, make_engine, make_problem, make_uq_problem, rel_err
+from util import PATTERNS, cosine, make_engine, make_problem, make_uq_problem, probe_rows, rel_err, target_row
 
 pytestmark = pytest.mark.gpu
 
@@ -191,24 +191,10 @@ ROW_BOUNDS = {
     },
 }
 LOSS_TOL = 1e-2          # loss of the probe row, relative (worst 4.0e-3)
-PATTERNS = ('all', 't0', 'last', 'ends')    # which steps of the probe row have nonzero targets
 
 
 def _kind(name):
     return name if name.startswith('OUTPUT') else name.split('/')[-1]
-
-
-def _target_row(rng, T, pattern):
-    y = rng.normal(size=(T, O)).astype(np.float32)
-    keep = np.zeros(T, dtype=bool)
-    if pattern == 'all':
-        keep[:] = True
-    if pattern in ('t0', 'ends'):
-        keep[0] = True
-    if pattern in ('last', 'ends'):
-        keep[-1] = True
-    y[~keep] = 0.0
-    return y
 
 
 def _oracle_row(params, x_row, y_row, L, row0, B, okw):
@@ -217,13 +203,6 @@ def _oracle_row(params, x_row, y_row, L, row0, B, okw):
     loss, mse, dpred, _ = orc.loss_point_estimate(y_row[None].astype(np.float64), preds, target_idx=TARGET,
                                                   target_lambda=0.5, rnn_lambda=0.7, batch_global=B)
     return loss, mse, preds, orc.backward(dpred, fc, num_layers=L)
-
-
-def _probe_rows(B, unit, extra=()):
-    rows = {0, B - 1} | set(extra)
-    for k in range(unit, B, unit):
-        rows |= {k - 1, k}
-    return sorted(r for r in rows if 0 <= r < B)
 
 
 def _run_probes(path, B, T, H, L, rows, okw):
@@ -242,7 +221,7 @@ def _run_probes(path, B, T, H, L, rows, okw):
     t_gpu = time.time()
     for i, r in enumerate(rows):
         pattern = PATTERNS[i % len(PATTERNS)]
-        y_row = _target_row(rng, T, pattern)
+        y_row = target_row(rng, T, O, pattern)
         yd[r] = _cuda(y_row)
         eng.backward(xd, yd, step=STEP, row0=row0)
         grads = eng.grads_list()
@@ -293,7 +272,7 @@ def _run_probes(path, B, T, H, L, rows, okw):
 def test_cluster_gradient_probes(B, T, dropout):
     """Cluster path (H=256, L=1): rows on both sides of every 64-row unit boundary, whatever the co-resident cluster
     count makes of the rounds."""
-    _run_probes('cluster', B, T, 256, 1, _probe_rows(B, 64), dict(dropout=dropout, seed=123))
+    _run_probes('cluster', B, T, 256, 1, probe_rows(B, 64), dict(dropout=dropout, seed=123))
 
 
 GEN_DROP = dict(dropout=0.2, recurrent_dropout=0.1, seed=123)
@@ -309,7 +288,7 @@ def test_general_gradient_probes(B, H, L, okw):
     """General path: rows on both sides of every 128-row tile boundary and of the split between the two chains."""
     nrt = (B + 127) // 128
     n_a = (nrt + 1) // 2 if nrt >= 16 else nrt
-    rows = _probe_rows(B, 128, extra=(128 * n_a - 1, 128 * n_a))
+    rows = probe_rows(B, 128, extra=(128 * n_a - 1, 128 * n_a))
     _run_probes('general', B, 48, H, L, rows, okw)
 
 

@@ -46,6 +46,31 @@ def cosine(a, b):
     return float(np.dot(a, b) / (np.linalg.norm(a) * np.linalg.norm(b) + 1e-30))
 
 
+PATTERNS = ('all', 't0', 'last', 'ends')    # which steps of a probe row have nonzero targets
+
+
+def target_row(rng, T, O, pattern):
+    """Targets of one probe row: normal values at the steps `pattern` names, zeros (masked steps) elsewhere."""
+    y = rng.normal(size=(T, O)).astype(np.float32)
+    keep = np.zeros(T, dtype=bool)
+    if pattern == 'all':
+        keep[:] = True
+    if pattern in ('t0', 'ends'):
+        keep[0] = True
+    if pattern in ('last', 'ends'):
+        keep[-1] = True
+    y[~keep] = 0.0
+    return y
+
+
+def probe_rows(B, unit, extra=()):
+    """Rows 0 and B-1, both sides of every multiple of `unit`, and `extra`."""
+    rows = {0, B - 1} | set(extra)
+    for k in range(unit, B, unit):
+        rows |= {k - 1, k}
+    return sorted(r for r in rows if 0 <= r < B)
+
+
 def make_engine(B, T, F, O, H, L, **kw):
     from lfm_quant_b200.engine import ForecasterEngine
     return ForecasterEngine(max_batch=B, seq_len=T, n_inputs=F, n_outputs=O, num_hidden=H, num_layers=L, **kw)
