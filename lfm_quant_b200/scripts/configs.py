@@ -79,6 +79,16 @@ class ConfigValues(object):
         c.__dict__['__parsed'] = True
         return c
 
+    # pickling (a hyper-parameter search saves its population, scripts/param_search/genetic_algorithm.py) stores the
+    # parsed values; without these, unpickling would look __setstate__ up through __getattr__, which parses argv
+    def __getstate__(self):
+        return self.as_dict()
+
+    def __setstate__(self, state):
+        self.__dict__['__configs'] = dict(state)
+        self.__dict__['__parsed'] = True
+        self.__dict__['__argv'] = None
+
 
 def _define(name, default, doc, typ):
     if name in _defined:

@@ -1,13 +1,15 @@
 """ModelExecution (reference: scripts/runtime/model_execution.py:19-241): ``fixed_dates`` training / prediction of
 one config in-process.  A point-estimate ensemble (num_procs > 1, :154-199) runs its members in this process too: NPE of
 them at a time, each on its own host thread and CUDA stream, side by side on the GPU(s) (DESIGN.md
-section 6a).  The reference starts one ``lfm_quant.py`` process per member instead (:142)."""
+section 6a).  The reference starts one ``lfm_quant.py`` process per member instead (:142).  The candidates of a
+hyper-parameter search generation run the same way (run_candidates, DESIGN.md section 6b)."""
 from __future__ import absolute_import, division, print_function
 
 import copy
 import os
 import pathlib
 import random
+import traceback
 from collections import Counter
 from concurrent.futures import FIRST_EXCEPTION, ThreadPoolExecutor, wait
 from itertools import cycle
@@ -40,24 +42,28 @@ def member_configs(config):
     return experiment_dir, members
 
 
-def write_member_conf(config):
-    """<member dir>/model-<member_id>.conf, the file format the reference writes for a member (model_execution.py:130-140):
-    one line per flag that has a value, in order of the flag names.  A scalar is written as ``--name<7 spaces>value``
-    with a trailing space; a list or tuple as its items joined by '-'.  ``lfm_quant.py --config`` on the file runs the
-    member alone."""
-    pathlib.Path(config.model_dir).mkdir(parents=True, exist_ok=True)
-    path = os.path.join(config.model_dir, 'model-%d.conf' % config.member_id)
-    flags = config.as_dict()
+def write_conf(flags, path):
+    """Writes the flags {name: value} to `path` in the file format the reference writes for an ensemble member or a
+    search candidate (model_execution.py:130-140, genetic_algorithm.py:171-182): one line per flag that has a value, in
+    order of the flag names.  A scalar (also a NumPy scalar, as values read from a CSV file are) is written as
+    ``--name<7 spaces>value`` with a trailing space; a list or tuple as its items joined by '-'."""
     lines = []
     for name in sorted(flags):
         value = flags[name]
         if isinstance(value, (list, tuple)):
             lines.append('--%s       %s\n' % (name, '-'.join(str(item) for item in value)))
-        elif isinstance(value, (bool, int, float, str)):
+        elif isinstance(value, (bool, int, float, str, np.bool_, np.integer, np.floating)):
             lines.append('--%s       %s \n' % (name, value))
     with open(path, 'w') as fh:
         fh.writelines(lines)
     return path
+
+
+def write_member_conf(config):
+    """<member dir>/model-<member_id>.conf (write_conf).  ``lfm_quant.py --config`` on the file runs the member
+    alone."""
+    pathlib.Path(config.model_dir).mkdir(parents=True, exist_ok=True)
+    return write_conf(config.as_dict(), os.path.join(config.model_dir, 'model-%d.conf' % config.member_id))
 
 
 def ensemble_point_estimate(frames, forecast_steps):
@@ -83,6 +89,61 @@ def ensemble_point_estimate(frames, forecast_steps):
         out['unscaled_squared_err_%d' % s] = (err / out['seq_norm']) ** 2
         print("Scaled MSE for step %i: %1.4f" % (s, out['norm_squared_diff_%d' % s].mean()))
     return out
+
+
+def candidate_config(conf_path):
+    """The config that ``lfm_quant.py --config <conf_path>`` runs: the file parsed with the forecaster's flag schema."""
+    from .. import configs, lfm_quant
+    configs.reset()
+    return lfm_quant.get_configs(['--config', conf_path])
+
+
+def run_candidates(conf_paths, npe):
+    """Trains (or, with train False, predicts) the hyper-parameter search candidates whose model.conf files are
+    `conf_paths`, in this process, `npe` at a time: each on its own host thread and CUDA stream, on its GPU (the last
+    character of default_gpu), with a device share of 1/min(npe, candidates on that GPU) (DESIGN.md section 6b).  Each
+    runs what ``lfm_quant.py --config <its model.conf>`` runs alone, and writes the same files.
+
+    A candidate that fails -- its file does not parse, the library refuses its config, or it raises while it runs --
+    does not stop the others: its error is printed and returned.  Returns one entry per candidate, None or the error.
+    A default_gpu that is not a CUDA device of this process is an error of the search and raises."""
+    import torch
+    errors = [None] * len(conf_paths)
+    candidates = {}
+    for i, path in enumerate(conf_paths):
+        try:
+            c = candidate_config(path)
+            if c.training_type == 'iterative' or c.cdrs_inference or c.num_procs > 1:
+                raise NotImplementedError('a search candidate runs as one fixed_dates model (training_type '
+                                          'fixed_dates, no cdrs_inference, num_procs 1); %s asks for more' % path)
+            candidates[i] = c
+        except (Exception, SystemExit) as e:        # argparse exits on a value it cannot convert
+            print('candidate %s refused: %r' % (path, e))
+            errors[i] = e
+    visible = torch.cuda.device_count() if torch.cuda.is_available() else 0
+    for c in candidates.values():
+        gpu = str(c.default_gpu)[-1]
+        if not (gpu.isdigit() and int(gpu) < visible):
+            raise RuntimeError('search candidate %s: default_gpu %s is not a CUDA device of this process (%d visible); '
+                               'set num_gpu to at most the number of GPUs' % (c.member_id, c.default_gpu, visible))
+    if not candidates:
+        return errors
+    npe = max(1, min(int(npe), len(candidates)))
+    on_gpu = Counter(c.default_gpu for c in candidates.values())
+
+    def run(i):
+        c = candidates[i]
+        try:
+            ModelExecution.member_execution(c, min(npe, on_gpu[c.default_gpu]))
+            return None
+        except Exception as e:
+            print('candidate %s failed:\n%s' % (conf_paths[i], traceback.format_exc()))
+            return e
+
+    with ThreadPoolExecutor(max_workers=npe) as pool:
+        for i, err in zip(list(candidates), pool.map(run, list(candidates))):
+            errors[i] = err
+    return errors
 
 
 class ModelExecution(object):
