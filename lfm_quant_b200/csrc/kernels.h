@@ -30,9 +30,6 @@ int bn_dropout_bwd(cudaStream_t s, int B, int T, int H, const float* dy, const f
 int add_bias_rows(cudaStream_t s, long rows, int N, float* C, const float* bias);
 int colsum(cudaStream_t s, long rows, int N, const float* A, float* out, float* scratch, size_t scratch_elems);
 int softplus_floor(cudaStream_t s, long n, const float* a, float* var);
-int uq_loss_grad(cudaStream_t s, int B, int T, int O, const float* pred, const float* var, const float* apre,
-                 const float* y, const float* counts_in, int target_idx, float p1, float p2, float* dpred, float* da,
-                 float* out_loss, float* out_uq0, float* out_mse0, float* counts_out, float* scratch);
 int mask_count(cudaStream_t s, int B, int T, int O, const float* y, float* out2, unsigned int* tickets);
 // out2 = {loss, mse_0}; maskout2 (nullable) = {B, mask_count_local}; dpred may be NULL (validation);
 // denom (nullable) = device {B_global, mask_count_global}.
@@ -56,7 +53,8 @@ int scale_inplace(cudaStream_t s, long n, float* p, float w);
 int chain_scatter_dx(cudaStream_t s, int B, int T, int F, int O, int stage, const float* dx, const ChainPtrs& dpred);
 int chain_combine(cudaStream_t s, int S, const ChainPtrs& scalars, float clip, const ChainPtrs& loss2,
                   const ChainWeights& w, float* out2);
-// forecast_steps > 1 of RNNUqRangeEstimate: every stage's uq loss rows in one launch, then one reduction launch.
+// The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
+// then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and
 // out3 (nullable) = the weighted sums {uq_loss, uq_loss_last_tar, mse}; counts_in = 1 takes the counts from counts.p[s]
 // (required with dpred), else the pass counts its own rows.  dpred / da (nullable) = w_s * dLoss_s / d(pred, apre).

@@ -908,16 +908,6 @@ __device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* _
   block_reduce4(cnt, partial + 4);
 }
 
-__global__ void __launch_bounds__(256) uq_loss_rows_kernel(int B, int T, int O, const float* __restrict__ pred,
-                                                           const float* __restrict__ var,
-                                                           const float* __restrict__ apre,
-                                                           const float* __restrict__ y,
-                                                           const float* __restrict__ counts, int target_idx, float p1,
-                                                           float p2, float* __restrict__ dpred,
-                                                           float* __restrict__ da, double* __restrict__ partial) {
-  uq_loss_rows(B, T, O, pred, var, apre, y, counts, target_idx, p1, p2, 1.0f, dpred, da, partial + (long)blockIdx.x * 8);
-}
-
 // One warp reduces the nblk partial rows of one loss pass.  Lane 0 writes the counts and / or the three scalars
 // {uq_loss, uq_loss_last_tar, mse_0} (any output may be null) and returns them in vals3.
 __device__ __forceinline__ void uq_loss_final(int nblk, const double* __restrict__ partial,
@@ -947,16 +937,8 @@ __device__ __forceinline__ void uq_loss_final(int nblk, const double* __restrict
   if (out_mse0) *out_mse0 = vals3[2];
 }
 
-__global__ void uq_loss_final_kernel(int nblk, const double* __restrict__ partial, const float* __restrict__ counts_in,
-                                     int B, int O, float p1, float p2, float* __restrict__ out_loss,
-                                     float* __restrict__ out_uq0, float* __restrict__ out_mse0,
-                                     float* __restrict__ counts_out) {
-  float v[3];
-  uq_loss_final(nblk, partial, counts_in, B, O, p1, p2, out_loss, out_uq0, out_mse0, counts_out, v);
-}
-
-// forecast_steps > 1 of RNNUqRangeEstimate (losses.py:137-178): blockIdx.y = forecast stage.  Each stage runs the rows
-// above on its own tensors and counts, its gradients scaled by its weight w_s.
+// blockIdx.y = forecast stage (losses.py:137-178).  Each stage runs the rows above on its own tensors and counts, its
+// gradients scaled by its weight w_s.  A single uq handle is the chain of one stage with w_0 = 1.
 __global__ void __launch_bounds__(256) chain_uq_rows_kernel(int B, int T, int O, ChainUqArgs a, int target_idx, float p1,
                                                             float p2, double* __restrict__ partial) {
   const int s = blockIdx.y;
@@ -992,21 +974,6 @@ int chain_uq_loss_grad(cudaStream_t s, int S, int B, int T, int O, const ChainUq
   chain_uq_rows_kernel<<<dim3(LOSS_BLOCKS, S), 256, 0, s>>>(B, T, O, a, target_idx, p1, p2, partial);
   LFMQ_LAUNCH_CHECK();
   chain_uq_final_kernel<<<1, 32 * S, 0, s>>>(S, LOSS_BLOCKS, a, B, O, p1, p2, partial, out3);
-  LFMQ_LAUNCH_CHECK();
-  return 0;
-}
-
-// pred == nullptr: counts only -> counts_out.  Otherwise the three scalars; with dpred also the gradients (counts_in
-// from a counts-only pass is then required).
-int uq_loss_grad(cudaStream_t s, int B, int T, int O, const float* pred, const float* var, const float* apre,
-                 const float* y, const float* counts_in, int target_idx, float p1, float p2, float* dpred, float* da,
-                 float* out_loss, float* out_uq0, float* out_mse0, float* counts_out, float* scratch) {
-  double* partial = reinterpret_cast<double*>(scratch);
-  uq_loss_rows_kernel<<<LOSS_BLOCKS, 256, 0, s>>>(B, T, O, pred, var, apre, y, counts_in, target_idx, p1, p2, dpred, da,
-                                                  partial);
-  LFMQ_LAUNCH_CHECK();
-  uq_loss_final_kernel<<<1, 32, 0, s>>>(LOSS_BLOCKS, partial, counts_in, B, O, p1, p2, out_loss, out_uq0, out_mse0,
-                                        counts_out);
   LFMQ_LAUNCH_CHECK();
   return 0;
 }

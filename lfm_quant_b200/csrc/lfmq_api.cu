@@ -372,6 +372,121 @@ int apply_update(lfmq_handle h, float lr, int64_t iteration, cudaStream_t s) {
   return 0;
 }
 
+// ---- a model is a chain of S >= 1 stages; a single handle is the chain of one stage with weight 1 ----------------
+// None of these touch tc.stream_base: only the public chain entry points (chain_check) number the stages' dropout
+// streams, so a handle that is stage s > 0 of a chain keeps its streams when it is called on its own.
+
+// The forward of every stage in order.  Stage i > 0 reads the window built in work slot i - 1 from stage i - 1's target
+// predictions (rnn_uq_range_estimate.py:118: outputs[-2]; variances never feed forward); one stage needs no work.
+// preds == nullptr is the training path: forward_fp32 into each handle's own preds / var, which the backward reads.
+// Otherwise the predict path: preds[i] (and vars[i] on a uq chain) through lfmq_forward / lfmq_forward_uq, which
+// dispatch on the stage's precision.
+int run_stages(const lfmq_handle* st, int S, const float* x, int B, int64_t row0, int64_t step, float* const* preds,
+               float* const* vars, float* work, cudaStream_t s) {
+  const lfmq_config& c = st[0]->cfg;
+  const size_t slot = (size_t)B * c.seq_len * c.n_inputs;
+  const float* in = x;
+  for (int i = 0; i < S; ++i) {
+    lfmq_handle h = st[i];
+    if (i > 0) {
+      float* next = work + (size_t)(i - 1) * slot;
+      RUN(chain_next_input(s, B, c.seq_len, c.n_inputs, c.n_outputs, in, preds ? preds[i - 1] : st[i - 1]->preds, x,
+                           next));
+      in = next;
+    }
+    if (preds && c.uq) {
+      RUN(lfmq_forward_uq(h, in, B, row0, step, preds[i], vars[i], s));
+    } else if (preds) {
+      RUN(lfmq_forward(h, in, B, row0, step, preds[i], s));
+    } else {
+      h->last_step = step;
+      h->last_row0 = row0;
+      RUN(forward_fp32(h, in, B, row0, step, h->preds, h->var, s));
+    }
+  }
+  return 0;
+}
+
+// Every stage's {B, unmasked rows, unmasked last-step rows} into out_dev[3 * i], in one loss pass without predictions.
+int stage_counts(const lfmq_handle* st, int S, const float* const* y, int B, float* out_dev, cudaStream_t s) {
+  lfmq::ChainUqArgs a{};
+  for (int i = 0; i < S; ++i) {
+    a.y.p[i] = const_cast<float*>(y[i]);
+    a.counts.p[i] = out_dev + 3 * i;
+  }
+  const lfmq_config& c = st[0]->cfg;
+  return chain_uq_loss_grad(s, S, B, c.seq_len, c.n_outputs, a, c.target_idx, c.target_lambda, c.rnn_lambda, nullptr,
+                            st[0]->scratch);
+}
+
+// The uq loss of the stages' own preds / var (train.py:201-218): one loss pass over all stages for the mask counts
+// unless denom brings them, and one for the losses and w_s * dLoss_s / d(pred_s, variance pre-activation_s).
+int stages_loss_uq(const lfmq_handle* st, int S, const float* const* y, const float* weights, int B, const float* denom,
+                   float* loss_out_dev, cudaStream_t s) {
+  const lfmq_config& c0 = st[0]->cfg;
+  const int T = c0.seq_len, O = c0.n_outputs;
+  lfmq::ChainUqArgs a{};
+  for (int i = 0; i < S; ++i) {
+    a.y.p[i] = const_cast<float*>(y[i]);
+    a.counts.p[i] = denom ? const_cast<float*>(denom) + 3 * i : st[i]->denom;
+    a.w.w[i] = weights[i];
+  }
+  float* scratch = st[0]->scratch;
+  if (!denom) RUN(chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, nullptr, scratch));
+  for (int i = 0; i < S; ++i) {
+    a.pred.p[i] = st[i]->preds;
+    a.var.p[i] = st[i]->var;
+    a.apre.p[i] = st[i]->apre;
+    a.dpred.p[i] = st[i]->dpred;
+    a.da.p[i] = st[i]->da;
+    float* tail = st[i]->grads + st[i]->n_train;     // the stage's own {uq_loss, mse_0, .., .., uq_loss_last_tar}
+    a.loss.p[i] = tail;
+    a.mse0.p[i] = tail + 1;
+    a.uq0.p[i] = tail + 4;
+  }
+  a.counts_in = 1;
+  return chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, loss_out_dev, scratch);
+}
+
+// Forward, loss and BPTT of S training-mode fp32 stages of one kind: the body of lfmq_backward's fp32 branches and of
+// lfmq_chain_backward(_dp).  denom (nullable): three counts per stage, summed over the data-parallel ranks; a point
+// stage reads the two that lead them, {B, mask_count}.  Without it every stage counts its own batch.
+// loss_out_dev (nullable): the weighted sums over the stages.  work is read only when S > 1.
+int backward_stages(const lfmq_handle* st, int S, const float* x, const float* const* y, const float* weights, int B,
+                    int64_t row0, int64_t step, const float* denom, float* work, float* loss_out_dev, cudaStream_t s) {
+  const lfmq_config& c0 = st[0]->cfg;
+  const int T = c0.seq_len, F = c0.n_inputs, O = c0.n_outputs;
+  const size_t slot = (size_t)B * T * F;
+  // forward of every stage (each keeps its own saved state), then each stage's loss and dLoss/dpred_s, weighted
+  RUN(run_stages(st, S, x, B, row0, step, nullptr, nullptr, work, s));
+  lfmq::ChainPtrs dpred{}, l2{}, none{};
+  lfmq::ChainWeights w{};
+  if (c0.uq) RUN(stages_loss_uq(st, S, y, weights, B, denom, loss_out_dev, s));
+  for (int i = 0; i < S && !c0.uq; ++i) {
+    lfmq_handle h = st[i];
+    const lfmq_config& c = h->cfg;
+    const float* d = denom ? denom + 3 * i : h->denom;
+    if (!denom) RUN(mask_count(s, B, T, O, y[i], h->denom, h->tickets));
+    float* tail = h->grads + h->n_train;
+    RUN(loss_grad(s, B, T, O, h->preds, y[i], d, c.target_idx, c.target_lambda, c.rnn_lambda, h->dpred, tail, nullptr,
+                  h->scratch));
+    if (weights[i] != 1.0f) RUN(scale_inplace(s, (long)B * T * O, h->dpred, weights[i]));
+    l2.p[i] = tail;
+    w.w[i] = weights[i];
+  }
+  if (loss_out_dev && !c0.uq) RUN(chain_combine(s, S, none, 0.f, l2, w, loss_out_dev));
+  // BPTT from the last stage down; the input gradient of stage i lands on the last time step of earlier predictions
+  // (the target predictions on a uq chain: variances never feed forward, so there is no dvar feedback)
+  for (int i = 0; i < S; ++i) dpred.p[i] = st[i]->dpred;
+  for (int i = S - 1; i >= 1; --i) {
+    float* dx = work + (size_t)(S - 1) * slot;
+    const float* in_i = work + (size_t)(i - 1) * slot;
+    RUN(backward_fp32(st[i], in_i, B, s, dx));
+    RUN(chain_scatter_dx(s, B, T, F, O, i, dx, dpred));
+  }
+  return backward_fp32(st[0], x, B, s);
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -618,9 +733,13 @@ int32_t lfmq_loss_uq(lfmq_handle h, const float* preds, const float* var, const 
     return LFMQ_ERR_ARG;
   }
   const lfmq_config& c = h->cfg;
-  return uq_loss_grad((cudaStream_t)stream, B, c.seq_len, c.n_outputs, preds, var, nullptr, y, nullptr, c.target_idx,
-                      c.target_lambda, c.rnn_lambda, nullptr, nullptr, out_dev, out_dev + 1, out_dev + 2, nullptr,
-                      h->scratch);
+  lfmq::ChainUqArgs a{};      // one stage of weight 1: the weighted sums {uq_loss, uq_loss_last_tar, mse} are its own
+  a.pred.p[0] = const_cast<float*>(preds);
+  a.var.p[0] = const_cast<float*>(var);
+  a.y.p[0] = const_cast<float*>(y);
+  a.w.w[0] = 1.0f;
+  return chain_uq_loss_grad((cudaStream_t)stream, 1, B, c.seq_len, c.n_outputs, a, c.target_idx, c.target_lambda,
+                            c.rnn_lambda, out_dev, h->scratch);
 }
 
 int32_t lfmq_mask_count(lfmq_handle h, const float* y, int32_t B, float* out_dev, void* stream) {
@@ -638,10 +757,7 @@ int32_t lfmq_mask_count_uq(lfmq_handle h, const float* y, int32_t B, float* out_
     LFMQ_SET_ERR("lfmq_mask_count_uq: null pointer");
     return LFMQ_ERR_ARG;
   }
-  const lfmq_config& c = h->cfg;
-  return uq_loss_grad((cudaStream_t)stream, B, c.seq_len, c.n_outputs, nullptr, nullptr, nullptr, y, nullptr,
-                      c.target_idx, c.target_lambda, c.rnn_lambda, nullptr, nullptr, nullptr, nullptr, nullptr, out_dev,
-                      h->scratch);
+  return stage_counts(&h, 1, &y, B, out_dev, (cudaStream_t)stream);
 }
 
 int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, int64_t row0, int64_t step,
@@ -657,20 +773,10 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
   }
   cudaStream_t s = (cudaStream_t)stream;
   const lfmq_config& c = h->cfg;
-  h->last_step = step;
-  h->last_row0 = row0;
-  if (c.uq) {      // denom_dev: the three counts of lfmq_mask_count_uq, summed over the ranks
-    float* t = h->grads + h->n_train;
-    RUN(forward_fp32(h, x, B, row0, step, h->preds, h->var, s));
-    const float* counts = denom_dev;
-    if (!counts) {
-      RUN(uq_loss_grad(s, B, c.seq_len, c.n_outputs, nullptr, nullptr, nullptr, y, nullptr, c.target_idx,
-                       c.target_lambda, c.rnn_lambda, nullptr, nullptr, nullptr, nullptr, nullptr, h->denom, h->scratch));
-      counts = h->denom;
-    }
-    RUN(uq_loss_grad(s, B, c.seq_len, c.n_outputs, h->preds, h->var, h->apre, y, counts, c.target_idx, c.target_lambda,
-                     c.rnn_lambda, h->dpred, h->da, t, t + 4, t + 1, nullptr, h->scratch));
-    return backward_fp32(h, x, B, s);
+  if (c.precision == LFMQ_PREC_FP32) {      // a trainable uq handle is always fp32
+    // denom_dev: stage 0's counts, the three of lfmq_mask_count_uq or the two of lfmq_mask_count
+    const float one = 1.0f;
+    return backward_stages(&h, 1, x, &y, &one, B, row0, step, denom_dev, nullptr, nullptr, s);
   }
   const float* denom = denom_dev;
   if (!denom) {
@@ -679,12 +785,7 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
   }
   float* tail = h->grads + h->n_train;
   if (h->use_gen) return lfmq::gen_backward(h->tc, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
-  if (c.precision == LFMQ_PREC_BF16)
-    return lfmq::tc_backward(h->tc, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
-  RUN(forward_fp32(h, x, B, row0, step, h->preds, nullptr, s));
-  RUN(loss_grad(s, B, c.seq_len, c.n_outputs, h->preds, y, denom, c.target_idx, c.target_lambda, c.rnn_lambda,
-                h->dpred, tail, nullptr, h->scratch));
-  return backward_fp32(h, x, B, s);
+  return lfmq::tc_backward(h->tc, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
 }
 
 int32_t lfmq_apply(lfmq_handle h, float lr, int64_t iteration, void* stream) {
@@ -763,23 +864,12 @@ int32_t lfmq_chain_forward(const lfmq_handle* stages, int32_t n_stages, const fl
     LFMQ_SET_ERR("lfmq_chain_forward: uq chain, call lfmq_chain_forward_uq");
     return LFMQ_ERR_ARG;
   }
-  cudaStream_t s = (cudaStream_t)stream;
-  const lfmq_config& c = stages[0]->cfg;
-  const size_t slot = (size_t)B * c.seq_len * c.n_inputs;
-  const float* in = x;
-  for (int i = 0; i < n_stages; ++i) {
+  for (int i = 0; i < n_stages; ++i)
     if (!preds[i]) {
       LFMQ_SET_ERR("lfmq_chain_forward: preds[%d] == NULL", i);
       return LFMQ_ERR_ARG;
     }
-    if (i > 0) {
-      float* next = work + (size_t)(i - 1) * slot;
-      RUN(chain_next_input(s, B, c.seq_len, c.n_inputs, c.n_outputs, in, preds[i - 1], x, next));
-      in = next;
-    }
-    RUN(lfmq_forward(stages[i], in, B, row0, step, preds[i], stream));
-  }
-  return LFMQ_OK;
+  return run_stages(stages, n_stages, x, B, row0, step, preds, nullptr, work, (cudaStream_t)stream);
 }
 
 int32_t lfmq_chain_forward_uq(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
@@ -793,23 +883,12 @@ int32_t lfmq_chain_forward_uq(const lfmq_handle* stages, int32_t n_stages, const
     LFMQ_SET_ERR("lfmq_chain_forward_uq: point-estimate chain, call lfmq_chain_forward");
     return LFMQ_ERR_ARG;
   }
-  cudaStream_t s = (cudaStream_t)stream;
-  const lfmq_config& c = stages[0]->cfg;
-  const size_t slot = (size_t)B * c.seq_len * c.n_inputs;
-  const float* in = x;
-  for (int i = 0; i < n_stages; ++i) {
+  for (int i = 0; i < n_stages; ++i)
     if (!preds[i] || !vars[i]) {
       LFMQ_SET_ERR("lfmq_chain_forward_uq: preds[%d] or vars[%d] == NULL", i, i);
       return LFMQ_ERR_ARG;
     }
-    if (i > 0) {      // the next window is built from the target predictions (outputs[-2], :118); variances stay put
-      float* next = work + (size_t)(i - 1) * slot;
-      RUN(chain_next_input(s, B, c.seq_len, c.n_inputs, c.n_outputs, in, preds[i - 1], x, next));
-      in = next;
-    }
-    RUN(lfmq_forward_uq(stages[i], in, B, row0, step, preds[i], vars[i], stream));
-  }
-  return LFMQ_OK;
+  return run_stages(stages, n_stages, x, B, row0, step, preds, vars, work, (cudaStream_t)stream);
 }
 
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,
@@ -858,50 +937,6 @@ int32_t lfmq_chain_loss_uq(const lfmq_handle* stages, int32_t n_stages, const fl
 }
 
 namespace {
-// lfmq_chain_backward of a uq chain (train.py:201-218): every stage's forward, then one loss pass over all stages for
-// the mask counts and one for the losses and w_s * dLoss_s / d(pred_s, variance pre-activation_s).
-// denom (nullable): every stage's three counts (lfmq_chain_mask_count), summed over the data-parallel ranks.
-int chain_forward_loss_uq(const lfmq_handle* st, int S, const float* x, const float* const* y, const float* weights,
-                          int B, int64_t row0, int64_t step, const float* denom, float* work, float* loss_out_dev,
-                          cudaStream_t s) {
-  const lfmq_config& c0 = st[0]->cfg;
-  const int T = c0.seq_len, F = c0.n_inputs, O = c0.n_outputs;
-  const size_t slot = (size_t)B * T * F;
-  lfmq::ChainUqArgs a{};
-  const float* in = x;
-  for (int i = 0; i < S; ++i) {
-    lfmq_handle h = st[i];
-    h->last_step = step;
-    h->last_row0 = row0;
-    if (i > 0) {
-      float* next = work + (size_t)(i - 1) * slot;
-      RUN(chain_next_input(s, B, T, F, O, in, st[i - 1]->preds, x, next));
-      in = next;
-    }
-    RUN(forward_fp32(h, in, B, row0, step, h->preds, h->var, s));
-    a.y.p[i] = const_cast<float*>(y[i]);
-    a.counts.p[i] = denom ? const_cast<float*>(denom) + 3 * i : h->denom;
-    a.w.w[i] = weights[i];
-  }
-  float* scratch = st[0]->scratch;
-  if (!denom) RUN(chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, nullptr, scratch));
-  for (int i = 0; i < S; ++i) {
-    a.pred.p[i] = st[i]->preds;
-    a.var.p[i] = st[i]->var;
-    a.apre.p[i] = st[i]->apre;
-    a.dpred.p[i] = st[i]->dpred;
-    a.da.p[i] = st[i]->da;
-    float* tail = st[i]->grads + st[i]->n_train;     // the stage's own {uq_loss, mse_0, .., .., uq_loss_last_tar}
-    a.loss.p[i] = tail;
-    a.mse0.p[i] = tail + 1;
-    a.uq0.p[i] = tail + 4;
-  }
-  a.counts_in = 1;
-  return chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, loss_out_dev, scratch);
-}
-}  // namespace
-
-namespace {
 int chain_backward(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
                    const float* weights, int32_t B, int64_t row0, int64_t step, const float* denom, float* work,
                    float* loss_out_dev, void* stream) {
@@ -910,54 +945,13 @@ int chain_backward(const lfmq_handle* stages, int32_t n_stages, const float* x, 
     LFMQ_SET_ERR("lfmq_chain_backward: null pointer");
     return LFMQ_ERR_ARG;
   }
-  cudaStream_t s = (cudaStream_t)stream;
-  const int S = n_stages;
-  const lfmq_config& c0 = stages[0]->cfg;
-  const int T = c0.seq_len, F = c0.n_inputs, O = c0.n_outputs;
-  const size_t slot = (size_t)B * T * F;
-  float* dx = work + (size_t)(S - 1) * slot;
-  // forward of every stage (each keeps its own saved state), then each stage's loss and dLoss/dpred_s, weighted
-  lfmq::ChainPtrs dpred{}, l2{}, none{};
-  lfmq::ChainWeights w{};
-  for (int i = 0; i < S; ++i)
+  for (int i = 0; i < n_stages; ++i)
     if (!y[i]) {
       LFMQ_SET_ERR("lfmq_chain_backward: y[%d] == NULL", i);
       return LFMQ_ERR_ARG;
     }
-  if (c0.uq) {
-    RUN(chain_forward_loss_uq(stages, S, x, y, weights, B, row0, step, denom, work, loss_out_dev, s));
-    for (int i = 0; i < S; ++i) dpred.p[i] = stages[i]->dpred;      // variances never feed forward: no dvar feedback
-  }
-  const float* in = x;
-  for (int i = 0; i < S && !c0.uq; ++i) {
-    lfmq_handle h = stages[i];
-    const lfmq_config& c = h->cfg;
-    h->last_step = step;
-    h->last_row0 = row0;
-    if (i > 0) {
-      float* next = work + (size_t)(i - 1) * slot;
-      RUN(chain_next_input(s, B, T, F, O, in, stages[i - 1]->preds, x, next));
-      in = next;
-    }
-    RUN(forward_fp32(h, in, B, row0, step, h->preds, nullptr, s));
-    const float* d = denom ? denom + 3 * i : h->denom;      // {B, mask_count} lead the stage's three counts
-    if (!denom) RUN(mask_count(s, B, T, O, y[i], h->denom, h->tickets));
-    float* tail = h->grads + h->n_train;
-    RUN(loss_grad(s, B, T, O, h->preds, y[i], d, c.target_idx, c.target_lambda, c.rnn_lambda, h->dpred, tail, nullptr,
-                  h->scratch));
-    if (weights[i] != 1.0f) RUN(scale_inplace(s, (long)B * T * O, h->dpred, weights[i]));
-    dpred.p[i] = h->dpred;
-    l2.p[i] = tail;
-    w.w[i] = weights[i];
-  }
-  if (loss_out_dev && !c0.uq) RUN(chain_combine(s, S, none, 0.f, l2, w, loss_out_dev));
-  // BPTT from the last stage down; the input gradient of stage i lands on the last time step of earlier predictions
-  for (int i = S - 1; i >= 1; --i) {
-    const float* in_i = work + (size_t)(i - 1) * slot;
-    RUN(backward_fp32(stages[i], in_i, B, s, dx));
-    RUN(chain_scatter_dx(s, B, T, F, O, i, dx, dpred));
-  }
-  return backward_fp32(stages[0], x, B, s);
+  return backward_stages(stages, n_stages, x, y, weights, B, row0, step, denom, work, loss_out_dev,
+                         (cudaStream_t)stream);
 }
 
 // the handles whose gradients one flat vector carries: all trainable, all of one kind (uq or point estimate)
@@ -1006,18 +1000,12 @@ int32_t lfmq_chain_mask_count(const lfmq_handle* stages, int32_t n_stages, const
     LFMQ_SET_ERR("lfmq_chain_mask_count: null pointer");
     return LFMQ_ERR_ARG;
   }
-  lfmq::ChainUqArgs a{};
-  for (int i = 0; i < n_stages; ++i) {
+  for (int i = 0; i < n_stages; ++i)
     if (!y[i]) {
       LFMQ_SET_ERR("lfmq_chain_mask_count: y[%d] == NULL", i);
       return LFMQ_ERR_ARG;
     }
-    a.y.p[i] = const_cast<float*>(y[i]);
-    a.counts.p[i] = out_dev + 3 * i;
-  }
-  const lfmq_config& c = stages[0]->cfg;
-  return chain_uq_loss_grad((cudaStream_t)stream, n_stages, B, c.seq_len, c.n_outputs, a, c.target_idx, c.target_lambda,
-                            c.rnn_lambda, nullptr, stages[0]->scratch);
+  return stage_counts(stages, n_stages, y, B, out_dev, (cudaStream_t)stream);
 }
 
 int32_t lfmq_chain_grad_pack_size(const lfmq_handle* stages, int32_t n_stages, int64_t* n_elems) {

@@ -14,8 +14,9 @@ def shard_rows(batch_global, rank, world):
 
 
 def global_denominators(local_denom, dist):
-    """{B_local, mask_count_local} -> {B_global, mask_count_global}: the loss denominators are global
-    (losses.py:87,90,131-135), so each rank scales dLoss/dpred with them before the gradient all-reduce.
+    """{B_local, mask_count_local} -> {B_global, mask_count_global}, or any engine's loss_counts -> their sums over the
+    ranks: the loss denominators are global (losses.py:87,90,131-135), so each rank scales dLoss/dpred with them before
+    the gradient all-reduce.
     Targets only -- done once per batch when it is built, not on the step path."""
     out = local_denom.clone()
     dist.all_reduce(out, op=dist.ReduceOp.SUM)

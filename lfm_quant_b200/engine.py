@@ -228,8 +228,8 @@ class ForecasterEngine(object):
         """Data-parallel step: local BPTT with global denominators, ONE NCCL all-reduce over the flat
         gradient (+ loss/mse tail), then the replicated clip + optimizer (SURVEY 8e).
         uq engine: the gradient and {uq_loss, mse_0, uq_loss_last_tar} travel as one packed vector (a chain of one
-        stage, lfmq_chain_grad_pack); x None joins the step without rows.  Returns the global
-        {uq_loss_last_tar, mse_0}, as train_step."""
+        stage, lfmq_chain_grad_pack).  x None (a rank without rows) joins the collective with zeros.  Returns the global
+        {loss, mse_0}, uq engine {uq_loss_last_tar, mse_0}, as train_step."""
         import torch.distributed as dist
         from .dp import allreduce_flat_gradient
         if self.uq:
@@ -239,7 +239,10 @@ class ForecasterEngine(object):
             self.apply(lr, step)
             t = self.grads[self.n_trainable:]
             return torch.stack([t[4], t[1]])
-        self.backward(x, y, step=step, row0=row0, denom=denom_global)
+        if x is None:
+            self.grads[:self.n_trainable + 2].zero_()
+        else:
+            self.backward(x, y, step=step, row0=row0, denom=denom_global)
         allreduce_flat_gradient(self.grads, self.n_trainable, dist)
         self.apply(lr, step)
         return self.grads[self.n_trainable:self.n_trainable + 2].clone()   # not a live view of the workspace tail
@@ -397,6 +400,10 @@ class ForecastChainEngine(object):
         N.check(self.lib.lfmq_chain_mask_count(self._handles, self.S, self._ptrs([y.contiguous() for y in ys]), B,
                                                _ptr(out), _stream()))
         return out
+
+    def loss_counts(self, ys):
+        """mask_count under the name ForecasterEngine gives the counts data parallelism all-reduces."""
+        return self.mask_count(ys)
 
     def backward_dp(self, x, ys, denoms, step=0, row0=0, out=None):
         """backward with the global batch's stage counts (device [S, 3]) as the loss denominators; every stage's tail

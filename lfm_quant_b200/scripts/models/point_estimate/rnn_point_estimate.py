@@ -25,6 +25,14 @@ class _Variable(object):
         return self._model.engine.get_weights()[self._index]
 
 
+def _to_device(engine, inp):
+    """A tensor or ndarray as a contiguous fp32 tensor on the engine's device."""
+    import torch
+    if isinstance(inp, torch.Tensor):
+        return inp.to(engine.device, torch.float32).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(inp, dtype=np.float32)).to(engine.device)
+
+
 class NativeChainForecaster(object):
     """The model object for forecast_steps > 1 (reference :109-150): ``model(inp)`` and ``model.predict(inp)`` return
     the list [pred_1 .. pred_S]; ``train_step`` takes the list of S targets.  Every extra forecast step is one more
@@ -61,11 +69,11 @@ class NativeChainForecaster(object):
 
     def __call__(self, inp, training=None):
         self._calls += 1
-        return self.engine.forward(self._to_device(inp), step=self._calls)
+        return self.engine.forward(_to_device(self.engine, inp), step=self._calls)
 
     def predict_device(self, inp):
         import torch
-        x = self._to_device(inp)
+        x = _to_device(self.engine, inp)
         B, mb = x.shape[0], self.engine.cfg.max_batch
         self._calls += 1
         outs = [self.engine.forward(x[s:s + mb].contiguous(), step=self._calls, row0=s) for s in range(0, B, mb)]
@@ -79,14 +87,15 @@ class NativeChainForecaster(object):
         """Train._train_step_point (train.py:178-199) over the S-output graph; device tensor {loss, mse}.  uq graph:
         Train._train_step_uq_range (train.py:201-225), {uq_loss_last_tar, mse}."""
         assert isinstance(targets, (list, tuple)), 'targets must be the list of forecast_steps targets (train.py:188)'
-        return self.engine.train_step(self._to_device(inp), [self._to_device(t) for t in targets], iteration, lr)
+        return self.engine.train_step(_to_device(self.engine, inp), [_to_device(self.engine, t) for t in targets],
+                                      iteration, lr)
 
     def train_step_dp(self, x, ys, step, lr, row0, denoms):
         """train_step under data parallelism: this rank's rows (x None: none) with the global stage counts `denoms`
         (dp.global_stage_counts), one all-reduce, the replicated apply; returns the global values train_step does."""
         if x is not None:
             assert isinstance(ys, (list, tuple)), 'ys must be the list of forecast_steps targets'
-            x, ys = self._to_device(x), [self._to_device(t) for t in ys]
+            x, ys = _to_device(self.engine, x), [_to_device(self.engine, t) for t in ys]
         return self.engine.train_step_dp(x, ys, step, lr, row0, denoms)
 
     def reset_states(self):
@@ -154,22 +163,16 @@ class NativeForecaster(object):
         self._calls = 0
 
     # -- forward ---------------------------------------------------------------------------------------
-    def _to_device(self, inp):
-        import torch
-        if isinstance(inp, torch.Tensor):
-            return inp.to(self.engine.device, torch.float32).contiguous()
-        return torch.from_numpy(np.ascontiguousarray(inp, dtype=np.float32)).to(self.engine.device)
-
     def __call__(self, inp, training=None):
         """model(inp) (train.py:182): preds [B,T,O] on the device; dropout follows config.train.
         uq model (train.py:204-206): the list [target_preds, variance_preds]; dropout is always on."""
         self._calls += 1
-        out = self.engine.forward(self._to_device(inp), step=self._calls)
+        out = self.engine.forward(_to_device(self.engine, inp), step=self._calls)
         return list(out) if self.uq else out
 
     def predict(self, inp, batch_size=None):
         """model.predict(inp) (train.py:289, predict.py:129): ndarray [B,T,O]."""
-        x = self._to_device(inp)
+        x = _to_device(self.engine, inp)
         B = x.shape[0]
         mb = self.engine.cfg.max_batch
         if self.uq:       # every call draws fresh masks: MC dropout (rnn_uq_range_estimate.py:86,88)
@@ -188,7 +191,7 @@ class NativeForecaster(object):
         HBM, train.py:284-336).  Same dropout semantics as predict()."""
         import torch
         assert not self.uq
-        x = self._to_device(inp)
+        x = _to_device(self.engine, inp)
         B = x.shape[0]
         mb = self.engine.cfg.max_batch
         self._calls += 1
@@ -197,7 +200,7 @@ class NativeForecaster(object):
 
     def train_step(self, inp, targets, lr, iteration):
         """Fused fwd + loss + BPTT + clip + optimizer + MaxNorm; returns a device tensor {loss, mse_0}."""
-        return self.engine.train_step(self._to_device(inp), self._to_device(targets), iteration, lr)
+        return self.engine.train_step(_to_device(self.engine, inp), _to_device(self.engine, targets), iteration, lr)
 
     # -- Keras API surface -------------------------------------------------------------------------------
     def reset_states(self):
@@ -265,9 +268,6 @@ class NativeForecaster(object):
         L = self.config.num_layers
         bn = [(weights[n_tr + 2 * l], weights[n_tr + 2 * l + 1]) for l in range(L)] if len(weights) > n_tr else None
         self.engine.set_weights(weights[:n_tr], bn)
-
-
-NativeChainForecaster._to_device = NativeForecaster._to_device
 
 
 class RNNPointEstimate(BaseModelClass):

@@ -84,15 +84,8 @@ class Train(object):
         x = y = md = None
         if len(inp_idx) > 0:                     # else fewer windows than ranks: this rank only joins the collectives
             x, y, md = self.dataset.get_batch(inp_idx, tar_idx, meta)
-        if self.config.forecast_steps > 1:
-            denom = _dp.global_stage_counts(eng.mask_count(None if y is None else self._step_targets(y)), dist)
-        elif self.config.UQ:
-            denom = _dp.global_stage_counts(eng.loss_counts(y), dist)
-        elif y is None:
-            import torch
-            denom = _dp.global_denominators(torch.zeros(2, dtype=torch.float32, device=eng.device), dist)
-        else:                                    # loss denominators are global (losses.py:87,90,131-135)
-            denom = _dp.global_denominators(eng.mask_count(y), dist)
+        # loss denominators are global (losses.py:87,90,131-135); a rank without rows adds zeros
+        denom = _dp.global_denominators(eng.loss_counts(None if y is None else self._step_targets(y)), dist)
         return (x, y, md, row0, denom)
 
     def train(self):
@@ -168,40 +161,16 @@ class Train(object):
         self.optimizer.iterations += 1
         return out[1]
 
-    def _train_step_point_dp(self, cur_batch):
-        """train.py:178-199 under data parallelism: local BPTT with global denominators, ONE all-reduce of the flat
-        gradient (+ loss / mse tail), replicated clip + optimizer + MaxNorm.  Same trajectory as one GPU."""
-        assert not self.config.UQ, 'data parallelism is built for the point-estimate model'
-        import torch.distributed as dist
-        from ..dp import allreduce_flat_gradient
-        eng = self.model.engine
-        inp, targets, _, row0, denom = cur_batch
-        lr = self.optimizer.current_lr()
-        it = self.optimizer.iterations
-        if inp is None:
-            eng.grads[:eng.n_trainable + 2].zero_()
-            allreduce_flat_gradient(eng.grads, eng.n_trainable, dist)
-            eng.apply(lr, it)
-            out = eng.grads[eng.n_trainable:eng.n_trainable + 2].clone()
-        else:
-            out = eng.train_step_dp(inp, targets, it, lr, row0, denom)
-        self.optimizer.iterations += 1
-        return out[1]
-
     def _train_step_dp(self, cur_batch):
-        """One data-parallel step of any model: (uq_loss_last_tar or None, mse), both global device scalars.  The point
-        estimate reduces its flat gradient in place; RNNUqRangeEstimate and multi-step forecasts all-reduce the packed
-        vector of every stage's gradients and loss tail (ForecastChainEngine.train_step_dp)."""
-        if self.config.forecast_steps == 1 and not self.config.UQ:
-            return None, self._train_step_point_dp(cur_batch)
+        """One data-parallel step of any model (train.py:178-225): local BPTT with global denominators, ONE all-reduce,
+        replicated clip + optimizer + MaxNorm; a rank without rows joins with zeros.  Same trajectory as one GPU.
+        Returns (uq_loss_last_tar or None, mse), both global device scalars.  The point estimate reduces its flat
+        gradient in place (ForecasterEngine.train_step_dp); RNNUqRangeEstimate and multi-step forecasts all-reduce the
+        packed vector of every stage's gradients and loss tail (ForecastChainEngine.train_step_dp)."""
         inp, targets, _, row0, denom = cur_batch
-        lr = self.optimizer.current_lr()
-        it = self.optimizer.iterations
-        if self.config.forecast_steps > 1:
-            out = self.model.train_step_dp(inp, None if inp is None else self._step_targets(targets), it, lr, row0,
-                                           denom)
-        else:
-            out = self.model.engine.train_step_dp(inp, targets, it, lr, row0, denom)
+        step = self.model.train_step_dp if self.config.forecast_steps > 1 else self.model.engine.train_step_dp
+        out = step(inp, None if inp is None else self._step_targets(targets), self.optimizer.iterations,
+                   self.optimizer.current_lr(), row0, denom)
         self.optimizer.iterations += 1
         return (out[0] if self.config.UQ else None), out[1]
 

@@ -71,6 +71,20 @@ def test_uq_chain_forward_loss_and_gradients_match_oracle(shape, cell):
     eng.close()
 
 
+def test_later_stage_called_on_its_own_keeps_its_dropout_streams():
+    """Stage 1's engine alone, on the window the chain built for it, draws the masks it drew inside the chain: the
+    single-handle entry points leave the Philox stream numbering of the chain in place."""
+    B, T, F, O, H, L, S = 9, 6, 8, 4, 16, 2, 2
+    P, x, _ = _problem(B, T, F, O, H, L, S, seed=7)
+    eng = _engine(B, T, F, O, H, L, S, [1.0, 0.5], train=True, **KW, **DROP)
+    eng.set_weights(P)
+    out = [o.cpu().numpy() for o in eng.forward(_cuda(x), step=3, row0=17)]
+    window = eng._work[:B * T * F].view(B, T, F).clone()
+    p1, v1 = eng.stages[1].forward(window, step=3, row0=17)
+    assert np.array_equal(p1.cpu().numpy(), out[2]) and np.array_equal(v1.cpu().numpy(), out[3])
+    eng.close()
+
+
 @pytest.mark.parametrize('optimizer', ['Adadelta', 'Adam'])
 def test_uq_chain_train_steps_match_oracle(optimizer):
     """Joint clip_by_global_norm over every stage (train.py:214-216), the optimizer, MaxNorm on every recurrent kernel."""
