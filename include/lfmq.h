@@ -104,6 +104,46 @@ int32_t lfmq_set_device_share(lfmq_handle h, int32_t num, int32_t den);
  * whole device, else floor(sm_count * num / den), one CTA per SM. */
 int32_t lfmq_persistent_cta_budget(int32_t sm_count, int32_t ctas_per_sm, int32_t num, int32_t den, int64_t* budget);
 
+/* ---- the linear baseline: MLPLinearPointEstimate (models/point_estimate/mlp_linear_point_estimate.py:66-77) ----
+ * One Dense(O) layer OUTPUT_1 over the flattened input window: preds[B,O] = x[B, T*F] W[T*F, O] + b.  x is the [B,T,F]
+ * batch viewed as [B, T*F] (data_processing.py:363-365); y and preds are the last step only, [B,O].  A dense handle is
+ * an ordinary lfmq_handle: lfmq_param_count / lfmq_param_spec (OUTPUT_1/kernel [T*F, O], OUTPUT_1/bias [O]), the
+ * parameter, gradient and optimizer-slot pointers, lfmq_set_params / lfmq_get_params, lfmq_apply (clip and optimizer;
+ * no MaxNorm), lfmq_set_device_share, profiling and lfmq_destroy work on it unchanged, and
+ *   lfmq_forward     x [B, T*F] -> preds [B,O] (step and row0 are ignored: the model has no dropout)
+ *   lfmq_loss        the MLP branch of Losses._get_loss_point_estimate (losses.py:69-75,100-115) in its MSE form, as
+ *                    validation evaluates it (is_validation=True): out_dev = {target_lambda * mse_0 +
+ *                    (1 - target_lambda) * mse_all, mse_0}; rows whose targets are all zero have their predictions
+ *                    zeroed and count in both denominators, B and B * O
+ *   lfmq_mask_count  out_dev = {B, rows whose targets are not all zero}, as on a recurrent handle
+ *   lfmq_backward    forward, the loss (Keras Huber terms when huber_loss, losses.py:102-105) and the gradients of the
+ *                    kernel and the bias; denom_dev = {B_global, ...} (lfmq_mask_count summed over the ranks) or NULL
+ *   lfmq_train_step  lfmq_backward + lfmq_apply, loss_out_dev = {loss, mse_0}
+ * dispatch on it.  The uq and chain entry points refuse it.  fp32 only: the model reads every byte of x once for O
+ * multiply-adds each, so it is bound by memory, not arithmetic, and LFMQ_PREC_BF16 / LFMQ_PREC_BF16X3 are refused at
+ * create with LFMQ_ERR_UNSUPPORTED.  All kernels are deterministic (fixed reduction orders, no atomics); a row's
+ * prediction does not depend on the other rows of the batch. */
+typedef struct lfmq_dense_config {   /* 56 bytes: 10 int32 + 4 float */
+  int32_t struct_size;       /* sizeof(lfmq_dense_config), ABI guard */
+  int32_t max_batch;         /* largest B any call will pass (per rank) */
+  int32_t seq_len;           /* T */
+  int32_t n_inputs;          /* F; the kernel has T * F rows (<= 48 * 1024) */
+  int32_t n_outputs;         /* O */
+  int32_t target_idx;        /* Dataset.target_index */
+  int32_t precision;         /* LFMQ_PREC_FP32 */
+  int32_t optimizer;         /* LFMQ_OPT_* */
+  int32_t forward_only;      /* 1: no gradient or optimizer workspace (predict.py) */
+  int32_t huber_loss;        /* config.huber_loss: the training loss uses Keras Huber terms (losses.py:102-105) */
+  float target_lambda;       /* lfm_quant.py:69 */
+  float huber_delta;         /* config.huber_delta */
+  float max_grad_norm;       /* <= 0 disables clipping (train.py:195) */
+  float sgd_momentum;
+} lfmq_dense_config;
+int32_t lfmq_dense_workspace_bytes(const lfmq_dense_config* cfg, uint64_t* bytes);
+/* Replaces MLPLinearPointEstimate(config, dataset).model.  Parameters start zeroed; the host initialiser uploads them
+ * with lfmq_set_params. */
+int32_t lfmq_dense_create(const lfmq_dense_config* cfg, void* workspace, uint64_t workspace_bytes, lfmq_handle* out);
+
 /* model.trainable_variables / model.weights (train.py:192,198): tensors are listed in Keras order,
  * trainable ones first: per layer lstm_l/{kernel,recurrent_kernel,bias} (gru_l/... with bias [2][3H] for LFMQ_CELL_GRU), batch_normalization[_k]/{gamma,beta};
  * OUTPUT_1/{kernel,bias} (uq: OUTPUT_TARGET_1/{kernel,bias}, OUTPUT_VARIANCE_1/{kernel,bias}); then per layer batch_normalization[_k]/{moving_mean,moving_variance}. */

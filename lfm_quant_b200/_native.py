@@ -27,6 +27,13 @@ class LfmqConfig(C.Structure):
                 ('sgd_momentum', C.c_float), ('bn_epsilon', C.c_float), ('seed', C.c_uint64)]
 
 
+class LfmqDenseConfig(C.Structure):
+    _fields_ = [('struct_size', C.c_int32), ('max_batch', C.c_int32), ('seq_len', C.c_int32), ('n_inputs', C.c_int32),
+                ('n_outputs', C.c_int32), ('target_idx', C.c_int32), ('precision', C.c_int32), ('optimizer', C.c_int32),
+                ('forward_only', C.c_int32), ('huber_loss', C.c_int32), ('target_lambda', C.c_float),
+                ('huber_delta', C.c_float), ('max_grad_norm', C.c_float), ('sgd_momentum', C.c_float)]
+
+
 class LfmqGatherArgs(C.Structure):
     _fields_ = [('struct_size', C.c_int32), ('n_rows', C.c_int32), ('n_cols', C.c_int32), ('B', C.c_int32),
                 ('T', C.c_int32), ('F', C.c_int32), ('O', C.c_int32), ('stride', C.c_int32),
@@ -53,6 +60,8 @@ SYMBOLS = {
     'lfmq_workspace_bytes': (C.c_int32, [C.POINTER(LfmqConfig), C.POINTER(C.c_uint64)]),
     'lfmq_create': (C.c_int32, [C.POINTER(LfmqConfig), _P, C.c_uint64, C.POINTER(_P)]),
     'lfmq_destroy': (C.c_int32, [_P]),
+    'lfmq_dense_workspace_bytes': (C.c_int32, [C.POINTER(LfmqDenseConfig), C.POINTER(C.c_uint64)]),
+    'lfmq_dense_create': (C.c_int32, [C.POINTER(LfmqDenseConfig), _P, C.c_uint64, C.POINTER(_P)]),
     'lfmq_set_device_share': (C.c_int32, [_P, C.c_int32, C.c_int32]),
     'lfmq_persistent_cta_budget': (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     'lfmq_param_count': (C.c_int32, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),

@@ -8,6 +8,7 @@
 #include <string>
 #include <vector>
 
+#include "dense.h"
 #include "kernels.h"
 #include "lstm_tc.h"
 #include "rnn_tc.h"
@@ -53,6 +54,12 @@ struct lfmq_handle_s {
   int64_t last_row0 = 0;
   int use_gen;               // 1: the general tensor-core path (rnn_tc.cu) runs this handle's bf16 / bf16x3 work
   lfmq::Profiler prof;
+  // the linear baseline (lfmq_dense_create): cfg carries its shapes, target, loss weight, optimizer and clip, with
+  // num_layers = 0; params = [OUTPUT_1/kernel [T*F, O], OUTPUT_1/bias [O]]
+  int dense = 0;
+  int huber = 0;
+  float huber_delta = 1.f;
+  float* wpart = nullptr;    // row-block partials of the weight gradient (dense_wgrad)
 };
 
 namespace {
@@ -214,6 +221,90 @@ size_t layout(lfmq_handle_s* h, char* base) {
     }
   }
   return cv.off;
+}
+
+int validate_dense(const lfmq_dense_config* c) {
+  if (!c || c->struct_size != (int32_t)sizeof(lfmq_dense_config)) {
+    LFMQ_SET_ERR("lfmq_dense_config: struct_size mismatch (got %d, want %zu)", c ? c->struct_size : -1,
+                 sizeof(lfmq_dense_config));
+    return LFMQ_ERR_ARG;
+  }
+  if (c->max_batch <= 0 || c->seq_len <= 0 || c->n_inputs <= 0 || c->n_outputs <= 0) {
+    LFMQ_SET_ERR("lfmq_dense_config: non-positive dimension");
+    return LFMQ_ERR_ARG;
+  }
+  if ((int64_t)c->seq_len * c->n_inputs > 48 * 1024) {
+    LFMQ_SET_ERR("lfmq_dense_config: seq_len * n_inputs = %lld exceeds %d", (long long)c->seq_len * c->n_inputs,
+                 48 * 1024);
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  if (c->target_idx < 0 || c->target_idx >= c->n_outputs) {
+    LFMQ_SET_ERR("lfmq_dense_config: target_idx %d outside [0,%d)", c->target_idx, c->n_outputs);
+    return LFMQ_ERR_ARG;
+  }
+  if (c->optimizer < 0 || c->optimizer > 3) {
+    LFMQ_SET_ERR("lfmq_dense_config: unknown optimizer %d", c->optimizer);
+    return LFMQ_ERR_ARG;
+  }
+  if (c->huber_loss && !(c->huber_delta > 0.f)) {
+    LFMQ_SET_ERR("lfmq_dense_config: huber_delta must be positive (got %g)", c->huber_delta);
+    return LFMQ_ERR_ARG;
+  }
+  if (c->precision == LFMQ_PREC_BF16 || c->precision == LFMQ_PREC_BF16X3) {
+    LFMQ_SET_ERR("lfmq_dense_config: the linear model runs in fp32 only: it reads each input once for n_outputs "
+                 "multiply-adds, so it is bound by memory bandwidth and tensor cores would not make it faster; "
+                 "use LFMQ_PREC_FP32");
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  if (c->precision != LFMQ_PREC_FP32) {
+    LFMQ_SET_ERR("lfmq_dense_config: unknown precision %d", c->precision);
+    return LFMQ_ERR_ARG;
+  }
+  return LFMQ_OK;
+}
+
+// The dense handle's specs and workspace; with base == nullptr only sizes are computed.
+size_t dense_layout(lfmq_handle_s* h, char* base) {
+  const lfmq_config& c = h->cfg;
+  const int K = c.seq_len * c.n_inputs, O = c.n_outputs;
+  h->specs.clear();
+  h->specs.push_back(ParamSpec{"OUTPUT_1/kernel", 2, {K, O}, 0, 1});
+  h->specs.push_back(ParamSpec{"OUTPUT_1/bias", 1, {O, 1}, (int64_t)K * O, 1});
+  h->layers.clear();
+  h->oWo = 0;
+  h->obo = (int64_t)K * O;
+  h->oWv = h->obv = -1;
+  h->n_train = h->n_total = (int64_t)(K + 1) * O;
+  h->n_grad_buf = (h->n_train + 8 + 3) / 4 * 4;
+  h->n_slots = (c.optimizer == LFMQ_OPT_ADADELTA || c.optimizer == LFMQ_OPT_ADAM) ? 2 : 1;
+  Carver cv{base, 0};
+  h->params = cv.take<float>(h->n_total);
+  h->grads = cv.take<float>(h->n_grad_buf);
+  h->slots = c.forward_only ? nullptr : cv.take<float>((size_t)h->n_slots * h->n_train);
+  h->scalars = cv.take<float>(16);
+  h->denom = h->scalars + 8;
+  h->tickets = reinterpret_cast<unsigned int*>(h->scalars);
+  h->z = h->zh = h->hm = h->var = h->apre = nullptr;
+  h->dz = h->dz2 = h->dy = h->dh_out = h->hp = h->dh_rec = h->dc = h->da = nullptr;
+  h->preds = h->dpred = h->wpart = nullptr;
+  if (!c.forward_only) {
+    h->preds = cv.take<float>((size_t)c.max_batch * O);
+    h->dpred = cv.take<float>((size_t)c.max_batch * O);
+    h->wpart = cv.take<float>(lfmq::dense_wgrad_scratch(c.max_batch, K, O));
+  }
+  h->scratch_elems = (size_t)4 << 20;      // lfmq_loss (any B) and grad_norm_scale
+  h->scratch = cv.take<float>(h->scratch_elems);
+  h->use_gen = 0;
+  return cv.off;
+}
+
+// Entry points that serve recurrent handles only.
+int refuse_dense(lfmq_handle h, const char* fn) {
+  if (h && h->dense) {
+    LFMQ_SET_ERR("%s: not defined for a dense handle (lfmq_dense_create)", fn);
+    return LFMQ_ERR_ARG;
+  }
+  return 0;
 }
 
 #define RUN(expr)                 \
@@ -570,6 +661,71 @@ int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_
   return LFMQ_OK;
 }
 
+namespace {
+void dense_handle_config(const lfmq_dense_config* d, lfmq_handle_s* h) {
+  lfmq_config& c = h->cfg;
+  memset(&c, 0, sizeof(c));
+  c.struct_size = (int32_t)sizeof(lfmq_config);
+  c.max_batch = d->max_batch;
+  c.seq_len = d->seq_len;
+  c.n_inputs = d->n_inputs;
+  c.n_outputs = d->n_outputs;
+  c.target_idx = d->target_idx;
+  c.precision = d->precision;
+  c.optimizer = d->optimizer;
+  c.forward_only = d->forward_only;
+  c.target_lambda = d->target_lambda;
+  c.max_grad_norm = d->max_grad_norm;
+  c.sgd_momentum = d->sgd_momentum;
+  h->dense = 1;
+  h->huber = d->huber_loss ? 1 : 0;
+  h->huber_delta = d->huber_delta;
+}
+}  // namespace
+
+int32_t lfmq_dense_workspace_bytes(const lfmq_dense_config* cfg, uint64_t* bytes) {
+  RUN(validate_dense(cfg));
+  if (!bytes) {
+    LFMQ_SET_ERR("bytes == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  lfmq_handle_s tmp;
+  dense_handle_config(cfg, &tmp);
+  *bytes = dense_layout(&tmp, nullptr) + WS_ALIGN;
+  return LFMQ_OK;
+}
+
+int32_t lfmq_dense_create(const lfmq_dense_config* cfg, void* workspace, uint64_t workspace_bytes, lfmq_handle* out) {
+  RUN(validate_dense(cfg));
+  if (!workspace || !out) {
+    LFMQ_SET_ERR("workspace/out == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  lfmq_handle_s* h = new lfmq_handle_s;
+  dense_handle_config(cfg, h);
+  char* base = reinterpret_cast<char*>(ws_align_up(reinterpret_cast<size_t>(workspace)));
+  const size_t need = dense_layout(h, nullptr) + (base - reinterpret_cast<char*>(workspace));
+  if (need > workspace_bytes) {
+    LFMQ_SET_ERR("workspace too small: need %zu bytes, got %llu", need, (unsigned long long)workspace_bytes);
+    delete h;
+    return LFMQ_ERR_WORKSPACE;
+  }
+  dense_layout(h, base);
+  h->tc.prof = &h->prof;
+  cudaError_t e = cudaMemsetAsync(h->params, 0, sizeof(float) * h->n_total, 0);
+  if (e == cudaSuccess) e = cudaMemsetAsync(h->grads, 0, sizeof(float) * h->n_grad_buf, 0);
+  if (e == cudaSuccess && h->slots) e = cudaMemsetAsync(h->slots, 0, sizeof(float) * h->n_slots * h->n_train, 0);
+  if (e == cudaSuccess) e = cudaMemsetAsync(h->scalars, 0, sizeof(float) * 16, 0);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+  if (e != cudaSuccess) {
+    LFMQ_SET_ERR("lfmq_dense_create: %s", cudaGetErrorString(e));
+    delete h;
+    return LFMQ_ERR_CUDA;
+  }
+  *out = h;
+  return LFMQ_OK;
+}
+
 int32_t lfmq_destroy(lfmq_handle h) {
   if (h) {
     lfmq::tc_destroy(h->tc);
@@ -688,6 +844,13 @@ int32_t lfmq_forward(lfmq_handle h, const float* x, int32_t B, int64_t row0, int
     LFMQ_SET_ERR("lfmq_forward: uq handle, call lfmq_forward_uq");
     return LFMQ_ERR_ARG;
   }
+  if (h->dense) {
+    const lfmq_config& c = h->cfg;
+    h->prof.begin(LFMQ_REGION_FWD, s);
+    RUN(dense_forward(s, x, B, c.seq_len * c.n_inputs, c.n_outputs, h->params + h->oWo, h->params + h->obo, preds));
+    h->prof.end(LFMQ_REGION_FWD, s);
+    return LFMQ_OK;
+  }
   if (h->use_gen) return lfmq::gen_forward(h->tc, h->cfg, h->params, x, B, row0, step, preds, s);
   if (h->cfg.precision == LFMQ_PREC_BF16)
     return lfmq::tc_forward(h->tc, h->cfg, h->params, x, B, row0, step, preds, /*save=*/false, s);
@@ -722,6 +885,9 @@ int32_t lfmq_loss(lfmq_handle h, const float* preds, const float* y, int32_t B, 
     return LFMQ_ERR_ARG;
   }
   const lfmq_config& c = h->cfg;
+  if (h->dense)      // validation: the MSE form whatever huber_loss is (losses.py:102, is_validation=True)
+    return dense_loss((cudaStream_t)stream, preds, y, B, c.n_outputs, nullptr, c.target_idx, c.target_lambda, 0, 1.f,
+                      nullptr, out_dev, h->scratch);
   return loss_grad((cudaStream_t)stream, B, c.seq_len, c.n_outputs, preds, y, nullptr, c.target_idx, c.target_lambda,
                    c.rnn_lambda, nullptr, out_dev, nullptr, h->scratch);
 }
@@ -732,6 +898,7 @@ int32_t lfmq_loss_uq(lfmq_handle h, const float* preds, const float* var, const 
     LFMQ_SET_ERR("lfmq_loss_uq: bad handle, batch %d or null pointer", B);
     return LFMQ_ERR_ARG;
   }
+  RUN(refuse_dense(h, "lfmq_loss_uq"));
   const lfmq_config& c = h->cfg;
   lfmq::ChainUqArgs a{};      // one stage of weight 1: the weighted sums {uq_loss, uq_loss_last_tar, mse} are its own
   a.pred.p[0] = const_cast<float*>(preds);
@@ -748,6 +915,9 @@ int32_t lfmq_mask_count(lfmq_handle h, const float* y, int32_t B, float* out_dev
     LFMQ_SET_ERR("lfmq_mask_count: null pointer");
     return LFMQ_ERR_ARG;
   }
+  if (h->dense)
+    return dense_loss((cudaStream_t)stream, nullptr, y, B, h->cfg.n_outputs, nullptr, 0, 0.f, 0, 1.f, nullptr, out_dev,
+                      h->scratch);
   return mask_count((cudaStream_t)stream, B, h->cfg.seq_len, h->cfg.n_outputs, y, out_dev, h->tickets);
 }
 
@@ -757,6 +927,7 @@ int32_t lfmq_mask_count_uq(lfmq_handle h, const float* y, int32_t B, float* out_
     LFMQ_SET_ERR("lfmq_mask_count_uq: null pointer");
     return LFMQ_ERR_ARG;
   }
+  RUN(refuse_dense(h, "lfmq_mask_count_uq"));
   return stage_counts(&h, 1, &y, B, out_dev, (cudaStream_t)stream);
 }
 
@@ -773,6 +944,21 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
   }
   cudaStream_t s = (cudaStream_t)stream;
   const lfmq_config& c = h->cfg;
+  if (h->dense) {    // the forward into the handle's own preds, the loss and dLoss/dpred, then dW and db
+    const int K = c.seq_len * c.n_inputs, O = c.n_outputs;
+    float* tail = h->grads + h->n_train;
+    h->prof.begin(LFMQ_REGION_FWD, s);
+    RUN(dense_forward(s, x, B, K, O, h->params + h->oWo, h->params + h->obo, h->preds));
+    h->prof.end(LFMQ_REGION_FWD, s);
+    h->prof.begin(LFMQ_REGION_HEAD, s);
+    RUN(dense_loss(s, h->preds, y, B, O, denom_dev, c.target_idx, c.target_lambda, h->huber, h->huber_delta, h->dpred,
+                   tail, h->scratch));
+    h->prof.end(LFMQ_REGION_HEAD, s);
+    h->prof.begin(LFMQ_REGION_WGRAD, s);
+    RUN(dense_wgrad(s, x, h->dpred, B, K, O, h->wpart, h->grads));
+    h->prof.end(LFMQ_REGION_WGRAD, s);
+    return LFMQ_OK;
+  }
   if (c.precision == LFMQ_PREC_FP32) {      // a trainable uq handle is always fp32
     // denom_dev: stage 0's counts, the three of lfmq_mask_count_uq or the two of lfmq_mask_count
     const float one = 1.0f;
@@ -831,6 +1017,7 @@ int chain_check(const lfmq_handle* st, int32_t S, int32_t B, bool training) {
   }
   for (int i = 0; i < S; ++i) {
     RUN(check_batch(st[i], B));
+    RUN(refuse_dense(st[i], "lfmq_chain"));
     const lfmq_config& c = st[i]->cfg;
     const lfmq_config& c0 = st[0]->cfg;
     if (c.seq_len != c0.seq_len || c.n_inputs != c0.n_inputs || c.n_outputs != c0.n_outputs || c.uq != c0.uq ||
@@ -905,6 +1092,7 @@ int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float
       LFMQ_SET_ERR("lfmq_chain_loss: null handle");
       return LFMQ_ERR_ARG;
     }
+    RUN(refuse_dense(stages[i], "lfmq_chain_loss"));
     l2.p[i] = stages[i]->scalars + 12;      // two spare floats of the handle's scalar block (denom uses 8..10)
     RUN(lfmq_loss(stages[i], preds[i], y[i], B, l2.p[i], stream));
     w.w[i] = weights[i];
@@ -922,7 +1110,7 @@ int32_t lfmq_chain_loss_uq(const lfmq_handle* stages, int32_t n_stages, const fl
   }
   lfmq::ChainUqArgs a{};
   for (int i = 0; i < n_stages; ++i) {
-    if (!stages[i] || !stages[i]->cfg.uq || !preds[i] || !vars[i] || !y[i]) {
+    if (!stages[i] || !stages[i]->cfg.uq || stages[i]->dense || !preds[i] || !vars[i] || !y[i]) {
       LFMQ_SET_ERR("lfmq_chain_loss_uq: stage %d: null pointer or a point-estimate handle", i);
       return LFMQ_ERR_ARG;
     }
@@ -962,8 +1150,8 @@ int pack_check(const lfmq_handle* st, int32_t S, const char* fn, lfmq::GradPack*
   }
   int64_t off = 0;
   for (int i = 0; i < S; ++i) {
-    if (!st[i] || st[i]->cfg.forward_only || st[i]->cfg.uq != st[0]->cfg.uq) {
-      LFMQ_SET_ERR("%s: stage %d is null, forward_only or of another kind than stage 0", fn, i);
+    if (!st[i] || st[i]->cfg.forward_only || st[i]->cfg.uq != st[0]->cfg.uq || st[i]->dense) {
+      LFMQ_SET_ERR("%s: stage %d is null, forward_only, a dense handle or of another kind than stage 0", fn, i);
       return LFMQ_ERR_ARG;
     }
     p->g[i] = st[i]->grads;
@@ -1055,8 +1243,8 @@ int32_t lfmq_chain_apply(const lfmq_handle* stages, int32_t n_stages, float lr, 
   lfmq::ChainWeights w{};
   for (int i = 0; i < n_stages; ++i) {
     lfmq_handle h = stages[i];
-    if (!h || h->cfg.forward_only) {
-      LFMQ_SET_ERR("lfmq_chain_apply: bad handle");
+    if (!h || h->cfg.forward_only || h->dense) {
+      LFMQ_SET_ERR("lfmq_chain_apply: bad handle (null, forward_only or dense)");
       return LFMQ_ERR_ARG;
     }
     float* tail = h->grads + h->n_train;

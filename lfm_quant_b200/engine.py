@@ -21,51 +21,11 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-class ForecasterEngine(object):
-    """fwd / loss / BPTT / clip / optimizer / MaxNorm for RNNPointEstimate on one GPU.
+class _HandleEngine(object):
+    """What every native handle offers whatever its model: parameter specs and views, weights in Keras order, the
+    device share, the optimizer apply, the mask count, un-scaling and profiling."""
 
-    Mirrors what the reference builds in RNNPointEstimate._build_model
-    (scripts/models/point_estimate/rnn_point_estimate.py:40-107) plus the step body of
-    Train._train_step_point (scripts/train.py:178-199).
-    """
-
-    def __init__(self, *, max_batch, seq_len, n_inputs, n_outputs, num_hidden, num_layers=1, target_idx=0,
-                 train=True, precision='fp32', optimizer='Adadelta', dropout=0.0, recurrent_dropout=0.0,
-                 target_lambda=0.5, rnn_lambda=0.7, max_grad_norm=50.0, max_norm=3.0, sgd_momentum=0.0,
-                 seed=521, forward_only=False, device=None, rnn_cell='lstm', uq=False):
-        if not torch.cuda.is_available():
-            raise N.LfmqError('ForecasterEngine needs a CUDA device (no CPU fallback)')
-        self.lib = N.load()
-        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-        if optimizer not in N.OPTIMIZERS:
-            raise ValueError("%s optimizer not found in tf.keras.optimizers" % optimizer)
-        cfg = N.LfmqConfig()
-        cfg.struct_size = C.sizeof(N.LfmqConfig)
-        cfg.max_batch, cfg.seq_len, cfg.n_inputs, cfg.n_outputs = max_batch, seq_len, n_inputs, n_outputs
-        cfg.num_hidden, cfg.num_layers, cfg.target_idx = num_hidden, num_layers, target_idx
-        cfg.train = 1 if train else 0
-        cfg.precision = {'fp32': N.PREC_FP32, 'bf16': N.PREC_BF16, 'bf16x3': N.PREC_BF16X3}[precision]
-        cfg.optimizer = N.OPTIMIZERS[optimizer]
-        cfg.forward_only = 1 if forward_only else 0
-        if rnn_cell not in N.CELLS:
-            raise NotImplementedError('rnn_cell=%s (rnn_point_estimate.py:80-102 knows lstm and gru)' % rnn_cell)
-        cfg.rnn_cell = N.CELLS[rnn_cell]
-        cfg.uq = 1 if uq else 0
-        self.uq = bool(uq)
-        cfg.dropout, cfg.recurrent_dropout = dropout, recurrent_dropout
-        cfg.target_lambda, cfg.rnn_lambda = target_lambda, rnn_lambda
-        cfg.max_grad_norm, cfg.max_norm, cfg.sgd_momentum = max_grad_norm, max_norm, sgd_momentum
-        cfg.bn_epsilon = 1e-3
-        cfg.seed = seed
-        self.cfg = cfg
-        self.precision = precision
-        self.T, self.F, self.O, self.H, self.L = seq_len, n_inputs, n_outputs, num_hidden, num_layers
-        nbytes = C.c_uint64(0)
-        N.check(self.lib.lfmq_workspace_bytes(C.byref(cfg), C.byref(nbytes)))
-        with torch.cuda.device(self.device):
-            self.workspace = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
-            self.handle = C.c_void_p(0)
-            N.check(self.lib.lfmq_create(C.byref(cfg), _ptr(self.workspace), nbytes, C.byref(self.handle)))
+    def _read_specs(self):
         nt, ntr, ntot = C.c_int32(0), C.c_int64(0), C.c_int64(0)
         N.check(self.lib.lfmq_param_count(self.handle, C.byref(nt), C.byref(ntr), C.byref(ntot)))
         self.n_trainable, self.n_total = ntr.value, ntot.value
@@ -80,8 +40,6 @@ class ForecasterEngine(object):
             self.specs.append((name.value.decode(), shp, off.value, bool(tr.value)))
         self.params = self._view('lfmq_params_ptr', self.n_total)
         self.grads = self._view('lfmq_grads_ptr', self.n_trainable + 8)   # tail: loss, mse_0, grad_norm, clip_scale, uq_loss_last_tar
-        self._denom = torch.zeros(2, dtype=torch.float32, device=self.device)
-        self._dp = None
 
     def _view(self, fn, n):
         p = C.c_void_p(0)
@@ -155,32 +113,6 @@ class ForecasterEngine(object):
         assert x.dim() == 3 and x.shape[1] == self.T and x.shape[2] == self.F, tuple(x.shape)
         return x.shape[0]
 
-    def forward(self, x, step=0, row0=0, out=None):
-        """preds [B,T,O]; on a uq engine the pair (preds, variance) -- model(inp)[0], model(inp)[1] of RNNUqRangeEstimate."""
-        B = self._check_x(x)
-        if self.uq:
-            preds = torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device)
-            var = torch.empty_like(preds)
-            N.check(self.lib.lfmq_forward_uq(self.handle, _ptr(x), B, row0, step, _ptr(preds), _ptr(var), _stream()))
-            return preds, var
-        if out is None:
-            out = torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device)
-        N.check(self.lib.lfmq_forward(self.handle, _ptr(x), B, row0, step, _ptr(out), _stream()))
-        return out
-
-    def loss(self, preds, y):
-        out = torch.empty(2, dtype=torch.float32, device=preds.device)
-        N.check(self.lib.lfmq_loss(self.handle, _ptr(preds.contiguous()), _ptr(y.contiguous()), preds.shape[0],
-                                   _ptr(out), _stream()))
-        return out
-
-    def loss_uq(self, preds, var, y):
-        """Device tensor {uq_loss, uq_loss_last_tar, mse_0} (Losses.weight_adjusted_uq_loss, losses.py:137-284)."""
-        out = torch.empty(3, dtype=torch.float32, device=preds.device)
-        N.check(self.lib.lfmq_loss_uq(self.handle, _ptr(preds.contiguous()), _ptr(var.contiguous()), _ptr(y.contiguous()),
-                                      preds.shape[0], _ptr(out), _stream()))
-        return out
-
     def unscale(self, arr, scale, center, log_squasher):
         """Train._unscale_preds (train.py:420-432) on the device: arr [..., O] fp32, scale / center fp64 CUDA tensors."""
         a = arr.contiguous()
@@ -194,26 +126,14 @@ class ForecasterEngine(object):
         N.check(self.lib.lfmq_mask_count(self.handle, _ptr(y), y.shape[0], _ptr(out), _stream()))
         return out
 
-    def mask_count_uq(self, y):
-        """Device {B, unmasked rows, unmasked last-step rows}: the denominators of the uq loss (losses.py:179-284)."""
-        out = torch.empty(3, dtype=torch.float32, device=y.device)
-        N.check(self.lib.lfmq_mask_count_uq(self.handle, _ptr(y), y.shape[0], _ptr(out), _stream()))
-        return out
-
-    def loss_counts(self, y):
-        """The loss denominators of one batch that data parallelism all-reduces: mask_count_uq on a uq engine, else
-        mask_count.  y None (a rank without rows): zeros of the same length."""
-        if y is None:
-            return torch.zeros(3 if self.uq else 2, dtype=torch.float32, device=self.device)
-        return self.mask_count_uq(y) if self.uq else self.mask_count(y)
-
-    def backward(self, x, y, step=0, row0=0, denom=None):
-        B = self._check_x(x)
-        assert y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and tuple(y.shape) == (B, self.T, self.O)
-        N.check(self.lib.lfmq_backward(self.handle, _ptr(x), _ptr(y), B, row0, step, _ptr(denom), _stream()))
-
     def apply(self, lr, iteration):
         N.check(self.lib.lfmq_apply(self.handle, float(lr), int(iteration), _stream()))
+
+    def loss(self, preds, y):
+        out = torch.empty(2, dtype=torch.float32, device=preds.device)
+        N.check(self.lib.lfmq_loss(self.handle, _ptr(preds.contiguous()), _ptr(y.contiguous()), preds.shape[0],
+                                   _ptr(out), _stream()))
+        return out
 
     def train_step(self, x, y, step, lr, out=None):
         """One Train._train_step_point on this GPU; returns a device tensor {loss, mse_0} (no host sync).
@@ -224,21 +144,12 @@ class ForecasterEngine(object):
         N.check(self.lib.lfmq_train_step(self.handle, _ptr(x), _ptr(y), B, 0, step, float(lr), _ptr(out), _stream()))
         return out
 
-    def train_step_dp(self, x, y, step, lr, row0, denom_global):
-        """Data-parallel step: local BPTT with global denominators, ONE NCCL all-reduce over the flat
-        gradient (+ loss/mse tail), then the replicated clip + optimizer (SURVEY 8e).
-        uq engine: the gradient and {uq_loss, mse_0, uq_loss_last_tar} travel as one packed vector (a chain of one
-        stage, lfmq_chain_grad_pack).  x None (a rank without rows) joins the collective with zeros.  Returns the global
-        {loss, mse_0}, uq engine {uq_loss_last_tar, mse_0}, as train_step."""
+    def _train_step_dp_flat(self, x, y, step, lr, row0, denom_global):
+        """The data-parallel step of a handle whose gradient and {loss, mse_0} tail are one contiguous vector: local
+        backward with the global denominators, ONE all-reduce of grads[0 : n_trainable + 2], the replicated apply.
+        x None (a rank without rows) joins with zeros.  Returns the global {loss, mse_0}."""
         import torch.distributed as dist
         from .dp import allreduce_flat_gradient
-        if self.uq:
-            if self._dp is None:
-                self._dp = _PackedStep([self], [1.0])
-            self._dp.step(lambda: self.backward(x, y, step=step, row0=row0, denom=denom_global), x is not None, dist)
-            self.apply(lr, step)
-            t = self.grads[self.n_trainable:]
-            return torch.stack([t[4], t[1]])
         if x is None:
             self.grads[:self.n_trainable + 2].zero_()
         else:
@@ -265,6 +176,187 @@ class ForecasterEngine(object):
     def launch_count(self):
         return int(self.lib.lfmq_launch_count())
 
+
+class ForecasterEngine(_HandleEngine):
+    """fwd / loss / BPTT / clip / optimizer / MaxNorm for RNNPointEstimate on one GPU.
+
+    Mirrors what the reference builds in RNNPointEstimate._build_model
+    (scripts/models/point_estimate/rnn_point_estimate.py:40-107) plus the step body of
+    Train._train_step_point (scripts/train.py:178-199).
+    """
+
+    def __init__(self, *, max_batch, seq_len, n_inputs, n_outputs, num_hidden, num_layers=1, target_idx=0,
+                 train=True, precision='fp32', optimizer='Adadelta', dropout=0.0, recurrent_dropout=0.0,
+                 target_lambda=0.5, rnn_lambda=0.7, max_grad_norm=50.0, max_norm=3.0, sgd_momentum=0.0,
+                 seed=521, forward_only=False, device=None, rnn_cell='lstm', uq=False):
+        if not torch.cuda.is_available():
+            raise N.LfmqError('ForecasterEngine needs a CUDA device (no CPU fallback)')
+        self.lib = N.load()
+        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        if optimizer not in N.OPTIMIZERS:
+            raise ValueError("%s optimizer not found in tf.keras.optimizers" % optimizer)
+        cfg = N.LfmqConfig()
+        cfg.struct_size = C.sizeof(N.LfmqConfig)
+        cfg.max_batch, cfg.seq_len, cfg.n_inputs, cfg.n_outputs = max_batch, seq_len, n_inputs, n_outputs
+        cfg.num_hidden, cfg.num_layers, cfg.target_idx = num_hidden, num_layers, target_idx
+        cfg.train = 1 if train else 0
+        cfg.precision = {'fp32': N.PREC_FP32, 'bf16': N.PREC_BF16, 'bf16x3': N.PREC_BF16X3}[precision]
+        cfg.optimizer = N.OPTIMIZERS[optimizer]
+        cfg.forward_only = 1 if forward_only else 0
+        if rnn_cell not in N.CELLS:
+            raise NotImplementedError('rnn_cell=%s (rnn_point_estimate.py:80-102 knows lstm and gru)' % rnn_cell)
+        cfg.rnn_cell = N.CELLS[rnn_cell]
+        cfg.uq = 1 if uq else 0
+        self.uq = bool(uq)
+        cfg.dropout, cfg.recurrent_dropout = dropout, recurrent_dropout
+        cfg.target_lambda, cfg.rnn_lambda = target_lambda, rnn_lambda
+        cfg.max_grad_norm, cfg.max_norm, cfg.sgd_momentum = max_grad_norm, max_norm, sgd_momentum
+        cfg.bn_epsilon = 1e-3
+        cfg.seed = seed
+        self.cfg = cfg
+        self.precision = precision
+        self.T, self.F, self.O, self.H, self.L = seq_len, n_inputs, n_outputs, num_hidden, num_layers
+        nbytes = C.c_uint64(0)
+        N.check(self.lib.lfmq_workspace_bytes(C.byref(cfg), C.byref(nbytes)))
+        with torch.cuda.device(self.device):
+            self.workspace = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
+            self.handle = C.c_void_p(0)
+            N.check(self.lib.lfmq_create(C.byref(cfg), _ptr(self.workspace), nbytes, C.byref(self.handle)))
+        self._read_specs()
+        self._denom = torch.zeros(2, dtype=torch.float32, device=self.device)
+        self._dp = None
+
+    def forward(self, x, step=0, row0=0, out=None):
+        """preds [B,T,O]; on a uq engine the pair (preds, variance) -- model(inp)[0], model(inp)[1] of RNNUqRangeEstimate."""
+        B = self._check_x(x)
+        if self.uq:
+            preds = torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device)
+            var = torch.empty_like(preds)
+            N.check(self.lib.lfmq_forward_uq(self.handle, _ptr(x), B, row0, step, _ptr(preds), _ptr(var), _stream()))
+            return preds, var
+        if out is None:
+            out = torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device)
+        N.check(self.lib.lfmq_forward(self.handle, _ptr(x), B, row0, step, _ptr(out), _stream()))
+        return out
+
+    def loss_uq(self, preds, var, y):
+        """Device tensor {uq_loss, uq_loss_last_tar, mse_0} (Losses.weight_adjusted_uq_loss, losses.py:137-284)."""
+        out = torch.empty(3, dtype=torch.float32, device=preds.device)
+        N.check(self.lib.lfmq_loss_uq(self.handle, _ptr(preds.contiguous()), _ptr(var.contiguous()), _ptr(y.contiguous()),
+                                      preds.shape[0], _ptr(out), _stream()))
+        return out
+
+    def mask_count_uq(self, y):
+        """Device {B, unmasked rows, unmasked last-step rows}: the denominators of the uq loss (losses.py:179-284)."""
+        out = torch.empty(3, dtype=torch.float32, device=y.device)
+        N.check(self.lib.lfmq_mask_count_uq(self.handle, _ptr(y), y.shape[0], _ptr(out), _stream()))
+        return out
+
+    def loss_counts(self, y):
+        """The loss denominators of one batch that data parallelism all-reduces: mask_count_uq on a uq engine, else
+        mask_count.  y None (a rank without rows): zeros of the same length."""
+        if y is None:
+            return torch.zeros(3 if self.uq else 2, dtype=torch.float32, device=self.device)
+        return self.mask_count_uq(y) if self.uq else self.mask_count(y)
+
+    def backward(self, x, y, step=0, row0=0, denom=None):
+        B = self._check_x(x)
+        assert y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and tuple(y.shape) == (B, self.T, self.O)
+        N.check(self.lib.lfmq_backward(self.handle, _ptr(x), _ptr(y), B, row0, step, _ptr(denom), _stream()))
+
+    def train_step_dp(self, x, y, step, lr, row0, denom_global):
+        """Data-parallel step: local BPTT with global denominators, ONE NCCL all-reduce over the flat
+        gradient (+ loss/mse tail), then the replicated clip + optimizer (SURVEY 8e).
+        uq engine: the gradient and {uq_loss, mse_0, uq_loss_last_tar} travel as one packed vector (a chain of one
+        stage, lfmq_chain_grad_pack).  x None (a rank without rows) joins the collective with zeros.  Returns the global
+        {loss, mse_0}, uq engine {uq_loss_last_tar, mse_0}, as train_step."""
+        import torch.distributed as dist
+        if self.uq:
+            if self._dp is None:
+                self._dp = _PackedStep([self], [1.0])
+            self._dp.step(lambda: self.backward(x, y, step=step, row0=row0, denom=denom_global), x is not None, dist)
+            self.apply(lr, step)
+            t = self.grads[self.n_trainable:]
+            return torch.stack([t[4], t[1]])
+        return self._train_step_dp_flat(x, y, step, lr, row0, denom_global)
+
+
+
+class DenseEngine(_HandleEngine):
+    """MLPLinearPointEstimate on one GPU (scripts/models/point_estimate/mlp_linear_point_estimate.py:66-77): one Dense(O)
+    layer OUTPUT_1 over the flattened input window, its MLP-branch loss (model_utils/losses.py:69-75,100-115) with the
+    Huber option, the clip and the optimizer -- a dense handle of include/lfmq.h (lfmq_dense_create).  x is the
+    [B, T, F] batch or its [B, T*F] view; targets and predictions are [B, O]."""
+
+    def __init__(self, *, max_batch, seq_len, n_inputs, n_outputs, target_idx=0, precision='fp32',
+                 optimizer='Adadelta', target_lambda=0.5, max_grad_norm=50.0, sgd_momentum=0.0, huber_loss=False,
+                 huber_delta=1.0, forward_only=False, device=None):
+        if not torch.cuda.is_available():
+            raise N.LfmqError('DenseEngine needs a CUDA device (no CPU fallback)')
+        self.lib = N.load()
+        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        if optimizer not in N.OPTIMIZERS:
+            raise ValueError("%s optimizer not found in tf.keras.optimizers" % optimizer)
+        cfg = N.LfmqDenseConfig()
+        cfg.struct_size = C.sizeof(N.LfmqDenseConfig)
+        cfg.max_batch, cfg.seq_len, cfg.n_inputs, cfg.n_outputs = max_batch, seq_len, n_inputs, n_outputs
+        cfg.target_idx = target_idx
+        cfg.precision = {'fp32': N.PREC_FP32, 'bf16': N.PREC_BF16, 'bf16x3': N.PREC_BF16X3}[precision]
+        cfg.optimizer = N.OPTIMIZERS[optimizer]
+        cfg.forward_only = 1 if forward_only else 0
+        cfg.huber_loss = 1 if huber_loss else 0
+        cfg.target_lambda, cfg.huber_delta = target_lambda, huber_delta
+        cfg.max_grad_norm, cfg.sgd_momentum = max_grad_norm, sgd_momentum
+        self.cfg = cfg
+        self.precision = precision
+        self.uq = False
+        self.T, self.F, self.O = seq_len, n_inputs, n_outputs
+        nbytes = C.c_uint64(0)
+        N.check(self.lib.lfmq_dense_workspace_bytes(C.byref(cfg), C.byref(nbytes)))
+        with torch.cuda.device(self.device):
+            self.workspace = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
+            self.handle = C.c_void_p(0)
+            N.check(self.lib.lfmq_dense_create(C.byref(cfg), _ptr(self.workspace), nbytes, C.byref(self.handle)))
+        self._read_specs()
+
+    def _check_x(self, x):
+        assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous(), 'x must be a contiguous CUDA fp32 tensor'
+        assert x.shape[0] * self.T * self.F == x.numel() and x.shape[1:] in ((self.T * self.F,), (self.T, self.F)), \
+            tuple(x.shape)
+        return x.shape[0]
+
+    def _check_y(self, y, B):
+        assert y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and tuple(y.shape) == (B, self.O), \
+            'y must be a contiguous CUDA fp32 tensor [B, O]'
+
+    def forward(self, x, step=0, row0=0, out=None):
+        """model(inp) / model.predict(inp): preds [B, O].  step and row0 are accepted for the drivers' sake; the model
+        has no dropout."""
+        B = self._check_x(x)
+        if out is None:
+            out = torch.empty(B, self.O, dtype=torch.float32, device=x.device)
+        N.check(self.lib.lfmq_forward(self.handle, _ptr(x), B, row0, step, _ptr(out), _stream()))
+        return out
+
+    def loss_counts(self, y):
+        """{B, rows whose targets are not all zero}, the denominators data parallelism all-reduces; zeros for y None."""
+        if y is None:
+            return torch.zeros(2, dtype=torch.float32, device=self.device)
+        return self.mask_count(y)
+
+    def backward(self, x, y, step=0, row0=0, denom=None):
+        B = self._check_x(x)
+        self._check_y(y, B)
+        N.check(self.lib.lfmq_backward(self.handle, _ptr(x), _ptr(y), B, row0, step, _ptr(denom), _stream()))
+
+    def train_step(self, x, y, step, lr, out=None):
+        self._check_y(y, self._check_x(x))
+        return super(DenseEngine, self).train_step(x, y, step, lr, out)
+
+    def train_step_dp(self, x, y, step, lr, row0, denom_global):
+        """Data-parallel step (the point estimate's): local backward with the global {B, mask count}, ONE all-reduce
+        of the flat gradient and its {loss, mse_0} tail, the replicated clip and optimizer."""
+        return self._train_step_dp_flat(x, y, step, lr, row0, denom_global)
 
 class _PackedStep(object):
     """The collective of a data-parallel step over the handles of a chain (or one uq handle): the backward fills every

@@ -287,8 +287,6 @@ class Dataset(object):
         """data_processing.py:307-368 -> (inp f32 [B,T,F], tar f32 [B,T,O], metadata [B,3]) on the GPU."""
         import torch
         from ..engine import gather_batch
-        if 'MLP' in self.config.nn_type or 'Naive' in self.config.nn_type:
-            raise NotImplementedError('only the recurrent forecaster (RNNPointEstimate) is built on this path')
         d = self._device_state()
         inp_idx = torch.from_numpy(np.ascontiguousarray(inp_indices, dtype=np.int32)).cuda()
         tar_idx = torch.from_numpy(np.ascontiguousarray(tar_indices, dtype=np.int32)).cuda()
@@ -300,6 +298,10 @@ class Dataset(object):
                                 aux_masking=self.config.aux_masking)
         metadata = np.array(pre_metadata, dtype=object)
         metadata[:, 2] = sn.cpu().numpy()              # :349 overwrite tar_key with seq_norm
+        if 'MLP' in self.config.nn_type or 'Naive' in self.config.nn_type:
+            # :363-365: the window flattened to [B, T*F] (a view of the gathered batch), the targets of the last step
+            x = x.view(x.shape[0], self.seq_len * x.shape[2])
+            y = y[:, -1, :].contiguous()
         return x, y, metadata
 
     # ---- helpers kept from the reference ------------------------------------------------------------------

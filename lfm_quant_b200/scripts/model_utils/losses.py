@@ -1,7 +1,8 @@
 """Losses(config, target_idx).weight_adjusted_mse (reference: scripts/model_utils/losses.py:19-135), evaluated by
 the native loss kernel (lfmq_loss; lfmq_chain_loss for forecast_steps > 1), and Losses.weight_adjusted_uq_loss
-(:137-284) by lfmq_loss_uq (lfmq_chain_loss_uq for forecast_steps > 1).  Only the RNN branches are built; the MLP / Huber branches belong to
-other model families."""
+(:137-284) by lfmq_loss_uq (lfmq_chain_loss_uq for forecast_steps > 1).  The MLP branch of weight_adjusted_mse
+(:100-115, MLPLinearPointEstimate) is lfmq_loss on a dense handle in its MSE form, the form validation evaluates; its
+Huber form is the training loss, evaluated inside the training step (lfmq_backward)."""
 from __future__ import absolute_import, division, print_function
 
 import numpy as np
@@ -37,8 +38,11 @@ class Losses(object):
             'arguments to loss function need to be a list [y_true], [y_true1, y_true2, ..]'
         assert isinstance(y_pred, (list, tuple)), \
             'arguments to loss function need to be a list [y_pred], [y_pred1, y_pred2, ..]'
-        if 'RNN' not in self.config.nn_type:
-            raise NotImplementedError('only RNN point estimates are built on this path')
+        if 'RNN' not in self.config.nn_type and 'MLP' not in self.config.nn_type:
+            raise NotImplementedError('%s NN type not implemented' % self.config.nn_type)      # losses.py:117-119
+        if 'MLP' in self.config.nn_type and self.config.huber_loss and not is_validation:
+            raise NotImplementedError('the Huber training loss of the MLP branch (losses.py:102-105) is evaluated by '
+                                      'the training step; Losses evaluates the MSE form (is_validation=True)')
         S = self.config.forecast_steps
         if S == 1:
             if len(self.config.forecast_steps_weights) == 1:

@@ -3,10 +3,13 @@ to a class by name in this module's globals; ``Cls(config, dataset).model`` is r
 from __future__ import absolute_import, division, print_function
 
 # All models should be imported here
+from ..models.point_estimate.mlp_linear_point_estimate import MLPLinearPointEstimate  # noqa: F401
+from ..models.point_estimate.naive_point_estimate import NaivePointEstimate  # noqa: F401
 from ..models.point_estimate.rnn_point_estimate import RNNPointEstimate  # noqa: F401
 from ..models.uq_range_estimate.rnn_uq_range_estimate import RNNUqRangeEstimate  # noqa: F401
 
-_NOT_BUILT = ('MLPPointEstimate', 'MLPLinearPointEstimate', 'NaivePointEstimate', 'MLPUqRangeEstimate')
+# the hidden-layer MLPs (Dense -> BatchNormalization -> ReLU -> Dropout stacks)
+_NOT_BUILT = ('MLPPointEstimate', 'MLPUqRangeEstimate')
 
 
 class Model(object):
@@ -20,8 +23,7 @@ class Model(object):
         if self._config.nn_type in all_objects:
             model_constructor = all_objects[self._config.nn_type]
         elif self._config.nn_type in _NOT_BUILT:
-            raise NotImplementedError("nn_type = %s is a reference model family outside the recurrent-forecaster "
-                                      "hot path" % self._config.nn_type)
+            raise NotImplementedError("nn_type = %s: the hidden-layer MLP models are not built" % self._config.nn_type)
         else:
             raise RuntimeError("Unknown nn_type = %s" % self._config.nn_type)
         m = model_constructor(self._config, self._dataset)

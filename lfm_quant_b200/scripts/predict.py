@@ -39,7 +39,8 @@ class Predict(object):
         self._batches = [self.dataset.get_batch(*items) for items in self.test_set]
 
     def predict(self):
-        self.model.load_weights(os.path.join(self.chkpts_dir, "chkpt"))
+        if 'Naive' not in self.config.nn_type:            # predict.py:90-93: the naive forecast has no variables
+            self.model.load_weights(os.path.join(self.chkpts_dir, "chkpt"))
         outputs = defaultdict(list)
         for (inp_dev, target_dev, metadata) in self._batches:
             # one target window per input window: every forecast step is compared with it (Train._step_targets)
@@ -113,11 +114,21 @@ class Predict(object):
             print("Scaled MSE for step %i: %1.4f" % (i + 1, df['norm_squared_diff_' + str(i + 1)].mean()))
         return df
 
+    def _flat(self):
+        """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""
+        return 'MLP' in self.config.nn_type or 'Naive' in self.config.nn_type
+
     def _extract_targets(self, targets):
+        if self._flat():
+            return [np.expand_dims(x[:, self.target_index], -1) for x in targets]
         return [np.expand_dims(x[:, -1, self.target_index], -1) for x in targets]
 
     def _extract_preds(self, preds):
+        if self._flat():
+            return [np.expand_dims(x[:, self.target_index], -1) for x in preds]
         return [np.expand_dims(x[:, -1, self.target_index], -1) for x in preds]
 
     def _extract_inputs(self, inp, i):
+        if self._flat():                                 # step i of the target field: column i * F + target_index
+            return np.expand_dims(inp[:, i * self.n_inputs + self.target_index], -1)
         return np.expand_dims(inp[:, i, self.target_index], -1)

@@ -210,7 +210,8 @@ class ModelExecution(object):
         stream = torch.cuda.Stream()
         with torch.cuda.stream(stream):
             runner = (Train if config.train else Predict)(config, Dataset(config))
-            runner.model.engine.set_device_share(1, share_den)
+            if runner.model.engine is not None:           # NaivePointEstimate runs no kernels of its own
+                runner.model.engine.set_device_share(1, share_den)
             out = runner.train() if config.train else runner.predict()
         stream.synchronize()
         return out
