@@ -1,7 +1,9 @@
-"""Data parallelism over the company-batch axis (SURVEY section 8e): host-side plumbing shared by
-ForecasterEngine.train_step_dp, ForecastChainEngine.train_step_dp, bench.py and the gloo tests.  One process per GPU;
+"""Data parallelism over the company-batch axis (SURVEY section 8e): host-side plumbing shared by the handle engines'
+train_step_dp (ForecasterEngine, DenseEngine), ForecastChainEngine.train_step_dp -- which every model object's step
+goes through, delegating to the handle's own with one stage -- bench.py and the gloo tests.  One process per GPU;
 exactly ONE collective on the data path per step -- the SUM all-reduce of the flat gradient (+ its loss / mse tail)
-over NCCL; for chains and uq handles, of the packed vector of every stage's gradients and loss tail."""
+over NCCL for a point or dense handle; for chains and uq handles, of the packed vector of every stage's gradients and
+loss tail."""
 from __future__ import absolute_import, division, print_function
 
 

@@ -1,4 +1,5 @@
-"""Thin Python owner of one native forecaster instance (one per process / GPU).
+"""Thin Python owners of the native handles: one handle engine per handle (ForecasterEngine, DenseEngine), and
+ForecastChainEngine, the engine of every model object, over one handle or a forecast chain of them.
 
 PyTorch is used for device allocation, streams and torch.distributed only; every piece of arithmetic
 happens in lfm_quant_b200/_lfmq.so through the C-ABI of include/lfmq.h.
@@ -136,8 +137,9 @@ class _HandleEngine(object):
         return out
 
     def train_step(self, x, y, step, lr, out=None):
-        """One Train._train_step_point on this GPU; returns a device tensor {loss, mse_0} (no host sync).
-        uq engine: one Train._train_step_uq_range, {uq_loss_last_tar, mse_0} (train.py:225)."""
+        """One training step of the point estimate (train.py:178-199) on this GPU; returns a device tensor
+        {loss, mse_0} (no host sync).  uq engine: the uq range estimate's step (train.py:201-225),
+        {uq_loss_last_tar, mse_0}."""
         B = self._check_x(x)
         if out is None:
             out = torch.empty(2, dtype=torch.float32, device=x.device)
@@ -181,8 +183,8 @@ class ForecasterEngine(_HandleEngine):
     """fwd / loss / BPTT / clip / optimizer / MaxNorm for RNNPointEstimate on one GPU.
 
     Mirrors what the reference builds in RNNPointEstimate._build_model
-    (scripts/models/point_estimate/rnn_point_estimate.py:40-107) plus the step body of
-    Train._train_step_point (scripts/train.py:178-199).
+    (scripts/models/point_estimate/rnn_point_estimate.py:40-107) plus the body of its training step
+    (scripts/train.py:178-199).
     """
 
     def __init__(self, *, max_batch, seq_len, n_inputs, n_outputs, num_hidden, num_layers=1, target_idx=0,
@@ -385,21 +387,32 @@ class _PackedStep(object):
 
 
 class ForecastChainEngine(object):
-    """forecast_steps > 1 (scripts/models/point_estimate/rnn_point_estimate.py:109-150): stage 0 is the trunk, every
-    further stage one more recurrent layer + BatchNormalization + Dropout + Dense on the shifted input window.  One
-    ForecasterEngine (one C-ABI handle) per stage; the lfmq_chain_* entry points run the whole graph.
-    uq=True: RNNUqRangeEstimate's graph (models/uq_range_estimate/rnn_uq_range_estimate.py:114-157), every stage with a
-    target and a variance head and dropout always on; the next window is built from the target predictions."""
+    """The engine behind every model object: S >= 1 stages, list-valued throughout -- forward returns the Keras output
+    list and the losses and steps take the list of S targets.
 
-    def __init__(self, *, forecast_steps, weights, num_layers, uq=False, **kw):
-        assert forecast_steps >= 1
-        self.S = int(forecast_steps)
-        self.uq = bool(uq)
-        self.stages = [ForecasterEngine(num_layers=num_layers if s == 0 else 1, uq=self.uq, **kw) for s in range(self.S)]
+    S > 1 (scripts/models/point_estimate/rnn_point_estimate.py:109-150): stage 0 is the trunk, every further stage one
+    more recurrent layer + BatchNormalization + Dropout + Dense on the shifted input window.  One ForecasterEngine (one
+    C-ABI handle) per stage; the lfmq_chain_* entry points run the whole graph.
+    uq=True: RNNUqRangeEstimate's graph (models/uq_range_estimate/rnn_uq_range_estimate.py:114-157), every stage with a
+    target and a variance head and dropout always on; the next window is built from the target predictions.
+
+    S == 1: every call goes to the one stage's own engine -- a ForecasterEngine, or the DenseEngine passed as
+    ``stages=[engine]`` -- and its result is wrapped in a list.  A one-stage model so issues exactly its handle's library
+    calls: lfmq_train_step as one call, bf16 / bf16x3 training handles (which the chain entry points refuse), and the
+    handle's own data-parallel step.  Its step weights are [1.0] (losses.py:44-45) whatever ``weights`` holds."""
+
+    def __init__(self, *, forecast_steps=1, weights=None, num_layers=1, uq=False, stages=None, **kw):
+        if stages is None:
+            assert forecast_steps >= 1
+            stages = [ForecasterEngine(num_layers=num_layers if s == 0 else 1, uq=uq, **kw)
+                      for s in range(forecast_steps)]
+        self.stages = list(stages)
+        self.S = len(self.stages)
         e0 = self.stages[0]
-        self.lib, self.device, self.cfg, self.precision = e0.lib, e0.device, e0.cfg, e0.precision
-        self.T, self.F, self.O, self.H, self.L = e0.T, e0.F, e0.O, e0.H, e0.L
-        self.weights = [float(w) for w in weights]
+        self._one = e0 if self.S == 1 else None
+        self.lib, self.device, self.cfg, self.precision, self.uq = e0.lib, e0.device, e0.cfg, e0.precision, e0.uq
+        self.T, self.F, self.O = e0.T, e0.F, e0.O
+        self.weights = [float(w) for w in weights] if self._one is None else [1.0]
         assert len(self.weights) == self.S, (self.weights, self.S)
         self._handles = (C.c_void_p * self.S)(*[e.handle.value for e in self.stages])
         self._w = (C.c_float * self.S)(*self.weights)
@@ -411,8 +424,9 @@ class ForecastChainEngine(object):
         for s, e in enumerate(self.stages):
             for name, shp, off, tr in e.specs:
                 if s > 0:
-                    name = name.replace('%s_1/' % cell, '%s_%d/' % (cell, self.L + s))
-                    name = name.replace('batch_normalization/', 'batch_normalization_%d/' % (self.L + s - 1))
+                    L = e0.L
+                    name = name.replace('%s_1/' % cell, '%s_%d/' % (cell, L + s))
+                    name = name.replace('batch_normalization/', 'batch_normalization_%d/' % (L + s - 1))
                     name = name.replace('OUTPUT_1/', 'OUTPUT_%d/' % (s + 1))
                     name = name.replace('OUTPUT_TARGET_1/', 'OUTPUT_TARGET_%d/' % (s + 1))
                     name = name.replace('OUTPUT_VARIANCE_1/', 'OUTPUT_VARIANCE_%d/' % (s + 1))
@@ -435,8 +449,12 @@ class ForecastChainEngine(object):
         return self._work
 
     def forward(self, x, step=0, row0=0):
-        """model(inp) -> [pred_1 .. pred_S], device tensors [B,T,O]; a uq chain returns the Keras output list
-        [tar_1, var_1, .., tar_S, var_S] (rnn_uq_range_estimate.py:107-108,152-155)."""
+        """model(inp) -> the Keras output list of device tensors [B,T,O] ([B,O] on a dense stage): [pred],
+        [tar, var], [pred_1 .. pred_S] or, on a uq chain, [tar_1, var_1, .., tar_S, var_S]
+        (rnn_uq_range_estimate.py:107-108,152-155)."""
+        if self._one is not None:
+            out = self._one.forward(x, step=step, row0=row0)
+            return list(out) if self.uq else [out]
         B = self.stages[0]._check_x(x)
         preds = [torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device) for _ in range(self.S)]
         if self.uq:
@@ -450,6 +468,8 @@ class ForecastChainEngine(object):
 
     def loss(self, preds, ys):
         """Losses.weight_adjusted_mse(ys, preds): device tensor {loss, mse}."""
+        if self._one is not None:
+            return self._one.loss(preds[0], ys[0])
         out = torch.empty(2, dtype=torch.float32, device=preds[0].device)
         preds = [p.contiguous() for p in preds]
         ys = [y.contiguous() for y in ys]
@@ -460,6 +480,8 @@ class ForecastChainEngine(object):
     def loss_uq(self, preds, var, ys):
         """Losses.weight_adjusted_uq_loss(ys, preds, var) (losses.py:137-178): device tensor
         {uq_loss, uq_loss_last_tar, mse}, each summed over the steps with forecast_steps_weights."""
+        if self._one is not None:
+            return self._one.loss_uq(preds[0], var[0], ys[0])
         out = torch.empty(3, dtype=torch.float32, device=preds[0].device)
         preds, var, ys = ([t.contiguous() for t in a] for a in (preds, var, ys))
         N.check(self.lib.lfmq_chain_loss_uq(self._handles, self.S, self._ptrs(preds), self._ptrs(var), self._ptrs(ys),
@@ -478,6 +500,8 @@ class ForecastChainEngine(object):
         return out
 
     def apply(self, lr, iteration):
+        if self._one is not None:
+            return self._one.apply(lr, iteration)
         N.check(self.lib.lfmq_chain_apply(self._handles, self.S, float(lr), int(iteration), _stream()))
 
     # ---- data parallelism over the company-batch axis --------------------------------------------
@@ -494,7 +518,10 @@ class ForecastChainEngine(object):
         return out
 
     def loss_counts(self, ys):
-        """mask_count under the name ForecasterEngine gives the counts data parallelism all-reduces."""
+        """The loss denominators of one batch that data parallelism all-reduces: the stage's own loss_counts, or
+        mask_count of a chain.  ys None (a rank without rows): zeros."""
+        if self._one is not None:
+            return self._one.loss_counts(None if ys is None else ys[0])
         return self.mask_count(ys)
 
     def backward_dp(self, x, ys, denoms, step=0, row0=0, out=None):
@@ -538,7 +565,10 @@ class ForecastChainEngine(object):
     def train_step_dp(self, x, ys, step, lr, row0, denoms):
         """Data-parallel step of the whole graph: local BPTT of this rank's rows with the global stage counts, ONE
         all-reduce of the packed vector, then the joint clip, optimizer and MaxNorm on every rank.  x None joins the
-        step without rows.  Returns the global {loss, mse}; uq chain {uq_loss_last_tar, mse}, as train_step."""
+        step without rows.  Returns the global {loss, mse}; uq chain {uq_loss_last_tar, mse}, as train_step.
+        One stage: its own train_step_dp (a point or dense handle reduces its flat gradient in place)."""
+        if self._one is not None:
+            return self._one.train_step_dp(x, None if ys is None else ys[0], step, lr, row0, denoms)
         import torch.distributed as dist
         out = torch.empty(3 if self.uq else 2, dtype=torch.float32, device=self.device)
         self._packed().step(lambda: self.backward_dp(x, ys, denoms, step=step, row0=row0), x is not None, dist,
@@ -547,8 +577,10 @@ class ForecastChainEngine(object):
         return out[1:] if self.uq else out
 
     def train_step(self, x, ys, step, lr):
-        """One Train._train_step_point over the S-output model; device tensor {loss, mse}.  uq chain: one
-        Train._train_step_uq_range, {uq_loss_last_tar, mse} (train.py:225), both weighted over the steps."""
+        """One training step (train.py:178-225) over the S-output model; device tensor {loss, mse}, on a uq model
+        {uq_loss_last_tar, mse} (train.py:225), both weighted over the steps.  One stage: one lfmq_train_step."""
+        if self._one is not None:
+            return self._one.train_step(x, ys[0], step, lr)
         out = self.backward(x, ys, step=step)
         self.apply(lr, step)
         return out[1:] if self.uq else out
@@ -567,13 +599,17 @@ class ForecastChainEngine(object):
         return [w for e in self.stages for w in e.get_weights(trainable_only)]
 
     def set_weights(self, weights):
-        """weights in trainable_variables order: the trunk's, then 7 per extra stage (9 on a uq chain)."""
+        """weights in trainable_variables order (the trunk's, then 7 per extra stage, 9 on a uq chain), or all of
+        get_weights(trainable_only=False): every stage's trainable arrays followed by its BatchNormalization
+        statistics."""
+        full = len(weights) == len(self.specs)
         i = 0
         for e in self.stages:
             n = len(e.trainable_specs)
-            e.set_weights(weights[i:i + n])
-            i += n
-        assert i == len(weights)
+            bn = weights[i + n:i + len(e.specs)] if full else []
+            e.set_weights(weights[i:i + n], list(zip(bn[0::2], bn[1::2])) if full else None)
+            i += n + len(bn)
+        assert i == len(weights), (i, len(weights))
 
     def named_arrays(self):
         out = {}

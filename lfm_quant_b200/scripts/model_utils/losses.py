@@ -1,8 +1,8 @@
-"""Losses(config, target_idx).weight_adjusted_mse (reference: scripts/model_utils/losses.py:19-135), evaluated by
-the native loss kernel (lfmq_loss; lfmq_chain_loss for forecast_steps > 1), and Losses.weight_adjusted_uq_loss
-(:137-284) by lfmq_loss_uq (lfmq_chain_loss_uq for forecast_steps > 1).  The MLP branch of weight_adjusted_mse
-(:100-115, MLPLinearPointEstimate) is lfmq_loss on a dense handle in its MSE form, the form validation evaluates; its
-Huber form is the training loss, evaluated inside the training step (lfmq_backward)."""
+"""Losses(config, target_idx).weight_adjusted_mse (reference: scripts/model_utils/losses.py:19-135) and
+Losses.weight_adjusted_uq_loss (:137-284), evaluated by the model's engine (ForecastChainEngine.loss / loss_uq: the
+one stage's lfmq_loss / lfmq_loss_uq, or lfmq_chain_loss / lfmq_chain_loss_uq over the forecast steps).  The MLP
+branch of weight_adjusted_mse (:100-115, MLPLinearPointEstimate) is lfmq_loss on a dense handle in its MSE form, the
+form validation evaluates; its Huber form is the training loss, evaluated inside the training step (lfmq_backward)."""
 from __future__ import absolute_import, division, print_function
 
 import numpy as np
@@ -32,6 +32,7 @@ class Losses(object):
         self.engine = engine
 
     def weight_adjusted_mse(self, y_true, y_pred, is_validation=False):
+        """losses.py:19-53: per-step loss / mse, linearly weighted -- one native call over the S pairs."""
         assert self.config.forecast_steps > 0, 'forecasts_steps should be a positive integer. %i was provided' % \
             self.config.forecast_steps
         assert isinstance(y_true, (list, tuple)), \
@@ -44,29 +45,9 @@ class Losses(object):
             raise NotImplementedError('the Huber training loss of the MLP branch (losses.py:102-105) is evaluated by '
                                       'the training step; Losses evaluates the MSE form (is_validation=True)')
         S = self.config.forecast_steps
-        if S == 1:
-            if len(self.config.forecast_steps_weights) == 1:
-                self.config.forecast_steps_weights = [1.0]       # losses.py:44-45
-            return self._get_loss_point_estimate(y_true[0], y_pred[0], is_validation)
-        # losses.py:36-51: per-step loss / mse, linearly weighted -- one native call over the S pairs
         assert len(y_true) == S and len(y_pred) == S
-        assert len(self.config.forecast_steps_weights) == S
-        import torch
-        assert self.engine is not None, 'Losses is not bound to a native engine'
-        dev = self.engine.device
-        to = lambda a: (a if isinstance(a, torch.Tensor) else
-                        torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))).to(dev, torch.float32).contiguous()
-        out = self.engine.loss([to(p) for p in y_pred], [to(y) for y in y_true])
-        return _Scalar(out[0]), _Scalar(out[1])
-
-    def _get_loss_point_estimate(self, y_true, y_pred, is_validation=False):
-        import torch
-        assert self.engine is not None, 'Losses is not bound to a native engine'
-        dev = self.engine.device
-        to = lambda a: a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
-        yt = to(y_true).to(dev, torch.float32).contiguous()
-        yp = to(y_pred).to(dev, torch.float32).contiguous()
-        out = self.engine.loss(yp, yt)
+        self._step_weights()
+        out = self.engine.loss([self._to(p) for p in y_pred], [self._to(y) for y in y_true])
         return _Scalar(out[0]), _Scalar(out[1])
 
     def weight_adjusted_uq_loss(self, y_true, y_pred, y_var):
@@ -83,19 +64,22 @@ class Losses(object):
         S = self.config.forecast_steps
         for name, v in (('y_true', y_true), ('y_pred', y_pred), ('y_var', y_var)):
             assert len(v) >= S, '%s holds %d forecast steps, forecast_steps is %d' % (name, len(v), S)
-        if S == 1:
-            if len(self.config.forecast_steps_weights) == 1:
-                self.config.forecast_steps_weights = [1.0]
-        else:
-            assert len(self.config.forecast_steps_weights) == S     # losses.py:164-166
-        import torch
-        assert self.engine is not None, 'Losses is not bound to a native engine'
-        dev = self.engine.device
-        to = lambda a: (a if isinstance(a, torch.Tensor) else
-                        torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))).to(dev, torch.float32).contiguous()
-        if S == 1:
-            out = self.engine.loss_uq(to(y_pred[0]), to(y_var[0]), to(y_true[0]))
-        else:                       # losses.py:159-177: per-step losses with their own masks, linearly weighted
-            out = self.engine.loss_uq([to(p) for p in y_pred[:S]], [to(v) for v in y_var[:S]],
-                                      [to(y) for y in y_true[:S]])
+        self._step_weights()
+        out = self.engine.loss_uq([self._to(p) for p in y_pred[:S]], [self._to(v) for v in y_var[:S]],
+                                  [self._to(y) for y in y_true[:S]])
         return _Scalar(out[0]), _Scalar(out[1]), _Scalar(out[2])
+
+    def _step_weights(self):
+        """losses.py:41-45,165-170: one weight per forecast step; the weights of a single step become [1.0].  The
+        engine weighs the steps with the weights it was built with."""
+        S, w = self.config.forecast_steps, self.config.forecast_steps_weights
+        assert S == 1 or len(w) == S
+        if len(w) == S == 1:
+            self.config.forecast_steps_weights = [1.0]
+        assert self.engine is not None, 'Losses is not bound to a native engine'
+
+    def _to(self, a):
+        """An ndarray or tensor as a contiguous fp32 tensor on the engine's device."""
+        import torch
+        t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
+        return t.to(self.engine.device, torch.float32).contiguous()

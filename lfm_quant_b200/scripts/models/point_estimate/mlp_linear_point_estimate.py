@@ -10,41 +10,31 @@ import numpy as np
 from ..model_base_class import BaseModelClass
 from ...model_utils.initializers import Initializer
 from ...model_utils.optimizers import Optimizers
-from .rnn_point_estimate import NativeForecaster, _Variable
+from .rnn_point_estimate import NativeForecaster
 
 
 class NativeDenseForecaster(NativeForecaster):
-    """The Keras-subset model object of NativeForecaster over a DenseEngine: __call__, predict, predict_device,
-    train_step, trainable_variables, save_weights / load_weights (``.lfmq.npz`` and the TF-format container, where
-    OUTPUT_1 is ``layer_with_weights-0``), summary."""
+    """NativeForecaster over one DenseEngine stage: the same model object, whose TF-format container holds OUTPUT_1 as
+    ``layer_with_weights-0``."""
 
-    def __init__(self, config, seq_len, n_inputs, n_outputs, target_idx):
-        from ....engine import DenseEngine
-        self.config = config
-        self.uq = False
+    title = 'MLPLinearPointEstimate'
+
+    def _build_engine(self, config, seq_len, n_inputs, n_outputs, target_idx):
+        from ....engine import DenseEngine, ForecastChainEngine
         if config.forecast_steps != 1:
             raise NotImplementedError('MLPLinearPointEstimate has one output (mlp_linear_point_estimate.py:66-77); '
                                       'forecast_steps = %d needs one per step, which the reference cannot train '
                                       'either' % config.forecast_steps)
-        self.engine = DenseEngine(
+        engine = DenseEngine(
             max_batch=config.batch_size, seq_len=seq_len, n_inputs=n_inputs, n_outputs=n_outputs,
             target_idx=target_idx, precision=getattr(config, 'precision', 'fp32'), optimizer=config.optimizer,
             target_lambda=config.target_lambda, max_grad_norm=config.max_grad_norm, sgd_momentum=config.sgd_momentum,
             huber_loss=bool(config.huber_loss), huber_delta=config.huber_delta, forward_only=not config.train)
-        specs = [(n, s) for (n, s, _, tr) in self.engine.specs if tr]
+        specs = [(n, s) for (n, s, _, tr) in engine.specs if tr]
         rng = np.random.RandomState(config.seed)
         kernel = Initializer(config).get_initializer()(specs[0][1], rng)      # :69-73
-        self.engine.set_weights([np.asarray(kernel, dtype=np.float32), np.zeros(specs[1][1], dtype=np.float32)])
-        self.trainable_variables = [_Variable(self, i, n, s) for i, (n, s) in enumerate(specs)]
-        self._calls = 0
-
-    def summary(self):
-        lines = ['Model: "MLPLinearPointEstimate" (native sm_90a, precision=%s)' % self.engine.precision,
-                 '%-44s %-16s %10s' % ('Variable', 'Shape', 'Param #'), '=' * 72]
-        for name, shape, _, _ in self.engine.specs:
-            lines.append('%-44s %-16s %10d' % (name, str(tuple(shape)), int(np.prod(shape))))
-        lines += ['=' * 72, 'Total params: %d' % self.engine.n_total, 'Trainable params: %d' % self.engine.n_trainable]
-        return '\n'.join(lines)
+        engine.set_weights([np.asarray(kernel, dtype=np.float32), np.zeros(specs[1][1], dtype=np.float32)])
+        return ForecastChainEngine(stages=[engine])
 
 
 class MLPLinearPointEstimate(BaseModelClass):

@@ -9,7 +9,7 @@ from __future__ import absolute_import, division, print_function
 from ...model_utils.initializers import Initializer
 from ...model_utils.optimizers import Optimizers
 from ..model_base_class import BaseModelClass
-from ..point_estimate.rnn_point_estimate import NativeChainForecaster, NativeForecaster
+from ..point_estimate.rnn_point_estimate import NativeForecaster
 
 
 class RNNUqRangeEstimate(BaseModelClass):
@@ -29,8 +29,5 @@ class RNNUqRangeEstimate(BaseModelClass):
         self.model = self._build_model()
 
     def _build_model(self):
-        if self.forecast_steps > 1:                      # reference :114-157
-            return NativeChainForecaster(self.config, self.seq_len, self.n_inputs, self.n_outputs,
-                                         self.dataset.target_index, uq=True)
         return NativeForecaster(self.config, self.seq_len, self.n_inputs, self.n_outputs, self.dataset.target_index,
                                 uq=True)

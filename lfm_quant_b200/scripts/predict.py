@@ -52,8 +52,10 @@ class Predict(object):
                 for i, t_step in enumerate(range(1 - self.seq_len, 1)):
                     outputs['inp_t' + str(t_step)].append(self._extract_inputs(inp, i))
             outputs['targets'].append(self._extract_targets(targets))
-            if not self.config.UQ:
-                preds = [self.model.predict(inp_dev)]
+            if not self.config.UQ:      # predict.py:128-133: model.predict returns a list when forecast_steps > 1
+                preds = self.model.predict(inp_dev)
+                if self.config.forecast_steps == 1:
+                    preds = [preds]
                 variance = [np.zeros(x.shape) for x in preds]   # predict.py:133
             else:                       # predict.py:135-138: [tar_1, var_1, .., tar_S, var_S]
                 model_preds = self.model.predict(inp_dev)

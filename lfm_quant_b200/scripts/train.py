@@ -2,7 +2,7 @@
 
 Same life cycle -- build model/optimizer/losses, materialise every batch up front (train.py:64-80), epoch loop
 with shuffled batch order, CSV logs (train.py:133-147,156-167,227-238), save-best / early-stop
-(train.py:240-266) -- but the step body ``_train_step_point`` (train.py:178-199) is ONE native call
+(train.py:240-266) -- but the step body of every model (``_train_step``, train.py:178-225) is ONE native call
 (fwd + loss + BPTT + clip + optimizer + MaxNorm on the GPU) and the per-step ``mse.numpy()`` host sync of the
 reference (train.py:199) is deferred: device scalars are read back only when a log line is due.
 """
@@ -38,7 +38,7 @@ class Train(object):
         if self.world > 1:                       # one set of initial weights: rank 0's, for every forecast stage
             import torch
             import torch.distributed as dist
-            for eng in getattr(self.model.engine, 'stages', [self.model.engine]):
+            for eng in self.model.engine.stages:
                 flat = torch.from_numpy(eng.get_flat()).to(eng.device)
                 dist.broadcast(flat, 0)
                 eng.set_flat(flat.cpu().numpy())
@@ -110,14 +110,7 @@ class Train(object):
             else:                                               # every rank must walk the same batch order
                 random.Random(self.config.seed + epoch).shuffle(self._batches)
             for (batch_n, cur_batch) in enumerate(self._batches):
-                inp, target = cur_batch[0], cur_batch[1]
-                if self.world > 1:
-                    uq_loss, mse = self._train_step_dp(cur_batch)
-                elif self.config.UQ:
-                    uq_loss, mse = self._train_step_uq_range(inp, target)
-                else:
-                    mse = self._train_step_point(inp, target)   # device scalar, no host sync here
-                    uq_loss = None
+                uq_loss, mse = self._train_step(cur_batch)      # device scalars, no host sync here
                 mse_steps.append(mse)
                 uq_loss_steps.append(uq_loss)
                 if batch_n % self.config.logging_interval == 0:
@@ -153,42 +146,27 @@ class Train(object):
         import torch
         return float(torch.stack(list(device_scalars)).mean().item())
 
-    def _train_step_point(self, inp, targets):
-        """train.py:178-199 as one fused native step; returns the step's mse_0 as a device scalar."""
-        assert not self.config.UQ
-        lr = self.optimizer.current_lr()
-        out = self.model.train_step(inp, self._step_targets(targets), lr, self.optimizer.iterations)
-        self.optimizer.iterations += 1
-        return out[1]
-
-    def _train_step_dp(self, cur_batch):
-        """One data-parallel step of any model (train.py:178-225): local BPTT with global denominators, ONE all-reduce,
-        replicated clip + optimizer + MaxNorm; a rank without rows joins with zeros.  Same trajectory as one GPU.
-        Returns (uq_loss_last_tar or None, mse), both global device scalars.  The point estimate reduces its flat
-        gradient in place (ForecasterEngine.train_step_dp); RNNUqRangeEstimate and multi-step forecasts all-reduce the
-        packed vector of every stage's gradients and loss tail (ForecastChainEngine.train_step_dp)."""
-        inp, targets, _, row0, denom = cur_batch
-        step = self.model.train_step_dp if self.config.forecast_steps > 1 else self.model.engine.train_step_dp
-        out = step(inp, None if inp is None else self._step_targets(targets), self.optimizer.iterations,
-                   self.optimizer.current_lr(), row0, denom)
+    def _train_step(self, cur_batch):
+        """One training step of any model (train.py:178-225) as one fused native step; returns
+        (uq_loss_last_tar or None, mse) as device scalars, weighted over the forecast steps.  Under torchrun: local BPTT
+        of this rank's rows with the global denominators, ONE all-reduce, the replicated clip + optimizer + MaxNorm; a
+        rank without rows joins with zeros.  Same trajectory as one GPU."""
+        inp = cur_batch[0]
+        ys = None if inp is None else self._step_targets(cur_batch[1])
+        lr, it = self.optimizer.current_lr(), self.optimizer.iterations
+        if self.world > 1:
+            out = self.model.train_step_dp(inp, ys, it, lr, cur_batch[3], cur_batch[4])
+        else:
+            out = self.model.train_step(inp, ys, lr, it)
         self.optimizer.iterations += 1
         return (out[0] if self.config.UQ else None), out[1]
 
     def _step_targets(self, targets):
         """The list of forecast_steps targets of one batch.  The dataset materialises one target window per input window
         (forecast_n ahead); every forecast step of a multi-step graph is scored against it."""
-        if self.config.forecast_steps == 1 or isinstance(targets, (list, tuple)):
+        if isinstance(targets, (list, tuple)):
             return targets
         return [targets] * self.config.forecast_steps
-
-    def _train_step_uq_range(self, inp, targets):
-        """train.py:201-225 as one fused native step; returns device scalars (uq_loss_last_tar, mse_0), weighted over
-        the forecast steps when forecast_steps > 1."""
-        assert self.config.UQ
-        lr = self.optimizer.current_lr()
-        out = self.model.train_step(inp, self._step_targets(targets), lr, self.optimizer.iterations)
-        self.optimizer.iterations += 1
-        return out[0], out[1]
 
     def _write_train_logs(self, train_logs, name):
         if self.rank != 0:
@@ -219,13 +197,8 @@ class Train(object):
         import torch
         if not self._valid_batches:
             return None, float('nan'), float('nan')
-        preds = [self.model.predict_device(cur_batch[0]) for cur_batch in self._valid_batches]
+        preds = [self.model.predict_device(cur_batch[0]) for cur_batch in self._valid_batches]    # lists of S
         targets = [self._step_targets(cur_batch[1]) for cur_batch in self._valid_batches]
-        if self.config.forecast_steps == 1:              # preds, targets need to be lists (train.py:291-294)
-            preds = [[p] for p in preds]
-            targets = [[t] for t in targets]
-        assert all(isinstance(t, (list, tuple)) for t in targets), \
-            'forecast_steps > 1 needs a list of forecast_steps targets per batch (train.py:296-299)'
         scale, center = self._scaling_dev()
         eng = self.model.engine
         S = self.config.forecast_steps
@@ -251,7 +224,7 @@ class Train(object):
 
     def _validation_metrics_uq_range_estimate(self):
         """train.py:338-416: predict every validation batch (dropout stays on), uq loss over the stacked arrays, MSE of
-        the un-scaled target predictions.  forecast_steps > 1: every step's arrays, the losses weighted over the steps
+        the un-scaled target predictions: every forecast step's arrays, the losses weighted over the steps
         (train.py:387-416)."""
         S = self.config.forecast_steps
         preds, var, targets = [], [], []
@@ -259,8 +232,7 @@ class Train(object):
             batch_pred = self.model.predict(cur_batch[0])
             preds.append(batch_pred[0::2])
             var.append(batch_pred[1::2])
-            tar = self._step_targets(cur_batch[1])
-            targets.append([t.cpu().numpy() for t in (tar if S > 1 else [tar])])
+            targets.append([t.cpu().numpy() for t in self._step_targets(cur_batch[1])])
         if not preds:
             return float('nan'), float('nan'), float('nan')
         pred_all, var_all, target_all = ([np.vstack([b[i] for b in a]).astype('float32') for i in range(S)]

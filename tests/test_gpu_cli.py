@@ -243,3 +243,61 @@ def test_predict_driver_and_preds_file_match_the_reference_golden(tmp_path, monk
         bad = np.abs(a - b) > (atol + 5e-4 * np.abs(b))
         assert not (bad & ok).any(), (col, int((bad & ok).sum()), float(np.abs(a - b)[bad & ok].max()))
     configs.reset()
+
+
+def test_predict_writes_every_step_of_a_multi_step_point_model(tmp_path, monkeypatch):
+    """predict.py:128-133: a point model with forecast_steps > 1 returns the list of its steps from model.predict, which
+    Predict uses as it is (it wraps only a single step's array): preds_1 and preds_2 are the two outputs' last step."""
+    import pickle
+    from lfm_quant_b200.scripts import base_config, predict as predict_mod
+    from lfm_quant_b200.scripts.data_processing import Dataset
+    gold_dir = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+
+    def step(x, s):
+        return (np.tanh(x.mean(axis=2, keepdims=True)) * s + 0.1 * np.arange(16)[None, None, :]).astype(np.float32)
+
+    class _StubModel(object):
+        def predict(self, inp, batch_size=None):
+            x = inp.detach().cpu().numpy().astype(np.float64)
+            return [step(x, 1.0), step(x, 2.0)]
+
+        def load_weights(self, path):
+            return None
+
+    class _StubFactory(object):
+        def __init__(self, config, dataset):
+            pass
+
+        def get_model(self):
+            return _StubModel()
+
+    monkeypatch.setattr(predict_mod, 'Model', _StubFactory)
+    d = tmp_path / 'datasets'
+    write_open_dataset(str(d / 'open-dataset.dat'), n_keys=8, n_months=120, seed=11)
+    mdir = tmp_path / 'experiments' / 'm'
+    os.makedirs(str(mdir / 'chkpts'))
+    g = np.load(os.path.join(gold_dir, 'reference_batcher_train.npz'))
+    pickle.dump({'center': g['center'], 'scale': g['scale']}, open(str(mdir / 'scales.dat'), 'wb'))
+    configs.reset()
+    c = base_config.get_configs(['--datafile', 'open-dataset.dat', '--data_dir', str(d), '--experiments_dir',
+                                 str(tmp_path / 'experiments'), '--model_dir', 'm', '--financial_fields',
+                                 'saleq_ttm-ltq_mrq', '--aux_fields', 'rel_mom1m-rel_mom9m', '--target_field',
+                                 'oiadpq_ttm', '--scale_field', 'mrkcap', '--stride', '12', '--forecast_n', '12',
+                                 '--min_unrollings', '3', '--max_unrollings', '5', '--start_date', '197001', '--end_date',
+                                 '209912', '--validation_size', '0.3', '--seed', '521', '--batch_size', '64',
+                                 '--forecast_steps', '2', '--forecast_steps_weights', '1.0-0.5', '--train=False'])
+    try:
+        p = predict_mod.Predict(c, Dataset(c))
+        df = p.predict()
+        x = np.vstack([b[0].cpu().numpy() for b in p._batches]).astype(np.float64)
+    finally:
+        configs.reset()
+    got = pd.read_csv(str(mdir / 'pred' / c.preds_fname), sep=' ', dtype={'gvkey': str})
+    assert len(got) == len(df) == len(x) > 0
+    for s in (1, 2):
+        for col in ('targets_%d', 'norm_preds_%d', 'norm_variance_%d', 'preds_%d', 'variance_%d'):
+            assert col % s in got.columns
+        np.testing.assert_allclose(got['norm_preds_%d' % s].values, step(x, float(s))[:, -1, p.target_index],
+                                   rtol=1e-6)
+        assert (got['norm_variance_%d' % s] == 0).all()
+    np.testing.assert_array_equal(got['targets_1'].values, got['targets_2'].values)

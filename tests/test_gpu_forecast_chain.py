@@ -116,17 +116,17 @@ def _cfg(train, precision='fp32'):
                                     precision, '--nn_type', 'RNNPointEstimate'])
 
 
-def test_chain_model_object_predict_checkpoint_and_refusals(tmp_path):
-    """NativeChainForecaster through the reference's model interface: list outputs, save/load round trip (native and
-    TF-format container), a bf16 forward-only graph within bf16 tolerance of the fp32 one, training graphs refused off
-    the fp32 kernels; Losses.weight_adjusted_mse over the lists."""
+def test_native_forecaster_chain_predict_checkpoint_and_refusals(tmp_path):
+    """The two-step NativeForecaster (a ForecastChainEngine of two stages) through the reference's model interface: list
+    outputs, save/load round trip (native and TF-format container), a bf16 forward-only graph within bf16 tolerance of
+    the fp32 one, training graphs refused off the fp32 kernels; Losses.weight_adjusted_mse over the lists."""
     import os
-    from lfm_quant_b200.scripts.models.point_estimate.rnn_point_estimate import NativeChainForecaster
+    from lfm_quant_b200.scripts.models.point_estimate.rnn_point_estimate import NativeForecaster
     from lfm_quant_b200.scripts.model_utils.losses import Losses
     T, F, O = 5, 12, 6
     cfg = _cfg(True)
     assert cfg.forecast_steps_weights == [1.0, 0.5]
-    m = NativeChainForecaster(cfg, T, F, O, 0)
+    m = NativeForecaster(cfg, T, F, O, 0)
     x = np.random.RandomState(0).normal(size=(16, T, F)).astype(np.float32)
     out = m.predict(x)
     assert isinstance(out, list) and len(out) == 2 and out[0].shape == (16, T, O)
@@ -142,19 +142,19 @@ def test_chain_model_object_predict_checkpoint_and_refusals(tmp_path):
     assert np.isfinite(r).all()
     prefix = str(tmp_path / 'chkpt')
     m.save_weights(prefix)
-    m2 = NativeChainForecaster(_cfg(False), T, F, O, 0)
+    m2 = NativeForecaster(_cfg(False), T, F, O, 0)
     m2.load_weights(prefix)
     a = m2.predict(x)
     os.remove(prefix + '.lfmq.npz')          # the TF-format container alone restores the same weights
-    m3 = NativeChainForecaster(_cfg(False), T, F, O, 0)
+    m3 = NativeForecaster(_cfg(False), T, F, O, 0)
     m3.load_weights(prefix)
     b = m3.predict(x)
     for s in range(2):
         np.testing.assert_array_equal(a[s], b[s])
-    m4 = NativeChainForecaster(_cfg(False, 'bf16'), T, F, O, 0)
+    m4 = NativeForecaster(_cfg(False, 'bf16'), T, F, O, 0)
     m4.load_weights(prefix)
     c = m4.predict(x)
     for s in range(2):
         assert rel_err(c[s], a[s]) < 5e-2, s
     with pytest.raises(NotImplementedError):
-        NativeChainForecaster(_cfg(True, 'bf16'), T, F, O, 0)
+        NativeForecaster(_cfg(True, 'bf16'), T, F, O, 0)

@@ -179,12 +179,14 @@ def _cfg(train, precision='fp32'):
                                     precision, '--nn_type', 'RNNUqRangeEstimate', '--UQ=True', '--dropout', '0.1'])
 
 
-def test_uq_chain_model_object_and_refusals():
-    from lfm_quant_b200.scripts.models.point_estimate.rnn_point_estimate import NativeChainForecaster
+def test_native_forecaster_uq_chain_and_refusals():
+    """The two-step uq NativeForecaster: summary, the interleaved output list, Losses.weight_adjusted_uq_loss over the
+    lists, a train step, and a bf16 training chain refused."""
+    from lfm_quant_b200.scripts.models.point_estimate.rnn_point_estimate import NativeForecaster
     from lfm_quant_b200.scripts.model_utils.losses import Losses
     T, F, O = 5, 12, 6
     cfg = _cfg(True)
-    m = NativeChainForecaster(cfg, T, F, O, 0, uq=True)
+    m = NativeForecaster(cfg, T, F, O, 0, uq=True)
     assert 'RNNUqRangeEstimate' in m.summary() and 'OUTPUT_VARIANCE_2/kernel' in m.summary()
     x = np.random.RandomState(0).normal(size=(16, T, F)).astype(np.float32)
     out = m.predict(x)
@@ -199,7 +201,7 @@ def test_uq_chain_model_object_and_refusals():
     r = m.train_step(x, ys, 0.6, 0).cpu().numpy()
     assert r.shape == (2,) and np.isfinite(r).all()
     with pytest.raises(NotImplementedError):
-        NativeChainForecaster(_cfg(True, 'bf16'), T, F, O, 0, uq=True)
+        NativeForecaster(_cfg(True, 'bf16'), T, F, O, 0, uq=True)
 
 
 @pytest.fixture(scope='module')
