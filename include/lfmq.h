@@ -232,6 +232,31 @@ int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float
  * each [B,T,O], Dropout masks drawn for (step, row0) on every call */
 int32_t lfmq_chain_forward_uq(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
                               int64_t step, float* const* preds, float* const* vars, float* work, void* stream);
+
+/* ---- Monte-Carlo dropout samples of a uq model in one prediction --------------------------------------------------
+ * The reference's UQ inference (runtime/model_execution.py:201-241, utils/post_processing.py:39-75) runs one dropout
+ * sample per process and combines the members' files.  These entry points draw `samples` >= 1 samples of every window
+ * in one call: sample s of window b is global row row0 + s * B + b of the batch tiled `samples` times, with that row's
+ * dropout masks.  Sample 0 is therefore lfmq_forward_uq / lfmq_chain_forward_uq at (step, row0), and the samples are
+ * independent draws.  The samples * B rows run in launches of at most max_batch rows (the smallest of the stages'), so
+ * B and samples are not bounded by max_batch; a chain runs each replica's own trajectory.  After each launch one pass
+ * folds its samples, in increasing s, into four [B,T,O] fp32 arrays per stage (Welford, fixed order, no atomics):
+ *   mean_pred, mean_var   the sample means of the target predictions and of the predicted variances
+ *   var_pred, var_var     their population variances (divided by samples)
+ * The results do not depend on how the rows are cut into launches, nor on the other windows of the batch.  Point-estimate
+ * and dense handles are refused with LFMQ_ERR_ARG (their dropout is off at prediction time).  `work`: caller-owned device
+ * scratch, 256-byte aligned, of the size the matching *_work_bytes query gives for (B, samples). */
+int32_t lfmq_forward_uq_mc_work_bytes(lfmq_handle h, int32_t B, int32_t samples, uint64_t* bytes);
+int32_t lfmq_forward_uq_mc(lfmq_handle h, const float* x, int32_t B, int64_t row0, int64_t step, int32_t samples,
+                           float* mean_pred, float* mean_var, float* var_pred, float* var_var, void* work,
+                           uint64_t work_bytes, void* stream);
+/* The same for a uq chain (stages as lfmq_chain_forward_uq); the four outputs are host arrays of n_stages pointers. */
+int32_t lfmq_chain_forward_uq_mc_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t B, int32_t samples,
+                                            uint64_t* bytes);
+int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
+                                 int64_t step, int32_t samples, float* const* mean_pred, float* const* mean_var,
+                                 float* const* var_pred, float* const* var_var, void* work, uint64_t work_bytes,
+                                 void* stream);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

@@ -53,6 +53,14 @@ int scale_inplace(cudaStream_t s, long n, float* p, float w);
 int chain_scatter_dx(cudaStream_t s, int B, int T, int F, int O, int stage, const float* dx, const ChainPtrs& dpred);
 int chain_combine(cudaStream_t s, int S, const ChainPtrs& scalars, float clip, const ChainPtrs& loss2,
                   const ChainWeights& w, float* out2);
+// Monte-Carlo dropout samples of a uq model: sample s of window b is row s * B + b of the batch tiled `samples` times.
+// mc_replicate: xrep = rows [r0, r0 + n) of that tiled batch (row_elems floats per row).
+int mc_replicate(cudaStream_t s, int B, int64_t r0, int n, long row_elems, const float* x, float* xrep);
+// mc_moments: folds every stage's sampled pred / var [n, T, O] of tiled rows [r0, r0 + n) into the per-element moments
+// [B, T, O] of the samples; chunks must arrive in increasing r0 and cover [0, samples * B) without gaps.  After the last
+// one, mean_pred / mean_var hold the sample means and var_pred / var_var the population variances.
+struct McMoments { ChainPtrs pred, var, mean_pred, mean_var, var_pred, var_var; };
+int mc_moments(cudaStream_t s, int n_stages, int B, int TO, int64_t r0, int n, int samples, const McMoments& m);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

@@ -649,6 +649,80 @@ int chain_scatter_dx(cudaStream_t s, int B, int T, int F, int O, int stage, cons
   return 0;
 }
 
+// ---- Monte-Carlo dropout samples: rows [r0, r0 + n) of the batch x tiled `samples` times (row r = s * B + b) ----------
+__global__ void mc_replicate_kernel(long n_elems, long B, long r0, long row_elems, const float* __restrict__ x,
+                                    float* __restrict__ xrep) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_elems) return;
+  const long r = r0 + i / row_elems;
+  xrep[i] = x[(r % B) * row_elems + i % row_elems];
+}
+
+int mc_replicate(cudaStream_t s, int B, int64_t r0, int n, long row_elems, const float* x, float* xrep) {
+  const long n_elems = (long)n * row_elems;
+  mc_replicate_kernel<<<cdiv(n_elems, 256), 256, 0, s>>>(n_elems, B, r0, row_elems, x, xrep);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+// One thread per (window b, element k of [T,O]) that has samples among the chunk's rows [r0, r0 + n): j < min(n, B)
+// walks the windows of the chunk in row order, b = (r0 + j) mod B, whose samples there are s_lo, s_lo + 1, .. at local
+// rows j, j + B, ...  Welford updates in increasing s; the running means live in mean_pred / mean_var and the sums of
+// squared deviations in var_pred / var_var until the update of the last sample divides them by `samples`.  Sample 0
+// starts the state, so nothing needs zeroing, and every element sees the same updates in the same order whatever the
+// chunking.
+__global__ void mc_moments_kernel(int B, int TO, int64_t r0, int n, int samples, McMoments m) {
+  const int st = blockIdx.y;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int nb = min(n, B);
+  if (i >= (long)nb * TO) return;
+  const int j = (int)(i / TO), k = (int)(i % TO);
+  const int64_t rj = r0 + j;
+  const int b = (int)(rj % B);
+  const int s_lo = (int)(rj / B);
+  const int s_hi = s_lo + (n - 1 - j) / B;
+  const long o = (long)b * TO + k;
+  const float* pr = m.pred.p[st] + (long)j * TO + k;
+  const float* vr = m.var.p[st] + (long)j * TO + k;
+  float mp, mv, qp, qv;
+  if (s_lo == 0) {
+    mp = pr[0];
+    mv = vr[0];
+    qp = qv = 0.f;
+  } else {
+    mp = m.mean_pred.p[st][o];
+    mv = m.mean_var.p[st][o];
+    qp = m.var_pred.p[st][o];
+    qv = m.var_var.p[st][o];
+  }
+  for (int s = (s_lo == 0) ? 1 : s_lo; s <= s_hi; ++s) {
+    const long off = (long)(s - s_lo) * B * TO;
+    const float x = pr[off], v = vr[off];
+    const float cnt = (float)(s + 1);
+    const float dp = x - mp, dv = v - mv;
+    mp += dp / cnt;
+    mv += dv / cnt;
+    qp = fmaf(dp, x - mp, qp);
+    qv = fmaf(dv, v - mv, qv);
+  }
+  if (s_hi == samples - 1) {
+    qp /= (float)samples;
+    qv /= (float)samples;
+  }
+  m.mean_pred.p[st][o] = mp;
+  m.mean_var.p[st][o] = mv;
+  m.var_pred.p[st][o] = qp;
+  m.var_var.p[st][o] = qv;
+}
+
+int mc_moments(cudaStream_t s, int n_stages, int B, int TO, int64_t r0, int n, int samples, const McMoments& m) {
+  const long threads = (long)min(n, B) * TO;
+  dim3 grid(cdiv(threads, 256), n_stages);
+  mc_moments_kernel<<<grid, 256, 0, s>>>(B, TO, r0, n, samples, m);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
 // tf.clip_by_global_norm over ALL stages' variables (train.py:196): every stage's tail holds its own ||g||; this
 // writes the joint norm and the joint clip scale into each of them.  out2 (nullable) = sum_s w_s {loss_s, mse_s}
 // (Losses.weight_adjusted_mse, losses.py:47-51), read from the stages' {loss, mse_0} pairs.

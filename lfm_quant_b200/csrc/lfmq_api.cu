@@ -5,6 +5,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -1076,6 +1077,140 @@ int32_t lfmq_chain_forward_uq(const lfmq_handle* stages, int32_t n_stages, const
       return LFMQ_ERR_ARG;
     }
   return run_stages(stages, n_stages, x, B, row0, step, preds, vars, work, (cudaStream_t)stream);
+}
+
+// ---- Monte-Carlo dropout samples of a uq model (lfmq_forward_uq_mc, lfmq_chain_forward_uq_mc) ----------------------
+namespace {
+// The stages' common checks; rows per launch = the smallest max_batch.  Leaves tc.stream_base alone: the chain entry
+// point has numbered the streams already, and a single handle keeps its own.
+int mc_check(const lfmq_handle* st, int32_t S, int32_t B, int32_t samples, const char* fn, int* chunk_max) {
+  if (!st || S < 1 || S > lfmq::LFMQ_MAX_STAGES || B < 1 || samples < 1) {
+    LFMQ_SET_ERR("%s: need 1 <= n_stages <= %d, B >= 1 and samples >= 1 (got %d, %d, %d)", fn, lfmq::LFMQ_MAX_STAGES, S,
+                 B, samples);
+    return LFMQ_ERR_ARG;
+  }
+  int mb = 0;
+  for (int i = 0; i < S; ++i) {
+    if (!st[i] || st[i]->dense || !st[i]->cfg.uq) {
+      LFMQ_SET_ERR("%s: stage %d is not a uq handle: only RNNUqRangeEstimate keeps dropout on at prediction time, a "
+                   "point-estimate model would give the same prediction for every sample", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+    mb = (i == 0) ? st[i]->cfg.max_batch : std::min(mb, (int)st[i]->cfg.max_batch);
+  }
+  *chunk_max = mb;
+  return 0;
+}
+
+// floats of caller scratch for `rows` replicated rows per launch: the replicated input, the chain's next-stage windows,
+// and every stage's sampled preds and vars; each buffer starts on a 256-byte boundary of the (aligned) work pointer
+size_t mc_align(size_t floats) { return (floats + 63) / 64 * 64; }
+size_t mc_work_floats(const lfmq_config& c, int S, size_t rows) {
+  return (size_t)S * mc_align(rows * c.seq_len * c.n_inputs) + 2 * (size_t)S * mc_align(rows * c.seq_len * c.n_outputs);
+}
+
+size_t mc_rows(int B, int samples, int chunk_max) {
+  return (size_t)std::min<int64_t>((int64_t)samples * B, chunk_max);
+}
+
+// Sample s of window b is global row row0 + s * B + b of the batch tiled `samples` times, so sample 0 is
+// lfmq_(chain_)forward_uq at (step, row0).  The tiled rows run in launches of at most chunk_max rows, in row order, and
+// each launch's samples are folded into the moments at once.
+int mc_run(const lfmq_handle* st, int S, const float* x, int B, int64_t row0, int64_t step, int samples, int chunk_max,
+           float* const* mean_pred, float* const* mean_var, float* const* var_pred, float* const* var_var, void* work,
+           uint64_t work_bytes, cudaStream_t s) {
+  const lfmq_config& c = st[0]->cfg;
+  const long row_in = (long)c.seq_len * c.n_inputs, row_out = (long)c.seq_len * c.n_outputs;
+  const size_t rows = mc_rows(B, samples, chunk_max);
+  const size_t need = mc_work_floats(c, S, rows) * sizeof(float);
+  if (!work || work_bytes < need) {
+    LFMQ_SET_ERR("forward_uq_mc: work needs %zu bytes, got %llu", need, (unsigned long long)work_bytes);
+    return LFMQ_ERR_WORKSPACE;
+  }
+  const size_t in_sz = mc_align(rows * row_in), out_sz = mc_align(rows * row_out);
+  float* xrep = static_cast<float*>(work);
+  float* slots = xrep + in_sz;                    // run_stages' windows of stages 1 .. S-1, rows * row_in apart
+  float* sp = xrep + (size_t)S * in_sz;
+  lfmq::McMoments m{};
+  float* pp[lfmq::LFMQ_MAX_STAGES];
+  float* vp[lfmq::LFMQ_MAX_STAGES];
+  for (int i = 0; i < S; ++i) {
+    pp[i] = m.pred.p[i] = sp + (size_t)(2 * i) * out_sz;
+    vp[i] = m.var.p[i] = sp + (size_t)(2 * i + 1) * out_sz;
+    m.mean_pred.p[i] = mean_pred[i];
+    m.mean_var.p[i] = mean_var[i];
+    m.var_pred.p[i] = var_pred[i];
+    m.var_var.p[i] = var_var[i];
+  }
+  const int64_t total = (int64_t)samples * B;
+  for (int64_t r0 = 0; r0 < total; r0 += (int64_t)rows) {
+    const int n = (int)std::min<int64_t>((int64_t)rows, total - r0);
+    const int64_t b0 = r0 % B;
+    const float* in = x + b0 * row_in;            // rows of one sample are a slice of x
+    if (b0 + n > B) {
+      RUN(mc_replicate(s, B, r0, n, row_in, x, xrep));
+      in = xrep;
+    }
+    RUN(run_stages(st, S, in, n, row0 + r0, step, pp, vp, slots, s));
+    RUN(mc_moments(s, S, B, (int)row_out, r0, n, samples, m));
+  }
+  return 0;
+}
+
+int mc_out_check(int S, float* const* a, float* const* b, float* const* c, float* const* d, const char* fn) {
+  for (int i = 0; i < S; ++i)
+    if (!a || !b || !c || !d || !a[i] || !b[i] || !c[i] || !d[i]) {
+      LFMQ_SET_ERR("%s: null output of stage %d", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+  return 0;
+}
+}  // namespace
+
+int32_t lfmq_forward_uq_mc_work_bytes(lfmq_handle h, int32_t B, int32_t samples, uint64_t* bytes) {
+  return lfmq_chain_forward_uq_mc_work_bytes(&h, 1, B, samples, bytes);
+}
+
+int32_t lfmq_chain_forward_uq_mc_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t B, int32_t samples,
+                                            uint64_t* bytes) {
+  int mb = 0;
+  RUN(mc_check(stages, n_stages, B, samples, "lfmq_forward_uq_mc_work_bytes", &mb));
+  if (!bytes) {
+    LFMQ_SET_ERR("lfmq_forward_uq_mc_work_bytes: bytes == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  *bytes = mc_work_floats(stages[0]->cfg, n_stages, mc_rows(B, samples, mb)) * sizeof(float);
+  return LFMQ_OK;
+}
+
+int32_t lfmq_forward_uq_mc(lfmq_handle h, const float* x, int32_t B, int64_t row0, int64_t step, int32_t samples,
+                           float* mean_pred, float* mean_var, float* var_pred, float* var_var, void* work,
+                           uint64_t work_bytes, void* stream) {
+  int mb = 0;
+  RUN(mc_check(&h, 1, B, samples, "lfmq_forward_uq_mc", &mb));
+  RUN(mc_out_check(1, &mean_pred, &mean_var, &var_pred, &var_var, "lfmq_forward_uq_mc"));
+  if (!x) {
+    LFMQ_SET_ERR("lfmq_forward_uq_mc: x == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  return mc_run(&h, 1, x, B, row0, step, samples, mb, &mean_pred, &mean_var, &var_pred, &var_var, work, work_bytes,
+                (cudaStream_t)stream);
+}
+
+int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
+                                 int64_t step, int32_t samples, float* const* mean_pred, float* const* mean_var,
+                                 float* const* var_pred, float* const* var_var, void* work, uint64_t work_bytes,
+                                 void* stream) {
+  int mb = 0;
+  RUN(mc_check(stages, n_stages, B, samples, "lfmq_chain_forward_uq_mc", &mb));
+  RUN(chain_check(stages, n_stages, 1, false));     // numbers the stages' dropout streams; launches hold <= mb rows
+  RUN(mc_out_check(n_stages, mean_pred, mean_var, var_pred, var_var, "lfmq_chain_forward_uq_mc"));
+  if (!x) {
+    LFMQ_SET_ERR("lfmq_chain_forward_uq_mc: x == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  return mc_run(stages, n_stages, x, B, row0, step, samples, mb, mean_pred, mean_var, var_pred, var_var, work,
+                work_bytes, (cudaStream_t)stream);
 }
 
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,

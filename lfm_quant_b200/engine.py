@@ -241,6 +241,18 @@ class ForecasterEngine(_HandleEngine):
         N.check(self.lib.lfmq_forward(self.handle, _ptr(x), B, row0, step, _ptr(out), _stream()))
         return out
 
+    def forward_mc(self, x, samples, step=0, row0=0):
+        """`samples` Monte-Carlo dropout samples of every window in one call (lfmq_forward_uq_mc): the device tensors
+        (mean_pred, mean_var, var_pred, var_var) [B,T,O] -- the sample means of the target predictions and of the
+        variances, and their population variances.  Sample s of window b is row row0 + s * B + b; sample 0 is
+        forward(x, step, row0).  uq engines only."""
+        B = self._check_x(x)
+        out = [torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device) for _ in range(4)]
+        work = _mc_work(self, [self], B, samples)
+        N.check(self.lib.lfmq_forward_uq_mc(self.handle, _ptr(x), B, row0, step, samples, *[_ptr(t) for t in out],
+                                            _ptr(work), work.numel(), _stream()))
+        return tuple(out)
+
     def loss_uq(self, preds, var, y):
         """Device tensor {uq_loss, uq_loss_last_tar, mse_0} (Losses.weight_adjusted_uq_loss, losses.py:137-284)."""
         out = torch.empty(3, dtype=torch.float32, device=preds.device)
@@ -360,6 +372,17 @@ class DenseEngine(_HandleEngine):
         of the flat gradient and its {loss, mse_0} tail, the replicated clip and optimizer."""
         return self._train_step_dp_flat(x, y, step, lr, row0, denom_global)
 
+def _mc_work(owner, engines, B, samples):
+    """The scratch of lfmq_(chain_)forward_uq_mc for (B, samples), kept on `owner` and grown as needed."""
+    n = C.c_uint64(0)
+    handles = (C.c_void_p * len(engines))(*[e.handle.value for e in engines])
+    N.check(owner.lib.lfmq_chain_forward_uq_mc_work_bytes(handles, len(engines), B, int(samples), C.byref(n)))
+    work = getattr(owner, '_mc_buf', None)
+    if work is None or work.numel() < n.value:
+        work = owner._mc_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=engines[0].device)
+    return work
+
+
 class _PackedStep(object):
     """The collective of a data-parallel step over the handles of a chain (or one uq handle): the backward fills every
     stage's gradient buffer, one launch packs them with their reduced loss tails into one contiguous vector, ONE SUM
@@ -465,6 +488,20 @@ class ForecastChainEngine(object):
         N.check(self.lib.lfmq_chain_forward(self._handles, self.S, _ptr(x), B, row0, step, self._ptrs(preds),
                                             _ptr(self._workbuf(B)), _stream()))
         return preds
+
+    def forward_mc(self, x, samples, step=0, row0=0):
+        """`samples` Monte-Carlo dropout samples of every window of a uq model in one call: per stage the device tensors
+        (mean_pred, mean_var, var_pred, var_var) [B,T,O] (ForecasterEngine.forward_mc; a chain runs each sample's own
+        trajectory, lfmq_chain_forward_uq_mc)."""
+        if self._one is not None:
+            return [self._one.forward_mc(x, samples, step=step, row0=row0)]
+        B = self.stages[0]._check_x(x)
+        out = [[torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device) for _ in range(self.S)]
+               for _ in range(4)]
+        work = _mc_work(self, self.stages, B, samples)
+        N.check(self.lib.lfmq_chain_forward_uq_mc(self._handles, self.S, _ptr(x), B, row0, step, samples,
+                                                  *[self._ptrs(o) for o in out], _ptr(work), work.numel(), _stream()))
+        return [tuple(o[s] for o in out) for s in range(self.S)]
 
     def loss(self, preds, ys):
         """Losses.weight_adjusted_mse(ys, preds): device tensor {loss, mse}."""

@@ -102,6 +102,19 @@ class NativeForecaster(object):
         outs = [self.engine.forward(x[s:s + mb].contiguous(), step=self._calls, row0=s) for s in range(0, B, mb)]
         return [outs[0][k] if len(outs) == 1 else torch.cat([o[k] for o in outs], dim=0) for k in range(len(outs[0]))]
 
+    def predict_mc(self, inp, samples):
+        """`samples` Monte-Carlo dropout samples of every window in one prediction, the in-process form of the
+        reference's UQ ensemble (runtime/model_execution.py:201-241): per forecast step the device tensors
+        (mean_pred, mean_var, var_pred, var_var) [B,T,O].  One step per call, as predict_device; sample 0 is what
+        predict_device returns at that step, sample s of window b is keyed by row s * B + b."""
+        if not self.uq:
+            raise ValueError('predict_mc needs a uq model (RNNUqRangeEstimate): a point estimate predicts with dropout '
+                             'off (training=config.train), so every sample would be the same')
+        if int(samples) < 1:
+            raise ValueError('predict_mc: samples must be >= 1 (got %r)' % (samples,))
+        self._calls += 1
+        return self.engine.forward_mc(_to_device(self.engine, inp), int(samples), step=self._calls)
+
     def predict(self, inp, batch_size=None):
         """model.predict(inp) (train.py:289, predict.py:129): ndarrays [B,T,O], as model(inp) returns them."""
         return _keras([p.cpu().numpy() for p in self.predict_device(inp)])

@@ -57,6 +57,14 @@ class Predict(object):
                 if self.config.forecast_steps == 1:
                     preds = [preds]
                 variance = [np.zeros(x.shape) for x in preds]   # predict.py:133
+            elif self.config.mc_samples > 1:
+                # the reference's UQ ensemble in one prediction: the mean of the samples, and mean of the variances +
+                # variance of the variances (utils/post_processing.py:52-55); var_pred, the spread of the sampled
+                # predictions, is the one added column
+                moments = [[t.cpu().numpy() for t in m] for m in self.model.predict_mc(inp_dev, self.config.mc_samples)]
+                preds = [m[0] for m in moments]
+                variance = [m[1] + m[3] for m in moments]
+                outputs['norm_preds_var'].append(self._extract_preds([m[2] for m in moments]))
             else:                       # predict.py:135-138: [tar_1, var_1, .., tar_S, var_S]
                 model_preds = self.model.predict(inp_dev)
                 preds, variance = model_preds[0::2], model_preds[1::2]
@@ -66,7 +74,7 @@ class Predict(object):
         single_outputs = ['date', 'gvkey', 'seq_norm'] + [x for x in outputs.keys() if 'inp_t' in x]
         for key in single_outputs:
             outputs[key] = np.vstack(outputs[key])
-        for key in ['targets', 'norm_preds', 'norm_variance']:
+        for key in [k for k in ('targets', 'norm_preds', 'norm_variance', 'norm_preds_var') if k in outputs]:
             for i in range(self.config.forecast_steps):
                 outputs[key + '_' + str(i + 1)] = np.vstack([x[i] for x in outputs[key]])
             outputs.pop(key)
@@ -98,7 +106,7 @@ class Predict(object):
         if self.config.write_inp_to_out_file:
             for c in [x for x in df.columns if 'inp_t' in x]:
                 df[c] = unscale(df[c])
-        preds_keys = [x for x in df.columns if 'norm_preds_' in x]
+        preds_keys = [x for x in df.columns if 'norm_preds_' in x and 'norm_preds_var_' not in x]
         for pred_key in preds_keys:
             df['preds_' + pred_key.split('_')[-1]] = unscale(df[pred_key])
         for var_key in [x for x in df.columns if 'norm_variance_' in x]:

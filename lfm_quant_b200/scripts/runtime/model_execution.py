@@ -152,6 +152,10 @@ class ModelExecution(object):
         self.config = config
 
     def __call__(self):
+        if self.config.mc_samples != 1 and (self.config.mc_samples < 1 or not self.config.UQ or self.config.train):
+            raise ValueError('--mc_samples %d: Monte-Carlo dropout samples are drawn at UQ prediction only (--UQ=True '
+                             '--train=False); a point estimate predicts with dropout off, and training and validation '
+                             'take one sample' % self.config.mc_samples)
         if self.config.training_type == 'iterative':
             raise NotImplementedError
         return self.fixed_dates_execution()
