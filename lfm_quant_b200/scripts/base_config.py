@@ -103,7 +103,8 @@ SCHEMA = [
     ('cdrs_inference_date', _STRING, None, "CDRS Inference date. Format: '%Y-%m-%d' "),
     # ---- native-path extensions (not in the reference) -------------------------------------------------
     ('precision', _STRING, 'fp32', "'fp32' (parity mode) or 'bf16' (tensor-core gate GEMMs)"),
-    ('mc_samples', _INT, 1, 'Monte-Carlo dropout samples per window at UQ prediction'),
+    ('mc_samples', _INT, 1, 'Monte-Carlo dropout samples per window at UQ prediction; more than 1 also writes the '
+                            "UQ ensemble's ensemble_preds.dat with the calibrated lower bounds"),
 ]
 
 _DEFINERS = {_STRING: configs.DEFINE_string, _INT: configs.DEFINE_integer, _FLOAT: configs.DEFINE_float,

@@ -14,6 +14,10 @@ from ..model_base_class import BaseModelClass
 from ...model_utils.initializers import Initializer
 from ...model_utils.optimizers import Optimizers
 
+# Rows per launch of NativeForecaster.predict_mc: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to
+# 10x (bf16x3) faster than a handle of B rows on an H100 (DESIGN.md section 5c).
+MC_ROWS = 8192
+
 
 class _Variable(object):
     """The slice of tf.Variable the drivers touch: name, shape, numpy()."""
@@ -58,6 +62,7 @@ class NativeForecaster(object):
         specs = [(n, s) for (_, n, s, _, tr) in self.engine.specs if tr]
         self.trainable_variables = [_Variable(self, i, n, s) for i, (n, s) in enumerate(specs)]
         self._calls = 0
+        self._mc_engine, self._mc_stale = None, True
 
     @property
     def title(self):
@@ -71,7 +76,7 @@ class NativeForecaster(object):
         precision = getattr(config, 'precision', 'fp32')
         if config.forecast_steps > 1 and config.train and precision != 'fp32':
             raise NotImplementedError('forecast_steps > 1 trains on the fp32 kernels (precision=%s)' % precision)
-        engine = ForecastChainEngine(
+        self._engine_kw = dict(
             forecast_steps=config.forecast_steps, weights=list(config.forecast_steps_weights),
             max_batch=config.batch_size, seq_len=seq_len, n_inputs=n_inputs, n_outputs=n_outputs,
             num_hidden=config.num_hidden, num_layers=config.num_layers, target_idx=target_idx,
@@ -80,6 +85,7 @@ class NativeForecaster(object):
             rnn_lambda=config.rnn_lambda, max_grad_norm=config.max_grad_norm, max_norm=float(config.max_norm),
             sgd_momentum=config.sgd_momentum, seed=config.seed, forward_only=not config.train,
             rnn_cell=config.rnn_cell, uq=self.uq)
+        engine = ForecastChainEngine(**self._engine_kw)
         engine.set_weights(Initializer(config).initial_weights([(n, s) for (_, n, s, _, tr) in engine.specs if tr]))
         return engine
 
@@ -106,14 +112,48 @@ class NativeForecaster(object):
         """`samples` Monte-Carlo dropout samples of every window in one prediction, the in-process form of the
         reference's UQ ensemble (runtime/model_execution.py:201-241): per forecast step the device tensors
         (mean_pred, mean_var, var_pred, var_var) [B,T,O].  One step per call, as predict_device; sample 0 is what
-        predict_device returns at that step, sample s of window b is keyed by row s * B + b."""
+        predict_device returns at that step, sample s of window b is keyed by row s * B + b.
+
+        The samples run on an engine with room for min(samples * batch_size, MC_ROWS) rows per launch (_mc_rows_engine),
+        so that the samples of a batch share launches; the moments are the same bits on any launch size."""
         if not self.uq:
             raise ValueError('predict_mc needs a uq model (RNNUqRangeEstimate): a point estimate predicts with dropout '
                              'off (training=config.train), so every sample would be the same')
         if int(samples) < 1:
             raise ValueError('predict_mc: samples must be >= 1 (got %r)' % (samples,))
         self._calls += 1
-        return self.engine.forward_mc(_to_device(self.engine, inp), int(samples), step=self._calls)
+        return self._mc_rows_engine(int(samples)).forward_mc(_to_device(self.engine, inp), int(samples),
+                                                             step=self._calls)
+
+    def _mc_rows_engine(self, samples):
+        """The engine predict_mc runs on: the model's own (batch_size rows) when it is as wide as samples * batch_size
+        rows or MC_ROWS, as at samples = 1, where a wider handle is slower (DESIGN.md section 5c).  Else a forward-only
+        chain of the same stages and precision with max_batch = min(samples * batch_size, MC_ROWS), created at the first
+        such call (again for a larger count) and owned by the model.  It holds a copy of the weights, renewed after
+        set_weights, load_weights and the train steps."""
+        from ....engine import ForecastChainEngine
+        rows = min(samples * self.config.batch_size, MC_ROWS)
+        if rows <= self.engine.cfg.max_batch:
+            return self.engine
+        if self._mc_engine is None or self._mc_engine.cfg.max_batch < rows:
+            self._close_mc_engine()
+            self._mc_engine = ForecastChainEngine(**dict(self._engine_kw, max_batch=rows, forward_only=True))
+            self._mc_stale = True
+        if self._mc_stale:
+            for src, dst in zip(self.engine.stages, self._mc_engine.stages):
+                dst.set_flat(src.get_flat())
+            self._mc_stale = False
+        return self._mc_engine
+
+    def _close_mc_engine(self):
+        if self._mc_engine is not None:
+            self._mc_engine.close()
+            self._mc_engine = None
+
+    def close(self):
+        """Releases the device memory of the model's handles."""
+        self._close_mc_engine()
+        self.engine.close()
 
     def predict(self, inp, batch_size=None):
         """model.predict(inp) (train.py:289, predict.py:129): ndarrays [B,T,O], as model(inp) returns them."""
@@ -123,6 +163,7 @@ class NativeForecaster(object):
         """Fused fwd + loss + BPTT + clip + optimizer + MaxNorm (train.py:178-225); returns the device tensor
         {loss, mse}, on a uq model {uq_loss_last_tar, mse}."""
         assert isinstance(targets, (list, tuple)), 'targets must be the list of forecast_steps targets (train.py:188)'
+        self._mc_stale = True
         return self.engine.train_step(_to_device(self.engine, inp), [_to_device(self.engine, t) for t in targets],
                                       iteration, lr)
 
@@ -133,6 +174,7 @@ class NativeForecaster(object):
         if x is not None:
             assert isinstance(ys, (list, tuple)), 'ys must be the list of forecast_steps targets'
             x, ys = _to_device(self.engine, x), [_to_device(self.engine, t) for t in ys]
+        self._mc_stale = True
         return self.engine.train_step_dp(x, ys, step, lr, row0, denoms)
 
     # -- Keras API surface -------------------------------------------------------------------------------
@@ -180,6 +222,7 @@ class NativeForecaster(object):
                                     '%s.index (Keras save_weights) exists' % (prefix, os.path.basename(prefix),
                                                                               os.path.basename(prefix)))
         self.engine.load_named(lambda name: data[name])
+        self._mc_stale = True
 
     def get_weights(self):
         return self.engine.get_weights(trainable_only=False)
@@ -187,6 +230,7 @@ class NativeForecaster(object):
     def set_weights(self, weights):
         """The trainable arrays, optionally followed by the BatchNormalization statistics (get_weights' order)."""
         self.engine.set_weights(weights)
+        self._mc_stale = True
 
 
 class RNNPointEstimate(BaseModelClass):

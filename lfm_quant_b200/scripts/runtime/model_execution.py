@@ -2,7 +2,9 @@
 one config in-process.  A point-estimate ensemble (num_procs > 1, :154-199) runs its members in this process too: NPE of
 them at a time, each on its own host thread and CUDA stream, side by side on the GPU(s) (DESIGN.md
 section 6a).  The reference starts one ``lfm_quant.py`` process per member instead (:142).  The candidates of a
-hyper-parameter search generation run the same way (run_candidates, DESIGN.md section 6b)."""
+hyper-parameter search generation run the same way (run_candidates, DESIGN.md section 6b).  The ensembles'
+post-processing (utils/post_processing.py) is here too: ensemble_point_estimate, and ensemble_uq_estimate of a UQ
+prediction with Monte-Carlo samples (DESIGN.md section 5c)."""
 from __future__ import absolute_import, division, print_function
 
 import copy
@@ -16,6 +18,8 @@ from itertools import cycle
 
 import numpy as np
 import pandas as pd
+import scipy.optimize
+import scipy.stats
 
 
 def member_configs(config):
@@ -80,6 +84,14 @@ def ensemble_point_estimate(frames, forecast_steps):
     out = frames[0].copy()
     averaged = [c for c in out.columns if 'preds' in c]
     out[averaged] = np.stack([f[averaged].to_numpy(dtype=np.float64) for f in frames]).mean(axis=0)
+    _recompute_errors(out, forecast_steps)
+    _print_scaled_mse(out, forecast_steps)
+    return out
+
+
+def _recompute_errors(out, forecast_steps):
+    """Each forecast step's squared scaled error, absolute error, relative error and seq_norm-scaled squared error,
+    recomputed in place from the frame's predictions (utils/post_processing.py:62-73)."""
     for s in range(1, forecast_steps + 1):
         target, pred = out['targets_%d' % s], out['preds_%d' % s]
         err = (target - pred).abs()
@@ -87,7 +99,84 @@ def ensemble_point_estimate(frames, forecast_steps):
         out['abs_err_%d' % s] = err
         out['fcst_err_%d' % s] = err / target.abs()
         out['unscaled_squared_err_%d' % s] = (err / out['seq_norm']) ** 2
+
+
+def _print_scaled_mse(out, forecast_steps):
+    for s in range(1, forecast_steps + 1):
         print("Scaled MSE for step %i: %1.4f" % (s, out['norm_squared_diff_%d' % s].mean()))
+
+
+# The reference calibrates its lower bounds at this one level (post_processing.py:91-92): the interval that holds 50 % of
+# the true values, over the z-scores of 100 p-values (:109-110).
+CERTAINTY_LEVEL = 0.5
+CALIBRATION_Z = scipy.stats.norm.ppf(np.linspace(0.0001, 0.999999, 100))
+
+
+def coverage(pred, var, target, z):
+    """The fraction of the true values inside pred ± z·sqrt(var), for each z (post_processing.py:126-144).  A NaN target
+    counts as outside, and the denominator is the number of non-NaN targets."""
+    sd = np.sqrt(var)
+    zc = np.asarray(z, dtype=np.float64)[:, None]
+    inside = np.less_equal(pred - zc * sd, target) & np.less_equal(target, pred + zc * sd)
+    return inside.sum(axis=1) / (len(target) - np.isnan(target).sum())
+
+
+def calibrated_z(freq, z, level):
+    """sklearn.isotonic.IsotonicRegression().fit(freq, z).predict([level])[0] without scikit-learn: the increasing
+    least-squares fit of z on freq, tied frequencies merged into the mean of their z, linear between the fitted points,
+    NaN outside [min freq, max freq].  A single distinct frequency gives a constant fit, at every level."""
+    freq, z = np.asarray(freq, dtype=np.float64), np.asarray(z, dtype=np.float64)
+    order = np.lexsort((z, freq))
+    freq, z = freq[order], z[order]
+    xs, first, counts = np.unique(freq, return_index=True, return_counts=True)
+    ys = scipy.optimize.isotonic_regression(np.add.reduceat(z, first) / counts, weights=counts.astype(np.float64),
+                                            increasing=True).x
+    if len(ys) == 1:
+        return float(ys[0])
+    if not xs[0] <= level <= xs[-1]:
+        return np.nan
+    # the interior points of a flat run are dropped, as scikit-learn does, so that a level on a fitted point takes the
+    # same segment and rounds the same way
+    keep = np.ones(len(ys), dtype=bool)
+    keep[1:-1] = (ys[1:-1] != ys[:-2]) | (ys[1:-1] != ys[2:])
+    xs, ys = xs[keep], ys[keep]
+    hi = int(np.clip(np.searchsorted(xs, level), 1, len(xs) - 1))      # scipy.interpolate.interp1d, kind='linear'
+    lo = hi - 1
+    return float((ys[hi] - ys[lo]) / (xs[hi] - xs[lo]) * (level - xs[lo]) + ys[lo])
+
+
+def ensemble_uq_estimate(frame, forecast_steps):
+    """ensemble_preds.dat of a UQ prediction with Monte-Carlo dropout samples: what the reference's
+    aggregate_uq_estimate (utils/post_processing.py:83-124) returns for the one frame `frame` (preds.dat as read_results
+    reads it) at certainty level 0.5.  The frame already holds the ensemble's moments, so the mean over one member and
+    its zero variance leave them as they are.
+
+    The norm_preds_var_<k> columns are dropped first.  Added: pred_var_<k> = preds_<k> / sqrt(variance_<k>), the error
+    columns recomputed, and the calibrated lower bounds <pred field>_50 = pred - z_50 · sqrt(variance) of every
+    prediction column, where z_50 is the z-score whose interval covers 50 % of the true values (calibrated_z over
+    coverage).  When every target is NaN (a prediction for dates without targets) the lower bounds are NaN."""
+    out = frame.drop(columns=[c for c in frame.columns if c.startswith('norm_preds_var_')])
+    pred_fields = sorted(c for c in out.columns if 'preds' in c)
+    var_fields = sorted(c for c in out.columns if 'variance' in c)
+    tar_fields = sorted(c for c in out.columns if 'targets' in c)
+    if not (len(pred_fields) == len(var_fields) == len(tar_fields)
+            and all(p.split('_')[-1] == v.split('_')[-1] for p, v in zip(pred_fields, var_fields))):
+        raise ValueError('a UQ prediction holds one variance and one target column per prediction column; got %s, %s '
+                         'and %s' % (pred_fields, var_fields, tar_fields))
+    for p, v in zip(pred_fields, var_fields):
+        if 'norm' not in p:
+            out['pred_var_' + p.split('_')[-1]] = out[p] / np.sqrt(out[v])
+    _recompute_errors(out, forecast_steps)
+    suffix = '_%d' % int(CERTAINTY_LEVEL * 100)
+    if out[tar_fields[0]].isnull().all():
+        for p in pred_fields:
+            out[p + suffix] = np.nan
+        return out
+    for p, v, t in zip(pred_fields, var_fields, tar_fields):
+        pred, var = out[p].values, out[v].values
+        z = calibrated_z(coverage(pred, var, out[t].values, CALIBRATION_Z), CALIBRATION_Z, CERTAINTY_LEVEL)
+        out[p + suffix] = pred - z * np.sqrt(var)
+    _print_scaled_mse(out, forecast_steps)
     return out
 
 
@@ -254,12 +343,27 @@ class ModelExecution(object):
         df.to_csv(os.path.join(experiment_dir, 'ensemble_preds.dat'), sep=' ', index=False)
         return df
 
+    @classmethod
+    def write_uq_ensemble(cls, config):
+        """<experiments_dir>/<model_dir>/ensemble_preds.dat of a prediction with mc_samples > 1 Monte-Carlo samples
+        (ensemble_uq_estimate of pred/<preds_fname> as read_results reads it), the file the reference's UQ ensemble
+        writes (model_execution.py:237-241).  Returns that frame, or None when there are no predictions to read."""
+        frame = cls.read_results(config)[2]
+        if frame is None:
+            return None
+        df = ensemble_uq_estimate(frame, config.forecast_steps)
+        df.to_csv(os.path.join(config.experiments_dir, config.model_dir, 'ensemble_preds.dat'), sep=' ', index=False)
+        return df
+
     def uq_estimate_execution(self):
-        """runtime/model_execution.py:201-241: training, or prediction with one process, is a single execution; the
-        multi-process MC-dropout ensemble (num_procs > 1 at predict time: many dropout samples of one model) is not
-        built."""
+        """runtime/model_execution.py:201-241: training, or prediction with one process, is a single execution.  A
+        prediction with mc_samples > 1 holds the samples' moments and is followed by the ensemble's post-processing
+        (write_uq_ensemble).  The multi-process MC-dropout ensemble (num_procs > 1 at predict time) is not built."""
         if self.config.train or self.config.num_procs == 1:
-            return self.single_execution(self.config)
+            out = self.single_execution(self.config)
+            if not self.config.train and self.config.mc_samples > 1:
+                self.write_uq_ensemble(self.config)
+            return out
         raise NotImplementedError('UQ ensemble prediction (num_procs > 1) fans out whole predictions through files; run '
                                   'one lfm_quant.py per member')
 
