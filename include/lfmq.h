@@ -38,8 +38,15 @@ enum { LFMQ_OPT_ADADELTA = 0, LFMQ_OPT_ADAM = 1, LFMQ_OPT_RMSPROP = 2, LFMQ_OPT_
  * LFMQ_PREC_BF16X3: fp32-tolerance forward on tensor cores (forward_only handles: predict.py:129), same cells and heads
  *                   as forward_only LFMQ_PREC_BF16: every operand split into bf16 high + low halves, three wgmma products
  *                   per GEMM (hi*hi + lo*hi + hi*lo), accurate expf / tanhf gate nonlinearities, fp32 head -- <=1e-4 rel
- *                   vs the oracle. */
-enum { LFMQ_PREC_FP32 = 0, LFMQ_PREC_BF16 = 1, LFMQ_PREC_BF16X3 = 2 };
+ *                   vs the oracle.
+ * LFMQ_PREC_TF32:   the LFMQ_PREC_FP32 step with its GEMMs on wgmma tensor cores: operands rounded to tf32 (cvt.rna:
+ *                   nearest, ties away from zero), fp32 accumulation.  Pointwise cell algebra, carried state, BN /
+ *                   dropout, heads' activations, losses, clip, optimizer and MaxNorm are the fp32 path's own.  Any cell,
+ *                   head, num_layers and chain, trainable or forward_only, and the same parameter layout as fp32 (a
+ *                   checkpoint moves freely between precisions).  Deterministic like fp32: a row's outputs do not depend
+ *                   on the other rows or the launch size, and two backward calls give the same bits.  Dense handles
+ *                   refuse it. */
+enum { LFMQ_PREC_FP32 = 0, LFMQ_PREC_BF16 = 1, LFMQ_PREC_BF16X3 = 2, LFMQ_PREC_TF32 = 3 };
 
 /* config.rnn_cell (lfm_quant.py:39; rnn_point_estimate.py:80-102).  GRU is Keras' default reset_after=True cell:
  * 3 gate blocks z|r|h, bias [2][3H] (input row, recurrent row).  The tensor-core precisions train the LSTM cell only;
@@ -217,7 +224,8 @@ int32_t lfmq_train_step(lfmq_handle h, const float* x, const float* y, int32_t B
  * `stages`, `preds`, `y` are host arrays of n_stages (<= 8) entries; `weights` = config.forecast_steps_weights (host).
  * `work`: device floats, n_stages * B * seq_len * n_inputs (stage inputs + one input-gradient buffer).
  * Dropout streams of stage s continue the trunk's layer numbering (layer num_layers + s - 1).
- * Training-mode stages (cfg.train) run on the LFMQ_PREC_FP32 kernels; forward_only stages may use any precision.
+ * Training-mode stages (cfg.train) run on the LFMQ_PREC_FP32 or LFMQ_PREC_TF32 kernels; forward_only stages may use any
+ * precision.
  * Every stage of one chain has the same cfg.uq.  A uq chain (models/uq_range_estimate/rnn_uq_range_estimate.py:114-157)
  * gives every stage the heads OUTPUT_TARGET_{s+1} and OUTPUT_VARIANCE_{s+1}, keeps Dropout / recurrent dropout on in
  * every stage and builds each next window from the previous stage's TARGET predictions (variances never feed forward).

@@ -11,7 +11,7 @@ import os
 _LIB_PATH = os.environ.get('LFMQ_LIB_PATH') or os.path.join(os.path.dirname(os.path.abspath(__file__)), '_lfmq.so')
 
 OPTIMIZERS = {'Adadelta': 0, 'Adam': 1, 'RMSprop': 2, 'SGD': 3}
-PREC_FP32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
+PREC_FP32, PREC_BF16, PREC_BF16X3, PREC_TF32 = 0, 1, 2, 3
 CELLS = {'lstm': 0, 'gru': 1}           # LFMQ_CELL_*
 ABI_VERSION = 4                         # LFMQ_ABI_VERSION in include/lfmq.h (4: lfmq_chain_*, forecast_steps > 1)
 

@@ -9,6 +9,12 @@ namespace lfmq {
 // `scratch` (>= scratch_elems floats) is used for deterministic split-K partials.
 int sgemm(cudaStream_t s, int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBk,
           long sBn, float* C, long ldc, float beta, float* scratch, size_t scratch_elems);
+// C[M,N] = sum_z partial[z][M][N] (in z order) + beta*C: the reduction of a deterministic split-K product
+int splitk_reduce(cudaStream_t s, int M, int N, int S, const float* partial, float* C, long ldc, float beta);
+// sgemm's contract on sm_90a wgmma with tf32 operands (cvt.rna) and fp32 accumulation (tf32_gemm.cu): the GEMMs of a
+// LFMQ_PREC_TF32 handle
+int tf32_gemm(cudaStream_t s, int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBk,
+              long sBn, float* C, long ldc, float beta, float* scratch, size_t scratch_elems);
 
 int lstm_pointwise_fwd(cudaStream_t s, int B, int T, int H, int t, const float* z, const float* bias, float* gates,
                        float* c, float* h, const float* rmask, float* hm);

@@ -115,10 +115,13 @@ int sgemm(cudaStream_t s, int M, int N, int K, const float* A, long sAm, long sA
   else
     sgemm_kernel<false, false><<<grid, 256, 0, s>>>(M, N, K, A, sAm, sAk, B, sBk, sBn, C, ldc, beta, kchunk, partial);
   LFMQ_LAUNCH_CHECK();
-  if (S > 1) {
-    splitk_reduce_kernel<<<cdiv((long)M * N, 256), 256, 0, s>>>(M, N, S, partial, C, ldc, beta);
-    LFMQ_LAUNCH_CHECK();
-  }
+  if (S > 1) return splitk_reduce(s, M, N, S, partial, C, ldc, beta);
+  return 0;
+}
+
+int splitk_reduce(cudaStream_t s, int M, int N, int S, const float* partial, float* C, long ldc, float beta) {
+  splitk_reduce_kernel<<<cdiv((long)M * N, 256), 256, 0, s>>>(M, N, S, partial, C, ldc, beta);
+  LFMQ_LAUNCH_CHECK();
   return 0;
 }
 

@@ -96,7 +96,8 @@ int validate(const lfmq_config* c) {
                  c->uq);
     return LFMQ_ERR_ARG;
   }
-  if (c->precision != LFMQ_PREC_FP32 && c->precision != LFMQ_PREC_BF16 && c->precision != LFMQ_PREC_BF16X3) {
+  if (c->precision != LFMQ_PREC_FP32 && c->precision != LFMQ_PREC_BF16 && c->precision != LFMQ_PREC_BF16X3 &&
+      c->precision != LFMQ_PREC_TF32) {
     LFMQ_SET_ERR("lfmq_config: unknown precision %d", c->precision);
     return LFMQ_ERR_ARG;
   }
@@ -159,10 +160,12 @@ size_t layout(lfmq_handle_s* h, char* base) {
   h->tickets = reinterpret_cast<unsigned int*>(h->scalars);   // [0] mask count, [1] mask ticket, [2] norm ticket;
                                                               // zeroed at create, every user resets what it used
   const size_t BT = B * T;
-  // The fp32 path's activations.  The tensor-core paths carve their own (tc_layout / gen_layout) and never touch these.
+  // The fp32 path's activations (LFMQ_PREC_TF32 runs the same path).  The bf16 tensor-core paths carve their own
+  // (tc_layout / gen_layout) and never touch these.
+  const bool fp32_path = c.precision == LFMQ_PREC_FP32 || c.precision == LFMQ_PREC_TF32;
   h->z = h->zh = h->hm = h->preds = h->var = h->apre = nullptr;
   h->dz = h->dz2 = h->dy = h->dh_out = h->hp = h->dh_rec = h->dc = h->dpred = h->da = nullptr;
-  if (c.precision == LFMQ_PREC_FP32) {
+  if (fp32_path) {
     for (int l = 0; l < L; ++l) {
       LayerBuf& lb = h->layers[l];
       lb.h = cv.take<float>(BT * H);
@@ -201,7 +204,7 @@ size_t layout(lfmq_handle_s* h, char* base) {
   // (LSTM, H = 256, one layer, no recurrent dropout; LFMQ_FORCE_GENERIC=1 sends it to the general path as well), every
   // other supported configuration runs the general stepped path (rnn_tc.cu).
   h->use_gen = 0;
-  if (c.precision != LFMQ_PREC_FP32) {
+  if (!fp32_path) {
     const char* fg = getenv("LFMQ_FORCE_GENERIC");
     const bool force_gen = fg != nullptr && atoi(fg) != 0;
     const bool fast = c.precision == LFMQ_PREC_BF16 && !force_gen && lfmq::tc_shape_supported(c);
@@ -251,7 +254,7 @@ int validate_dense(const lfmq_dense_config* c) {
     LFMQ_SET_ERR("lfmq_dense_config: huber_delta must be positive (got %g)", c->huber_delta);
     return LFMQ_ERR_ARG;
   }
-  if (c->precision == LFMQ_PREC_BF16 || c->precision == LFMQ_PREC_BF16X3) {
+  if (c->precision == LFMQ_PREC_BF16 || c->precision == LFMQ_PREC_BF16X3 || c->precision == LFMQ_PREC_TF32) {
     LFMQ_SET_ERR("lfmq_dense_config: the linear model runs in fp32 only: it reads each input once for n_outputs "
                  "multiply-adds, so it is bound by memory bandwidth and tensor cores would not make it faster; "
                  "use LFMQ_PREC_FP32");
@@ -326,7 +329,15 @@ int check_batch(lfmq_handle h, int32_t B) {
   return 0;
 }
 
-// fp32 SIMT forward of all layers; fills layers[l].{h,c,y,(gates)} and `preds`.
+// Every GEMM of the fp32 step: the fp32 SIMT sgemm, or on a LFMQ_PREC_TF32 handle the same product on wgmma with tf32
+// operands (tf32_gemm.cu).  Everything else in forward_fp32 / backward_fp32 is shared by both precisions.
+int gemm(lfmq_handle h, cudaStream_t s, int M, int N, int K, const float* A, long sAm, long sAk, const float* B, long sBk,
+         long sBn, float* C, long ldc, float beta, float* scratch, size_t scratch_elems) {
+  return (h->cfg.precision == LFMQ_PREC_TF32 ? tf32_gemm : sgemm)(s, M, N, K, A, sAm, sAk, B, sBk, sBn, C, ldc, beta,
+                                                                  scratch, scratch_elems);
+}
+
+// fp32 SIMT (or tf32 GEMM) forward of all layers; fills layers[l].{h,c,y,(gates)} and `preds`.
 // uq handles also fill `var` [B,T,O] (and keep the variance head's pre-activation when a backward pass can follow).
 int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t step, float* preds, float* var,
                  cudaStream_t s) {
@@ -346,21 +357,21 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
       rmask = lb.rmask;
     }
     for (int t = 0; t < T && c.rnn_cell == LFMQ_CELL_GRU; ++t) {
-      RUN(sgemm(s, B, 3 * H, I, in + (long)t * I, (long)T * I, 1, P + lb.oW, 3 * H, 1, h->z, 3 * H, 0.f, nullptr, 0));
+      RUN(gemm(h, s, B, 3 * H, I, in + (long)t * I, (long)T * I, 1, P + lb.oW, 3 * H, 1, h->z, 3 * H, 0.f, nullptr, 0));
       if (t > 0) {
         const float* hp = rmask ? h->hm : lb.h + (long)(t - 1) * H;
         const long ld = rmask ? H : (long)T * H;
-        RUN(sgemm(s, B, 3 * H, H, hp, ld, 1, P + lb.oU, 3 * H, 1, h->zh, 3 * H, 0.f, nullptr, 0));
+        RUN(gemm(h, s, B, 3 * H, H, hp, ld, 1, P + lb.oU, 3 * H, 1, h->zh, 3 * H, 0.f, nullptr, 0));
       }
       RUN(gru_pointwise_fwd(s, B, T, H, t, h->z, t > 0 ? h->zh : nullptr, P + lb.ob, lb.gates, lb.h, rmask,
                             rmask ? h->hm : nullptr));
     }
     for (int t = 0; t < T && c.rnn_cell == LFMQ_CELL_LSTM; ++t) {
-      RUN(sgemm(s, B, 4 * H, I, in + (long)t * I, (long)T * I, 1, P + lb.oW, 4 * H, 1, h->z, 4 * H, 0.f, nullptr, 0));
+      RUN(gemm(h, s, B, 4 * H, I, in + (long)t * I, (long)T * I, 1, P + lb.oW, 4 * H, 1, h->z, 4 * H, 0.f, nullptr, 0));
       if (t > 0) {
         const float* hp = rmask ? h->hm : lb.h + (long)(t - 1) * H;
         const long ld = rmask ? H : (long)T * H;
-        RUN(sgemm(s, B, 4 * H, H, hp, ld, 1, P + lb.oU, 4 * H, 1, h->z, 4 * H, 1.f, nullptr, 0));
+        RUN(gemm(h, s, B, 4 * H, H, hp, ld, 1, P + lb.oU, 4 * H, 1, h->z, 4 * H, 1.f, nullptr, 0));
       }
       RUN(lstm_pointwise_fwd(s, B, T, H, t, h->z, P + lb.ob, lb.gates, lb.c, lb.h, rmask, rmask ? h->hm : nullptr));
     }
@@ -371,11 +382,11 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
   h->prof.end(LFMQ_REGION_FWD, s);
   h->prof.begin(LFMQ_REGION_HEAD, s);
   const float* yl = h->layers[L - 1].y;
-  RUN(sgemm(s, B * T, O, H, yl, H, 1, P + h->oWo, O, 1, preds, O, 0.f, nullptr, 0));
+  RUN(gemm(h, s, B * T, O, H, yl, H, 1, P + h->oWo, O, 1, preds, O, 0.f, nullptr, 0));
   RUN(add_bias_rows(s, (long)B * T, O, preds, P + h->obo));
   if (c.uq) {
     float* a = h->apre ? h->apre : var;           // forward-only handles activate in place
-    RUN(sgemm(s, B * T, O, H, yl, H, 1, P + h->oWv, O, 1, a, O, 0.f, nullptr, 0));
+    RUN(gemm(h, s, B * T, O, H, yl, H, 1, P + h->oWv, O, 1, a, O, 0.f, nullptr, 0));
     RUN(add_bias_rows(s, (long)B * T, O, a, P + h->obv));
     RUN(softplus_floor(s, (long)B * T * O, a, var));
   }
@@ -393,13 +404,13 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
   const float* yl = h->layers[L - 1].y;
   // head: dWo = y^T dpred, dbo = colsum(dpred), dy = dpred Wo^T
   h->prof.begin(LFMQ_REGION_HEAD, s);
-  RUN(sgemm(s, H, O, (int)BT, yl, 1, H, h->dpred, O, 1, G + h->oWo, O, 0.f, h->scratch, h->scratch_elems));
+  RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->dpred, O, 1, G + h->oWo, O, 0.f, h->scratch, h->scratch_elems));
   RUN(colsum(s, BT, O, h->dpred, G + h->obo, h->scratch, h->scratch_elems));
-  RUN(sgemm(s, (int)BT, H, O, h->dpred, O, 1, P + h->oWo, 1, O, h->dy, H, 0.f, nullptr, 0));
+  RUN(gemm(h, s, (int)BT, H, O, h->dpred, O, 1, P + h->oWo, 1, O, h->dy, H, 0.f, nullptr, 0));
   if (c.uq) {      // variance head: same three products on da, dy accumulates
-    RUN(sgemm(s, H, O, (int)BT, yl, 1, H, h->da, O, 1, G + h->oWv, O, 0.f, h->scratch, h->scratch_elems));
+    RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->da, O, 1, G + h->oWv, O, 0.f, h->scratch, h->scratch_elems));
     RUN(colsum(s, BT, O, h->da, G + h->obv, h->scratch, h->scratch_elems));
-    RUN(sgemm(s, (int)BT, H, O, h->da, O, 1, P + h->oWv, 1, O, h->dy, H, 1.f, nullptr, 0));
+    RUN(gemm(h, s, (int)BT, H, O, h->da, O, 1, P + h->oWv, 1, O, h->dy, H, 1.f, nullptr, 0));
   }
   h->prof.end(LFMQ_REGION_HEAD, s);
   for (int l = L - 1; l >= 0; --l) {
@@ -417,14 +428,14 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
       RUN(gru_pointwise_bwd(s, B, T, H, t, lb.gates, lb.h, h->dh_out, (t < T - 1) ? h->dh_rec : nullptr, rmask, h->dc,
                             h->dz, h->dz2));
       if (t > 0)
-        RUN(sgemm(s, B, H, 3 * H, h->dz2 + (long)t * 3 * H, (long)T * 3 * H, 1, P + lb.oU, 1, 3 * H, h->dh_rec, H, 0.f,
+        RUN(gemm(h, s, B, H, 3 * H, h->dz2 + (long)t * 3 * H, (long)T * 3 * H, 1, P + lb.oU, 1, 3 * H, h->dh_rec, H, 0.f,
                   nullptr, 0));
     }
     for (int t = T - 1; t >= 0 && !gru; --t) {
       RUN(lstm_pointwise_bwd(s, B, T, H, t, lb.gates, lb.c, h->dh_out, (t < T - 1) ? h->dh_rec : nullptr, rmask, h->dc,
                              h->dz));
       if (t > 0)
-        RUN(sgemm(s, B, H, 4 * H, h->dz + (long)t * 4 * H, (long)T * 4 * H, 1, P + lb.oU, 1, 4 * H, h->dh_rec, H, 0.f,
+        RUN(gemm(h, s, B, H, 4 * H, h->dz + (long)t * 4 * H, (long)T * 4 * H, 1, P + lb.oU, 1, 4 * H, h->dh_rec, H, 0.f,
                   nullptr, 0));
     }
     h->prof.end(LFMQ_REGION_BWD, s);
@@ -434,13 +445,13 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
     // bias rows [2][3H] = colsum of each.
     const float* dzr = gru ? h->dz2 : h->dz;
     const int GH = NG * H;
-    RUN(sgemm(s, I, GH, (int)BT, in, 1, I, h->dz, GH, 1, G + lb.oW, GH, 0.f, h->scratch, h->scratch_elems));
+    RUN(gemm(h, s, I, GH, (int)BT, in, 1, I, h->dz, GH, 1, G + lb.oW, GH, 0.f, h->scratch, h->scratch_elems));
     RUN(shift_mask(s, B, T, H, lb.h, rmask, h->hp));
-    RUN(sgemm(s, H, GH, (int)BT, h->hp, 1, H, dzr, GH, 1, G + lb.oU, GH, 0.f, h->scratch, h->scratch_elems));
+    RUN(gemm(h, s, H, GH, (int)BT, h->hp, 1, H, dzr, GH, 1, G + lb.oU, GH, 0.f, h->scratch, h->scratch_elems));
     RUN(colsum(s, BT, GH, h->dz, G + lb.ob, h->scratch, h->scratch_elems));
     if (gru) RUN(colsum(s, BT, GH, h->dz2, G + lb.ob + GH, h->scratch, h->scratch_elems));
     if (l > 0 || dx_out)
-      RUN(sgemm(s, (int)BT, I, GH, h->dz, GH, 1, P + lb.oW, 1, GH, l > 0 ? h->dy : dx_out, I, 0.f, nullptr, 0));
+      RUN(gemm(h, s, (int)BT, I, GH, h->dz, GH, 1, P + lb.oW, 1, GH, l > 0 ? h->dy : dx_out, I, 0.f, nullptr, 0));
     h->prof.end(LFMQ_REGION_WGRAD, s);
   }
   return 0;
@@ -960,7 +971,7 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
     h->prof.end(LFMQ_REGION_WGRAD, s);
     return LFMQ_OK;
   }
-  if (c.precision == LFMQ_PREC_FP32) {      // a trainable uq handle is always fp32
+  if (c.precision == LFMQ_PREC_FP32 || c.precision == LFMQ_PREC_TF32) {   // a trainable uq handle is always one of these
     // denom_dev: stage 0's counts, the three of lfmq_mask_count_uq or the two of lfmq_mask_count
     const float one = 1.0f;
     return backward_stages(&h, 1, x, &y, &one, B, row0, step, denom_dev, nullptr, nullptr, s);
@@ -1026,8 +1037,9 @@ int chain_check(const lfmq_handle* st, int32_t S, int32_t B, bool training) {
       LFMQ_SET_ERR("lfmq_chain: stage %d does not continue stage 0 (same T/F/O, one layer, same uq flag)", i);
       return LFMQ_ERR_ARG;
     }
-    if ((training || c.train) && c.precision != LFMQ_PREC_FP32) {
-      LFMQ_SET_ERR("lfmq_chain: training-mode stages run on the fp32 kernels (stage %d has precision %d)", i, c.precision);
+    if ((training || c.train) && c.precision != LFMQ_PREC_FP32 && c.precision != LFMQ_PREC_TF32) {
+      LFMQ_SET_ERR("lfmq_chain: training-mode stages run on the fp32 or tf32 kernels (stage %d has precision %d)", i,
+                   c.precision);
       return LFMQ_ERR_UNSUPPORTED;
     }
     if (training && c.forward_only) {

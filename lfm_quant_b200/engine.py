@@ -13,6 +13,10 @@ import torch
 
 from . import _native as N
 
+# config.precision -> LFMQ_PREC_*.  'tf32' runs the fp32 step with its GEMMs on tensor cores (tf32 operands, fp32
+# accumulation); dense handles refuse everything but 'fp32' in the library.
+PRECISIONS = {'fp32': N.PREC_FP32, 'bf16': N.PREC_BF16, 'bf16x3': N.PREC_BF16X3, 'tf32': N.PREC_TF32}
+
 
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
@@ -202,7 +206,7 @@ class ForecasterEngine(_HandleEngine):
         cfg.max_batch, cfg.seq_len, cfg.n_inputs, cfg.n_outputs = max_batch, seq_len, n_inputs, n_outputs
         cfg.num_hidden, cfg.num_layers, cfg.target_idx = num_hidden, num_layers, target_idx
         cfg.train = 1 if train else 0
-        cfg.precision = {'fp32': N.PREC_FP32, 'bf16': N.PREC_BF16, 'bf16x3': N.PREC_BF16X3}[precision]
+        cfg.precision = PRECISIONS[precision]
         cfg.optimizer = N.OPTIMIZERS[optimizer]
         cfg.forward_only = 1 if forward_only else 0
         if rnn_cell not in N.CELLS:
@@ -315,7 +319,7 @@ class DenseEngine(_HandleEngine):
         cfg.struct_size = C.sizeof(N.LfmqDenseConfig)
         cfg.max_batch, cfg.seq_len, cfg.n_inputs, cfg.n_outputs = max_batch, seq_len, n_inputs, n_outputs
         cfg.target_idx = target_idx
-        cfg.precision = {'fp32': N.PREC_FP32, 'bf16': N.PREC_BF16, 'bf16x3': N.PREC_BF16X3}[precision]
+        cfg.precision = PRECISIONS[precision]
         cfg.optimizer = N.OPTIMIZERS[optimizer]
         cfg.forward_only = 1 if forward_only else 0
         cfg.huber_loss = 1 if huber_loss else 0

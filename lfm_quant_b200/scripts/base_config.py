@@ -102,7 +102,8 @@ SCHEMA = [
     ('model_ranking_factor', _STRING, 'pred_var_entval', 'Model ranking factor'),
     ('cdrs_inference_date', _STRING, None, "CDRS Inference date. Format: '%Y-%m-%d' "),
     # ---- native-path extensions (not in the reference) -------------------------------------------------
-    ('precision', _STRING, 'fp32', "'fp32' (parity mode) or 'bf16' (tensor-core gate GEMMs)"),
+    ('precision', _STRING, 'fp32', "'fp32' (parity mode), 'tf32' (the fp32 step with tf32 tensor-core GEMMs: any "
+                                   "cell, head and forecast_steps), 'bf16' (tensor-core gate GEMMs) or 'bf16x3'"),
     ('mc_samples', _INT, 1, 'Monte-Carlo dropout samples per window at UQ prediction; more than 1 also writes the '
                             "UQ ensemble's ensemble_preds.dat with the calibrated lower bounds"),
 ]

@@ -116,7 +116,7 @@ SCHEMA = [
     ('piecewise_lr_values', configs.DEFINE_string, None, 'Values of the piecewise constant learning rate'),
     ('lr_schedule', configs.DEFINE_string, 'ExponentialDecay', 'Learning rate schedule'),
     # native-path extension (not in the reference), tunable like the model flags
-    ('precision', configs.DEFINE_list_string, 'fp32', "'fp32', 'bf16' or 'bf16x3'"),
+    ('precision', configs.DEFINE_list_string, 'fp32', "'fp32', 'tf32', 'bf16' or 'bf16x3'"),
 ]
 
 

@@ -51,7 +51,8 @@ class NativeForecaster(object):
     The engine is a ForecastChainEngine of config.forecast_steps stages (reference :109-150): every extra forecast step
     is one more recurrent layer + BatchNormalization + Dropout + Dense over the input window shifted by one, with
     [latest prediction's last time step, last available aux features] appended (models/model_base_class.py:18-51).
-    Multi-step training graphs run on the fp32 kernels; a forward-only graph (predict.py) may use any precision.
+    Multi-step training graphs run on the fp32 kernels (precision 'fp32' or 'tf32'); a forward-only graph (predict.py)
+    may use any precision.
     uq=True: RNNUqRangeEstimate's graph (rnn_uq_range_estimate.py:66-110,114-157): the outputs are
     [tar_1, var_1, .., tar_S, var_S] and the step returns {uq_loss_last_tar, mse}."""
 
@@ -74,8 +75,8 @@ class NativeForecaster(object):
         if config.rnn_cell not in ('lstm', 'gru'):
             raise NotImplementedError                    # rnn_point_estimate.py:101-102,148-149
         precision = getattr(config, 'precision', 'fp32')
-        if config.forecast_steps > 1 and config.train and precision != 'fp32':
-            raise NotImplementedError('forecast_steps > 1 trains on the fp32 kernels (precision=%s)' % precision)
+        if config.forecast_steps > 1 and config.train and precision not in ('fp32', 'tf32'):
+            raise NotImplementedError('forecast_steps > 1 trains on the fp32 or tf32 kernels (precision=%s)' % precision)
         self._engine_kw = dict(
             forecast_steps=config.forecast_steps, weights=list(config.forecast_steps_weights),
             max_batch=config.batch_size, seq_len=seq_len, n_inputs=n_inputs, n_outputs=n_outputs,
