@@ -158,9 +158,11 @@ int32_t lfmq_param_count(lfmq_handle h, int32_t* n_tensors, int64_t* n_trainable
 int32_t lfmq_param_spec(lfmq_handle h, int32_t index, char* name, int32_t name_cap, int32_t* ndim,
                         int64_t shape[2], int64_t* offset_elems, int32_t* trainable);
 /* Device pointers into the workspace: flat fp32 parameters [n_total]; flat gradients
- * [n_trainable + 8] whose tail holds {loss, mse_0} contributions of the last lfmq_backward,
- * {grad_norm, clip_scale} of the last lfmq_apply and, on a uq handle, [4] = uq_loss_last_tar (tail[0] is then the
+ * [n_trainable + LFMQ_TAIL_LEN] whose tail holds {loss, mse_0} contributions of the last lfmq_backward,
+ * {grad_norm, clip_scale} of the last lfmq_apply and, on a uq handle, uq_loss_last_tar (the loss slot is then the
  * weighted uq loss); optimizer slots [n_slots * n_trainable]. */
+enum { LFMQ_TAIL_LOSS = 0, LFMQ_TAIL_MSE0 = 1, LFMQ_TAIL_GRAD_NORM = 2, LFMQ_TAIL_CLIP_SCALE = 3,
+       LFMQ_TAIL_UQ_LOSS_LAST_TAR = 4, LFMQ_TAIL_LEN = 8 };   /* grads[n_trainable + LFMQ_TAIL_*] */
 int32_t lfmq_params_ptr(lfmq_handle h, float** dev);
 int32_t lfmq_grads_ptr(lfmq_handle h, float** dev);
 int32_t lfmq_opt_state_ptr(lfmq_handle h, float** dev, int64_t* n_elems);

@@ -12,6 +12,8 @@ _LIB_PATH = os.environ.get('LFMQ_LIB_PATH') or os.path.join(os.path.dirname(os.p
 
 OPTIMIZERS = {'Adadelta': 0, 'Adam': 1, 'RMSprop': 2, 'SGD': 3}
 PREC_FP32, PREC_BF16, PREC_BF16X3, PREC_TF32 = 0, 1, 2, 3
+# LFMQ_TAIL_*: the slots of the gradient vector's tail, grads[n_trainable + TAIL_*], and its length
+TAIL_LOSS, TAIL_MSE0, TAIL_GRAD_NORM, TAIL_CLIP_SCALE, TAIL_UQ_LOSS_LAST_TAR, TAIL_LEN = 0, 1, 2, 3, 4, 8
 CELLS = {'lstm': 0, 'gru': 1}           # LFMQ_CELL_*
 ABI_VERSION = 4                         # LFMQ_ABI_VERSION in include/lfmq.h (4: lfmq_chain_*, forecast_steps > 1)
 

@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -26,41 +27,69 @@ struct ParamSpec {
   int trainable;
 };
 
+// The fp32 path's activations of one layer
 struct LayerBuf {
   float *h, *c, *y, *gates, *rmask;
-  // offsets of this layer's tensors in the flat parameter vector
-  int64_t oW, oU, ob, ogamma, obeta, omean, ovar;
-  int I;
 };
+
+// The code that runs a handle, chosen once at create (choose_path).  Fp32 is the fp32 step (forward_fp32 /
+// backward_fp32) of LFMQ_PREC_FP32 and LFMQ_PREC_TF32 handles (gemm() picks the GEMM); Cluster the persistent cluster
+// kernels (lstm_tc.cu); General the general stepped tensor-core path (rnn_tc.cu); Dense the linear model (dense.cu).
+enum class Path { Fp32, Cluster, General, Dense };
+
+// The handle's block of device scalars (zeroed at create).  Each user resets the tickets it used.
+struct Scalars {
+  unsigned int mask_tickets[2];   // mask_count: the count and the last-block ticket
+  unsigned int norm_ticket;       // grad_norm_scale
+  unsigned int unused0[5];
+  float denom[3];                 // the loss counts of the handle's own batch (mask_count, stages_loss_uq)
+  float unused1;
+  float chain_loss[2];            // lfmq_chain_loss: this stage's {loss, mse}
+  float unused2[2];
+};
+static_assert(sizeof(Scalars) == 16 * sizeof(float), "one 64-byte block");
 
 }  // namespace
 
 struct lfmq_handle_s {
   lfmq_config cfg;
+  Path path = Path::Fp32;
   std::vector<ParamSpec> specs;
-  int64_t n_train, n_total, n_grad_buf;
-  int n_slots;
-  int64_t oWo, obo;
-  int64_t oWv, obv;          // uq: OUTPUT_VARIANCE_1 (oWo/obo are OUTPUT_TARGET_1 then)
+  lfmq::ParamLayout pl;      // offsets of the specs' tensors
+  int64_t n_train = 0, n_total = 0, n_grad_buf = 0;
+  int n_slots = 0;
   // workspace carve
-  float *params, *grads, *slots, *scalars, *denom;
-  unsigned int* tickets;
+  float *params = nullptr, *grads = nullptr, *slots = nullptr, *scratch = nullptr;
+  Scalars* sc = nullptr;
+  size_t scratch_elems = 0;
+  // the fp32 path's activations
   std::vector<LayerBuf> layers;
-  float *z, *hm, *dz, *dy, *dh_out, *hp, *dh_rec, *dc, *dpred, *preds, *scratch;
-  float *var, *apre, *da;   // uq only: variance output, its pre-activation, gradient w.r.t. the pre-activation
-  float *zh, *dz2;   // GRU only: recurrent projection of one step, gradient w.r.t. the recurrent projection
-  size_t scratch_elems;
+  float *z = nullptr, *hm = nullptr, *dz = nullptr, *dy = nullptr, *dh_out = nullptr, *hp = nullptr;
+  float *dh_rec = nullptr, *dc = nullptr, *dpred = nullptr, *preds = nullptr;
+  // uq only: variance output, its pre-activation, gradient w.r.t. the pre-activation
+  float *var = nullptr, *apre = nullptr, *da = nullptr;
+  // GRU only: recurrent projection of one step, gradient w.r.t. the recurrent projection
+  float *zh = nullptr, *dz2 = nullptr;
   lfmq::TcState tc;
   int64_t last_step = 0;     // step and row0 of the last forward: the fp32 backward regenerates that call's dropout masks
   int64_t last_row0 = 0;
-  int use_gen;               // 1: the general tensor-core path (rnn_tc.cu) runs this handle's bf16 / bf16x3 work
   lfmq::Profiler prof;
   // the linear baseline (lfmq_dense_create): cfg carries its shapes, target, loss weight, optimizer and clip, with
-  // num_layers = 0; params = [OUTPUT_1/kernel [T*F, O], OUTPUT_1/bias [O]]
-  int dense = 0;
+  // num_layers = 0; preds / dpred are its [B, O] outputs and their gradient
   int huber = 0;
   float huber_delta = 1.f;
   float* wpart = nullptr;    // row-block partials of the weight gradient (dense_wgrad)
+
+  ~lfmq_handle_s() {
+    lfmq::tc_destroy(tc);
+    lfmq::gen_destroy(tc);
+    if (prof.created)
+      for (int r = 0; r < lfmq::Profiler::kRegions; ++r)
+        for (int i = 0; i < lfmq::Profiler::kCap; ++i) {
+          cudaEventDestroy(prof.a[r][i]);
+          cudaEventDestroy(prof.b[r][i]);
+        }
+  }
 };
 
 namespace {
@@ -104,125 +133,130 @@ int validate(const lfmq_config* c) {
   return LFMQ_OK;
 }
 
-// Lays out specs + workspace; with base == nullptr only sizes are computed.
-size_t layout(lfmq_handle_s* h, char* base) {
+// The one place that decides which code runs a recurrent handle: the fp32 step for LFMQ_PREC_FP32 and LFMQ_PREC_TF32;
+// for LFMQ_PREC_BF16 the persistent cluster kernels on the shape family they are built for (LFMQ_FORCE_GENERIC=1 sends
+// that family to the general path as well); the general path for every other tensor-core configuration it supports.
+// Anything else is LFMQ_ERR_UNSUPPORTED, with *path = General.
+int choose_path(const lfmq_config& c, Path* path) {
+  char why[160];
+  const char* fg = getenv("LFMQ_FORCE_GENERIC");
+  const bool force_gen = fg != nullptr && atoi(fg) != 0;
+  if (c.precision == LFMQ_PREC_FP32 || c.precision == LFMQ_PREC_TF32) {
+    *path = Path::Fp32;
+  } else if (c.precision == LFMQ_PREC_BF16 && !force_gen && lfmq::tc_supported(c, why, sizeof(why))) {
+    *path = Path::Cluster;
+  } else {
+    *path = Path::General;
+    if (!lfmq::gen_supported(c, why, sizeof(why))) {
+      LFMQ_SET_ERR("tensor-core precision unsupported for this configuration: %s; use LFMQ_PREC_FP32", why);
+      return LFMQ_ERR_UNSUPPORTED;
+    }
+  }
+  return 0;
+}
+
+// The parameter specs in Keras order, with their offsets in h->pl, and the workspace carve: parameters, gradients,
+// optimizer slots, scalars and scratch, then the buffers of h->path (with_path = false leaves those out: the size of a
+// configuration no path supports, which lfmq_create refuses).  With base == nullptr only sizes are computed.
+size_t layout(lfmq_handle_s* h, char* base, bool with_path) {
   const lfmq_config& c = h->cfg;
   const int H = c.num_hidden, L = c.num_layers, T = c.seq_len, O = c.n_outputs;
-  const size_t B = (size_t)c.max_batch;
+  const size_t B = (size_t)c.max_batch, BT = B * T;
+  const bool gru = c.rnn_cell == LFMQ_CELL_GRU;
+  lfmq::ParamLayout& pl = h->pl;
+  pl = lfmq::ParamLayout{};
   h->specs.clear();
   int64_t off = 0;
   auto add = [&](const std::string& name, int ndim, int64_t s0, int64_t s1, int trainable) {
-    ParamSpec p{name, ndim, {s0, s1}, off, trainable};
+    h->specs.push_back(ParamSpec{name, ndim, {s0, s1}, off, trainable});
     off += s0 * (ndim == 2 ? s1 : 1);
-    h->specs.push_back(p);
-    return p.offset;
+    return h->specs.back().offset;
   };
-  h->layers.assign(L, LayerBuf{});
+  auto bn = [](int l) {
+    return l == 0 ? std::string("batch_normalization") : "batch_normalization_" + std::to_string(l);
+  };
+  pl.layers.resize(L);       // none on a dense handle
   for (int l = 0; l < L; ++l) {
-    LayerBuf& lb = h->layers[l];
-    lb.I = (l == 0) ? c.n_inputs : H;
-    const bool gru = c.rnn_cell == LFMQ_CELL_GRU;
+    lfmq::ParamLayout::Layer& o = pl.layers[l];
+    o.I = (l == 0) ? c.n_inputs : H;
     const int NG = gru ? 3 : 4;
     const std::string ls = std::string(gru ? "gru_" : "lstm_") + std::to_string(l + 1);
-    const std::string bn = (l == 0) ? "batch_normalization" : "batch_normalization_" + std::to_string(l);
-    lb.oW = add(ls + "/kernel", 2, lb.I, NG * H, 1);
-    lb.oU = add(ls + "/recurrent_kernel", 2, H, NG * H, 1);
-    lb.ob = gru ? add(ls + "/bias", 2, 2, 3 * H, 1) : add(ls + "/bias", 1, 4 * H, 1, 1);
-    lb.ogamma = add(bn + "/gamma", 1, H, 1, 1);
-    lb.obeta = add(bn + "/beta", 1, H, 1, 1);
+    o.oW = add(ls + "/kernel", 2, o.I, NG * H, 1);
+    o.oU = add(ls + "/recurrent_kernel", 2, H, NG * H, 1);
+    o.ob = gru ? add(ls + "/bias", 2, 2, 3 * H, 1) : add(ls + "/bias", 1, 4 * H, 1, 1);
+    o.ogamma = add(bn(l) + "/gamma", 1, H, 1, 1);
+    o.obeta = add(bn(l) + "/beta", 1, H, 1, 1);
   }
   if (c.uq) {
-    h->oWo = add("OUTPUT_TARGET_1/kernel", 2, H, O, 1);
-    h->obo = add("OUTPUT_TARGET_1/bias", 1, O, 1, 1);
-    h->oWv = add("OUTPUT_VARIANCE_1/kernel", 2, H, O, 1);
-    h->obv = add("OUTPUT_VARIANCE_1/bias", 1, O, 1, 1);
-  } else {
-    h->oWo = add("OUTPUT_1/kernel", 2, H, O, 1);
-    h->obo = add("OUTPUT_1/bias", 1, O, 1, 1);
-    h->oWv = h->obv = -1;
+    pl.oWo = add("OUTPUT_TARGET_1/kernel", 2, H, O, 1);
+    pl.obo = add("OUTPUT_TARGET_1/bias", 1, O, 1, 1);
+    pl.oWv = add("OUTPUT_VARIANCE_1/kernel", 2, H, O, 1);
+    pl.obv = add("OUTPUT_VARIANCE_1/bias", 1, O, 1, 1);
+  } else {       // the dense model's OUTPUT_1 reads the flattened input window
+    pl.oWo = add("OUTPUT_1/kernel", 2, h->path == Path::Dense ? (int64_t)T * c.n_inputs : H, O, 1);
+    pl.obo = add("OUTPUT_1/bias", 1, O, 1, 1);
   }
   h->n_train = off;
   for (int l = 0; l < L; ++l) {
-    const std::string bn = (l == 0) ? "batch_normalization" : "batch_normalization_" + std::to_string(l);
-    h->layers[l].omean = add(bn + "/moving_mean", 1, H, 1, 0);
-    h->layers[l].ovar = add(bn + "/moving_variance", 1, H, 1, 0);
+    pl.layers[l].omean = add(bn(l) + "/moving_mean", 1, H, 1, 0);
+    pl.layers[l].ovar = add(bn(l) + "/moving_variance", 1, H, 1, 0);
   }
   h->n_total = off;
-  h->n_grad_buf = (h->n_train + 8 + 3) / 4 * 4;
+  h->n_grad_buf = (h->n_train + LFMQ_TAIL_LEN + 3) / 4 * 4;
   h->n_slots = (c.optimizer == LFMQ_OPT_ADADELTA || c.optimizer == LFMQ_OPT_ADAM) ? 2 : 1;
 
   Carver cv{base, 0};
   h->params = cv.take<float>(h->n_total);
   h->grads = cv.take<float>(h->n_grad_buf);
   h->slots = c.forward_only ? nullptr : cv.take<float>((size_t)h->n_slots * h->n_train);
-  h->scalars = cv.take<float>(16);
-  h->denom = h->scalars + 8;
-  h->tickets = reinterpret_cast<unsigned int*>(h->scalars);   // [0] mask count, [1] mask ticket, [2] norm ticket;
-                                                              // zeroed at create, every user resets what it used
-  const size_t BT = B * T;
-  // The fp32 path's activations (LFMQ_PREC_TF32 runs the same path).  The bf16 tensor-core paths carve their own
-  // (tc_layout / gen_layout) and never touch these.
-  const bool fp32_path = c.precision == LFMQ_PREC_FP32 || c.precision == LFMQ_PREC_TF32;
-  h->z = h->zh = h->hm = h->preds = h->var = h->apre = nullptr;
-  h->dz = h->dz2 = h->dy = h->dh_out = h->hp = h->dh_rec = h->dc = h->dpred = h->da = nullptr;
-  if (fp32_path) {
-    for (int l = 0; l < L; ++l) {
-      LayerBuf& lb = h->layers[l];
-      lb.h = cv.take<float>(BT * H);
-      lb.c = cv.take<float>(BT * H);
-      lb.y = cv.take<float>(BT * H);
-      lb.gates = c.forward_only ? nullptr : cv.take<float>(BT * 4 * H);
-      lb.rmask = cv.take<float>(B * H);
-    }
-    h->z = cv.take<float>(B * 4 * H);
-    h->zh = (c.rnn_cell == LFMQ_CELL_GRU) ? cv.take<float>(B * 3 * H) : nullptr;
-    h->hm = cv.take<float>(B * H);
-    h->preds = cv.take<float>(BT * O);
-    h->var = c.uq ? cv.take<float>(BT * O) : nullptr;
-    h->apre = (c.uq && !c.forward_only) ? cv.take<float>(BT * O) : nullptr;
-    if (!c.forward_only) {
-      h->dz = cv.take<float>(BT * 4 * H);
-      h->dz2 = (c.rnn_cell == LFMQ_CELL_GRU) ? cv.take<float>(BT * 3 * H) : nullptr;
-      h->dy = cv.take<float>(BT * H);
-      h->dh_out = cv.take<float>(BT * H);
-      h->hp = cv.take<float>(BT * H);
-      h->dh_rec = cv.take<float>(B * H);
-      h->dc = cv.take<float>(B * H);
-      h->dpred = cv.take<float>(BT * O);
-      h->da = c.uq ? cv.take<float>(BT * O) : nullptr;
-    }
-  }
-  // scratch serves every precision (lfmq_loss, grad_norm_scale)
-  size_t scratch = (size_t)4 << 20;
-  if (!c.forward_only) {
-    const size_t bn_need = ((BT + 127) / 128) * 2 * H + (size_t)1024 * 2 * H;
-    if (bn_need > scratch) scratch = bn_need;
-  }
-  h->scratch_elems = scratch;
-  h->scratch = cv.take<float>(scratch);
-  // Tensor-core precisions: the persistent cluster kernels (lstm_tc.cu) take the shape family they are specialised for
-  // (LSTM, H = 256, one layer, no recurrent dropout; LFMQ_FORCE_GENERIC=1 sends it to the general path as well), every
-  // other supported configuration runs the general stepped path (rnn_tc.cu).
-  h->use_gen = 0;
-  if (!fp32_path) {
-    const char* fg = getenv("LFMQ_FORCE_GENERIC");
-    const bool force_gen = fg != nullptr && atoi(fg) != 0;
-    const bool fast = c.precision == LFMQ_PREC_BF16 && !force_gen && lfmq::tc_shape_supported(c);
-    if (!fast) {
-      h->use_gen = 1;
-      std::vector<lfmq::GenLayerOff> lo(L);
-      for (int l = 0; l < L; ++l) {
-        const LayerBuf& lb = h->layers[l];
-        lo[l] = lfmq::GenLayerOff{lb.oW, lb.oU, lb.ob, lb.ogamma, lb.obeta, lb.omean, lb.ovar, lb.I};
+  h->sc = cv.take<Scalars>(1);
+  // scratch serves every path (lfmq_loss, grad_norm_scale; the fp32 BN backward)
+  h->scratch_elems = (size_t)4 << 20;
+  if (!c.forward_only && h->path != Path::Dense)
+    h->scratch_elems = std::max(h->scratch_elems, ((BT + 127) / 128) * 2 * H + (size_t)1024 * 2 * H);
+  h->scratch = cv.take<float>(h->scratch_elems);
+  if (!with_path) return cv.off;
+  switch (h->path) {
+    case Path::Fp32:
+      h->layers.assign(L, LayerBuf{});
+      for (LayerBuf& lb : h->layers) {
+        lb.h = cv.take<float>(BT * H);
+        lb.c = cv.take<float>(BT * H);
+        lb.y = cv.take<float>(BT * H);
+        lb.gates = c.forward_only ? nullptr : cv.take<float>(BT * 4 * H);
+        lb.rmask = cv.take<float>(B * H);
       }
-      char why[160];
-      if (lfmq::gen_supported(c, why, sizeof(why)))      // lfmq_create reports unsupported configurations (gen_init)
-        lfmq::gen_layout(h->tc, c, lo.data(), h->oWo, h->obo, h->oWv, h->obv, cv);
-    } else {
-      const LayerBuf& lb = h->layers[0];
-      lfmq::tc_layout(h->tc, c, lfmq::TcParamOff{lb.oW, lb.oU, lb.ob, lb.ogamma, lb.obeta, lb.omean, lb.ovar, h->oWo, h->obo},
-                      cv);
-    }
+      h->z = cv.take<float>(B * 4 * H);
+      h->zh = gru ? cv.take<float>(B * 3 * H) : nullptr;
+      h->hm = cv.take<float>(B * H);
+      h->preds = cv.take<float>(BT * O);
+      h->var = c.uq ? cv.take<float>(BT * O) : nullptr;
+      h->apre = (c.uq && !c.forward_only) ? cv.take<float>(BT * O) : nullptr;
+      if (!c.forward_only) {
+        h->dz = cv.take<float>(BT * 4 * H);
+        h->dz2 = gru ? cv.take<float>(BT * 3 * H) : nullptr;
+        h->dy = cv.take<float>(BT * H);
+        h->dh_out = cv.take<float>(BT * H);
+        h->hp = cv.take<float>(BT * H);
+        h->dh_rec = cv.take<float>(B * H);
+        h->dc = cv.take<float>(B * H);
+        h->dpred = cv.take<float>(BT * O);
+        h->da = c.uq ? cv.take<float>(BT * O) : nullptr;
+      }
+      break;
+    case Path::Cluster:
+      lfmq::tc_layout(h->tc, c, cv);
+      break;
+    case Path::General:
+      lfmq::gen_layout(h->tc, c, pl, cv);
+      break;
+    case Path::Dense:
+      if (!c.forward_only) {
+        h->preds = cv.take<float>(B * O);
+        h->dpred = cv.take<float>(B * O);
+        h->wpart = cv.take<float>(lfmq::dense_wgrad_scratch(c.max_batch, T * c.n_inputs, O));
+      }
+      break;
   }
   return cv.off;
 }
@@ -267,44 +301,9 @@ int validate_dense(const lfmq_dense_config* c) {
   return LFMQ_OK;
 }
 
-// The dense handle's specs and workspace; with base == nullptr only sizes are computed.
-size_t dense_layout(lfmq_handle_s* h, char* base) {
-  const lfmq_config& c = h->cfg;
-  const int K = c.seq_len * c.n_inputs, O = c.n_outputs;
-  h->specs.clear();
-  h->specs.push_back(ParamSpec{"OUTPUT_1/kernel", 2, {K, O}, 0, 1});
-  h->specs.push_back(ParamSpec{"OUTPUT_1/bias", 1, {O, 1}, (int64_t)K * O, 1});
-  h->layers.clear();
-  h->oWo = 0;
-  h->obo = (int64_t)K * O;
-  h->oWv = h->obv = -1;
-  h->n_train = h->n_total = (int64_t)(K + 1) * O;
-  h->n_grad_buf = (h->n_train + 8 + 3) / 4 * 4;
-  h->n_slots = (c.optimizer == LFMQ_OPT_ADADELTA || c.optimizer == LFMQ_OPT_ADAM) ? 2 : 1;
-  Carver cv{base, 0};
-  h->params = cv.take<float>(h->n_total);
-  h->grads = cv.take<float>(h->n_grad_buf);
-  h->slots = c.forward_only ? nullptr : cv.take<float>((size_t)h->n_slots * h->n_train);
-  h->scalars = cv.take<float>(16);
-  h->denom = h->scalars + 8;
-  h->tickets = reinterpret_cast<unsigned int*>(h->scalars);
-  h->z = h->zh = h->hm = h->var = h->apre = nullptr;
-  h->dz = h->dz2 = h->dy = h->dh_out = h->hp = h->dh_rec = h->dc = h->da = nullptr;
-  h->preds = h->dpred = h->wpart = nullptr;
-  if (!c.forward_only) {
-    h->preds = cv.take<float>((size_t)c.max_batch * O);
-    h->dpred = cv.take<float>((size_t)c.max_batch * O);
-    h->wpart = cv.take<float>(lfmq::dense_wgrad_scratch(c.max_batch, K, O));
-  }
-  h->scratch_elems = (size_t)4 << 20;      // lfmq_loss (any B) and grad_norm_scale
-  h->scratch = cv.take<float>(h->scratch_elems);
-  h->use_gen = 0;
-  return cv.off;
-}
-
 // Entry points that serve recurrent handles only.
 int refuse_dense(lfmq_handle h, const char* fn) {
-  if (h && h->dense) {
+  if (h && h->path == Path::Dense) {
     LFMQ_SET_ERR("%s: not defined for a dense handle (lfmq_dense_create)", fn);
     return LFMQ_ERR_ARG;
   }
@@ -347,8 +346,9 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
   h->prof.begin(LFMQ_REGION_FWD, s);
   for (int l = 0; l < L; ++l) {
     LayerBuf& lb = h->layers[l];
+    const lfmq::ParamLayout::Layer& o = h->pl.layers[l];
     const float* in = (l == 0) ? x : h->layers[l - 1].y;
-    const int I = lb.I;
+    const int I = o.I;
     const float* rmask = nullptr;
     const bool stochastic = c.train || c.uq;       // rnn_uq_range_estimate.py:86,88: training=True is a literal there
     if (stochastic && c.recurrent_dropout > 0.f) {
@@ -357,37 +357,37 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
       rmask = lb.rmask;
     }
     for (int t = 0; t < T && c.rnn_cell == LFMQ_CELL_GRU; ++t) {
-      RUN(gemm(h, s, B, 3 * H, I, in + (long)t * I, (long)T * I, 1, P + lb.oW, 3 * H, 1, h->z, 3 * H, 0.f, nullptr, 0));
+      RUN(gemm(h, s, B, 3 * H, I, in + (long)t * I, (long)T * I, 1, P + o.oW, 3 * H, 1, h->z, 3 * H, 0.f, nullptr, 0));
       if (t > 0) {
         const float* hp = rmask ? h->hm : lb.h + (long)(t - 1) * H;
         const long ld = rmask ? H : (long)T * H;
-        RUN(gemm(h, s, B, 3 * H, H, hp, ld, 1, P + lb.oU, 3 * H, 1, h->zh, 3 * H, 0.f, nullptr, 0));
+        RUN(gemm(h, s, B, 3 * H, H, hp, ld, 1, P + o.oU, 3 * H, 1, h->zh, 3 * H, 0.f, nullptr, 0));
       }
-      RUN(gru_pointwise_fwd(s, B, T, H, t, h->z, t > 0 ? h->zh : nullptr, P + lb.ob, lb.gates, lb.h, rmask,
+      RUN(gru_pointwise_fwd(s, B, T, H, t, h->z, t > 0 ? h->zh : nullptr, P + o.ob, lb.gates, lb.h, rmask,
                             rmask ? h->hm : nullptr));
     }
     for (int t = 0; t < T && c.rnn_cell == LFMQ_CELL_LSTM; ++t) {
-      RUN(gemm(h, s, B, 4 * H, I, in + (long)t * I, (long)T * I, 1, P + lb.oW, 4 * H, 1, h->z, 4 * H, 0.f, nullptr, 0));
+      RUN(gemm(h, s, B, 4 * H, I, in + (long)t * I, (long)T * I, 1, P + o.oW, 4 * H, 1, h->z, 4 * H, 0.f, nullptr, 0));
       if (t > 0) {
         const float* hp = rmask ? h->hm : lb.h + (long)(t - 1) * H;
         const long ld = rmask ? H : (long)T * H;
-        RUN(gemm(h, s, B, 4 * H, H, hp, ld, 1, P + lb.oU, 4 * H, 1, h->z, 4 * H, 1.f, nullptr, 0));
+        RUN(gemm(h, s, B, 4 * H, H, hp, ld, 1, P + o.oU, 4 * H, 1, h->z, 4 * H, 1.f, nullptr, 0));
       }
-      RUN(lstm_pointwise_fwd(s, B, T, H, t, h->z, P + lb.ob, lb.gates, lb.c, lb.h, rmask, rmask ? h->hm : nullptr));
+      RUN(lstm_pointwise_fwd(s, B, T, H, t, h->z, P + o.ob, lb.gates, lb.c, lb.h, rmask, rmask ? h->hm : nullptr));
     }
     const bool drop = stochastic && c.dropout > 0.f;
-    RUN(bn_dropout_fwd(s, B, T, H, lb.h, P + lb.ogamma, P + lb.obeta, P + lb.omean, P + lb.ovar, c.bn_epsilon, drop,
+    RUN(bn_dropout_fwd(s, B, T, H, lb.h, P + o.ogamma, P + o.obeta, P + o.omean, P + o.ovar, c.bn_epsilon, drop,
                        dropout_key(c.seed, h->tc.stream_base + 2 * l, step, c.dropout), row0, lb.y));
   }
   h->prof.end(LFMQ_REGION_FWD, s);
   h->prof.begin(LFMQ_REGION_HEAD, s);
   const float* yl = h->layers[L - 1].y;
-  RUN(gemm(h, s, B * T, O, H, yl, H, 1, P + h->oWo, O, 1, preds, O, 0.f, nullptr, 0));
-  RUN(add_bias_rows(s, (long)B * T, O, preds, P + h->obo));
+  RUN(gemm(h, s, B * T, O, H, yl, H, 1, P + h->pl.oWo, O, 1, preds, O, 0.f, nullptr, 0));
+  RUN(add_bias_rows(s, (long)B * T, O, preds, P + h->pl.obo));
   if (c.uq) {
     float* a = h->apre ? h->apre : var;           // forward-only handles activate in place
-    RUN(gemm(h, s, B * T, O, H, yl, H, 1, P + h->oWv, O, 1, a, O, 0.f, nullptr, 0));
-    RUN(add_bias_rows(s, (long)B * T, O, a, P + h->obv));
+    RUN(gemm(h, s, B * T, O, H, yl, H, 1, P + h->pl.oWv, O, 1, a, O, 0.f, nullptr, 0));
+    RUN(add_bias_rows(s, (long)B * T, O, a, P + h->pl.obv));
     RUN(softplus_floor(s, (long)B * T * O, a, var));
   }
   h->prof.end(LFMQ_REGION_HEAD, s);
@@ -404,38 +404,39 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
   const float* yl = h->layers[L - 1].y;
   // head: dWo = y^T dpred, dbo = colsum(dpred), dy = dpred Wo^T
   h->prof.begin(LFMQ_REGION_HEAD, s);
-  RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->dpred, O, 1, G + h->oWo, O, 0.f, h->scratch, h->scratch_elems));
-  RUN(colsum(s, BT, O, h->dpred, G + h->obo, h->scratch, h->scratch_elems));
-  RUN(gemm(h, s, (int)BT, H, O, h->dpred, O, 1, P + h->oWo, 1, O, h->dy, H, 0.f, nullptr, 0));
+  RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->dpred, O, 1, G + h->pl.oWo, O, 0.f, h->scratch, h->scratch_elems));
+  RUN(colsum(s, BT, O, h->dpred, G + h->pl.obo, h->scratch, h->scratch_elems));
+  RUN(gemm(h, s, (int)BT, H, O, h->dpred, O, 1, P + h->pl.oWo, 1, O, h->dy, H, 0.f, nullptr, 0));
   if (c.uq) {      // variance head: same three products on da, dy accumulates
-    RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->da, O, 1, G + h->oWv, O, 0.f, h->scratch, h->scratch_elems));
-    RUN(colsum(s, BT, O, h->da, G + h->obv, h->scratch, h->scratch_elems));
-    RUN(gemm(h, s, (int)BT, H, O, h->da, O, 1, P + h->oWv, 1, O, h->dy, H, 1.f, nullptr, 0));
+    RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->da, O, 1, G + h->pl.oWv, O, 0.f, h->scratch, h->scratch_elems));
+    RUN(colsum(s, BT, O, h->da, G + h->pl.obv, h->scratch, h->scratch_elems));
+    RUN(gemm(h, s, (int)BT, H, O, h->da, O, 1, P + h->pl.oWv, 1, O, h->dy, H, 1.f, nullptr, 0));
   }
   h->prof.end(LFMQ_REGION_HEAD, s);
   for (int l = L - 1; l >= 0; --l) {
     LayerBuf& lb = h->layers[l];
-    const int I = lb.I;
+    const lfmq::ParamLayout::Layer& o = h->pl.layers[l];
+    const int I = o.I;
     const float* rmask = ((c.train || c.uq) && c.recurrent_dropout > 0.f) ? lb.rmask : nullptr;
     const bool drop = (c.train || c.uq) && c.dropout > 0.f;
     h->prof.begin(LFMQ_REGION_BWD, s);
-    RUN(bn_dropout_bwd(s, B, T, H, h->dy, lb.h, P + lb.ogamma, P + lb.omean, P + lb.ovar, c.bn_epsilon, drop,
+    RUN(bn_dropout_bwd(s, B, T, H, h->dy, lb.h, P + o.ogamma, P + o.omean, P + o.ovar, c.bn_epsilon, drop,
                        dropout_key(c.seed, h->tc.stream_base + 2 * l, h->last_step, c.dropout), h->last_row0, h->dh_out,
-                       G + lb.ogamma, G + lb.obeta, h->scratch, h->scratch_elems));
+                       G + o.ogamma, G + o.obeta, h->scratch, h->scratch_elems));
     const bool gru = c.rnn_cell == LFMQ_CELL_GRU;
     const int NG = gru ? 3 : 4;
     for (int t = T - 1; t >= 0 && gru; --t) {
       RUN(gru_pointwise_bwd(s, B, T, H, t, lb.gates, lb.h, h->dh_out, (t < T - 1) ? h->dh_rec : nullptr, rmask, h->dc,
                             h->dz, h->dz2));
       if (t > 0)
-        RUN(gemm(h, s, B, H, 3 * H, h->dz2 + (long)t * 3 * H, (long)T * 3 * H, 1, P + lb.oU, 1, 3 * H, h->dh_rec, H, 0.f,
+        RUN(gemm(h, s, B, H, 3 * H, h->dz2 + (long)t * 3 * H, (long)T * 3 * H, 1, P + o.oU, 1, 3 * H, h->dh_rec, H, 0.f,
                   nullptr, 0));
     }
     for (int t = T - 1; t >= 0 && !gru; --t) {
       RUN(lstm_pointwise_bwd(s, B, T, H, t, lb.gates, lb.c, h->dh_out, (t < T - 1) ? h->dh_rec : nullptr, rmask, h->dc,
                              h->dz));
       if (t > 0)
-        RUN(gemm(h, s, B, H, 4 * H, h->dz + (long)t * 4 * H, (long)T * 4 * H, 1, P + lb.oU, 1, 4 * H, h->dh_rec, H, 0.f,
+        RUN(gemm(h, s, B, H, 4 * H, h->dz + (long)t * 4 * H, (long)T * 4 * H, 1, P + o.oU, 1, 4 * H, h->dh_rec, H, 0.f,
                   nullptr, 0));
     }
     h->prof.end(LFMQ_REGION_BWD, s);
@@ -445,19 +446,20 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
     // bias rows [2][3H] = colsum of each.
     const float* dzr = gru ? h->dz2 : h->dz;
     const int GH = NG * H;
-    RUN(gemm(h, s, I, GH, (int)BT, in, 1, I, h->dz, GH, 1, G + lb.oW, GH, 0.f, h->scratch, h->scratch_elems));
+    RUN(gemm(h, s, I, GH, (int)BT, in, 1, I, h->dz, GH, 1, G + o.oW, GH, 0.f, h->scratch, h->scratch_elems));
     RUN(shift_mask(s, B, T, H, lb.h, rmask, h->hp));
-    RUN(gemm(h, s, H, GH, (int)BT, h->hp, 1, H, dzr, GH, 1, G + lb.oU, GH, 0.f, h->scratch, h->scratch_elems));
-    RUN(colsum(s, BT, GH, h->dz, G + lb.ob, h->scratch, h->scratch_elems));
-    if (gru) RUN(colsum(s, BT, GH, h->dz2, G + lb.ob + GH, h->scratch, h->scratch_elems));
+    RUN(gemm(h, s, H, GH, (int)BT, h->hp, 1, H, dzr, GH, 1, G + o.oU, GH, 0.f, h->scratch, h->scratch_elems));
+    RUN(colsum(s, BT, GH, h->dz, G + o.ob, h->scratch, h->scratch_elems));
+    if (gru) RUN(colsum(s, BT, GH, h->dz2, G + o.ob + GH, h->scratch, h->scratch_elems));
     if (l > 0 || dx_out)
-      RUN(gemm(h, s, (int)BT, I, GH, h->dz, GH, 1, P + lb.oW, 1, GH, l > 0 ? h->dy : dx_out, I, 0.f, nullptr, 0));
+      RUN(gemm(h, s, (int)BT, I, GH, h->dz, GH, 1, P + o.oW, 1, GH, l > 0 ? h->dy : dx_out, I, 0.f, nullptr, 0));
     h->prof.end(LFMQ_REGION_WGRAD, s);
   }
   return 0;
 }
 
-// optimizer update with the clip scale already in the gradient tail (tail[3]) + the MaxNorm kernel constraint
+// optimizer update with the clip scale already in the gradient tail (LFMQ_TAIL_CLIP_SCALE) + the MaxNorm kernel
+// constraint
 int apply_update(lfmq_handle h, float lr, int64_t iteration, cudaStream_t s) {
   const lfmq_config& c = h->cfg;
   float* tail = h->grads + h->n_train;
@@ -467,10 +469,10 @@ int apply_update(lfmq_handle h, float lr, int64_t iteration, cudaStream_t s) {
     lr_eff = (float)((double)lr * sqrt(1.0 - pow(0.999, t)) / (1.0 - pow(0.9, t)));
   }
   RUN(opt_update(s, c.optimizer, h->n_train, h->params, h->grads, h->slots,
-                 h->n_slots > 1 ? h->slots + h->n_train : nullptr, tail + 2, lr_eff, 0.f, 0.f, c.sgd_momentum));
-  for (int l = 0; l < c.num_layers; ++l)
-    RUN(maxnorm_cols(s, h->layers[l].I, (c.rnn_cell == LFMQ_CELL_GRU ? 3 : 4) * c.num_hidden, h->params + h->layers[l].oW,
-                     c.max_norm));
+                 h->n_slots > 1 ? h->slots + h->n_train : nullptr, tail + LFMQ_TAIL_GRAD_NORM, lr_eff, 0.f, 0.f,
+                 c.sgd_momentum));
+  for (const lfmq::ParamLayout::Layer& o : h->pl.layers)
+    RUN(maxnorm_cols(s, o.I, (c.rnn_cell == LFMQ_CELL_GRU ? 3 : 4) * c.num_hidden, h->params + o.oW, c.max_norm));
   h->tc.weights_dirty = 1;
   return 0;
 }
@@ -531,7 +533,7 @@ int stages_loss_uq(const lfmq_handle* st, int S, const float* const* y, const fl
   lfmq::ChainUqArgs a{};
   for (int i = 0; i < S; ++i) {
     a.y.p[i] = const_cast<float*>(y[i]);
-    a.counts.p[i] = denom ? const_cast<float*>(denom) + 3 * i : st[i]->denom;
+    a.counts.p[i] = denom ? const_cast<float*>(denom) + 3 * i : st[i]->sc->denom;
     a.w.w[i] = weights[i];
   }
   float* scratch = st[0]->scratch;
@@ -542,10 +544,10 @@ int stages_loss_uq(const lfmq_handle* st, int S, const float* const* y, const fl
     a.apre.p[i] = st[i]->apre;
     a.dpred.p[i] = st[i]->dpred;
     a.da.p[i] = st[i]->da;
-    float* tail = st[i]->grads + st[i]->n_train;     // the stage's own {uq_loss, mse_0, .., .., uq_loss_last_tar}
-    a.loss.p[i] = tail;
-    a.mse0.p[i] = tail + 1;
-    a.uq0.p[i] = tail + 4;
+    float* tail = st[i]->grads + st[i]->n_train;
+    a.loss.p[i] = tail + LFMQ_TAIL_LOSS;
+    a.mse0.p[i] = tail + LFMQ_TAIL_MSE0;
+    a.uq0.p[i] = tail + LFMQ_TAIL_UQ_LOSS_LAST_TAR;
   }
   a.counts_in = 1;
   return chain_uq_loss_grad(s, S, B, T, O, a, c0.target_idx, c0.target_lambda, c0.rnn_lambda, loss_out_dev, scratch);
@@ -568,8 +570,8 @@ int backward_stages(const lfmq_handle* st, int S, const float* x, const float* c
   for (int i = 0; i < S && !c0.uq; ++i) {
     lfmq_handle h = st[i];
     const lfmq_config& c = h->cfg;
-    const float* d = denom ? denom + 3 * i : h->denom;
-    if (!denom) RUN(mask_count(s, B, T, O, y[i], h->denom, h->tickets));
+    const float* d = denom ? denom + 3 * i : h->sc->denom;
+    if (!denom) RUN(mask_count(s, B, T, O, y[i], h->sc->denom, h->sc->mask_tickets));
     float* tail = h->grads + h->n_train;
     RUN(loss_grad(s, B, T, O, h->preds, y[i], d, c.target_idx, c.target_lambda, c.rnn_lambda, h->dpred, tail, nullptr,
                   h->scratch));
@@ -599,80 +601,6 @@ const char* lfmq_last_error(void) { return lfmq::g_err; }
 int32_t lfmq_abi_version(void) { return LFMQ_ABI_VERSION; }
 int64_t lfmq_launch_count(void) { return lfmq::g_launches; }
 
-int32_t lfmq_workspace_bytes(const lfmq_config* cfg, uint64_t* bytes) {
-  RUN(validate(cfg));
-  if (!bytes) {
-    LFMQ_SET_ERR("bytes == NULL");
-    return LFMQ_ERR_ARG;
-  }
-  lfmq_handle_s tmp;
-  tmp.cfg = *cfg;
-  *bytes = layout(&tmp, nullptr) + WS_ALIGN;
-  lfmq::tc_destroy(tmp.tc);
-  lfmq::gen_destroy(tmp.tc);
-  return LFMQ_OK;
-}
-
-int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_bytes, lfmq_handle* out) {
-  RUN(validate(cfg));
-  if (!workspace || !out) {
-    LFMQ_SET_ERR("workspace/out == NULL");
-    return LFMQ_ERR_ARG;
-  }
-  lfmq_handle_s* h = new lfmq_handle_s;
-  h->cfg = *cfg;
-  char* base = reinterpret_cast<char*>(ws_align_up(reinterpret_cast<size_t>(workspace)));
-  const size_t need = layout(h, nullptr) + (base - reinterpret_cast<char*>(workspace));
-  if (need > workspace_bytes) {
-    LFMQ_SET_ERR("workspace too small: need %zu bytes, got %llu", need, (unsigned long long)workspace_bytes);
-    delete h;
-    return LFMQ_ERR_WORKSPACE;
-  }
-  layout(h, base);
-  h->tc.prof = &h->prof;
-  int rc = 0;
-  if (h->use_gen) {
-    char why[160];
-    if (!lfmq::gen_supported(h->cfg, why, sizeof(why))) {
-      LFMQ_SET_ERR("tensor-core precision unsupported for this configuration: %s; use LFMQ_PREC_FP32", why);
-      rc = LFMQ_ERR_UNSUPPORTED;
-    } else {
-      rc = lfmq::gen_init(h->tc, h->cfg);
-    }
-  } else {
-    rc = lfmq::tc_init(h->tc, h->cfg);
-  }
-  if (rc != 0) {
-    delete h;
-    return rc;
-  }
-  // zero parameters / gradients / optimizer slots; BN moving_variance = 1
-  cudaError_t e = cudaMemsetAsync(h->params, 0, sizeof(float) * h->n_total, 0);
-  if (e == cudaSuccess) e = cudaMemsetAsync(h->grads, 0, sizeof(float) * h->n_grad_buf, 0);
-  if (e == cudaSuccess && h->slots) e = cudaMemsetAsync(h->slots, 0, sizeof(float) * h->n_slots * h->n_train, 0);
-  if (e == cudaSuccess) e = cudaMemsetAsync(h->scalars, 0, sizeof(float) * 16, 0);
-  if (e != cudaSuccess) {
-    LFMQ_SET_ERR("lfmq_create: memset failed: %s", cudaGetErrorString(e));
-    delete h;
-    return LFMQ_ERR_CUDA;
-  }
-  for (int l = 0; l < cfg->num_layers; ++l) {
-    rc = lfmq::fill(0, h->params + h->layers[l].ovar, cfg->num_hidden, 1.0f);
-    if (rc) {
-      delete h;
-      return rc;
-    }
-  }
-  e = cudaStreamSynchronize(0);
-  if (e != cudaSuccess) {
-    LFMQ_SET_ERR("lfmq_create: %s", cudaGetErrorString(e));
-    delete h;
-    return LFMQ_ERR_CUDA;
-  }
-  *out = h;
-  return LFMQ_OK;
-}
-
 namespace {
 void dense_handle_config(const lfmq_dense_config* d, lfmq_handle_s* h) {
   lfmq_config& c = h->cfg;
@@ -689,67 +617,85 @@ void dense_handle_config(const lfmq_dense_config* d, lfmq_handle_s* h) {
   c.target_lambda = d->target_lambda;
   c.max_grad_norm = d->max_grad_norm;
   c.sgd_momentum = d->sgd_momentum;
-  h->dense = 1;
+  h->path = Path::Dense;
   h->huber = d->huber_loss ? 1 : 0;
   h->huber_delta = d->huber_delta;
 }
-}  // namespace
 
-int32_t lfmq_dense_workspace_bytes(const lfmq_dense_config* cfg, uint64_t* bytes) {
-  RUN(validate_dense(cfg));
+// The body of lfmq_workspace_bytes and lfmq_dense_workspace_bytes
+int32_t workspace_bytes_of(lfmq_handle_s& h, bool with_path, uint64_t* bytes) {
   if (!bytes) {
     LFMQ_SET_ERR("bytes == NULL");
     return LFMQ_ERR_ARG;
   }
-  lfmq_handle_s tmp;
-  dense_handle_config(cfg, &tmp);
-  *bytes = dense_layout(&tmp, nullptr) + WS_ALIGN;
+  *bytes = layout(&h, nullptr, with_path) + WS_ALIGN;
   return LFMQ_OK;
 }
 
-int32_t lfmq_dense_create(const lfmq_dense_config* cfg, void* workspace, uint64_t workspace_bytes, lfmq_handle* out) {
-  RUN(validate_dense(cfg));
+// The body of lfmq_create and lfmq_dense_create.  h carries its config and path; path_rc is choose_path's result (its
+// message still in g_err), reported once the workspace is large enough for what lfmq_workspace_bytes sized.
+int32_t create(std::unique_ptr<lfmq_handle_s> h, int path_rc, void* workspace, uint64_t workspace_bytes,
+               lfmq_handle* out) {
   if (!workspace || !out) {
     LFMQ_SET_ERR("workspace/out == NULL");
     return LFMQ_ERR_ARG;
   }
-  lfmq_handle_s* h = new lfmq_handle_s;
-  dense_handle_config(cfg, h);
   char* base = reinterpret_cast<char*>(ws_align_up(reinterpret_cast<size_t>(workspace)));
-  const size_t need = dense_layout(h, nullptr) + (base - reinterpret_cast<char*>(workspace));
+  const size_t need = layout(h.get(), nullptr, path_rc == 0) + (base - reinterpret_cast<char*>(workspace));
   if (need > workspace_bytes) {
     LFMQ_SET_ERR("workspace too small: need %zu bytes, got %llu", need, (unsigned long long)workspace_bytes);
-    delete h;
     return LFMQ_ERR_WORKSPACE;
   }
-  dense_layout(h, base);
+  RUN(path_rc);
+  layout(h.get(), base, true);
   h->tc.prof = &h->prof;
-  cudaError_t e = cudaMemsetAsync(h->params, 0, sizeof(float) * h->n_total, 0);
-  if (e == cudaSuccess) e = cudaMemsetAsync(h->grads, 0, sizeof(float) * h->n_grad_buf, 0);
-  if (e == cudaSuccess && h->slots) e = cudaMemsetAsync(h->slots, 0, sizeof(float) * h->n_slots * h->n_train, 0);
-  if (e == cudaSuccess) e = cudaMemsetAsync(h->scalars, 0, sizeof(float) * 16, 0);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-  if (e != cudaSuccess) {
-    LFMQ_SET_ERR("lfmq_dense_create: %s", cudaGetErrorString(e));
-    delete h;
-    return LFMQ_ERR_CUDA;
-  }
-  *out = h;
+  if (h->path == Path::Cluster) RUN(lfmq::tc_init(h->tc, h->cfg));
+  if (h->path == Path::General) RUN(lfmq::gen_init(h->tc, h->cfg));
+  // zero parameters / gradients / optimizer slots / scalars; BN moving_variance = 1
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(h->params, 0, sizeof(float) * h->n_total, 0));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(h->grads, 0, sizeof(float) * h->n_grad_buf, 0));
+  if (h->slots) LFMQ_CUDA_CHECK(cudaMemsetAsync(h->slots, 0, sizeof(float) * h->n_slots * h->n_train, 0));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(h->sc, 0, sizeof(Scalars), 0));
+  for (const lfmq::ParamLayout::Layer& o : h->pl.layers)
+    RUN(lfmq::fill(0, h->params + o.ovar, h->cfg.num_hidden, 1.0f));
+  LFMQ_CUDA_CHECK(cudaStreamSynchronize(0));
+  *out = h.release();
   return LFMQ_OK;
+}
+}  // namespace
+
+int32_t lfmq_workspace_bytes(const lfmq_config* cfg, uint64_t* bytes) {
+  RUN(validate(cfg));
+  lfmq_handle_s h;
+  h.cfg = *cfg;
+  const bool supported = choose_path(h.cfg, &h.path) == 0;     // lfmq_create reports an unsupported configuration
+  return workspace_bytes_of(h, supported, bytes);
+}
+
+int32_t lfmq_create(const lfmq_config* cfg, void* workspace, uint64_t workspace_bytes, lfmq_handle* out) {
+  RUN(validate(cfg));
+  auto h = std::make_unique<lfmq_handle_s>();
+  h->cfg = *cfg;
+  const int path_rc = choose_path(h->cfg, &h->path);
+  return create(std::move(h), path_rc, workspace, workspace_bytes, out);
+}
+
+int32_t lfmq_dense_workspace_bytes(const lfmq_dense_config* cfg, uint64_t* bytes) {
+  RUN(validate_dense(cfg));
+  lfmq_handle_s h;
+  dense_handle_config(cfg, &h);
+  return workspace_bytes_of(h, true, bytes);
+}
+
+int32_t lfmq_dense_create(const lfmq_dense_config* cfg, void* workspace, uint64_t workspace_bytes, lfmq_handle* out) {
+  RUN(validate_dense(cfg));
+  auto h = std::make_unique<lfmq_handle_s>();
+  dense_handle_config(cfg, h.get());
+  return create(std::move(h), 0, workspace, workspace_bytes, out);
 }
 
 int32_t lfmq_destroy(lfmq_handle h) {
-  if (h) {
-    lfmq::tc_destroy(h->tc);
-    lfmq::gen_destroy(h->tc);
-    if (h->prof.created)
-      for (int r = 0; r < Profiler::kRegions; ++r)
-        for (int i = 0; i < Profiler::kCap; ++i) {
-          cudaEventDestroy(h->prof.a[r][i]);
-          cudaEventDestroy(h->prof.b[r][i]);
-        }
-    delete h;
-  }
+  delete h;
   return LFMQ_OK;
 }
 
@@ -856,17 +802,21 @@ int32_t lfmq_forward(lfmq_handle h, const float* x, int32_t B, int64_t row0, int
     LFMQ_SET_ERR("lfmq_forward: uq handle, call lfmq_forward_uq");
     return LFMQ_ERR_ARG;
   }
-  if (h->dense) {
-    const lfmq_config& c = h->cfg;
-    h->prof.begin(LFMQ_REGION_FWD, s);
-    RUN(dense_forward(s, x, B, c.seq_len * c.n_inputs, c.n_outputs, h->params + h->oWo, h->params + h->obo, preds));
-    h->prof.end(LFMQ_REGION_FWD, s);
-    return LFMQ_OK;
+  const lfmq_config& c = h->cfg;
+  switch (h->path) {
+    case Path::Fp32:
+      return forward_fp32(h, x, B, row0, step, preds, nullptr, s);
+    case Path::Cluster:
+      return lfmq::tc_forward(h->tc, c, h->pl, h->params, x, B, row0, step, preds, /*save=*/false, s);
+    case Path::General:
+      return lfmq::gen_forward(h->tc, c, h->pl, h->params, x, B, row0, step, preds, s);
+    case Path::Dense:
+      break;
   }
-  if (h->use_gen) return lfmq::gen_forward(h->tc, h->cfg, h->params, x, B, row0, step, preds, s);
-  if (h->cfg.precision == LFMQ_PREC_BF16)
-    return lfmq::tc_forward(h->tc, h->cfg, h->params, x, B, row0, step, preds, /*save=*/false, s);
-  return forward_fp32(h, x, B, row0, step, preds, nullptr, s);
+  h->prof.begin(LFMQ_REGION_FWD, s);
+  RUN(dense_forward(s, x, B, c.seq_len * c.n_inputs, c.n_outputs, h->params + h->pl.oWo, h->params + h->pl.obo, preds));
+  h->prof.end(LFMQ_REGION_FWD, s);
+  return LFMQ_OK;
 }
 
 int32_t lfmq_forward_uq(lfmq_handle h, const float* x, int32_t B, int64_t row0, int64_t step, float* preds, float* var,
@@ -882,7 +832,8 @@ int32_t lfmq_forward_uq(lfmq_handle h, const float* x, int32_t B, int64_t row0, 
   }
   h->last_step = step;
   h->last_row0 = row0;
-  if (h->use_gen) return lfmq::gen_forward_uq(h->tc, h->cfg, h->params, x, B, row0, step, preds, var, (cudaStream_t)stream);
+  if (h->path == Path::General)      // a uq handle runs the fp32 step or the general path
+    return lfmq::gen_forward_uq(h->tc, h->cfg, h->pl, h->params, x, B, row0, step, preds, var, (cudaStream_t)stream);
   return forward_fp32(h, x, B, row0, step, preds, var, (cudaStream_t)stream);
 }
 
@@ -897,7 +848,7 @@ int32_t lfmq_loss(lfmq_handle h, const float* preds, const float* y, int32_t B, 
     return LFMQ_ERR_ARG;
   }
   const lfmq_config& c = h->cfg;
-  if (h->dense)      // validation: the MSE form whatever huber_loss is (losses.py:102, is_validation=True)
+  if (h->path == Path::Dense)    // validation: the MSE form whatever huber_loss is (losses.py:102, is_validation=True)
     return dense_loss((cudaStream_t)stream, preds, y, B, c.n_outputs, nullptr, c.target_idx, c.target_lambda, 0, 1.f,
                       nullptr, out_dev, h->scratch);
   return loss_grad((cudaStream_t)stream, B, c.seq_len, c.n_outputs, preds, y, nullptr, c.target_idx, c.target_lambda,
@@ -927,10 +878,10 @@ int32_t lfmq_mask_count(lfmq_handle h, const float* y, int32_t B, float* out_dev
     LFMQ_SET_ERR("lfmq_mask_count: null pointer");
     return LFMQ_ERR_ARG;
   }
-  if (h->dense)
+  if (h->path == Path::Dense)
     return dense_loss((cudaStream_t)stream, nullptr, y, B, h->cfg.n_outputs, nullptr, 0, 0.f, 0, 1.f, nullptr, out_dev,
                       h->scratch);
-  return mask_count((cudaStream_t)stream, B, h->cfg.seq_len, h->cfg.n_outputs, y, out_dev, h->tickets);
+  return mask_count((cudaStream_t)stream, B, h->cfg.seq_len, h->cfg.n_outputs, y, out_dev, h->sc->mask_tickets);
 }
 
 int32_t lfmq_mask_count_uq(lfmq_handle h, const float* y, int32_t B, float* out_dev, void* stream) {
@@ -956,34 +907,40 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
   }
   cudaStream_t s = (cudaStream_t)stream;
   const lfmq_config& c = h->cfg;
-  if (h->dense) {    // the forward into the handle's own preds, the loss and dLoss/dpred, then dW and db
-    const int K = c.seq_len * c.n_inputs, O = c.n_outputs;
-    float* tail = h->grads + h->n_train;
-    h->prof.begin(LFMQ_REGION_FWD, s);
-    RUN(dense_forward(s, x, B, K, O, h->params + h->oWo, h->params + h->obo, h->preds));
-    h->prof.end(LFMQ_REGION_FWD, s);
-    h->prof.begin(LFMQ_REGION_HEAD, s);
-    RUN(dense_loss(s, h->preds, y, B, O, denom_dev, c.target_idx, c.target_lambda, h->huber, h->huber_delta, h->dpred,
-                   tail, h->scratch));
-    h->prof.end(LFMQ_REGION_HEAD, s);
-    h->prof.begin(LFMQ_REGION_WGRAD, s);
-    RUN(dense_wgrad(s, x, h->dpred, B, K, O, h->wpart, h->grads));
-    h->prof.end(LFMQ_REGION_WGRAD, s);
-    return LFMQ_OK;
-  }
-  if (c.precision == LFMQ_PREC_FP32 || c.precision == LFMQ_PREC_TF32) {   // a trainable uq handle is always one of these
-    // denom_dev: stage 0's counts, the three of lfmq_mask_count_uq or the two of lfmq_mask_count
-    const float one = 1.0f;
-    return backward_stages(&h, 1, x, &y, &one, B, row0, step, denom_dev, nullptr, nullptr, s);
-  }
-  const float* denom = denom_dev;
-  if (!denom) {
-    RUN(mask_count(s, B, c.seq_len, c.n_outputs, y, h->denom, h->tickets));
-    denom = h->denom;
-  }
   float* tail = h->grads + h->n_train;
-  if (h->use_gen) return lfmq::gen_backward(h->tc, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
-  return lfmq::tc_backward(h->tc, c, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
+  switch (h->path) {
+    case Path::Fp32: {    // a trainable uq handle always runs this path
+      // denom_dev: stage 0's counts, the three of lfmq_mask_count_uq or the two of lfmq_mask_count
+      const float one = 1.0f;
+      return backward_stages(&h, 1, x, &y, &one, B, row0, step, denom_dev, nullptr, nullptr, s);
+    }
+    case Path::Cluster:
+    case Path::General: {
+      const float* denom = denom_dev;
+      if (!denom) {
+        RUN(mask_count(s, B, c.seq_len, c.n_outputs, y, h->sc->denom, h->sc->mask_tickets));
+        denom = h->sc->denom;
+      }
+      if (h->path == Path::Cluster)
+        return lfmq::tc_backward(h->tc, c, h->pl, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
+      return lfmq::gen_backward(h->tc, c, h->pl, h->params, h->grads, x, y, B, row0, step, denom, tail, s);
+    }
+    case Path::Dense:
+      break;
+  }
+  // the dense model: the forward into the handle's own preds, the loss and dLoss/dpred, then dW and db
+  const int K = c.seq_len * c.n_inputs, O = c.n_outputs;
+  h->prof.begin(LFMQ_REGION_FWD, s);
+  RUN(dense_forward(s, x, B, K, O, h->params + h->pl.oWo, h->params + h->pl.obo, h->preds));
+  h->prof.end(LFMQ_REGION_FWD, s);
+  h->prof.begin(LFMQ_REGION_HEAD, s);
+  RUN(dense_loss(s, h->preds, y, B, O, denom_dev, c.target_idx, c.target_lambda, h->huber, h->huber_delta, h->dpred,
+                 tail, h->scratch));
+  h->prof.end(LFMQ_REGION_HEAD, s);
+  h->prof.begin(LFMQ_REGION_WGRAD, s);
+  RUN(dense_wgrad(s, x, h->dpred, B, K, O, h->wpart, h->grads));
+  h->prof.end(LFMQ_REGION_WGRAD, s);
+  return LFMQ_OK;
 }
 
 int32_t lfmq_apply(lfmq_handle h, float lr, int64_t iteration, void* stream) {
@@ -995,7 +952,8 @@ int32_t lfmq_apply(lfmq_handle h, float lr, int64_t iteration, void* stream) {
   const lfmq_config& c = h->cfg;
   float* tail = h->grads + h->n_train;
   h->prof.begin(LFMQ_REGION_OPT, s);
-  RUN(grad_norm_scale(s, h->n_train, h->grads, c.max_grad_norm, tail + 2, h->scratch, h->tickets + 2));
+  RUN(grad_norm_scale(s, h->n_train, h->grads, c.max_grad_norm, tail + LFMQ_TAIL_GRAD_NORM, h->scratch,
+                      &h->sc->norm_ticket));
   RUN(apply_update(h, lr, iteration, s));
   h->prof.end(LFMQ_REGION_OPT, s);
   return LFMQ_OK;
@@ -1005,13 +963,14 @@ int32_t lfmq_train_step(lfmq_handle h, const float* x, const float* y, int32_t B
                         float* loss_out_dev, void* stream) {
   RUN(lfmq_backward(h, x, y, B, row0, step, nullptr, stream));
   RUN(lfmq_apply(h, lr, step, stream));
-  if (loss_out_dev && !h->cfg.uq)
-    LFMQ_CUDA_CHECK(cudaMemcpyAsync(loss_out_dev, h->grads + h->n_train, 2 * sizeof(float), cudaMemcpyDeviceToDevice,
+  const float* tail = h->grads + h->n_train;
+  if (loss_out_dev && !h->cfg.uq)      // {loss, mse_0}
+    LFMQ_CUDA_CHECK(cudaMemcpyAsync(loss_out_dev, tail + LFMQ_TAIL_LOSS, 2 * sizeof(float), cudaMemcpyDeviceToDevice,
                                     (cudaStream_t)stream));
   if (loss_out_dev && h->cfg.uq) {      // {uq_loss_last_tar, mse_0}
-    LFMQ_CUDA_CHECK(cudaMemcpyAsync(loss_out_dev, h->grads + h->n_train + 4, sizeof(float), cudaMemcpyDeviceToDevice,
-                                    (cudaStream_t)stream));
-    LFMQ_CUDA_CHECK(cudaMemcpyAsync(loss_out_dev + 1, h->grads + h->n_train + 1, sizeof(float), cudaMemcpyDeviceToDevice,
+    LFMQ_CUDA_CHECK(cudaMemcpyAsync(loss_out_dev, tail + LFMQ_TAIL_UQ_LOSS_LAST_TAR, sizeof(float),
+                                    cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    LFMQ_CUDA_CHECK(cudaMemcpyAsync(loss_out_dev + 1, tail + LFMQ_TAIL_MSE0, sizeof(float), cudaMemcpyDeviceToDevice,
                                     (cudaStream_t)stream));
   }
   return LFMQ_OK;
@@ -1037,7 +996,7 @@ int chain_check(const lfmq_handle* st, int32_t S, int32_t B, bool training) {
       LFMQ_SET_ERR("lfmq_chain: stage %d does not continue stage 0 (same T/F/O, one layer, same uq flag)", i);
       return LFMQ_ERR_ARG;
     }
-    if ((training || c.train) && c.precision != LFMQ_PREC_FP32 && c.precision != LFMQ_PREC_TF32) {
+    if ((training || c.train) && st[i]->path != Path::Fp32) {
       LFMQ_SET_ERR("lfmq_chain: training-mode stages run on the fp32 or tf32 kernels (stage %d has precision %d)", i,
                    c.precision);
       return LFMQ_ERR_UNSUPPORTED;
@@ -1103,7 +1062,7 @@ int mc_check(const lfmq_handle* st, int32_t S, int32_t B, int32_t samples, const
   }
   int mb = 0;
   for (int i = 0; i < S; ++i) {
-    if (!st[i] || st[i]->dense || !st[i]->cfg.uq) {
+    if (!st[i] || !st[i]->cfg.uq) {
       LFMQ_SET_ERR("%s: stage %d is not a uq handle: only RNNUqRangeEstimate keeps dropout on at prediction time, a "
                    "point-estimate model would give the same prediction for every sample", fn, i);
       return LFMQ_ERR_ARG;
@@ -1240,7 +1199,7 @@ int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float
       return LFMQ_ERR_ARG;
     }
     RUN(refuse_dense(stages[i], "lfmq_chain_loss"));
-    l2.p[i] = stages[i]->scalars + 12;      // two spare floats of the handle's scalar block (denom uses 8..10)
+    l2.p[i] = stages[i]->sc->chain_loss;
     RUN(lfmq_loss(stages[i], preds[i], y[i], B, l2.p[i], stream));
     w.w[i] = weights[i];
   }
@@ -1257,7 +1216,7 @@ int32_t lfmq_chain_loss_uq(const lfmq_handle* stages, int32_t n_stages, const fl
   }
   lfmq::ChainUqArgs a{};
   for (int i = 0; i < n_stages; ++i) {
-    if (!stages[i] || !stages[i]->cfg.uq || stages[i]->dense || !preds[i] || !vars[i] || !y[i]) {
+    if (!stages[i] || !stages[i]->cfg.uq || !preds[i] || !vars[i] || !y[i]) {
       LFMQ_SET_ERR("lfmq_chain_loss_uq: stage %d: null pointer or a point-estimate handle", i);
       return LFMQ_ERR_ARG;
     }
@@ -1297,7 +1256,7 @@ int pack_check(const lfmq_handle* st, int32_t S, const char* fn, lfmq::GradPack*
   }
   int64_t off = 0;
   for (int i = 0; i < S; ++i) {
-    if (!st[i] || st[i]->cfg.forward_only || st[i]->cfg.uq != st[0]->cfg.uq || st[i]->dense) {
+    if (!st[i] || st[i]->cfg.forward_only || st[i]->cfg.uq != st[0]->cfg.uq || st[i]->path == Path::Dense) {
       LFMQ_SET_ERR("%s: stage %d is null, forward_only, a dense handle or of another kind than stage 0", fn, i);
       return LFMQ_ERR_ARG;
     }
@@ -1390,13 +1349,13 @@ int32_t lfmq_chain_apply(const lfmq_handle* stages, int32_t n_stages, float lr, 
   lfmq::ChainWeights w{};
   for (int i = 0; i < n_stages; ++i) {
     lfmq_handle h = stages[i];
-    if (!h || h->cfg.forward_only || h->dense) {
+    if (!h || h->cfg.forward_only || h->path == Path::Dense) {
       LFMQ_SET_ERR("lfmq_chain_apply: bad handle (null, forward_only or dense)");
       return LFMQ_ERR_ARG;
     }
     float* tail = h->grads + h->n_train;
-    RUN(grad_norm_scale(s, h->n_train, h->grads, 0.f, tail + 2, h->scratch, h->tickets + 2));   // tail[2] = ||g_stage||
-    sc.p[i] = tail + 2;
+    RUN(grad_norm_scale(s, h->n_train, h->grads, 0.f, tail + LFMQ_TAIL_GRAD_NORM, h->scratch, &h->sc->norm_ticket));
+    sc.p[i] = tail + LFMQ_TAIL_GRAD_NORM;     // ||g_stage||
   }
   // tf.clip_by_global_norm over all stages' variables (train.py:196)
   RUN(chain_combine(s, n_stages, sc, stages[0]->cfg.max_grad_norm, none, w, nullptr));

@@ -55,11 +55,8 @@ constexpr int TC_OPAD = 16;        // head handles n_outputs <= 16
 }  // namespace
 
 struct TcImpl {
-  bool enabled = false;
   int maxB = 0, T = 0, I = 0, O = 0;
   float eps = 1e-3f;
-  // parameter offsets in the flat fp32 vector (L = 1)
-  int64_t oW, oU, ob, ogamma, obeta, oWo, obo, omean, ovar;
   // workspace
   bool train = false;                          // training handle: saved state and the backward recurrence exist
   // c.train && dropout > 0: the head runs as the SIMT dropout head (head_rows_kernel, head_wgrad_kernel), which hands
@@ -1480,7 +1477,7 @@ __global__ void wgrad_reduce_kernel(int S, int I, const float* __restrict__ part
 // =============================================================================================
 // Host side
 // =============================================================================================
-static bool tc_supported(const lfmq_config& c, char* why, size_t n) {
+bool tc_supported(const lfmq_config& c, char* why, size_t n) {
   if (c.rnn_cell != LFMQ_CELL_LSTM) { snprintf(why, n, "the bf16 tensor-core path is built for the LSTM cell only"); return false; }
   if (c.uq) { snprintf(why, n, "the bf16 tensor-core path is built for the point-estimate head only"); return false; }
   if (c.num_hidden != TC_H) { snprintf(why, n, "num_hidden must be 256 (got %d)", c.num_hidden); return false; }
@@ -1491,15 +1488,7 @@ static bool tc_supported(const lfmq_config& c, char* why, size_t n) {
   return true;
 }
 
-bool tc_shape_supported(const lfmq_config& c) {
-  char why[128];
-  return tc_supported(c, why, sizeof(why));
-}
-
-void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& cv) {
-  if (c.precision != LFMQ_PREC_BF16) return;
-  char why[128];
-  if (!tc_supported(c, why, sizeof(why))) return;   // tc_init reports the error
+void tc_layout(TcState& st, const lfmq_config& c, Carver& cv) {
   if (!st.impl) st.impl = new TcImpl;
   TcImpl& m = *st.impl;
   const size_t B = (size_t)c.max_batch, T = (size_t)c.seq_len, H = TC_H;
@@ -1539,9 +1528,6 @@ void tc_layout(TcState& st, const lfmq_config& c, const TcParamOff& po, Carver& 
     m.dpred = nullptr; m.head_wpart = nullptr; m.dpb = nullptr;
     m.wg_part_elems = 0;
   }
-  // offsets of the tensors in the flat parameter vector: the API layer's layout() is the one place that defines them
-  m.oW = po.oW; m.oU = po.oU; m.ob = po.ob; m.ogamma = po.ogamma; m.obeta = po.obeta;
-  m.oWo = po.oWo; m.obo = po.obo; m.omean = po.omean; m.ovar = po.ovar;
 }
 
 // The instantiations of the two recurrences, [flag][i]: flag = SAVE / FUSED, i = 0 for 128-row tiles and 1 for 64-row
@@ -1580,12 +1566,6 @@ static int tc_cluster_setup(Kernel const (&kernels)[2][2], int threads, int smem
 }
 
 int tc_init(TcState& st, const lfmq_config& c) {
-  if (c.precision != LFMQ_PREC_BF16) return 0;
-  char why[128];
-  if (!tc_supported(c, why, sizeof(why))) {
-    LFMQ_SET_ERR("LFMQ_PREC_BF16 supports the H=256 single-layer forecaster only: %s; use LFMQ_PREC_FP32", why);
-    return LFMQ_ERR_UNSUPPORTED;
-  }
   TcImpl& m = *st.impl;
   const size_t B = (size_t)m.maxB, T = (size_t)m.T;
   LFMQ_CUDA_CHECK(cudaMemset(m.xh, 0, B * (T + 1) * TC_XH_LD * 2));
@@ -1619,7 +1599,6 @@ int tc_init(TcState& st, const lfmq_config& c) {
   // LFMQ_TC_HALF_TILES=0 keeps every round at 128-row tiles (A/B measurements, tests comparing the two schedules)
   const char* ht = getenv("LFMQ_TC_HALF_TILES");
   m.half_tiles = !(ht != nullptr && atoi(ht) == 0);
-  m.enabled = true;
   st.weights_dirty = 1;
   return 0;
 }
@@ -1629,8 +1608,9 @@ void tc_destroy(TcState& st) {
   st.impl = nullptr;
 }
 
-static int tc_pack_weights(TcState& st, const float* params, cudaStream_t s) {
+static int tc_pack_weights(TcState& st, const ParamLayout& pl, const float* params, cudaStream_t s) {
   TcImpl& m = *st.impl;
+  const ParamLayout::Layer& o = pl.layers[0];
   if (!st.weights_dirty) return 0;
   const int nblk = (int)(((long)4 * TC_H * TC_H + 255) / 256);
   PackArgs a;
@@ -1638,9 +1618,9 @@ static int tc_pack_weights(TcState& st, const float* params, cudaStream_t s) {
   a.nb_w = nblk;
   a.nb_h = (TC_H * 32 + 255) / 256;
   a.nb_u = m.train ? nblk : 0;      // K-slices of U for the backward recurrence
-  a.W = params + m.oW; a.U = params + m.oU; a.bias = params + m.ob;
-  a.Wo = params + m.oWo; a.bo = params + m.obo; a.gamma = params + m.ogamma; a.beta = params + m.obeta;
-  a.mean = params + m.omean; a.var = params + m.ovar;
+  a.W = params + o.oW; a.U = params + o.oU; a.bias = params + o.ob;
+  a.Wo = params + pl.oWo; a.bo = params + pl.obo; a.gamma = params + o.ogamma; a.beta = params + o.obeta;
+  a.mean = params + o.omean; a.var = params + o.ovar;
   a.Up = m.Up; a.Wp = m.Wp; a.Ubk = m.Ubk; a.WoTp = m.WoTp; a.WoSp = m.WoSp; a.biasp = m.biasp; a.bop = m.bop;
   if (int rc = launch_pdl(pack_all_kernel, dim3(a.nb_w + a.nb_h + a.nb_u), dim3(256), 0, s, 1, true, a)) return rc;
   st.weights_dirty = 0;
@@ -1714,16 +1694,17 @@ static int tc_run_recurrence(TcState& st, const float* x, int B, bool save, cuda
   return tc_run_rounds(m, p, save, s);
 }
 
-static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* y, int B,
-                       int64_t row0, int64_t step, const float* denom, float* preds, float* out2, bool train,
-                       cudaStream_t s) {
+static int tc_run_head(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, float* grads,
+                       const float* y, int B, int64_t row0, int64_t step, const float* denom, float* preds, float* out2,
+                       bool train, cudaStream_t s) {
   TcImpl& m = *st.impl;
+  const ParamLayout::Layer& o = pl.layers[0];
   HeadParams h;
   h.B = B; h.T = m.T; h.O = m.O; h.target_idx = c.target_idx;
   h.xh = m.xh;
-  h.gamma = params + m.ogamma; h.beta = params + m.obeta; h.mean = params + m.omean; h.var = params + m.ovar;
+  h.gamma = params + o.ogamma; h.beta = params + o.obeta; h.mean = params + o.omean; h.var = params + o.ovar;
   h.eps = c.bn_epsilon;
-  h.Wo = params + m.oWo; h.bo = params + m.obo;
+  h.Wo = params + pl.oWo; h.bo = params + pl.obo;
   h.y = y; h.denom = denom; h.p1 = c.target_lambda; h.p2 = c.rnn_lambda;
   h.use_dropout = m.dropout_head ? 1 : 0;
   h.key = dropout_key(c.seed, 0, step, c.dropout);
@@ -1767,54 +1748,49 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const float* params, f
     const int n_out = HWG_PART + HEAD_PART;
     if (int rc = launch_pdl(head_reduce_kernel, dim3((n_out * 32 + 255) / 256), dim3(256), 0, s, 1, true, grid,
                             (const float*)m.head_part, n_wcta, (const float*)m.head_wpart, m.O, B, denom, c.target_lambda,
-                            c.rnn_lambda, train ? 1 : 0, grads ? grads + m.oWo : (float*)nullptr,
-                            grads ? grads + m.obo : (float*)nullptr, grads ? grads + m.ogamma : (float*)nullptr,
-                            grads ? grads + m.obeta : (float*)nullptr, out2))
+                            c.rnn_lambda, train ? 1 : 0, grads ? grads + pl.oWo : (float*)nullptr,
+                            grads ? grads + pl.obo : (float*)nullptr, grads ? grads + o.ogamma : (float*)nullptr,
+                            grads ? grads + o.obeta : (float*)nullptr, out2))
       return rc;
     if (train && use_tc) {
-      if (int rc = launch_pdl(head_fold_kernel, dim3((TC_H + 127) / 128), dim3(128), 0, s, 1, true, m.O, grads + m.oWo,
-                              (const float*)(grads + m.obo), grads + m.ogamma, grads + m.obeta, params + m.oWo,
-                              params + m.ogamma, params + m.obeta, params + m.omean, params + m.ovar, c.bn_epsilon))
+      if (int rc = launch_pdl(head_fold_kernel, dim3((TC_H + 127) / 128), dim3(128), 0, s, 1, true, m.O, grads + pl.oWo,
+                              (const float*)(grads + pl.obo), grads + o.ogamma, grads + o.obeta, params + pl.oWo,
+                              params + o.ogamma, params + o.obeta, params + o.omean, params + o.ovar, c.bn_epsilon))
         return rc;
     }
   }
   return 0;
 }
 
-int tc_forward(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
-               int64_t step, float* preds, bool save, cudaStream_t s) {
-  if (!st.impl || !st.impl->enabled) {
-    LFMQ_SET_ERR("bf16 path not initialised");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
+int tc_forward(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, const float* x, int B,
+               int64_t row0, int64_t step, float* preds, bool save, cudaStream_t s) {
   int rc;
-  if ((rc = tc_pack_weights(st, params, s))) return rc;
+  if ((rc = tc_pack_weights(st, pl, params, s))) return rc;
   st.prof->begin(LFMQ_REGION_FWD, s);
   if ((rc = tc_run_recurrence(st, x, B, save, s))) return rc;
   st.prof->end(LFMQ_REGION_FWD, s);
   if (preds) {
     st.prof->begin(LFMQ_REGION_HEAD, s);
-    if ((rc = tc_run_head(st, c, params, nullptr, nullptr, B, row0, step, nullptr, preds, nullptr, false, s))) return rc;
+    if ((rc = tc_run_head(st, c, pl, params, nullptr, nullptr, B, row0, step, nullptr, preds, nullptr, false, s)))
+      return rc;
     st.prof->end(LFMQ_REGION_HEAD, s);
   }
   return 0;
 }
 
-int tc_backward(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* x, const float* y,
-                int B, int64_t row0, int64_t step, const float* denom, float* tail, cudaStream_t s) {
-  if (!st.impl || !st.impl->enabled) {
-    LFMQ_SET_ERR("bf16 path not initialised");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
+int tc_backward(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, float* grads,
+                const float* x, const float* y, int B, int64_t row0, int64_t step, const float* denom, float* tail,
+                cudaStream_t s) {
   TcImpl& m = *st.impl;
+  const ParamLayout::Layer& o = pl.layers[0];
   const size_t T = (size_t)m.T;
   int rc;
-  if ((rc = tc_pack_weights(st, params, s))) return rc;
+  if ((rc = tc_pack_weights(st, pl, params, s))) return rc;
   st.prof->begin(LFMQ_REGION_FWD, s);
   if ((rc = tc_run_recurrence(st, x, B, true, s))) return rc;
   st.prof->end(LFMQ_REGION_FWD, s);
   st.prof->begin(LFMQ_REGION_HEAD, s);
-  if ((rc = tc_run_head(st, c, params, grads, y, B, row0, step, denom, nullptr, tail, true, s))) return rc;
+  if ((rc = tc_run_head(st, c, pl, params, grads, y, B, row0, step, denom, nullptr, tail, true, s))) return rc;
   st.prof->end(LFMQ_REGION_HEAD, s);
 
   st.prof->begin(LFMQ_REGION_BWD, s);
@@ -1845,7 +1821,7 @@ int tc_backward(TcState& st, const lfmq_config& c, const float* params, float* g
   if ((rc = wgrad_gemm(tm_a, tm_b, (long)rows, TC_XH_LD, 4 * TC_H, m.wg_part, m.wg_part_elems, true, s, &S, &Mpad)))
     return rc;
   if ((rc = launch_pdl(wgrad_reduce_kernel, dim3((384 * 1024 + 255) / 256), dim3(256), 0, s, 1, true, S, m.I,
-                       (const float*)m.wg_part, grads + m.oU, grads + m.oW, grads + m.ob)))
+                       (const float*)m.wg_part, grads + o.oU, grads + o.oW, grads + o.ob)))
     return rc;
   st.prof->end(LFMQ_REGION_WGRAD, s);
   return 0;

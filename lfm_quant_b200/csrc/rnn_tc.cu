@@ -1063,7 +1063,6 @@ __global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial
 // Host side
 // =============================================================================================
 struct GenLayer {
-  GenLayerOff off;
   int I, Ipad, Kp;
   __nv_bfloat16 *hseq, *hseq_lo, *hmseq, *hmseq_lo, *in, *in_lo, *gates, *cst;
   __nv_bfloat16 *Wf, *Wf_lo, *Ub, *Wb;
@@ -1073,14 +1072,12 @@ struct GenLayer {
 };
 
 struct GenImpl {
-  bool enabled = false;
   unsigned int* gbar = nullptr;         // grid-barrier counters of the persistent step launches (GBAR_N, zeroed per call)
   int gbar_next = 0;
   cudaStream_t side = nullptr;          // second half of the batch in the backward recurrence (see gen_backward)
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   int maxB = 0, Bp = 0, NRT = 0, T = 0, F = 0, O = 0, H = 0, L = 0, NB16 = 0;
   bool x3 = false, train_ws = false, gru = false, uq = false;
-  int64_t oWo = 0, obo = 0, oWv = -1, obv = -1;
   std::vector<GenLayer> layers;
   __nv_bfloat16 *head_in = nullptr, *head_in_lo = nullptr;      // in[L]
   CUtensorMap tm_head_in;
@@ -1125,8 +1122,7 @@ bool gen_supported(const lfmq_config& c, char* why, size_t n) {
 // literal in rnn_uq_range_estimate.py:86,88), as on the fp32 path.
 static bool gen_stochastic(const lfmq_config& c) { return c.train || c.uq; }
 
-void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_t oWo, int64_t obo, int64_t oWv,
-                int64_t obv, Carver& cv) {
+void gen_layout(TcState& st, const lfmq_config& c, const ParamLayout& pl, Carver& cv) {
   if (!st.gen) st.gen = new GenImpl;
   GenImpl& m = *st.gen;
   m.maxB = c.max_batch; m.T = c.seq_len; m.F = c.n_inputs; m.O = c.n_outputs; m.H = c.num_hidden; m.L = c.num_layers;
@@ -1137,15 +1133,13 @@ void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_
   m.train_ws = !c.forward_only;
   m.gru = c.rnn_cell == LFMQ_CELL_GRU;
   m.uq = c.uq != 0;
-  m.oWo = oWo; m.obo = obo; m.oWv = oWv; m.obv = obv;
   m.BNU = (m.H % 128 == 0) ? 128 : 64;
   const size_t T = m.T, Bp = m.Bp, H = m.H;
   const bool rec = (gen_stochastic(c) && c.recurrent_dropout > 0.f);
   m.layers.assign(m.L, GenLayer{});
   for (int l = 0; l < m.L; ++l) {
     GenLayer& ly = m.layers[l];
-    ly.off = lo[l];
-    ly.I = lo[l].I;
+    ly.I = pl.layers[l].I;
     ly.Ipad = (ly.I + 63) / 64 * 64;
     ly.Kp = (int)H + ly.Ipad;
     ly.hseq = cv.take<__nv_bfloat16>((T + 1) * Bp * H);
@@ -1196,11 +1190,6 @@ void gen_layout(TcState& st, const lfmq_config& c, const GenLayerOff* lo, int64_
 }
 
 int gen_init(TcState& st, const lfmq_config& c) {
-  char why[160];
-  if (!gen_supported(c, why, sizeof(why))) {
-    LFMQ_SET_ERR("tensor-core precision unsupported for this configuration: %s; use LFMQ_PREC_FP32", why);
-    return LFMQ_ERR_UNSUPPORTED;
-  }
   GenImpl& m = *st.gen;
   const size_t T = m.T, Bp = m.Bp, H = m.H;
   int rc;
@@ -1271,7 +1260,6 @@ int gen_init(TcState& st, const lfmq_config& c) {
   }
   LFMQ_CUDA_CHECK(cudaMalloc(&m.gbar, GBAR_N * sizeof(unsigned int)));
   LFMQ_CUDA_CHECK(cudaMemset(m.gbar, 0, GBAR_N * sizeof(unsigned int)));
-  m.enabled = true;
   st.weights_dirty = 1;
   return 0;
 }
@@ -1310,26 +1298,27 @@ static int launch_tile_gemm(dim3 grid, cudaStream_t s, bool pdl, const GArgs& g,
                     a0, a1, a2, a3, b0, b1);
 }
 
-static int gen_pack(TcState& st, const float* params, float eps, cudaStream_t s) {
+static int gen_pack(TcState& st, const ParamLayout& pl, const float* params, float eps, cudaStream_t s) {
   GenImpl& m = *st.gen;
   if (!st.weights_dirty) return 0;
   for (int l = 0; l < m.L; ++l) {
     GenLayer& ly = m.layers[l];
+    const ParamLayout::Layer& o = pl.layers[l];
     GPackArgs a;
     a.H = m.H; a.I = ly.I; a.Ipad = ly.Ipad; a.Kp = ly.Kp; a.gru = m.gru ? 1 : 0;
     a.hs = m.x3 ? 1.0f : 0.5f;
     a.eps = eps;
-    a.W = params + ly.off.oW; a.U = params + ly.off.oU; a.bias = params + ly.off.ob;
-    a.gamma = params + ly.off.ogamma; a.beta = params + ly.off.obeta; a.mean = params + ly.off.omean; a.var = params + ly.off.ovar;
+    a.W = params + o.oW; a.U = params + o.oU; a.bias = params + o.ob;
+    a.gamma = params + o.ogamma; a.beta = params + o.obeta; a.mean = params + o.omean; a.var = params + o.ovar;
     a.Wf = ly.Wf; a.Wf_lo = ly.Wf_lo; a.Ub = ly.Ub; a.Wb = ly.Wb; a.biasp = ly.biasp; a.bn = ly.bn;
     const long n = (long)4 * m.H * ly.Kp;
     gpack_kernel<<<(int)cdivl(n, 256), 256, 0, s>>>(a);
     LFMQ_LAUNCH_CHECK();
   }
-  gpack_head_kernel<<<(int)cdivl((long)m.H * 64, 256), 256, 0, s>>>(m.H, m.O, params + m.oWo, m.WoT, m.WoS);
+  gpack_head_kernel<<<(int)cdivl((long)m.H * 64, 256), 256, 0, s>>>(m.H, m.O, params + pl.oWo, m.WoT, m.WoS);
   LFMQ_LAUNCH_CHECK();
   if (m.uq) {
-    gpack_head_kernel<<<(int)cdivl((long)m.H * 16, 256), 256, 0, s>>>(m.H, m.O, params + m.oWv, m.WoT + 16 * m.H, nullptr);
+    gpack_head_kernel<<<(int)cdivl((long)m.H * 16, 256), 256, 0, s>>>(m.H, m.O, params + pl.oWv, m.WoT + 16 * m.H, nullptr);
     LFMQ_LAUNCH_CHECK();
   }
   st.weights_dirty = 0;
@@ -1439,14 +1428,15 @@ static int gen_wgrad(GenImpl& m, const CUtensorMap& tm_a, int Mvalid, float* dst
   return 0;
 }
 
-static int gen_run_head(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* y, int B,
-                        const float* denom, float* preds, float* out2, bool train, cudaStream_t s) {
+static int gen_run_head(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, float* grads,
+                        const float* y, int B, const float* denom, float* preds, float* out2, bool train,
+                        cudaStream_t s) {
   GenImpl& m = *st.gen;
   if (m.x3) {
     // LFMQ_PREC_BF16X3 (1e-4 tolerance): the fp32-accumulating SIMT head.  Its handles are forward-only, so it predicts.
     GHeadParams h = {};
     h.B = B; h.T = m.T; h.O = m.O; h.H = m.H; h.Bp = m.Bp; h.NRT = (B + 127) / 128;
-    h.Wo = params + m.oWo; h.bo = params + m.obo;
+    h.Wo = params + pl.oWo; h.bo = params + pl.obo;
     h.preds = preds;
     h.yin_lo = m.head_in_lo;
     int grid = m.T * h.NRT;
@@ -1461,7 +1451,7 @@ static int gen_run_head(TcState& st, const lfmq_config& c, const float* params, 
   const int ntile = m.T * m.NRT;                  // every row tile of the time-major buffers (zeros beyond the batch)
   EpiParams ep = {};
   ep.T = m.T; ep.B = B; ep.Bp = m.Bp; ep.H = m.H; ep.NRT = m.NRT; ep.NB16 = m.NB16;
-  ep.hy = y; ep.hdenom = denom; ep.hbo = params + m.obo; ep.hpreds = preds; ep.hdpb = m.dpb;
+  ep.hy = y; ep.hdenom = denom; ep.hbo = params + pl.obo; ep.hpreds = preds; ep.hdpb = m.dpb;
   ep.hpartial = m.head_tc_part; ep.hp1 = c.target_lambda; ep.hp2 = c.rnn_lambda; ep.hO = m.O;
   ep.htarget = c.target_idx; ep.htrain = train ? 1 : 0;
   GArgs g = {};
@@ -1492,38 +1482,35 @@ static int gen_run_head(TcState& st, const lfmq_config& c, const float* params, 
     if ((rc = wgrad_gemm(m.tm_head_in_mn, m.tm_dpb_mn, (long)m.T * m.Bp, m.H, 256, m.wg_part, m.wg_part_elems, false, s,
                          &S, &Mpad)))
       return rc;
-    ghead_wo_reduce_kernel<<<(m.H * m.O + 255) / 256, 256, 0, s>>>(S, m.H, m.O, Mpad, m.wg_part, grads + m.oWo);
+    ghead_wo_reduce_kernel<<<(m.H * m.O + 255) / 256, 256, 0, s>>>(S, m.H, m.O, Mpad, m.wg_part, grads + pl.oWo);
     LFMQ_LAUNCH_CHECK();
   }
   if (y) {
     ghead_reduce_kernel<<<(GH_PART * 32 + 255) / 256, 256, 0, s>>>(ntile, m.head_tc_part, m.O, denom, c.target_lambda,
                                                                   c.rnn_lambda, train ? 1 : 0,
-                                                                  grads ? grads + m.obo : nullptr, out2);
+                                                                  grads ? grads + pl.obo : nullptr, out2);
     LFMQ_LAUNCH_CHECK();
   }
   return 0;
 }
 
-int gen_forward(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
-                int64_t step, float* preds, cudaStream_t s) {
-  if (!st.gen || !st.gen->enabled) {
-    LFMQ_SET_ERR("general tensor-core path not initialised");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
+int gen_forward(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, const float* x, int B,
+                int64_t row0, int64_t step, float* preds, cudaStream_t s) {
   int rc;
-  if ((rc = gen_pack(st, params, c.bn_epsilon, s))) return rc;
+  if ((rc = gen_pack(st, pl, params, c.bn_epsilon, s))) return rc;
   st.prof->begin(LFMQ_REGION_FWD, s);
   if ((rc = gen_run_trunk(st, c, params, x, B, row0, step, false, s))) return rc;
   st.prof->end(LFMQ_REGION_FWD, s);
   st.prof->begin(LFMQ_REGION_HEAD, s);
-  if ((rc = gen_run_head(st, c, params, nullptr, nullptr, B, nullptr, preds, nullptr, false, s))) return rc;
+  if ((rc = gen_run_head(st, c, pl, params, nullptr, nullptr, B, nullptr, preds, nullptr, false, s))) return rc;
   st.prof->end(LFMQ_REGION_HEAD, s);
   return 0;
 }
 
 // The two heads of a uq handle on y = in[L]: bf16, one N = 32 GEMM over [Wo | Wv]; bf16x3, the fp32-accumulating SIMT
 // head once per head.
-static int gen_run_head_uq(GenImpl& m, const float* params, int B, float* preds, float* var, cudaStream_t s) {
+static int gen_run_head_uq(GenImpl& m, const ParamLayout& pl, const float* params, int B, float* preds, float* var,
+                           cudaStream_t s) {
   if (m.x3) {
     GHeadParams h = {};
     h.B = B; h.T = m.T; h.O = m.O; h.H = m.H; h.Bp = m.Bp; h.NRT = (B + 127) / 128;
@@ -1532,8 +1519,8 @@ static int gen_run_head_uq(GenImpl& m, const float* params, int B, float* preds,
     if (grid > m.head_ctas) grid = m.head_ctas;
     const int hsmem = (m.H / 64) * 16384 + m.H * GH_O * 4 + 64 + 1024;
     for (int v = 0; v < 2; ++v) {
-      h.Wo = params + (v ? m.oWv : m.oWo);
-      h.bo = params + (v ? m.obv : m.obo);
+      h.Wo = params + (v ? pl.oWv : pl.oWo);
+      h.bo = params + (v ? pl.obv : pl.obo);
       h.preds = v ? var : preds;
       h.softplus_floor = v;
       ghead_rows_kernel<<<grid, 128, hsmem, s>>>(h, m.tm_head_in);
@@ -1543,8 +1530,8 @@ static int gen_run_head_uq(GenImpl& m, const float* params, int B, float* preds,
   }
   EpiParams ep = {};
   ep.T = m.T; ep.B = B; ep.Bp = m.Bp; ep.H = m.H; ep.NRT = m.NRT; ep.NB16 = m.NB16;
-  ep.hbo = params + m.obo; ep.hpreds = preds; ep.hO = m.O;
-  ep.hbv = params + m.obv; ep.hvar = var;
+  ep.hbo = params + pl.obo; ep.hpreds = preds; ep.hO = m.O;
+  ep.hbv = params + pl.obv; ep.hvar = var;
   GArgs g = {};
   g.n_seg = 1;
   g.seg[0] = GSeg{0, 0, m.H / 64, 0, 0};
@@ -1552,36 +1539,29 @@ static int gen_run_head_uq(GenImpl& m, const float* params, int B, float* preds,
                                            m.tm_head_in, m.tm_head_in, m.tm_wot, m.tm_wot);
 }
 
-int gen_forward_uq(TcState& st, const lfmq_config& c, const float* params, const float* x, int B, int64_t row0,
-                   int64_t step, float* preds, float* var, cudaStream_t s) {
-  if (!st.gen || !st.gen->enabled || !st.gen->uq) {
-    LFMQ_SET_ERR("general tensor-core path not initialised for a uq handle");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
+int gen_forward_uq(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, const float* x,
+                   int B, int64_t row0, int64_t step, float* preds, float* var, cudaStream_t s) {
   int rc;
-  if ((rc = gen_pack(st, params, c.bn_epsilon, s))) return rc;
+  if ((rc = gen_pack(st, pl, params, c.bn_epsilon, s))) return rc;
   st.prof->begin(LFMQ_REGION_FWD, s);
   if ((rc = gen_run_trunk(st, c, params, x, B, row0, step, false, s))) return rc;
   st.prof->end(LFMQ_REGION_FWD, s);
   st.prof->begin(LFMQ_REGION_HEAD, s);
-  if ((rc = gen_run_head_uq(*st.gen, params, B, preds, var, s))) return rc;
+  if ((rc = gen_run_head_uq(*st.gen, pl, params, B, preds, var, s))) return rc;
   st.prof->end(LFMQ_REGION_HEAD, s);
   return 0;
 }
 
-int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* grads, const float* x, const float* y,
-                 int B, int64_t row0, int64_t step, const float* denom, float* tail, cudaStream_t s) {
-  if (!st.gen || !st.gen->enabled || !st.gen->train_ws) {
-    LFMQ_SET_ERR("general tensor-core path not initialised for training");
-    return LFMQ_ERR_UNSUPPORTED;
-  }
+int gen_backward(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, float* grads,
+                 const float* x, const float* y, int B, int64_t row0, int64_t step, const float* denom, float* tail,
+                 cudaStream_t s) {
   GenImpl& m = *st.gen;
   const int T = m.T, H = m.H, Bp = m.Bp;
   const int nrt = (B + 127) / 128;
   const bool rec = c.train && c.recurrent_dropout > 0.f;
   const bool drop = c.train && c.dropout > 0.f;
   int rc;
-  if ((rc = gen_pack(st, params, c.bn_epsilon, s))) return rc;
+  if ((rc = gen_pack(st, pl, params, c.bn_epsilon, s))) return rc;
   st.prof->begin(LFMQ_REGION_FWD, s);
   if ((rc = gen_run_trunk(st, c, params, x, B, row0, step, true, s))) return rc;
   st.prof->end(LFMQ_REGION_FWD, s);
@@ -1592,10 +1572,11 @@ int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* 
     LFMQ_CUDA_CHECK(cudaMemset2DAsync(m.dz + (size_t)nrt * 128 * 4 * H, (size_t)Bp * 4 * H * 2, 0, tail_rows * 4 * H * 2, T, s));
   }
   st.prof->begin(LFMQ_REGION_HEAD, s);
-  if ((rc = gen_run_head(st, c, params, grads, y, B, denom, nullptr, tail, true, s))) return rc;
+  if ((rc = gen_run_head(st, c, pl, params, grads, y, B, denom, nullptr, tail, true, s))) return rc;
   st.prof->end(LFMQ_REGION_HEAD, s);
   for (int l = m.L - 1; l >= 0; --l) {
     GenLayer& ly = m.layers[l];
+    const ParamLayout::Layer& o = pl.layers[l];
     st.prof->begin(LFMQ_REGION_BWD, s);
     {   // Dropout / BN backward of this layer's output: dy -> dhout, dgamma, dbeta
       const int ctas = (int)cdivl((long)T * B, GBN_ROWS);
@@ -1603,8 +1584,8 @@ int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* 
       gbn_drop_bwd_kernel<<<ctas, 256, RL * 2 * H * 4, s>>>(B, T, H, Bp, m.dy, ly.hseq, ly.bn, drop ? 1 : 0,
                                                            dropout_key(c.seed, st.stream_base + 2 * l, step, c.dropout), row0, m.dhout, m.bn_part);
       LFMQ_LAUNCH_CHECK();
-      gpartial_reduce_kernel<<<(2 * H * 32 + 255) / 256, 256, 0, s>>>(ctas, H, H, m.bn_part, grads + ly.off.ogamma,
-                                                                    grads + ly.off.obeta);
+      gpartial_reduce_kernel<<<(2 * H * 32 + 255) / 256, 256, 0, s>>>(ctas, H, H, m.bn_part, grads + o.ogamma,
+                                                                    grads + o.obeta);
       LFMQ_LAUNCH_CHECK();
     }
     EpiParams ep = {};
@@ -1664,17 +1645,17 @@ int gen_backward(TcState& st, const lfmq_config& c, const float* params, float* 
     }
     st.prof->end(LFMQ_REGION_BWD, s);
     st.prof->begin(LFMQ_REGION_WGRAD, s);
-    if ((rc = gen_wgrad(m, ly.tm_hA_mn, H, grads + ly.off.oU, s))) return rc;
+    if ((rc = gen_wgrad(m, ly.tm_hA_mn, H, grads + o.oU, s))) return rc;
     // first layer: the input buffer's first padding column is constant one (gcast_x_kernel), so db falls out of the dW GEMM
     const bool ones_db = (l == 0) && !m.x3 && ly.Ipad > ly.I;
-    if ((rc = gen_wgrad(m, ly.tm_in_mn, ly.I, grads + ly.off.oW, s, ones_db ? grads + ly.off.ob : nullptr))) return rc;
+    if ((rc = gen_wgrad(m, ly.tm_in_mn, ly.I, grads + o.oW, s, ones_db ? grads + o.ob : nullptr))) return rc;
     if (!ones_db) {   // db = column sums of dz over the T*Bp rows (rows beyond the batch are zero)
       const long rows = (long)T * Bp;
       const long rpc = cdivl(rows, m.cs_chunks);
       gcolsum_kernel<<<dim3((4 * H / 8 + 127) / 128, m.cs_chunks), 128, 0, s>>>(rows, 4 * H, rpc, m.dz, m.cs_part);
       LFMQ_LAUNCH_CHECK();
       gpartial_reduce_kernel<<<(4 * H * 32 + 255) / 256, 256, 0, s>>>(m.cs_chunks, 4 * H, 0, m.cs_part,
-                                                                    grads + ly.off.ob, nullptr);
+                                                                    grads + o.ob, nullptr);
       LFMQ_LAUNCH_CHECK();
     }
     if (l > 0) {   // dLoss/dy_{l-1} = dz W^T  -> dy (bf16 [T*Bp][H])

@@ -7,27 +7,20 @@
 
 namespace lfmq {
 
-// offsets of one layer's tensors in the flat fp32 parameter / gradient vectors (from layout() in lfmq_api.cu)
-struct GenLayerOff {
-  int64_t oW, oU, ob, ogamma, obeta, omean, ovar;
-  int I;
-};
-
 bool gen_supported(const lfmq_config& cfg, char* why, size_t n);
 // Carves the general path's buffers from the workspace (only sizes them when the carver has no base).
-// oWv / obv: the variance head of a uq handle (-1 otherwise)
-void gen_layout(TcState& st, const lfmq_config& cfg, const GenLayerOff* layers, int64_t oWo, int64_t obo, int64_t oWv,
-                int64_t obv, Carver& cv);
+void gen_layout(TcState& st, const lfmq_config& cfg, const ParamLayout& pl, Carver& cv);
 int gen_init(TcState& st, const lfmq_config& cfg);
 void gen_destroy(TcState& st);
 // preds [B,T,O] fp32 (predict / validation forward)
-int gen_forward(TcState& st, const lfmq_config& cfg, const float* params, const float* x, int B, int64_t row0,
-                int64_t step, float* preds, cudaStream_t s);
+int gen_forward(TcState& st, const lfmq_config& cfg, const ParamLayout& pl, const float* params, const float* x, int B,
+                int64_t row0, int64_t step, float* preds, cudaStream_t s);
 // uq handles: preds and var [B,T,O] fp32, Dropout / recurrent dropout active with the keys of (step, row0)
-int gen_forward_uq(TcState& st, const lfmq_config& cfg, const float* params, const float* x, int B, int64_t row0,
-                   int64_t step, float* preds, float* var, cudaStream_t s);
+int gen_forward_uq(TcState& st, const lfmq_config& cfg, const ParamLayout& pl, const float* params, const float* x,
+                   int B, int64_t row0, int64_t step, float* preds, float* var, cudaStream_t s);
 // forward + loss + BPTT: fills grads[0 : n_trainable] and tail = {loss, mse_0}
-int gen_backward(TcState& st, const lfmq_config& cfg, const float* params, float* grads, const float* x,
-                 const float* y, int B, int64_t row0, int64_t step, const float* denom, float* tail, cudaStream_t s);
+int gen_backward(TcState& st, const lfmq_config& cfg, const ParamLayout& pl, const float* params, float* grads,
+                 const float* x, const float* y, int B, int64_t row0, int64_t step, const float* denom, float* tail,
+                 cudaStream_t s);
 
 }  // namespace lfmq

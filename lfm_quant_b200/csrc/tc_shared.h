@@ -3,6 +3,8 @@
 #pragma once
 #include <cuda.h>
 
+#include <vector>
+
 #include "../../include/lfmq.h"
 #include "common.cuh"
 
@@ -10,6 +12,18 @@ namespace lfmq {
 
 struct TcImpl;
 struct GenImpl;
+
+// Where each tensor of a handle sits in its flat parameter vector, in floats (the gradient vector has the same layout
+// over its trainable part).  layout() in lfmq_api.cu fills it with the parameter specs; every path reads it.
+struct ParamLayout {
+  struct Layer {
+    int64_t oW, oU, ob, ogamma, obeta, omean, ovar;
+    int I;                      // input width: n_inputs for layer 0, num_hidden above
+  };
+  std::vector<Layer> layers;    // none on a dense handle
+  int64_t oWo = 0, obo = 0;     // OUTPUT_1, or OUTPUT_TARGET_1 on a uq handle
+  int64_t oWv = -1, obv = -1;   // uq: OUTPUT_VARIANCE_1
+};
 
 // Tensor-core state of a handle.  layout() in lfmq_api.cu sets up at most one of the two paths.
 struct TcState {

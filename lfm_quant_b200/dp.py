@@ -6,6 +6,8 @@ over NCCL for a point or dense handle; for chains and uq handles, of the packed 
 loss tail."""
 from __future__ import absolute_import, division, print_function
 
+from ._native import TAIL_MSE0
+
 
 def shard_rows(batch_global, rank, world):
     """Rank r takes rows [r*B/R, (r+1)*B/R) of each global batch; returns (row0, n_rows)."""
@@ -28,7 +30,7 @@ def global_denominators(local_denom, dist):
 def allreduce_flat_gradient(flat_grads, n_trainable, dist):
     """The single data-path collective: SUM over ranks of grads[0 : n_trainable + 2] (gradient, loss, mse_0).
     clip_by_global_norm, the optimizer and MaxNorm then run redundantly on every rank on the reduced gradient."""
-    dist.all_reduce(flat_grads[:n_trainable + 2], op=dist.ReduceOp.SUM)
+    dist.all_reduce(flat_grads[:n_trainable + TAIL_MSE0 + 1], op=dist.ReduceOp.SUM)
     return flat_grads
 
 

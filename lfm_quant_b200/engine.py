@@ -44,7 +44,7 @@ class _HandleEngine(object):
             shp = (shape[0], shape[1]) if ndim.value == 2 else (shape[0],)
             self.specs.append((name.value.decode(), shp, off.value, bool(tr.value)))
         self.params = self._view('lfmq_params_ptr', self.n_total)
-        self.grads = self._view('lfmq_grads_ptr', self.n_trainable + 8)   # tail: loss, mse_0, grad_norm, clip_scale, uq_loss_last_tar
+        self.grads = self._view('lfmq_grads_ptr', self.n_trainable + N.TAIL_LEN)
 
     def _view(self, fn, n):
         p = C.c_void_p(0)
@@ -156,13 +156,14 @@ class _HandleEngine(object):
         x None (a rank without rows) joins with zeros.  Returns the global {loss, mse_0}."""
         import torch.distributed as dist
         from .dp import allreduce_flat_gradient
+        loss_end = self.n_trainable + N.TAIL_MSE0 + 1
         if x is None:
-            self.grads[:self.n_trainable + 2].zero_()
+            self.grads[:loss_end].zero_()
         else:
             self.backward(x, y, step=step, row0=row0, denom=denom_global)
         allreduce_flat_gradient(self.grads, self.n_trainable, dist)
         self.apply(lr, step)
-        return self.grads[self.n_trainable:self.n_trainable + 2].clone()   # not a live view of the workspace tail
+        return self.grads[self.n_trainable:loss_end].clone()   # not a live view of the workspace tail
 
     REGIONS = ('fwd', 'head', 'bwd', 'wgrad', 'opt')
 
@@ -295,7 +296,7 @@ class ForecasterEngine(_HandleEngine):
             self._dp.step(lambda: self.backward(x, y, step=step, row0=row0, denom=denom_global), x is not None, dist)
             self.apply(lr, step)
             t = self.grads[self.n_trainable:]
-            return torch.stack([t[4], t[1]])
+            return torch.stack([t[N.TAIL_UQ_LOSS_LAST_TAR], t[N.TAIL_MSE0]])
         return self._train_step_dp_flat(x, y, step, lr, row0, denom_global)
 
 

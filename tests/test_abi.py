@@ -26,6 +26,15 @@ def test_library_exports_every_declared_symbol():
     assert lib.lfmq_abi_version() == N.ABI_VERSION == 4
 
 
+def test_gradient_tail_slots_match_header():
+    """The engine reads the loss and its parts from the gradient vector's tail by position: _native's TAIL_* must be
+    the header's LFMQ_TAIL_*."""
+    src = open(os.path.join(ROOT, 'include', 'lfmq.h')).read()
+    header = {k: int(v) for k, v in re.findall(r'\bLFMQ_TAIL_(\w+)\s*=\s*(\d+)', src)}
+    mirror = {k[len('TAIL_'):]: v for k, v in vars(N).items() if k.startswith('TAIL_')}
+    assert header == mirror and header['LEN'] == 8, (header, mirror)
+
+
 def test_struct_sizes_match_header_layout():
     # 12 int32 + 8 float + uint64, naturally aligned
     assert C.sizeof(N.LfmqConfig) == 14 * 4 + 8 * 4 + 8
