@@ -195,4 +195,109 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
+// Dropout scale factors of hidden units 8c .. 8c+7 of global row `grow` at step t: quads 2c and 2c+1 of the row's H/4,
+// the quads the oracle draws for them.  All ones when `on` is false.
+__device__ __forceinline__ void dropout8(const DropoutKey& key, bool on, int64_t grow, int t, int T, int H, int c,
+                                         float m[8]) {
+  if (on) {
+    const uint64_t q = ((uint64_t)grow * T + t) * (uint64_t)(H / 4) + c * 2;
+    dropout_quad(key, q, m);
+    dropout_quad(key, q + 1, m + 4);
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m[e] = 1.f;
+  }
+}
+
+// Fixed-order sum of the n partials p[0], p[stride], ..., p[(n-1) stride]: lanes stride over them in fp64, then
+// warp_sum.  Deterministic; every lane returns the sum.
+template <typename T>
+__device__ __forceinline__ double sum_partials(const T* __restrict__ p, long stride, int n) {
+  double s = 0.0;
+  for (int c = threadIdx.x & 31; c < n; c += 32) s += p[(long)c * stride];
+  return warp_sum(s);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Weighted loss of the point estimate and of RNNUqRangeEstimate (model_utils/losses.py:55-135, 180-284):
+//   loss = p1 x0 + (1 - p1) (p2 x1 + (1 - p2) x2)
+// x0: mean over the last step's target column, x1: mean over the last step, x2: mean over every unmasked row.
+// ---------------------------------------------------------------------------------------------
+// A row is masked when all its targets are zero (losses.py:72).
+__device__ __forceinline__ bool row_mask(const float* y, int n) {
+  bool any = false;
+  for (int k = 0; k < n; ++k) any |= (y[k] != 0.0f);
+  return any;
+}
+
+// dLoss/d(term) of one element of each mean: denom_all and denom_last count the rows the means over every row and over
+// the last step divide by.
+struct LossWeights {
+  float all, last, tar;
+};
+__device__ __forceinline__ LossWeights loss_weights(float p1, float p2, int O, float denom_all, float denom_last) {
+  return {(1.f - p1) * (1.f - p2) / ((float)O * denom_all), (1.f - p1) * p2 / (denom_last * (float)O), p1 / denom_last};
+}
+
+// The squared-error terms of one row of predictions pr (masked by m) against targets y: adds them to s0 (last step,
+// column tidx), s1 (last step) and s2 (every column), and with `train` writes dLoss/dpred to dp.  NCOL > 0: the row is
+// NCOL padded registers, and columns >= O and rows that are not valid contribute exactly zero; NCOL = 0: O columns.
+template <int NCOL, typename Acc>
+__device__ __forceinline__ void point_loss_row(const float* pr, const float* y, int O, bool valid, float m, bool last,
+                                               int tidx, const LossWeights& w, bool train, float* dp, Acc& s0, Acc& s1,
+                                               Acc& s2) {
+#pragma unroll
+  for (int k = 0; k < (NCOL > 0 ? NCOL : O); ++k) {
+    const float d = (k < O && valid) ? (pr[k] * m - y[k]) : 0.f;  // losses.py:75: masked predictions are zeroed
+    const float d2 = d * d;
+    s2 += d2;
+    float coef = w.all;
+    if (last) {
+      s1 += d2;
+      coef += w.last;
+      if (k == tidx) {
+        s0 += d2;
+        coef += w.tar;
+      }
+    }
+    if (train) dp[k] = 2.f * d * coef * m;
+  }
+}
+
+__device__ __forceinline__ double weighted_loss(double p1, double p2, double x0, double x1, double x2) {
+  return p1 * x0 + (1.0 - p1) * (p2 * x1 + (1.0 - p2) * x2);
+}
+
+// The tensor-core heads keep s0 s1 s2 in three consecutive slots of a [value][cta] partial array.  The warp of the first
+// slot, whose sum s0 it holds, sums the other two and writes {loss, mse_0} with the batch denominators {B, unmasked
+// rows} (losses.py:87-98).
+__device__ __forceinline__ void point_loss_final(const float* __restrict__ slot0, int n_cta, double s0,
+                                                 const float* denom, int O, float p1, float p2, float* out2) {
+  const double s1 = sum_partials(slot0 + n_cta, 1, n_cta);
+  const double s2 = sum_partials(slot0 + 2L * n_cta, 1, n_cta);
+  if ((threadIdx.x & 31) == 0 && out2) {
+    const double Bg = denom[0], Mg = denom[1];
+    const double mse0 = s0 / Bg, mse1 = s1 / (Bg * O), mse2 = s2 / (Mg * O);
+    out2[0] = (float)weighted_loss(p1, p2, mse0, mse1, mse2);
+    out2[1] = (float)mse0;
+  }
+}
+
+// End of a head kernel: each warp's sums of s0 s1 s2 and, with `train`, of the N columns of dLoss/dpred are added
+// into the CTA's partial row red_s at loss_at (three slots) and dbo_at (N slots).
+template <int N>
+__device__ __forceinline__ void flush_loss_sums(float* red_s, int loss_at, int dbo_at, float s0, float s1, float s2,
+                                                float (&dbo)[N], bool train) {
+  s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
+#pragma unroll
+  for (int k = 0; k < N; ++k) dbo[k] = warp_sum(dbo[k]);
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&red_s[loss_at + 0], s0);
+    atomicAdd(&red_s[loss_at + 1], s1);
+    atomicAdd(&red_s[loss_at + 2], s2);
+    if (train)
+      for (int k = 0; k < N; ++k) atomicAdd(&red_s[dbo_at + k], dbo[k]);
+  }
+}
+
 }  // namespace lfmq

@@ -114,9 +114,7 @@ __global__ void __launch_bounds__(kLossThreads) dense_loss_rows(const float* __r
   float s0 = 0.f, sall = 0.f;
   if (b < B) {
     const float* yr = y + b * O;
-    bool any = false;
-    for (int o = 0; o < O; ++o) any |= yr[o] != 0.f;          // losses.py:69: ~all(y_true == 0)
-    const float mask = any ? 1.f : 0.f;
+    const float mask = row_mask(yr, O) ? 1.f : 0.f;          // losses.py:69: ~all(y_true == 0)
     if (!pred) {
       s0 = 1.f;
       sall = mask;

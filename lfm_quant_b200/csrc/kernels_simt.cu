@@ -858,35 +858,17 @@ __global__ void __launch_bounds__(256) loss_rows_kernel(int B, int T, int O, con
                                                         float p2, float* __restrict__ dpred,
                                                         double* __restrict__ partial) {
   double acc[4] = {0, 0, 0, 0};  // s0, s1, s2, mask count
-  float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
-  if (dpred) {
-    const float Bg = denom[0], Mg = denom[1];
-    c_all = (1.f - p1) * (1.f - p2) / ((float)O * Mg);
-    c_last = (1.f - p1) * p2 / (Bg * (float)O);
-    c_tar = p1 / Bg;
-  }
+  LossWeights lw = {0.f, 0.f, 0.f};
+  if (dpred) lw = loss_weights(p1, p2, O, denom[1], denom[0]);
   const long rows = (long)B * T;
   for (long r = (long)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (long)gridDim.x * blockDim.x) {
     const float* yr = y + r * O;
-    const float* pr = pred ? pred + r * O : nullptr;
-    bool any = false;
-    for (int k = 0; k < O; ++k) any |= (yr[k] != 0.0f);          // losses.py:72
-    const float m = any ? 1.f : 0.f;
+    const float m = row_mask(yr, O) ? 1.f : 0.f;
     acc[3] += m;
-    if (!pr) continue;
+    if (!pred) continue;
     const bool last = ((int)(r % T) == T - 1);
-    for (int k = 0; k < O; ++k) {
-      const float d = pr[k] * m - yr[k];                           // losses.py:75
-      const float d2 = d * d;
-      acc[2] += d2;
-      float coef = c_all;
-      if (last) {
-        acc[1] += d2;
-        coef += c_last;
-        if (k == target_idx) { acc[0] += d2; coef += c_tar; }
-      }
-      if (dpred) dpred[r * O + k] = 2.f * d * coef * m;
-    }
+    point_loss_row<0>(pred + r * O, yr, O, true, m, last, target_idx, lw, dpred != nullptr,
+                      dpred ? dpred + r * O : nullptr, acc[0], acc[1], acc[2]);
   }
   block_reduce4(acc, partial + (long)blockIdx.x * 4);
 }
@@ -896,10 +878,8 @@ __global__ void loss_final_kernel(int nblk, const double* __restrict__ partial, 
                                   int B, int O, float p1, float p2, int mode, float* __restrict__ out,
                                   float* __restrict__ maskout) {
   // one warp, fixed summation order (lane-strided then butterfly): deterministic
-  double s[4] = {0, 0, 0, 0};
-  for (int b = threadIdx.x; b < nblk; b += 32)
-    for (int i = 0; i < 4; ++i) s[i] += partial[(long)b * 4 + i];
-  for (int i = 0; i < 4; ++i) s[i] = warp_sum(s[i]);
+  double s[4];
+  for (int i = 0; i < 4; ++i) s[i] = sum_partials(partial + i, 4, nblk);
   if (threadIdx.x != 0) return;
   if (maskout) {
     maskout[0] = (float)B;
@@ -909,7 +889,7 @@ __global__ void loss_final_kernel(int nblk, const double* __restrict__ partial, 
   const double Bg = denom ? (double)denom[0] : (double)B;
   const double Mg = denom ? (double)denom[1] : s[3];
   const double mse0 = s[0] / Bg, mse1 = s[1] / (Bg * O), mse2 = s[2] / (Mg * O);
-  out[0] = (float)(p1 * mse0 + (1.0 - p1) * (p2 * mse1 + (1.0 - p2) * mse2));
+  out[0] = (float)weighted_loss(p1, p2, mse0, mse1, mse2);
   out[1] = (float)mse0;
 }
 
@@ -943,19 +923,12 @@ __device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* _
                                              float* __restrict__ da, double* __restrict__ partial) {
   double acc[4] = {0, 0, 0, 0};   // uq_0, uq_1, uq_2 numerators, mse_0 numerator
   double cnt[4] = {0, 0, 0, 0};   // unmasked rows, unmasked last-step rows
-  float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
-  if (dpred) {
-    const float ms_all = counts[1], ms_last = counts[2];
-    c_all = (1.f - p1) * (1.f - p2) / (ms_all * (float)O);
-    c_last = (1.f - p1) * p2 / (ms_last * (float)O);
-    c_tar = p1 / ms_last;
-  }
+  LossWeights lw = {0.f, 0.f, 0.f};
+  if (dpred) lw = loss_weights(p1, p2, O, counts[1], counts[2]);
   const long rows = (long)B * T;
   for (long r = (long)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (long)gridDim.x * blockDim.x) {
     const float* yr = y + r * O;
-    bool any = false;
-    for (int k = 0; k < O; ++k) any |= (yr[k] != 0.0f);
-    const float m = any ? 1.f : 0.f;
+    const float m = row_mask(yr, O) ? 1.f : 0.f;
     const bool last = ((int)(r % T) == T - 1);
     cnt[0] += m;
     if (last) cnt[1] += m;
@@ -966,11 +939,11 @@ __device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* _
       const float diff = d * d;
       const float term = diff * (1.f / vm) + logf(vm);
       acc[2] += term;
-      float coef = c_all;
+      float coef = lw.all;
       if (last) {
         acc[1] += term;
-        coef += c_last;
-        if (k == target_idx) { acc[0] += term; acc[3] += diff; coef += c_tar; }
+        coef += lw.last;
+        if (k == target_idx) { acc[0] += term; acc[3] += diff; coef += lw.tar; }
       }
       if (dpred) {
         dpred[r * O + k] = coef * (2.f * d / vm) * m * w;
@@ -992,10 +965,8 @@ __device__ __forceinline__ void uq_loss_final(int nblk, const double* __restrict
                                               float* out_loss, float* out_uq0, float* out_mse0, float* counts_out,
                                               float* vals3) {
   const int lane = threadIdx.x & 31;
-  double s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (int b = lane; b < nblk; b += 32)
-    for (int i = 0; i < 8; ++i) s[i] += partial[(long)b * 8 + i];
-  for (int i = 0; i < 8; ++i) s[i] = warp_sum(s[i]);
+  double s[8];
+  for (int i = 0; i < 8; ++i) s[i] = sum_partials(partial + i, 8, nblk);
   if (lane != 0) return;
   if (counts_out) {
     counts_out[0] = (float)B;
@@ -1006,7 +977,7 @@ __device__ __forceinline__ void uq_loss_final(int nblk, const double* __restrict
   const double ms_all = counts_in ? (double)counts_in[1] : s[4];
   const double ms_last = counts_in ? (double)counts_in[2] : s[5];
   const double uq0 = s[0] / ms_last, uq1 = s[1] / (ms_last * O), uq2 = s[2] / (ms_all * O);
-  vals3[0] = (float)(p1 * uq0 + (1.0 - p1) * (p2 * uq1 + (1.0 - p2) * uq2));
+  vals3[0] = (float)weighted_loss(p1, p2, uq0, uq1, uq2);
   vals3[1] = (float)uq0;
   vals3[2] = (float)(s[3] / Bd);
   if (out_loss) *out_loss = vals3[0];

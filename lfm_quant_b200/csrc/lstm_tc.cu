@@ -462,19 +462,13 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
     fence_mbar_init();
   }
   __syncthreads();
-  float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
-  if (TRAIN) {
-    const float Bg = p.denom[0], Mg = p.denom[1];
-    c_all = (1.f - p.p1) * (1.f - p.p2) / ((float)p.O * Mg);
-    c_last = (1.f - p.p1) * p.p2 / (Bg * (float)p.O);
-    c_tar = p.p1 / Bg;
-  }
+  LossWeights lw = {0.f, 0.f, 0.f};
+  if (TRAIN) lw = loss_weights(p.p1, p.p2, p.O, p.denom[1], p.denom[0]);
   float s0 = 0.f, s1 = 0.f, s2 = 0.f;
   float accbo[TC_OPAD];
 #pragma unroll
   for (int k = 0; k < TC_OPAD; ++k) accbo[k] = 0.f;
   const int sw = tid & 7;
-  const int nq = TC_H / 4;
   uint32_t phase = 0;
   const int n_tiles = p.T * n_btiles;
   for (int ti = blockIdx.x; ti < n_tiles; ti += gridDim.x) {
@@ -504,14 +498,7 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
       const uint4 raw = *reinterpret_cast<const uint4*>(hrow + (c >> 3) * 16384 + (((c & 7) ^ sw) << 4));
       const uint32_t hw[4] = {raw.x, raw.y, raw.z, raw.w};
       float dm[8];
-      if (p.use_dropout) {
-        const uint64_t qbase = ((uint64_t)(p.row0 + b) * p.T + t) * nq + c * 2;
-        dropout_quad(p.key, qbase, dm);
-        dropout_quad(p.key, qbase + 1, dm + 4);
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) dm[e] = 1.f;
-      }
+      dropout8(p.key, p.use_dropout, p.row0 + b, t, p.T, TC_H, c, dm);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         const int j = c * 8 + e;
@@ -532,30 +519,12 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
       for (int k = 0; k < p.O; ++k) p.preds[r * p.O + k] = pr[k];
     }
     if (p.y) {
-      bool any = false;
-#pragma unroll
-      for (int k = 0; k < TC_OPAD; ++k) any |= (yt[k] != 0.0f);          // losses.py:72
-      const float mk = (any && valid) ? 1.f : 0.f;
-      const bool last = (t == p.T - 1);
-      float dp[TC_OPAD];
-#pragma unroll
-      for (int k = 0; k < TC_OPAD; ++k) {
-        const float d = (k < p.O && valid) ? (pr[k] * mk - yt[k]) : 0.f;  // losses.py:75
-        const float d2 = d * d;
-        s2 += d2;
-        float coef = c_all;
-        if (last) {
-          s1 += d2;
-          coef += c_last;
-          if (k == p.target_idx) {
-            s0 += d2;
-            coef += c_tar;
-          }
-        }
-        dp[k] = TRAIN ? 2.f * d * coef * mk : 0.f;
-        if (TRAIN) accbo[k] += dp[k];
-      }
+      const float mk = (row_mask(yt, TC_OPAD) && valid) ? 1.f : 0.f;
+      float dp[TC_OPAD] = {};
+      point_loss_row<TC_OPAD>(pr, yt, p.O, valid, mk, t == p.T - 1, p.target_idx, lw, TRAIN, dp, s0, s1, s2);
       if (TRAIN) {
+#pragma unroll
+        for (int k = 0; k < TC_OPAD; ++k) accbo[k] += dp[k];
         if (valid) {
 #pragma unroll
           for (int k4 = 0; k4 < TC_OPAD; k4 += 4)
@@ -572,14 +541,7 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
             const uint4 raw = *reinterpret_cast<const uint4*>(hrow + (c >> 3) * 16384 + (((c & 7) ^ sw) << 4));
             const uint32_t hw[4] = {raw.x, raw.y, raw.z, raw.w};
             float dm[8];
-            if (p.use_dropout) {
-              const uint64_t qbase = ((uint64_t)(p.row0 + b) * p.T + t) * nq + c * 2;
-              dropout_quad(p.key, qbase, dm);
-              dropout_quad(p.key, qbase + 1, dm + 4);
-            } else {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) dm[e] = 1.f;
-            }
+            dropout8(p.key, p.use_dropout, p.row0 + b, t, p.T, TC_H, c, dm);
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
               const int j = c * 8 + e;
@@ -636,17 +598,7 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
     __syncthreads();        // everyone is done with the tile before it is overwritten
   }
   if (p.y) {
-    // block-level sums of the loss terms and dbo
-    s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
-#pragma unroll
-    for (int k = 0; k < TC_OPAD; ++k) accbo[k] = warp_sum(accbo[k]);
-    if (lane == 0) {
-      atomicAdd(&red_s[2 * TC_H + TC_OPAD + 0], s0);
-      atomicAdd(&red_s[2 * TC_H + TC_OPAD + 1], s1);
-      atomicAdd(&red_s[2 * TC_H + TC_OPAD + 2], s2);
-      if (TRAIN)
-        for (int k = 0; k < TC_OPAD; ++k) atomicAdd(&red_s[2 * TC_H + k], accbo[k]);
-    }
+    flush_loss_sums(red_s, 2 * TC_H + TC_OPAD, 2 * TC_H, s0, s1, s2, accbo, TRAIN);
     __syncthreads();
     for (int i = tid; i < HEAD_PART; i += 128) p.partial[(long)i * gridDim.x + blockIdx.x] = red_s[i];
   }
@@ -792,13 +744,8 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
   } else {
     const int mrow = tid;                   // row of the tile this thread owns
     const int fw = warp, cq = lane & 3;     // accumulator fragment: rows 16 fw + lane / 4 (+ 8) of each 64-row half
-    float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
-    if (TRAIN) {
-      const float Bg = p.denom[0], Mg = p.denom[1];
-      c_all = (1.f - p.p1) * (1.f - p.p2) / ((float)p.O * Mg);
-      c_last = (1.f - p.p1) * p.p2 / (Bg * (float)p.O);
-      c_tar = p.p1 / Bg;
-    }
+    LossWeights lw = {0.f, 0.f, 0.f};
+    if (TRAIN) lw = loss_weights(p.p1, p.p2, p.O, p.denom[1], p.denom[0]);
     float bop[TC_OPAD];
 #pragma unroll
     for (int k = 0; k < TC_OPAD; ++k) bop[k] = w.bop[k];
@@ -862,35 +809,12 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
           if (k < p.O) p.preds[r * p.O + k] = pr[k];
       }
       if (p.y) {
-        bool any = false;
-#pragma unroll
-        for (int k = 0; k < TC_OPAD; ++k) any |= (yt[k] != 0.0f);          // losses.py:72
-        const float mk = (any && valid) ? 1.f : 0.f;
-        const bool last = (t == p.T - 1);
-        float dp[TC_OPAD];
-#pragma unroll
-        for (int k = 0; k < TC_OPAD; ++k) {
-          const float d = (k < p.O && valid) ? (pr[k] * mk - yt[k]) : 0.f;  // losses.py:75
-          const float d2 = d * d;
-          s2 += d2;
-          float coef = c_all;
-          if (last) {
-            s1 += d2;
-            coef += c_last;
-            if (k == p.target_idx) {
-              s0 += d2;
-              coef += c_tar;
-            }
-          }
-          dp[k] = TRAIN ? 2.f * d * coef * mk : 0.f;
-          if (TRAIN) accbo[k] += dp[k];
-        }
+        const float mk = (row_mask(yt, TC_OPAD) && valid) ? 1.f : 0.f;
+        float dp[TC_OPAD] = {};
+        point_loss_row<TC_OPAD>(pr, yt, p.O, valid, mk, t == p.T - 1, p.target_idx, lw, TRAIN, dp, s0, s1, s2);
         if (TRAIN) {
-          if (valid && p.dpred) {        // fp32 copy: only the dropout path's SIMT weight-gradient kernel reads it
 #pragma unroll
-            for (int k4 = 0; k4 < TC_OPAD; k4 += 4)
-              *reinterpret_cast<float4*>(p.dpred + r * TC_OPAD + k4) = make_float4(dp[k4], dp[k4 + 1], dp[k4 + 2], dp[k4 + 3]);
-          }
+          for (int k = 0; k < TC_OPAD; ++k) accbo[k] += dp[k];
           // the TMA store of the previous tile's dpred has read the staging tile (the MMAs that read it are complete)
           if (n > 0 && tid == 0) bulk_wait_group_read0();
           named_bar_sync(1, 128);
@@ -932,18 +856,7 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
       named_bar_sync(1, 128);               // the tile and the pred rows have been read by everybody
       if (tid == 0) mbar_arrive(&bars->tile_free);
     }
-    if (p.y) {
-      s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
-#pragma unroll
-      for (int k = 0; k < TC_OPAD; ++k) accbo[k] = warp_sum(accbo[k]);
-      if (lane == 0) {
-        atomicAdd(&red_s[2 * TC_H + TC_OPAD + 0], s0);
-        atomicAdd(&red_s[2 * TC_H + TC_OPAD + 1], s1);
-        atomicAdd(&red_s[2 * TC_H + TC_OPAD + 2], s2);
-        if (TRAIN)
-          for (int k = 0; k < TC_OPAD; ++k) atomicAdd(&red_s[2 * TC_H + k], accbo[k]);
-      }
-    }
+    if (p.y) flush_loss_sums(red_s, 2 * TC_H + TC_OPAD, 2 * TC_H, s0, s1, s2, accbo, TRAIN);
     if (TRAIN) {
       // this CTA's h^T dpred, [hidden unit][16]
       float* wp = wpartial + (long)blockIdx.x * HWG_PART;
@@ -981,7 +894,6 @@ __global__ void __launch_bounds__(256, 2) head_wgrad_kernel(HeadParams p, float*
 #pragma unroll
     for (int b = 0; b < 4; ++b) acc[a][b] = 0.f;
   const long rows = (long)p.B * p.T;
-  const int nq = TC_H / 4;
   __syncthreads();
   for (long r0 = (long)blockIdx.x * HWG_ROWS; r0 < rows; r0 += (long)gridDim.x * HWG_ROWS) {
     // stage: 32 rows x 256 cols, each thread converts 4 x (8 bf16)
@@ -997,14 +909,7 @@ __global__ void __launch_bounds__(256, 2) head_wgrad_kernel(HeadParams p, float*
         const uint4 raw = *reinterpret_cast<const uint4*>(p.xh + (b * (p.T + 1) + t + 1) * TC_XH_LD + ch * 8);
         const uint32_t hw[4] = {raw.x, raw.y, raw.z, raw.w};
         float dm[8];
-        if (p.use_dropout) {
-          const uint64_t qbase = ((uint64_t)(p.row0 + b) * p.T + t) * nq + ch * 2;
-          dropout_quad(p.key, qbase, dm);
-          dropout_quad(p.key, qbase + 1, dm + 4);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) dm[e] = 1.f;
-        }
+        dropout8(p.key, p.use_dropout, p.row0 + b, t, p.T, TC_H, ch, dm);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           v[2 * e] = fmaf(bn_s[0][ch * 8 + 2 * e], bf16_lo(hw[e]), bn_s[1][ch * 8 + 2 * e]) * dm[2 * e];
@@ -1054,17 +959,13 @@ __global__ void head_reduce_kernel(int n_cta, const float* __restrict__ partial,
   if (i < HWG_PART) {
     if (!train) return;
     const int j = i / TC_OPAD, k = i % TC_OPAD;
-    double s = 0.0;
-    for (int c = lane; c < n_wcta; c += 32) s += wpartial[(long)c * HWG_PART + i];
-    s = warp_sum(s);
+    const double s = sum_partials(wpartial + i, HWG_PART, n_wcta);
     if (lane == 0 && k < O) gWo[j * O + k] = (float)s;
     return;
   }
   const int q = i - HWG_PART;
   if (q >= HEAD_PART) return;
-  double s = 0.0;
-  for (int c = lane; c < n_cta; c += 32) s += partial[(long)q * n_cta + c];
-  s = warp_sum(s);
+  const double s = sum_partials(partial + (long)q * n_cta, 1, n_cta);
   if (q < TC_H) {
     if (train && lane == 0) ggamma[q] = (float)s;
   } else if (q < 2 * TC_H) {
@@ -1073,20 +974,7 @@ __global__ void head_reduce_kernel(int n_cta, const float* __restrict__ partial,
     const int k = q - 2 * TC_H;
     if (train && lane == 0 && k < O) gbo[k] = (float)s;
   } else if (q == 2 * TC_H + TC_OPAD) {
-    // the three loss sums live in consecutive slots; this warp finishes the loss (losses.py:87-98)
-    double s1 = 0.0, s2 = 0.0;
-    for (int c = lane; c < n_cta; c += 32) {
-      s1 += partial[(long)(q + 1) * n_cta + c];
-      s2 += partial[(long)(q + 2) * n_cta + c];
-    }
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
-    if (lane == 0) {
-      const double Bg = denom[0], Mg = denom[1];
-      const double mse0 = s / Bg, mse1 = s1 / (Bg * O), mse2 = s2 / (Mg * O);
-      out2[0] = (float)(p1 * mse0 + (1.0 - p1) * (p2 * mse1 + (1.0 - p2) * mse2));
-      out2[1] = (float)mse0;
-    }
+    point_loss_final(partial + (long)q * n_cta, n_cta, s, denom, O, p1, p2, out2);
   }
 }
 

@@ -407,7 +407,7 @@ __device__ __forceinline__ void epi_store(const EpiParams& p, const float (&acc)
 constexpr int GH_O = 16;
 constexpr int GH_PART = GH_O + 4;      // dbo | s0 s1 s2
 __device__ __forceinline__ void epi_head(const EpiParams& p, const float (&acc)[8], Frag f, float* rows_s, float* red_s) {
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x;
 #pragma unroll
   for (int i = 0; i < 8; ++i) rows_s[(f.m0 + 8 * ((i >> 1) & 1)) * 17 + 8 * (i >> 2) + 2 * f.cq + (i & 1)] = acc[i];
   if (tid < GH_PART) red_s[tid] = 0.f;
@@ -430,52 +430,19 @@ __device__ __forceinline__ void epi_head(const EpiParams& p, const float (&acc)[
   if (p.hpreds && valid)
     for (int k = 0; k < p.hO; ++k) p.hpreds[r * p.hO + k] = pr[k];
   if (!p.hy) return;
-  float c_all = 0.f, c_last = 0.f, c_tar = 0.f;
-  if (p.htrain) {
-    const float Bg = p.hdenom[0], Mg = p.hdenom[1];
-    c_all = (1.f - p.hp1) * (1.f - p.hp2) / ((float)p.hO * Mg);
-    c_last = (1.f - p.hp1) * p.hp2 / (Bg * (float)p.hO);
-    c_tar = p.hp1 / Bg;
-  }
-  bool any = false;
-#pragma unroll
-  for (int k = 0; k < GH_O; ++k) any |= (yt[k] != 0.0f);          // losses.py:72
-  const float mk = (any && valid) ? 1.f : 0.f;
-  const bool last = (t == p.T - 1);
+  LossWeights lw = {0.f, 0.f, 0.f};
+  if (p.htrain) lw = loss_weights(p.hp1, p.hp2, p.hO, p.hdenom[1], p.hdenom[0]);
+  const float mk = (row_mask(yt, GH_O) && valid) ? 1.f : 0.f;
   float s0 = 0.f, s1 = 0.f, s2 = 0.f;
-  float dp[GH_O];
-#pragma unroll
-  for (int k = 0; k < GH_O; ++k) {
-    const float d = (k < p.hO && valid) ? (pr[k] * mk - yt[k]) : 0.f;  // losses.py:75
-    const float d2 = d * d;
-    s2 += d2;
-    float coef = c_all;
-    if (last) {
-      s1 += d2;
-      coef += c_last;
-      if (k == p.htarget) {
-        s0 += d2;
-        coef += c_tar;
-      }
-    }
-    dp[k] = p.htrain ? 2.f * d * coef * mk : 0.f;
-  }
+  float dp[GH_O] = {};
+  point_loss_row<GH_O>(pr, yt, p.hO, valid, mk, t == p.T - 1, p.htarget, lw, p.htrain, dp, s0, s1, s2);
   if (p.htrain) {       // every row of the tile is written (zeros beyond the batch): the dy / dWo GEMMs run over all rows
     uint32_t w[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) w[e] = pack_bf16x2(dp[2 * e], dp[2 * e + 1]);
     st_global_v8(p.hdpb + ((long)t * p.Bp + b) * 64, w);
   }
-  s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
-#pragma unroll
-  for (int k = 0; k < GH_O; ++k) dp[k] = warp_sum(dp[k]);
-  if (lane == 0) {
-    atomicAdd(&red_s[GH_O + 0], s0);
-    atomicAdd(&red_s[GH_O + 1], s1);
-    atomicAdd(&red_s[GH_O + 2], s2);
-    if (p.htrain)
-      for (int k = 0; k < GH_O; ++k) atomicAdd(&red_s[k], dp[k]);
-  }
+  flush_loss_sums(red_s, GH_O, 0, s0, s1, s2, dp, p.htrain);
   named_bar_sync(2, 128);
   if (m < GH_PART) p.hpartial[(long)m * gridDim.x + blockIdx.x] = red_s[m];
 }
@@ -814,14 +781,7 @@ __global__ void __launch_bounds__(256)
     for (int e = 0; e < 8; ++e) hv[e] += lv[e];
   }
   float mk[8];
-  if (use_dropout) {
-    const uint64_t qb = ((uint64_t)(row0 + b) * T + t) * (uint64_t)(H / 4) + c * 2;
-    dropout_quad(key, qb, mk);
-    dropout_quad(key, qb + 1, mk + 4);
-  } else {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) mk[e] = 1.f;
-  }
+  dropout8(key, use_dropout, row0 + b, t, T, H, c, mk);
   const float4 a0 = __ldg(reinterpret_cast<const float4*>(bn + c * 8)), a1 = __ldg(reinterpret_cast<const float4*>(bn + c * 8 + 4));
   const float4 b0 = __ldg(reinterpret_cast<const float4*>(bn + H + c * 8)), b1 = __ldg(reinterpret_cast<const float4*>(bn + H + c * 8 + 4));
   const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
@@ -878,9 +838,7 @@ __global__ void __launch_bounds__(256)
       const float hv[8] = {bf16_lo(hw.x), bf16_hi(hw.x), bf16_lo(hw.y), bf16_hi(hw.y), bf16_lo(hw.z), bf16_hi(hw.z), bf16_lo(hw.w), bf16_hi(hw.w)};
       if (use_dropout) {
         float mk[8];
-        const uint64_t qb = ((uint64_t)(row0 + b) * T + t) * (uint64_t)(H / 4) + c * 2;
-        dropout_quad(key, qb, mk);
-        dropout_quad(key, qb + 1, mk + 4);
+        dropout8(key, true, row0 + b, t, T, H, c, mk);
 #pragma unroll
         for (int e = 0; e < 8; ++e) d[e] *= mk[e];
       }
@@ -916,9 +874,7 @@ __global__ void gpartial_reduce_kernel(int n_cta, int n0, int n1, const float* _
   const int k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (k >= n0 + n1) return;
-  double s = 0.0;
-  for (int c = lane; c < n_cta; c += 32) s += partial[(long)k * n_cta + c];
-  s = warp_sum(s);
+  const double s = sum_partials(partial + (long)k * n_cta, 1, n_cta);
   if (lane == 0) {
     if (k < n0) dst0[k] = (float)s;
     else dst1[k - n0] = (float)s;
@@ -1037,25 +993,11 @@ __global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial
   const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // one warp per output value
   const int lane = threadIdx.x & 31;
   if (q >= GH_PART) return;
-  double s = 0.0;
-  for (int c = lane; c < n_cta; c += 32) s += partial[(long)q * n_cta + c];
-  s = warp_sum(s);
+  const double s = sum_partials(partial + (long)q * n_cta, 1, n_cta);
   if (q < GH_O) {
     if (train && lane == 0 && q < O) gbo[q] = (float)s;
   } else if (q == GH_O) {
-    double s1 = 0.0, s2 = 0.0;
-    for (int c = lane; c < n_cta; c += 32) {
-      s1 += partial[(long)(q + 1) * n_cta + c];
-      s2 += partial[(long)(q + 2) * n_cta + c];
-    }
-    s1 = warp_sum(s1);
-    s2 = warp_sum(s2);
-    if (lane == 0 && out2) {
-      const double Bg = denom[0], Mg = denom[1];
-      const double mse0 = s / Bg, mse1 = s1 / (Bg * O), mse2 = s2 / (Mg * O);
-      out2[0] = (float)(p1 * mse0 + (1.0 - p1) * (p2 * mse1 + (1.0 - p2) * mse2));
-      out2[1] = (float)mse0;
-    }
+    point_loss_final(partial + (long)q * n_cta, n_cta, s, denom, O, p1, p2, out2);
   }
 }
 

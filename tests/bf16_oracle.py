@@ -15,36 +15,36 @@ Rounding plans, one per path (file:line in lfm_quant_b200/csrc):
   * h_t, the next step's A operand    lstm_tc.cu:378-380 (xh row t+1); the head and the dW/dU GEMM read the same bf16 h
   * W, U as packed (x 0.5 on i|f|o)   pack_weights_body, lstm_tc.cu:117-143; the 0.5 is exact, the bias stays fp32
   * saved gates i|f|g|o, cell states  lstm_tc.cu:290-310 (save_chunk), :377 (held chunks)
-  * head without Dropout: bf16(Wo gamma inv) for pred and for dLoss/dh (WoTp / WoSp, pack_head_body lstm_tc.cu:669-683);
-    bias bo + sum_j (beta - gamma mean inv)_j Wo_j in fp32 (:685-701); dLoss/dpred tile bf16 (head_tc_kernel
-    lstm_tc.cu:900-906), dbo from the fp32 dLoss/dpred (:889); dWo, dgamma, dbeta folded from h^T bf16(dpred) and the
-    fp32 column sums (head_fold_kernel lstm_tc.cu:1096-1119)
-  * head with Dropout (head_rows_kernel lstm_tc.cu:441-656): everything fp32 on the bf16 h, dLoss/dh stored as bf16
-    (dhout, :613); dWo from the fp32 Dropout(BN(h)) and fp32 dLoss/dpred (head_wgrad_kernel :970-1046)
-  * backward: U as packed (Ubk, pack_ubk_body :705-713); dLoss/dh_{t-1} = dz_t U^T reduce-scattered over the 4 CTAs of
-    a cluster: the own 64-unit slice stays fp32, the three foreign partial slices arrive as bf16 (lstm_tc.cu:1355-1362,
-    1440-1442); the FUSED head term dpred (Wo gamma inv)^T joins the own slice in fp32 (:1165-1167, :1423)
-  * gate algebra in packed bf16x2 (lstm_tc.cu:1371-1385): dh = bf16(dhout + bf16(rec)) (FUSED: bf16(rec)),
+  * head without Dropout: bf16(Wo gamma inv) for pred and for dLoss/dh (WoTp / WoSp, pack_head_body lstm_tc.cu:621-635);
+    bias bo + sum_j (beta - gamma mean inv)_j Wo_j in fp32 (:637-653); dLoss/dpred tile bf16 (head_tc_kernel
+    lstm_tc.cu:824-830), dbo from the fp32 dLoss/dpred (:817); dWo, dgamma, dbeta folded from h^T bf16(dpred) and the
+    fp32 column sums (head_fold_kernel lstm_tc.cu:984-1007)
+  * head with Dropout (head_rows_kernel lstm_tc.cu:441-608): everything fp32 on the bf16 h, dLoss/dh stored as bf16
+    (dhout, :575); dWo from the fp32 Dropout(BN(h)) and fp32 dLoss/dpred (head_wgrad_kernel :883-951)
+  * backward: U as packed (Ubk, pack_ubk_body :657-665); dLoss/dh_{t-1} = dz_t U^T reduce-scattered over the 4 CTAs of
+    a cluster: the own 64-unit slice stays fp32, the three foreign partial slices arrive as bf16 (lstm_tc.cu:1243-1250,
+    1328-1330); the FUSED head term dpred (Wo gamma inv)^T joins the own slice in fp32 (:1053-1055, :1311)
+  * gate algebra in packed bf16x2 (lstm_tc.cu:1259-1273): dh = bf16(dhout + bf16(rec)) (FUSED: bf16(rec)),
     tc = bf16(tanh c), every bf16x2 mul / fma rounds once; the carried dLoss/dc stays fp32; dz stored bf16
-  * dW, dU, db = bf16 xh^T bf16 dz over all rows, fp32 accumulation (wgrad GEMM, lstm_tc.cu:1457-1478)
+  * dW, dU, db = bf16 xh^T bf16 dz over all rows, fp32 accumulation (wgrad GEMM, lstm_tc.cu:1345-1366)
 
 ``general`` -- rnn_tc.cu, any H multiple of 64 up to 512, any L, both dropouts; also GRU and UQ forward-only handles
-  * x_t cast to bf16 (in[0])          gcast_x_kernel rnn_tc.cu:668-695
+  * x_t cast to bf16 (in[0])          gcast_x_kernel rnn_tc.cu:635-662
   * h_t (hseq) and the masked h_t * mask (hmseq, recurrent dropout): the A operand is the masked copy rounded once
                                       epi_fwd rnn_tc.cu:218-233, epi_gru_fwd :296-310 (GRU carries h in fp32, :295)
   * W, U as packed (x 0.5 on the sigmoid gates, exact); the backward's Ub = bf16(U), Wb = bf16(W)
-                                      gpack_kernel rnn_tc.cu:716-765
-  * layer inputs in[l] = bf16(Dropout(BN(bf16 h))) for l > 0 and the head input in[L]   gbn_drop_fwd_kernel :796-843
+                                      gpack_kernel rnn_tc.cu:683-732
+  * layer inputs in[l] = bf16(Dropout(BN(bf16 h))) for l > 0 and the head input in[L]   gbn_drop_fwd_kernel :763-803
   * saved gates i|f|g|o and cell states                                               epi_fwd :234-241
-  * head: pred = bf16(y) bf16(Wo) + bo (fp32 bias), gpack_head_kernel :770-781, epi_head :429; dLoss/dpred stored
-    bf16 (hdpb, :463-468), dbo from fp32 dpred (:471); dy = bf16(bf16(dpred) bf16(Wo)^T) (EPI_STORE :394-402);
+  * head: pred = bf16(y) bf16(Wo) + bo (fp32 bias), gpack_head_kernel :737-748, epi_head :429; dLoss/dpred stored
+    bf16 (hdpb, :439-444), dbo from fp32 dpred (:445); dy = bf16(bf16(dpred) bf16(Wo)^T) (EPI_STORE :394-402);
     dWo = bf16(y)^T bf16(dpred)
-  * UQ heads: [pred | var] = bf16(y) [bf16(Wo) | bf16(Wv)] + fp32 biases, softplus floor  epi_head_uq :486-501
-  * BN/Dropout backward: fp32 on bf16 dy and bf16 h, dhout = bf16(d gamma inv)           gbn_drop_bwd_kernel :848-910
+  * UQ heads: [pred | var] = bf16(y) [bf16(Wo) | bf16(Wv)] + fp32 biases, softplus floor  epi_head_uq :453-468
+  * BN/Dropout backward: fp32 on bf16 dy and bf16 h, dhout = bf16(d gamma inv)           gbn_drop_bwd_kernel :808-868
   * backward step: rec = dz_{t+1} bf16(U)^T times the recurrent mask, rounded once; then the same bf16x2 gate algebra as
     the cluster path (epi_bwd :352-388), dz stored bf16
-  * dW = bf16(in)^T dz, dU = bf16(masked h_{t-1})^T dz, db = colsum(bf16 dz) (gen_wgrad :1426-1440, gcolsum :929-953);
-    dLoss/d(input) of layers above the first = bf16(dz bf16(W)^T) (EPI_STORE, :1680-1698)
+  * dW = bf16(in)^T dz, dU = bf16(masked h_{t-1})^T dz, db = colsum(bf16 dz) (gen_wgrad :1368-1382, gcolsum :885-909);
+    dLoss/d(input) of layers above the first = bf16(dz bf16(W)^T) (EPI_STORE, :1603-1620)
 
 With ``rb`` replaced by the identity each plan is the fp64 oracle's own arithmetic (tests/test_bf16_oracle_host.py
 holds it to orc.forward / orc.backward / orc.forward_uq to 1e-12).
