@@ -267,6 +267,27 @@ int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, co
                                  int64_t step, int32_t samples, float* const* mean_pred, float* const* mean_var,
                                  float* const* var_pred, float* const* var_var, void* work, uint64_t work_bytes,
                                  void* stream);
+/* ---- integrated gradients of the point forecast ---------------------------------------------------------------------
+ * Which input fields and quarters of each window drive its forecast f(x) = pred[b, T-1, target_idx] (predict.py's
+ * norm_preds_1), with dropout off and BatchNormalization in its inference form.  With the baseline x' = 0 (the value
+ * the batcher pads with) and `steps` = M >= 1 midpoint-rule interpolants alpha_k = (k + 1/2) / M:
+ *   attr[b,t,f] = x[b,t,f] * (1/M) sum_{k<M} df/dx[t,f] (alpha_k x[b])        attr [B,T,F]
+ *   f_x[b] = f(x[b]), f_base[b] = f(0)                                           f_x, f_base [B]
+ * so that sum_{t,f} attr[b] = f_x[b] - f_base[b] up to the quadrature error (completeness).  Interpolant k of window b
+ * is row k * B + b of the batch tiled M times; those rows run in launches of at most max_batch rows, each one forward,
+ * a one-hot seed of d pred at [T-1, target_idx], and the backward of the dz / dh chain and the dx GEMMs only (no
+ * parameter gradient is formed).  One pass per launch adds its input gradients into attr in increasing k (fixed order,
+ * no atomics).  A window's outputs do not depend on the other windows, their order, max_batch or where launches are
+ * cut; two calls give the same bits; f_x and f_base are lfmq_forward's target column at x and at 0 bit for bit.  The
+ * handle's parameters, gradient buffer (tail included) and optimizer slots are left untouched: a model may be
+ * attributed between train steps.  B and steps are not bounded by max_batch.
+ * Accepted: point-estimate handles with forward_only = 0 and train = 0, precision LFMQ_PREC_FP32 or LFMQ_PREC_TF32, either
+ * cell, any num_layers.  LFMQ_PREC_BF16 / LFMQ_PREC_BF16X3 handles: LFMQ_ERR_UNSUPPORTED (their backward does not form
+ * the lowest layer's input gradient).  forward_only, train = 1, uq and dense handles: LFMQ_ERR_ARG.
+ * `work`: caller-owned device scratch, 256-byte aligned, of the size the *_work_bytes query gives for (B, steps). */
+int32_t lfmq_integrated_gradients_work_bytes(lfmq_handle h, int32_t B, int32_t steps, uint64_t* bytes);
+int32_t lfmq_integrated_gradients(lfmq_handle h, const float* x, int32_t B, int32_t steps, float* attr, float* f_x,
+                                  float* f_base, void* work, uint64_t work_bytes, void* stream);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

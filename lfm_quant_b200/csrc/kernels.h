@@ -30,6 +30,7 @@ int shift_mask(cudaStream_t s, int B, int T, int H, const float* h, const float*
 int bn_dropout_fwd(cudaStream_t s, int B, int T, int H, const float* h, const float* gamma, const float* beta,
                    const float* mean, const float* var, float eps, bool use_dropout, DropoutKey key, int64_t row0,
                    float* y);
+// dgamma == nullptr: dh_out only (no dgamma / dbeta, no scratch)
 int bn_dropout_bwd(cudaStream_t s, int B, int T, int H, const float* dy, const float* h, const float* gamma,
                    const float* mean, const float* var, float eps, bool use_dropout, DropoutKey key, int64_t row0,
                    float* dh_out, float* dgamma, float* dbeta, float* scratch, size_t scratch_elems);
@@ -67,6 +68,18 @@ int mc_replicate(cudaStream_t s, int B, int64_t r0, int n, long row_elems, const
 // one, mean_pred / mean_var hold the sample means and var_pred / var_var the population variances.
 struct McMoments { ChainPtrs pred, var, mean_pred, mean_var, var_pred, var_var; };
 int mc_moments(cudaStream_t s, int n_stages, int B, int TO, int64_t r0, int n, int samples, const McMoments& m);
+// Integrated gradients (lfmq_integrated_gradients): interpolant k of window b is row k * B + b of the batch tiled M
+// times, with input alpha_k * x[b], alpha_k = (k + 1/2) / M.
+// ig_scale_inputs: xs = rows [r0, r0 + n) of that tiled batch, each scaled by its alpha_k (row_elems = T * F).
+int ig_scale_inputs(cudaStream_t s, int B, int M, int64_t r0, int n, long row_elems, const float* x, float* xs);
+// ig_seed: dpred [n, T, O] = 1 at [T-1, target_idx] of every row, 0 elsewhere.
+int ig_seed(cudaStream_t s, int n, int T, int O, int target_idx, float* dpred);
+// ig_pick: out[i] = preds[i mod n_src, T-1, target_idx] for i < n_out.
+int ig_pick(cudaStream_t s, int n_out, int n_src, int T, int O, int target_idx, const float* preds, float* out);
+// ig_fold: adds the input gradients dx [n, T, F] of tiled rows [r0, r0 + n) into attr [B, T, F] in increasing k; the
+// last interpolant multiplies the sum by x / M.  Launches must arrive in increasing r0 and cover [0, M * B).
+int ig_fold(cudaStream_t s, int B, int M, int64_t r0, int n, long row_elems, const float* dx, const float* x,
+            float* attr);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

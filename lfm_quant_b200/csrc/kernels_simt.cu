@@ -387,6 +387,7 @@ __global__ void bn_dropout_bwd_kernel(long rows, int T, int H, const float* __re
       }
       *reinterpret_cast<float4*>(dh_out + q * 4) = make_float4(o[0], o[1], o[2], o[3]);
     }
+    if (!partial) return;      // input gradient only: no dgamma / dbeta (uniform over the block)
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       red[(long)rl * 2 * H + j + i] = sg[i];
@@ -432,7 +433,7 @@ int colsum(cudaStream_t s, long rows, int N, const float* A, float* out, float* 
 int bn_dropout_bwd(cudaStream_t s, int B, int T, int H, const float* dy, const float* h, const float* gamma,
                    const float* mean, const float* var, float eps, bool use_dropout, DropoutKey key, int64_t row0,
                    float* dh_out, float* dgamma, float* dbeta, float* scratch, size_t scratch_elems) {
-  if (dbeta != dgamma + H) {
+  if (dgamma && dbeta != dgamma + H) {
     LFMQ_SET_ERR("bn_dropout_bwd: dgamma/dbeta must be adjacent");
     return 1;
   }
@@ -444,6 +445,12 @@ int bn_dropout_bwd(cudaStream_t s, int B, int T, int H, const float* dy, const f
   }
   const int RL = max(1, 256 / nq);
   const int nblk = cdiv(rows, BN_ROWS_PER_BLOCK);
+  if (!dgamma) {      // dh_out only (integrated gradients): no partial sums, no scratch
+    bn_dropout_bwd_kernel<<<nblk, nq * RL, 0, s>>>(rows, T, H, dy, h, gamma, mean, var, eps, use_dropout, key, row0,
+                                                   dh_out, nullptr);
+    LFMQ_LAUNCH_CHECK();
+    return 0;
+  }
   const size_t need = (size_t)nblk * 2 * H + (size_t)1024 * 2 * H;
   if (need > scratch_elems) {
     LFMQ_SET_ERR("bn_dropout_bwd: scratch too small (%zu > %zu)", need, scratch_elems);
@@ -722,6 +729,77 @@ int mc_moments(cudaStream_t s, int n_stages, int B, int TO, int64_t r0, int n, i
   const long threads = (long)min(n, B) * TO;
   dim3 grid(cdiv(threads, 256), n_stages);
   mc_moments_kernel<<<grid, 256, 0, s>>>(B, TO, r0, n, samples, m);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- integrated gradients: interpolant k of window b is row r = k * B + b of the batch tiled M times -----------------
+// xs = alpha_k * x for rows [r0, r0 + n), alpha_k = (k + 1/2) / M (the midpoint rule)
+__global__ void ig_scale_inputs_kernel(long n_elems, long B, int M, long r0, long row_elems, const float* __restrict__ x,
+                                       float* __restrict__ xs) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_elems) return;
+  const long r = r0 + i / row_elems;
+  const float alpha = ((float)(r / B) + 0.5f) / (float)M;
+  xs[i] = alpha * x[(r % B) * row_elems + i % row_elems];
+}
+int ig_scale_inputs(cudaStream_t s, int B, int M, int64_t r0, int n, long row_elems, const float* x, float* xs) {
+  const long n_elems = (long)n * row_elems;
+  ig_scale_inputs_kernel<<<cdiv(n_elems, 256), 256, 0, s>>>(n_elems, B, M, r0, row_elems, x, xs);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+// dpred [n, T, O] = the one-hot at [T-1, target_idx] of every row: d pred[b, T-1, target_idx] / d pred
+__global__ void ig_seed_kernel(long n_elems, int TO, int hot, float* __restrict__ dpred) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_elems) dpred[i] = (i % TO == hot) ? 1.0f : 0.0f;
+}
+int ig_seed(cudaStream_t s, int n, int T, int O, int target_idx, float* dpred) {
+  const long n_elems = (long)n * T * O;
+  ig_seed_kernel<<<cdiv(n_elems, 256), 256, 0, s>>>(n_elems, T * O, (T - 1) * O + target_idx, dpred);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+// out[i] = preds[i mod n_src][T-1][target_idx] for i < n_out
+__global__ void ig_pick_kernel(int n_out, int n_src, int TO, int hot, const float* __restrict__ preds,
+                               float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_out) out[i] = preds[(long)(i % n_src) * TO + hot];
+}
+int ig_pick(cudaStream_t s, int n_out, int n_src, int T, int O, int target_idx, const float* preds, float* out) {
+  ig_pick_kernel<<<cdiv(n_out, 256), 256, 0, s>>>(n_out, n_src, T * O, (T - 1) * O + target_idx, preds, out);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+// One thread per (window b, element e of [T,F]) with interpolants among the launch's rows [r0, r0 + n): as mc_moments,
+// j < min(n, B) walks the windows in row order and finds interpolants k_lo, k_lo + 1, .. at local rows j, j + B, ...
+// The running sum of the gradients lives in attr and is added to in increasing k, so every element sees the same
+// additions in the same order however the rows are cut; interpolant 0 starts it and interpolant M - 1 scales it by x / M.
+__global__ void ig_fold_kernel(int B, int M, int64_t r0, int n, long row_elems, const float* __restrict__ dx,
+                               const float* __restrict__ x, float* __restrict__ attr) {
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int nb = min(n, B);
+  if (i >= (long)nb * row_elems) return;
+  const int j = (int)(i / row_elems);
+  const long e = i % row_elems;
+  const int64_t rj = r0 + j;
+  const int b = (int)(rj % B);
+  const int k_lo = (int)(rj / B);
+  const int k_hi = k_lo + (n - 1 - j) / B;
+  const long o = (long)b * row_elems + e;
+  const float* g = dx + (long)j * row_elems + e;
+  float acc = (k_lo == 0) ? 0.f : attr[o];
+  for (int k = k_lo; k <= k_hi; ++k) acc += g[(long)(k - k_lo) * B * row_elems];
+  if (k_hi == M - 1) acc *= x[o] / (float)M;
+  attr[o] = acc;
+}
+int ig_fold(cudaStream_t s, int B, int M, int64_t r0, int n, long row_elems, const float* dx, const float* x,
+            float* attr) {
+  const long threads = (long)min(n, B) * row_elems;
+  ig_fold_kernel<<<cdiv(threads, 256), 256, 0, s>>>(B, M, r0, n, row_elems, dx, x, attr);
   LFMQ_LAUNCH_CHECK();
   return 0;
 }

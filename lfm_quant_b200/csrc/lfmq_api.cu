@@ -394,8 +394,11 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
   return 0;
 }
 
-// dx_out (nullable): dLoss/dx [B,T,F] of the lowest layer (the stages of a forecast chain feed predictions back in)
-int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* dx_out = nullptr) {
+// dx_out (nullable): dLoss/dx [B,T,F] of the lowest layer (the stages of a forecast chain feed predictions back in).
+// input_only: the dz / dh chain and the dx GEMMs alone, for integrated gradients: no parameter gradient (head, BN, dW,
+// dU, db) is formed, and the handle's gradient buffer is not written.
+int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* dx_out = nullptr,
+                  bool input_only = false) {
   const lfmq_config& c = h->cfg;
   const int H = c.num_hidden, T = c.seq_len, O = c.n_outputs, L = c.num_layers;
   const long BT = (long)B * T;
@@ -404,12 +407,16 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
   const float* yl = h->layers[L - 1].y;
   // head: dWo = y^T dpred, dbo = colsum(dpred), dy = dpred Wo^T
   h->prof.begin(LFMQ_REGION_HEAD, s);
-  RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->dpred, O, 1, G + h->pl.oWo, O, 0.f, h->scratch, h->scratch_elems));
-  RUN(colsum(s, BT, O, h->dpred, G + h->pl.obo, h->scratch, h->scratch_elems));
+  if (!input_only) {
+    RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->dpred, O, 1, G + h->pl.oWo, O, 0.f, h->scratch, h->scratch_elems));
+    RUN(colsum(s, BT, O, h->dpred, G + h->pl.obo, h->scratch, h->scratch_elems));
+  }
   RUN(gemm(h, s, (int)BT, H, O, h->dpred, O, 1, P + h->pl.oWo, 1, O, h->dy, H, 0.f, nullptr, 0));
   if (c.uq) {      // variance head: same three products on da, dy accumulates
-    RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->da, O, 1, G + h->pl.oWv, O, 0.f, h->scratch, h->scratch_elems));
-    RUN(colsum(s, BT, O, h->da, G + h->pl.obv, h->scratch, h->scratch_elems));
+    if (!input_only) {
+      RUN(gemm(h, s, H, O, (int)BT, yl, 1, H, h->da, O, 1, G + h->pl.oWv, O, 0.f, h->scratch, h->scratch_elems));
+      RUN(colsum(s, BT, O, h->da, G + h->pl.obv, h->scratch, h->scratch_elems));
+    }
     RUN(gemm(h, s, (int)BT, H, O, h->da, O, 1, P + h->pl.oWv, 1, O, h->dy, H, 1.f, nullptr, 0));
   }
   h->prof.end(LFMQ_REGION_HEAD, s);
@@ -422,7 +429,8 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
     h->prof.begin(LFMQ_REGION_BWD, s);
     RUN(bn_dropout_bwd(s, B, T, H, h->dy, lb.h, P + o.ogamma, P + o.omean, P + o.ovar, c.bn_epsilon, drop,
                        dropout_key(c.seed, h->tc.stream_base + 2 * l, h->last_step, c.dropout), h->last_row0, h->dh_out,
-                       G + o.ogamma, G + o.obeta, h->scratch, h->scratch_elems));
+                       input_only ? nullptr : G + o.ogamma, input_only ? nullptr : G + o.obeta, h->scratch,
+                       h->scratch_elems));
     const bool gru = c.rnn_cell == LFMQ_CELL_GRU;
     const int NG = gru ? 3 : 4;
     for (int t = T - 1; t >= 0 && gru; --t) {
@@ -446,11 +454,13 @@ int backward_fp32(lfmq_handle h, const float* x, int B, cudaStream_t s, float* d
     // bias rows [2][3H] = colsum of each.
     const float* dzr = gru ? h->dz2 : h->dz;
     const int GH = NG * H;
-    RUN(gemm(h, s, I, GH, (int)BT, in, 1, I, h->dz, GH, 1, G + o.oW, GH, 0.f, h->scratch, h->scratch_elems));
-    RUN(shift_mask(s, B, T, H, lb.h, rmask, h->hp));
-    RUN(gemm(h, s, H, GH, (int)BT, h->hp, 1, H, dzr, GH, 1, G + o.oU, GH, 0.f, h->scratch, h->scratch_elems));
-    RUN(colsum(s, BT, GH, h->dz, G + o.ob, h->scratch, h->scratch_elems));
-    if (gru) RUN(colsum(s, BT, GH, h->dz2, G + o.ob + GH, h->scratch, h->scratch_elems));
+    if (!input_only) {
+      RUN(gemm(h, s, I, GH, (int)BT, in, 1, I, h->dz, GH, 1, G + o.oW, GH, 0.f, h->scratch, h->scratch_elems));
+      RUN(shift_mask(s, B, T, H, lb.h, rmask, h->hp));
+      RUN(gemm(h, s, H, GH, (int)BT, h->hp, 1, H, dzr, GH, 1, G + o.oU, GH, 0.f, h->scratch, h->scratch_elems));
+      RUN(colsum(s, BT, GH, h->dz, G + o.ob, h->scratch, h->scratch_elems));
+      if (gru) RUN(colsum(s, BT, GH, h->dz2, G + o.ob + GH, h->scratch, h->scratch_elems));
+    }
     if (l > 0 || dx_out)
       RUN(gemm(h, s, (int)BT, I, GH, h->dz, GH, 1, P + o.oW, 1, GH, l > 0 ? h->dy : dx_out, I, 0.f, nullptr, 0));
     h->prof.end(LFMQ_REGION_WGRAD, s);
@@ -1182,6 +1192,99 @@ int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, co
   }
   return mc_run(stages, n_stages, x, B, row0, step, samples, mb, mean_pred, mean_var, var_pred, var_var, work,
                 work_bytes, (cudaStream_t)stream);
+}
+
+// ---- integrated gradients of the point forecast (lfmq_integrated_gradients) ----------------------------------------
+namespace {
+// Built with -DLFMQ_IG_PARAM_GRADS (`make alt`), every interpolant's backward also forms the parameter gradients, into
+// the handle's gradient buffer: tools/bench_ig.py measures what skipping them saves.  Not a mode to run in.
+#ifdef LFMQ_IG_PARAM_GRADS
+constexpr bool kIgInputOnly = false;
+#else
+constexpr bool kIgInputOnly = true;
+#endif
+
+int ig_check(lfmq_handle h, int32_t B, int32_t steps, const char* fn) {
+  if (!h) {
+    LFMQ_SET_ERR("%s: null handle", fn);
+    return LFMQ_ERR_ARG;
+  }
+  RUN(refuse_dense(h, fn));
+  const lfmq_config& c = h->cfg;
+  if (c.precision == LFMQ_PREC_BF16 || c.precision == LFMQ_PREC_BF16X3) {
+    LFMQ_SET_ERR("%s: the bf16 and bf16x3 paths never form the lowest layer's input gradient; attribute through an "
+                 "LFMQ_PREC_FP32 or LFMQ_PREC_TF32 handle holding the same parameters", fn);
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  if (c.forward_only || c.train || c.uq) {
+    LFMQ_SET_ERR("%s: needs a point-estimate handle created with forward_only = 0 and train = 0 (got forward_only %d, "
+                 "train %d, uq %d): a forward_only handle keeps no backward buffers, and dropout (train = 1, or any uq "
+                 "handle) makes the forecast random", fn, c.forward_only, c.train, c.uq);
+    return LFMQ_ERR_ARG;
+  }
+  if (B < 1 || steps < 1) {
+    LFMQ_SET_ERR("%s: need B >= 1 and steps >= 1 (got %d, %d)", fn, B, steps);
+    return LFMQ_ERR_ARG;
+  }
+  return 0;
+}
+
+// rows per launch and caller scratch: the scaled inputs and their input gradients, one launch each
+size_t ig_rows(const lfmq_config& c, int B, int steps) {
+  return (size_t)std::min<int64_t>((int64_t)steps * B, c.max_batch);
+}
+size_t ig_work_floats(const lfmq_config& c, size_t rows) { return 2 * mc_align(rows * c.seq_len * c.n_inputs); }
+}  // namespace
+
+int32_t lfmq_integrated_gradients_work_bytes(lfmq_handle h, int32_t B, int32_t steps, uint64_t* bytes) {
+  RUN(ig_check(h, B, steps, "lfmq_integrated_gradients_work_bytes"));
+  if (!bytes) {
+    LFMQ_SET_ERR("lfmq_integrated_gradients_work_bytes: bytes == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  *bytes = ig_work_floats(h->cfg, ig_rows(h->cfg, B, steps)) * sizeof(float);
+  return LFMQ_OK;
+}
+
+int32_t lfmq_integrated_gradients(lfmq_handle h, const float* x, int32_t B, int32_t steps, float* attr, float* f_x,
+                                  float* f_base, void* work, uint64_t work_bytes, void* stream) {
+  RUN(ig_check(h, B, steps, "lfmq_integrated_gradients"));
+  if (!x || !attr || !f_x || !f_base) {
+    LFMQ_SET_ERR("lfmq_integrated_gradients: null pointer");
+    return LFMQ_ERR_ARG;
+  }
+  const lfmq_config& c = h->cfg;
+  const int T = c.seq_len, O = c.n_outputs, ti = c.target_idx;
+  const long row_in = (long)T * c.n_inputs;
+  const size_t rows = ig_rows(c, B, steps);
+  const size_t need = ig_work_floats(c, rows) * sizeof(float);
+  if (!work || work_bytes < need) {
+    LFMQ_SET_ERR("lfmq_integrated_gradients: work needs %zu bytes, got %llu", need, (unsigned long long)work_bytes);
+    return LFMQ_ERR_WORKSPACE;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  float* xs = static_cast<float*>(work);
+  float* dx = xs + mc_align(rows * row_in);
+  // f(0): a row's forecast depends on that row alone, so one row of zeros gives every window's baseline
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(xs, 0, row_in * sizeof(float), s));
+  RUN(forward_fp32(h, xs, 1, 0, 0, h->preds, nullptr, s));
+  RUN(ig_pick(s, B, 1, T, O, ti, h->preds, f_base));
+  for (int b0 = 0; b0 < B; b0 += c.max_batch) {       // f(x)
+    const int n = std::min(B - b0, c.max_batch);
+    RUN(forward_fp32(h, x + b0 * row_in, n, 0, 0, h->preds, nullptr, s));
+    RUN(ig_pick(s, n, n, T, O, ti, h->preds, f_x + b0));
+  }
+  // the interpolants: rows [r0, r0 + n) of the batch tiled `steps` times, their input gradients folded in order
+  const int64_t total = (int64_t)steps * B;
+  for (int64_t r0 = 0; r0 < total; r0 += (int64_t)rows) {
+    const int n = (int)std::min<int64_t>((int64_t)rows, total - r0);
+    RUN(ig_scale_inputs(s, B, steps, r0, n, row_in, x, xs));
+    RUN(forward_fp32(h, xs, n, 0, 0, h->preds, nullptr, s));
+    RUN(ig_seed(s, n, T, O, ti, h->dpred));
+    RUN(backward_fp32(h, xs, n, s, dx, kIgInputOnly));
+    RUN(ig_fold(s, B, steps, r0, n, row_in, dx, x, attr));
+  }
+  return LFMQ_OK;
 }
 
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,

@@ -258,6 +258,25 @@ class ForecasterEngine(_HandleEngine):
                                             _ptr(work), work.numel(), _stream()))
         return tuple(out)
 
+    def integrated_gradients(self, x, steps):
+        """Integrated-gradients attributions of the point forecast pred[:, T-1, target_idx] in one call
+        (lfmq_integrated_gradients): the device tensors (attr [B,T,F], f_x [B], f_base [B]) for the zero baseline and
+        `steps` midpoint-rule interpolants; sum(attr[b]) approximates f_x[b] - f_base[b].  An fp32 or tf32 engine
+        created with train=False, forward_only=False and uq=False; B and steps are not bounded by max_batch.  The
+        engine's parameters, gradients and optimizer state are left as they were."""
+        B = self._check_x(x)
+        n = C.c_uint64(0)
+        N.check(self.lib.lfmq_integrated_gradients_work_bytes(self.handle, B, int(steps), C.byref(n)))
+        work = getattr(self, '_ig_buf', None)
+        if work is None or work.numel() < n.value:
+            work = self._ig_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=self.device)
+        attr = torch.empty(B, self.T, self.F, dtype=torch.float32, device=x.device)
+        f_x = torch.empty(B, dtype=torch.float32, device=x.device)
+        f_base = torch.empty_like(f_x)
+        N.check(self.lib.lfmq_integrated_gradients(self.handle, _ptr(x), B, int(steps), _ptr(attr), _ptr(f_x),
+                                                   _ptr(f_base), _ptr(work), work.numel(), _stream()))
+        return attr, f_x, f_base
+
     def loss_uq(self, preds, var, y):
         """Device tensor {uq_loss, uq_loss_last_tar, mse_0} (Losses.weight_adjusted_uq_loss, losses.py:137-284)."""
         out = torch.empty(3, dtype=torch.float32, device=preds.device)

@@ -106,6 +106,8 @@ SCHEMA = [
                                    "cell, head and forecast_steps), 'bf16' (tensor-core gate GEMMs) or 'bf16x3'"),
     ('mc_samples', _INT, 1, 'Monte-Carlo dropout samples per window at UQ prediction; more than 1 also writes the '
                             "UQ ensemble's ensemble_preds.dat with the calibrated lower bounds"),
+    ('ig_steps', _INT, 0, 'Integrated-gradients interpolants per window at point-estimate prediction; more than 0 also '
+                          'writes pred/attributions.npz: which input fields and quarters drive each forecast'),
 ]
 
 _DEFINERS = {_STRING: configs.DEFINE_string, _INT: configs.DEFINE_integer, _FLOAT: configs.DEFINE_float,

@@ -17,6 +17,9 @@ from ...model_utils.optimizers import Optimizers
 # Rows per launch of NativeForecaster.predict_mc: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to
 # 10x (bf16x3) faster than a handle of B rows on an H100 (DESIGN.md section 5c).
 MC_ROWS = 8192
+# Rows per launch of NativeForecaster.attribute: the saved activations and gradients of the fp32 step grow with the rows
+# (DESIGN.md section 5d gives the workspace and the times that chose it).
+IG_ROWS = 4096
 
 
 class _Variable(object):
@@ -64,6 +67,7 @@ class NativeForecaster(object):
         self.trainable_variables = [_Variable(self, i, n, s) for i, (n, s) in enumerate(specs)]
         self._calls = 0
         self._mc_engine, self._mc_stale = None, True
+        self._ig_engine, self._ig_stale = None, True
 
     @property
     def title(self):
@@ -151,9 +155,48 @@ class NativeForecaster(object):
             self._mc_engine.close()
             self._mc_engine = None
 
+    def attribute(self, inp, steps):
+        """Integrated-gradients attributions of the point forecast norm_preds_1 = pred[:, T-1, target_idx] of every
+        window, against the zero baseline with `steps` midpoint-rule interpolants (ForecasterEngine.integrated_gradients):
+        the device tensors (attr [B,T,F], f_x [B], f_base [B]), sum(attr[b]) ~ f_x[b] - f_base[b].  Point estimates with
+        forecast_steps = 1 only.  A tf32 model is explained through its tf32 arithmetic; every other precision,
+        bf16 and bf16x3 included, through the fp32 arithmetic of the same weights (the bf16 paths form no input
+        gradient), so f_x may differ from what model.predict returns by that precision's rounding."""
+        if self.uq or self.config.forecast_steps != 1:
+            raise ValueError('attribute explains a point estimate with forecast_steps = 1 (got %s, forecast_steps=%d)'
+                             % (self.title, self.config.forecast_steps))
+        if int(steps) < 1:
+            raise ValueError('attribute: steps must be >= 1 (got %r)' % (steps,))
+        return self._ig_rows_engine(int(steps)).integrated_gradients(_to_device(self.engine, inp), int(steps))
+
+    def _ig_rows_engine(self, steps):
+        """The engine attribute runs on: a trainable-mode handle with train = 0 (dropout off) of the model's stage,
+        tf32 for a tf32 model and fp32 otherwise, with max_batch = min(steps * batch_size, IG_ROWS).  Created at the first
+        call (again for a larger count) and owned by the model; its copy of the weights is renewed after set_weights,
+        load_weights and the train steps."""
+        from ....engine import ForecasterEngine
+        rows = min(steps * self.config.batch_size, IG_ROWS)
+        if self._ig_engine is None or self._ig_engine.cfg.max_batch < rows:
+            self._close_ig_engine()
+            kw = {k: v for k, v in self._engine_kw.items() if k not in ('forecast_steps', 'weights')}
+            kw.update(max_batch=rows, train=False, forward_only=False, device=self.engine.device,
+                      precision='tf32' if kw['precision'] == 'tf32' else 'fp32')
+            self._ig_engine = ForecasterEngine(**kw)
+            self._ig_stale = True
+        if self._ig_stale:
+            self._ig_engine.set_flat(self.engine.stages[0].get_flat())
+            self._ig_stale = False
+        return self._ig_engine
+
+    def _close_ig_engine(self):
+        if self._ig_engine is not None:
+            self._ig_engine.close()
+            self._ig_engine = None
+
     def close(self):
         """Releases the device memory of the model's handles."""
         self._close_mc_engine()
+        self._close_ig_engine()
         self.engine.close()
 
     def predict(self, inp, batch_size=None):
@@ -164,7 +207,7 @@ class NativeForecaster(object):
         """Fused fwd + loss + BPTT + clip + optimizer + MaxNorm (train.py:178-225); returns the device tensor
         {loss, mse}, on a uq model {uq_loss_last_tar, mse}."""
         assert isinstance(targets, (list, tuple)), 'targets must be the list of forecast_steps targets (train.py:188)'
-        self._mc_stale = True
+        self._mc_stale = self._ig_stale = True
         return self.engine.train_step(_to_device(self.engine, inp), [_to_device(self.engine, t) for t in targets],
                                       iteration, lr)
 
@@ -175,7 +218,7 @@ class NativeForecaster(object):
         if x is not None:
             assert isinstance(ys, (list, tuple)), 'ys must be the list of forecast_steps targets'
             x, ys = _to_device(self.engine, x), [_to_device(self.engine, t) for t in ys]
-        self._mc_stale = True
+        self._mc_stale = self._ig_stale = True
         return self.engine.train_step_dp(x, ys, step, lr, row0, denoms)
 
     # -- Keras API surface -------------------------------------------------------------------------------
@@ -223,7 +266,7 @@ class NativeForecaster(object):
                                     '%s.index (Keras save_weights) exists' % (prefix, os.path.basename(prefix),
                                                                               os.path.basename(prefix)))
         self.engine.load_named(lambda name: data[name])
-        self._mc_stale = True
+        self._mc_stale = self._ig_stale = True
 
     def get_weights(self):
         return self.engine.get_weights(trainable_only=False)
@@ -231,7 +274,7 @@ class NativeForecaster(object):
     def set_weights(self, weights):
         """The trainable arrays, optionally followed by the BatchNormalization statistics (get_weights' order)."""
         self.engine.set_weights(weights)
-        self._mc_stale = True
+        self._mc_stale = self._ig_stale = True
 
 
 class RNNPointEstimate(BaseModelClass):

@@ -42,6 +42,7 @@ class Predict(object):
         if 'Naive' not in self.config.nn_type:            # predict.py:90-93: the naive forecast has no variables
             self.model.load_weights(os.path.join(self.chkpts_dir, "chkpt"))
         outputs = defaultdict(list)
+        ig = defaultdict(list)
         for (inp_dev, target_dev, metadata) in self._batches:
             # one target window per input window: every forecast step is compared with it (Train._step_targets)
             inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()] * self.config.forecast_steps
@@ -70,6 +71,11 @@ class Predict(object):
                 preds, variance = model_preds[0::2], model_preds[1::2]
             outputs['norm_preds'].append(self._extract_preds(preds))
             outputs['norm_variance'].append(self._extract_preds(variance))
+            if self.config.ig_steps > 0:
+                for key, t in zip(('attr', 'f_x', 'f_base'), self.model.attribute(inp_dev, self.config.ig_steps)):
+                    ig[key].append(t.cpu().numpy())
+        if self.config.ig_steps > 0:
+            self._write_attributions(outputs, ig)
 
         single_outputs = ['date', 'gvkey', 'seq_norm'] + [x for x in outputs.keys() if 'inp_t' in x]
         for key in single_outputs:
@@ -123,6 +129,18 @@ class Predict(object):
         for i in range(self.config.forecast_steps):
             print("Scaled MSE for step %i: %1.4f" % (i + 1, df['norm_squared_diff_' + str(i + 1)].mean()))
         return df
+
+    def _write_attributions(self, outputs, ig):
+        """<model_dir>/pred/attributions.npz: the integrated-gradients attributions of norm_preds_1 (--ig_steps), one
+        row per preds.dat row in its order -- date [N] (yyyymmdd), gvkey [N], fields [F] (the input fields in the
+        Dataset's column order), attr [N,T,F], f_x [N] and f_base [N] (the forecast at the window and at the zero
+        baseline)."""
+        gvkey = np.vstack(outputs['gvkey']).flatten()
+        np.savez(os.path.join(self.pred_dir, 'attributions.npz'),
+                 date=np.vstack(outputs['date']).flatten().astype(np.int32),
+                 gvkey=np.array([g.decode('utf-8') if isinstance(g, bytes) else str(g) for g in gvkey]),
+                 fields=np.array(self.dataset.fin_col_names + self.dataset.aux_col_names),
+                 **{k: np.concatenate(v).astype(np.float32) for k, v in ig.items()})
 
     def _flat(self):
         """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""

@@ -245,6 +245,12 @@ class ModelExecution(object):
             raise ValueError('--mc_samples %d: Monte-Carlo dropout samples are drawn at UQ prediction only (--UQ=True '
                              '--train=False); a point estimate predicts with dropout off, and training and validation '
                              'take one sample' % self.config.mc_samples)
+        c = self.config
+        if c.ig_steps != 0 and (c.ig_steps < 0 or c.train or c.UQ or c.nn_type != 'RNNPointEstimate'
+                                or c.forecast_steps != 1):
+            raise ValueError('--ig_steps %d: integrated-gradients attributions explain the forecast of a trained '
+                             'RNNPointEstimate with forecast_steps = 1 at prediction (--train=False, --UQ=False), with '
+                             'ig_steps >= 1 interpolants (0 = off)' % c.ig_steps)
         if self.config.training_type == 'iterative':
             raise NotImplementedError
         return self.fixed_dates_execution()
