@@ -51,7 +51,7 @@ SCHEMA = [
     ('max_grad_norm', _FLOAT, 50.0, 'Gradient clipping'),
     ('start_date', _INT, 197501, 'First date to train on as YYYYMM'),
     ('end_date', _INT, 199912, 'Last date to train on as YYYYMM'),
-    ('split_date', _INT, None, 'Date to split train/test on.'),
+    ('split_date', _INT, None, 'Date to split train/test on as YYYYMM: the first origin of training_type iterative'),
     ('train', _BOOL, True, 'Train model otherwise inference only'),
     ('dropout', _FLOAT, 0.0, 'Dropout rate for hidden layers'),
     ('recurrent_dropout', _FLOAT, 0.0, 'Dropout rate for recurrent connections'),
@@ -75,7 +75,9 @@ SCHEMA = [
     ('forecast_steps_weights', _STRING, '1.0', 'weights for the forecast steps'),
     ('logging_interval', _INT, 100, 'Number of batches for logging interval during training'),
     ('write_inp_to_out_file', _BOOL, True, 'Write input sequence to the output files'),
-    ('training_type', _STRING, 'fixed_dates', 'Choose between "fixed_dates" and "iterative" training'),
+    ('training_type', _STRING, 'fixed_dates', 'Choose between "fixed_dates" and "iterative" training; "iterative" is a '
+                                              'walk-forward backtest: one model trained through each origin split_date '
+                                              '+ k*stride months, each predicting the stride months after it'),
     ('NPE', _INT, 1, 'Number of Parallel Executions'),
     ('num_procs', _INT, 1, 'Total number of training/prediction processes'),
     ('num_gpu', _INT, 1, 'NUmber of GPUs'),

@@ -2,9 +2,10 @@
 one config in-process.  A point-estimate ensemble (num_procs > 1, :154-199) runs its members in this process too: NPE of
 them at a time, each on its own host thread and CUDA stream, side by side on the GPU(s) (DESIGN.md
 section 6a).  The reference starts one ``lfm_quant.py`` process per member instead (:142).  The candidates of a
-hyper-parameter search generation run the same way (run_candidates, DESIGN.md section 6b).  The ensembles'
-post-processing (utils/post_processing.py) is here too: ensemble_point_estimate, and ensemble_uq_estimate of a UQ
-prediction with Monte-Carlo samples (DESIGN.md section 5c)."""
+hyper-parameter search generation run the same way (run_candidates, DESIGN.md section 6b), and so do the origins of a
+walk-forward backtest (training_type ``iterative``, which the reference leaves unbuilt; DESIGN.md section 6c).  The
+ensembles' post-processing (utils/post_processing.py) is here too: ensemble_point_estimate, and ensemble_uq_estimate of
+a UQ prediction with Monte-Carlo samples (DESIGN.md section 5c)."""
 from __future__ import absolute_import, division, print_function
 
 import copy
@@ -44,6 +45,81 @@ def member_configs(config):
         c.NPE = 1
         members.append(c)
     return experiment_dir, members
+
+
+def add_months(yyyymm, months):
+    """The YYYYMM date `months` months after `yyyymm` (before it when negative)."""
+    m = (yyyymm // 100) * 12 + yyyymm % 100 - 1 + months
+    return (m // 12) * 100 + m % 12 + 1
+
+
+def walk_forward_origins(split_date, end_date, stride):
+    """The origins of a walk-forward backtest (DESIGN.md section 6c): d_0 = split_date, d_k = d_0 + k·stride months,
+    every d_k < end_date.  All dates YYYYMM."""
+    if stride < 1:
+        raise ValueError('--stride %d: walk-forward origins are stride >= 1 months apart' % stride)
+    origins = []
+    while add_months(split_date, len(origins) * stride) < end_date:
+        origins.append(add_months(split_date, len(origins) * stride))
+    return origins
+
+
+def check_walk_forward(config):
+    """Raises ValueError, naming the flag, for a walk-forward config (training_type iterative) that cannot run."""
+    c = config
+    if c.split_date is None or not (1 <= c.split_date % 100 <= 12 and c.start_date < c.split_date < c.end_date):
+        raise ValueError('--split_date %s: training_type iterative needs the first origin, a YYYYMM date strictly '
+                         'between --start_date %s and --end_date %s' % (c.split_date, c.start_date, c.end_date))
+    walk_forward_origins(c.split_date, c.end_date, c.stride)
+    if c.forecast_n > c.stride:
+        # training at origin d keeps windows dated <= d - stride; their targets lie forecast_n months later
+        raise ValueError('--forecast_n %d > --stride %d: the targets of an origin\'s last training windows would lie '
+                         'after the origin' % (c.forecast_n, c.stride))
+    if c.num_procs > 1:
+        raise ValueError('--num_procs %d: training_type iterative trains one model per origin, not an ensemble'
+                         % c.num_procs)
+    if c.cdrs_inference:
+        raise ValueError('--cdrs_inference: training_type iterative backtests on the datafile, not on CDRS data')
+    if c.scalesfile and 'Naive' not in c.nn_type:
+        raise ValueError('--scalesfile %s: with training_type iterative every origin fits scales.dat on its own data '
+                         'and predicts with it' % c.scalesfile)
+    if int(os.environ.get('WORLD_SIZE', '1')) > 1:
+        raise ValueError('torchrun (WORLD_SIZE %s): training_type iterative runs its origins side by side in one '
+                         'process and cannot be combined with data parallelism; run it without torchrun'
+                         % os.environ['WORLD_SIZE'])
+
+
+def origin_configs(config):
+    """The origins of a walk-forward backtest: origin k at d_k runs in <experiments_dir>/<model_dir>/<name>-wf-<d_k>
+    (absolute) as fixed_dates runs with member_id k, default_gpu /gpu:(k mod num_gpu), num_procs = NPE = 1 and the
+    backtest's seed.  Its training keeps start_date and ends at d_k; its prediction covers d_k + 1 month through
+    min(d_k + stride months, end_date).  Returns (<experiments_dir>/<model_dir>, [(d_k, training config, prediction
+    config)])."""
+    assert os.path.isdir(config.experiments_dir), "Experiments dir  %s does not exist" % config.experiments_dir
+    experiment_dir = os.path.join(os.path.abspath(config.experiments_dir), config.model_dir)
+    gpus = cycle(range(config.num_gpu))
+    out = []
+    for k, origin in enumerate(walk_forward_origins(config.split_date, config.end_date, config.stride)):
+        c = copy.deepcopy(config)
+        c.training_type = 'fixed_dates'
+        c.member_id = k
+        c.model_dir = os.path.join(experiment_dir, '%s-wf-%d' % (config.name, origin))
+        c.default_gpu = '/gpu:%d' % next(gpus)
+        c.num_procs = 1
+        c.NPE = 1
+        train, pred = copy.deepcopy(c), c
+        train.train = True
+        train.end_date = origin
+        pred.train = False
+        pred.start_date = add_months(origin, 1)
+        pred.end_date = min(add_months(origin, config.stride), config.end_date)
+        out.append((origin, train, pred))
+    return experiment_dir, out
+
+
+def stitch_walk_forward(frames, origins):
+    """walk_forward_preds.dat: the origins' preds.dat frames in origin order, each row with its origin (YYYYMM)."""
+    return pd.concat([f.assign(origin=o) for f, o in zip(frames, origins)], ignore_index=True)
 
 
 def write_conf(flags, path):
@@ -99,6 +175,15 @@ def _recompute_errors(out, forecast_steps):
         out['abs_err_%d' % s] = err
         out['fcst_err_%d' % s] = err / target.abs()
         out['unscaled_squared_err_%d' % s] = (err / out['seq_norm']) ** 2
+
+
+def _weighted_scaled_mse(df, config):
+    """The mean squared scaled error of a predictions frame, weighted over the forecast steps
+    (model_execution.py:70-72)."""
+    valid_loss = 0
+    for i in range(config.forecast_steps):
+        valid_loss += df['norm_squared_diff_' + str(i + 1)].mean() * config.forecast_steps_weights[i]
+    return valid_loss
 
 
 def _print_scaled_mse(out, forecast_steps):
@@ -251,14 +336,20 @@ class ModelExecution(object):
             raise ValueError('--ig_steps %d: integrated-gradients attributions explain the forecast of a trained '
                              'RNNPointEstimate with forecast_steps = 1 at prediction (--train=False, --UQ=False), with '
                              'ig_steps >= 1 interpolants (0 = off)' % c.ig_steps)
-        if self.config.training_type == 'iterative':
-            raise NotImplementedError
+        if c.training_type == 'iterative':
+            check_walk_forward(c)
+            return self.walk_forward_execution()
         return self.fixed_dates_execution()
 
     @staticmethod
     def read_results(config):
-        """Validation metrics after training, predictions after inference (model_execution.py:31-78)."""
+        """Validation metrics after training, predictions after inference (model_execution.py:31-78).  A walk-forward
+        config (training_type iterative) reads its stitched predictions, walk_forward_preds.dat, after either."""
         try:
+            if config.training_type == 'iterative':
+                df = pd.read_csv(os.path.join(config.experiments_dir, config.model_dir, 'walk_forward_preds.dat'),
+                                 sep=' ', dtype={'gvkey': str})
+                return _weighted_scaled_mse(df, config), None, df
             if config.train:
                 df = pd.read_csv(os.path.join(config.experiments_dir, config.model_dir, 'train_log',
                                               config.name + '-train-logs-epoch.csv'), sep=',')
@@ -266,10 +357,7 @@ class ModelExecution(object):
                 return df.iloc[0]['valid_mse'], None, None
             df = pd.read_csv(os.path.join(config.experiments_dir, config.model_dir, 'pred', config.preds_fname),
                              sep=' ', dtype={'gvkey': str})
-            valid_loss = 0
-            for i in range(config.forecast_steps):
-                valid_loss += df['norm_squared_diff_' + str(i + 1)].mean() * config.forecast_steps_weights[i]
-            return valid_loss, None, df
+            return _weighted_scaled_mse(df, config), None, df
         except FileNotFoundError:
             print("Output file not found")
             return np.inf, np.inf, None
@@ -315,6 +403,57 @@ class ModelExecution(object):
         stream.synchronize()
         return out
 
+    @classmethod
+    def run_members(cls, members, npe):
+        """member_execution of every config in `members`, NPE at a time on host threads of their own.  A member that
+        raises stops the run: members that have not started never start, the running ones finish, then its exception
+        is raised."""
+        npe = max(1, min(int(npe), len(members)))
+        # at most min(NPE, members on that GPU) members run on one GPU at a time: their shares sum to at most 1
+        on_gpu = Counter(m.default_gpu for m in members)
+        with ThreadPoolExecutor(max_workers=npe) as pool:
+            futures = [pool.submit(cls.member_execution, m, min(npe, on_gpu[m.default_gpu])) for m in members]
+            wait(futures, return_when=FIRST_EXCEPTION)
+            failed = [f for f in futures if f.done() and not f.cancelled() and f.exception() is not None]
+            if failed:
+                pool.shutdown(cancel_futures=True)
+                raise failed[0].exception()
+
+    def walk_forward_execution(self):
+        """A walk-forward backtest (training_type iterative, DESIGN.md section 6c): with train True every origin
+        trains (origin_configs), NPE at a time side by side like ensemble members; then, with train True or False,
+        every origin predicts its months the same way.  Writes <experiments_dir>/<model_dir>/walk_forward_preds.dat
+        (stitch_walk_forward) and returns that frame."""
+        cfg = self.config
+        experiment_dir, origins = origin_configs(cfg)
+        if cfg.train:
+            for _, train, _ in origins:
+                write_member_conf(train)
+            self.run_members([train for _, train, _ in origins], cfg.NPE)
+        elif 'Naive' not in cfg.nn_type:          # the naive forecast has no checkpoint to load
+            for origin, _, pred in origins:
+                if not os.path.isdir(pred.model_dir):
+                    raise FileNotFoundError('walk-forward origin %d has no directory %s: train the origins first '
+                                            '(--train=True)' % (origin, pred.model_dir))
+        preds = [pred for _, _, pred in origins]
+        for p in preds:
+            pathlib.Path(p.model_dir).mkdir(parents=True, exist_ok=True)
+            write_conf(p.as_dict(), os.path.join(p.model_dir, 'predict-%d.conf' % p.member_id))
+        self.run_members(preds, cfg.NPE)
+        frames = []
+        for origin, _, pred in origins:
+            path = os.path.join(pred.model_dir, 'pred', cfg.preds_fname)
+            if not os.path.isfile(path):
+                raise RuntimeError('walk-forward origin %d wrote no %s' % (origin, path))
+            if pred.UQ and pred.mc_samples > 1:
+                self.write_uq_ensemble(pred)
+            # read back exactly, so that the stitched rows are the origins' rows as they wrote them
+            frames.append(pd.read_csv(path, sep=' ', dtype={'gvkey': str}, float_precision='round_trip'))
+        df = stitch_walk_forward(frames, [origin for origin, _, _ in origins])
+        df.to_csv(os.path.join(experiment_dir, 'walk_forward_preds.dat'), sep=' ', index=False)
+        _print_scaled_mse(df, cfg.forecast_steps)
+        return df
+
     def point_estimate_ensemble(self):
         """model_execution.py:154-199 in one process.  Training returns every member's best validation MSE, as
         read_results reads it; prediction writes every member's pred/<preds_fname>, then
@@ -327,17 +466,7 @@ class ModelExecution(object):
         experiment_dir, members = member_configs(cfg)
         for m in members:
             write_member_conf(m)
-        npe = max(1, min(int(cfg.NPE), len(members)))
-        # at most min(NPE, members on that GPU) members run on one GPU at a time: their shares sum to at most 1
-        on_gpu = Counter(m.default_gpu for m in members)
-        with ThreadPoolExecutor(max_workers=npe) as pool:
-            futures = [pool.submit(self.member_execution, m, min(npe, on_gpu[m.default_gpu])) for m in members]
-            wait(futures, return_when=FIRST_EXCEPTION)
-            failed = [f for f in futures if f.done() and not f.cancelled() and f.exception() is not None]
-            if failed:
-                # members that have not started never start; the running ones finish before the error is raised
-                pool.shutdown(cancel_futures=True)
-                raise failed[0].exception()
+        self.run_members(members, cfg.NPE)
         results = [self.read_results(m) for m in members]
         if cfg.train:
             return [r[0] for r in results]
