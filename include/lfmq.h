@@ -163,6 +163,18 @@ int32_t lfmq_param_spec(lfmq_handle h, int32_t index, char* name, int32_t name_c
  * weighted uq loss); optimizer slots [n_slots * n_trainable]. */
 enum { LFMQ_TAIL_LOSS = 0, LFMQ_TAIL_MSE0 = 1, LFMQ_TAIL_GRAD_NORM = 2, LFMQ_TAIL_CLIP_SCALE = 3,
        LFMQ_TAIL_UQ_LOSS_LAST_TAR = 4, LFMQ_TAIL_LEN = 8 };   /* grads[n_trainable + LFMQ_TAIL_*] */
+/* Row weights of the training loss (DESIGN.md section 6d).  w_dev: a device vector of at least max_batch floats, each
+ * >= 0 and finite, or NULL (the default) for the unweighted step.  Row b of each later call's batch weighs w_dev[b]: b is
+ * the shard's own row, and row0 does not shift it.  The pointer is kept, not copied: write the next batch's weights
+ * into it on the handle's stream.  Every mean of the training loss becomes a weighted mean (the all-zero-target mask
+ * still multiplies in), so the tail's loss entries are the weighted loss; weights of 1 give the same bits as NULL.
+ * Read by lfmq_backward, lfmq_train_step, lfmq_mask_count, lfmq_mask_count_uq (their counts become {sum of weights,
+ * weighted unmasked rows[, weighted unmasked last-step rows]}, which data parallelism all-reduces as before; with
+ * weights, lfmq_mask_count forms the counts in the handle's own scalar block and copies the first two to out_dev),
+ * lfmq_chain_backward(_dp) and lfmq_chain_mask_count, where each stage reads its own handle's pointer.  No *_loss*
+ * entry point reads it: validation stays unweighted.  A batch whose weights sum to 0 has loss 0 and gradient 0 (a
+ * weighted count of 0 divides as 1).  Recurrent and dense handles; forward_only handles get LFMQ_ERR_UNSUPPORTED. */
+int32_t lfmq_set_row_weights(lfmq_handle h, const float* w_dev);
 int32_t lfmq_params_ptr(lfmq_handle h, float** dev);
 int32_t lfmq_grads_ptr(lfmq_handle h, float** dev);
 int32_t lfmq_opt_state_ptr(lfmq_handle h, float** dev, int64_t* n_elems);
@@ -357,6 +369,14 @@ typedef struct lfmq_gather_args {
   double* seq_norm;
 } lfmq_gather_args;
 int32_t lfmq_gather_batch(const lfmq_gather_args* args, void* stream);
+/* The row weights of one training batch for lfmq_set_row_weights (DESIGN.md section 6d), from the same fp64 table
+ * [n_rows, n_cols] and the batch's input triples inp_idx [B][3] (row 1 of a triple is the window's last input row, its
+ * forecast origin).  w_out[b] = fp32 of the fp64 product of the enabled sources: table[row][weight_col] with NaN as 0
+ * (weight_col >= 0), and 2^(-months / (12 halflife_years)) (halflife_years > 0), where months = ref_month - (12 year +
+ * month) of the yyyymmdd date in table[row][date_col].  At least one source must be enabled. */
+int32_t lfmq_row_weights(const double* table, int64_t n_rows, int32_t n_cols, const int32_t* inp_idx, int32_t B,
+                         int32_t weight_col, int32_t date_col, double halflife_years, int32_t ref_month, float* w_out,
+                         void* stream);
 
 /* Dataset._create_tf_dataset + _append_sequence_data (data_processing.py:170-305) on the device: the window index
  * triples (start, end, pad) of every table row that yields a window, in row order.

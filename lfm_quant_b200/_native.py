@@ -97,6 +97,9 @@ SYMBOLS = {
     'lfmq_chain_backward': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),
     'lfmq_chain_apply': (C.c_int32, [_P, C.c_int32, C.c_float, C.c_int64, _P]),
     'lfmq_mask_count_uq': (C.c_int32, [_P, _P, C.c_int32, _P, _P]),
+    'lfmq_set_row_weights': (C.c_int32, [_P, _P]),
+    'lfmq_row_weights': (C.c_int32, [_P, C.c_int64, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                     C.c_int32, _P, _P]),
     'lfmq_chain_mask_count': (C.c_int32, [_P, C.c_int32, _P, C.c_int32, _P, _P]),
     'lfmq_chain_backward_dp': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P,
                                            _P]),

@@ -230,26 +230,41 @@ __device__ __forceinline__ bool row_mask(const float* y, int n) {
   return any;
 }
 
+// Row weights (lfmq_set_row_weights, DESIGN.md section 6d): window b of a training batch weighs w[b] in every sum of the
+// loss and in every count a mean divides by; without them (w == nullptr) every window weighs 1.  b is the batch's own
+// row, not shifted by row0.  The mask multiplies in: the counts are sums of row_weight * row_mask.
+__device__ __forceinline__ float row_weight(const float* w, long b) { return w ? w[b] : 1.f; }
+
+// A weighted count of 0 (every window of the batch weighs 0) divides as 1: its numerators are 0 too, so the loss and
+// every gradient are 0.  Unweighted counts are used as they are.
+__device__ __forceinline__ float loss_denom(const float* w, float d) { return (w && d == 0.f) ? 1.f : d; }
+
 // dLoss/d(term) of one element of each mean: denom_all and denom_last count the rows the means over every row and over
-// the last step divide by.
+// the last step divide by; w: the batch's row weights (nullable).
 struct LossWeights {
   float all, last, tar;
 };
-__device__ __forceinline__ LossWeights loss_weights(float p1, float p2, int O, float denom_all, float denom_last) {
+__device__ __forceinline__ LossWeights loss_weights(float p1, float p2, int O, float denom_all, float denom_last,
+                                                    const float* w) {
+  denom_all = loss_denom(w, denom_all);
+  denom_last = loss_denom(w, denom_last);
   return {(1.f - p1) * (1.f - p2) / ((float)O * denom_all), (1.f - p1) * p2 / (denom_last * (float)O), p1 / denom_last};
 }
 
-// The squared-error terms of one row of predictions pr (masked by m) against targets y: adds them to s0 (last step,
-// column tidx), s1 (last step) and s2 (every column), and with `train` writes dLoss/dpred to dp.  NCOL > 0: the row is
-// NCOL padded registers, and columns >= O and rows that are not valid contribute exactly zero; NCOL = 0: O columns.
+// The squared-error terms of one row of predictions pr (masked by m) against targets y, times the row's weight rw: adds
+// them to s0 (last step, column tidx), s1 (last step) and s2 (every column), and with `train` writes dLoss/dpred to dp.
+// NCOL > 0: the row is NCOL padded registers, and columns >= O and rows that are not valid contribute exactly zero;
+// NCOL = 0: O columns.  The weight scales the first factor of each product (d rw * d, 2 (d rw) ...): rw = 1 leaves every
+// operand, and so every rounding and every contraction into an FMA, as it is without weights.
 template <int NCOL, typename Acc>
-__device__ __forceinline__ void point_loss_row(const float* pr, const float* y, int O, bool valid, float m, bool last,
-                                               int tidx, const LossWeights& w, bool train, float* dp, Acc& s0, Acc& s1,
-                                               Acc& s2) {
+__device__ __forceinline__ void point_loss_row(const float* pr, const float* y, int O, bool valid, float m, float rw,
+                                               bool last, int tidx, const LossWeights& w, bool train, float* dp,
+                                               Acc& s0, Acc& s1, Acc& s2) {
 #pragma unroll
   for (int k = 0; k < (NCOL > 0 ? NCOL : O); ++k) {
     const float d = (k < O && valid) ? (pr[k] * m - y[k]) : 0.f;  // losses.py:75: masked predictions are zeroed
-    const float d2 = d * d;
+    const float dw = d * rw;
+    const float d2 = dw * d;
     s2 += d2;
     float coef = w.all;
     if (last) {
@@ -260,7 +275,7 @@ __device__ __forceinline__ void point_loss_row(const float* pr, const float* y, 
         coef += w.tar;
       }
     }
-    if (train) dp[k] = 2.f * d * coef * m;
+    if (train) dp[k] = 2.f * dw * coef * m;
   }
 }
 
@@ -270,13 +285,14 @@ __device__ __forceinline__ double weighted_loss(double p1, double p2, double x0,
 
 // The tensor-core heads keep s0 s1 s2 in three consecutive slots of a [value][cta] partial array.  The warp of the first
 // slot, whose sum s0 it holds, sums the other two and writes {loss, mse_0} with the batch denominators {B, unmasked
-// rows} (losses.py:87-98).
+// rows} (losses.py:87-98), or their weighted sums when the batch has row weights rw.
 __device__ __forceinline__ void point_loss_final(const float* __restrict__ slot0, int n_cta, double s0,
-                                                 const float* denom, int O, float p1, float p2, float* out2) {
+                                                 const float* denom, const float* rw, int O, float p1, float p2,
+                                                 float* out2) {
   const double s1 = sum_partials(slot0 + n_cta, 1, n_cta);
   const double s2 = sum_partials(slot0 + 2L * n_cta, 1, n_cta);
   if ((threadIdx.x & 31) == 0 && out2) {
-    const double Bg = denom[0], Mg = denom[1];
+    const double Bg = loss_denom(rw, denom[0]), Mg = loss_denom(rw, denom[1]);
     const double mse0 = s0 / Bg, mse1 = s1 / (Bg * O), mse2 = s2 / (Mg * O);
     out2[0] = (float)weighted_loss(p1, p2, mse0, mse1, mse2);
     out2[1] = (float)mse0;

@@ -103,10 +103,13 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 }
 
 // One row per thread.  pred != nullptr: the row's loss terms {f(r_target), sum_o f(r_o)} and, with dpred, the row's
-// dLoss/dpred; pred == nullptr: the counts {1, mask}.  Writes the block's two sums to part[2 * blockIdx.x].
+// dLoss/dpred; pred == nullptr: the counts {1, mask}.  With row weights rw (nullable) both are multiplied by the row's
+// weight, which scales the first factor of each product (rw = 1 changes no rounding).  Writes the block's two sums to
+// part[2 * blockIdx.x].
 __global__ void __launch_bounds__(kLossThreads) dense_loss_rows(const float* __restrict__ pred,
                                                                   const float* __restrict__ y, int B, int O,
-                                                                  const float* __restrict__ denom, int tidx, float lam,
+                                                                  const float* __restrict__ denom,
+                                                                  const float* __restrict__ rw, int tidx, float lam,
                                                                   int huber, float delta, float* __restrict__ dpred,
                                                                   float* __restrict__ part) {
   __shared__ float red[kLossThreads / 32];
@@ -115,24 +118,25 @@ __global__ void __launch_bounds__(kLossThreads) dense_loss_rows(const float* __r
   if (b < B) {
     const float* yr = y + b * O;
     const float mask = row_mask(yr, O) ? 1.f : 0.f;          // losses.py:69: ~all(y_true == 0)
+    const float wb = row_weight(rw, b);
     if (!pred) {
-      s0 = 1.f;
-      sall = mask;
+      s0 = wb;
+      sall = mask * wb;
     } else {
-      const float bg = denom ? denom[0] : (float)B;
+      const float bg = denom ? loss_denom(rw, denom[0]) : (float)B;
       const float g_all = (1.f - lam) / (bg * (float)O), g_tar = lam / bg;
       for (int o = 0; o < O; ++o) {
         const float r = yr[o] - pred[b * O + o] * mask;     // losses.py:75: predictions of masked rows are zeroed
         const float ar = fabsf(r);
         float f, df;                                         // f(r) and df/dr
         if (huber && ar > delta) {                           // keras Huber: delta * (|r| - delta / 2)
-          f = delta * (ar - 0.5f * delta);
+          f = (delta * wb) * (ar - 0.5f * delta);
           df = copysignf(delta, r);
         } else if (huber) {
-          f = 0.5f * r * r;
+          f = (0.5f * wb) * r * r;
           df = r;
         } else {
-          f = r * r;
+          f = (r * wb) * r;
           df = 2.f * r;
         }
         sall += f;
@@ -141,7 +145,7 @@ __global__ void __launch_bounds__(kLossThreads) dense_loss_rows(const float* __r
           s0 = f;
           g += g_tar;
         }
-        if (dpred) dpred[b * O + o] = -mask * g * df;
+        if (dpred) dpred[b * O + o] = -mask * g * df * wb;
       }
     }
   }
@@ -155,7 +159,8 @@ __global__ void __launch_bounds__(kLossThreads) dense_loss_rows(const float* __r
 
 // Sums the n block partials in a fixed order: out = {loss, mse_0} (or the counts {B, mask}).
 __global__ void __launch_bounds__(kLossThreads) dense_loss_reduce(const float* __restrict__ part, int n, int B, int O,
-                                                                    const float* __restrict__ denom, float lam,
+                                                                    const float* __restrict__ denom,
+                                                                    const float* __restrict__ rw, float lam,
                                                                     int counts, float* __restrict__ out) {
   __shared__ float red[kLossThreads / 32];
   float s0 = 0.f, sall = 0.f;
@@ -171,7 +176,7 @@ __global__ void __launch_bounds__(kLossThreads) dense_loss_reduce(const float* _
     out[1] = sall;
     return;
   }
-  const float bg = denom ? denom[0] : (float)B;
+  const float bg = denom ? loss_denom(rw, denom[0]) : (float)B;
   const float mse0 = s0 / bg, mall = sall / (bg * (float)O);   // masked rows count in both denominators
   out[0] = lam * mse0 + (1.f - lam) * mall;
   out[1] = mse0;
@@ -236,12 +241,12 @@ int dense_forward(cudaStream_t s, const float* x, int B, int K, int O, const flo
 
 size_t dense_loss_scratch(long B) { return 2 * (size_t)((B + kLossThreads - 1) / kLossThreads); }
 
-int dense_loss(cudaStream_t s, const float* pred, const float* y, int B, int O, const float* denom, int tidx, float lam,
-               int huber, float delta, float* dpred, float* out2, float* scratch) {
+int dense_loss(cudaStream_t s, const float* pred, const float* y, int B, int O, const float* denom, const float* rw,
+               int tidx, float lam, int huber, float delta, float* dpred, float* out2, float* scratch) {
   const int nb = (B + kLossThreads - 1) / kLossThreads;
-  dense_loss_rows<<<nb, kLossThreads, 0, s>>>(pred, y, B, O, denom, tidx, lam, huber, delta, dpred, scratch);
+  dense_loss_rows<<<nb, kLossThreads, 0, s>>>(pred, y, B, O, denom, rw, tidx, lam, huber, delta, dpred, scratch);
   LFMQ_LAUNCH_CHECK();
-  dense_loss_reduce<<<1, kLossThreads, 0, s>>>(scratch, nb, B, O, denom, lam, pred ? 0 : 1, out2);
+  dense_loss_reduce<<<1, kLossThreads, 0, s>>>(scratch, nb, B, O, denom, rw, lam, pred ? 0 : 1, out2);
   LFMQ_LAUNCH_CHECK();
   return 0;
 }

@@ -9,10 +9,11 @@ int dense_forward(cudaStream_t s, const float* x, int B, int K, int O, const flo
 // The MLP branch of Losses._get_loss_point_estimate (losses.py:69-75,100-115) over pred, y [B,O]:
 // out2 = {target_lambda * mse_0 + (1 - target_lambda) * mse_all, mse_0}, MSE or (huber != 0) Keras Huber terms.
 // denom (nullable, device) = {B_global}: both means divide by it (mse_all by B_global * O).  dpred (nullable) =
-// dLoss/dpred.  pred == nullptr: out2 = the counts {B, rows whose targets are not all zero}.
-// scratch: dense_loss_scratch(B) floats.
-int dense_loss(cudaStream_t s, const float* pred, const float* y, int B, int O, const float* denom, int tidx, float lam,
-               int huber, float delta, float* dpred, float* out2, float* scratch);
+// dLoss/dpred.  pred == nullptr: out2 = the counts {B, rows whose targets are not all zero}.  rw (nullable): the
+// batch's row weights, which weigh every term and count (the counts become {sum of weights, weighted unmasked rows});
+// with rw and pred, denom is required.  scratch: dense_loss_scratch(B) floats.
+int dense_loss(cudaStream_t s, const float* pred, const float* y, int B, int O, const float* denom, const float* rw,
+               int tidx, float lam, int huber, float delta, float* dpred, float* out2, float* scratch);
 size_t dense_loss_scratch(long B);
 // g[0 : (K+1)*O] = [x^T dpred ; colsum(dpred)]: the kernel gradient [K,O] then the bias gradient [O], through
 // dense_wgrad_scratch(B, K, O) floats of row-block partials summed in a fixed order.

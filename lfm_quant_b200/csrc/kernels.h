@@ -39,9 +39,14 @@ int colsum(cudaStream_t s, long rows, int N, const float* A, float* out, float* 
 int softplus_floor(cudaStream_t s, long n, const float* a, float* var);
 int mask_count(cudaStream_t s, int B, int T, int O, const float* y, float* out2, unsigned int* tickets);
 // out2 = {loss, mse_0}; maskout2 (nullable) = {B, mask_count_local}; dpred may be NULL (validation);
-// denom (nullable) = device {B_global, mask_count_global}.
+// denom (nullable) = device {B_global, mask_count_global}, or their weighted sums when rw (nullable, the batch's row
+// weights, common.cuh row_weight) is given: then denom is required.
+// lfmq_row_weights (include/lfmq.h)
+int row_weights(cudaStream_t s, const double* table, int n_cols, const int* inp_idx, int B, int weight_col,
+                int date_col, double halflife, int ref_month, float* w);
 int loss_grad(cudaStream_t s, int B, int T, int O, const float* pred, const float* y, const float* denom,
-              int target_idx, float p1, float p2, float* dpred, float* out2, float* maskout2, float* scratch);
+              const float* rw, int target_idx, float p1, float p2, float* dpred, float* out2, float* maskout2,
+              float* scratch);
 // scalars[0] = ||g||, scalars[1] = clip scale (1 when clip <= 0)
 int grad_norm_scale(cudaStream_t s, long n, const float* g, float clip, float* scalars, float* scratch,
                     unsigned int* ticket);
@@ -54,6 +59,7 @@ int fill(cudaStream_t s, float* p, long n, float v);
 constexpr int LFMQ_MAX_STAGES = 8;
 struct ChainPtrs { float* p[LFMQ_MAX_STAGES]; };
 struct ChainWeights { float w[LFMQ_MAX_STAGES]; };
+struct ChainCPtrs { const float* p[LFMQ_MAX_STAGES]; };
 int chain_next_input(cudaStream_t s, int B, int T, int F, int O, const float* prev, const float* pred, const float* x0,
                      float* next);
 int scale_inplace(cudaStream_t s, long n, float* p, float w);
@@ -85,8 +91,11 @@ int ig_fold(cudaStream_t s, int B, int M, int64_t r0, int n, long row_elems, con
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and
 // out3 (nullable) = the weighted sums {uq_loss, uq_loss_last_tar, mse}; counts_in = 1 takes the counts from counts.p[s]
 // (required with dpred), else the pass counts its own rows.  dpred / da (nullable) = w_s * dLoss_s / d(pred, apre).
+// rw.p[s] (nullable): stage s's row weights; its counts are then {sum of weights, weighted unmasked rows, weighted
+// unmasked last-step rows}.
 struct ChainUqArgs {
   ChainPtrs pred, var, apre, y, dpred, da, counts, loss, uq0, mse0;
+  ChainCPtrs rw;
   ChainWeights w;
   int counts_in;
 };

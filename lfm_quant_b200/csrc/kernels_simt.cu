@@ -932,12 +932,12 @@ __device__ __forceinline__ void block_reduce4(double v[4], double* out4) {
 
 __global__ void __launch_bounds__(256) loss_rows_kernel(int B, int T, int O, const float* __restrict__ pred,
                                                         const float* __restrict__ y,
-                                                        const float* __restrict__ denom, int target_idx, float p1,
-                                                        float p2, float* __restrict__ dpred,
+                                                        const float* __restrict__ denom, const float* __restrict__ rw,
+                                                        int target_idx, float p1, float p2, float* __restrict__ dpred,
                                                         double* __restrict__ partial) {
   double acc[4] = {0, 0, 0, 0};  // s0, s1, s2, mask count
   LossWeights lw = {0.f, 0.f, 0.f};
-  if (dpred) lw = loss_weights(p1, p2, O, denom[1], denom[0]);
+  if (dpred) lw = loss_weights(p1, p2, O, denom[1], denom[0], rw);
   const long rows = (long)B * T;
   for (long r = (long)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (long)gridDim.x * blockDim.x) {
     const float* yr = y + r * O;
@@ -945,7 +945,7 @@ __global__ void __launch_bounds__(256) loss_rows_kernel(int B, int T, int O, con
     acc[3] += m;
     if (!pred) continue;
     const bool last = ((int)(r % T) == T - 1);
-    point_loss_row<0>(pred + r * O, yr, O, true, m, last, target_idx, lw, dpred != nullptr,
+    point_loss_row<0>(pred + r * O, yr, O, true, m, row_weight(rw, r / T), last, target_idx, lw, dpred != nullptr,
                       dpred ? dpred + r * O : nullptr, acc[0], acc[1], acc[2]);
   }
   block_reduce4(acc, partial + (long)blockIdx.x * 4);
@@ -953,8 +953,8 @@ __global__ void __launch_bounds__(256) loss_rows_kernel(int B, int T, int O, con
 
 // mode 0: maskout = {B, mask_count};  mode 1: out = {loss, mse_0} (+ maskout when given)
 __global__ void loss_final_kernel(int nblk, const double* __restrict__ partial, const float* __restrict__ denom,
-                                  int B, int O, float p1, float p2, int mode, float* __restrict__ out,
-                                  float* __restrict__ maskout) {
+                                  const float* __restrict__ rw, int B, int O, float p1, float p2, int mode,
+                                  float* __restrict__ out, float* __restrict__ maskout) {
   // one warp, fixed summation order (lane-strided then butterfly): deterministic
   double s[4];
   for (int i = 0; i < 4; ++i) s[i] = sum_partials(partial + i, 4, nblk);
@@ -964,8 +964,8 @@ __global__ void loss_final_kernel(int nblk, const double* __restrict__ partial, 
     maskout[1] = (float)s[3];
   }
   if (mode == 0) return;
-  const double Bg = denom ? (double)denom[0] : (double)B;
-  const double Mg = denom ? (double)denom[1] : s[3];
+  const double Bg = denom ? (double)loss_denom(rw, denom[0]) : (double)B;
+  const double Mg = denom ? (double)loss_denom(rw, denom[1]) : s[3];
   const double mse0 = s[0] / Bg, mse1 = s[1] / (Bg * O), mse2 = s[2] / (Mg * O);
   out[0] = (float)weighted_loss(p1, p2, mse0, mse1, mse2);
   out[1] = (float)mse0;
@@ -993,41 +993,48 @@ int softplus_floor(cudaStream_t s, long n, const float* a, float* var) {
 // variance head's pre-activation `apre` (tf.maximum passes the gradient to softplus above the floor), using the counts
 // of a previous pass (or their sums over the data-parallel ranks), both multiplied by the forecast step's weight w
 // (exactly 1 for forecast_steps = 1).  Counts are {B, unmasked rows, unmasked last-step rows}: the denominators of
-// mse_0, of the mean over the mask and of the means over the last step.
+// mse_0, of the mean over the mask and of the means over the last step.  With row weights rw every term and every count
+// of window b is multiplied by rw[b], and the first count is the sum of the weights.
 __device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* __restrict__ pred,
                                              const float* __restrict__ var, const float* __restrict__ apre,
                                              const float* __restrict__ y, const float* __restrict__ counts,
-                                             int target_idx, float p1, float p2, float w, float* __restrict__ dpred,
-                                             float* __restrict__ da, double* __restrict__ partial) {
+                                             const float* __restrict__ rw, int target_idx, float p1, float p2, float w,
+                                             float* __restrict__ dpred, float* __restrict__ da,
+                                             double* __restrict__ partial) {
   double acc[4] = {0, 0, 0, 0};   // uq_0, uq_1, uq_2 numerators, mse_0 numerator
-  double cnt[4] = {0, 0, 0, 0};   // unmasked rows, unmasked last-step rows
+  double cnt[4] = {0, 0, 0, 0};   // unmasked rows, unmasked last-step rows, weight sum (rw only)
   LossWeights lw = {0.f, 0.f, 0.f};
-  if (dpred) lw = loss_weights(p1, p2, O, counts[1], counts[2]);
+  if (dpred) lw = loss_weights(p1, p2, O, counts[1], counts[2], rw);
   const long rows = (long)B * T;
   for (long r = (long)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (long)gridDim.x * blockDim.x) {
     const float* yr = y + r * O;
     const float m = row_mask(yr, O) ? 1.f : 0.f;
     const bool last = ((int)(r % T) == T - 1);
-    cnt[0] += m;
-    if (last) cnt[1] += m;
+    const float wb = row_weight(rw, r / T);
+    const float mw = m * wb;
+    cnt[0] += mw;
+    if (last) {
+      cnt[1] += mw;
+      cnt[2] += wb;
+    }
     if (!pred) continue;
     for (int k = 0; k < O; ++k) {
       const float pm = pred[r * O + k] * m, vm = var[r * O + k] * m;
       const float d = pm - yr[k];
       const float diff = d * d;
-      const float term = diff * (1.f / vm) + logf(vm);
+      const float term = (diff * (1.f / vm) + logf(vm)) * wb;
       acc[2] += term;
       float coef = lw.all;
       if (last) {
         acc[1] += term;
         coef += lw.last;
-        if (k == target_idx) { acc[0] += term; acc[3] += diff; coef += lw.tar; }
+        if (k == target_idx) { acc[0] += term; acc[3] += diff * wb; coef += lw.tar; }
       }
       if (dpred) {
-        dpred[r * O + k] = coef * (2.f * d / vm) * m * w;
+        dpred[r * O + k] = coef * (2.f * d / vm) * m * w * wb;
         const float dv = coef * (-diff / (vm * vm) + 1.f / vm) * m;
         const float a = apre[r * O + k];
-        da[r * O + k] = dv * ((softplus_f(a) > 1e-6f) ? sigmoid_f(a) : 0.f) * w;
+        da[r * O + k] = dv * ((softplus_f(a) > 1e-6f) ? sigmoid_f(a) : 0.f) * w * wb;
       }
     }
   }
@@ -1039,21 +1046,21 @@ __device__ __forceinline__ void uq_loss_rows(int B, int T, int O, const float* _
 // One warp reduces the nblk partial rows of one loss pass.  Lane 0 writes the counts and / or the three scalars
 // {uq_loss, uq_loss_last_tar, mse_0} (any output may be null) and returns them in vals3.
 __device__ __forceinline__ void uq_loss_final(int nblk, const double* __restrict__ partial,
-                                              const float* __restrict__ counts_in, int B, int O, float p1, float p2,
-                                              float* out_loss, float* out_uq0, float* out_mse0, float* counts_out,
-                                              float* vals3) {
+                                              const float* __restrict__ counts_in, const float* __restrict__ rw, int B,
+                                              int O, float p1, float p2, float* out_loss, float* out_uq0,
+                                              float* out_mse0, float* counts_out, float* vals3) {
   const int lane = threadIdx.x & 31;
   double s[8];
   for (int i = 0; i < 8; ++i) s[i] = sum_partials(partial + i, 8, nblk);
   if (lane != 0) return;
   if (counts_out) {
-    counts_out[0] = (float)B;
+    counts_out[0] = rw ? (float)s[6] : (float)B;
     counts_out[1] = (float)s[4];
     counts_out[2] = (float)s[5];
   }
-  const double Bd = counts_in ? (double)counts_in[0] : (double)B;
-  const double ms_all = counts_in ? (double)counts_in[1] : s[4];
-  const double ms_last = counts_in ? (double)counts_in[2] : s[5];
+  const double Bd = counts_in ? (double)loss_denom(rw, counts_in[0]) : (double)B;
+  const double ms_all = counts_in ? (double)loss_denom(rw, counts_in[1]) : s[4];
+  const double ms_last = counts_in ? (double)loss_denom(rw, counts_in[2]) : s[5];
   const double uq0 = s[0] / ms_last, uq1 = s[1] / (ms_last * O), uq2 = s[2] / (ms_all * O);
   vals3[0] = (float)weighted_loss(p1, p2, uq0, uq1, uq2);
   vals3[1] = (float)uq0;
@@ -1069,7 +1076,7 @@ __global__ void __launch_bounds__(256) chain_uq_rows_kernel(int B, int T, int O,
                                                             float p2, double* __restrict__ partial) {
   const int s = blockIdx.y;
   uq_loss_rows(B, T, O, a.pred.p[s], a.var.p[s], a.apre.p[s], a.y.p[s], a.counts_in ? a.counts.p[s] : nullptr,
-               target_idx, p1, p2, a.w.w[s], a.dpred.p[s], a.da.p[s],
+               a.rw.p[s], target_idx, p1, p2, a.w.w[s], a.dpred.p[s], a.da.p[s],
                partial + ((long)s * gridDim.x + blockIdx.x) * 8);
 }
 
@@ -1079,7 +1086,7 @@ __global__ void chain_uq_final_kernel(int S, int nblk, ChainUqArgs a, int B, int
                                       const double* __restrict__ partial, float* __restrict__ out3) {
   __shared__ float vals[LFMQ_MAX_STAGES][3];
   const int s = threadIdx.x >> 5;
-  uq_loss_final(nblk, partial + (long)s * nblk * 8, a.counts_in ? a.counts.p[s] : nullptr, B, O, p1, p2,
+  uq_loss_final(nblk, partial + (long)s * nblk * 8, a.counts_in ? a.counts.p[s] : nullptr, a.rw.p[s], B, O, p1, p2,
                 a.loss.p[s], a.uq0.p[s], a.mse0.p[s], a.counts_in ? nullptr : a.counts.p[s], vals[s]);
   __syncthreads();
   if (threadIdx.x != 0 || !out3) return;
@@ -1145,12 +1152,44 @@ int mask_count(cudaStream_t s, int B, int T, int O, const float* y, float* out2,
   return 0;
 }
 
-int loss_grad(cudaStream_t s, int B, int T, int O, const float* pred, const float* y, const float* denom,
-              int target_idx, float p1, float p2, float* dpred, float* out2, float* maskout2, float* scratch) {
-  double* partial = reinterpret_cast<double*>(scratch);
-  loss_rows_kernel<<<LOSS_BLOCKS, 256, 0, s>>>(B, T, O, pred, y, denom, target_idx, p1, p2, dpred, partial);
+// Row weights of one training batch (DESIGN.md section 6d), computed in fp64 and stored as fp32: window b's weight is
+// the product of the table's weight_col at its last input row (inp_idx[3b + 1]; NaN counts as 0) and, with
+// halflife > 0, 2^(-months / (12 halflife)) with months = ref_month - the month of that row's yyyymmdd date.
+__global__ void row_weights_kernel(const double* __restrict__ table, int n_cols, const int* __restrict__ inp_idx,
+                                   int B, int weight_col, int date_col, double halflife, int ref_month,
+                                   float* __restrict__ w) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const double* row = table + (long)inp_idx[3 * b + 1] * n_cols;
+  double v = 1.0;
+  if (weight_col >= 0) {
+    v = row[weight_col];
+    if (isnan(v)) v = 0.0;
+  }
+  if (halflife > 0.0) {
+    const long ymd = (long)row[date_col];
+    const long months = ref_month - ((ymd / 10000) * 12 + (ymd / 100) % 100);
+    v *= exp2(-(double)months / (12.0 * halflife));
+  }
+  w[b] = (float)v;
+}
+
+int row_weights(cudaStream_t s, const double* table, int n_cols, const int* inp_idx, int B, int weight_col,
+                int date_col, double halflife, int ref_month, float* w) {
+  if (B == 0) return 0;
+  row_weights_kernel<<<cdiv(B, 256), 256, 0, s>>>(table, n_cols, inp_idx, B, weight_col, date_col, halflife, ref_month,
+                                                  w);
   LFMQ_LAUNCH_CHECK();
-  loss_final_kernel<<<1, 32, 0, s>>>(LOSS_BLOCKS, partial, denom, B, O, p1, p2, 1, out2, maskout2);
+  return 0;
+}
+
+int loss_grad(cudaStream_t s, int B, int T, int O, const float* pred, const float* y, const float* denom,
+              const float* rw, int target_idx, float p1, float p2, float* dpred, float* out2, float* maskout2,
+              float* scratch) {
+  double* partial = reinterpret_cast<double*>(scratch);
+  loss_rows_kernel<<<LOSS_BLOCKS, 256, 0, s>>>(B, T, O, pred, y, denom, rw, target_idx, p1, p2, dpred, partial);
+  LFMQ_LAUNCH_CHECK();
+  loss_final_kernel<<<1, 32, 0, s>>>(LOSS_BLOCKS, partial, denom, rw, B, O, p1, p2, 1, out2, maskout2);
   LFMQ_LAUNCH_CHECK();
   return 0;
 }

@@ -522,16 +522,25 @@ int run_stages(const lfmq_handle* st, int S, const float* x, int B, int64_t row0
   return 0;
 }
 
-// Every stage's {B, unmasked rows, unmasked last-step rows} into out_dev[3 * i], in one loss pass without predictions.
+// Every stage's {B, unmasked rows, unmasked last-step rows} into out_dev[3 * i], in one loss pass without predictions;
+// their weighted sums for a stage with row weights.
 int stage_counts(const lfmq_handle* st, int S, const float* const* y, int B, float* out_dev, cudaStream_t s) {
   lfmq::ChainUqArgs a{};
   for (int i = 0; i < S; ++i) {
     a.y.p[i] = const_cast<float*>(y[i]);
     a.counts.p[i] = out_dev + 3 * i;
+    a.rw.p[i] = st[i]->tc.row_w;
   }
   const lfmq_config& c = st[0]->cfg;
   return chain_uq_loss_grad(s, S, B, c.seq_len, c.n_outputs, a, c.target_idx, c.target_lambda, c.rnn_lambda, nullptr,
                             st[0]->scratch);
+}
+
+// A point handle's own batch counts into h->sc->denom: {B, unmasked rows}, or with row weights {sum of weights,
+// weighted unmasked rows} (and a third count), from the weighted count pass of stage_counts.
+int point_counts(lfmq_handle h, const float* y, int B, cudaStream_t s) {
+  if (h->tc.row_w) return stage_counts(&h, 1, &y, B, h->sc->denom, s);
+  return mask_count(s, B, h->cfg.seq_len, h->cfg.n_outputs, y, h->sc->denom, h->sc->mask_tickets);
 }
 
 // The uq loss of the stages' own preds / var (train.py:201-218): one loss pass over all stages for the mask counts
@@ -544,6 +553,7 @@ int stages_loss_uq(const lfmq_handle* st, int S, const float* const* y, const fl
   for (int i = 0; i < S; ++i) {
     a.y.p[i] = const_cast<float*>(y[i]);
     a.counts.p[i] = denom ? const_cast<float*>(denom) + 3 * i : st[i]->sc->denom;
+    a.rw.p[i] = st[i]->tc.row_w;
     a.w.w[i] = weights[i];
   }
   float* scratch = st[0]->scratch;
@@ -581,10 +591,10 @@ int backward_stages(const lfmq_handle* st, int S, const float* x, const float* c
     lfmq_handle h = st[i];
     const lfmq_config& c = h->cfg;
     const float* d = denom ? denom + 3 * i : h->sc->denom;
-    if (!denom) RUN(mask_count(s, B, T, O, y[i], h->sc->denom, h->sc->mask_tickets));
+    if (!denom) RUN(point_counts(h, y[i], B, s));
     float* tail = h->grads + h->n_train;
-    RUN(loss_grad(s, B, T, O, h->preds, y[i], d, c.target_idx, c.target_lambda, c.rnn_lambda, h->dpred, tail, nullptr,
-                  h->scratch));
+    RUN(loss_grad(s, B, T, O, h->preds, y[i], d, h->tc.row_w, c.target_idx, c.target_lambda, c.rnn_lambda, h->dpred,
+                  tail, nullptr, h->scratch));
     if (weights[i] != 1.0f) RUN(scale_inplace(s, (long)B * T * O, h->dpred, weights[i]));
     l2.p[i] = tail;
     w.w[i] = weights[i];
@@ -859,10 +869,10 @@ int32_t lfmq_loss(lfmq_handle h, const float* preds, const float* y, int32_t B, 
   }
   const lfmq_config& c = h->cfg;
   if (h->path == Path::Dense)    // validation: the MSE form whatever huber_loss is (losses.py:102, is_validation=True)
-    return dense_loss((cudaStream_t)stream, preds, y, B, c.n_outputs, nullptr, c.target_idx, c.target_lambda, 0, 1.f,
-                      nullptr, out_dev, h->scratch);
-  return loss_grad((cudaStream_t)stream, B, c.seq_len, c.n_outputs, preds, y, nullptr, c.target_idx, c.target_lambda,
-                   c.rnn_lambda, nullptr, out_dev, nullptr, h->scratch);
+    return dense_loss((cudaStream_t)stream, preds, y, B, c.n_outputs, nullptr, nullptr, c.target_idx, c.target_lambda, 0,
+                      1.f, nullptr, out_dev, h->scratch);
+  return loss_grad((cudaStream_t)stream, B, c.seq_len, c.n_outputs, preds, y, nullptr, nullptr, c.target_idx,
+                   c.target_lambda, c.rnn_lambda, nullptr, out_dev, nullptr, h->scratch);
 }
 
 int32_t lfmq_loss_uq(lfmq_handle h, const float* preds, const float* var, const float* y, int32_t B, float* out_dev,
@@ -889,9 +899,14 @@ int32_t lfmq_mask_count(lfmq_handle h, const float* y, int32_t B, float* out_dev
     return LFMQ_ERR_ARG;
   }
   if (h->path == Path::Dense)
-    return dense_loss((cudaStream_t)stream, nullptr, y, B, h->cfg.n_outputs, nullptr, 0, 0.f, 0, 1.f, nullptr, out_dev,
-                      h->scratch);
-  return mask_count((cudaStream_t)stream, B, h->cfg.seq_len, h->cfg.n_outputs, y, out_dev, h->sc->mask_tickets);
+    return dense_loss((cudaStream_t)stream, nullptr, y, B, h->cfg.n_outputs, nullptr, h->tc.row_w, 0, 0.f, 0, 1.f,
+                      nullptr, out_dev, h->scratch);
+  if (!h->tc.row_w)
+    return mask_count((cudaStream_t)stream, B, h->cfg.seq_len, h->cfg.n_outputs, y, out_dev, h->sc->mask_tickets);
+  RUN(point_counts(h, y, B, (cudaStream_t)stream));     // three counts: the first two are the caller's
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(out_dev, h->sc->denom, 2 * sizeof(float), cudaMemcpyDeviceToDevice,
+                                  (cudaStream_t)stream));
+  return LFMQ_OK;
 }
 
 int32_t lfmq_mask_count_uq(lfmq_handle h, const float* y, int32_t B, float* out_dev, void* stream) {
@@ -902,6 +917,19 @@ int32_t lfmq_mask_count_uq(lfmq_handle h, const float* y, int32_t B, float* out_
   }
   RUN(refuse_dense(h, "lfmq_mask_count_uq"));
   return stage_counts(&h, 1, &y, B, out_dev, (cudaStream_t)stream);
+}
+
+int32_t lfmq_set_row_weights(lfmq_handle h, const float* w_dev) {
+  if (!h) {
+    LFMQ_SET_ERR("lfmq_set_row_weights: null handle");
+    return LFMQ_ERR_ARG;
+  }
+  if (h->cfg.forward_only) {
+    LFMQ_SET_ERR("lfmq_set_row_weights: handle was created forward_only");
+    return LFMQ_ERR_UNSUPPORTED;
+  }
+  h->tc.row_w = w_dev;
+  return LFMQ_OK;
 }
 
 int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, int64_t row0, int64_t step,
@@ -928,7 +956,7 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
     case Path::General: {
       const float* denom = denom_dev;
       if (!denom) {
-        RUN(mask_count(s, B, c.seq_len, c.n_outputs, y, h->sc->denom, h->sc->mask_tickets));
+        RUN(point_counts(h, y, B, s));
         denom = h->sc->denom;
       }
       if (h->path == Path::Cluster)
@@ -944,8 +972,13 @@ int32_t lfmq_backward(lfmq_handle h, const float* x, const float* y, int32_t B, 
   RUN(dense_forward(s, x, B, K, O, h->params + h->pl.oWo, h->params + h->pl.obo, h->preds));
   h->prof.end(LFMQ_REGION_FWD, s);
   h->prof.begin(LFMQ_REGION_HEAD, s);
-  RUN(dense_loss(s, h->preds, y, B, O, denom_dev, c.target_idx, c.target_lambda, h->huber, h->huber_delta, h->dpred,
-                 tail, h->scratch));
+  const float* denom = denom_dev;
+  if (!denom && h->tc.row_w) {    // the weighted means divide by the batch's weight sum
+    RUN(dense_loss(s, nullptr, y, B, O, nullptr, h->tc.row_w, 0, 0.f, 0, 1.f, nullptr, h->sc->denom, h->scratch));
+    denom = h->sc->denom;
+  }
+  RUN(dense_loss(s, h->preds, y, B, O, denom, h->tc.row_w, c.target_idx, c.target_lambda, h->huber, h->huber_delta,
+                 h->dpred, tail, h->scratch));
   h->prof.end(LFMQ_REGION_HEAD, s);
   h->prof.begin(LFMQ_REGION_WGRAD, s);
   RUN(dense_wgrad(s, x, h->dpred, B, K, O, h->wpart, h->grads));
@@ -1547,6 +1580,18 @@ int32_t lfmq_gather_batch(const lfmq_gather_args* a, void* stream) {
   g.fin_cols = a->fin_cols; g.center = a->center; g.scale = a->scale; g.scale_flag = a->scale_flag;
   g.aux_flag = a->aux_flag; g.x = a->x; g.y = a->y; g.seq_norm = a->seq_norm;
   return gather_batch((cudaStream_t)stream, g);
+}
+
+int32_t lfmq_row_weights(const double* table, int64_t n_rows, int32_t n_cols, const int32_t* inp_idx, int32_t B,
+                         int32_t weight_col, int32_t date_col, double halflife_years, int32_t ref_month, float* w_out,
+                         void* stream) {
+  if (!table || !inp_idx || !w_out || B < 0 || n_rows <= 0 || n_cols <= 0 || weight_col >= n_cols ||
+      date_col < 0 || date_col >= n_cols || halflife_years < 0.0 || (weight_col < 0 && halflife_years == 0.0)) {
+    LFMQ_SET_ERR("lfmq_row_weights: null pointer, bad column, negative half-life or no weight source");
+    return LFMQ_ERR_ARG;
+  }
+  return row_weights((cudaStream_t)stream, table, n_cols, inp_idx, B, weight_col, date_col, halflife_years, ref_month,
+                     w_out);
 }
 
 int32_t lfmq_unscale(const float* in, float* out, int64_t n_rows, int32_t O, const double* scale, const double* center,

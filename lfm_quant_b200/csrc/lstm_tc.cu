@@ -414,6 +414,7 @@ struct HeadParams {
   const float *Wo, *bo;
   const float* y;
   const float* denom;
+  const float* rw;      // row weights of the training batch (nullable)
   float p1, p2;
   int use_dropout;
   DropoutKey key;
@@ -463,7 +464,7 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
   }
   __syncthreads();
   LossWeights lw = {0.f, 0.f, 0.f};
-  if (TRAIN) lw = loss_weights(p.p1, p.p2, p.O, p.denom[1], p.denom[0]);
+  if (TRAIN) lw = loss_weights(p.p1, p.p2, p.O, p.denom[1], p.denom[0], p.rw);
   float s0 = 0.f, s1 = 0.f, s2 = 0.f;
   float accbo[TC_OPAD];
 #pragma unroll
@@ -520,8 +521,9 @@ __global__ void __launch_bounds__(128, 2) head_rows_kernel(HeadParams p, const _
     }
     if (p.y) {
       const float mk = (row_mask(yt, TC_OPAD) && valid) ? 1.f : 0.f;
+      const float wb = valid ? row_weight(p.rw, b) : 0.f;
       float dp[TC_OPAD] = {};
-      point_loss_row<TC_OPAD>(pr, yt, p.O, valid, mk, t == p.T - 1, p.target_idx, lw, TRAIN, dp, s0, s1, s2);
+      point_loss_row<TC_OPAD>(pr, yt, p.O, valid, mk, wb, t == p.T - 1, p.target_idx, lw, TRAIN, dp, s0, s1, s2);
       if (TRAIN) {
 #pragma unroll
         for (int k = 0; k < TC_OPAD; ++k) accbo[k] += dp[k];
@@ -745,7 +747,7 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
     const int mrow = tid;                   // row of the tile this thread owns
     const int fw = warp, cq = lane & 3;     // accumulator fragment: rows 16 fw + lane / 4 (+ 8) of each 64-row half
     LossWeights lw = {0.f, 0.f, 0.f};
-    if (TRAIN) lw = loss_weights(p.p1, p.p2, p.O, p.denom[1], p.denom[0]);
+    if (TRAIN) lw = loss_weights(p.p1, p.p2, p.O, p.denom[1], p.denom[0], p.rw);
     float bop[TC_OPAD];
 #pragma unroll
     for (int k = 0; k < TC_OPAD; ++k) bop[k] = w.bop[k];
@@ -810,8 +812,9 @@ __global__ void __launch_bounds__(HT_THREADS, 2)
       }
       if (p.y) {
         const float mk = (row_mask(yt, TC_OPAD) && valid) ? 1.f : 0.f;
+        const float wb = valid ? row_weight(p.rw, b) : 0.f;
         float dp[TC_OPAD] = {};
-        point_loss_row<TC_OPAD>(pr, yt, p.O, valid, mk, t == p.T - 1, p.target_idx, lw, TRAIN, dp, s0, s1, s2);
+        point_loss_row<TC_OPAD>(pr, yt, p.O, valid, mk, wb, t == p.T - 1, p.target_idx, lw, TRAIN, dp, s0, s1, s2);
         if (TRAIN) {
 #pragma unroll
           for (int k = 0; k < TC_OPAD; ++k) accbo[k] += dp[k];
@@ -950,8 +953,8 @@ __global__ void __launch_bounds__(256, 2) head_wgrad_kernel(HeadParams p, float*
 // Sums the per-CTA head partials (stored [value][cta]: one warp per value, lanes over CTAs, fixed order) and
 // scatters them into the flat gradient vector / loss tail.  wpartial is [cta][256*16].
 __global__ void head_reduce_kernel(int n_cta, const float* __restrict__ partial, int n_wcta,
-                                   const float* __restrict__ wpartial, int O, int B, const float* denom, float p1,
-                                   float p2, int train, float* __restrict__ gWo, float* __restrict__ gbo,
+                                   const float* __restrict__ wpartial, int O, int B, const float* denom,
+                                   const float* rw, float p1, float p2, int train, float* __restrict__ gWo, float* __restrict__ gbo,
                                    float* __restrict__ ggamma, float* __restrict__ gbeta, float* __restrict__ out2) {
   pdl_sync();
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // one warp per output value
@@ -974,7 +977,7 @@ __global__ void head_reduce_kernel(int n_cta, const float* __restrict__ partial,
     const int k = q - 2 * TC_H;
     if (train && lane == 0 && k < O) gbo[k] = (float)s;
   } else if (q == 2 * TC_H + TC_OPAD) {
-    point_loss_final(partial + (long)q * n_cta, n_cta, s, denom, O, p1, p2, out2);
+    point_loss_final(partial + (long)q * n_cta, n_cta, s, denom, rw, O, p1, p2, out2);
   }
 }
 
@@ -1594,6 +1597,7 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const ParamLayout& pl,
   h.eps = c.bn_epsilon;
   h.Wo = params + pl.oWo; h.bo = params + pl.obo;
   h.y = y; h.denom = denom; h.p1 = c.target_lambda; h.p2 = c.rnn_lambda;
+  h.rw = train ? st.row_w : nullptr;
   h.use_dropout = m.dropout_head ? 1 : 0;
   h.key = dropout_key(c.seed, 0, step, c.dropout);
   h.row0 = row0;
@@ -1635,7 +1639,7 @@ static int tc_run_head(TcState& st, const lfmq_config& c, const ParamLayout& pl,
   if (y) {
     const int n_out = HWG_PART + HEAD_PART;
     if (int rc = launch_pdl(head_reduce_kernel, dim3((n_out * 32 + 255) / 256), dim3(256), 0, s, 1, true, grid,
-                            (const float*)m.head_part, n_wcta, (const float*)m.head_wpart, m.O, B, denom, c.target_lambda,
+                            (const float*)m.head_part, n_wcta, (const float*)m.head_wpart, m.O, B, denom, h.rw, c.target_lambda,
                             c.rnn_lambda, train ? 1 : 0, grads ? grads + pl.oWo : (float*)nullptr,
                             grads ? grads + pl.obo : (float*)nullptr, grads ? grads + o.ogamma : (float*)nullptr,
                             grads ? grads + o.obeta : (float*)nullptr, out2))

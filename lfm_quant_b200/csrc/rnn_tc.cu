@@ -115,6 +115,7 @@ struct EpiParams {
   // head (EPI_HEAD): pred = y Wo + bo, weighted MSE (losses.py:55-135), dLoss/dpred
   const float* hy;              // targets [B][T][O] fp32 or null
   const float* hdenom;          // {B_global, mask_count_global}
+  const float* hrw;             // row weights of the training batch (nullable)
   const float* hbo;             // [O]
   float* hpreds;                // [B][T][O] fp32 or null
   __nv_bfloat16* hdpb;          // [T*Bp][64] bf16, cols >= 16 stay zero: dLoss/dpred rows (operand of the dy and dWo GEMMs)
@@ -431,11 +432,12 @@ __device__ __forceinline__ void epi_head(const EpiParams& p, const float (&acc)[
     for (int k = 0; k < p.hO; ++k) p.hpreds[r * p.hO + k] = pr[k];
   if (!p.hy) return;
   LossWeights lw = {0.f, 0.f, 0.f};
-  if (p.htrain) lw = loss_weights(p.hp1, p.hp2, p.hO, p.hdenom[1], p.hdenom[0]);
+  if (p.htrain) lw = loss_weights(p.hp1, p.hp2, p.hO, p.hdenom[1], p.hdenom[0], p.hrw);
   const float mk = (row_mask(yt, GH_O) && valid) ? 1.f : 0.f;
+  const float wb = valid ? row_weight(p.hrw, b) : 0.f;
   float s0 = 0.f, s1 = 0.f, s2 = 0.f;
   float dp[GH_O] = {};
-  point_loss_row<GH_O>(pr, yt, p.hO, valid, mk, t == p.T - 1, p.htarget, lw, p.htrain, dp, s0, s1, s2);
+  point_loss_row<GH_O>(pr, yt, p.hO, valid, mk, wb, t == p.T - 1, p.htarget, lw, p.htrain, dp, s0, s1, s2);
   if (p.htrain) {       // every row of the tile is written (zeros beyond the batch): the dy / dWo GEMMs run over all rows
     uint32_t w[8];
 #pragma unroll
@@ -988,8 +990,9 @@ __global__ void __launch_bounds__(128, 1) ghead_rows_kernel(GHeadParams p, const
 }
 
 // Sums the tensor-core head's per-tile partials: loss terms -> {loss, mse_0}, dbo.
-__global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial, int O, const float* denom, float p1,
-                                    float p2, int train, float* __restrict__ gbo, float* __restrict__ out2) {
+__global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial, int O, const float* denom,
+                                    const float* rw, float p1, float p2, int train, float* __restrict__ gbo,
+                                    float* __restrict__ out2) {
   const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // one warp per output value
   const int lane = threadIdx.x & 31;
   if (q >= GH_PART) return;
@@ -997,7 +1000,7 @@ __global__ void ghead_reduce_kernel(int n_cta, const float* __restrict__ partial
   if (q < GH_O) {
     if (train && lane == 0 && q < O) gbo[q] = (float)s;
   } else if (q == GH_O) {
-    point_loss_final(partial + (long)q * n_cta, n_cta, s, denom, O, p1, p2, out2);
+    point_loss_final(partial + (long)q * n_cta, n_cta, s, denom, rw, O, p1, p2, out2);
   }
 }
 
@@ -1393,7 +1396,7 @@ static int gen_run_head(TcState& st, const lfmq_config& c, const ParamLayout& pl
   const int ntile = m.T * m.NRT;                  // every row tile of the time-major buffers (zeros beyond the batch)
   EpiParams ep = {};
   ep.T = m.T; ep.B = B; ep.Bp = m.Bp; ep.H = m.H; ep.NRT = m.NRT; ep.NB16 = m.NB16;
-  ep.hy = y; ep.hdenom = denom; ep.hbo = params + pl.obo; ep.hpreds = preds; ep.hdpb = m.dpb;
+  ep.hy = y; ep.hdenom = denom; ep.hrw = train ? st.row_w : nullptr; ep.hbo = params + pl.obo; ep.hpreds = preds; ep.hdpb = m.dpb;
   ep.hpartial = m.head_tc_part; ep.hp1 = c.target_lambda; ep.hp2 = c.rnn_lambda; ep.hO = m.O;
   ep.htarget = c.target_idx; ep.htrain = train ? 1 : 0;
   GArgs g = {};
@@ -1428,7 +1431,8 @@ static int gen_run_head(TcState& st, const lfmq_config& c, const ParamLayout& pl
     LFMQ_LAUNCH_CHECK();
   }
   if (y) {
-    ghead_reduce_kernel<<<(GH_PART * 32 + 255) / 256, 256, 0, s>>>(ntile, m.head_tc_part, m.O, denom, c.target_lambda,
+    ghead_reduce_kernel<<<(GH_PART * 32 + 255) / 256, 256, 0, s>>>(ntile, m.head_tc_part, m.O, denom, ep.hrw,
+                                                                  c.target_lambda,
                                                                   c.rnn_lambda, train ? 1 : 0,
                                                                   grads ? grads + pl.obo : nullptr, out2);
     LFMQ_LAUNCH_CHECK();

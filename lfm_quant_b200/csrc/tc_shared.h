@@ -32,6 +32,7 @@ struct TcState {
   int share_num = 1;            // lfmq_set_device_share: the fraction of the SMs this handle may count on for the
   int share_den = 1;            // co-residency of a persistent launch (persistent_cta_budget)
   Profiler* prof = nullptr;
+  const float* row_w = nullptr; // lfmq_set_row_weights: the training batch's row weights, read by the head's loss
   TcImpl* impl = nullptr;       // cluster path
   GenImpl* gen = nullptr;       // general path
 };

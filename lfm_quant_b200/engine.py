@@ -131,6 +131,17 @@ class _HandleEngine(object):
         N.check(self.lib.lfmq_mask_count(self.handle, _ptr(y), y.shape[0], _ptr(out), _stream()))
         return out
 
+    def set_row_weights(self, w):
+        """Row weights of the training loss (lfmq_set_row_weights, DESIGN.md section 6d): w is a contiguous CUDA fp32
+        tensor of at least max_batch entries, and row b of every later training batch weighs w[b]; None restores the
+        unweighted step.  The handle keeps the pointer, so the engine keeps w alive and the caller may refill it in
+        place between steps."""
+        if w is not None:
+            assert w.dtype == torch.float32 and w.is_cuda and w.is_contiguous(), 'row weights: a CUDA fp32 vector'
+            assert w.numel() >= self.cfg.max_batch, (w.numel(), self.cfg.max_batch)
+        N.check(self.lib.lfmq_set_row_weights(self.handle, _ptr(w)))
+        self.row_weights = w
+
     def apply(self, lr, iteration):
         N.check(self.lib.lfmq_apply(self.handle, float(lr), int(iteration), _stream()))
 
@@ -486,6 +497,11 @@ class ForecastChainEngine(object):
         for e in self.stages:
             e.set_device_share(num, den)
 
+    def set_row_weights(self, w):
+        """_HandleEngine.set_row_weights for every stage: each stage's loss weighs row b of the batch by w[b]."""
+        for e in self.stages:
+            e.set_row_weights(w)
+
     def _ptrs(self, tensors):
         return (C.c_void_p * self.S)(*[t.data_ptr() for t in tensors])
 
@@ -704,6 +720,10 @@ class HostBatchPipeline(object):
         for i, (x_pinned, y_pinned) in enumerate(batches):
             loss_mse = pipe.step(x_pinned, y_pinned, i, lr)     # host tensor of the PREVIOUS step (None at i=0)
         last = pipe.finish()
+
+    Row weights (DESIGN.md section 6d): pass each batch's fp32 host weights as `w_host` (and as the third entry of
+    `next_batch`); they are staged with the batch into a device vector of max_batch entries and set on the engine for
+    the step that reads the batch.
     """
 
     def __init__(self, engine, batch, step_fn=None):
@@ -716,32 +736,41 @@ class HostBatchPipeline(object):
         self.consumed = [torch.cuda.Event() for _ in range(2)]
         self.out_host = [torch.empty(2, dtype=torch.float32).pin_memory() for _ in range(2)]
         self.out_ready = [torch.cuda.Event() for _ in range(2)]
+        self.w = [None, None]
         self.step_fn = step_fn or (lambda x, y, i, lr: engine.train_step(x, y, i, lr))
         self.n = 0
         self._staged = None
 
-    def _stage(self, x_host, y_host, slot):
+    def _stage(self, x_host, y_host, slot, w_host=None):
         with torch.cuda.stream(self.copy_stream):
             if self.n >= 2:
                 self.copy_stream.wait_event(self.consumed[slot])      # the step that used this buffer is done
             self.x[slot].copy_(x_host, non_blocking=True)
             self.y[slot].copy_(y_host, non_blocking=True)
+            if w_host is not None:
+                if self.w[slot] is None:
+                    self.w[slot] = torch.zeros(self.eng.cfg.max_batch, dtype=torch.float32, device=self.x[slot].device)
+                self.w[slot][w_host.shape[0]:].zero_()
+                self.w[slot][:w_host.shape[0]].copy_(w_host, non_blocking=True)
             self.copied[slot].record(self.copy_stream)
 
-    def step(self, x_host, y_host, index, lr, next_batch=None):
-        """Runs one step on (x_host, y_host); `next_batch` (optional) is staged while it computes."""
+    def step(self, x_host, y_host, index, lr, next_batch=None, w_host=None):
+        """Runs one step on (x_host, y_host[, row weights w_host]); `next_batch` (optional) is staged while it
+        computes."""
         slot = self.n & 1
         if self._staged != self.n:
-            self._stage(x_host, y_host, slot)
+            self._stage(x_host, y_host, slot, w_host)
         cur = torch.cuda.current_stream()
         cur.wait_event(self.copied[slot])
+        if w_host is not None:
+            self.eng.set_row_weights(self.w[slot])
         out = self.step_fn(self.x[slot], self.y[slot], index, lr)
         self.consumed[slot].record(cur)
         self.out_host[slot].copy_(out, non_blocking=True)
         self.out_ready[slot].record(cur)
         self.n += 1
         if next_batch is not None:
-            self._stage(next_batch[0], next_batch[1], self.n & 1)
+            self._stage(next_batch[0], next_batch[1], self.n & 1, next_batch[2] if len(next_batch) > 2 else None)
             self._staged = self.n
         prev = None
         if self.n >= 2:
@@ -786,6 +815,19 @@ def gather_batch(table, inp_idx, tar_idx, *, seq_len, stride, inp_cols, fin_cols
     a.x, a.y, a.seq_norm = x.data_ptr(), y.data_ptr(), sn.data_ptr()
     N.check(lib.lfmq_gather_batch(C.byref(a), _stream()))
     return x, y, sn
+
+
+def row_weights(table, inp_idx, *, weight_col, date_col, halflife, ref_month, out=None):
+    """Device row weights of one training batch (lfmq_row_weights, DESIGN.md section 6d): table f64 [n_rows, n_cols] and
+    inp_idx int32 [B, 3] CUDA tensors; weight_col < 0 turns the field source off, halflife = 0 the recency source.
+    Returns fp32 [B] (or fills out[:B])."""
+    for name, t, dt in (('table', table, torch.float64), ('inp_idx', inp_idx, torch.int32)):
+        assert t.is_cuda and t.dtype == dt and t.is_contiguous(), name
+    B = inp_idx.shape[0]
+    w = torch.empty(B, dtype=torch.float32, device=table.device) if out is None else out
+    N.check(N.load().lfmq_row_weights(_ptr(table), table.shape[0], table.shape[1], _ptr(inp_idx), B, int(weight_col),
+                                      int(date_col), float(halflife), int(ref_month), _ptr(w), _stream()))
+    return w
 
 
 def window_index(key_codes, active, dates, *, train, stride, forecast_n, min_unrollings, max_unrollings, start_date,

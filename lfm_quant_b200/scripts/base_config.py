@@ -110,6 +110,12 @@ SCHEMA = [
                             "UQ ensemble's ensemble_preds.dat with the calibrated lower bounds"),
     ('ig_steps', _INT, 0, 'Integrated-gradients interpolants per window at point-estimate prediction; more than 0 also '
                           'writes pred/attributions.npz: which input fields and quarters drive each forecast'),
+    ('sample_weight_field', _STRING, None, 'Datafile column that weighs each training window in the training loss, read '
+                                         'raw at the window\'s last input row (NaN counts as 0; negative or infinite '
+                                         'values are refused); unset = off.  Ignored with --train=False'),
+    ('recency_halflife', _FLOAT, 0.0, 'Half-life in years of a recency weight 2^(-months / (12 Y)) on each training '
+                                      'window, months counted back from the latest last-input date of the training '
+                                      'set (per walk-forward origin); 0 = off.  Ignored with --train=False'),
 ]
 
 _DEFINERS = {_STRING: configs.DEFINE_string, _INT: configs.DEFINE_integer, _FLOAT: configs.DEFINE_float,

@@ -123,7 +123,26 @@ class Dataset(object):
         self._cols_offset = 3
         if self.config.scale_field in self.data.columns and self.config.scale_field not in self._cols:
             self._cols.append(self.config.scale_field)
+        # row weights of the training loss (DESIGN.md section 6d); ignored at prediction
+        wfield = getattr(self.config, 'sample_weight_field', '') if self.config.train else ''
+        self.recency_halflife = float(getattr(self.config, 'recency_halflife', 0.0)) if self.config.train else 0.0
+        if self.recency_halflife < 0:
+            raise ValueError('--recency_halflife %g: the half-life is in years, > 0 (0 = off)' % self.recency_halflife)
+        if wfield:
+            if wfield not in self.data.columns or wfield in ('date', 'gvkey'):
+                raise ValueError('--sample_weight_field %s: not a numeric column of %s' % (wfield, self.config.datafile))
+            vals = self.data[wfield].values.astype(np.float64)
+            bad = np.flatnonzero((vals < 0) | np.isinf(vals))
+            if bad.size:
+                r = bad[0]
+                raise ValueError('--sample_weight_field %s: %g at date %s, gvkey %s; weights must be >= 0 and finite '
+                                 '(NaN counts as 0)' % (wfield, vals[r], self.data['date'].iloc[r].strftime('%Y%m%d'),
+                                                       self.data['gvkey'].iloc[r]))
+            if wfield not in self._cols:
+                self._cols.append(wfield)
         self.data = self.data[self._cols]
+        self._weight_col = self._cols.index(wfield) if wfield else -1
+        self.ref_month = None
         self._gvkey_idx = self._cols.index(self.config.key_field)
         self._date_idx = self._cols.index(self.config.date_field)
         self._active_idx = self._cols.index(self.config.active_field)
@@ -166,7 +185,48 @@ class Dataset(object):
             assert os.path.isfile(scales_path), "scalesfile not provided. Ensure to use the same scalesfile as used " \
                                                 "during training "
             self.scaling_params = pickle.load(open(scales_path, 'rb'))
+        if self.recency_halflife > 0:
+            # the recency reference: the latest last-input month of this run's training windows (so per walk-forward
+            # origin, whose run ends at its own origin)
+            self.ref_month = int(np.max(self._months(self._dataset['train_X'][:, 1]))) \
+                if len(self._dataset['train_X']) else 0
         self._dev = None
+
+    # ---- row weights of the training loss (DESIGN.md section 6d) --------------------------------------------------
+    @property
+    def row_weighted(self):
+        return self._weight_col >= 0 or self.recency_halflife > 0
+
+    def _months(self, rows):
+        ymd = self.table[rows, self._date_idx].astype(np.int64)
+        return (ymd // 10000) * 12 + (ymd // 100) % 100
+
+    def row_weights_host(self, inp_indices):
+        """The NumPy form of lfmq_row_weights: fp32 [B] weights of the windows inp_indices [B, 3], computed in fp64 --
+        the sample_weight_field value at the window's last input row (NaN -> 0) times 2^(-months / (12 Y))."""
+        rows = np.asarray(inp_indices)[:, 1].astype(np.int64)
+        v = np.ones(rows.size, dtype=np.float64)
+        if self._weight_col >= 0:
+            v = self.table[rows, self._weight_col].copy()
+            v[np.isnan(v)] = 0.0
+        if self.recency_halflife > 0:
+            months = (self.ref_month - self._months(rows)).astype(np.float64)
+            v = v * np.exp2(-months / (12.0 * self.recency_halflife))
+        return v.astype(np.float32)
+
+    def row_weights(self, inp_indices, length=None):
+        """The same weights computed on the GPU from the resident table (lfmq_row_weights): a CUDA fp32 vector of
+        max(B, length) entries, zero beyond B."""
+        import torch
+        from ..engine import row_weights
+        d = self._device_state()
+        B = len(inp_indices)
+        out = torch.zeros(max(B, length or 0), dtype=torch.float32, device=d['table'].device)
+        if B:
+            inp_idx = torch.from_numpy(np.ascontiguousarray(inp_indices, dtype=np.int32)).cuda()
+            row_weights(d['table'], inp_idx, weight_col=self._weight_col, date_col=self._date_idx,
+                        halflife=self.recency_halflife, ref_month=self.ref_month or 0, out=out)
+        return out
 
     def _create_index(self):
         """Vectorised data_processing.py:170-305 (_create_tf_dataset + _append_sequence_data)."""

@@ -320,6 +320,16 @@ def run_candidates(conf_paths, npe):
     return errors
 
 
+def check_row_weights(c):
+    """The refusals of --sample_weight_field / --recency_halflife that need no data (DESIGN.md section 6d); the field's
+    values are checked when the dataset loads."""
+    if getattr(c, 'recency_halflife', 0.0) < 0:
+        raise ValueError('--recency_halflife %g: the half-life is in years, > 0 (0 = off)' % c.recency_halflife)
+    weighted = bool(getattr(c, 'sample_weight_field', '')) or getattr(c, 'recency_halflife', 0.0) > 0
+    if weighted and c.train and 'Naive' in c.nn_type:
+        raise ValueError('--sample_weight_field / --recency_halflife: %s has nothing to train' % c.nn_type)
+
+
 class ModelExecution(object):
 
     def __init__(self, config):
@@ -336,6 +346,7 @@ class ModelExecution(object):
             raise ValueError('--ig_steps %d: integrated-gradients attributions explain the forecast of a trained '
                              'RNNPointEstimate with forecast_steps = 1 at prediction (--train=False, --UQ=False), with '
                              'ig_steps >= 1 interpolants (0 = off)' % c.ig_steps)
+        check_row_weights(c)
         if c.training_type == 'iterative':
             check_walk_forward(c)
             return self.walk_forward_execution()

@@ -72,21 +72,30 @@ class Train(object):
         self._valid_batches = [self.dataset.get_batch(*items) for items in self.valid_set]
 
     def _build_train_batch(self, items):
-        """(inp, target, metadata[, row0, global denominators]) of one global batch; the shard of this rank under DP.
-        The denominators: {B, mask count} of the point estimate; the uq loss's {B, mask count, last-step mask count};
-        with forecast_steps > 1 those three per forecast stage."""
+        """(inp, target, metadata[, row0, global denominators][, row weights]) of one global batch; the shard of this
+        rank under DP.  The denominators: {B, mask count} of the point estimate; the uq loss's {B, mask count, last-step
+        mask count}; with forecast_steps > 1 those three per forecast stage -- their weighted sums with row weights
+        (--sample_weight_field / --recency_halflife, DESIGN.md section 6d), a device vector of the batch's weights,
+        zero-padded to the engine's max_batch."""
+        eng = self.model.engine
+        weighted = self.dataset.row_weighted
         if self.world == 1:
-            return self.dataset.get_batch(*items)
+            batch = self.dataset.get_batch(*items)
+            if not weighted:
+                return batch
+            return tuple(batch) + (0, None, self.dataset.row_weights(items[0], eng.cfg.max_batch))
         import torch.distributed as dist
         from .. import dp as _dp
         inp_idx, tar_idx, meta, row0 = _dp.shard_batch_indices(items[0], items[1], items[2], self.rank, self.world)
-        eng = self.model.engine
-        x = y = md = None
+        x = y = md = w = None
         if len(inp_idx) > 0:                     # else fewer windows than ranks: this rank only joins the collectives
             x, y, md = self.dataset.get_batch(inp_idx, tar_idx, meta)
+        if weighted:                             # the counts below read the handles' weights
+            w = self.dataset.row_weights(inp_idx, eng.cfg.max_batch)
+            eng.set_row_weights(w)
         # loss denominators are global (losses.py:87,90,131-135); a rank without rows adds zeros
         denom = _dp.global_denominators(eng.loss_counts(None if y is None else self._step_targets(y)), dist)
-        return (x, y, md, row0, denom)
+        return (x, y, md, row0, denom) + ((w,) if weighted else ())
 
     def train(self):
         if self.config.load_saved_weights:
@@ -154,6 +163,8 @@ class Train(object):
         inp = cur_batch[0]
         ys = None if inp is None else self._step_targets(cur_batch[1])
         lr, it = self.optimizer.current_lr(), self.optimizer.iterations
+        if len(cur_batch) > 5:                  # row weights: the batch's own vector for this step
+            self.model.engine.set_row_weights(cur_batch[5])
         if self.world > 1:
             out = self.model.train_step_dp(inp, ys, it, lr, cur_batch[3], cur_batch[4])
         else:
