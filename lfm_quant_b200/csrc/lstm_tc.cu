@@ -21,7 +21,8 @@
 //
 // Forward recurrence = ONE persistent kernel (lstm_fwd_tc_kernel<SAVE, 128>): clusters of 4 CTAs, one 128-row batch
 // tile per cluster, all clusters co-resident (a last round that fits as 64-row half tiles is a second launch, of
-// lstm_fwd_tc_kernel<SAVE, 64>, see tc_rounds).  CTA r keeps the weight slice of hidden units [64r, 64r+64) (all four
+// lstm_fwd_tc_kernel<SAVE, 64>; a batch that fits in one round of pair groups, two 2-CTA clusters per tile, runs as
+// lstm_fwd_pair_kernel<SAVE>; see tc_rounds).  CTA r keeps the weight slice of hidden units [64r, 64r+64) (all four
 // gates, 256 gate columns) resident in shared memory for the whole unroll.  h_t is exchanged through global memory (it
 // is an output anyway) and comes back as the next step's A operand via TMA multicast.  The backward recurrence
 // (lstm_bwd_tc_kernel<FUSED, ROWS>) runs the same rounds.  tc_init sets both up when a handle is created,
@@ -75,8 +76,13 @@ struct TcImpl {
   CUtensorMap tm_wos, tm_dpb[2];               // tm_dpb[0]: also the head's dpred tile stores
   float* bop;
   CUtensorMap tm_ubk;                          // backward recurrence
-  int max_clusters = 0, bwd_max_clusters = 0;
+  int max_clusters = 0, bwd_max_clusters = 0;  // co-resident 4-CTA clusters
+  int max_groups = 0, bwd_max_groups = 0;      // co-resident pair groups (half the co-resident 2-CTA clusters)
   bool half_tiles = true;                      // a last round that fits as 64-row half tiles runs as such (tc_rounds)
+  int pair_groups = -1;                        // -1: tc_rounds chooses; 0 / 1: 4-CTA clusters / pair groups wherever allowed
+  uint64_t* flags = nullptr;                   // pair groups: [CTA][2] step flags (FwdParams::flags)
+  uint8_t* xscr = nullptr;                     // pair groups: [CTA][BWD_XSCR] backward slices for the other cluster
+  uint64_t seq = 0;                            // every flag is below it: the next pair launch's seq0
   int head_ctas = 0, head_wctas = 0;
   int n_sms = 0;
 };
@@ -143,14 +149,28 @@ __device__ __forceinline__ void pack_weights_body(int bid, int I, const float* _
 // Persistent forward recurrence
 // =============================================================================================
 // One launch runs the row units unit0 .. unit0 + n_units - 1, of ROWS rows each (unit u covers rows ROWS u ..), over
-// n_iters rounds of n_clusters clusters.
+// n_iters rounds of n_clusters groups of 4 CTAs (a 4-CTA cluster or a pair group).
 struct FwdParams {
   int B, T, n_iters, n_clusters, unit0, n_units, k16_x, n_tiles_cap;
   __nv_bfloat16* xh;
   __nv_bfloat16* gates;   // null: do not save
   __nv_bfloat16* cst;     // null: do not save
   const float* biasp;
+  uint64_t* flags;        // pair groups: the step flags, two per CTA (TcImpl::flags)
+  uint64_t seq0;          // pair groups: every flag is below seq0 when the launch starts
 };
+
+// Pair groups (a tile's four CTAs as two 2-CTA clusters, see tc_rounds): what crosses between the two clusters goes
+// through L2.  A CTA publishes step k of the launch by a release store of seq0 + k + 1 to its flag; a reader polls the
+// flag with acquire loads.  Flags only grow (each launch starts above every value written before), so no launch resets
+// them.  All four CTAs of a group are co-resident (tc_rounds), so the poll is bounded only against a broken schedule:
+// after ~2 s it fails the launch instead of hanging the device.
+__device__ __forceinline__ void wait_flag(const uint64_t* flag, uint64_t target) {
+  if (ld_acquire_gpu(flag) >= target) return;
+  const uint32_t t0 = (uint32_t)clock();
+  while (ld_acquire_gpu(flag) < target)
+    if ((uint32_t)clock() - t0 > 4000000000u) __trap();
+}
 
 // Warps 0-7: two consumer warpgroups (rows 0-63 / 64-127 of the tile; each issues its own wgmma and runs the cell
 // update on its accumulator fragment); warpgroup 2: warp 8 = TMA producer.  setmaxnreg moves the registers of the
@@ -188,16 +208,23 @@ __device__ __forceinline__ void fwd_gates(const float* a, const float* bs, int h
 // last round that would otherwise leave most clusters idle).  At 64 rows both consumer warpgroups take the same rows
 // and split the gate columns: warpgroup wg issues and updates only its 128-column half (chunks 2 wg, 2 wg + 1).  The
 // maps tm_h and tm_x come with boxes of ROWS / 4 and ROWS rows.
-template <bool SAVE, int ROWS>
-__global__ void __launch_bounds__(FWD_THREADS, 1)
-    lstm_fwd_tc_kernel(FwdParams p, const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_x,
-                       const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w) {
+// PAIR: the group kind.  false: the four CTAs of a tile are one 4-CTA cluster; rank = cluster rank, and the h exchange
+// is the cluster's (h_written, then every CTA multicasts a quarter of the rows to all four).  true: they are a pair
+// group, two 2-CTA clusters (rank = 2 x cluster of the group + cluster rank = blockIdx.x mod 4), 128-row tiles only.
+// h_written then counts the cluster's two slices; the other cluster's two are acquired from their flags, and every CTA
+// multicasts half of the rows to both CTAs of its cluster.  Everything else is the same code.
+template <bool PAIR, bool SAVE, int ROWS>
+__device__ __forceinline__ void lstm_fwd_tc(const FwdParams& p, const CUtensorMap& tm_h, const CUtensorMap& tm_x,
+                                            const CUtensorMap& tm_u, const CUtensorMap& tm_w) {
+  static_assert(!PAIR || ROWS == 128, "pair groups run 128-row tiles");
+  constexpr uint32_t NCL = PAIR ? 2 : TC_NC;    // CTAs per cluster
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   FwdBars* bars = reinterpret_cast<FwdBars*>(smem + SM_BARS);
   float* bias_s = reinterpret_cast<float*>(smem + SM_BIAS);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = cluster_ctarank();
+  const uint32_t crank = cluster_ctarank();
+  const uint32_t rank = PAIR ? (blockIdx.x & 3) : crank;
   const int cid = blockIdx.x / TC_NC;
 
   if (tid == 0) {
@@ -205,7 +232,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
     mbar_init(&bars->x_full, 1);
     mbar_init(&bars->x_empty, 8);           // one arrive per consumer warp
     mbar_init(&bars->h_full, 1);
-    mbar_init(&bars->h_written, TC_NC);
+    mbar_init(&bars->h_written, NCL);
     fence_mbar_init();
   }
   if (tid < TC_NSL) bias_s[tid] = p.biasp[rank * TC_NSL + tid];
@@ -235,12 +262,19 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
           mbar_arrive_expect_tx(&bars->x_full, ROWS * 64);
           tma_load_2d(xbuf, &tm_x, &bars->x_full, t * TC_XH_LD + TC_XOFF, b0);
           if (t >= 1) {
-            mbar_wait_cluster(&bars->h_written, (n_hw++) & 1);   // all 4 slices of h_{t-1} are in global memory
+            mbar_wait_cluster(&bars->h_written, (n_hw++) & 1);   // the cluster's slices of h_{t-1} are in global memory
+            if (PAIR) {                                            // and the other cluster's two
+              const uint64_t seq = p.seq0 + (uint64_t)it * T + t;
+              wait_flag(p.flags + 2 * (blockIdx.x ^ 2), seq);
+              wait_flag(p.flags + 2 * (blockIdx.x ^ 3), seq);
+            }
             fence_proxy_async_global();
             mbar_arrive_expect_tx(&bars->h_full, ROWS * 512);
-            for (int kb = 0; kb < 4; ++kb)
-              tma_load_2d_mcast(hbuf + kb * 16384 + rank * (ROWS * 32), &tm_h, &bars->h_full, t * TC_XH_LD + kb * 64,
-                                b0 + (ROWS / 4) * (int)rank, 0xF);
+            // row quadrants (ROWS / 4 rows each) to the cluster: one each from 4 CTAs, two each from 2
+            for (uint32_t qd = crank * (4 / NCL); qd < (crank + 1) * (4 / NCL); ++qd)
+              for (int kb = 0; kb < 4; ++kb)
+                tma_load_2d_mcast(hbuf + kb * 16384 + qd * (ROWS * 32), &tm_h, &bars->h_full, t * TC_XH_LD + kb * 64,
+                                  b0 + (ROWS / 4) * (int)qd, (1u << NCL) - 1);
           }
         }
         mbar_wait_cluster(&bars->h_written, (n_hw++) & 1);       // phase of step T-1 (keeps parities aligned)
@@ -386,7 +420,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
         // at cluster scope and cross into the async proxy before their TMA loads.  All MMAs of the step are complete
         // here, so the h buffer may be overwritten by the multicast of the next step.
         named_bar_sync(1, 256);
-        if (warp == 0 && lane < TC_NC) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->h_written), (uint32_t)lane));
+        if (warp == 0 && lane < NCL) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->h_written), (uint32_t)lane));
+        if (PAIR && warp == 1 && lane == 0) st_release_gpu(p.flags + 2 * blockIdx.x, p.seq0 + (uint64_t)it * T + t + 1);
         if (SAVE) {
           // The other chunks' saved state is not needed by the h exchange: it goes out after the publish, so that the
           // release above does not wait for it.
@@ -399,6 +434,20 @@ __global__ void __launch_bounds__(FWD_THREADS, 1)
   }
   __syncwarp();
   cluster_sync_all();          // nobody leaves while peers may still multicast into / arrive on this CTA
+}
+
+template <bool SAVE, int ROWS>
+__global__ void __launch_bounds__(FWD_THREADS, 1)
+    lstm_fwd_tc_kernel(FwdParams p, const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_x,
+                       const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w) {
+  lstm_fwd_tc<false, SAVE, ROWS>(p, tm_h, tm_x, tm_u, tm_w);
+}
+
+template <bool SAVE>
+__global__ void __launch_bounds__(FWD_THREADS, 1)
+    lstm_fwd_pair_kernel(FwdParams p, const __grid_constant__ CUtensorMap tm_h, const __grid_constant__ CUtensorMap tm_x,
+                         const __grid_constant__ CUtensorMap tm_u, const __grid_constant__ CUtensorMap tm_w) {
+  lstm_fwd_tc<true, SAVE, 128>(p, tm_h, tm_x, tm_u, tm_w);
 }
 
 // =============================================================================================
@@ -1025,6 +1074,9 @@ struct BwdParams {
   const __nv_bfloat16* gates;
   const __nv_bfloat16* cst;
   const __nv_bfloat16* dhout;
+  uint64_t* flags;        // pair groups: as in FwdParams
+  uint64_t seq0;
+  uint8_t* xscr;          // pair groups: the slices bound for the other cluster, BWD_XSCR bytes per CTA
 };
 
 constexpr int BWD_NC = 4;
@@ -1040,12 +1092,16 @@ constexpr uint32_t SB_DPB = 212992;             // FUSED: dLoss/dpred tile of on
 constexpr uint32_t SB_WOS = 221184;             // FUSED: (Wo gamma inv) rows of this CTA's 64 hidden units [64 x 64 B], SW64
 constexpr uint32_t SB_BARS = 225280;
 constexpr uint32_t BWD_SMEM = SB_BARS + 256 + 1024;
+// Pair groups: a CTA's slices for the other cluster, [peer offset d - 1][send parity][warpgroup][chunk jb][consumer
+// thread][16 B]; one warpgroup's slice for one step is 8 KB, in the receive slot's order, chunk by chunk.
+constexpr size_t BWD_XSCR = (size_t)3 * 2 * 2 * 8192;
 
 struct BwdBars {
   uint64_t w_full;
   uint64_t recv_full[2];         // per consumer warpgroup: the peers' partial slices for its 64 rows have landed
-  uint64_t slot_free[2];         // per consumer warpgroup: the peers have read the slices this CTA last sent them
+  uint64_t slot_free[2];         // per consumer warpgroup: the peers in the cluster have read what this CTA sent them
   uint64_t dpb_full, dpb_free;   // FUSED: the dpred tile has landed / the MMAs reading it have completed
+  uint64_t slot_read[2];         // pair groups: the warpgroup has read its receive slots (the producer may refill them)
 };
 
 __device__ __forceinline__ uint32_t ld_b32(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
@@ -1055,10 +1111,16 @@ __device__ __forceinline__ uint32_t ld_b32(const __nv_bfloat16* p) { return *rei
 // dpred tile) into the own-slice columns of its accumulator.
 // ROWS: rows per cluster and round, 128 (a tile) or 64 (half a tile, see lstm_fwd_tc_kernel).  At 64 rows warpgroup 0
 // carries them exactly as it carries rows 0-63 of a tile, and warpgroup 1 has no rows; tm_dpb comes with 64-row boxes.
-template <bool FUSED, int ROWS>
-__global__ void __launch_bounds__(BWD_THREADS, 1)
-    lstm_bwd_tc_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
-                       const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
+// PAIR: the group kind, as in lstm_fwd_tc.  In a pair group the slice for the peer in the same cluster goes by st.async
+// as in a 4-CTA cluster.  The two for the other cluster go to the sender's L2 scratch (p.xscr, double-buffered by the
+// parity of the send), and the warpgroup's flag is released; the receiver's producer acquires it and loads the two
+// slices by bulk copy into the same receive slots, completing tx on the same recv_full.  So the consumers add the
+// three slices in the same order, and dz is bit-identical to the 4-CTA cluster's.  The scratch needs no "slot free":
+// a CTA sends k + 2 only after it has received every peer's k + 1, which each peer sent after it had received k.
+template <bool PAIR, bool FUSED, int ROWS>
+__device__ __forceinline__ void lstm_bwd_tc(const BwdParams& p, const CUtensorMap& tm_ubk, const CUtensorMap& tm_dzst,
+                                            const CUtensorMap& tm_dpb, const CUtensorMap& tm_wos) {
+  static_assert(!PAIR || ROWS == 128, "pair groups run 128-row tiles");
   extern __shared__ uint8_t smem_raw[];
   // Aligned by an offset from smem_raw rather than by masking a generic address, so that the compiler still knows the
   // pointer is shared: the staging stores and slice reads below then take 32-bit shared addresses (STS / LDS), not
@@ -1066,7 +1128,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   BwdBars* bars = reinterpret_cast<BwdBars*>(smem + SB_BARS);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = cluster_ctarank();
+  const uint32_t rank = PAIR ? (blockIdx.x & 3) : cluster_ctarank();
   const int cid = blockIdx.x / BWD_NC;
   const int T = p.T;
 
@@ -1074,7 +1136,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
     mbar_init(&bars->w_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&bars->recv_full[i], 1);
-      mbar_init(&bars->slot_free[i], BWD_NC - 1);   // one arrive per peer
+      mbar_init(&bars->slot_free[i], PAIR ? 1 : BWD_NC - 1);   // one arrive per peer in the cluster
+      mbar_init(&bars->slot_read[i], 1);
     }
     mbar_init(&bars->dpb_full, 1);
     mbar_init(&bars->dpb_free, ROWS / 16);  // one arrive per consumer warp with rows
@@ -1096,17 +1159,41 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
                       (int)rank * 256 + (int)((rank + d) & 3) * 64);
       if (FUSED) tma_load_2d(smem + SB_WOS, &tm_wos, &bars->w_full, 0, rank * 64);
       pdl_sync();
-      if (FUSED) {
-        uint32_t n_dp = 0;
+      if (FUSED || PAIR) {
+        uint32_t n_dp = 0, n_rx = 0;
         for (int it = 0; it < p.n_iters; ++it) {
           if (it * p.n_clusters + cid >= p.n_units) break;   // clusters without a unit in the last round
           const int b0 = (p.unit0 + it * p.n_clusters + cid) * ROWS;
-          // dpred rows of time step td into the single staging buffer, once the MMAs that read the previous ones are done
           for (int td = T - 1; td >= 0; --td) {
-            if (n_dp > 0) mbar_wait(&bars->dpb_free, (n_dp - 1) & 1);
-            ++n_dp;
-            mbar_arrive_expect_tx(&bars->dpb_full, ROWS * 64);
-            tma_load_2d(smem + SB_DPB, &tm_dpb, &bars->dpb_full, 0, (td * p.n_tiles_cap + (b0 >> 7)) * 128 + (b0 & 127));
+            if (FUSED) {
+              // dpred rows of time step td into the single staging buffer, once the MMAs that read the previous ones
+              // are done
+              if (n_dp > 0) mbar_wait(&bars->dpb_free, (n_dp - 1) & 1);
+              ++n_dp;
+              mbar_arrive_expect_tx(&bars->dpb_full, ROWS * 64);
+              tma_load_2d(smem + SB_DPB, &tm_dpb, &bars->dpb_full, 0, (td * p.n_tiles_cap + (b0 >> 7)) * 128 + (b0 & 127));
+            }
+            if (PAIR && td < T - 1) {
+              // the other cluster's slices of the partials of step td + 1 (send n_rx of the launch), per warpgroup
+              // once it has read its slots
+#pragma unroll 1
+              for (int g = 0; g < 2; ++g) {
+                mbar_wait(&bars->slot_read[g], n_rx & 1);
+                wait_flag(p.flags + 2 * (blockIdx.x ^ 2) + g, p.seq0 + n_rx + 1);
+                wait_flag(p.flags + 2 * (blockIdx.x ^ 3) + g, p.seq0 + n_rx + 1);
+                fence_proxy_async_global();
+#pragma unroll 1
+                for (uint32_t x = 2; x < 4; ++x) {
+                  // peer blockIdx.x ^ x sits at offset d: it sent with offset 4 - d (its scratch entry 3 - d), and
+                  // the slice lands in slot d - 1
+                  const uint32_t d = ((blockIdx.x ^ x) - blockIdx.x) & 3;
+                  const uint8_t* src = p.xscr + (blockIdx.x ^ x) * BWD_XSCR + (((3 - d) * 2 + (n_rx & 1)) * 2 + g) * 8192;
+                  uint8_t* dst = smem + SB_R + (d - 1) * 16384 + g * 2048;
+                  for (int jb = 0; jb < 4; ++jb) bulk_load(dst + jb * 4096, src + jb * 2048, 2048, &bars->recv_full[g]);
+                }
+              }
+              ++n_rx;
+            }
           }
         }
       }
@@ -1305,8 +1392,13 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
         // lets any peer send, so no tx completes on a phase before it is armed.
         if (elected && t > 0) {
           mbar_arrive_expect_tx(&bars->recv_full[wg], (BWD_NC - 1) * 8192);
+          if (PAIR) {
+            mbar_arrive_cluster(mapa_u32(smem_u32(&bars->slot_free[wg]), (rank & 1) ^ 1));
+            mbar_arrive(&bars->slot_read[wg]);
+          } else {
 #pragma unroll
-          for (uint32_t d = 1; d < BWD_NC; ++d) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->slot_free[wg]), (rank + d) & 3));
+            for (uint32_t d = 1; d < BWD_NC; ++d) mbar_arrive_cluster(mapa_u32(smem_u32(&bars->slot_free[wg]), (rank + d) & 3));
+          }
         }
         if (FUSED && t > 0) dy_mma(1);         // head part of dLoss/dh_{t-1}, read (acc[0..7], rown) next step
         wgmma_wait<0>();
@@ -1316,21 +1408,38 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
           // ---- export the foreign slices of partial_t (needed by the peers for step t-1) into their shared memory ----
           // Peer (rank + d) mod 4 files this CTA's slice in its slot 3 - d.  Its warpgroup wg has read what this CTA
           // sent last step once slot_free[wg] completes; the stores complete tx on its recv_full[wg].
-          mbar_wait_cluster(&bars->slot_free[wg], (n_ex++) & 1);
+          mbar_wait_cluster(&bars->slot_free[wg], n_ex & 1);     // n_ex: this send's index in the launch
 #pragma unroll
           for (int d = 1; d < BWD_NC; ++d) {
             const uint32_t peer = (rank + (uint32_t)d) & 3;
-            const uint32_t dst = mapa_u32(smem_u32(smem + recv_off + (3 - d) * 16384), peer);
-            const uint32_t bar = mapa_u32(smem_u32(&bars->recv_full[wg]), peer);
+            if (!PAIR || peer == (rank ^ 1)) {
+              const uint32_t peer_cr = PAIR ? (rank & 1) ^ 1 : peer;
+              const uint32_t dst = mapa_u32(smem_u32(smem + recv_off + (3 - d) * 16384), peer_cr);
+              const uint32_t bar = mapa_u32(smem_u32(&bars->recv_full[wg]), peer_cr);
 #pragma unroll
-            for (int jb = 0; jb < 4; ++jb) {
-              const int i = 32 * d + 8 * jb;
-              st_async_v4(dst + jb * 4096,
-                          make_uint4(pack_bf16x2(acc[i], acc[i + 1]), pack_bf16x2(acc[i + 4], acc[i + 5]),
-                                     pack_bf16x2(acc[i + 2], acc[i + 3]), pack_bf16x2(acc[i + 6], acc[i + 7])),
-                          bar);
+              for (int jb = 0; jb < 4; ++jb) {
+                const int i = 32 * d + 8 * jb;
+                st_async_v4(dst + jb * 4096,
+                            make_uint4(pack_bf16x2(acc[i], acc[i + 1]), pack_bf16x2(acc[i + 4], acc[i + 5]),
+                                       pack_bf16x2(acc[i + 2], acc[i + 3]), pack_bf16x2(acc[i + 6], acc[i + 7])),
+                            bar);
+              }
+            } else {
+              uint8_t* dst = p.xscr + blockIdx.x * BWD_XSCR + (((d - 1) * 2 + (n_ex & 1)) * 2 + wg) * 8192 + (tid & 127) * 16;
+#pragma unroll
+              for (int jb = 0; jb < 4; ++jb) {
+                const int i = 32 * d + 8 * jb;
+                st_global_v4(dst + jb * 2048,
+                             make_uint4(pack_bf16x2(acc[i], acc[i + 1]), pack_bf16x2(acc[i + 4], acc[i + 5]),
+                                        pack_bf16x2(acc[i + 2], acc[i + 3]), pack_bf16x2(acc[i + 6], acc[i + 7])));
+              }
             }
           }
+          if (PAIR) {                           // publish the warpgroup's two scratch slices
+            named_bar_sync(wg_bar, 128);
+            if (elected) st_release_gpu(p.flags + 2 * blockIdx.x + wg, p.seq0 + n_ex + 1);
+          }
+          ++n_ex;
 #pragma unroll
           for (int i = 0; i < 24; ++i) rown[i] = acc[8 + i];
         }
@@ -1340,6 +1449,20 @@ __global__ void __launch_bounds__(BWD_THREADS, 1)
   }
   __syncwarp();
   cluster_sync_all();          // nobody leaves while peers may still store into / arrive on this CTA
+}
+
+template <bool FUSED, int ROWS>
+__global__ void __launch_bounds__(BWD_THREADS, 1)
+    lstm_bwd_tc_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
+                       const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
+  lstm_bwd_tc<false, FUSED, ROWS>(p, tm_ubk, tm_dzst, tm_dpb, tm_wos);
+}
+
+template <bool FUSED>
+__global__ void __launch_bounds__(BWD_THREADS, 1)
+    lstm_bwd_pair_kernel(BwdParams p, const __grid_constant__ CUtensorMap tm_ubk, const __grid_constant__ CUtensorMap tm_dzst,
+                         const __grid_constant__ CUtensorMap tm_dpb, const __grid_constant__ CUtensorMap tm_wos) {
+  lstm_bwd_tc<true, FUSED, 128>(p, tm_ubk, tm_dzst, tm_dpb, tm_wos);
 }
 
 // =============================================================================================
@@ -1400,6 +1523,9 @@ void tc_layout(TcState& st, const lfmq_config& c, Carver& cv) {
   m.head_wctas = m.n_sms * 2;
   m.head_part_elems = (size_t)m.head_ctas * HEAD_PART;
   m.head_part = cv.take<float>(m.head_part_elems);
+  // pair groups: a group's CTAs are blockIdx.x 4 g .. 4 g + 3 of a grid of at most one CTA per SM
+  m.flags = cv.take<uint64_t>((size_t)2 * m.n_sms);
+  m.xscr = m.train ? cv.take<uint8_t>((size_t)m.n_sms * BWD_XSCR) : nullptr;
   if (m.train) {
     // Saved state is blocked by 128-row tiles; both recurrences move it in 16- and 8-byte vectors, which the carver's
     // 1024-byte alignment of every buffer keeps aligned.
@@ -1421,36 +1547,51 @@ void tc_layout(TcState& st, const lfmq_config& c, Carver& cv) {
   }
 }
 
-// The instantiations of the two recurrences, [flag][i]: flag = SAVE / FUSED, i = 0 for 128-row tiles and 1 for 64-row
-// half tiles, as the pairs of maps in TcImpl.
+// The instantiations of the two recurrences, [flag][i]: flag = SAVE / FUSED; i = 0 for 128-row tiles and 1 for 64-row
+// half tiles on 4-CTA clusters, 2 for 128-row tiles on pair groups.  Maps with batch rows in their boxes are
+// TcImpl's [0] / [1] pairs, indexed by i == 1.
 using FwdKernel = void (*)(FwdParams, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap);
 using BwdKernel = void (*)(BwdParams, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap);
-static const FwdKernel fwd_kernels[2][2] = {{lstm_fwd_tc_kernel<false, 128>, lstm_fwd_tc_kernel<false, 64>},
-                                            {lstm_fwd_tc_kernel<true, 128>, lstm_fwd_tc_kernel<true, 64>}};
-static const BwdKernel bwd_kernels[2][2] = {{lstm_bwd_tc_kernel<false, 128>, lstm_bwd_tc_kernel<false, 64>},
-                                            {lstm_bwd_tc_kernel<true, 128>, lstm_bwd_tc_kernel<true, 64>}};
-static_assert(BWD_NC == TC_NC, "both recurrences run on 4-CTA clusters");
+static const FwdKernel fwd_kernels[2][3] = {
+    {lstm_fwd_tc_kernel<false, 128>, lstm_fwd_tc_kernel<false, 64>, lstm_fwd_pair_kernel<false>},
+    {lstm_fwd_tc_kernel<true, 128>, lstm_fwd_tc_kernel<true, 64>, lstm_fwd_pair_kernel<true>}};
+static const BwdKernel bwd_kernels[2][3] = {
+    {lstm_bwd_tc_kernel<false, 128>, lstm_bwd_tc_kernel<false, 64>, lstm_bwd_pair_kernel<false>},
+    {lstm_bwd_tc_kernel<true, 128>, lstm_bwd_tc_kernel<true, 64>, lstm_bwd_pair_kernel<true>}};
+static_assert(BWD_NC == TC_NC, "both recurrences run 4 CTAs per tile");
 
-// Sets the dynamic shared memory of the four instantiations of a recurrence, and how many of its 4-CTA clusters can be
-// co-resident (one CTA per SM because of shared memory); fails if not even one fits.
+// How many clusters of cluster_x CTAs of a kernel can be co-resident (one CTA per SM because of shared memory).
 template <class Kernel>
-static int tc_cluster_setup(Kernel const (&kernels)[2][2], int threads, int smem, const char* what, int* max_clusters) {
-  for (const auto& by_rows : kernels)
-    for (Kernel k : by_rows) LFMQ_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+static int tc_max_clusters(Kernel k, int threads, int smem, int cluster_x, int* n) {
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(TC_NC * (device_sm_count() / TC_NC));
+  cfg.gridDim = dim3(cluster_x * (device_sm_count() / cluster_x));
   cfg.blockDim = dim3(threads);
   cfg.dynamicSmemBytes = smem;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = TC_NC;
+  attr[0].val.clusterDim.x = cluster_x;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  LFMQ_CUDA_CHECK(cudaOccupancyMaxActiveClusters(max_clusters, kernels[1][0], &cfg));
-  if (*max_clusters < 1) {
-    LFMQ_SET_ERR("no 4-CTA cluster of the %s kernel fits on this device", what);
+  LFMQ_CUDA_CHECK(cudaOccupancyMaxActiveClusters(n, k, &cfg));
+  return 0;
+}
+
+// Sets the dynamic shared memory of the six instantiations of a recurrence, and how many of its 4-CTA clusters and of
+// its pair groups can be co-resident; fails if not even one of either fits.
+template <class Kernel>
+static int tc_cluster_setup(Kernel const (&kernels)[2][3], int threads, int smem, const char* what, int* max_clusters,
+                            int* max_groups) {
+  for (const auto& by_kind : kernels)
+    for (Kernel k : by_kind) LFMQ_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int n2 = 0, rc;
+  if ((rc = tc_max_clusters(kernels[1][0], threads, smem, TC_NC, max_clusters))) return rc;
+  if ((rc = tc_max_clusters(kernels[1][2], threads, smem, 2, &n2))) return rc;
+  *max_groups = n2 / 2;
+  if (*max_clusters < 1 || *max_groups < 1) {
+    LFMQ_SET_ERR("no 4-CTA cluster or pair group of the %s kernel fits on this device (%d, %d)", what, *max_clusters,
+                 *max_groups);
     return LFMQ_ERR_UNSUPPORTED;
   }
   return 0;
@@ -1480,16 +1621,23 @@ int tc_init(TcState& st, const lfmq_config& c) {
   LFMQ_CUDA_CHECK(cudaFuncSetAttribute(head_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, HROWS_SMEM));
   if ((rc = encode_map_2d(&m.tm_u, m.Up, TC_H, 4 * TC_H, TC_H * 2, 64, 256, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   if ((rc = encode_map_2d(&m.tm_w, m.Wp, 32, 4 * TC_H, 64, 32, 256, CU_TENSOR_MAP_SWIZZLE_64B))) return rc;
-  if ((rc = tc_cluster_setup(fwd_kernels, FWD_THREADS, FWD_SMEM, "forward", &m.max_clusters))) return rc;
+  if ((rc = tc_cluster_setup(fwd_kernels, FWD_THREADS, FWD_SMEM, "forward", &m.max_clusters, &m.max_groups))) return rc;
   if (m.train) {
     if ((rc = wgrad_gemm_init())) return rc;
     // boxes of 64 hidden units: the kernel loads its K-slice of U in rotated N order (own hidden slice first)
     if ((rc = encode_map_2d(&m.tm_ubk, m.Ubk, 256, 4 * TC_H, 512, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-    if ((rc = tc_cluster_setup(bwd_kernels, BWD_THREADS, BWD_SMEM, "backward", &m.bwd_max_clusters))) return rc;
+    if ((rc = tc_cluster_setup(bwd_kernels, BWD_THREADS, BWD_SMEM, "backward", &m.bwd_max_clusters, &m.bwd_max_groups)))
+      return rc;
   }
   // LFMQ_TC_HALF_TILES=0 keeps every round at 128-row tiles (A/B measurements, tests comparing the two schedules)
   const char* ht = getenv("LFMQ_TC_HALF_TILES");
   m.half_tiles = !(ht != nullptr && atoi(ht) == 0);
+  // LFMQ_TC_PAIR_GROUPS=0 / 1 runs every recurrence on 4-CTA clusters / pair groups wherever the handle may use them
+  // (A/B measurements, tests comparing the two schedules); unset, tc_rounds chooses
+  const char* pg = getenv("LFMQ_TC_PAIR_GROUPS");
+  m.pair_groups = pg != nullptr && *pg != '\0' ? (atoi(pg) != 0) : -1;
+  LFMQ_CUDA_CHECK(cudaMemset(m.flags, 0, (size_t)2 * m.n_sms * sizeof(uint64_t)));
+  m.seq = 0;
   st.weights_dirty = 1;
   return 0;
 }
@@ -1518,25 +1666,37 @@ static int tc_pack_weights(TcState& st, const ParamLayout& pl, const float* para
   return 0;
 }
 
-// The rounds of a persistent recurrence over B rows with at most max_clusters co-resident clusters: n_full 128-row tiles
-// (units 0 .. n_full - 1 of 128 rows), then n_half 64-row half tiles (units 2 n_full .. of 64 rows) in one more round.
-// Rounds are independent (each unit starts from zero state), so the two kinds are two launches in stream order.  The
-// last round runs as half tiles whenever they fit on the co-resident clusters: a round of a few whole tiles leaves
-// most clusters idle for all T steps while the busy ones carry 128 rows through every step's dependency chain.
+// The rounds of a persistent recurrence over B rows.  On 4-CTA clusters (at most max_clusters co-resident): n_full
+// 128-row tiles (units 0 .. n_full - 1 of 128 rows), then n_half 64-row half tiles (units 2 n_full .. of 64 rows) in one
+// more round.  Rounds are independent (each unit starts from zero state), so the two kinds are two launches in stream
+// order.  The last round runs as half tiles whenever they fit on the co-resident clusters: a round of a few whole tiles
+// leaves most clusters idle for all T steps while the busy ones carry 128 rows through every step's dependency chain.
+// On pair groups (pair: at most max_groups co-resident): n_full = all tiles, in rounds of 128-row tiles.  A 4-CTA
+// cluster must sit in one GPC, so only 30 fit on the 132 SMs of an H100 SXM; 2-CTA clusters pack every TPC, 33 groups.
+// Pair groups pay an exchange through L2 on every step, which makes each step 10-16 % slower (DESIGN.md section 5a), so
+// they run only where all tiles fit in one round of them and 4-CTA clusters need more, the half-tile round counted as
+// one (B = 4096: 1 round against 2).  Over several rounds that cost is not made up: B = 65536 takes 16 pair rounds
+// against 18 on clusters and is 4 % slower.  pair_mode (TcImpl::pair_groups) may force a choice.
 struct TcRounds {
   int n_full, n_half;
+  bool pair;
 };
 
-static TcRounds tc_rounds(int B, int max_clusters, bool half_tiles) {
+static int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+static TcRounds tc_rounds(int B, int max_clusters, int max_groups, bool half_tiles, int pair_mode) {
   const int n_tiles = (B + 127) / 128;
   const int n_cl = n_tiles < max_clusters ? n_tiles : max_clusters;
-  const int full_rounds = (n_tiles + n_cl - 1) / n_cl - 1;
+  const int full_rounds = ceil_div(n_tiles, n_cl) - 1;
   const int rows_last = B - full_rounds * n_cl * 128;
-  if (half_tiles && (rows_last + 63) / 64 <= max_clusters) return {full_rounds * n_cl, (rows_last + 63) / 64};
-  return {n_tiles, 0};
+  TcRounds r = {n_tiles, 0, false};
+  if (half_tiles && ceil_div(rows_last, 64) <= max_clusters) r = {full_rounds * n_cl, ceil_div(rows_last, 64), false};
+  const int cluster_rounds = ceil_div(r.n_full, max_clusters) + (r.n_half > 0 ? 1 : 0);
+  if (pair_mode == 1 || (pair_mode < 0 && n_tiles <= max_groups && cluster_rounds > 1)) return {n_tiles, 0, true};
+  return r;
 }
 
-// n_units units of ROWS rows from unit0 on, in rounds of at most max_clusters clusters
+// n_units units of ROWS rows from unit0 on, in rounds of at most max_clusters groups
 template <class Params>
 static void tc_set_rounds(Params& p, int unit0, int n_units, int max_clusters) {
   p.unit0 = unit0;
@@ -1546,24 +1706,37 @@ static void tc_set_rounds(Params& p, int unit0, int n_units, int max_clusters) {
 }
 
 // Runs a recurrence over the rounds of its p.B rows (tc_rounds): the 128-row instantiation over the n_full tiles, then
-// the 64-row one over the n_half half tiles.  FwdParams runs lstm_fwd_tc_kernel<flag = SAVE, ·>, BwdParams
-// lstm_bwd_tc_kernel<flag = FUSED, ·>, whose dz stores go through tm_dzst.
+// the 64-row one over the n_half half tiles, or the pair-group one over all tiles.  FwdParams runs
+// lstm_fwd_tc_kernel<flag = SAVE, ·> / lstm_fwd_pair_kernel<SAVE>, BwdParams lstm_bwd_tc_kernel<flag = FUSED, ·> /
+// lstm_bwd_pair_kernel<FUSED>, whose dz stores go through tm_dzst.
 template <class Params>
-static int tc_run_rounds(const TcImpl& m, Params p, bool flag, cudaStream_t s, const CUtensorMap* tm_dzst = nullptr) {
+static int tc_run_rounds(TcState& st, Params p, bool flag, cudaStream_t s, const CUtensorMap* tm_dzst = nullptr) {
   constexpr bool fwd = std::is_same<Params, FwdParams>::value;
+  TcImpl& m = *st.impl;
   const int max_clusters = fwd ? m.max_clusters : m.bwd_max_clusters;
-  const TcRounds r = tc_rounds(p.B, max_clusters, m.half_tiles);
+  const int max_groups = fwd ? m.max_groups : m.bwd_max_groups;
+  // A pair group's clusters wait for each other, so all of them must be resident together.  Only a handle with the
+  // whole device can count on that: a neighbour's kernels may hold one SM of a TPC each, and a 2-CTA cluster needs both.
+  const int pair_mode = st.share_num < st.share_den ? 0 : m.pair_groups;
+  const TcRounds r = tc_rounds(p.B, max_clusters, max_groups, m.half_tiles, pair_mode);
+  p.flags = m.flags;
   for (int i = 0; i < 2; ++i) {
     const int n_units = i == 0 ? r.n_full : r.n_half;
     if (n_units == 0) continue;
-    tc_set_rounds(p, i == 0 ? 0 : 2 * r.n_full, n_units, max_clusters);
+    tc_set_rounds(p, i == 0 ? 0 : 2 * r.n_full, n_units, r.pair ? max_groups : max_clusters);
+    const int k = r.pair ? 2 : i;
+    const int cluster_x = r.pair ? 2 : TC_NC;
+    if (r.pair) {
+      p.seq0 = m.seq;                      // the launch publishes at most n_iters T steps per flag
+      m.seq += (uint64_t)p.n_iters * p.T;
+    }
     const dim3 grid(TC_NC * p.n_clusters);
     int rc;
     if constexpr (fwd)
-      rc = launch_pdl(fwd_kernels[flag][i], grid, dim3(FWD_THREADS), FWD_SMEM, s, TC_NC, true, p, m.tm_h[i], m.tm_x[i],
-                      m.tm_u, m.tm_w);
+      rc = launch_pdl(fwd_kernels[flag][k], grid, dim3(FWD_THREADS), FWD_SMEM, s, cluster_x, true, p, m.tm_h[i],
+                      m.tm_x[i], m.tm_u, m.tm_w);
     else
-      rc = launch_pdl(bwd_kernels[flag][i], grid, dim3(BWD_THREADS), BWD_SMEM, s, TC_NC, true, p, m.tm_ubk, *tm_dzst,
+      rc = launch_pdl(bwd_kernels[flag][k], grid, dim3(BWD_THREADS), BWD_SMEM, s, cluster_x, true, p, m.tm_ubk, *tm_dzst,
                       m.tm_dpb[i], m.tm_wos);
     if (rc) return rc;
   }
@@ -1582,7 +1755,7 @@ static int tc_run_recurrence(TcState& st, const float* x, int B, bool save, cuda
   p.gates = save ? m.gates : nullptr;
   p.cst = save ? m.cst : nullptr;
   p.biasp = m.biasp;
-  return tc_run_rounds(m, p, save, s);
+  return tc_run_rounds(st, p, save, s);
 }
 
 static int tc_run_head(TcState& st, const lfmq_config& c, const ParamLayout& pl, const float* params, float* grads,
@@ -1690,6 +1863,7 @@ int tc_backward(TcState& st, const lfmq_config& c, const ParamLayout& pl, const 
   bp.B = B; bp.T = m.T;
   bp.n_tiles_cap = (m.maxB + 127) / 128;
   bp.gates = m.gates; bp.cst = m.cst; bp.dhout = m.dhout;
+  bp.xscr = m.xscr;
   // dz as [b][t][1024] with columns ordered [16-unit block][gate][16]: one warpgroup's part of a staged chunk =
   // 64 rows x 64 columns
   CUtensorMap tm_dzst;
@@ -1700,7 +1874,7 @@ int tc_backward(TcState& st, const lfmq_config& c, const ParamLayout& pl, const 
     if ((rc = encode_map_bf16(&tm_dzst, m.dz, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   }
   // the tensor-core head (no dropout) leaves dLoss/dpred tiles for the backward kernel to expand on its own MMAs
-  if ((rc = tc_run_rounds(m, bp, /*fused=*/!m.dropout_head, s, &tm_dzst))) return rc;
+  if ((rc = tc_run_rounds(st, bp, /*fused=*/!m.dropout_head, s, &tm_dzst))) return rc;
   st.prof->end(LFMQ_REGION_BWD, s);
 
   st.prof->begin(LFMQ_REGION_WGRAD, s);

@@ -66,6 +66,14 @@ __device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
+__device__ __forceinline__ uint64_t ld_acquire_gpu(const uint64_t* p) {
+  uint64_t v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_gpu(uint64_t* p, uint64_t v) {
+  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
 
 // ---- proxies / fences -------------------------------------------------------------------------
 // generic-proxy smem writes -> visible to the async proxy (TMA, wgmma operand reads)
@@ -117,6 +125,12 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* s
 __device__ __forceinline__ void st_async_v4(uint32_t dst, uint4 v, uint32_t bar) {
   asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
                ::"r"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(bar)
+               : "memory");
+}
+// bytes (a multiple of 16) from global memory into this CTA's shared memory, completing tx on its mbarrier
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(smem_dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
