@@ -300,6 +300,33 @@ int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, co
 int32_t lfmq_integrated_gradients_work_bytes(lfmq_handle h, int32_t B, int32_t steps, uint64_t* bytes);
 int32_t lfmq_integrated_gradients(lfmq_handle h, const float* x, int32_t B, int32_t steps, float* attr, float* f_x,
                                   float* f_base, void* work, uint64_t work_bytes, void* stream);
+/* ---- permutation importance -----------------------------------------------------------------------------------------
+ * How much the held-out loss depends on each group of input columns (Breiman 2001; Fisher, Rudin & Dominici 2019).
+ * x [N,T,F] (or [N,T*F] on a dense handle) are the model's inputs, y[s] its targets; column c = t * F + f of a window
+ * belongs to group col_group[c] in [0, G) (host int32 [T*F]).  Copy (g, r), for g < G and r < repeats, is the held-out
+ * set with group g's columns taken from window pi(i) of the bijection pi = pi_{seed,g,r} of [0, N)
+ * (lfmq_permutation_index); the targets stay.  Each copy runs in launches of at most max_batch rows keyed by the window
+ * index (row0 = the launch's first window), so window i draws the same dropout masks at `step` in every copy.  Its
+ * predictions fill a copy-sized buffer in `work`, which the loss entry point of the model then reduces: lfmq_loss (one
+ * point or dense stage), lfmq_chain_loss with `weights` (host float [n_stages], the forecast-step weights), lfmq_loss_uq
+ * or lfmq_chain_loss_uq.  out_dev [1 + G * repeats][3] (device): row 0 the unpermuted set, row 1 + g * repeats + r copy
+ * (g, r); {loss, mse_0, 0} on point and dense stages, {uq_loss, uq_loss_last_tar, mse} on uq stages.
+ * Accepted: S >= 1 point or uq stages of one chain (any precision, forward_only or not), or one dense handle.  The
+ * handles' parameters, gradient buffers (tail included) and optimizer slots are left untouched.  repeats, N or G < 1, a
+ * col_group value outside [0, G) or a null pointer: LFMQ_ERR_ARG.  `work`: caller-owned device scratch, 256-byte
+ * aligned, of the size the *_work_bytes query gives for N: one launch's rows (per stage), the col_group copy and one
+ * copy's predictions (and variances). */
+int32_t lfmq_chain_permutation_importance_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N,
+                                                     uint64_t* bytes);
+int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_stages, const float* x,
+                                          const float* const* y, const float* weights, int32_t N,
+                                          const int32_t* col_group, int32_t G, int32_t repeats, uint64_t seed,
+                                          int64_t step, float* out_dev, void* work, uint64_t work_bytes, void* stream);
+/* The bijection of lfmq_chain_permutation_importance (host arithmetic, no device): *out = pi_{seed,group,repeat}(i).
+ * m is the smallest even integer >= 2 with 2^m >= N and h = m / 2.  A 4-round Feistel network on [0, 2^m) splits
+ * v = (L << h) | R; round j in 0..3 sets (L, R) <- (R, L ^ (philox4x32_10(R, j, group, repeat; seed_lo, seed_hi)[0] &
+ * (2^h - 1))).  Starting from v = i, the network is applied until v < N (cycle walking). */
+int32_t lfmq_permutation_index(int32_t N, uint64_t seed, int32_t group, int32_t repeat, int32_t i, int32_t* out);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

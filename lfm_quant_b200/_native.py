@@ -92,6 +92,11 @@ SYMBOLS = {
                                               _P, _P, C.c_uint64, _P]),
     'lfmq_integrated_gradients_work_bytes': (C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
     'lfmq_integrated_gradients': (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_uint64, _P]),
+    'lfmq_chain_permutation_importance_work_bytes': (C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
+    'lfmq_chain_permutation_importance': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int32, C.c_int32,
+                                                       C.c_uint64, C.c_int64, _P, _P, C.c_uint64, _P]),
+    'lfmq_permutation_index': (C.c_int32, [C.c_int32, C.c_uint64, C.c_int32, C.c_int32, C.c_int32,
+                                           C.POINTER(C.c_int32)]),
     'lfmq_chain_loss': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_loss_uq': (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_backward': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),

@@ -86,6 +86,13 @@ int ig_pick(cudaStream_t s, int n_out, int n_src, int T, int O, int target_idx, 
 // last interpolant multiplies the sum by x / M.  Launches must arrive in increasing r0 and cover [0, M * B).
 int ig_fold(cudaStream_t s, int B, int M, int64_t r0, int n, long row_elems, const float* dx, const float* x,
             float* attr);
+// Permutation importance (importance.cu, lfmq_chain_permutation_importance): perm_index is the bijection pi_{seed,g,r}
+// of [0, N) (a 4-round Philox Feistel network on [0, 2^m), cycle-walked into [0, N)); perm_importance_gather writes rows
+// [a, a + n) of copy (g, r) of x [N, row_elems] to out [n, row_elems]: columns c with col_group[c] == g (device int32
+// [row_elems]) come from window pi(i), the others from window i.
+__host__ __device__ uint32_t perm_index(int32_t N, uint64_t seed, int32_t group, int32_t repeat, uint32_t i);
+int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems, const int32_t* col_group, int g, int r,
+                           uint64_t seed, int a, int n, float* out);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

@@ -1320,6 +1320,139 @@ int32_t lfmq_integrated_gradients(lfmq_handle h, const float* x, int32_t B, int3
   return LFMQ_OK;
 }
 
+// ---- permutation importance (lfmq_chain_permutation_importance) -----------------------------------------------------
+namespace {
+// S >= 1 point or uq stages of one chain (chain_check numbers their dropout streams), or one dense handle.  Rows per
+// launch: N, at most the smallest max_batch.
+int pi_check(const lfmq_handle* st, int32_t S, int32_t N, const char* fn, int* rows) {
+  if (!st || S < 1 || S > lfmq::LFMQ_MAX_STAGES || N < 1) {
+    LFMQ_SET_ERR("%s: need 1 <= n_stages <= %d and N >= 1 (got %d, %d)", fn, lfmq::LFMQ_MAX_STAGES, S, N);
+    return LFMQ_ERR_ARG;
+  }
+  for (int i = 0; i < S; ++i)
+    if (!st[i]) {
+      LFMQ_SET_ERR("%s: stage %d is a null handle", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+  int mb = st[0]->cfg.max_batch;
+  if (st[0]->path == Path::Dense) {
+    if (S != 1) {
+      LFMQ_SET_ERR("%s: a dense handle is a model of one stage (got n_stages %d)", fn, S);
+      return LFMQ_ERR_ARG;
+    }
+  } else {
+    RUN(chain_check(st, S, 1, false));
+    for (int i = 1; i < S; ++i) mb = std::min(mb, (int)st[i]->cfg.max_batch);
+  }
+  *rows = std::min(N, mb);
+  return 0;
+}
+
+// floats of caller scratch: the launch's permuted rows, the chain's next-stage windows of a launch, the device copy of
+// col_group, and one copy's predictions (and variances on a uq chain) of every stage, each on a 256-byte boundary
+size_t pi_work_floats(const lfmq_handle* st, int S, int rows, int N) {
+  const lfmq_config& c = st[0]->cfg;
+  const size_t row_in = (size_t)c.seq_len * c.n_inputs;
+  const size_t row_out = st[0]->path == Path::Dense ? (size_t)c.n_outputs : (size_t)c.seq_len * c.n_outputs;
+  return (size_t)S * mc_align(rows * row_in) + mc_align(row_in) + (c.uq ? 2 : 1) * (size_t)S * mc_align(N * row_out);
+}
+}  // namespace
+
+int32_t lfmq_chain_permutation_importance_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N,
+                                                     uint64_t* bytes) {
+  int rows = 0;
+  RUN(pi_check(stages, n_stages, N, "lfmq_chain_permutation_importance_work_bytes", &rows));
+  if (!bytes) {
+    LFMQ_SET_ERR("lfmq_chain_permutation_importance_work_bytes: bytes == NULL");
+    return LFMQ_ERR_ARG;
+  }
+  *bytes = pi_work_floats(stages, n_stages, rows, N) * sizeof(float);
+  return LFMQ_OK;
+}
+
+int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_stages, const float* x,
+                                          const float* const* y, const float* weights, int32_t N,
+                                          const int32_t* col_group, int32_t G, int32_t repeats, uint64_t seed,
+                                          int64_t step, float* out_dev, void* work, uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_chain_permutation_importance";
+  int rows = 0;
+  RUN(pi_check(stages, n_stages, N, fn, &rows));
+  const int S = n_stages;
+  const lfmq_config& c = stages[0]->cfg;
+  const bool dense = stages[0]->path == Path::Dense, uq = c.uq != 0;
+  const long row_in = (long)c.seq_len * c.n_inputs;
+  const long row_out = dense ? c.n_outputs : (long)c.seq_len * c.n_outputs;
+  if (G < 1 || repeats < 1) {
+    LFMQ_SET_ERR("%s: need G >= 1 and repeats >= 1 (got %d, %d)", fn, G, repeats);
+    return LFMQ_ERR_ARG;
+  }
+  if (!x || !y || !weights || !col_group || !out_dev) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  for (int i = 0; i < S; ++i)
+    if (!y[i]) {
+      LFMQ_SET_ERR("%s: y[%d] == NULL", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+  for (long k = 0; k < row_in; ++k)
+    if (col_group[k] < 0 || col_group[k] >= G) {
+      LFMQ_SET_ERR("%s: col_group[%ld] = %d outside [0, G = %d)", fn, k, col_group[k], G);
+      return LFMQ_ERR_ARG;
+    }
+  const size_t need = pi_work_floats(stages, S, rows, N) * sizeof(float);
+  if (!work || work_bytes < need) {
+    LFMQ_SET_ERR("%s: work needs %zu bytes, got %llu", fn, need, (unsigned long long)work_bytes);
+    return LFMQ_ERR_WORKSPACE;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t in_sz = mc_align((size_t)rows * row_in), out_sz = mc_align((size_t)N * row_out);
+  float* xin = static_cast<float*>(work);
+  float* slots = xin + in_sz;                          // run_stages' windows of stages 1 .. S-1
+  int32_t* cg = reinterpret_cast<int32_t*>(xin + (size_t)S * in_sz);
+  float* pbuf = xin + (size_t)S * in_sz + mc_align(row_in);
+  float* preds[lfmq::LFMQ_MAX_STAGES];
+  float* vars[lfmq::LFMQ_MAX_STAGES];
+  float* pp[lfmq::LFMQ_MAX_STAGES];
+  float* vp[lfmq::LFMQ_MAX_STAGES];
+  for (int i = 0; i < S; ++i) {
+    preds[i] = pbuf + (size_t)i * out_sz;
+    vars[i] = uq ? pbuf + (size_t)(S + i) * out_sz : nullptr;
+  }
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(cg, col_group, row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  const int64_t copies = 1 + (int64_t)G * repeats;
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(out_dev, 0, copies * 3 * sizeof(float), s));
+  // copy 0 is the held-out set as it is; copy 1 + g * repeats + r has group g's columns from window pi_{seed,g,r}(i).
+  // Every launch keys its rows by window index (row0 = a), so window i draws the same dropout masks in every copy.
+  for (int64_t k = 0; k < copies; ++k) {
+    const int g = k == 0 ? -1 : (int)((k - 1) / repeats), r = k == 0 ? -1 : (int)((k - 1) % repeats);
+    for (int a = 0; a < N; a += rows) {
+      const int n = std::min(rows, N - a);
+      const float* in = x + (long)a * row_in;
+      if (k > 0) {
+        RUN(perm_importance_gather(s, x, N, row_in, cg, g, r, seed, a, n, xin));
+        in = xin;
+      }
+      for (int i = 0; i < S; ++i) {
+        pp[i] = preds[i] + (long)a * row_out;
+        vp[i] = uq ? vars[i] + (long)a * row_out : nullptr;
+      }
+      RUN(run_stages(stages, S, in, n, a, step, pp, uq ? vp : nullptr, slots, s));
+    }
+    float* o = out_dev + 3 * k;
+    if (uq && S == 1) {
+      RUN(lfmq_loss_uq(stages[0], preds[0], vars[0], y[0], N, o, stream));
+    } else if (uq) {
+      RUN(lfmq_chain_loss_uq(stages, S, preds, vars, y, weights, N, o, stream));
+    } else if (S == 1) {
+      RUN(lfmq_loss(stages[0], preds[0], y[0], N, o, stream));
+    } else {
+      RUN(lfmq_chain_loss(stages, S, preds, y, weights, N, o, stream));
+    }
+  }
+  return LFMQ_OK;
+}
+
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,
                         const float* weights, int32_t B, float* out_dev, void* stream) {
   if (!stages || n_stages < 1 || n_stages > lfmq::LFMQ_MAX_STAGES || !preds || !y || !weights || !out_dev || B <= 0) {

@@ -476,6 +476,7 @@ class ForecastChainEngine(object):
         self._w = (C.c_float * self.S)(*self.weights)
         self._work = None
         self._dp = None
+        self.device_share = None
         # Keras names: the extra layer of stage s is lstm_{L+s} / batch_normalization_{L+s-1} / OUTPUT_{s+1}
         self.specs = []            # (stage, name, shape, offset in the stage's flat vector, trainable)
         cell = kw.get('rnn_cell', 'lstm')
@@ -493,9 +494,11 @@ class ForecastChainEngine(object):
         self.n_trainable = sum(e.n_trainable for e in self.stages)
 
     def set_device_share(self, num, den):
-        """ForecasterEngine.set_device_share for every stage: the stages of a chain run one after another on one stream."""
+        """ForecasterEngine.set_device_share for every stage: the stages of a chain run one after another on one stream.
+        The share is kept in ``device_share`` (None: the whole device), for engines that run beside this one's model."""
         for e in self.stages:
             e.set_device_share(num, den)
+        self.device_share = (int(num), int(den))
 
     def set_row_weights(self, w):
         """_HandleEngine.set_row_weights for every stage: each stage's loss weighs row b of the batch by w[b]."""
@@ -542,6 +545,31 @@ class ForecastChainEngine(object):
         N.check(self.lib.lfmq_chain_forward_uq_mc(self._handles, self.S, _ptr(x), B, row0, step, samples,
                                                   *[self._ptrs(o) for o in out], _ptr(work), work.numel(), _stream()))
         return [tuple(o[s] for o in out) for s in range(self.S)]
+
+    def permutation_importance(self, x, ys, col_group, repeats, seed, step):
+        """Permutation importance of the held-out set (x, ys) in one call (lfmq_chain_permutation_importance, DESIGN.md
+        section 5e): the device tensor [1 + G * repeats, 3] of the model's loss on the unpermuted set (row 0) and on
+        every copy with group g's columns shuffled across the windows (row 1 + g * repeats + r).  col_group [T*F] maps
+        column t * F + f to its group; G = max(col_group) + 1.  Rows hold {loss, mse_0, 0}, on a uq model
+        {uq_loss, uq_loss_last_tar, mse}.  Window i draws its dropout masks at (step, row i) in every copy.  N is not
+        bounded by max_batch; the engine's parameters, gradients and optimizer state are left as they were."""
+        B = self.stages[0]._check_x(x)
+        assert len(ys) == self.S
+        ys = [y.contiguous() for y in ys]
+        for y in ys:
+            assert y.is_cuda and y.dtype == torch.float32 and y.shape[0] == B
+        cg = np.ascontiguousarray(col_group, dtype=np.int32)
+        G = int(cg.max()) + 1
+        n = C.c_uint64(0)
+        N.check(self.lib.lfmq_chain_permutation_importance_work_bytes(self._handles, self.S, B, C.byref(n)))
+        work = getattr(self, '_pi_buf', None)
+        if work is None or work.numel() < n.value:
+            work = self._pi_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=self.device)
+        out = torch.empty(max(1 + G * int(repeats), 1), 3, dtype=torch.float32, device=self.device)
+        N.check(self.lib.lfmq_chain_permutation_importance(
+            self._handles, self.S, _ptr(x), self._ptrs(ys), self._w, B, cg.ctypes.data_as(C.c_void_p), G,
+            int(repeats), int(seed), int(step), _ptr(out), _ptr(work), work.numel(), _stream()))
+        return out
 
     def loss(self, preds, ys):
         """Losses.weight_adjusted_mse(ys, preds): device tensor {loss, mse}."""

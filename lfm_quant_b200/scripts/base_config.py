@@ -110,6 +110,9 @@ SCHEMA = [
                             "UQ ensemble's ensemble_preds.dat with the calibrated lower bounds"),
     ('ig_steps', _INT, 0, 'Integrated-gradients interpolants per window at point-estimate prediction; more than 0 also '
                           'writes pred/attributions.npz: which input fields and quarters drive each forecast'),
+    ('perm_importance', _INT, 0, 'Permutation-importance repeats at prediction; more than 0 also writes '
+                                 'pred/importance.dat: how much the loss on the predicted windows rises when one input '
+                                 'field, or one quarter, is shuffled across them'),
     ('sample_weight_field', _STRING, None, 'Datafile column that weighs each training window in the training loss, read '
                                          'raw at the window\'s last input row (NaN counts as 0; negative or infinite '
                                          'values are refused); unset = off.  Ignored with --train=False'),

@@ -25,16 +25,21 @@ class NativeDenseForecaster(NativeForecaster):
             raise NotImplementedError('MLPLinearPointEstimate has one output (mlp_linear_point_estimate.py:66-77); '
                                       'forecast_steps = %d needs one per step, which the reference cannot train '
                                       'either' % config.forecast_steps)
-        engine = DenseEngine(
+        self._engine_kw = dict(
             max_batch=config.batch_size, seq_len=seq_len, n_inputs=n_inputs, n_outputs=n_outputs,
             target_idx=target_idx, precision=getattr(config, 'precision', 'fp32'), optimizer=config.optimizer,
             target_lambda=config.target_lambda, max_grad_norm=config.max_grad_norm, sgd_momentum=config.sgd_momentum,
             huber_loss=bool(config.huber_loss), huber_delta=config.huber_delta, forward_only=not config.train)
+        engine = DenseEngine(**self._engine_kw)
         specs = [(n, s) for (n, s, _, tr) in engine.specs if tr]
         rng = np.random.RandomState(config.seed)
         kernel = Initializer(config).get_initializer()(specs[0][1], rng)      # :69-73
         engine.set_weights([np.asarray(kernel, dtype=np.float32), np.zeros(specs[1][1], dtype=np.float32)])
         return ForecastChainEngine(stages=[engine])
+
+    def _new_wide_engine(self, rows):
+        from ....engine import DenseEngine, ForecastChainEngine
+        return ForecastChainEngine(stages=[DenseEngine(**dict(self._engine_kw, max_batch=rows, forward_only=True))])
 
 
 class MLPLinearPointEstimate(BaseModelClass):

@@ -14,8 +14,9 @@ from ..model_base_class import BaseModelClass
 from ...model_utils.initializers import Initializer
 from ...model_utils.optimizers import Optimizers
 
-# Rows per launch of NativeForecaster.predict_mc: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to
-# 10x (bf16x3) faster than a handle of B rows on an H100 (DESIGN.md section 5c).
+# Rows per launch of the model's wide engine (NativeForecaster._wide_engine), on which predict_mc and
+# permutation_importance run: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to 10x (bf16x3) faster
+# than a handle of B rows on an H100 (DESIGN.md section 5c).
 MC_ROWS = 8192
 # Rows per launch of NativeForecaster.attribute: the saved activations and gradients of the fp32 step grow with the rows
 # (DESIGN.md section 5d gives the workspace and the times that chose it).
@@ -119,7 +120,7 @@ class NativeForecaster(object):
         (mean_pred, mean_var, var_pred, var_var) [B,T,O].  One step per call, as predict_device; sample 0 is what
         predict_device returns at that step, sample s of window b is keyed by row s * B + b.
 
-        The samples run on an engine with room for min(samples * batch_size, MC_ROWS) rows per launch (_mc_rows_engine),
+        The samples run on an engine with room for min(samples * batch_size, MC_ROWS) rows per launch (_wide_engine),
         so that the samples of a batch share launches; the moments are the same bits on any launch size."""
         if not self.uq:
             raise ValueError('predict_mc needs a uq model (RNNUqRangeEstimate): a point estimate predicts with dropout '
@@ -127,28 +128,52 @@ class NativeForecaster(object):
         if int(samples) < 1:
             raise ValueError('predict_mc: samples must be >= 1 (got %r)' % (samples,))
         self._calls += 1
-        return self._mc_rows_engine(int(samples)).forward_mc(_to_device(self.engine, inp), int(samples),
-                                                             step=self._calls)
+        return self._wide_engine(int(samples) * self.config.batch_size).forward_mc(
+            _to_device(self.engine, inp), int(samples), step=self._calls)
 
-    def _mc_rows_engine(self, samples):
-        """The engine predict_mc runs on: the model's own (batch_size rows) when it is as wide as samples * batch_size
-        rows or MC_ROWS, as at samples = 1, where a wider handle is slower (DESIGN.md section 5c).  Else a forward-only
-        chain of the same stages and precision with max_batch = min(samples * batch_size, MC_ROWS), created at the first
-        such call (again for a larger count) and owned by the model.  It holds a copy of the weights, renewed after
-        set_weights, load_weights and the train steps."""
-        from ....engine import ForecastChainEngine
-        rows = min(samples * self.config.batch_size, MC_ROWS)
+    def permutation_importance(self, inp, targets, repeats):
+        """Permutation importance of the held-out windows (inp, targets) (ForecastChainEngine.permutation_importance,
+        DESIGN.md section 5e): the device tensors (fields [1 + F * repeats, 3], quarters [1 + T * repeats, 3]) of the
+        model's loss on the windows as they are (row 0) and with one input field's whole trajectory (column f), or all
+        fields of one quarter (t = 0 the oldest), shuffled across the windows, repeat r in row 1 + g * repeats + r.  Rows
+        hold {loss, mse_0, 0}, on a uq model {uq_loss, uq_loss_last_tar, mse}.  Both tables use config.seed and one
+        step, the model's next call, so row 0 is the same in both and a uq window draws the same dropout masks in
+        every copy.  Runs on the wide engine of min(N, MC_ROWS) rows per launch."""
+        if int(repeats) < 1:
+            raise ValueError('permutation_importance: repeats must be >= 1 (got %r)' % (repeats,))
+        x = _to_device(self.engine, inp)
+        ys = [_to_device(self.engine, t) for t in targets]
+        T, F = self.engine.T, self.engine.F
+        self._calls += 1
+        eng = self._wide_engine(x.shape[0])
+        cols = np.arange(T * F)
+        return tuple(eng.permutation_importance(x, ys, groups, int(repeats), self.config.seed, self._calls)
+                     for groups in (cols % F, cols // F))
+
+    def _wide_engine(self, rows):
+        """The forward-only engine that predict_mc and permutation_importance run on: the model's own (batch_size
+        rows) when it is as wide as `rows` or MC_ROWS, as at one sample, where a wider handle is slower (DESIGN.md
+        section 5c).  Else a forward-only chain of the same stages and precision with max_batch = min(rows, MC_ROWS)
+        and the model engine's device share, created at the first such call (again for a larger count) and owned by
+        the model.  It holds a copy of the weights, renewed after set_weights, load_weights and the train steps."""
+        rows = min(rows, MC_ROWS)
         if rows <= self.engine.cfg.max_batch:
             return self.engine
         if self._mc_engine is None or self._mc_engine.cfg.max_batch < rows:
             self._close_mc_engine()
-            self._mc_engine = ForecastChainEngine(**dict(self._engine_kw, max_batch=rows, forward_only=True))
+            self._mc_engine = self._new_wide_engine(rows)
+            if self.engine.device_share is not None:
+                self._mc_engine.set_device_share(*self.engine.device_share)
             self._mc_stale = True
         if self._mc_stale:
             for src, dst in zip(self.engine.stages, self._mc_engine.stages):
                 dst.set_flat(src.get_flat())
             self._mc_stale = False
         return self._mc_engine
+
+    def _new_wide_engine(self, rows):
+        from ....engine import ForecastChainEngine
+        return ForecastChainEngine(**dict(self._engine_kw, max_batch=rows, forward_only=True))
 
     def _close_mc_engine(self):
         if self._mc_engine is not None:

@@ -43,6 +43,7 @@ class Predict(object):
             self.model.load_weights(os.path.join(self.chkpts_dir, "chkpt"))
         outputs = defaultdict(list)
         ig = defaultdict(list)
+        held_out = []
         for (inp_dev, target_dev, metadata) in self._batches:
             # one target window per input window: every forecast step is compared with it (Train._step_targets)
             inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()] * self.config.forecast_steps
@@ -74,8 +75,12 @@ class Predict(object):
             if self.config.ig_steps > 0:
                 for key, t in zip(('attr', 'f_x', 'f_base'), self.model.attribute(inp_dev, self.config.ig_steps)):
                     ig[key].append(t.cpu().numpy())
+            if self.config.perm_importance > 0:
+                held_out.append((inp_dev, target_dev))
         if self.config.ig_steps > 0:
             self._write_attributions(outputs, ig)
+        if self.config.perm_importance > 0:
+            self._write_importance(held_out)
 
         single_outputs = ['date', 'gvkey', 'seq_norm'] + [x for x in outputs.keys() if 'inp_t' in x]
         for key in single_outputs:
@@ -142,6 +147,24 @@ class Predict(object):
                  fields=np.array(self.dataset.fin_col_names + self.dataset.aux_col_names),
                  **{k: np.concatenate(v).astype(np.float32) for k, v in ig.items()})
 
+    def _write_importance(self, held_out):
+        """<model_dir>/pred/importance.dat (--perm_importance R): the permutation importance of every input field and
+        quarter on the predicted windows (NativeForecaster.permutation_importance over all batches at once, seeded by
+        config.seed), one row per group (importance_table).  Only the windows whose targets are all known count: the
+        batcher fills the targets that lie past the data with NaN, and one NaN makes the loss NaN."""
+        import torch
+        x = torch.cat([b[0] for b in held_out])
+        y = torch.cat([b[1] for b in held_out])
+        known = torch.isfinite(y.reshape(y.shape[0], -1)).all(dim=1)
+        if not bool(known.any()):
+            raise ValueError('--perm_importance: no predicted window has known targets, so there is no loss to measure')
+        x, y = x[known].contiguous(), y[known].contiguous()
+        R = self.config.perm_importance
+        fields, quarters = self.model.permutation_importance(x, [y] * self.config.forecast_steps, R)
+        df = importance_table(fields.cpu().numpy(), quarters.cpu().numpy(), R,
+                              self.dataset.fin_col_names + self.dataset.aux_col_names, self.config.UQ)
+        df.to_csv(os.path.join(self.pred_dir, 'importance.dat'), sep=' ', index=False)
+
     def _flat(self):
         """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""
         return 'MLP' in self.config.nn_type or 'Naive' in self.config.nn_type
@@ -160,3 +183,23 @@ class Predict(object):
         if self._flat():                                 # step i of the target field: column i * F + target_index
             return np.expand_dims(inp[:, i * self.n_inputs + self.target_index], -1)
         return np.expand_dims(inp[:, i, self.target_index], -1)
+
+
+def importance_table(fields, quarters, repeats, field_names, uq):
+    """The rows of importance.dat from the two outputs of NativeForecaster.permutation_importance (fields
+    [1 + F * repeats, 3], quarters [1 + T * repeats, 3]): the fields in Dataset order, then the quarters from the oldest
+    (group 1 - T, as inp_t<k> numbers them) to the latest (0).  base_* is the unpermuted row, perm_* the mean over the
+    repeats (perm_loss_std their population standard deviation) and delta_* = perm_* - base_*.  The loss is column 0
+    (uq_loss on a uq model) and the mse column 1, column 2 on a uq model."""
+    mse = 2 if uq else 1
+    frames = []
+    for kind, out, names in (('field', fields, list(field_names)),
+                             ('quarter', quarters, list(range(1 - (len(quarters) - 1) // repeats, 1)))):
+        out = np.asarray(out, dtype=np.float64)
+        perm = out[1:].reshape(len(names), repeats, 3)
+        base_loss, base_mse = out[0, 0], out[0, mse]
+        perm_loss, perm_mse = perm[:, :, 0].mean(axis=1), perm[:, :, mse].mean(axis=1)
+        frames.append(pd.DataFrame({'kind': kind, 'group': names, 'base_loss': base_loss, 'perm_loss': perm_loss,
+                                    'perm_loss_std': perm[:, :, 0].std(axis=1), 'delta_loss': perm_loss - base_loss,
+                                    'base_mse': base_mse, 'perm_mse': perm_mse, 'delta_mse': perm_mse - base_mse}))
+    return pd.concat(frames, ignore_index=True)

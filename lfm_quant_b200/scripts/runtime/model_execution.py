@@ -346,6 +346,10 @@ class ModelExecution(object):
             raise ValueError('--ig_steps %d: integrated-gradients attributions explain the forecast of a trained '
                              'RNNPointEstimate with forecast_steps = 1 at prediction (--train=False, --UQ=False), with '
                              'ig_steps >= 1 interpolants (0 = off)' % c.ig_steps)
+        if c.perm_importance != 0 and (c.perm_importance < 0 or c.train or 'Naive' in c.nn_type):
+            raise ValueError('--perm_importance %d: permutation importance measures how a trained model uses its inputs, '
+                             'at prediction (--train=False), with perm_importance >= 1 repeats (0 = off); '
+                             'NaivePointEstimate has no model to measure' % c.perm_importance)
         check_row_weights(c)
         if c.training_type == 'iterative':
             check_walk_forward(c)
@@ -462,6 +466,11 @@ class ModelExecution(object):
             frames.append(pd.read_csv(path, sep=' ', dtype={'gvkey': str}, float_precision='round_trip'))
         df = stitch_walk_forward(frames, [origin for origin, _, _ in origins])
         df.to_csv(os.path.join(experiment_dir, 'walk_forward_preds.dat'), sep=' ', index=False)
+        if cfg.perm_importance > 0:         # how the importance drifts across the origins
+            stitch_walk_forward([pd.read_csv(os.path.join(pred.model_dir, 'pred', 'importance.dat'), sep=' ',
+                                             dtype={'group': str}, float_precision='round_trip')
+                                 for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
+                os.path.join(experiment_dir, 'walk_forward_importance.dat'), sep=' ', index=False)
         _print_scaled_mse(df, cfg.forecast_steps)
         return df
 
