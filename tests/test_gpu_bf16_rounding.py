@@ -37,11 +37,14 @@ RATIO = 1.25
 HEAD_TOL = 1e-5          # relative to the tensor's largest entry: fp32 atomics summed in another order
 
 # Max-norm relative error against the emulated oracle, per path and quantity: at least 1.5x the worst value over the
-# path's cases below, measured on an H100 80GB HBM3 (700 W power limit), rounded up to one significant digit; the worst
-# value is in the comment.  The fp64 bounds the other suites hold the same quantities to are 3e-2 (outputs, loss,
-# weights after steps) and 5e-2 / 6e-2 (gradients).  Gradients on the general path stay within 3x of those (worst
-# 1.06e-2 at T=48): the backward's tanh(c) is tanh.approx.bf16x2, off the rounded exact tanh by about one bf16 ulp, and
-# that enters every dz; the emulated oracle is no closer to the kernel than the fp64 oracle there (ratio 0.7 to 1.0).
+# path's cases below, measured on an H100 80GB HBM3 (700 W power limit), rounded up to one significant digit, except
+# where an entry says "below 1.5x"; the worst value is in the comment.  The fp64 bounds the other suites hold the same
+# quantities to are 3e-2 (outputs, loss, weights after steps) and 5e-2 / 6e-2 (gradients).  Gradients on the general path stay within 3x of those (worst
+# 1.54e-2, H=512 at T=48): the backward's tanh(c) is tanh.approx.bf16x2, off the rounded exact tanh by about one bf16
+# ulp, and that enters every dz; the emulated oracle is no closer to the kernel than the fp64 oracle there (ratio 0.7 to
+# 1.3).  The h512-l2-t48 gradients come within 1.3x of their bounds (and test_gpu_general_schedules.py's b2100 within
+# 1.4x); they were not loosened, since the kernels compute them deterministically (no atomics), so a run cannot drift
+# past a bound it once met.
 BOUNDS = {
     'cluster': {
         'pred': 2e-3,                 # 7.09e-4 (t48-f32)
@@ -59,13 +62,13 @@ BOUNDS = {
     'general': {
         'pred': 3e-3,                 # 1.90e-3 (h192-l2-t48)
         'loss': 1e-4,                 # 6.01e-5
-        'mse_0': 2e-4,                # 9.38e-5
-        'kernel': 2e-2,               # 8.10e-3
-        'recurrent_kernel': 2e-2,     # 1.06e-2
-        'bias': 2e-2,                 # 9.97e-3
+        'mse_0': 2e-4,                # 9.55e-5 (h512-l2-t48)
+        'kernel': 2e-2,               # 1.54e-2 (h512-l2-t48), below 1.5x
+        'recurrent_kernel': 2e-2,     # 1.35e-2 (h512-l2-t48), below 1.5x with b2100's 1.45e-2
+        'bias': 2e-2,                 # 1.09e-2 (h512-l2-t48), below 1.5x with b2100's 1.46e-2
         'gamma': 2e-2,                # 8.60e-3
-        'beta': 2e-2,                 # 1.03e-2
-        'OUTPUT_1/kernel': 8e-4,      # 4.84e-4
+        'beta': 2e-2,                 # 1.38e-2 (h512-l2-t48)
+        'OUTPUT_1/kernel': 8e-4,      # 4.84e-4 (H=512: CASE_BOUNDS)
         'OUTPUT_1/bias': 2e-4,        # 1.04e-4
         'weights': 3e-3,              # 1.34e-3
     },
@@ -116,13 +119,15 @@ class _Report:
     """Worst error per quantity against the emulated oracle, its bound and the ratio of the fp64-oracle error to it.
     Everything is printed before anything is asserted, so a failing case still reports all its numbers."""
 
-    def __init__(self, path, case):
+    def __init__(self, path, case, bounds=None):
         self.path, self.case = path, case
+        self.bounds = dict(BOUNDS[path], **(bounds or {}))      # `bounds`: per quantity or kind, over BOUNDS[path]
         self.rows = []
 
     def check(self, what, kind, got, emu, ref, ratio=False):
         assert np.isfinite(got).all(), (self.case, what)
-        self.rows.append((what, rel_err(got, emu), BOUNDS[self.path][kind], rel_err(got, ref), ratio))
+        bound = self.bounds.get(what, self.bounds[kind])
+        self.rows.append((what, rel_err(got, emu), bound, rel_err(got, ref), ratio))
 
     def done(self):
         for what, e, bound, e64, _ in self.rows:
@@ -138,7 +143,7 @@ def _loss_tail(eng):
     return eng.grads[eng.n_trainable:eng.n_trainable + 2].cpu().numpy()
 
 
-def _run_training_case(path, case, shape, drop, env=None):
+def _run_training_case(path, case, shape, drop, env=None, bounds=None):
     B, T, F, O, H, L = shape
     params, x, y = make_problem(B, T, F, O, H, L, seed=21, init_scale=0.3 * min(1.0, np.sqrt(32.0 / F)))
     bn = _bn_stats(L, H, seed=19)
@@ -147,7 +152,7 @@ def _run_training_case(path, case, shape, drop, env=None):
     eng = _engine(B, T, F, O, H, L, env=env, target_idx=O - 1, precision='bf16', optimizer='Adadelta',
                   max_norm=max_norm, **drop)
     eng.set_weights(params, bn_stats=bn)
-    rep = _Report(path, case)
+    rep = _Report(path, case, bounds)
     emu_p, exact_p = bo.Plan(path), bo.Plan(path, bo.identity)
     x64, y64 = x.astype(np.float64), y.astype(np.float64)
     fkw = dict(num_layers=L, training=True, step=STEP, row0=ROW0, **bkw, **drop)
@@ -219,16 +224,35 @@ GENERAL_CASES = {
     'h192-l2-f20': ((160, 5, 20, 7, 192, 2), D21, None),
     'h192-l1-f300': ((129, 4, 300, 16, 192, 1), D2, None),
     'h192-l2-t48': ((256, 48, 32, 16, 192, 2), D21, None),
+    'h512-l2-t48': ((256, 48, 32, 16, 512, 2), D21, None),        # cfg3's model (test_gpu_general_schedules.py)
     'h512-l2-f20': ((130, 4, 20, 7, 512, 2), D21, None),
     'h512-l1-f300': ((129, 4, 300, 16, 512, 1), {}, None),
     'h256-forced': ((300, 6, 32, 16, 256, 1), D2, {'LFMQ_FORCE_GENERIC': '1'}),
 }
 
 
+# Bounds looser than BOUNDS['general'], per case and quantity; worst values measured on an H100 80GB HBM3 (700 W power
+# limit) in the comments.
+# * OUTPUT_1/kernel at H=512 (here, and b2100 in test_gpu_general_schedules.py: 1.09e-3).  What is established: the
+#   kernel is closer to the emulated oracle than to the fp64 one (x3.4, b2100 x1.4); the predictions it is computed
+#   from, and every other gradient, stay within BOUNDS['general']; the error follows neither the number of rows summed
+#   (cfg3, B T = 65536, has 3.26e-4) nor the size of the prediction error (h192-l2-t48, pred 1.90e-3, stays under
+#   4.84e-4).  Its cause is not isolated.  A forward fault of 2^-7 in h at H=512 moves it to 2.7e-2 to 4.7e-2.
+# * The loss and mse_0 after the first Adadelta step follow from the first step's gradients, 1.5e-2 from both oracles
+#   (tanh.approx.bf16x2, above; ratio 0.8); the first step's own loss and mse_0 stay within BOUNDS['general'].
+CASE_BOUNDS = {
+    'h512-l2-t48': {
+        'OUTPUT_1/kernel': 2e-3,      # 1.11e-3
+        'step 1 loss': 5e-4,          # 3.18e-4
+        'step 1 mse_0': 4e-4,         # 2.05e-4
+    },
+}
+
+
 @pytest.mark.parametrize('case', list(GENERAL_CASES))
 def test_general_matches_emulated_oracle(case):
     shape, drop, env = GENERAL_CASES[case]
-    _run_training_case('general', case, shape, drop, env)
+    _run_training_case('general', case, shape, drop, env, CASE_BOUNDS.get(case))
 
 
 # test_gpu_infer_cells.py shapes
