@@ -327,6 +327,32 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
  * v = (L << h) | R; round j in 0..3 sets (L, R) <- (R, L ^ (philox4x32_10(R, j, group, repeat; seed_lo, seed_hi)[0] &
  * (2^h - 1))).  Starting from v = i, the network is applied until v < N (cycle walking). */
 int32_t lfmq_permutation_index(int32_t N, uint64_t seed, int32_t group, int32_t repeat, int32_t i, int32_t* out);
+/* ---- Shapley attributions ------------------------------------------------------------------------------------------
+ * Which groups of input columns move each window's forecast, by permutation-sampling Shapley values (Strumbelj &
+ * Kononenko 2014) with antithetic orderings (Mitchell et al. 2022).  x [N,T,F] (or [N,T*F] on a dense handle) are the
+ * model's inputs; column c = t * F + f belongs to group col_group[c] in [0, G) (host int32 [T*F]), as for permutation
+ * importance.  The K explained outputs of a window are at time step T-1 and column target_idx: pred_s of each stage
+ * (K = S), tar_1, var_1, .., tar_S, var_S on a uq chain (K = 2S), pred[:, target_idx] on a dense handle (K = 1).
+ * Sample m < samples belongs to pair p = m / 2: window i's donor is d_p(i) = lfmq_permutation_index(N, seed,
+ * 0x40000000, p, i); an even sample orders the groups by o_m[q] = lfmq_permutation_index(G, seed, 0x40000001, p, q), an
+ * odd one by the reverse of o_{m-1}.  Copy (m, k), k = 0..G, is x with the columns whose group ranks >= k in o_m taken
+ * from window d_p(i) (k = 0: the donor, k = G: x itself).  Every launch of sample m keys window i as row m * N + i at
+ * `step`: on a uq model all copies of a sample share window i's dropout masks, the ones lfmq_forward_uq_mc draws for
+ * sample m at B = N; point and dense models predict with dropout off.  Outputs (device fp32):
+ *   phi [N][K][G]: (1/M) sum_m f_m(copy (m, r + 1)) - f_m(copy (m, r)), r = the rank of g in o_m;
+ *   f_x [N][K] = (1/M) sum_m f_m(copy (m, G)), f_bg [N][K] = (1/M) sum_m f_m(copy (m, 0)),
+ * so sum_g phi = f_x - f_bg.  A window's terms are added in increasing (m, k) in fp32 without atomics and scaled by 1/M
+ * at the end: the outputs do not depend on max_batch or on where launches are cut.  Accepted: what
+ * lfmq_chain_permutation_importance accepts.  The handles' parameters, gradient buffers (tail included) and optimizer
+ * slots are left untouched.  N, G or samples < 1, a col_group value outside [0, G) or a null pointer: LFMQ_ERR_ARG.
+ * `work`: caller-owned device scratch, 256-byte aligned, of the size the *_work_bytes query gives: one launch's rows
+ * (per stage), the col_group copy, the orderings and ranks [samples][G], prev [N][K] and one launch's predictions (and
+ * variances). */
+int32_t lfmq_chain_shapley_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N, int32_t G,
+                                      int32_t samples, uint64_t* bytes);
+int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N,
+                           const int32_t* col_group, int32_t G, int32_t samples, uint64_t seed, int64_t step,
+                           float* phi, float* f_x, float* f_bg, void* work, uint64_t work_bytes, void* stream);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

@@ -1,5 +1,6 @@
-// Permutation importance (lfmq_chain_permutation_importance): the bijection that shuffles one group of input columns
-// across the held-out windows, and the kernel that builds the rows of a permuted copy.  DESIGN.md section 5e.
+// Permutation importance and Shapley attributions (lfmq_chain_permutation_importance, lfmq_chain_shapley): the
+// bijection that draws donor windows and group orderings, the kernel that builds the rows of a copy whose high-ranked
+// groups come from a donor window, and the fold of a Shapley launch's outputs.  DESIGN.md sections 5e and 5f.
 #include "../../include/lfmq.h"
 #include "kernels.h"
 
@@ -30,32 +31,68 @@ namespace {
 
 constexpr int kPermThreads = 256;
 constexpr int kPermRows = 8;      // window rows per CTA: their donors are found once, by one thread each
+constexpr int kFoldThreads = 256;
 
-// Rows [a, a + n) of copy (g, r): out[i - a, c] = x[pi(i), c] when col_group[c] == g, else x[i, c].  Each element reads
-// the one source it needs, and a CTA writes whole rows in order, so reads and writes are coalesced.
+// Rows [a, a + n) of a copy: out[i - a, c] = x[pi(i), c] when rank[col_group[c]] >= k, else x[i, c], with
+// pi = perm_index(N, seed, key, rep, .).  Each element reads the one source it needs, and a CTA writes whole rows in
+// order, so reads and writes are coalesced.
 __global__ void __launch_bounds__(kPermThreads) perm_importance_gather_kernel(
-    const float* __restrict__ x, int N, long row_elems, const int32_t* __restrict__ col_group, int g, int r,
-    uint64_t seed, int a, int n, float* __restrict__ out) {
+    const float* __restrict__ x, int N, long row_elems, const int32_t* __restrict__ col_group,
+    const int32_t* __restrict__ rank, int k, uint64_t seed, int key, int rep, int a, int n, float* __restrict__ out) {
   __shared__ int donor[kPermRows];
   const int i0 = blockIdx.x * kPermRows;
   if (threadIdx.x < kPermRows && i0 + (int)threadIdx.x < n)
-    donor[threadIdx.x] = (int)perm_index(N, seed, g, r, (uint32_t)(a + i0 + threadIdx.x));
+    donor[threadIdx.x] = (int)perm_index(N, seed, key, rep, (uint32_t)(a + i0 + threadIdx.x));
   __syncthreads();
   const int rows = min(kPermRows, n - i0);
-  for (int k = 0; k < rows; ++k) {
-    const float* own = x + (long)(a + i0 + k) * row_elems;
-    const float* don = x + (long)donor[k] * row_elems;
-    float* dst = out + (long)(i0 + k) * row_elems;
-    for (long c = threadIdx.x; c < row_elems; c += kPermThreads) dst[c] = (__ldg(col_group + c) == g ? don : own)[c];
+  for (int j = 0; j < rows; ++j) {
+    const float* own = x + (long)(a + i0 + j) * row_elems;
+    const float* don = x + (long)donor[j] * row_elems;
+    float* dst = out + (long)(i0 + j) * row_elems;
+    for (long c = threadIdx.x; c < row_elems; c += kPermThreads)
+      dst[c] = (__ldg(rank + __ldg(col_group + c)) >= k ? don : own)[c];
   }
+}
+
+// One thread per (window a + i, output o) of a launch of copy (m, k): v = src.p[o][i * stride + off].  k = 0 adds v
+// into f_bg; k > 0 adds v - prev into phi[w][o][order[k - 1]], the group copy k adds; k = G also adds v into f_x.
+// prev[w][o] = v.  A window's terms arrive in increasing (m, k), one launch after another, so its sums do not depend on
+// where launches are cut.
+__global__ void __launch_bounds__(kFoldThreads) shapley_fold_kernel(
+    ShapleySrc src, int K, long stride, long off, int a, int n, int k, int G, const int32_t* __restrict__ order,
+    float* __restrict__ prev, float* __restrict__ phi, float* __restrict__ f_x, float* __restrict__ f_bg) {
+  const int t = blockIdx.x * kFoldThreads + threadIdx.x;
+  if (t >= n * K) return;
+  const int i = t / K, o = t - i * K;
+  const float* p = src.p[0];
+#pragma unroll
+  for (int j = 1; j < 2 * LFMQ_MAX_STAGES; ++j)   // selects, not a dynamic index into the parameter array
+    if (j == o) p = src.p[j];
+  const float v = p[(long)i * stride + off];
+  const long wo = (long)(a + i) * K + o;
+  if (k == 0) {
+    f_bg[wo] += v;
+  } else {
+    phi[wo * G + order[k - 1]] += v - prev[wo];
+    if (k == G) f_x[wo] += v;
+  }
+  prev[wo] = v;
 }
 
 }  // namespace
 
-int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems, const int32_t* col_group, int g, int r,
-                           uint64_t seed, int a, int n, float* out) {
-  perm_importance_gather_kernel<<<(n + kPermRows - 1) / kPermRows, kPermThreads, 0, s>>>(x, N, row_elems, col_group, g,
-                                                                                        r, seed, a, n, out);
+int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems, const int32_t* col_group,
+                           const int32_t* rank, int k, uint64_t seed, int key, int rep, int a, int n, float* out) {
+  perm_importance_gather_kernel<<<(n + kPermRows - 1) / kPermRows, kPermThreads, 0, s>>>(
+      x, N, row_elems, col_group, rank, k, seed, key, rep, a, n, out);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+int shapley_fold(cudaStream_t s, const ShapleySrc& src, int K, long stride, long off, int a, int n, int k, int G,
+                 const int32_t* order, float* prev, float* phi, float* f_x, float* f_bg) {
+  shapley_fold_kernel<<<(n * K + kFoldThreads - 1) / kFoldThreads, kFoldThreads, 0, s>>>(src, K, stride, off, a, n, k,
+                                                                                        G, order, prev, phi, f_x, f_bg);
   LFMQ_LAUNCH_CHECK();
   return 0;
 }

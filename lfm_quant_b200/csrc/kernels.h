@@ -86,13 +86,20 @@ int ig_pick(cudaStream_t s, int n_out, int n_src, int T, int O, int target_idx, 
 // last interpolant multiplies the sum by x / M.  Launches must arrive in increasing r0 and cover [0, M * B).
 int ig_fold(cudaStream_t s, int B, int M, int64_t r0, int n, long row_elems, const float* dx, const float* x,
             float* attr);
-// Permutation importance (importance.cu, lfmq_chain_permutation_importance): perm_index is the bijection pi_{seed,g,r}
-// of [0, N) (a 4-round Philox Feistel network on [0, 2^m), cycle-walked into [0, N)); perm_importance_gather writes rows
-// [a, a + n) of copy (g, r) of x [N, row_elems] to out [n, row_elems]: columns c with col_group[c] == g (device int32
-// [row_elems]) come from window pi(i), the others from window i.
+// Permutation importance and Shapley attributions (importance.cu, lfmq_chain_permutation_importance,
+// lfmq_chain_shapley): perm_index is the bijection pi_{seed,key,rep} of [0, N) (a 4-round Philox Feistel network on
+// [0, 2^m), cycle-walked into [0, N)); perm_importance_gather writes rows [a, a + n) of a copy of x [N, row_elems] to
+// out [n, row_elems]: columns c with rank[col_group[c]] >= k (device int32 [row_elems] and [G]) come from window
+// pi_{seed,key,rep}(i), the others from window i.
 __host__ __device__ uint32_t perm_index(int32_t N, uint64_t seed, int32_t group, int32_t repeat, uint32_t i);
-int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems, const int32_t* col_group, int g, int r,
-                           uint64_t seed, int a, int n, float* out);
+int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems, const int32_t* col_group,
+                           const int32_t* rank, int k, uint64_t seed, int key, int rep, int a, int n, float* out);
+// shapley_fold: folds the K explained outputs of windows [a, a + n), src.p[o][i * stride + off] for output o of launch
+// row i, of coalition copy k (0..G) of one sample into the sums of lfmq_chain_shapley: f_bg at k = 0, f_x at k = G, and
+// for k > 0 the difference to the window's previous copy (prev [N][K]) into phi [N][K][G] at group order[k - 1].
+struct ShapleySrc { const float* p[2 * LFMQ_MAX_STAGES]; };
+int shapley_fold(cudaStream_t s, const ShapleySrc& src, int K, long stride, long off, int a, int n, int k, int G,
+                 const int32_t* order, float* prev, float* phi, float* f_x, float* f_bg);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

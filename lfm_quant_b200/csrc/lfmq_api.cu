@@ -1320,7 +1320,7 @@ int32_t lfmq_integrated_gradients(lfmq_handle h, const float* x, int32_t B, int3
   return LFMQ_OK;
 }
 
-// ---- permutation importance (lfmq_chain_permutation_importance) -----------------------------------------------------
+// ---- permutation importance and Shapley attributions (lfmq_chain_permutation_importance, lfmq_chain_shapley) -------
 namespace {
 // S >= 1 point or uq stages of one chain (chain_check numbers their dropout streams), or one dense handle.  Rows per
 // launch: N, at most the smallest max_batch.
@@ -1348,13 +1348,110 @@ int pi_check(const lfmq_handle* st, int32_t S, int32_t N, const char* fn, int* r
   return 0;
 }
 
-// floats of caller scratch: the launch's permuted rows, the chain's next-stage windows of a launch, the device copy of
-// col_group, and one copy's predictions (and variances on a uq chain) of every stage, each on a 256-byte boundary
-size_t pi_work_floats(const lfmq_handle* st, int S, int rows, int N) {
+int col_group_check(const int32_t* col_group, long row_in, int32_t G, const char* fn) {
+  for (long c = 0; c < row_in; ++c)
+    if (col_group[c] < 0 || col_group[c] >= G) {
+      LFMQ_SET_ERR("%s: col_group[%ld] = %d outside [0, G = %d)", fn, c, col_group[c], G);
+      return LFMQ_ERR_ARG;
+    }
+  return 0;
+}
+
+long row_in_of(const lfmq_handle* st) { return (long)st[0]->cfg.seq_len * st[0]->cfg.n_inputs; }
+long row_out_of(const lfmq_handle* st) {
   const lfmq_config& c = st[0]->cfg;
-  const size_t row_in = (size_t)c.seq_len * c.n_inputs;
-  const size_t row_out = st[0]->path == Path::Dense ? (size_t)c.n_outputs : (size_t)c.seq_len * c.n_outputs;
-  return (size_t)S * mc_align(rows * row_in) + mc_align(row_in) + (c.uq ? 2 : 1) * (size_t)S * mc_align(N * row_out);
+  return st[0]->path == Path::Dense ? (long)c.n_outputs : (long)c.seq_len * c.n_outputs;
+}
+
+// Where a Shapley launch's outputs are folded (shapley_fold): the K value pointers with their row stride and offset,
+// the ordering of the sample being run, and the sums.
+struct ShapleyFold {
+  lfmq::ShapleySrc src;
+  int K;
+  long stride, off;
+  int G;
+  const int32_t* order;  // o_m of the sample being run
+  float *prev, *phi, *f_x, *f_bg;
+};
+
+// The forward of one copy of x [N, row_in] in launches of at most `rows` windows, in window order.  Launch [a, a + n)
+// builds its rows with the columns whose group ranks >= k in `rank` (device int32, indexed by the device col_group cg)
+// taken from window perm_index(N, seed, key, rep, i), or forwards x's own rows when rank == nullptr, and runs every
+// stage with dropout keyed by row row_base + i.  Predictions (and variances on a uq chain) go to preds / vars at row a
+// when `whole` (copy-sized buffers), else at row 0 (launch-sized ones), where `fold` (nullable) folds each launch's
+// outputs as copy k into the Shapley sums.
+struct CopyForward {
+  const lfmq_handle* st;
+  int S;
+  const float* x;
+  int N, rows;
+  long row_in, row_out;
+  const int32_t* cg;
+  uint64_t seed;
+  int64_t step;
+  float* xin;       // the launch's gathered rows
+  float* slots;     // run_stages' windows of stages 1 .. S-1
+  float* const* preds;
+  float* const* vars;  // nullptr on a point or dense model
+  bool whole;
+  cudaStream_t s;
+
+  int run(const int32_t* rank, int k, int key, int rep, int64_t row_base, const ShapleyFold* fold) const {
+    float* pp[lfmq::LFMQ_MAX_STAGES];
+    float* vp[lfmq::LFMQ_MAX_STAGES];
+    for (int a = 0; a < N; a += rows) {
+      const int n = std::min(rows, N - a);
+      const float* in = x + (long)a * row_in;
+      if (rank) {
+        RUN(perm_importance_gather(s, x, N, row_in, cg, rank, k, seed, key, rep, a, n, xin));
+        in = xin;
+      }
+      const long off = whole ? (long)a * row_out : 0;
+      for (int i = 0; i < S; ++i) {
+        pp[i] = preds[i] + off;
+        vp[i] = vars ? vars[i] + off : nullptr;
+      }
+      RUN(run_stages(st, S, in, n, row_base + a, step, pp, vars ? vp : nullptr, slots, s));
+      if (fold)
+        RUN(shapley_fold(s, fold->src, fold->K, fold->stride, fold->off, a, n, k, fold->G, fold->order, fold->prev,
+                         fold->phi, fold->f_x, fold->f_bg));
+    }
+    return 0;
+  }
+};
+
+// floats of caller scratch: the launch's permuted rows, the chain's next-stage windows of a launch, the device copy of
+// col_group with its groups numbered densely, the one-hot rank rows, and one copy's predictions (and variances on a uq
+// chain) of every stage, each on a 256-byte boundary
+size_t pi_work_floats(const lfmq_handle* st, int S, int rows, int N) {
+  const size_t row_in = row_in_of(st), row_out = row_out_of(st);
+  return (size_t)S * mc_align(rows * row_in) + mc_align(row_in) + mc_align(2 * row_in) +
+         (st[0]->cfg.uq ? 2 : 1) * (size_t)S * mc_align(N * row_out);
+}
+
+// Shapley: the perm_index keys of the donor windows and of the group orderings (DESIGN.md section 5f)
+constexpr int kShapleyDonorKey = 0x40000000, kShapleyOrderKey = 0x40000001;
+
+// Shapley: one output per stage (two on a uq chain: target and variance), one on a dense handle
+int shapley_outputs(const lfmq_handle* st, int S) {
+  return st[0]->path == Path::Dense ? 1 : (st[0]->cfg.uq ? 2 * S : S);
+}
+
+// floats of caller scratch: the launch's coalition rows, the chain's next-stage windows of a launch, the device copy of
+// col_group, the samples' group orderings and ranks [samples][G] each, prev [N][K], and one launch's predictions (and
+// variances on a uq chain) of every stage, each on a 256-byte boundary
+size_t shapley_work_floats(const lfmq_handle* st, int S, int rows, int N, int G, int samples) {
+  const size_t row_in = row_in_of(st), row_out = row_out_of(st);
+  return (size_t)S * mc_align(rows * row_in) + mc_align(row_in) + 2 * mc_align((size_t)samples * G) +
+         mc_align((size_t)N * shapley_outputs(st, S)) + (st[0]->cfg.uq ? 2 : 1) * (size_t)S * mc_align(rows * row_out);
+}
+
+int shapley_args_check(int32_t N, int32_t G, int32_t samples, const char* fn) {
+  if (N < 1 || G < 1 || samples < 1) {
+    LFMQ_SET_ERR("%s: need N, G and samples >= 1 (got %d, %d, %d)", fn, N, G, samples);
+    return LFMQ_ERR_ARG;
+  }
+  return 0;
 }
 }  // namespace
 
@@ -1379,9 +1476,8 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
   RUN(pi_check(stages, n_stages, N, fn, &rows));
   const int S = n_stages;
   const lfmq_config& c = stages[0]->cfg;
-  const bool dense = stages[0]->path == Path::Dense, uq = c.uq != 0;
-  const long row_in = (long)c.seq_len * c.n_inputs;
-  const long row_out = dense ? c.n_outputs : (long)c.seq_len * c.n_outputs;
+  const bool uq = c.uq != 0;
+  const long row_in = row_in_of(stages), row_out = row_out_of(stages);
   if (G < 1 || repeats < 1) {
     LFMQ_SET_ERR("%s: need G >= 1 and repeats >= 1 (got %d, %d)", fn, G, repeats);
     return LFMQ_ERR_ARG;
@@ -1395,11 +1491,7 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
       LFMQ_SET_ERR("%s: y[%d] == NULL", fn, i);
       return LFMQ_ERR_ARG;
     }
-  for (long k = 0; k < row_in; ++k)
-    if (col_group[k] < 0 || col_group[k] >= G) {
-      LFMQ_SET_ERR("%s: col_group[%ld] = %d outside [0, G = %d)", fn, k, col_group[k], G);
-      return LFMQ_ERR_ARG;
-    }
+  RUN(col_group_check(col_group, row_in, G, fn));
   const size_t need = pi_work_floats(stages, S, rows, N) * sizeof(float);
   if (!work || work_bytes < need) {
     LFMQ_SET_ERR("%s: work needs %zu bytes, got %llu", fn, need, (unsigned long long)work_bytes);
@@ -1408,37 +1500,43 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
   cudaStream_t s = (cudaStream_t)stream;
   const size_t in_sz = mc_align((size_t)rows * row_in), out_sz = mc_align((size_t)N * row_out);
   float* xin = static_cast<float*>(work);
-  float* slots = xin + in_sz;                          // run_stages' windows of stages 1 .. S-1
   int32_t* cg = reinterpret_cast<int32_t*>(xin + (size_t)S * in_sz);
-  float* pbuf = xin + (size_t)S * in_sz + mc_align(row_in);
+  int32_t* onehot = cg + mc_align(row_in);
+  float* pbuf = xin + (size_t)S * in_sz + mc_align(row_in) + mc_align(2 * row_in);
   float* preds[lfmq::LFMQ_MAX_STAGES];
   float* vars[lfmq::LFMQ_MAX_STAGES];
-  float* pp[lfmq::LFMQ_MAX_STAGES];
-  float* vp[lfmq::LFMQ_MAX_STAGES];
   for (int i = 0; i < S; ++i) {
     preds[i] = pbuf + (size_t)i * out_sz;
     vars[i] = uq ? pbuf + (size_t)(S + i) * out_sz : nullptr;
   }
-  LFMQ_CUDA_CHECK(cudaMemcpyAsync(cg, col_group, row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  // The gather takes group g's columns from the donor through a rank row that is 1 at g and 0 elsewhere.  G may exceed
+  // the columns, so the device col_group numbers the D <= row_in groups present densely (u), and the rank row of
+  // group g is the window onehot + D - 1 - u(g) of onehot [2D] = e_{D-1}; a group with no columns reads onehot + D,
+  // all zeros, and its copy is x.
+  std::vector<int32_t> ids(col_group, col_group + row_in);
+  std::sort(ids.begin(), ids.end());
+  ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+  const int D = (int)ids.size();
+  std::vector<int32_t> dense_cg(row_in), hot(2 * D, 0);
+  for (long k = 0; k < row_in; ++k)
+    dense_cg[k] = (int32_t)(std::lower_bound(ids.begin(), ids.end(), col_group[k]) - ids.begin());
+  hot[D - 1] = 1;
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(cg, dense_cg.data(), row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(onehot, hot.data(), 2 * D * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   const int64_t copies = 1 + (int64_t)G * repeats;
   LFMQ_CUDA_CHECK(cudaMemsetAsync(out_dev, 0, copies * 3 * sizeof(float), s));
+  const CopyForward cf{stages, S, x, N, rows, row_in, row_out, cg, seed, step, xin, xin + in_sz, preds,
+                       uq ? vars : nullptr, true, s};
   // copy 0 is the held-out set as it is; copy 1 + g * repeats + r has group g's columns from window pi_{seed,g,r}(i).
   // Every launch keys its rows by window index (row0 = a), so window i draws the same dropout masks in every copy.
   for (int64_t k = 0; k < copies; ++k) {
     const int g = k == 0 ? -1 : (int)((k - 1) / repeats), r = k == 0 ? -1 : (int)((k - 1) % repeats);
-    for (int a = 0; a < N; a += rows) {
-      const int n = std::min(rows, N - a);
-      const float* in = x + (long)a * row_in;
-      if (k > 0) {
-        RUN(perm_importance_gather(s, x, N, row_in, cg, g, r, seed, a, n, xin));
-        in = xin;
-      }
-      for (int i = 0; i < S; ++i) {
-        pp[i] = preds[i] + (long)a * row_out;
-        vp[i] = uq ? vars[i] + (long)a * row_out : nullptr;
-      }
-      RUN(run_stages(stages, S, in, n, a, step, pp, uq ? vp : nullptr, slots, s));
+    const int32_t* rank = nullptr;
+    if (k > 0) {
+      const auto it = std::lower_bound(ids.begin(), ids.end(), g);
+      rank = onehot + (it != ids.end() && *it == g ? D - 1 - (int)(it - ids.begin()) : D);
     }
+    RUN(cf.run(rank, 1, g, r, 0, nullptr));
     float* o = out_dev + 3 * k;
     if (uq && S == 1) {
       RUN(lfmq_loss_uq(stages[0], preds[0], vars[0], y[0], N, o, stream));
@@ -1450,6 +1548,98 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
       RUN(lfmq_chain_loss(stages, S, preds, y, weights, N, o, stream));
     }
   }
+  return LFMQ_OK;
+}
+
+int32_t lfmq_chain_shapley_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N, int32_t G,
+                                      int32_t samples, uint64_t* bytes) {
+  const char* fn = "lfmq_chain_shapley_work_bytes";
+  int rows = 0;
+  RUN(pi_check(stages, n_stages, N, fn, &rows));
+  RUN(shapley_args_check(N, G, samples, fn));
+  if (!bytes) {
+    LFMQ_SET_ERR("%s: bytes == NULL", fn);
+    return LFMQ_ERR_ARG;
+  }
+  *bytes = shapley_work_floats(stages, n_stages, rows, N, G, samples) * sizeof(float);
+  return LFMQ_OK;
+}
+
+int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N,
+                           const int32_t* col_group, int32_t G, int32_t samples, uint64_t seed, int64_t step,
+                           float* phi, float* f_x, float* f_bg, void* work, uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_chain_shapley";
+  int rows = 0;
+  RUN(pi_check(stages, n_stages, N, fn, &rows));
+  RUN(shapley_args_check(N, G, samples, fn));
+  const int S = n_stages, M = samples, K = shapley_outputs(stages, S);
+  const lfmq_config& c = stages[0]->cfg;
+  const bool dense = stages[0]->path == Path::Dense, uq = c.uq != 0;
+  const long row_in = row_in_of(stages), row_out = row_out_of(stages);
+  if (!x || !col_group || !phi || !f_x || !f_bg) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  RUN(col_group_check(col_group, row_in, G, fn));
+  const size_t need = shapley_work_floats(stages, S, rows, N, G, M) * sizeof(float);
+  if (!work || work_bytes < need) {
+    LFMQ_SET_ERR("%s: work needs %zu bytes, got %llu", fn, need, (unsigned long long)work_bytes);
+    return LFMQ_ERR_WORKSPACE;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t in_sz = mc_align((size_t)rows * row_in), tab_sz = mc_align((size_t)M * G);
+  const size_t out_sz = mc_align((size_t)rows * row_out);
+  float* xin = static_cast<float*>(work);
+  int32_t* cg = reinterpret_cast<int32_t*>(xin + (size_t)S * in_sz);
+  int32_t* order = cg + mc_align(row_in);
+  int32_t* rank = order + tab_sz;
+  float* prev = reinterpret_cast<float*>(rank + tab_sz);
+  float* pbuf = prev + mc_align((size_t)N * K);
+  float* preds[lfmq::LFMQ_MAX_STAGES];
+  float* vars[lfmq::LFMQ_MAX_STAGES];
+  // the explained value of a launch row: pred[T-1, target_idx] ([target_idx] on a dense handle)
+  ShapleyFold fold{{}, K, row_out, dense ? c.target_idx : (long)(c.seq_len - 1) * c.n_outputs + c.target_idx, G,
+                   nullptr, prev, phi, f_x, f_bg};
+  for (int i = 0; i < S; ++i) {
+    preds[i] = pbuf + (size_t)i * out_sz;
+    vars[i] = uq ? pbuf + (size_t)(S + i) * out_sz : nullptr;
+    if (uq) {                                    // Keras list order: tar_1, var_1, .., tar_S, var_S
+      fold.src.p[2 * i] = preds[i];
+      fold.src.p[2 * i + 1] = vars[i];
+    } else {
+      fold.src.p[i] = preds[i];
+    }
+  }
+  // Sample m belongs to pair p = m / 2.  An even sample orders the groups by o[q] = perm_index(G, seed, 0x40000001,
+  // p, q); an odd one reverses its partner's ordering (antithetic) and keeps its donors.
+  std::vector<int32_t> ord((size_t)M * G), rk((size_t)M * G);
+  for (int m = 0; m < M; ++m)
+    for (int q = 0; q < G; ++q) {
+      int32_t* o = ord.data() + (size_t)m * G;
+      o[q] = (m % 2 == 0) ? (int32_t)lfmq::perm_index(G, seed, kShapleyOrderKey, m / 2, (uint32_t)q)
+                          : ord[(size_t)(m - 1) * G + (G - 1 - q)];
+      rk[(size_t)m * G + o[q]] = q;
+    }
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(cg, col_group, row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(order, ord.data(), ord.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(rank, rk.data(), rk.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(phi, 0, (size_t)N * K * G * sizeof(float), s));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(f_x, 0, (size_t)N * K * sizeof(float), s));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(f_bg, 0, (size_t)N * K * sizeof(float), s));
+  const CopyForward cf{stages, S, x, N, rows, row_in, row_out, cg, seed, step, xin, xin + in_sz, preds,
+                       uq ? vars : nullptr, false, s};
+  // Copy (m, k) takes the groups ranked >= k in o_m from window d_p(i) = perm_index(N, seed, 0x40000000, p, i): k = 0
+  // is the donor, k = G is x itself, forwarded without a gather.  Every launch of sample m keys window i as row
+  // m * N + i, so a uq window shares its dropout masks across the copies of one sample.
+  for (int m = 0; m < M; ++m) {
+    fold.order = order + (size_t)m * G;
+    for (int k = 0; k <= G; ++k)
+      RUN(cf.run(k < G ? rank + (size_t)m * G : nullptr, k, kShapleyDonorKey, m / 2, (int64_t)m * N, &fold));
+  }
+  const float inv = 1.0f / (float)M;
+  RUN(scale_inplace(s, (long)N * K * G, phi, inv));
+  RUN(scale_inplace(s, (long)N * K, f_x, inv));
+  RUN(scale_inplace(s, (long)N * K, f_bg, inv));
   return LFMQ_OK;
 }
 

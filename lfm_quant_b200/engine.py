@@ -571,6 +571,31 @@ class ForecastChainEngine(object):
             int(repeats), int(seed), int(step), _ptr(out), _ptr(work), work.numel(), _stream()))
         return out
 
+    def shapley(self, x, col_group, samples, seed, step):
+        """Shapley attributions of every window's forecast in one call (lfmq_chain_shapley, DESIGN.md section 5f):
+        device tensors (phi [N,K,G], f_x [N,K], f_bg [N,K]), sum_g phi = f_x - f_bg.  The K outputs are pred[:, T-1,
+        target_idx] of every stage (tar_1, var_1, .., tar_S, var_S on a uq model; pred[:, target_idx] on a dense
+        stage).  col_group [T*F] maps column t * F + f to its group; G = max(col_group) + 1.  `samples` orderings of the
+        groups, in antithetic pairs, each against a donor window; a uq window draws its dropout masks at (step, row
+        m * N + i) for sample m.  N is not bounded by max_batch; the engine's parameters, gradients and optimizer state
+        are left as they were."""
+        B = self.stages[0]._check_x(x)
+        cg = np.ascontiguousarray(col_group, dtype=np.int32)
+        G, M = int(cg.max()) + 1, int(samples)
+        K = 1 if isinstance(self.stages[0], DenseEngine) else (2 * self.S if self.uq else self.S)
+        n = C.c_uint64(0)
+        N.check(self.lib.lfmq_chain_shapley_work_bytes(self._handles, self.S, B, G, M, C.byref(n)))
+        work = getattr(self, '_sh_buf', None)
+        if work is None or work.numel() < n.value:
+            work = self._sh_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=self.device)
+        phi = torch.empty(B, K, G, dtype=torch.float32, device=self.device)
+        f_x = torch.empty(B, K, dtype=torch.float32, device=self.device)
+        f_bg = torch.empty(B, K, dtype=torch.float32, device=self.device)
+        N.check(self.lib.lfmq_chain_shapley(
+            self._handles, self.S, _ptr(x), B, cg.ctypes.data_as(C.c_void_p), G, M, int(seed), int(step), _ptr(phi),
+            _ptr(f_x), _ptr(f_bg), _ptr(work), work.numel(), _stream()))
+        return phi, f_x, f_bg
+
     def loss(self, preds, ys):
         """Losses.weight_adjusted_mse(ys, preds): device tensor {loss, mse}."""
         if self._one is not None:

@@ -113,6 +113,9 @@ SCHEMA = [
     ('perm_importance', _INT, 0, 'Permutation-importance repeats at prediction; more than 0 also writes '
                                  'pred/importance.dat: how much the loss on the predicted windows rises when one input '
                                  'field, or one quarter, is shuffled across them'),
+    ('shapley_samples', _INT, 0, 'Shapley permutation samples (antithetic pairs) per window at prediction; more than 0 '
+                                 'also writes pred/shapley.npz: how much each input field and each quarter moves every '
+                                 'window\'s forecast (and a UQ model\'s variance) away from a donor window\'s'),
     ('sample_weight_field', _STRING, None, 'Datafile column that weighs each training window in the training loss, read '
                                          'raw at the window\'s last input row (NaN counts as 0; negative or infinite '
                                          'values are refused); unset = off.  Ignored with --train=False'),

@@ -14,9 +14,9 @@ from ..model_base_class import BaseModelClass
 from ...model_utils.initializers import Initializer
 from ...model_utils.optimizers import Optimizers
 
-# Rows per launch of the model's wide engine (NativeForecaster._wide_engine), on which predict_mc and
-# permutation_importance run: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to 10x (bf16x3) faster
-# than a handle of B rows on an H100 (DESIGN.md section 5c).
+# Rows per launch of the model's wide engine (NativeForecaster._wide_engine), on which predict_mc,
+# permutation_importance and shapley run: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to 10x
+# (bf16x3) faster than a handle of B rows on an H100 (DESIGN.md section 5c).
 MC_ROWS = 8192
 # Rows per launch of NativeForecaster.attribute: the saved activations and gradients of the fp32 step grow with the rows
 # (DESIGN.md section 5d gives the workspace and the times that chose it).
@@ -150,12 +150,31 @@ class NativeForecaster(object):
         return tuple(eng.permutation_importance(x, ys, groups, int(repeats), self.config.seed, self._calls)
                      for groups in (cols % F, cols // F))
 
+    def shapley(self, inp, samples):
+        """Shapley attributions of every window's forecast (ForecastChainEngine.shapley, DESIGN.md section 5f): the
+        device tensors (phi_fields [N,K,F], phi_quarters [N,K,T], f_x [N,K], f_bg [N,K]) that split each explained
+        output, f_x - f_bg, over the input fields (column f of every quarter) and over the quarters (all fields of
+        quarter t, t = 0 the oldest).  The K outputs are norm_preds_s at the last step, and norm_variance_s after each
+        on a uq model (tar_1, var_1, ..).  Both partitions use config.seed and one step, the model's next call, so f_x
+        and f_bg are the same bits in both; on a uq model f_x is the mean of `samples` Monte-Carlo dropout draws.  Runs
+        on the wide engine of min(N, MC_ROWS) rows per launch."""
+        if int(samples) < 1:
+            raise ValueError('shapley: samples must be >= 1 (got %r)' % (samples,))
+        x = _to_device(self.engine, inp)
+        T, F = self.engine.T, self.engine.F
+        self._calls += 1
+        eng = self._wide_engine(x.shape[0])
+        cols = np.arange(T * F)
+        (phi_f, f_x, f_bg), (phi_q, _, _) = (eng.shapley(x, groups, int(samples), self.config.seed, self._calls)
+                                             for groups in (cols % F, cols // F))
+        return phi_f, phi_q, f_x, f_bg
+
     def _wide_engine(self, rows):
-        """The forward-only engine that predict_mc and permutation_importance run on: the model's own (batch_size
-        rows) when it is as wide as `rows` or MC_ROWS, as at one sample, where a wider handle is slower (DESIGN.md
-        section 5c).  Else a forward-only chain of the same stages and precision with max_batch = min(rows, MC_ROWS)
-        and the model engine's device share, created at the first such call (again for a larger count) and owned by
-        the model.  It holds a copy of the weights, renewed after set_weights, load_weights and the train steps."""
+        """The forward-only engine that predict_mc, permutation_importance and shapley run on: the model's own
+        (batch_size rows) when it is as wide as `rows` or MC_ROWS, as at one sample, where a wider handle is slower
+        (DESIGN.md section 5c).  Else a forward-only chain of the same stages and precision with max_batch =
+        min(rows, MC_ROWS) and the model engine's device share, created at the first such call (again for a larger
+        count) and owned by the model.  It holds a copy of the weights, renewed after set_weights, load_weights and the train steps."""
         rows = min(rows, MC_ROWS)
         if rows <= self.engine.cfg.max_batch:
             return self.engine

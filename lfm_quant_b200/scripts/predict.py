@@ -44,6 +44,7 @@ class Predict(object):
         outputs = defaultdict(list)
         ig = defaultdict(list)
         held_out = []
+        windows = []
         for (inp_dev, target_dev, metadata) in self._batches:
             # one target window per input window: every forecast step is compared with it (Train._step_targets)
             inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()] * self.config.forecast_steps
@@ -77,10 +78,14 @@ class Predict(object):
                     ig[key].append(t.cpu().numpy())
             if self.config.perm_importance > 0:
                 held_out.append((inp_dev, target_dev))
+            if self.config.shapley_samples > 0:
+                windows.append(inp_dev)
         if self.config.ig_steps > 0:
             self._write_attributions(outputs, ig)
         if self.config.perm_importance > 0:
             self._write_importance(held_out)
+        if self.config.shapley_samples > 0:
+            self._write_shapley(outputs, windows)
 
         single_outputs = ['date', 'gvkey', 'seq_norm'] + [x for x in outputs.keys() if 'inp_t' in x]
         for key in single_outputs:
@@ -165,6 +170,17 @@ class Predict(object):
                               self.dataset.fin_col_names + self.dataset.aux_col_names, self.config.UQ)
         df.to_csv(os.path.join(self.pred_dir, 'importance.dat'), sep=' ', index=False)
 
+    def _write_shapley(self, outputs, windows):
+        """<model_dir>/pred/shapley.npz (--shapley_samples M): the Shapley attributions of every predicted window, known
+        targets or not, in preds.dat's row order (NativeForecaster.shapley over all batches at once, seeded by
+        config.seed; write_shapley gives the layout)."""
+        import torch
+        phi_f, phi_q, f_x, f_bg = (t.cpu().numpy() for t in
+                                   self.model.shapley(torch.cat(windows), self.config.shapley_samples))
+        write_shapley(os.path.join(self.pred_dir, 'shapley.npz'), np.vstack(outputs['date']).flatten(),
+                      np.vstack(outputs['gvkey']).flatten(), self.dataset.fin_col_names + self.dataset.aux_col_names,
+                      shapley_output_names(self.config.forecast_steps, self.config.UQ), phi_f, phi_q, f_x, f_bg)
+
     def _flat(self):
         """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""
         return 'MLP' in self.config.nn_type or 'Naive' in self.config.nn_type
@@ -203,3 +219,23 @@ def importance_table(fields, quarters, repeats, field_names, uq):
                                     'perm_loss_std': perm[:, :, 0].std(axis=1), 'delta_loss': perm_loss - base_loss,
                                     'base_mse': base_mse, 'perm_mse': perm_mse, 'delta_mse': perm_mse - base_mse}))
     return pd.concat(frames, ignore_index=True)
+
+
+def shapley_output_names(forecast_steps, uq):
+    """The outputs NativeForecaster.shapley explains, as preds.dat names their normalised columns: norm_preds_s, and
+    on a uq model norm_variance_s after each."""
+    kinds = ('norm_preds', 'norm_variance') if uq else ('norm_preds',)
+    return ['%s_%d' % (k, s) for s in range(1, forecast_steps + 1) for k in kinds]
+
+
+def write_shapley(path, date, gvkey, field_names, outputs, phi_field, phi_quarter, f_x, f_bg):
+    """shapley.npz: date [N] (yyyymmdd), gvkey [N], fields [F] (Dataset order), quarters [T] (1 - T .. 0, as inp_t<k>
+    numbers them), outputs [K] (shapley_output_names), phi_field [N,K,F], phi_quarter [N,K,T], f_x [N,K] and f_bg
+    [N,K], in normalised units: phi_field[i, k].sum() and phi_quarter[i, k].sum() are each f_x[i, k] - f_bg[i, k]."""
+    T = np.shape(phi_quarter)[2]
+    np.savez(path, date=np.asarray(date).astype(np.int32),
+             gvkey=np.array([g.decode('utf-8') if isinstance(g, bytes) else str(g) for g in gvkey]),
+             fields=np.array(list(field_names)), quarters=np.arange(1 - T, 1, dtype=np.int32),
+             outputs=np.array(list(outputs)), phi_field=np.asarray(phi_field, dtype=np.float32),
+             phi_quarter=np.asarray(phi_quarter, dtype=np.float32), f_x=np.asarray(f_x, dtype=np.float32),
+             f_bg=np.asarray(f_bg, dtype=np.float32))

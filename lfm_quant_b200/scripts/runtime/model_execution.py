@@ -350,6 +350,10 @@ class ModelExecution(object):
             raise ValueError('--perm_importance %d: permutation importance measures how a trained model uses its inputs, '
                              'at prediction (--train=False), with perm_importance >= 1 repeats (0 = off); '
                              'NaivePointEstimate has no model to measure' % c.perm_importance)
+        if c.shapley_samples != 0 and (c.shapley_samples < 0 or c.train or 'Naive' in c.nn_type):
+            raise ValueError('--shapley_samples %d: Shapley attributions explain the forecasts of a trained model, at '
+                             'prediction (--train=False), with shapley_samples >= 1 permutation samples (0 = off); '
+                             'NaivePointEstimate has no model to explain' % c.shapley_samples)
         check_row_weights(c)
         if c.training_type == 'iterative':
             check_walk_forward(c)
