@@ -154,16 +154,18 @@ __device__ __forceinline__ void dropout_quad(const DropoutKey& k, uint64_t q, fl
 // softplus of the variance head (custom_layers.py:12-13), shared by the SIMT and tensor-core heads
 __device__ __forceinline__ float softplus_f(float a) { return fmaxf(a, 0.f) + log1pf(expf(-fabsf(a))); }
 
-// Carves the caller's workspace into buffers on 1024-byte boundaries; with base == nullptr it only sizes.
+// Carves the caller's workspace into buffers on `granule`-byte boundaries (the handle workspace's 1024 by default);
+// with base == nullptr it only sizes.
 constexpr size_t WS_ALIGN = 1024;
 inline size_t ws_align_up(size_t v) { return (v + WS_ALIGN - 1) / WS_ALIGN * WS_ALIGN; }
 struct Carver {
   char* base;
   size_t off;
+  size_t granule = WS_ALIGN;
   template <typename T>
   T* take(size_t n) {
     T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off = ws_align_up(off + n * sizeof(T));
+    off = (off + n * sizeof(T) + granule - 1) / granule * granule;
     return p;
   }
 };

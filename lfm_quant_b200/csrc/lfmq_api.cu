@@ -612,6 +612,39 @@ int backward_stages(const lfmq_handle* st, int S, const float* x, const float* c
   return backward_fp32(st[0], x, B, s);
 }
 
+// The analyses carve the caller's work on 256-byte granules of the work pointer, with one layout function each: run on
+// base == nullptr it gives the size their *_work_bytes report, run on work it gives the buffers.
+constexpr size_t kWorkGranule = 256;
+
+template <typename Layout>
+size_t work_size(const Layout& layout) {
+  Carver cv{nullptr, 0, kWorkGranule};
+  layout(cv);
+  return cv.off;
+}
+
+template <typename Layout>
+int32_t report_work_bytes(uint64_t* bytes, const char* fn, const Layout& layout) {
+  if (!bytes) {
+    LFMQ_SET_ERR("%s: bytes == NULL", fn);
+    return LFMQ_ERR_ARG;
+  }
+  *bytes = work_size(layout);
+  return LFMQ_OK;
+}
+
+// *out = the buffers `layout` carves from work, which must hold all of them
+template <typename Layout, typename Work>
+int carve_work(void* work, uint64_t work_bytes, const char* fn, const Layout& layout, Work* out) {
+  const size_t need = work_size(layout);
+  if (!work || work_bytes < need) {
+    LFMQ_SET_ERR("%s: work needs %zu bytes, got %llu", fn, need, (unsigned long long)work_bytes);
+    return LFMQ_ERR_WORKSPACE;
+  }
+  Carver cv{static_cast<char*>(work), 0, kWorkGranule};
+  *out = layout(cv);
+  return 0;
+}
 }  // namespace
 
 // =============================================================================================
@@ -1095,62 +1128,90 @@ int32_t lfmq_chain_forward_uq(const lfmq_handle* stages, int32_t n_stages, const
 
 // ---- Monte-Carlo dropout samples of a uq model (lfmq_forward_uq_mc, lfmq_chain_forward_uq_mc) ----------------------
 namespace {
-// The stages' common checks; rows per launch = the smallest max_batch.  Leaves tc.stream_base alone: the chain entry
-// point has numbered the streams already, and a single handle keeps its own.
-int mc_check(const lfmq_handle* st, int32_t S, int32_t B, int32_t samples, const char* fn, int* chunk_max) {
+// The stages of a forecast analysis, 1 <= S <= LFMQ_MAX_STAGES of them (the caller checks S beside its own sizes):
+// non-null handles of one chain, or one dense handle as a model of one stage.  With `chain`, chain_check numbers the
+// stages' dropout streams; without it a single handle keeps its own tc.stream_base.  *max_rows: the smallest
+// max_batch, the rows one launch may hold.
+int stages_check(const lfmq_handle* st, int32_t S, bool chain, const char* fn, int* max_rows) {
+  for (int i = 0; i < S; ++i)
+    if (!st[i]) {
+      LFMQ_SET_ERR("%s: stage %d is a null handle", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+  if (st[0]->path == Path::Dense && S != 1) {
+    LFMQ_SET_ERR("%s: a dense handle is a model of one stage (got n_stages %d)", fn, S);
+    return LFMQ_ERR_ARG;
+  }
+  if (chain && st[0]->path != Path::Dense) RUN(chain_check(st, S, 1, false));
+  int mb = st[0]->cfg.max_batch;
+  for (int i = 1; i < S; ++i) mb = std::min(mb, (int)st[i]->cfg.max_batch);
+  *max_rows = mb;
+  return 0;
+}
+
+// The sizes, uq handles only, then stages_check.  Rows per launch: at most the smallest max_batch.
+int mc_check(const lfmq_handle* st, int32_t S, int32_t B, int32_t samples, bool chain, const char* fn,
+             int* chunk_max) {
   if (!st || S < 1 || S > lfmq::LFMQ_MAX_STAGES || B < 1 || samples < 1) {
     LFMQ_SET_ERR("%s: need 1 <= n_stages <= %d, B >= 1 and samples >= 1 (got %d, %d, %d)", fn, lfmq::LFMQ_MAX_STAGES, S,
                  B, samples);
     return LFMQ_ERR_ARG;
   }
-  int mb = 0;
-  for (int i = 0; i < S; ++i) {
+  for (int i = 0; i < S; ++i)
     if (!st[i] || !st[i]->cfg.uq) {
       LFMQ_SET_ERR("%s: stage %d is not a uq handle: only RNNUqRangeEstimate keeps dropout on at prediction time, a "
                    "point-estimate model would give the same prediction for every sample", fn, i);
       return LFMQ_ERR_ARG;
     }
-    mb = (i == 0) ? st[i]->cfg.max_batch : std::min(mb, (int)st[i]->cfg.max_batch);
-  }
-  *chunk_max = mb;
-  return 0;
-}
-
-// floats of caller scratch for `rows` replicated rows per launch: the replicated input, the chain's next-stage windows,
-// and every stage's sampled preds and vars; each buffer starts on a 256-byte boundary of the (aligned) work pointer
-size_t mc_align(size_t floats) { return (floats + 63) / 64 * 64; }
-size_t mc_work_floats(const lfmq_config& c, int S, size_t rows) {
-  return (size_t)S * mc_align(rows * c.seq_len * c.n_inputs) + 2 * (size_t)S * mc_align(rows * c.seq_len * c.n_outputs);
+  return stages_check(st, S, chain, fn, chunk_max);
 }
 
 size_t mc_rows(int B, int samples, int chunk_max) {
   return (size_t)std::min<int64_t>((int64_t)samples * B, chunk_max);
 }
 
-// Sample s of window b is global row row0 + s * B + b of the batch tiled `samples` times, so sample 0 is
-// lfmq_(chain_)forward_uq at (step, row0).  The tiled rows run in launches of at most chunk_max rows, in row order, and
-// each launch's samples are folded into the moments at once.
-int mc_run(const lfmq_handle* st, int S, const float* x, int B, int64_t row0, int64_t step, int samples, int chunk_max,
+// Caller scratch for `rows` replicated rows per launch: the replicated input and the chain's next-stage windows
+// (win[0], and win[1 ..] read by run_stages as one array), then every stage's sampled preds and vars (m.pred, m.var).
+struct McWork {
+  float* win[lfmq::LFMQ_MAX_STAGES];
+  lfmq::McMoments m;
+};
+McWork mc_layout(const lfmq_config& c, int S, size_t rows, Carver& cv) {
+  McWork w{};
+  for (int i = 0; i < S; ++i) w.win[i] = cv.take<float>(rows * c.seq_len * c.n_inputs);
+  for (int i = 0; i < S; ++i) {
+    w.m.pred.p[i] = cv.take<float>(rows * c.seq_len * c.n_outputs);
+    w.m.var.p[i] = cv.take<float>(rows * c.seq_len * c.n_outputs);
+  }
+  return w;
+}
+
+// The body of both entry points; `chain` numbers the stages' dropout streams.  Sample s of window b is global row
+// row0 + s * B + b of the batch tiled `samples` times, so sample 0 is lfmq_(chain_)forward_uq at (step, row0).  The
+// tiled rows run in launches of at most chunk_max rows, in row order, and each launch's samples are folded into the
+// moments at once.
+int mc_run(const lfmq_handle* st, int S, bool chain, const float* x, int B, int64_t row0, int64_t step, int samples,
            float* const* mean_pred, float* const* mean_var, float* const* var_pred, float* const* var_var, void* work,
-           uint64_t work_bytes, cudaStream_t s) {
+           uint64_t work_bytes, cudaStream_t s, const char* fn) {
+  int chunk_max = 0;
+  RUN(mc_check(st, S, B, samples, chain, fn, &chunk_max));
+  for (int i = 0; i < S; ++i)
+    if (!mean_pred || !mean_var || !var_pred || !var_var || !mean_pred[i] || !mean_var[i] || !var_pred[i] ||
+        !var_var[i]) {
+      LFMQ_SET_ERR("%s: null output of stage %d", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+  if (!x) {
+    LFMQ_SET_ERR("%s: x == NULL", fn);
+    return LFMQ_ERR_ARG;
+  }
   const lfmq_config& c = st[0]->cfg;
   const long row_in = (long)c.seq_len * c.n_inputs, row_out = (long)c.seq_len * c.n_outputs;
   const size_t rows = mc_rows(B, samples, chunk_max);
-  const size_t need = mc_work_floats(c, S, rows) * sizeof(float);
-  if (!work || work_bytes < need) {
-    LFMQ_SET_ERR("forward_uq_mc: work needs %zu bytes, got %llu", need, (unsigned long long)work_bytes);
-    return LFMQ_ERR_WORKSPACE;
-  }
-  const size_t in_sz = mc_align(rows * row_in), out_sz = mc_align(rows * row_out);
-  float* xrep = static_cast<float*>(work);
-  float* slots = xrep + in_sz;                    // run_stages' windows of stages 1 .. S-1, rows * row_in apart
-  float* sp = xrep + (size_t)S * in_sz;
-  lfmq::McMoments m{};
-  float* pp[lfmq::LFMQ_MAX_STAGES];
-  float* vp[lfmq::LFMQ_MAX_STAGES];
+  McWork w;
+  RUN(carve_work(work, work_bytes, "forward_uq_mc", [&](Carver& cv) { return mc_layout(c, S, rows, cv); }, &w));
+  lfmq::McMoments& m = w.m;
   for (int i = 0; i < S; ++i) {
-    pp[i] = m.pred.p[i] = sp + (size_t)(2 * i) * out_sz;
-    vp[i] = m.var.p[i] = sp + (size_t)(2 * i + 1) * out_sz;
     m.mean_pred.p[i] = mean_pred[i];
     m.mean_var.p[i] = mean_var[i];
     m.var_pred.p[i] = var_pred[i];
@@ -1162,21 +1223,12 @@ int mc_run(const lfmq_handle* st, int S, const float* x, int B, int64_t row0, in
     const int64_t b0 = r0 % B;
     const float* in = x + b0 * row_in;            // rows of one sample are a slice of x
     if (b0 + n > B) {
-      RUN(mc_replicate(s, B, r0, n, row_in, x, xrep));
-      in = xrep;
+      RUN(mc_replicate(s, B, r0, n, row_in, x, w.win[0]));
+      in = w.win[0];
     }
-    RUN(run_stages(st, S, in, n, row0 + r0, step, pp, vp, slots, s));
+    RUN(run_stages(st, S, in, n, row0 + r0, step, m.pred.p, m.var.p, w.win[1], s));
     RUN(mc_moments(s, S, B, (int)row_out, r0, n, samples, m));
   }
-  return 0;
-}
-
-int mc_out_check(int S, float* const* a, float* const* b, float* const* c, float* const* d, const char* fn) {
-  for (int i = 0; i < S; ++i)
-    if (!a || !b || !c || !d || !a[i] || !b[i] || !c[i] || !d[i]) {
-      LFMQ_SET_ERR("%s: null output of stage %d", fn, i);
-      return LFMQ_ERR_ARG;
-    }
   return 0;
 }
 }  // namespace
@@ -1187,44 +1239,26 @@ int32_t lfmq_forward_uq_mc_work_bytes(lfmq_handle h, int32_t B, int32_t samples,
 
 int32_t lfmq_chain_forward_uq_mc_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t B, int32_t samples,
                                             uint64_t* bytes) {
+  const char* fn = "lfmq_forward_uq_mc_work_bytes";
   int mb = 0;
-  RUN(mc_check(stages, n_stages, B, samples, "lfmq_forward_uq_mc_work_bytes", &mb));
-  if (!bytes) {
-    LFMQ_SET_ERR("lfmq_forward_uq_mc_work_bytes: bytes == NULL");
-    return LFMQ_ERR_ARG;
-  }
-  *bytes = mc_work_floats(stages[0]->cfg, n_stages, mc_rows(B, samples, mb)) * sizeof(float);
-  return LFMQ_OK;
+  RUN(mc_check(stages, n_stages, B, samples, false, fn, &mb));
+  const size_t rows = mc_rows(B, samples, mb);
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return mc_layout(stages[0]->cfg, n_stages, rows, cv); });
 }
 
 int32_t lfmq_forward_uq_mc(lfmq_handle h, const float* x, int32_t B, int64_t row0, int64_t step, int32_t samples,
                            float* mean_pred, float* mean_var, float* var_pred, float* var_var, void* work,
                            uint64_t work_bytes, void* stream) {
-  int mb = 0;
-  RUN(mc_check(&h, 1, B, samples, "lfmq_forward_uq_mc", &mb));
-  RUN(mc_out_check(1, &mean_pred, &mean_var, &var_pred, &var_var, "lfmq_forward_uq_mc"));
-  if (!x) {
-    LFMQ_SET_ERR("lfmq_forward_uq_mc: x == NULL");
-    return LFMQ_ERR_ARG;
-  }
-  return mc_run(&h, 1, x, B, row0, step, samples, mb, &mean_pred, &mean_var, &var_pred, &var_var, work, work_bytes,
-                (cudaStream_t)stream);
+  return mc_run(&h, 1, false, x, B, row0, step, samples, &mean_pred, &mean_var, &var_pred, &var_var, work, work_bytes,
+                (cudaStream_t)stream, "lfmq_forward_uq_mc");
 }
 
 int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t B, int64_t row0,
                                  int64_t step, int32_t samples, float* const* mean_pred, float* const* mean_var,
                                  float* const* var_pred, float* const* var_var, void* work, uint64_t work_bytes,
                                  void* stream) {
-  int mb = 0;
-  RUN(mc_check(stages, n_stages, B, samples, "lfmq_chain_forward_uq_mc", &mb));
-  RUN(chain_check(stages, n_stages, 1, false));     // numbers the stages' dropout streams; launches hold <= mb rows
-  RUN(mc_out_check(n_stages, mean_pred, mean_var, var_pred, var_var, "lfmq_chain_forward_uq_mc"));
-  if (!x) {
-    LFMQ_SET_ERR("lfmq_chain_forward_uq_mc: x == NULL");
-    return LFMQ_ERR_ARG;
-  }
-  return mc_run(stages, n_stages, x, B, row0, step, samples, mb, mean_pred, mean_var, var_pred, var_var, work,
-                work_bytes, (cudaStream_t)stream);
+  return mc_run(stages, n_stages, true, x, B, row0, step, samples, mean_pred, mean_var, var_pred, var_var, work,
+                work_bytes, (cudaStream_t)stream, "lfmq_chain_forward_uq_mc");
 }
 
 // ---- integrated gradients of the point forecast (lfmq_integrated_gradients) ----------------------------------------
@@ -1262,45 +1296,44 @@ int ig_check(lfmq_handle h, int32_t B, int32_t steps, const char* fn) {
   return 0;
 }
 
-// rows per launch and caller scratch: the scaled inputs and their input gradients, one launch each
 size_t ig_rows(const lfmq_config& c, int B, int steps) {
   return (size_t)std::min<int64_t>((int64_t)steps * B, c.max_batch);
 }
-size_t ig_work_floats(const lfmq_config& c, size_t rows) { return 2 * mc_align(rows * c.seq_len * c.n_inputs); }
+
+// Caller scratch for `rows` rows per launch: the scaled inputs and their input gradients.
+struct IgWork { float *xs, *dx; };
+IgWork ig_layout(const lfmq_config& c, size_t rows, Carver& cv) {
+  IgWork w;
+  w.xs = cv.take<float>(rows * c.seq_len * c.n_inputs);
+  w.dx = cv.take<float>(rows * c.seq_len * c.n_inputs);
+  return w;
+}
 }  // namespace
 
 int32_t lfmq_integrated_gradients_work_bytes(lfmq_handle h, int32_t B, int32_t steps, uint64_t* bytes) {
-  RUN(ig_check(h, B, steps, "lfmq_integrated_gradients_work_bytes"));
-  if (!bytes) {
-    LFMQ_SET_ERR("lfmq_integrated_gradients_work_bytes: bytes == NULL");
-    return LFMQ_ERR_ARG;
-  }
-  *bytes = ig_work_floats(h->cfg, ig_rows(h->cfg, B, steps)) * sizeof(float);
-  return LFMQ_OK;
+  const char* fn = "lfmq_integrated_gradients_work_bytes";
+  RUN(ig_check(h, B, steps, fn));
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return ig_layout(h->cfg, ig_rows(h->cfg, B, steps), cv); });
 }
 
 int32_t lfmq_integrated_gradients(lfmq_handle h, const float* x, int32_t B, int32_t steps, float* attr, float* f_x,
                                   float* f_base, void* work, uint64_t work_bytes, void* stream) {
-  RUN(ig_check(h, B, steps, "lfmq_integrated_gradients"));
+  const char* fn = "lfmq_integrated_gradients";
+  RUN(ig_check(h, B, steps, fn));
   if (!x || !attr || !f_x || !f_base) {
-    LFMQ_SET_ERR("lfmq_integrated_gradients: null pointer");
+    LFMQ_SET_ERR("%s: null pointer", fn);
     return LFMQ_ERR_ARG;
   }
   const lfmq_config& c = h->cfg;
   const int T = c.seq_len, O = c.n_outputs, ti = c.target_idx;
   const long row_in = (long)T * c.n_inputs;
   const size_t rows = ig_rows(c, B, steps);
-  const size_t need = ig_work_floats(c, rows) * sizeof(float);
-  if (!work || work_bytes < need) {
-    LFMQ_SET_ERR("lfmq_integrated_gradients: work needs %zu bytes, got %llu", need, (unsigned long long)work_bytes);
-    return LFMQ_ERR_WORKSPACE;
-  }
+  IgWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return ig_layout(c, rows, cv); }, &w));
   cudaStream_t s = (cudaStream_t)stream;
-  float* xs = static_cast<float*>(work);
-  float* dx = xs + mc_align(rows * row_in);
   // f(0): a row's forecast depends on that row alone, so one row of zeros gives every window's baseline
-  LFMQ_CUDA_CHECK(cudaMemsetAsync(xs, 0, row_in * sizeof(float), s));
-  RUN(forward_fp32(h, xs, 1, 0, 0, h->preds, nullptr, s));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(w.xs, 0, row_in * sizeof(float), s));
+  RUN(forward_fp32(h, w.xs, 1, 0, 0, h->preds, nullptr, s));
   RUN(ig_pick(s, B, 1, T, O, ti, h->preds, f_base));
   for (int b0 = 0; b0 < B; b0 += c.max_batch) {       // f(x)
     const int n = std::min(B - b0, c.max_batch);
@@ -1311,11 +1344,11 @@ int32_t lfmq_integrated_gradients(lfmq_handle h, const float* x, int32_t B, int3
   const int64_t total = (int64_t)steps * B;
   for (int64_t r0 = 0; r0 < total; r0 += (int64_t)rows) {
     const int n = (int)std::min<int64_t>((int64_t)rows, total - r0);
-    RUN(ig_scale_inputs(s, B, steps, r0, n, row_in, x, xs));
-    RUN(forward_fp32(h, xs, n, 0, 0, h->preds, nullptr, s));
+    RUN(ig_scale_inputs(s, B, steps, r0, n, row_in, x, w.xs));
+    RUN(forward_fp32(h, w.xs, n, 0, 0, h->preds, nullptr, s));
     RUN(ig_seed(s, n, T, O, ti, h->dpred));
-    RUN(backward_fp32(h, xs, n, s, dx, kIgInputOnly));
-    RUN(ig_fold(s, B, steps, r0, n, row_in, dx, x, attr));
+    RUN(backward_fp32(h, w.xs, n, s, w.dx, kIgInputOnly));
+    RUN(ig_fold(s, B, steps, r0, n, row_in, w.dx, x, attr));
   }
   return LFMQ_OK;
 }
@@ -1329,22 +1362,8 @@ int pi_check(const lfmq_handle* st, int32_t S, int32_t N, const char* fn, int* r
     LFMQ_SET_ERR("%s: need 1 <= n_stages <= %d and N >= 1 (got %d, %d)", fn, lfmq::LFMQ_MAX_STAGES, S, N);
     return LFMQ_ERR_ARG;
   }
-  for (int i = 0; i < S; ++i)
-    if (!st[i]) {
-      LFMQ_SET_ERR("%s: stage %d is a null handle", fn, i);
-      return LFMQ_ERR_ARG;
-    }
-  int mb = st[0]->cfg.max_batch;
-  if (st[0]->path == Path::Dense) {
-    if (S != 1) {
-      LFMQ_SET_ERR("%s: a dense handle is a model of one stage (got n_stages %d)", fn, S);
-      return LFMQ_ERR_ARG;
-    }
-  } else {
-    RUN(chain_check(st, S, 1, false));
-    for (int i = 1; i < S; ++i) mb = std::min(mb, (int)st[i]->cfg.max_batch);
-  }
-  *rows = std::min(N, mb);
+  RUN(stages_check(st, S, true, fn, rows));
+  *rows = std::min(N, *rows);
   return 0;
 }
 
@@ -1420,13 +1439,28 @@ struct CopyForward {
   }
 };
 
-// floats of caller scratch: the launch's permuted rows, the chain's next-stage windows of a launch, the device copy of
-// col_group with its groups numbered densely, the one-hot rank rows, and one copy's predictions (and variances on a uq
-// chain) of every stage, each on a 256-byte boundary
-size_t pi_work_floats(const lfmq_handle* st, int S, int rows, int N) {
+// Caller scratch of permutation importance and Shapley: a launch's gathered rows and the chain's next-stage windows
+// (win[0], and win[1 ..] read by run_stages as one array), the device copy of col_group, the analysis's tables, and
+// every stage's predictions, then variances on a uq chain.
+struct CopyWork {
+  float* win[lfmq::LFMQ_MAX_STAGES];
+  int32_t *cg, *onehot, *order, *rank;
+  float* prev;
+  float* pred[lfmq::LFMQ_MAX_STAGES];
+  float* var[lfmq::LFMQ_MAX_STAGES];
+};
+
+// Permutation importance: col_group with its groups numbered densely, the one-hot rank rows, and one copy's outputs.
+CopyWork pi_layout(const lfmq_handle* st, int S, int rows, int N, Carver& cv) {
   const size_t row_in = row_in_of(st), row_out = row_out_of(st);
-  return (size_t)S * mc_align(rows * row_in) + mc_align(row_in) + mc_align(2 * row_in) +
-         (st[0]->cfg.uq ? 2 : 1) * (size_t)S * mc_align(N * row_out);
+  CopyWork w{};
+  for (int i = 0; i < S; ++i) w.win[i] = cv.take<float>(rows * row_in);
+  w.cg = cv.take<int32_t>(row_in);
+  w.onehot = cv.take<int32_t>(2 * row_in);
+  for (int i = 0; i < S; ++i) w.pred[i] = cv.take<float>(N * row_out);
+  if (st[0]->cfg.uq)
+    for (int i = 0; i < S; ++i) w.var[i] = cv.take<float>(N * row_out);
+  return w;
 }
 
 // Shapley: the perm_index keys of the donor windows and of the group orderings (DESIGN.md section 5f)
@@ -1437,13 +1471,19 @@ int shapley_outputs(const lfmq_handle* st, int S) {
   return st[0]->path == Path::Dense ? 1 : (st[0]->cfg.uq ? 2 * S : S);
 }
 
-// floats of caller scratch: the launch's coalition rows, the chain's next-stage windows of a launch, the device copy of
-// col_group, the samples' group orderings and ranks [samples][G] each, prev [N][K], and one launch's predictions (and
-// variances on a uq chain) of every stage, each on a 256-byte boundary
-size_t shapley_work_floats(const lfmq_handle* st, int S, int rows, int N, int G, int samples) {
+// Shapley: the samples' group orderings and ranks [samples][G] each, prev [N][K], and one launch's outputs.
+CopyWork shapley_layout(const lfmq_handle* st, int S, int rows, int N, int G, int samples, Carver& cv) {
   const size_t row_in = row_in_of(st), row_out = row_out_of(st);
-  return (size_t)S * mc_align(rows * row_in) + mc_align(row_in) + 2 * mc_align((size_t)samples * G) +
-         mc_align((size_t)N * shapley_outputs(st, S)) + (st[0]->cfg.uq ? 2 : 1) * (size_t)S * mc_align(rows * row_out);
+  CopyWork w{};
+  for (int i = 0; i < S; ++i) w.win[i] = cv.take<float>(rows * row_in);
+  w.cg = cv.take<int32_t>(row_in);
+  w.order = cv.take<int32_t>((size_t)samples * G);
+  w.rank = cv.take<int32_t>((size_t)samples * G);
+  w.prev = cv.take<float>((size_t)N * shapley_outputs(st, S));
+  for (int i = 0; i < S; ++i) w.pred[i] = cv.take<float>(rows * row_out);
+  if (st[0]->cfg.uq)
+    for (int i = 0; i < S; ++i) w.var[i] = cv.take<float>(rows * row_out);
+  return w;
 }
 
 int shapley_args_check(int32_t N, int32_t G, int32_t samples, const char* fn) {
@@ -1457,14 +1497,10 @@ int shapley_args_check(int32_t N, int32_t G, int32_t samples, const char* fn) {
 
 int32_t lfmq_chain_permutation_importance_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N,
                                                      uint64_t* bytes) {
+  const char* fn = "lfmq_chain_permutation_importance_work_bytes";
   int rows = 0;
-  RUN(pi_check(stages, n_stages, N, "lfmq_chain_permutation_importance_work_bytes", &rows));
-  if (!bytes) {
-    LFMQ_SET_ERR("lfmq_chain_permutation_importance_work_bytes: bytes == NULL");
-    return LFMQ_ERR_ARG;
-  }
-  *bytes = pi_work_floats(stages, n_stages, rows, N) * sizeof(float);
-  return LFMQ_OK;
+  RUN(pi_check(stages, n_stages, N, fn, &rows));
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return pi_layout(stages, n_stages, rows, N, cv); });
 }
 
 int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_stages, const float* x,
@@ -1492,23 +1528,9 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
       return LFMQ_ERR_ARG;
     }
   RUN(col_group_check(col_group, row_in, G, fn));
-  const size_t need = pi_work_floats(stages, S, rows, N) * sizeof(float);
-  if (!work || work_bytes < need) {
-    LFMQ_SET_ERR("%s: work needs %zu bytes, got %llu", fn, need, (unsigned long long)work_bytes);
-    return LFMQ_ERR_WORKSPACE;
-  }
+  CopyWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return pi_layout(stages, S, rows, N, cv); }, &w));
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t in_sz = mc_align((size_t)rows * row_in), out_sz = mc_align((size_t)N * row_out);
-  float* xin = static_cast<float*>(work);
-  int32_t* cg = reinterpret_cast<int32_t*>(xin + (size_t)S * in_sz);
-  int32_t* onehot = cg + mc_align(row_in);
-  float* pbuf = xin + (size_t)S * in_sz + mc_align(row_in) + mc_align(2 * row_in);
-  float* preds[lfmq::LFMQ_MAX_STAGES];
-  float* vars[lfmq::LFMQ_MAX_STAGES];
-  for (int i = 0; i < S; ++i) {
-    preds[i] = pbuf + (size_t)i * out_sz;
-    vars[i] = uq ? pbuf + (size_t)(S + i) * out_sz : nullptr;
-  }
   // The gather takes group g's columns from the donor through a rank row that is 1 at g and 0 elsewhere.  G may exceed
   // the columns, so the device col_group numbers the D <= row_in groups present densely (u), and the rank row of
   // group g is the window onehot + D - 1 - u(g) of onehot [2D] = e_{D-1}; a group with no columns reads onehot + D,
@@ -1521,12 +1543,12 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
   for (long k = 0; k < row_in; ++k)
     dense_cg[k] = (int32_t)(std::lower_bound(ids.begin(), ids.end(), col_group[k]) - ids.begin());
   hot[D - 1] = 1;
-  LFMQ_CUDA_CHECK(cudaMemcpyAsync(cg, dense_cg.data(), row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  LFMQ_CUDA_CHECK(cudaMemcpyAsync(onehot, hot.data(), 2 * D * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.cg, dense_cg.data(), row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.onehot, hot.data(), 2 * D * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   const int64_t copies = 1 + (int64_t)G * repeats;
   LFMQ_CUDA_CHECK(cudaMemsetAsync(out_dev, 0, copies * 3 * sizeof(float), s));
-  const CopyForward cf{stages, S, x, N, rows, row_in, row_out, cg, seed, step, xin, xin + in_sz, preds,
-                       uq ? vars : nullptr, true, s};
+  const CopyForward cf{stages, S, x, N, rows, row_in, row_out, w.cg, seed, step, w.win[0], w.win[1], w.pred,
+                       uq ? w.var : nullptr, true, s};
   // copy 0 is the held-out set as it is; copy 1 + g * repeats + r has group g's columns from window pi_{seed,g,r}(i).
   // Every launch keys its rows by window index (row0 = a), so window i draws the same dropout masks in every copy.
   for (int64_t k = 0; k < copies; ++k) {
@@ -1534,18 +1556,18 @@ int32_t lfmq_chain_permutation_importance(const lfmq_handle* stages, int32_t n_s
     const int32_t* rank = nullptr;
     if (k > 0) {
       const auto it = std::lower_bound(ids.begin(), ids.end(), g);
-      rank = onehot + (it != ids.end() && *it == g ? D - 1 - (int)(it - ids.begin()) : D);
+      rank = w.onehot + (it != ids.end() && *it == g ? D - 1 - (int)(it - ids.begin()) : D);
     }
     RUN(cf.run(rank, 1, g, r, 0, nullptr));
     float* o = out_dev + 3 * k;
     if (uq && S == 1) {
-      RUN(lfmq_loss_uq(stages[0], preds[0], vars[0], y[0], N, o, stream));
+      RUN(lfmq_loss_uq(stages[0], w.pred[0], w.var[0], y[0], N, o, stream));
     } else if (uq) {
-      RUN(lfmq_chain_loss_uq(stages, S, preds, vars, y, weights, N, o, stream));
+      RUN(lfmq_chain_loss_uq(stages, S, w.pred, w.var, y, weights, N, o, stream));
     } else if (S == 1) {
-      RUN(lfmq_loss(stages[0], preds[0], y[0], N, o, stream));
+      RUN(lfmq_loss(stages[0], w.pred[0], y[0], N, o, stream));
     } else {
-      RUN(lfmq_chain_loss(stages, S, preds, y, weights, N, o, stream));
+      RUN(lfmq_chain_loss(stages, S, w.pred, y, weights, N, o, stream));
     }
   }
   return LFMQ_OK;
@@ -1557,12 +1579,8 @@ int32_t lfmq_chain_shapley_work_bytes(const lfmq_handle* stages, int32_t n_stage
   int rows = 0;
   RUN(pi_check(stages, n_stages, N, fn, &rows));
   RUN(shapley_args_check(N, G, samples, fn));
-  if (!bytes) {
-    LFMQ_SET_ERR("%s: bytes == NULL", fn);
-    return LFMQ_ERR_ARG;
-  }
-  *bytes = shapley_work_floats(stages, n_stages, rows, N, G, samples) * sizeof(float);
-  return LFMQ_OK;
+  return report_work_bytes(bytes, fn,
+                           [&](Carver& cv) { return shapley_layout(stages, n_stages, rows, N, G, samples, cv); });
 }
 
 int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N,
@@ -1581,33 +1599,18 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
     return LFMQ_ERR_ARG;
   }
   RUN(col_group_check(col_group, row_in, G, fn));
-  const size_t need = shapley_work_floats(stages, S, rows, N, G, M) * sizeof(float);
-  if (!work || work_bytes < need) {
-    LFMQ_SET_ERR("%s: work needs %zu bytes, got %llu", fn, need, (unsigned long long)work_bytes);
-    return LFMQ_ERR_WORKSPACE;
-  }
+  CopyWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return shapley_layout(stages, S, rows, N, G, M, cv); }, &w));
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t in_sz = mc_align((size_t)rows * row_in), tab_sz = mc_align((size_t)M * G);
-  const size_t out_sz = mc_align((size_t)rows * row_out);
-  float* xin = static_cast<float*>(work);
-  int32_t* cg = reinterpret_cast<int32_t*>(xin + (size_t)S * in_sz);
-  int32_t* order = cg + mc_align(row_in);
-  int32_t* rank = order + tab_sz;
-  float* prev = reinterpret_cast<float*>(rank + tab_sz);
-  float* pbuf = prev + mc_align((size_t)N * K);
-  float* preds[lfmq::LFMQ_MAX_STAGES];
-  float* vars[lfmq::LFMQ_MAX_STAGES];
   // the explained value of a launch row: pred[T-1, target_idx] ([target_idx] on a dense handle)
   ShapleyFold fold{{}, K, row_out, dense ? c.target_idx : (long)(c.seq_len - 1) * c.n_outputs + c.target_idx, G,
-                   nullptr, prev, phi, f_x, f_bg};
+                   nullptr, w.prev, phi, f_x, f_bg};
   for (int i = 0; i < S; ++i) {
-    preds[i] = pbuf + (size_t)i * out_sz;
-    vars[i] = uq ? pbuf + (size_t)(S + i) * out_sz : nullptr;
     if (uq) {                                    // Keras list order: tar_1, var_1, .., tar_S, var_S
-      fold.src.p[2 * i] = preds[i];
-      fold.src.p[2 * i + 1] = vars[i];
+      fold.src.p[2 * i] = w.pred[i];
+      fold.src.p[2 * i + 1] = w.var[i];
     } else {
-      fold.src.p[i] = preds[i];
+      fold.src.p[i] = w.pred[i];
     }
   }
   // Sample m belongs to pair p = m / 2.  An even sample orders the groups by o[q] = perm_index(G, seed, 0x40000001,
@@ -1620,21 +1623,21 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
                           : ord[(size_t)(m - 1) * G + (G - 1 - q)];
       rk[(size_t)m * G + o[q]] = q;
     }
-  LFMQ_CUDA_CHECK(cudaMemcpyAsync(cg, col_group, row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  LFMQ_CUDA_CHECK(cudaMemcpyAsync(order, ord.data(), ord.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  LFMQ_CUDA_CHECK(cudaMemcpyAsync(rank, rk.data(), rk.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.cg, col_group, row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.order, ord.data(), ord.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.rank, rk.data(), rk.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   LFMQ_CUDA_CHECK(cudaMemsetAsync(phi, 0, (size_t)N * K * G * sizeof(float), s));
   LFMQ_CUDA_CHECK(cudaMemsetAsync(f_x, 0, (size_t)N * K * sizeof(float), s));
   LFMQ_CUDA_CHECK(cudaMemsetAsync(f_bg, 0, (size_t)N * K * sizeof(float), s));
-  const CopyForward cf{stages, S, x, N, rows, row_in, row_out, cg, seed, step, xin, xin + in_sz, preds,
-                       uq ? vars : nullptr, false, s};
+  const CopyForward cf{stages, S, x, N, rows, row_in, row_out, w.cg, seed, step, w.win[0], w.win[1], w.pred,
+                       uq ? w.var : nullptr, false, s};
   // Copy (m, k) takes the groups ranked >= k in o_m from window d_p(i) = perm_index(N, seed, 0x40000000, p, i): k = 0
   // is the donor, k = G is x itself, forwarded without a gather.  Every launch of sample m keys window i as row
   // m * N + i, so a uq window shares its dropout masks across the copies of one sample.
   for (int m = 0; m < M; ++m) {
-    fold.order = order + (size_t)m * G;
+    fold.order = w.order + (size_t)m * G;
     for (int k = 0; k <= G; ++k)
-      RUN(cf.run(k < G ? rank + (size_t)m * G : nullptr, k, kShapleyDonorKey, m / 2, (int64_t)m * N, &fold));
+      RUN(cf.run(k < G ? w.rank + (size_t)m * G : nullptr, k, kShapleyDonorKey, m / 2, (int64_t)m * N, &fold));
   }
   const float inv = 1.0f / (float)M;
   RUN(scale_inplace(s, (long)N * K * G, phi, inv));

@@ -26,6 +26,17 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _scratch(owner, key, work_bytes, *args):
+    """The caller scratch of one analysis: a device uint8 buffer of at least the bytes its lfmq_*_work_bytes query
+    reports for args, kept on `owner` under `key` and grown as needed."""
+    n = C.c_uint64(0)
+    N.check(work_bytes(*args, C.byref(n)))
+    bufs = owner.__dict__.setdefault('_scratch_bufs', {})
+    if key not in bufs or bufs[key].numel() < n.value:
+        bufs[key] = torch.empty(max(n.value, 1), dtype=torch.uint8, device=owner.device)
+    return bufs[key]
+
+
 class _HandleEngine(object):
     """What every native handle offers whatever its model: parameter specs and views, weights in Keras order, the
     device share, the optimizer apply, the mask count, un-scaling and profiling."""
@@ -264,7 +275,7 @@ class ForecasterEngine(_HandleEngine):
         forward(x, step, row0).  uq engines only."""
         B = self._check_x(x)
         out = [torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device) for _ in range(4)]
-        work = _mc_work(self, [self], B, samples)
+        work = _scratch(self, 'mc', self.lib.lfmq_forward_uq_mc_work_bytes, self.handle, B, int(samples))
         N.check(self.lib.lfmq_forward_uq_mc(self.handle, _ptr(x), B, row0, step, samples, *[_ptr(t) for t in out],
                                             _ptr(work), work.numel(), _stream()))
         return tuple(out)
@@ -276,11 +287,7 @@ class ForecasterEngine(_HandleEngine):
         created with train=False, forward_only=False and uq=False; B and steps are not bounded by max_batch.  The
         engine's parameters, gradients and optimizer state are left as they were."""
         B = self._check_x(x)
-        n = C.c_uint64(0)
-        N.check(self.lib.lfmq_integrated_gradients_work_bytes(self.handle, B, int(steps), C.byref(n)))
-        work = getattr(self, '_ig_buf', None)
-        if work is None or work.numel() < n.value:
-            work = self._ig_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=self.device)
+        work = _scratch(self, 'ig', self.lib.lfmq_integrated_gradients_work_bytes, self.handle, B, int(steps))
         attr = torch.empty(B, self.T, self.F, dtype=torch.float32, device=x.device)
         f_x = torch.empty(B, dtype=torch.float32, device=x.device)
         f_base = torch.empty_like(f_x)
@@ -407,16 +414,6 @@ class DenseEngine(_HandleEngine):
         of the flat gradient and its {loss, mse_0} tail, the replicated clip and optimizer."""
         return self._train_step_dp_flat(x, y, step, lr, row0, denom_global)
 
-def _mc_work(owner, engines, B, samples):
-    """The scratch of lfmq_(chain_)forward_uq_mc for (B, samples), kept on `owner` and grown as needed."""
-    n = C.c_uint64(0)
-    handles = (C.c_void_p * len(engines))(*[e.handle.value for e in engines])
-    N.check(owner.lib.lfmq_chain_forward_uq_mc_work_bytes(handles, len(engines), B, int(samples), C.byref(n)))
-    work = getattr(owner, '_mc_buf', None)
-    if work is None or work.numel() < n.value:
-        work = owner._mc_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=engines[0].device)
-    return work
-
 
 class _PackedStep(object):
     """The collective of a data-parallel step over the handles of a chain (or one uq handle): the backward fills every
@@ -541,7 +538,8 @@ class ForecastChainEngine(object):
         B = self.stages[0]._check_x(x)
         out = [[torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device) for _ in range(self.S)]
                for _ in range(4)]
-        work = _mc_work(self, self.stages, B, samples)
+        work = _scratch(self, 'mc', self.lib.lfmq_chain_forward_uq_mc_work_bytes, self._handles, self.S, B,
+                        int(samples))
         N.check(self.lib.lfmq_chain_forward_uq_mc(self._handles, self.S, _ptr(x), B, row0, step, samples,
                                                   *[self._ptrs(o) for o in out], _ptr(work), work.numel(), _stream()))
         return [tuple(o[s] for o in out) for s in range(self.S)]
@@ -560,11 +558,7 @@ class ForecastChainEngine(object):
             assert y.is_cuda and y.dtype == torch.float32 and y.shape[0] == B
         cg = np.ascontiguousarray(col_group, dtype=np.int32)
         G = int(cg.max()) + 1
-        n = C.c_uint64(0)
-        N.check(self.lib.lfmq_chain_permutation_importance_work_bytes(self._handles, self.S, B, C.byref(n)))
-        work = getattr(self, '_pi_buf', None)
-        if work is None or work.numel() < n.value:
-            work = self._pi_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=self.device)
+        work = _scratch(self, 'pi', self.lib.lfmq_chain_permutation_importance_work_bytes, self._handles, self.S, B)
         out = torch.empty(max(1 + G * int(repeats), 1), 3, dtype=torch.float32, device=self.device)
         N.check(self.lib.lfmq_chain_permutation_importance(
             self._handles, self.S, _ptr(x), self._ptrs(ys), self._w, B, cg.ctypes.data_as(C.c_void_p), G,
@@ -583,11 +577,7 @@ class ForecastChainEngine(object):
         cg = np.ascontiguousarray(col_group, dtype=np.int32)
         G, M = int(cg.max()) + 1, int(samples)
         K = 1 if isinstance(self.stages[0], DenseEngine) else (2 * self.S if self.uq else self.S)
-        n = C.c_uint64(0)
-        N.check(self.lib.lfmq_chain_shapley_work_bytes(self._handles, self.S, B, G, M, C.byref(n)))
-        work = getattr(self, '_sh_buf', None)
-        if work is None or work.numel() < n.value:
-            work = self._sh_buf = torch.empty(max(n.value, 1), dtype=torch.uint8, device=self.device)
+        work = _scratch(self, 'shapley', self.lib.lfmq_chain_shapley_work_bytes, self._handles, self.S, B, G, M)
         phi = torch.empty(B, K, G, dtype=torch.float32, device=self.device)
         f_x = torch.empty(B, K, dtype=torch.float32, device=self.device)
         f_bg = torch.empty(B, K, dtype=torch.float32, device=self.device)

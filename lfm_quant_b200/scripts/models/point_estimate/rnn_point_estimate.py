@@ -67,8 +67,8 @@ class NativeForecaster(object):
         specs = [(n, s) for (_, n, s, _, tr) in self.engine.specs if tr]
         self.trainable_variables = [_Variable(self, i, n, s) for i, (n, s) in enumerate(specs)]
         self._calls = 0
-        self._mc_engine, self._mc_stale = None, True
-        self._ig_engine, self._ig_stale = None, True
+        self._side = {}          # role -> side engine: 'wide' (_wide_engine), 'ig' (_ig_rows_engine)
+        self._stale = set()      # the roles whose side engine holds older weights than the model
 
     @property
     def title(self):
@@ -178,26 +178,36 @@ class NativeForecaster(object):
         rows = min(rows, MC_ROWS)
         if rows <= self.engine.cfg.max_batch:
             return self.engine
-        if self._mc_engine is None or self._mc_engine.cfg.max_batch < rows:
-            self._close_mc_engine()
-            self._mc_engine = self._new_wide_engine(rows)
-            if self.engine.device_share is not None:
-                self._mc_engine.set_device_share(*self.engine.device_share)
-            self._mc_stale = True
-        if self._mc_stale:
-            for src, dst in zip(self.engine.stages, self._mc_engine.stages):
-                dst.set_flat(src.get_flat())
-            self._mc_stale = False
-        return self._mc_engine
+        return self._side_engine('wide', rows, self._new_wide_engine, share=True)
 
     def _new_wide_engine(self, rows):
         from ....engine import ForecastChainEngine
         return ForecastChainEngine(**dict(self._engine_kw, max_batch=rows, forward_only=True))
 
-    def _close_mc_engine(self):
-        if self._mc_engine is not None:
-            self._mc_engine.close()
-            self._mc_engine = None
+    def _side_engine(self, role, rows, new, share=False):
+        """The side engine of `role` with room for `rows` rows per launch: new(rows), created at the first call (again
+        for a larger count) and owned by the model, with the model engine's device share when `share`.  Its copy of the
+        weights is renewed after _weights_changed."""
+        eng = self._side.get(role)
+        if eng is None or eng.cfg.max_batch < rows:
+            if eng is not None:
+                eng.close()
+            eng = self._side[role] = new(rows)
+            if share and self.engine.device_share is not None:
+                eng.set_device_share(*self.engine.device_share)
+            self._stale.add(role)
+        if role in self._stale:
+            for src, dst in zip(self.engine.stages, eng.stages):
+                dst.set_flat(src.get_flat())
+            self._stale.discard(role)
+        return eng
+
+    def _weights_changed(self):
+        self._stale = set(self._side)
+
+    # the wide side engine and the handle engine attribute runs on, None while they do not exist
+    _mc_engine = property(lambda self: self._side.get('wide'))
+    _ig_engine = property(lambda self: self._side['ig'].stages[0] if 'ig' in self._side else None)
 
     def attribute(self, inp, steps):
         """Integrated-gradients attributions of the point forecast norm_preds_1 = pred[:, T-1, target_idx] of every
@@ -218,29 +228,20 @@ class NativeForecaster(object):
         tf32 for a tf32 model and fp32 otherwise, with max_batch = min(steps * batch_size, IG_ROWS).  Created at the first
         call (again for a larger count) and owned by the model; its copy of the weights is renewed after set_weights,
         load_weights and the train steps."""
-        from ....engine import ForecasterEngine
-        rows = min(steps * self.config.batch_size, IG_ROWS)
-        if self._ig_engine is None or self._ig_engine.cfg.max_batch < rows:
-            self._close_ig_engine()
-            kw = {k: v for k, v in self._engine_kw.items() if k not in ('forecast_steps', 'weights')}
-            kw.update(max_batch=rows, train=False, forward_only=False, device=self.engine.device,
-                      precision='tf32' if kw['precision'] == 'tf32' else 'fp32')
-            self._ig_engine = ForecasterEngine(**kw)
-            self._ig_stale = True
-        if self._ig_stale:
-            self._ig_engine.set_flat(self.engine.stages[0].get_flat())
-            self._ig_stale = False
-        return self._ig_engine
+        return self._side_engine('ig', min(steps * self.config.batch_size, IG_ROWS), self._new_ig_engine).stages[0]
 
-    def _close_ig_engine(self):
-        if self._ig_engine is not None:
-            self._ig_engine.close()
-            self._ig_engine = None
+    def _new_ig_engine(self, rows):
+        from ....engine import ForecastChainEngine, ForecasterEngine
+        kw = {k: v for k, v in self._engine_kw.items() if k not in ('forecast_steps', 'weights')}
+        kw.update(max_batch=rows, train=False, forward_only=False, device=self.engine.device,
+                  precision='tf32' if kw['precision'] == 'tf32' else 'fp32')
+        return ForecastChainEngine(stages=[ForecasterEngine(**kw)])
 
     def close(self):
         """Releases the device memory of the model's handles."""
-        self._close_mc_engine()
-        self._close_ig_engine()
+        for eng in self._side.values():
+            eng.close()
+        self._side.clear()
         self.engine.close()
 
     def predict(self, inp, batch_size=None):
@@ -251,7 +252,7 @@ class NativeForecaster(object):
         """Fused fwd + loss + BPTT + clip + optimizer + MaxNorm (train.py:178-225); returns the device tensor
         {loss, mse}, on a uq model {uq_loss_last_tar, mse}."""
         assert isinstance(targets, (list, tuple)), 'targets must be the list of forecast_steps targets (train.py:188)'
-        self._mc_stale = self._ig_stale = True
+        self._weights_changed()
         return self.engine.train_step(_to_device(self.engine, inp), [_to_device(self.engine, t) for t in targets],
                                       iteration, lr)
 
@@ -262,7 +263,7 @@ class NativeForecaster(object):
         if x is not None:
             assert isinstance(ys, (list, tuple)), 'ys must be the list of forecast_steps targets'
             x, ys = _to_device(self.engine, x), [_to_device(self.engine, t) for t in ys]
-        self._mc_stale = self._ig_stale = True
+        self._weights_changed()
         return self.engine.train_step_dp(x, ys, step, lr, row0, denoms)
 
     # -- Keras API surface -------------------------------------------------------------------------------
@@ -310,7 +311,7 @@ class NativeForecaster(object):
                                     '%s.index (Keras save_weights) exists' % (prefix, os.path.basename(prefix),
                                                                               os.path.basename(prefix)))
         self.engine.load_named(lambda name: data[name])
-        self._mc_stale = self._ig_stale = True
+        self._weights_changed()
 
     def get_weights(self):
         return self.engine.get_weights(trainable_only=False)
@@ -318,7 +319,7 @@ class NativeForecaster(object):
     def set_weights(self, weights):
         """The trainable arrays, optionally followed by the BatchNormalization statistics (get_weights' order)."""
         self.engine.set_weights(weights)
-        self._mc_stale = self._ig_stale = True
+        self._weights_changed()
 
 
 class RNNPointEstimate(BaseModelClass):
