@@ -279,6 +279,34 @@ int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, co
                                  int64_t step, int32_t samples, float* const* mean_pred, float* const* mean_var,
                                  float* const* var_pred, float* const* var_var, void* work, uint64_t work_bytes,
                                  void* stream);
+/* ---- predictive quantiles and proper scores of those samples ------------------------------------------------------
+ * The samples of lfmq_chain_forward_uq_mc, and with them its four moment arrays, bit for bit (the same launches and
+ * the same fold).  Each launch's samples at [T-1, target_idx] are also gathered into `work` as mu[s][b][m] and
+ * v[s][b][m], and after the last launch one pass treats each (window, stage) as the Gaussian mixture
+ * F(q) = (1/M) sum_m Phi((q - mu_m) / sigma_m), sigma_m^2 = v_m, M = samples, and writes (device fp32):
+ *   quantiles[s] [B][n_levels]  the q with F(q) = levels[k]: bracketed by the smallest and largest component quantile
+ *                               mu_m + sigma_m Phi^-1(levels[k]), refined by safeguarded Newton steps until
+ *                               |F(q) - level| <= 1e-7, the bracket is narrower than 1e-6 min_m sigma_m, or 64 steps;
+ *   scores[s] [B][3]            with y (host array of n_stages device pointers, laid out as lfmq_chain_loss_uq takes
+ *                               the targets) and the target y[s][b, T-1, target_idx]: {crps, nll, pit} =
+ *                               {E|X - y| - E|X - X'| / 2 in the closed form for Gaussian mixtures (Grimit et al.
+ *                               2006) over the M components and the M (M + 1) / 2 pairs, -log f(y) by log-sum-exp,
+ *                               F(y)}.  A NaN target gives NaN scores (its quantiles are still written).  y == NULL:
+ *                               scores is not written and may be NULL.
+ * Every lane evaluates components in fp32 (the log-score terms in fp64) and sums in fp64; a warp adds its lanes in a
+ * fixed tree, without atomics, so a window's outputs depend neither on the other windows nor on max_batch or where
+ * launches are cut, and two calls give the same bits.  Accepted: uq chains as lfmq_chain_forward_uq_mc, any precision.
+ * Point-estimate and dense handles, n_levels outside [1, 32], levels not strictly increasing inside (0, 1) (host float
+ * [n_levels]) and null pointers: LFMQ_ERR_ARG.  The handles' parameters, gradients and optimizer slots are left
+ * untouched.  `work`: caller-owned device scratch, 256-byte aligned, of the size the *_work_bytes query gives: that of
+ * lfmq_chain_forward_uq_mc, then mu and v of every stage (2 * n_stages * B * samples floats). */
+int32_t lfmq_chain_forward_uq_dist_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t B, int32_t samples,
+                                              int32_t n_levels, uint64_t* bytes);
+int32_t lfmq_chain_forward_uq_dist(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
+                                   int32_t B, int64_t row0, int64_t step, int32_t samples, const float* levels,
+                                   int32_t n_levels, float* const* mean_pred, float* const* mean_var,
+                                   float* const* var_pred, float* const* var_var, float* const* quantiles,
+                                   float* const* scores, void* work, uint64_t work_bytes, void* stream);
 /* ---- integrated gradients of the point forecast ---------------------------------------------------------------------
  * Which input fields and quarters of each window drive its forecast f(x) = pred[b, T-1, target_idx] (predict.py's
  * norm_preds_1), with dropout off and BatchNormalization in its inference form.  With the baseline x' = 0 (the value

@@ -90,6 +90,10 @@ SYMBOLS = {
     'lfmq_chain_forward_uq_mc_work_bytes': (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
     'lfmq_chain_forward_uq_mc': (C.c_int32, [_P, C.c_int32, _P, C.c_int32, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P,
                                               _P, _P, C.c_uint64, _P]),
+    'lfmq_chain_forward_uq_dist_work_bytes': (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                          C.POINTER(C.c_uint64)]),
+    'lfmq_chain_forward_uq_dist': (C.c_int32, [_P, C.c_int32, _P, _P, C.c_int32, C.c_int64, C.c_int64, C.c_int32, _P,
+                                                C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_uint64, _P]),
     'lfmq_integrated_gradients_work_bytes': (C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
     'lfmq_integrated_gradients': (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_uint64, _P]),
     'lfmq_chain_permutation_importance_work_bytes': (C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),

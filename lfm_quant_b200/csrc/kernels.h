@@ -74,6 +74,16 @@ int mc_replicate(cudaStream_t s, int B, int64_t r0, int n, long row_elems, const
 // one, mean_pred / mean_var hold the sample means and var_pred / var_var the population variances.
 struct McMoments { ChainPtrs pred, var, mean_pred, mean_var, var_pred, var_var; };
 int mc_moments(cudaStream_t s, int n_stages, int B, int TO, int64_t r0, int n, int samples, const McMoments& m);
+// Predictive distributions of those samples (predictive.cu, lfmq_chain_forward_uq_dist).  dist_gather: the samples'
+// (pred, var) at element `off` of the [T, O] rows of tiled rows [r0, r0 + n) into mu.p[s] / v.p[s] [B][samples].
+// mixture_dist: per window and stage the mixture's quantiles at the host levels[n_levels] into quantiles.p[s] [B][Q]
+// and, where y.p[s] is not null, {crps, nll, pit} of the target y.p[s][b * y_stride + y_off] into scores.p[s] [B][3].
+constexpr int LFMQ_DIST_MAX_LEVELS = 32;
+int dist_gather(cudaStream_t s, int n_stages, int B, int TO, long off, int64_t r0, int n, int samples,
+                const ChainPtrs& pred, const ChainPtrs& var, const ChainPtrs& mu, const ChainPtrs& v);
+int mixture_dist(cudaStream_t s, int n_stages, int B, int samples, const float* levels, int n_levels,
+                 const ChainPtrs& mu, const ChainPtrs& v, const ChainCPtrs& y, long y_stride, long y_off,
+                 const ChainPtrs& quantiles, const ChainPtrs& scores);
 // Integrated gradients (lfmq_integrated_gradients): interpolant k of window b is row k * B + b of the batch tiled M
 // times, with input alpha_k * x[b], alpha_k = (k + 1/2) / M.
 // ig_scale_inputs: xs = rows [r0, r0 + n) of that tiled batch, each scaled by its alpha_k (row_elems = T * F).

@@ -1172,27 +1172,45 @@ size_t mc_rows(int B, int samples, int chunk_max) {
 
 // Caller scratch for `rows` replicated rows per launch: the replicated input and the chain's next-stage windows
 // (win[0], and win[1 ..] read by run_stages as one array), then every stage's sampled preds and vars (m.pred, m.var).
+// With dist_elems > 0 (lfmq_chain_forward_uq_dist, B * samples) every stage's gathered samples mu and v follow.
 struct McWork {
   float* win[lfmq::LFMQ_MAX_STAGES];
   lfmq::McMoments m;
+  lfmq::ChainPtrs mu, v;
 };
-McWork mc_layout(const lfmq_config& c, int S, size_t rows, Carver& cv) {
+McWork mc_layout(const lfmq_config& c, int S, size_t rows, size_t dist_elems, Carver& cv) {
   McWork w{};
   for (int i = 0; i < S; ++i) w.win[i] = cv.take<float>(rows * c.seq_len * c.n_inputs);
   for (int i = 0; i < S; ++i) {
     w.m.pred.p[i] = cv.take<float>(rows * c.seq_len * c.n_outputs);
     w.m.var.p[i] = cv.take<float>(rows * c.seq_len * c.n_outputs);
   }
+  if (dist_elems)
+    for (int i = 0; i < S; ++i) {
+      w.mu.p[i] = cv.take<float>(dist_elems);
+      w.v.p[i] = cv.take<float>(dist_elems);
+    }
   return w;
 }
+
+// The distribution pass of lfmq_chain_forward_uq_dist, run by mc_run after its last launch
+struct DistArgs {
+  const float* levels;
+  int n_levels;
+  const float* const* y;        // nullable
+  float* const* quantiles;
+  float* const* scores;
+};
 
 // The body of both entry points; `chain` numbers the stages' dropout streams.  Sample s of window b is global row
 // row0 + s * B + b of the batch tiled `samples` times, so sample 0 is lfmq_(chain_)forward_uq at (step, row0).  The
 // tiled rows run in launches of at most chunk_max rows, in row order, and each launch's samples are folded into the
 // moments at once.
+// With `dist`, each launch's samples at [T-1, target_idx] are also gathered into the work, and after the last launch
+// the distribution pass reads them.
 int mc_run(const lfmq_handle* st, int S, bool chain, const float* x, int B, int64_t row0, int64_t step, int samples,
            float* const* mean_pred, float* const* mean_var, float* const* var_pred, float* const* var_var, void* work,
-           uint64_t work_bytes, cudaStream_t s, const char* fn) {
+           uint64_t work_bytes, cudaStream_t s, const char* fn, const DistArgs* dist = nullptr) {
   int chunk_max = 0;
   RUN(mc_check(st, S, B, samples, chain, fn, &chunk_max));
   for (int i = 0; i < S; ++i)
@@ -1209,7 +1227,9 @@ int mc_run(const lfmq_handle* st, int S, bool chain, const float* x, int B, int6
   const long row_in = (long)c.seq_len * c.n_inputs, row_out = (long)c.seq_len * c.n_outputs;
   const size_t rows = mc_rows(B, samples, chunk_max);
   McWork w;
-  RUN(carve_work(work, work_bytes, "forward_uq_mc", [&](Carver& cv) { return mc_layout(c, S, rows, cv); }, &w));
+  const size_t dist_elems = dist ? (size_t)B * samples : 0;
+  RUN(carve_work(work, work_bytes, dist ? fn : "forward_uq_mc",
+                 [&](Carver& cv) { return mc_layout(c, S, rows, dist_elems, cv); }, &w));
   lfmq::McMoments& m = w.m;
   for (int i = 0; i < S; ++i) {
     m.mean_pred.p[i] = mean_pred[i];
@@ -1228,8 +1248,20 @@ int mc_run(const lfmq_handle* st, int S, bool chain, const float* x, int B, int6
     }
     RUN(run_stages(st, S, in, n, row0 + r0, step, m.pred.p, m.var.p, w.win[1], s));
     RUN(mc_moments(s, S, B, (int)row_out, r0, n, samples, m));
+    if (dist)
+      RUN(dist_gather(s, S, B, (int)row_out, (long)(c.seq_len - 1) * c.n_outputs + c.target_idx, r0, n, samples, m.pred,
+                      m.var, w.mu, w.v));
   }
-  return 0;
+  if (!dist) return 0;
+  lfmq::ChainCPtrs y{};
+  lfmq::ChainPtrs q{}, sc{};
+  for (int i = 0; i < S; ++i) {
+    y.p[i] = dist->y ? dist->y[i] : nullptr;
+    q.p[i] = dist->quantiles[i];
+    sc.p[i] = dist->y ? dist->scores[i] : nullptr;
+  }
+  return mixture_dist(s, S, B, samples, dist->levels, dist->n_levels, w.mu, w.v, y, row_out,
+                      (long)(c.seq_len - 1) * c.n_outputs + c.target_idx, q, sc);
 }
 }  // namespace
 
@@ -1243,7 +1275,7 @@ int32_t lfmq_chain_forward_uq_mc_work_bytes(const lfmq_handle* stages, int32_t n
   int mb = 0;
   RUN(mc_check(stages, n_stages, B, samples, false, fn, &mb));
   const size_t rows = mc_rows(B, samples, mb);
-  return report_work_bytes(bytes, fn, [&](Carver& cv) { return mc_layout(stages[0]->cfg, n_stages, rows, cv); });
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return mc_layout(stages[0]->cfg, n_stages, rows, 0, cv); });
 }
 
 int32_t lfmq_forward_uq_mc(lfmq_handle h, const float* x, int32_t B, int64_t row0, int64_t step, int32_t samples,
@@ -1259,6 +1291,60 @@ int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, co
                                  void* stream) {
   return mc_run(stages, n_stages, true, x, B, row0, step, samples, mean_pred, mean_var, var_pred, var_var, work,
                 work_bytes, (cudaStream_t)stream, "lfmq_chain_forward_uq_mc");
+}
+
+namespace {
+// The levels: 1 <= n_levels <= LFMQ_DIST_MAX_LEVELS of them, strictly increasing inside (0, 1)
+int dist_levels_check(const float* levels, int32_t n_levels, const char* fn) {
+  if (n_levels < 1 || n_levels > lfmq::LFMQ_DIST_MAX_LEVELS) {
+    LFMQ_SET_ERR("%s: need 1 <= n_levels <= %d (got %d)", fn, lfmq::LFMQ_DIST_MAX_LEVELS, n_levels);
+    return LFMQ_ERR_ARG;
+  }
+  if (!levels) {
+    LFMQ_SET_ERR("%s: levels == NULL", fn);
+    return LFMQ_ERR_ARG;
+  }
+  for (int k = 0; k < n_levels; ++k)
+    if (!(levels[k] > 0.f && levels[k] < 1.f) || (k > 0 && !(levels[k] > levels[k - 1]))) {
+      LFMQ_SET_ERR("%s: levels must be strictly increasing inside (0, 1) (level %d is %g)", fn, k, levels[k]);
+      return LFMQ_ERR_ARG;
+    }
+  return 0;
+}
+}  // namespace
+
+int32_t lfmq_chain_forward_uq_dist_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t B, int32_t samples,
+                                              int32_t n_levels, uint64_t* bytes) {
+  const char* fn = "lfmq_chain_forward_uq_dist_work_bytes";
+  int mb = 0;
+  RUN(mc_check(stages, n_stages, B, samples, false, fn, &mb));
+  if (n_levels < 1 || n_levels > lfmq::LFMQ_DIST_MAX_LEVELS) {
+    LFMQ_SET_ERR("%s: need 1 <= n_levels <= %d (got %d)", fn, lfmq::LFMQ_DIST_MAX_LEVELS, n_levels);
+    return LFMQ_ERR_ARG;
+  }
+  const size_t rows = mc_rows(B, samples, mb);
+  return report_work_bytes(bytes, fn, [&](Carver& cv) {
+    return mc_layout(stages[0]->cfg, n_stages, rows, (size_t)B * samples, cv);
+  });
+}
+
+int32_t lfmq_chain_forward_uq_dist(const lfmq_handle* stages, int32_t n_stages, const float* x, const float* const* y,
+                                   int32_t B, int64_t row0, int64_t step, int32_t samples, const float* levels,
+                                   int32_t n_levels, float* const* mean_pred, float* const* mean_var,
+                                   float* const* var_pred, float* const* var_var, float* const* quantiles,
+                                   float* const* scores, void* work, uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_chain_forward_uq_dist";
+  int chunk_max = 0;
+  RUN(mc_check(stages, n_stages, B, samples, true, fn, &chunk_max));
+  RUN(dist_levels_check(levels, n_levels, fn));
+  for (int i = 0; i < n_stages; ++i)
+    if (!quantiles || !quantiles[i] || (y && (!y[i] || !scores || !scores[i]))) {
+      LFMQ_SET_ERR("%s: null quantiles, target or scores of stage %d", fn, i);
+      return LFMQ_ERR_ARG;
+    }
+  const DistArgs dist{levels, n_levels, y, quantiles, scores};
+  return mc_run(stages, n_stages, true, x, B, row0, step, samples, mean_pred, mean_var, var_pred, var_var, work,
+                work_bytes, (cudaStream_t)stream, fn, &dist);
 }
 
 // ---- integrated gradients of the point forecast (lfmq_integrated_gradients) ----------------------------------------

@@ -544,6 +544,34 @@ class ForecastChainEngine(object):
                                                   *[self._ptrs(o) for o in out], _ptr(work), work.numel(), _stream()))
         return [tuple(o[s] for o in out) for s in range(self.S)]
 
+    def forward_dist(self, x, samples, levels, ys=None, step=0, row0=0):
+        """forward_mc's samples as each window's predictive mixture (lfmq_chain_forward_uq_dist, DESIGN.md section 5g):
+        (moments, quantiles, scores) -- moments per stage forward_mc's (mean_pred, mean_var, var_pred, var_var) bit for
+        bit, the device tensors quantiles [S,B,Q] at the host `levels` and, with ys (per stage targets [B,T,O]),
+        scores [S,B,3] = {crps, nll, pit} of the target at [T-1, target_idx] (NaN where it is NaN), else None."""
+        B = self.stages[0]._check_x(x)
+        lv = np.ascontiguousarray(levels, dtype=np.float32)
+        Q = int(lv.size)
+        out = [[torch.empty(B, self.T, self.O, dtype=torch.float32, device=x.device) for _ in range(self.S)]
+               for _ in range(4)]
+        quantiles = torch.empty(self.S, B, max(Q, 1), dtype=torch.float32, device=x.device)
+        scores = None
+        y_arg = None
+        if ys is not None:
+            assert len(ys) == self.S
+            ys = [y.contiguous() for y in ys]
+            for y in ys:
+                assert y.is_cuda and y.dtype == torch.float32 and y.shape == (B, self.T, self.O)
+            scores = torch.empty(self.S, B, 3, dtype=torch.float32, device=x.device)
+            y_arg = self._ptrs(ys)
+        work = _scratch(self, 'dist', self.lib.lfmq_chain_forward_uq_dist_work_bytes, self._handles, self.S, B,
+                        int(samples), Q)
+        N.check(self.lib.lfmq_chain_forward_uq_dist(
+            self._handles, self.S, _ptr(x), y_arg, B, row0, step, int(samples), lv.ctypes.data_as(C.c_void_p), Q,
+            *[self._ptrs(o) for o in out], self._ptrs(quantiles), self._ptrs(scores) if scores is not None else None,
+            _ptr(work), work.numel(), _stream()))
+        return [tuple(o[s] for o in out) for s in range(self.S)], quantiles, scores
+
     def permutation_importance(self, x, ys, col_group, repeats, seed, step):
         """Permutation importance of the held-out set (x, ys) in one call (lfmq_chain_permutation_importance, DESIGN.md
         section 5e): the device tensor [1 + G * repeats, 3] of the model's loss on the unpermuted set (row 0) and on

@@ -7,6 +7,8 @@ instead, available as ``list_sep=','``.
 """
 from __future__ import absolute_import, division, print_function
 
+import numpy as np
+
 from . import configs
 
 _STRING = 's'
@@ -116,6 +118,9 @@ SCHEMA = [
     ('shapley_samples', _INT, 0, 'Shapley permutation samples (antithetic pairs) per window at prediction; more than 0 '
                                  'also writes pred/shapley.npz: how much each input field and each quarter moves every '
                                  'window\'s forecast (and a UQ model\'s variance) away from a donor window\'s'),
+    ('pred_quantiles', _STRING, None, "'-'-separated levels in (0, 1), e.g. 0.05-0.25-0.5-0.75-0.95, at UQ prediction; "
+                                      'writes pred/quantiles.dat (the quantiles of each window\'s Monte-Carlo dropout '
+                                      'mixture, with its CRPS, log score and PIT) and pred/calibration.dat; unset = off'),
     ('sample_weight_field', _STRING, None, 'Datafile column that weighs each training window in the training loss, read '
                                          'raw at the window\'s last input row (NaN counts as 0; negative or infinite '
                                          'values are refused); unset = off.  Ignored with --train=False'),
@@ -156,3 +161,24 @@ def get_configs(argv=None, list_sep='-'):
         c.piecewise_lr_boundaries = [float(v) for v in str(c.piecewise_lr_boundaries).split('-')]
         c.piecewise_lr_values = [float(v) for v in str(c.piecewise_lr_values).split('-')]
     return c
+
+
+MAX_PRED_QUANTILES = 32      # lfmq_chain_forward_uq_dist's cap on the levels
+
+
+def pred_quantile_levels(spec):
+    """The levels of --pred_quantiles: None when unset, else the '-'-separated floats, which must be strictly
+    increasing inside (0, 1), at most MAX_PRED_QUANTILES of them.  A malformed value raises ValueError."""
+    if spec is None or str(spec).strip() == '':
+        return None
+    try:
+        levels = [float(v) for v in str(spec).split('-')]
+    except ValueError:
+        raise ValueError("--pred_quantiles %s: expected '-'-separated levels such as 0.05-0.5-0.95" % spec)
+    if not 1 <= len(levels) <= MAX_PRED_QUANTILES:
+        raise ValueError('--pred_quantiles %s: between 1 and %d levels' % (spec, MAX_PRED_QUANTILES))
+    if any(not 0.0 < v < 1.0 for v in levels) or any(b <= a for a, b in zip(levels, levels[1:])):
+        raise ValueError('--pred_quantiles %s: the levels must be strictly increasing inside (0, 1)' % spec)
+    if any(not 0.0 < v < 1.0 for v in np.float32(levels)) or any(np.diff(np.float32(levels)) <= 0):
+        raise ValueError('--pred_quantiles %s: the levels must stay distinct inside (0, 1) in single precision' % spec)
+    return levels

@@ -131,6 +131,22 @@ class NativeForecaster(object):
         return self._wide_engine(int(samples) * self.config.batch_size).forward_mc(
             _to_device(self.engine, inp), int(samples), step=self._calls)
 
+    def predict_dist(self, inp, samples, levels, targets=None):
+        """predict_mc's samples as each window's predictive mixture (ForecastChainEngine.forward_dist, DESIGN.md
+        section 5g): (moments, quantiles, scores) -- moments predict_mc's bit for bit, quantiles [S,B,Q] the mixture's
+        quantiles at `levels` and, with targets (the list of forecast_steps targets [B,T,O]), scores [S,B,3] =
+        {crps, nll, pit} of the target at the last step, else None.  One step per call, on the engine predict_mc
+        uses."""
+        if not self.uq:
+            raise ValueError('predict_dist needs a uq model (RNNUqRangeEstimate): a point estimate predicts with dropout '
+                             'off (training=config.train), so it has no predictive distribution')
+        if int(samples) < 1:
+            raise ValueError('predict_dist: samples must be >= 1 (got %r)' % (samples,))
+        ys = None if targets is None else [_to_device(self.engine, t) for t in targets]
+        self._calls += 1
+        return self._wide_engine(int(samples) * self.config.batch_size).forward_dist(
+            _to_device(self.engine, inp), int(samples), levels, ys=ys, step=self._calls)
+
     def permutation_importance(self, inp, targets, repeats):
         """Permutation importance of the held-out windows (inp, targets) (ForecastChainEngine.permutation_importance,
         DESIGN.md section 5e): the device tensors (fields [1 + F * repeats, 3], quarters [1 + T * repeats, 3]) of the

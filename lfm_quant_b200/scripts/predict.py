@@ -10,6 +10,7 @@ from collections import defaultdict
 import numpy as np
 import pandas as pd
 
+from .base_config import pred_quantile_levels
 from .model_utils.model import Model
 
 
@@ -45,6 +46,8 @@ class Predict(object):
         ig = defaultdict(list)
         held_out = []
         windows = []
+        levels = pred_quantile_levels(getattr(self.config, 'pred_quantiles', None))
+        dist = defaultdict(list)
         for (inp_dev, target_dev, metadata) in self._batches:
             # one target window per input window: every forecast step is compared with it (Train._step_targets)
             inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()] * self.config.forecast_steps
@@ -60,14 +63,24 @@ class Predict(object):
                 if self.config.forecast_steps == 1:
                     preds = [preds]
                 variance = [np.zeros(x.shape) for x in preds]   # predict.py:133
-            elif self.config.mc_samples > 1:
-                # the reference's UQ ensemble in one prediction: the mean of the samples, and mean of the variances +
-                # variance of the variances (utils/post_processing.py:52-55); var_pred, the spread of the sampled
-                # predictions, is the one added column
-                moments = [[t.cpu().numpy() for t in m] for m in self.model.predict_mc(inp_dev, self.config.mc_samples)]
+            elif self.config.mc_samples > 1 or levels is not None:
+                if levels is None:
+                    moments = self.model.predict_mc(inp_dev, self.config.mc_samples)
+                else:           # the same samples and moments, and each window's mixture (quantiles.dat)
+                    moments, q, scores = self.model.predict_dist(inp_dev, self.config.mc_samples, levels,
+                                                                 [target_dev] * self.config.forecast_steps)
+                    dist['quantiles'].append(q.cpu().numpy())
+                    dist['scores'].append(scores.cpu().numpy())
+                moments = [[t.cpu().numpy() for t in m] for m in moments]
                 preds = [m[0] for m in moments]
-                variance = [m[1] + m[3] for m in moments]
-                outputs['norm_preds_var'].append(self._extract_preds([m[2] for m in moments]))
+                if self.config.mc_samples > 1:
+                    # the reference's UQ ensemble in one prediction: the mean of the samples, and mean of the
+                    # variances + variance of the variances (utils/post_processing.py:52-55); var_pred, the spread of
+                    # the sampled predictions, is the one added column
+                    variance = [m[1] + m[3] for m in moments]
+                    outputs['norm_preds_var'].append(self._extract_preds([m[2] for m in moments]))
+                else:           # one sample: its prediction and variance, the bits model.predict returns
+                    variance = [m[1] for m in moments]
             else:                       # predict.py:135-138: [tar_1, var_1, .., tar_S, var_S]
                 model_preds = self.model.predict(inp_dev)
                 preds, variance = model_preds[0::2], model_preds[1::2]
@@ -134,11 +147,24 @@ class Predict(object):
 
         df['gvkey'] = df['gvkey'].apply(lambda x: x.decode('utf-8') if isinstance(x, bytes) else str(x))
         df.to_csv(os.path.join(self.pred_dir, self.config.preds_fname), sep=' ', index=False, date_format="%Y%m%d")
+        if levels is not None:
+            self._write_quantiles(df, levels, np.concatenate(dist['quantiles'], axis=1),
+                                  np.concatenate(dist['scores'], axis=1), unscale)
         print("Unscaled MSE normalized by Seq_Norm (%s)" % self.config.model_dir.split('/')[-1])
         print(df[[x for x in df.columns if 'unscaled' in x]].mean())
         for i in range(self.config.forecast_steps):
             print("Scaled MSE for step %i: %1.4f" % (i + 1, df['norm_squared_diff_' + str(i + 1)].mean()))
         return df
+
+    def _write_quantiles(self, df, levels, quantiles, scores, unscale):
+        """<model_dir>/pred/quantiles.dat and calibration.dat (--pred_quantiles): the predictive quantiles and scores
+        of every row of preds.dat (`df`, in its order) from NativeForecaster.predict_dist (quantiles [S,N,Q], scores
+        [S,N,3]); quantile_table and calibration_table give the layouts."""
+        targets = np.stack([df['norm_targets_%d' % (s + 1)].to_numpy() for s in range(len(quantiles))])
+        quantile_table(df[['date', 'gvkey']], levels, quantiles, scores, unscale).to_csv(
+            os.path.join(self.pred_dir, 'quantiles.dat'), sep=' ', index=False, date_format="%Y%m%d")
+        calibration_table(levels, quantiles, scores, targets).to_csv(
+            os.path.join(self.pred_dir, 'calibration.dat'), sep=' ', index=False)
 
     def _write_attributions(self, outputs, ig):
         """<model_dir>/pred/attributions.npz: the integrated-gradients attributions of norm_preds_1 (--ig_steps), one
@@ -239,3 +265,55 @@ def write_shapley(path, date, gvkey, field_names, outputs, phi_field, phi_quarte
              outputs=np.array(list(outputs)), phi_field=np.asarray(phi_field, dtype=np.float32),
              phi_quarter=np.asarray(phi_quarter, dtype=np.float32), f_x=np.asarray(f_x, dtype=np.float32),
              f_bg=np.asarray(f_bg, dtype=np.float32))
+
+
+def quantile_name(level):
+    """q<100 tau> of a level, as %g formats it: 0.05 -> q5, 0.5 -> q50, 0.125 -> q12.5."""
+    return 'q%g' % (100.0 * level)
+
+
+def quantile_table(keys, levels, quantiles, scores, unscale):
+    """The rows of quantiles.dat: `keys` (date, gvkey of preds.dat), then per forecast step s the mixture quantiles
+    norm_q<100 tau>_s (normalised units), q<100 tau>_s = unscale(norm_q<100 tau>_s) (the fundamentals' units: quantiles
+    pass through the increasing map of centre, scale, expm1 and seq_norm unchanged wherever seq_norm > 0, and their
+    order reverses where seq_norm < 0), and crps_s, nll_s and pit_s of the normalised target (NaN where it is unknown).
+    quantiles [S,N,Q] and scores [S,N,3] as NativeForecaster.predict_dist returns them."""
+    df = keys.reset_index(drop=True).copy()
+    for s in range(len(quantiles)):
+        for k, level in enumerate(levels):
+            df['norm_%s_%d' % (quantile_name(level), s + 1)] = quantiles[s][:, k]
+        for k, level in enumerate(levels):
+            df['%s_%d' % (quantile_name(level), s + 1)] = unscale(quantiles[s][:, k])
+        for j, name in enumerate(('crps', 'nll', 'pit')):
+            df['%s_%d' % (name, s + 1)] = scores[s][:, j]
+    return df
+
+
+def pit_ks(pit):
+    """The Kolmogorov-Smirnov distance sup |F_n(u) - u| of the PIT values from U(0, 1); NaN when there are none."""
+    p = np.sort(np.asarray(pit, dtype=np.float64))
+    n = len(p)
+    if n == 0:
+        return np.nan
+    i = np.arange(1, n + 1)
+    return float(max(np.max(i / n - p), np.max(p - (i - 1) / n)))
+
+
+def calibration_table(levels, quantiles, scores, targets):
+    """The rows of calibration.dat, one per (forecast step, level): frac_below, the share of the n_known windows with a
+    known normalised target (targets [S,N]) whose target lies below norm_q<100 tau> -- close to the level when the
+    forecast is calibrated -- and, repeated on every row of a step, the mean CRPS and log score of those windows and
+    pit_ks, the Kolmogorov-Smirnov distance of their PIT values from U(0, 1)."""
+    rows = []
+    for s in range(len(quantiles)):
+        y = np.asarray(targets[s], dtype=np.float64)
+        known = np.isfinite(y)
+        n = int(known.sum())
+        sc = np.asarray(scores[s], dtype=np.float64)[known]
+        mean_crps, mean_nll = (float(sc[:, 0].mean()), float(sc[:, 1].mean())) if n else (np.nan, np.nan)
+        ks = pit_ks(sc[:, 2])
+        for k, level in enumerate(levels):
+            below = float(np.mean(y[known] < np.asarray(quantiles[s])[known, k])) if n else np.nan
+            rows.append({'step': s + 1, 'level': level, 'frac_below': below, 'n_known': n, 'mean_crps': mean_crps,
+                         'mean_nll': mean_nll, 'pit_ks': ks})
+    return pd.DataFrame(rows, columns=['step', 'level', 'frac_below', 'n_known', 'mean_crps', 'mean_nll', 'pit_ks'])

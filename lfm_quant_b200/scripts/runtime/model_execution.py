@@ -22,6 +22,8 @@ import pandas as pd
 import scipy.optimize
 import scipy.stats
 
+from .. import base_config
+
 
 def member_configs(config):
     """The N = num_procs members of a point-estimate ensemble (model_execution.py:162-190): member k has member_id k,
@@ -354,6 +356,11 @@ class ModelExecution(object):
             raise ValueError('--shapley_samples %d: Shapley attributions explain the forecasts of a trained model, at '
                              'prediction (--train=False), with shapley_samples >= 1 permutation samples (0 = off); '
                              'NaivePointEstimate has no model to explain' % c.shapley_samples)
+        if getattr(c, 'pred_quantiles', None) is not None:
+            if not c.UQ or c.train:
+                raise ValueError('--pred_quantiles %s: predictive quantiles are those of a UQ model\'s Monte-Carlo '
+                                 'dropout mixture, at prediction (--UQ=True --train=False)' % c.pred_quantiles)
+            base_config.pred_quantile_levels(c.pred_quantiles)
         check_row_weights(c)
         if c.training_type == 'iterative':
             check_walk_forward(c)
@@ -475,6 +482,11 @@ class ModelExecution(object):
                                              dtype={'group': str}, float_precision='round_trip')
                                  for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
                 os.path.join(experiment_dir, 'walk_forward_importance.dat'), sep=' ', index=False)
+        if getattr(cfg, 'pred_quantiles', None) is not None:
+            stitch_walk_forward([pd.read_csv(os.path.join(pred.model_dir, 'pred', 'quantiles.dat'), sep=' ',
+                                             dtype={'gvkey': str}, float_precision='round_trip')
+                                 for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
+                os.path.join(experiment_dir, 'walk_forward_quantiles.dat'), sep=' ', index=False)
         _print_scaled_mse(df, cfg.forecast_steps)
         return df
 
