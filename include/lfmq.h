@@ -381,6 +381,35 @@ int32_t lfmq_chain_shapley_work_bytes(const lfmq_handle* stages, int32_t n_stage
 int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N,
                            const int32_t* col_group, int32_t G, int32_t samples, uint64_t seed, int64_t step,
                            float* phi, float* f_x, float* f_bg, void* work, uint64_t work_bytes, void* stream);
+/* ---- accumulated local effects -------------------------------------------------------------------------------------
+ * In which direction and with what shape the forecast responds to single input columns (ALE, Apley & Zhu 2020).
+ * x [N,T,F] (or [N,T*F] on a dense handle) are the model's inputs; feature g < G is column cols[g] in [0, T*F) (host
+ * int32 [G]), c = t * F + f.  The J explained outputs are those of lfmq_chain_shapley (J = S, 2S on a uq chain, 1 on a
+ * dense handle).  Per feature: v_i = x[i, cols[g]]; non-finite values are left out, N' counts the others.  With v_(1) <=
+ * .. <= v_(N') sorted, the type-1 quantiles q_0 = v_(1), q_k = v_(ceil(k N' / K)) for k = 1..K with repeated values
+ * dropped are the edges z_0 < .. < z_Kg, n_bins[g] = Kg <= K (0 with fewer than two distinct finite values).  Window i is
+ * in bin k (1-based) when z_{k-1} < v_i <= z_k, or v_i = z_0 for k = 1; n_k windows are.  Its local effect d_i =
+ * f(x_i with column cols[g] at z_k) - f(x_i with it at z_{k-1}), fp32, both copies keyed as row i at `step` (on a uq
+ * model they share window i's dropout masks; point and dense models predict with dropout off).  Outputs (device):
+ *   n_bins [G] int32; edges [G][K+1] fp32, z_k, NaN past Kg (and at 0 when N' = 0); counts [G][K] int32, n_k, 0 past Kg;
+ *   local_mean [G][K][J] and local_sd [G][K][J]: the mean and population standard deviation of d over bin k;
+ *   ale [G][K+1][J]: g(z_k) - (1/N') sum_k n_k (g(z_{k-1}) + g(z_k)) / 2 with g(z_0) = 0, g(z_k) = sum_{k'<=k}
+ *   local_mean_k' (ALEPlot's centring: the count-weighted mean effect is 0).  Every float output is NaN past Kg, and
+ *   ale, local_mean and local_sd are NaN throughout when Kg = 0.
+ * The values are sorted per feature by a stable segmented radix sort (ties keep window order, -0 counts as +0); each
+ * bin's sums run over its contiguous run of that order in fp64 in a fixed order, without atomics, so the outputs do not
+ * depend on max_batch or on where launches are cut, and two calls give the same bits.  The call waits once for n_bins
+ * on the host, to skip the copies of features without bins.  Accepted: what lfmq_chain_permutation_importance accepts.
+ * The handles' parameters, gradient buffers (tail included) and optimizer slots are left untouched.  N, G or K < 1,
+ * K > 1024, G * N >= 2^31, a column outside [0, T*F) or a null pointer: LFMQ_ERR_ARG.  `work`: caller-owned device
+ * scratch, 256-byte aligned, of the size the *_work_bytes query gives: one launch's rows (per stage), the cols copy, the
+ * sort's keys, windows and temp storage, the bin ends [G][K+1], every window's bin [G][N], d [N][J], the fp64 bin means
+ * [K][J] and one launch's predictions (and variances). */
+int32_t lfmq_chain_ale_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N, int32_t G, int32_t K,
+                                  uint64_t* bytes);
+int32_t lfmq_chain_ale(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N, const int32_t* cols,
+                       int32_t G, int32_t K, int64_t step, int32_t* n_bins, float* edges, int32_t* counts, float* ale,
+                       float* local_mean, float* local_sd, void* work, uint64_t work_bytes, void* stream);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

@@ -110,6 +110,27 @@ int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems
 struct ShapleySrc { const float* p[2 * LFMQ_MAX_STAGES]; };
 int shapley_fold(cudaStream_t s, const ShapleySrc& src, int K, long stride, long off, int a, int n, int k, int G,
                  const int32_t* order, float* prev, float* phi, float* f_x, float* f_bg);
+// Accumulated local effects (ale.cu, lfmq_chain_ale).  ale_sort_bytes: the temp storage of the segmented radix sort of
+// G segments of N (value, window) pairs.  ale_bins: the values x[i, cols[g]] sorted per feature into skey / sval, the
+// edges, counts and n_bins outputs, the sorted bin ends ends [G][K+1] and every window's bin bin_of [G][N] (0: none).
+constexpr int LFMQ_ALE_MAX_BINS = 1024;
+struct AleSort {
+  float *key, *skey;
+  int32_t *val, *sval, *off, *ends, *bin_of;
+};
+int ale_sort_bytes(int N, int G, size_t* bytes);
+int ale_bins(cudaStream_t s, const float* x, int N, long row_elems, const int32_t* cols, int G, int K, void* temp,
+             size_t temp_bytes, const AleSort& w, int32_t* n_bins, float* edges, int32_t* counts);
+// ale_gather: rows [a, a + n) of x [N, row_elems] into out with column col at edge[bin_of[i] - 1 + upper].
+int ale_gather(cudaStream_t s, const float* x, long row_elems, int col, const int32_t* bin_of, const float* edge,
+               int upper, int a, int n, float* out);
+// ale_pick: the J explained outputs of windows [a, a + n) (as shapley_fold reads them) into d [N][J] on the upper copy,
+// subtracted from it on the lower one.
+int ale_pick(cudaStream_t s, const ShapleySrc& src, int J, long stride, long off, int a, int n, int upper, float* d);
+// ale_fold: feature g's per-bin mean and population sd of d over each bin's sorted run, then ale = the centred prefix
+// sums of the means; mean [K][J] is fp64 scratch.
+int ale_fold(cudaStream_t s, const AleSort& w, const int32_t* n_bins, int g, int N, int K, int J, const float* d,
+             double* mean, float* ale, float* local_mean, float* local_sd);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

@@ -1572,6 +1572,26 @@ CopyWork shapley_layout(const lfmq_handle* st, int S, int rows, int N, int G, in
   return w;
 }
 
+// The explained outputs of a launch (Shapley, ALE): the pointers to every stage's predictions, tar_1, var_1, ..,
+// tar_S, var_S on a uq chain (Keras list order), read at row stride row_out_of and at explained_off within a row:
+// pred[T-1, target_idx] ([target_idx] on a dense handle).
+lfmq::ShapleySrc explained_src(const lfmq_handle* st, int S, float* const* pred, float* const* var) {
+  lfmq::ShapleySrc src{};
+  for (int i = 0; i < S; ++i) {
+    if (st[0]->cfg.uq) {
+      src.p[2 * i] = pred[i];
+      src.p[2 * i + 1] = var[i];
+    } else {
+      src.p[i] = pred[i];
+    }
+  }
+  return src;
+}
+long explained_off(const lfmq_handle* st) {
+  const lfmq_config& c = st[0]->cfg;
+  return st[0]->path == Path::Dense ? c.target_idx : (long)(c.seq_len - 1) * c.n_outputs + c.target_idx;
+}
+
 int shapley_args_check(int32_t N, int32_t G, int32_t samples, const char* fn) {
   if (N < 1 || G < 1 || samples < 1) {
     LFMQ_SET_ERR("%s: need N, G and samples >= 1 (got %d, %d, %d)", fn, N, G, samples);
@@ -1677,8 +1697,7 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
   RUN(pi_check(stages, n_stages, N, fn, &rows));
   RUN(shapley_args_check(N, G, samples, fn));
   const int S = n_stages, M = samples, K = shapley_outputs(stages, S);
-  const lfmq_config& c = stages[0]->cfg;
-  const bool dense = stages[0]->path == Path::Dense, uq = c.uq != 0;
+  const bool uq = stages[0]->cfg.uq != 0;
   const long row_in = row_in_of(stages), row_out = row_out_of(stages);
   if (!x || !col_group || !phi || !f_x || !f_bg) {
     LFMQ_SET_ERR("%s: null pointer", fn);
@@ -1688,17 +1707,8 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
   CopyWork w;
   RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return shapley_layout(stages, S, rows, N, G, M, cv); }, &w));
   cudaStream_t s = (cudaStream_t)stream;
-  // the explained value of a launch row: pred[T-1, target_idx] ([target_idx] on a dense handle)
-  ShapleyFold fold{{}, K, row_out, dense ? c.target_idx : (long)(c.seq_len - 1) * c.n_outputs + c.target_idx, G,
-                   nullptr, w.prev, phi, f_x, f_bg};
-  for (int i = 0; i < S; ++i) {
-    if (uq) {                                    // Keras list order: tar_1, var_1, .., tar_S, var_S
-      fold.src.p[2 * i] = w.pred[i];
-      fold.src.p[2 * i + 1] = w.var[i];
-    } else {
-      fold.src.p[i] = w.pred[i];
-    }
-  }
+  ShapleyFold fold{explained_src(stages, S, w.pred, w.var), K, row_out, explained_off(stages), G, nullptr, w.prev, phi,
+                   f_x, f_bg};
   // Sample m belongs to pair p = m / 2.  An even sample orders the groups by o[q] = perm_index(G, seed, 0x40000001,
   // p, q); an odd one reverses its partner's ordering (antithetic) and keeps its donors.
   std::vector<int32_t> ord((size_t)M * G), rk((size_t)M * G);
@@ -1729,6 +1739,111 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
   RUN(scale_inplace(s, (long)N * K * G, phi, inv));
   RUN(scale_inplace(s, (long)N * K, f_x, inv));
   RUN(scale_inplace(s, (long)N * K, f_bg, inv));
+  return LFMQ_OK;
+}
+
+// ---- accumulated local effects (lfmq_chain_ale) ---------------------------------------------------------------------
+namespace {
+// Caller scratch of ALE: a launch's rows and the chain's next-stage windows (as CopyWork), the device cols, the sort's
+// keys and windows before and after, its segment offsets, the bin ends [G][K+1], every window's bin [G][N], the local
+// effects d [N][J], the fp64 bin means [K][J], one launch's outputs, and the sort's temp storage.
+struct AleWork {
+  float* win[lfmq::LFMQ_MAX_STAGES];
+  int32_t* cols;
+  lfmq::AleSort sort;
+  float* d;
+  double* mean;
+  float* pred[lfmq::LFMQ_MAX_STAGES];
+  float* var[lfmq::LFMQ_MAX_STAGES];
+  void* temp;
+};
+AleWork ale_layout(const lfmq_handle* st, int S, int rows, int N, int G, int K, size_t temp_bytes, Carver& cv) {
+  const size_t row_in = row_in_of(st), row_out = row_out_of(st), J = shapley_outputs(st, S), GN = (size_t)G * N;
+  AleWork w{};
+  for (int i = 0; i < S; ++i) w.win[i] = cv.take<float>(rows * row_in);
+  w.cols = cv.take<int32_t>(G);
+  w.sort.key = cv.take<float>(GN);
+  w.sort.skey = cv.take<float>(GN);
+  w.sort.val = cv.take<int32_t>(GN);
+  w.sort.sval = cv.take<int32_t>(GN);
+  w.sort.off = cv.take<int32_t>(G + 1);
+  w.sort.ends = cv.take<int32_t>((size_t)G * (K + 1));
+  w.sort.bin_of = cv.take<int32_t>(GN);
+  w.d = cv.take<float>(N * J);
+  w.mean = cv.take<double>(K * J);
+  for (int i = 0; i < S; ++i) w.pred[i] = cv.take<float>(rows * row_out);
+  if (st[0]->cfg.uq)
+    for (int i = 0; i < S; ++i) w.var[i] = cv.take<float>(rows * row_out);
+  w.temp = cv.take<char>(temp_bytes);
+  return w;
+}
+
+// pi_check, then N, G, K >= 1 with K <= LFMQ_ALE_MAX_BINS and G * N within the sort's int32 item count; *temp_bytes =
+// the sort's temp storage.
+int ale_check(const lfmq_handle* st, int32_t S, int32_t N, int32_t G, int32_t K, const char* fn, int* rows,
+              size_t* temp_bytes) {
+  RUN(pi_check(st, S, N, fn, rows));
+  if (G < 1 || K < 1 || K > lfmq::LFMQ_ALE_MAX_BINS || (int64_t)G * N > INT32_MAX) {
+    LFMQ_SET_ERR("%s: need N, G >= 1 with G * N < 2^31 and 1 <= K <= %d (got %d, %d, %d)", fn,
+                 lfmq::LFMQ_ALE_MAX_BINS, N, G, K);
+    return LFMQ_ERR_ARG;
+  }
+  return lfmq::ale_sort_bytes(N, G, temp_bytes);
+}
+}  // namespace
+
+int32_t lfmq_chain_ale_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N, int32_t G, int32_t K,
+                                  uint64_t* bytes) {
+  const char* fn = "lfmq_chain_ale_work_bytes";
+  int rows = 0;
+  size_t tb = 0;
+  RUN(ale_check(stages, n_stages, N, G, K, fn, &rows, &tb));
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return ale_layout(stages, n_stages, rows, N, G, K, tb, cv); });
+}
+
+int32_t lfmq_chain_ale(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N, const int32_t* cols,
+                       int32_t G, int32_t K, int64_t step, int32_t* n_bins, float* edges, int32_t* counts, float* ale,
+                       float* local_mean, float* local_sd, void* work, uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_chain_ale";
+  int rows = 0;
+  size_t tb = 0;
+  RUN(ale_check(stages, n_stages, N, G, K, fn, &rows, &tb));
+  const int S = n_stages, J = shapley_outputs(stages, S);
+  const long row_in = row_in_of(stages), row_out = row_out_of(stages);
+  if (!x || !cols || !n_bins || !edges || !counts || !ale || !local_mean || !local_sd) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  for (int g = 0; g < G; ++g)
+    if (cols[g] < 0 || cols[g] >= row_in) {
+      LFMQ_SET_ERR("%s: cols[%d] = %d outside [0, T * F = %ld)", fn, g, cols[g], row_in);
+      return LFMQ_ERR_ARG;
+    }
+  AleWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return ale_layout(stages, S, rows, N, G, K, tb, cv); }, &w));
+  cudaStream_t s = (cudaStream_t)stream;
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.cols, cols, G * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  RUN(ale_bins(s, x, N, row_in, w.cols, G, K, w.temp, tb, w.sort, n_bins, edges, counts));
+  // the bins decide which features have copies to run: a feature with fewer than two distinct values has none
+  std::vector<int32_t> kg(G);
+  LFMQ_CUDA_CHECK(cudaMemcpyAsync(kg.data(), n_bins, G * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  LFMQ_CUDA_CHECK(cudaStreamSynchronize(s));
+  const lfmq::ShapleySrc src = explained_src(stages, S, w.pred, w.var);
+  const long off = explained_off(stages);
+  // Feature g's two copies set column cols[g] of window i to the upper and the lower edge of its bin.  Every launch
+  // keys its rows by window index (row0 = a), so both copies of window i share its dropout masks at `step`.
+  for (int g = 0; g < G; ++g) {
+    for (int a = 0; kg[g] > 0 && a < N; a += rows) {
+      const int n = std::min(rows, N - a);
+      for (int upper = 1; upper >= 0; --upper) {
+        RUN(ale_gather(s, x, row_in, cols[g], w.sort.bin_of + (size_t)g * N, edges + (size_t)g * (K + 1), upper, a, n,
+                       w.win[0]));
+        RUN(run_stages(stages, S, w.win[0], n, a, step, w.pred, stages[0]->cfg.uq ? w.var : nullptr, w.win[1], s));
+        RUN(ale_pick(s, src, J, row_out, off, a, n, upper, w.d));
+      }
+    }
+    RUN(ale_fold(s, w.sort, n_bins, g, N, K, J, w.d, w.mean, ale, local_mean, local_sd));
+  }
   return LFMQ_OK;
 }
 

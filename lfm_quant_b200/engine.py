@@ -614,6 +614,30 @@ class ForecastChainEngine(object):
             _ptr(f_x), _ptr(f_bg), _ptr(work), work.numel(), _stream()))
         return phi, f_x, f_bg
 
+    def ale(self, x, cols, bins, step):
+        """Accumulated local effects of single input columns in one call (lfmq_chain_ale, DESIGN.md section 5h): the
+        device tensors (n_bins [G] int32, edges [G,K+1], counts [G,K] int32, ale [G,K+1,J], local_mean [G,K,J],
+        local_sd [G,K,J]) of feature g = column cols[g] of the flattened window (t * F + f), with K = `bins` requested
+        quantile bins and the J outputs shapley explains.  Both copies of window i draw its dropout masks at (step,
+        row i).  N is not bounded by max_batch; the engine's parameters, gradients and optimizer state are left as they
+        were."""
+        B = self.stages[0]._check_x(x)
+        cols = np.ascontiguousarray(cols, dtype=np.int32)
+        G, K = int(cols.size), int(bins)
+        J = 1 if isinstance(self.stages[0], DenseEngine) else (2 * self.S if self.uq else self.S)
+        work = _scratch(self, 'ale', self.lib.lfmq_chain_ale_work_bytes, self._handles, self.S, B, G, K)
+        n_bins = torch.empty(G, dtype=torch.int32, device=self.device)
+        edges = torch.empty(G, K + 1, dtype=torch.float32, device=self.device)
+        counts = torch.empty(G, K, dtype=torch.int32, device=self.device)
+        ale = torch.empty(G, K + 1, J, dtype=torch.float32, device=self.device)
+        local_mean = torch.empty(G, K, J, dtype=torch.float32, device=self.device)
+        local_sd = torch.empty_like(local_mean)
+        N.check(self.lib.lfmq_chain_ale(
+            self._handles, self.S, _ptr(x), B, cols.ctypes.data_as(C.c_void_p), G, K, int(step), _ptr(n_bins),
+            _ptr(edges), _ptr(counts), _ptr(ale), _ptr(local_mean), _ptr(local_sd), _ptr(work), work.numel(),
+            _stream()))
+        return n_bins, edges, counts, ale, local_mean, local_sd
+
     def loss(self, preds, ys):
         """Losses.weight_adjusted_mse(ys, preds): device tensor {loss, mse}."""
         if self._one is not None:

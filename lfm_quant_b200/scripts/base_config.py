@@ -118,6 +118,9 @@ SCHEMA = [
     ('shapley_samples', _INT, 0, 'Shapley permutation samples (antithetic pairs) per window at prediction; more than 0 '
                                  'also writes pred/shapley.npz: how much each input field and each quarter moves every '
                                  'window\'s forecast (and a UQ model\'s variance) away from a donor window\'s'),
+    ('ale_bins', _INT, 0, 'Quantile bins per input field for accumulated local effects at prediction; more than 0 '
+                          'also writes pred/ale.dat: in which direction and with what shape the forecast (and a UQ '
+                          'model\'s variance) responds to each input field\'s latest value'),
     ('pred_quantiles', _STRING, None, "'-'-separated levels in (0, 1), e.g. 0.05-0.25-0.5-0.75-0.95, at UQ prediction; "
                                       'writes pred/quantiles.dat (the quantiles of each window\'s Monte-Carlo dropout '
                                       'mixture, with its CRPS, log score and PIT) and pred/calibration.dat; unset = off'),

@@ -15,7 +15,7 @@ from ...model_utils.initializers import Initializer
 from ...model_utils.optimizers import Optimizers
 
 # Rows per launch of the model's wide engine (NativeForecaster._wide_engine), on which predict_mc,
-# permutation_importance and shapley run: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to 10x
+# permutation_importance, shapley and ale run: the width at which one call of 32 samples at B = 256 ran 4x (fp32) to 10x
 # (bf16x3) faster than a handle of B rows on an H100 (DESIGN.md section 5c).
 MC_ROWS = 8192
 # Rows per launch of NativeForecaster.attribute: the saved activations and gradients of the fp32 step grow with the rows
@@ -185,8 +185,23 @@ class NativeForecaster(object):
                                              for groups in (cols % F, cols // F))
         return phi_f, phi_q, f_x, f_bg
 
+    def ale(self, inp, bins):
+        """Accumulated local effects of every input field's latest value (ForecastChainEngine.ale, DESIGN.md section
+        5h): column (T-1) * F + f of the flattened window for field f, always real data as the batcher pads at the
+        front.  The device tensors (n_bins [F], edges [F,K+1], counts [F,K], ale [F,K+1,J], local_mean [F,K,J],
+        local_sd [F,K,J]) for K = `bins` requested quantile bins and the J outputs shapley explains.  One step, the
+        model's next call, so a uq window draws the same dropout masks in both copies.  Runs on the wide engine of
+        min(N, MC_ROWS) rows per launch."""
+        if int(bins) < 1:
+            raise ValueError('ale: bins must be >= 1 (got %r)' % (bins,))
+        x = _to_device(self.engine, inp)
+        T, F = self.engine.T, self.engine.F
+        self._calls += 1
+        eng = self._wide_engine(x.shape[0])
+        return eng.ale(x, (T - 1) * F + np.arange(F), int(bins), self._calls)
+
     def _wide_engine(self, rows):
-        """The forward-only engine that predict_mc, permutation_importance and shapley run on: the model's own
+        """The forward-only engine that predict_mc, permutation_importance, shapley and ale run on: the model's own
         (batch_size rows) when it is as wide as `rows` or MC_ROWS, as at one sample, where a wider handle is slower
         (DESIGN.md section 5c).  Else a forward-only chain of the same stages and precision with max_batch =
         min(rows, MC_ROWS) and the model engine's device share, created at the first such call (again for a larger

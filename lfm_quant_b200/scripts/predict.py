@@ -91,7 +91,7 @@ class Predict(object):
                     ig[key].append(t.cpu().numpy())
             if self.config.perm_importance > 0:
                 held_out.append((inp_dev, target_dev))
-            if self.config.shapley_samples > 0:
+            if self.config.shapley_samples > 0 or self.config.ale_bins > 0:
                 windows.append(inp_dev)
         if self.config.ig_steps > 0:
             self._write_attributions(outputs, ig)
@@ -99,6 +99,8 @@ class Predict(object):
             self._write_importance(held_out)
         if self.config.shapley_samples > 0:
             self._write_shapley(outputs, windows)
+        if self.config.ale_bins > 0:
+            self._write_ale(windows)
 
         single_outputs = ['date', 'gvkey', 'seq_norm'] + [x for x in outputs.keys() if 'inp_t' in x]
         for key in single_outputs:
@@ -207,6 +209,16 @@ class Predict(object):
                       np.vstack(outputs['gvkey']).flatten(), self.dataset.fin_col_names + self.dataset.aux_col_names,
                       shapley_output_names(self.config.forecast_steps, self.config.UQ), phi_f, phi_q, f_x, f_bg)
 
+    def _write_ale(self, windows):
+        """<model_dir>/pred/ale.dat (--ale_bins K): the accumulated local effects of every input field's latest value
+        over every predicted window, known targets or not (NativeForecaster.ale over all batches at once; ale_table
+        gives the layout)."""
+        import torch
+        out = [t.cpu().numpy() for t in self.model.ale(torch.cat(windows), self.config.ale_bins)]
+        ale_table(self.dataset.fin_col_names + self.dataset.aux_col_names,
+                  shapley_output_names(self.config.forecast_steps, self.config.UQ), *out).to_csv(
+            os.path.join(self.pred_dir, 'ale.dat'), sep=' ', index=False)
+
     def _flat(self):
         """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""
         return 'MLP' in self.config.nn_type or 'Naive' in self.config.nn_type
@@ -265,6 +277,31 @@ def write_shapley(path, date, gvkey, field_names, outputs, phi_field, phi_quarte
              outputs=np.array(list(outputs)), phi_field=np.asarray(phi_field, dtype=np.float32),
              phi_quarter=np.asarray(phi_quarter, dtype=np.float32), f_x=np.asarray(f_x, dtype=np.float32),
              f_bg=np.asarray(f_bg, dtype=np.float32))
+
+
+def ale_table(field_names, outputs, n_bins, edges, counts, ale, local_mean, local_sd):
+    """The rows of ale.dat from NativeForecaster.ale's outputs (n_bins [F], edges [F,K+1], counts [F,K],
+    ale [F,K+1,J], local_mean and local_sd [F,K,J]): one row per field, in Dataset order, and edge k = 0..K_f, with the
+    edge in normalised input units and n the windows in the bin that ends at it (0 at k = 0); then per explained output
+    <out> (shapley_output_names) ale_<out>, the centred accumulated effect at the edge, and local_<out> and
+    local_sd_<out>, the mean and standard deviation of the bin's local effects (NaN at k = 0).  A field with fewer than
+    two distinct values (K_f = 0) has no rows."""
+    cols = {'field': [], 'edge_idx': [], 'edge': [], 'n': []}
+    for o in outputs:
+        cols.update({'ale_' + o: [], 'local_' + o: [], 'local_sd_' + o: []})
+    for f, name in enumerate(field_names):
+        kf = int(n_bins[f])
+        if kf == 0:
+            continue
+        cols['field'] += [name] * (kf + 1)
+        cols['edge_idx'] += list(range(kf + 1))
+        cols['edge'] += list(np.asarray(edges[f][:kf + 1], dtype=np.float64))
+        cols['n'] += [0] + [int(c) for c in counts[f][:kf]]
+        for j, o in enumerate(outputs):
+            cols['ale_' + o] += list(np.asarray(ale[f][:kf + 1, j], dtype=np.float64))
+            cols['local_' + o] += [np.nan] + list(np.asarray(local_mean[f][:kf, j], dtype=np.float64))
+            cols['local_sd_' + o] += [np.nan] + list(np.asarray(local_sd[f][:kf, j], dtype=np.float64))
+    return pd.DataFrame(cols)
 
 
 def quantile_name(level):

@@ -356,6 +356,10 @@ class ModelExecution(object):
             raise ValueError('--shapley_samples %d: Shapley attributions explain the forecasts of a trained model, at '
                              'prediction (--train=False), with shapley_samples >= 1 permutation samples (0 = off); '
                              'NaivePointEstimate has no model to explain' % c.shapley_samples)
+        if c.ale_bins != 0 and (c.ale_bins < 0 or c.train or 'Naive' in c.nn_type):
+            raise ValueError('--ale_bins %d: accumulated local effects explain the forecasts of a trained model, at '
+                             'prediction (--train=False), with ale_bins >= 1 quantile bins per field (0 = off); '
+                             'NaivePointEstimate has no model to explain' % c.ale_bins)
         if getattr(c, 'pred_quantiles', None) is not None:
             if not c.UQ or c.train:
                 raise ValueError('--pred_quantiles %s: predictive quantiles are those of a UQ model\'s Monte-Carlo '
@@ -482,6 +486,11 @@ class ModelExecution(object):
                                              dtype={'group': str}, float_precision='round_trip')
                                  for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
                 os.path.join(experiment_dir, 'walk_forward_importance.dat'), sep=' ', index=False)
+        if cfg.ale_bins > 0:
+            stitch_walk_forward([pd.read_csv(os.path.join(pred.model_dir, 'pred', 'ale.dat'), sep=' ',
+                                             dtype={'field': str}, float_precision='round_trip')
+                                 for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
+                os.path.join(experiment_dir, 'walk_forward_ale.dat'), sep=' ', index=False)
         if getattr(cfg, 'pred_quantiles', None) is not None:
             stitch_walk_forward([pd.read_csv(os.path.join(pred.model_dir, 'pred', 'quantiles.dat'), sep=' ',
                                              dtype={'gvkey': str}, float_precision='round_trip')
