@@ -285,8 +285,9 @@ int32_t lfmq_chain_forward_uq_mc(const lfmq_handle* stages, int32_t n_stages, co
  * v[s][b][m], and after the last launch one pass treats each (window, stage) as the Gaussian mixture
  * F(q) = (1/M) sum_m Phi((q - mu_m) / sigma_m), sigma_m^2 = v_m, M = samples, and writes (device fp32):
  *   quantiles[s] [B][n_levels]  the q with F(q) = levels[k]: bracketed by the smallest and largest component quantile
- *                               mu_m + sigma_m Phi^-1(levels[k]), refined by safeguarded Newton steps until
- *                               |F(q) - level| <= 1e-7, the bracket is narrower than 1e-6 min_m sigma_m, or 64 steps;
+ *                               mu_m + sigma_m Phi^-1(levels[k]), refined by safeguarded Newton steps on the smaller
+ *                               tail (1 - F(q) = 1 - level above the median) until |F(q) - level| <= 1e-6
+ *                               min(level, 1 - level), the bracket is narrower than 1e-6 min_m sigma_m, or 64 steps;
  *   scores[s] [B][3]            with y (host array of n_stages device pointers, laid out as lfmq_chain_loss_uq takes
  *                               the targets) and the target y[s][b, T-1, target_idx]: {crps, nll, pit} =
  *                               {E|X - y| - E|X - X'| / 2 in the closed form for Gaussian mixtures (Grimit et al.
@@ -369,13 +370,14 @@ int32_t lfmq_permutation_index(int32_t N, uint64_t seed, int32_t group, int32_t 
  * sample m at B = N; point and dense models predict with dropout off.  Outputs (device fp32):
  *   phi [N][K][G]: (1/M) sum_m f_m(copy (m, r + 1)) - f_m(copy (m, r)), r = the rank of g in o_m;
  *   f_x [N][K] = (1/M) sum_m f_m(copy (m, G)), f_bg [N][K] = (1/M) sum_m f_m(copy (m, 0)),
- * so sum_g phi = f_x - f_bg.  A window's terms are added in increasing (m, k) in fp32 without atomics and scaled by 1/M
- * at the end: the outputs do not depend on max_batch or on where launches are cut.  Accepted: what
+ * so sum_g phi = f_x - f_bg.  A window's terms are added in increasing (m, k) in fp64 without atomics and divided by M
+ * at the end, so a point model's f_x is its forward bit for bit: the outputs do not depend on max_batch or on where
+ * launches are cut.  Accepted: what
  * lfmq_chain_permutation_importance accepts.  The handles' parameters, gradient buffers (tail included) and optimizer
  * slots are left untouched.  N, G or samples < 1, a col_group value outside [0, G) or a null pointer: LFMQ_ERR_ARG.
  * `work`: caller-owned device scratch, 256-byte aligned, of the size the *_work_bytes query gives: one launch's rows
- * (per stage), the col_group copy, the orderings and ranks [samples][G], prev [N][K] and one launch's predictions (and
- * variances). */
+ * (per stage), the col_group copy, the orderings and ranks [samples][G], prev [N][K], the fp64 sums [N][K][G + 2] and
+ * one launch's predictions (and variances). */
 int32_t lfmq_chain_shapley_work_bytes(const lfmq_handle* stages, int32_t n_stages, int32_t N, int32_t G,
                                       int32_t samples, uint64_t* bytes);
 int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N,

@@ -57,10 +57,12 @@ __global__ void __launch_bounds__(kPermThreads) perm_importance_gather_kernel(
 // One thread per (window a + i, output o) of a launch of copy (m, k): v = src.p[o][i * stride + off].  k = 0 adds v
 // into f_bg; k > 0 adds v - prev into phi[w][o][order[k - 1]], the group copy k adds; k = G also adds v into f_x.
 // prev[w][o] = v.  A window's terms arrive in increasing (m, k), one launch after another, so its sums do not depend on
-// where launches are cut.
+// where launches are cut.  The sums are fp64 and v - prev is exact in fp64: a point model's f_x, M equal forwards over
+// M, is its forward bit for bit (an fp32 sum 3v times 1/3 is not v for a third of all v), and sum_g phi telescopes to
+// f_x - f_bg before the one rounding to fp32.
 __global__ void __launch_bounds__(kFoldThreads) shapley_fold_kernel(
     ShapleySrc src, int K, long stride, long off, int a, int n, int k, int G, const int32_t* __restrict__ order,
-    float* __restrict__ prev, float* __restrict__ phi, float* __restrict__ f_x, float* __restrict__ f_bg) {
+    float* __restrict__ prev, double* __restrict__ phi, double* __restrict__ f_x, double* __restrict__ f_bg) {
   const int t = blockIdx.x * kFoldThreads + threadIdx.x;
   if (t >= n * K) return;
   const int i = t / K, o = t - i * K;
@@ -73,10 +75,15 @@ __global__ void __launch_bounds__(kFoldThreads) shapley_fold_kernel(
   if (k == 0) {
     f_bg[wo] += v;
   } else {
-    phi[wo * G + order[k - 1]] += v - prev[wo];
+    phi[wo * G + order[k - 1]] += (double)v - (double)prev[wo];
     if (k == G) f_x[wo] += v;
   }
   prev[wo] = v;
+}
+
+__global__ void shapley_finish_kernel(long n, const double* __restrict__ sum, int samples, float* __restrict__ out) {
+  const long j = (long)blockIdx.x * kFoldThreads + threadIdx.x;
+  if (j < n) out[j] = (float)(sum[j] / (double)samples);
 }
 
 }  // namespace
@@ -90,9 +97,16 @@ int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems
 }
 
 int shapley_fold(cudaStream_t s, const ShapleySrc& src, int K, long stride, long off, int a, int n, int k, int G,
-                 const int32_t* order, float* prev, float* phi, float* f_x, float* f_bg) {
+                 const int32_t* order, float* prev, double* phi, double* f_x, double* f_bg) {
   shapley_fold_kernel<<<(n * K + kFoldThreads - 1) / kFoldThreads, kFoldThreads, 0, s>>>(src, K, stride, off, a, n, k,
                                                                                         G, order, prev, phi, f_x, f_bg);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+int shapley_finish(cudaStream_t s, long n, const double* sum, int samples, float* out) {
+  shapley_finish_kernel<<<(unsigned)((n + kFoldThreads - 1) / kFoldThreads), kFoldThreads, 0, s>>>(n, sum, samples,
+                                                                                                    out);
   LFMQ_LAUNCH_CHECK();
   return 0;
 }

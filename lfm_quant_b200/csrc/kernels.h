@@ -106,10 +106,12 @@ int perm_importance_gather(cudaStream_t s, const float* x, int N, long row_elems
                            const int32_t* rank, int k, uint64_t seed, int key, int rep, int a, int n, float* out);
 // shapley_fold: folds the K explained outputs of windows [a, a + n), src.p[o][i * stride + off] for output o of launch
 // row i, of coalition copy k (0..G) of one sample into the sums of lfmq_chain_shapley: f_bg at k = 0, f_x at k = G, and
-// for k > 0 the difference to the window's previous copy (prev [N][K]) into phi [N][K][G] at group order[k - 1].
+// for k > 0 the difference to the window's previous copy (prev [N][K]) into phi [N][K][G] at group order[k - 1], all
+// three sums in fp64.  shapley_finish: out[j] = (float)(sum[j] / samples) for j < n.
 struct ShapleySrc { const float* p[2 * LFMQ_MAX_STAGES]; };
 int shapley_fold(cudaStream_t s, const ShapleySrc& src, int K, long stride, long off, int a, int n, int k, int G,
-                 const int32_t* order, float* prev, float* phi, float* f_x, float* f_bg);
+                 const int32_t* order, float* prev, double* phi, double* f_x, double* f_bg);
+int shapley_finish(cudaStream_t s, long n, const double* sum, int samples, float* out);
 // Accumulated local effects (ale.cu, lfmq_chain_ale).  ale_sort_bytes: the temp storage of the segmented radix sort of
 // G segments of N (value, window) pairs.  ale_bins: the values x[i, cols[g]] sorted per feature into skey / sval, the
 // edges, counts and n_bins outputs, the sorted bin ends ends [G][K+1] and every window's bin bin_of [G][N] (0: none).

@@ -1469,14 +1469,15 @@ long row_out_of(const lfmq_handle* st) {
 }
 
 // Where a Shapley launch's outputs are folded (shapley_fold): the K value pointers with their row stride and offset,
-// the ordering of the sample being run, and the sums.
+// the ordering of the sample being run, and the fp64 sums.
 struct ShapleyFold {
   lfmq::ShapleySrc src;
   int K;
   long stride, off;
   int G;
   const int32_t* order;  // o_m of the sample being run
-  float *prev, *phi, *f_x, *f_bg;
+  float* prev;
+  double *phi, *f_x, *f_bg;
 };
 
 // The forward of one copy of x [N, row_in] in launches of at most `rows` windows, in window order.  Launch [a, a + n)
@@ -1532,6 +1533,7 @@ struct CopyWork {
   float* win[lfmq::LFMQ_MAX_STAGES];
   int32_t *cg, *onehot, *order, *rank;
   float* prev;
+  double *phi, *f_x, *f_bg;     // Shapley's fp64 sums
   float* pred[lfmq::LFMQ_MAX_STAGES];
   float* var[lfmq::LFMQ_MAX_STAGES];
 };
@@ -1557,15 +1559,19 @@ int shapley_outputs(const lfmq_handle* st, int S) {
   return st[0]->path == Path::Dense ? 1 : (st[0]->cfg.uq ? 2 * S : S);
 }
 
-// Shapley: the samples' group orderings and ranks [samples][G] each, prev [N][K], and one launch's outputs.
+// Shapley: the samples' group orderings and ranks [samples][G] each, prev [N][K], the fp64 sums of phi [N][K][G], f_x
+// and f_bg [N][K], and one launch's outputs.
 CopyWork shapley_layout(const lfmq_handle* st, int S, int rows, int N, int G, int samples, Carver& cv) {
-  const size_t row_in = row_in_of(st), row_out = row_out_of(st);
+  const size_t row_in = row_in_of(st), row_out = row_out_of(st), NK = (size_t)N * shapley_outputs(st, S);
   CopyWork w{};
   for (int i = 0; i < S; ++i) w.win[i] = cv.take<float>(rows * row_in);
   w.cg = cv.take<int32_t>(row_in);
   w.order = cv.take<int32_t>((size_t)samples * G);
   w.rank = cv.take<int32_t>((size_t)samples * G);
-  w.prev = cv.take<float>((size_t)N * shapley_outputs(st, S));
+  w.prev = cv.take<float>(NK);
+  w.phi = cv.take<double>(NK * G);
+  w.f_x = cv.take<double>(NK);
+  w.f_bg = cv.take<double>(NK);
   for (int i = 0; i < S; ++i) w.pred[i] = cv.take<float>(rows * row_out);
   if (st[0]->cfg.uq)
     for (int i = 0; i < S; ++i) w.var[i] = cv.take<float>(rows * row_out);
@@ -1707,8 +1713,8 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
   CopyWork w;
   RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return shapley_layout(stages, S, rows, N, G, M, cv); }, &w));
   cudaStream_t s = (cudaStream_t)stream;
-  ShapleyFold fold{explained_src(stages, S, w.pred, w.var), K, row_out, explained_off(stages), G, nullptr, w.prev, phi,
-                   f_x, f_bg};
+  ShapleyFold fold{explained_src(stages, S, w.pred, w.var), K, row_out, explained_off(stages), G, nullptr, w.prev,
+                   w.phi, w.f_x, w.f_bg};
   // Sample m belongs to pair p = m / 2.  An even sample orders the groups by o[q] = perm_index(G, seed, 0x40000001,
   // p, q); an odd one reverses its partner's ordering (antithetic) and keeps its donors.
   std::vector<int32_t> ord((size_t)M * G), rk((size_t)M * G);
@@ -1722,9 +1728,9 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
   LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.cg, col_group, row_in * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.order, ord.data(), ord.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   LFMQ_CUDA_CHECK(cudaMemcpyAsync(w.rank, rk.data(), rk.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  LFMQ_CUDA_CHECK(cudaMemsetAsync(phi, 0, (size_t)N * K * G * sizeof(float), s));
-  LFMQ_CUDA_CHECK(cudaMemsetAsync(f_x, 0, (size_t)N * K * sizeof(float), s));
-  LFMQ_CUDA_CHECK(cudaMemsetAsync(f_bg, 0, (size_t)N * K * sizeof(float), s));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(w.phi, 0, (size_t)N * K * G * sizeof(double), s));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(w.f_x, 0, (size_t)N * K * sizeof(double), s));
+  LFMQ_CUDA_CHECK(cudaMemsetAsync(w.f_bg, 0, (size_t)N * K * sizeof(double), s));
   const CopyForward cf{stages, S, x, N, rows, row_in, row_out, w.cg, seed, step, w.win[0], w.win[1], w.pred,
                        uq ? w.var : nullptr, false, s};
   // Copy (m, k) takes the groups ranked >= k in o_m from window d_p(i) = perm_index(N, seed, 0x40000000, p, i): k = 0
@@ -1735,10 +1741,9 @@ int32_t lfmq_chain_shapley(const lfmq_handle* stages, int32_t n_stages, const fl
     for (int k = 0; k <= G; ++k)
       RUN(cf.run(k < G ? w.rank + (size_t)m * G : nullptr, k, kShapleyDonorKey, m / 2, (int64_t)m * N, &fold));
   }
-  const float inv = 1.0f / (float)M;
-  RUN(scale_inplace(s, (long)N * K * G, phi, inv));
-  RUN(scale_inplace(s, (long)N * K, f_x, inv));
-  RUN(scale_inplace(s, (long)N * K, f_bg, inv));
+  RUN(shapley_finish(s, (long)N * K * G, w.phi, M, phi));
+  RUN(shapley_finish(s, (long)N * K, w.f_x, M, f_x));
+  RUN(shapley_finish(s, (long)N * K, w.f_bg, M, f_bg));
   return LFMQ_OK;
 }
 

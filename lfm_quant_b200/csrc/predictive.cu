@@ -12,6 +12,10 @@ namespace {
 constexpr int kGatherThreads = 256;
 constexpr int kDistWarps = 8;                 // (window, stage) problems per CTA, one warp each
 constexpr int kQuantileIters = 64;            // safeguarded Newton: each step at least bisects when Newton stalls
+// stop at |F(q) - tau| <= kQuantileRtol min(tau, 1 - tau): above the <= 4.8e-7 relative error of the fp32 erfcf terms,
+// and q is then within kQuantileRtol min(tau, 1 - tau) / f(q): for one Gaussian at most 1.25e-6 sd, and 1e-6 sd / |z|
+// in its tails
+constexpr double kQuantileRtol = 1e-6;
 constexpr float kInvSqrt2 = 0.70710678118654752f;
 constexpr float kInvSqrt2Pi = 0.39894228040143268f;
 constexpr double kLogSqrt2Pi = 0.91893853320467274;
@@ -66,17 +70,21 @@ __device__ __forceinline__ float abs_moment(float m, float var) {
   return 2.f * (var * inv) * kInvSqrt2Pi * __expf(-0.5f * z * z) + m * erff(z * kInvSqrt2);
 }
 
-// F(q) and the density f(q) of the mixture, every lane holding both: lane k evaluates components k, k + 32, ..
-__device__ __forceinline__ void mixture_cdf_pdf(const float* mu, const float* v, int M, double inv_m, float q,
-                                                double* F, double* f) {
+// The mixture's mass below q (upper = false: F(q)) or above it (upper = true: 1 - F(q)) and its density f(q), every
+// lane holding both: lane k evaluates components k, k + 32, ..  Each component's mass beyond |z|, Phi(-|z|) =
+// erfc(|z| / sqrt 2) / 2, is accurate relative to itself; the other side is 1 minus it in fp64.  So both tails keep
+// their relative accuracy: forming 1 - F from F would leave nothing of a 1e-4 upper tail below fp32's spacing at 1.
+__device__ __forceinline__ void mixture_tail_pdf(const float* mu, const float* v, int M, double inv_m, float q,
+                                                 bool upper, double* P, double* f) {
   double c = 0.0, d = 0.0;
   for (int s = threadIdx.x & 31; s < M; s += 32) {
     const float inv = rsqrtf(v[s]);
     const float z = (q - mu[s]) * inv;
-    c += (double)(0.5f * erfcf(-z * kInvSqrt2));
+    const double t = (double)(0.5f * erfcf(fabsf(z) * kInvSqrt2));
+    c += ((z < 0.f) != upper) ? t : 1.0 - t;
     d += (double)(kInvSqrt2Pi * __expf(-0.5f * z * z) * inv);
   }
-  *F = warp_sum(c) * inv_m;
+  *P = warp_sum(c) * inv_m;
   *f = warp_sum(d) * inv_m;
 }
 
@@ -126,12 +134,16 @@ __global__ void __launch_bounds__(kDistWarps * 32) dist_kernel(DistParams p) {
     }
     lo = warp_min(lo);
     hi = warp_max(hi);
+    // Above the median solve 1 - F(q) = 1 - tau: g = F - tau is formed from the smaller tail, and the stop is relative
+    // to it, so a level of 1e-4 or 0.9999 is met as closely, relative to its tail, as one of 0.5
+    const bool upper = tau > 0.5f;
+    const double t = upper ? 1.0 - (double)tau : (double)tau;
     float q = 0.5f * (lo + hi), dx = hi - lo;
     for (int it = 0; it < kQuantileIters && hi - lo > 1e-6f * min_sd; ++it) {
-      double F, f;
-      mixture_cdf_pdf(mu, v, M, inv_m, q, &F, &f);
-      const double g = F - tau;
-      if (fabs(g) <= 1e-7) break;
+      double P, f;
+      mixture_tail_pdf(mu, v, M, inv_m, q, upper, &P, &f);
+      const double g = upper ? t - P : P - t;
+      if (fabs(g) <= kQuantileRtol * t) break;
       if (g < 0.0) lo = q; else hi = q;
       // Newton from q when it lands inside the bracket and is under half the previous step, else bisection
       const float step = __fdividef((float)g, (float)f), qn = q - step;

@@ -1,6 +1,7 @@
 """fp64 reference of lfmq_chain_forward_uq_dist's distribution pass (DESIGN.md section 5g): the Gaussian mixture
 F(q) = (1/M) sum_s Phi((q - mu_s) / sigma_s) of one window's M Monte-Carlo samples (mu_s, sigma_s^2 = v_s), its
-quantiles by scipy.optimize.brentq, and the CRPS, log score and PIT of a target."""
+quantiles by scipy.optimize.brentq (or, for many windows at once, by bisection), and the CRPS, log score and PIT of a
+target."""
 import numpy as np
 from scipy import optimize, special, stats
 
@@ -34,6 +35,30 @@ def quantiles(mu, v, levels):
         lo, hi = lo - 1e-9 * (abs(lo) + 1), hi + 1e-9 * (abs(hi) + 1)
         out.append(optimize.brentq(lambda q: cdf(q, mu, v) - tau, lo, hi, xtol=1e-14, rtol=1e-15, maxiter=500))
     return np.array(out)
+
+
+def quantiles_batch(mu, v, levels, iters=200):
+    """quantiles for many windows at once: mu, v [N,M] -> q [N,Q] by bisection over every (window, level) together,
+    inside [min_s, max_s] of the component quantiles.  Above the median it solves the upper tail
+    mean_s Phi(-(q - mu_s) / sigma_s) = 1 - tau, which fp64 resolves relative to 1 - tau; below it F(q) = tau."""
+    mu, v = np.asarray(mu, dtype=np.float64), np.asarray(v, dtype=np.float64)
+    tau = np.asarray(levels, dtype=np.float64)
+    sd = np.sqrt(v)
+    comp = mu[:, None, :] + sd[:, None, :] * special.ndtri(tau)[None, :, None]       # [N,Q,M]
+    lo, hi = comp.min(axis=2), comp.max(axis=2)
+    upper = tau > 0.5
+    target = np.where(upper, 1.0 - tau, tau)[None, :]
+    sign = np.where(upper, -1.0, 1.0)[None, :, None]
+    for _ in range(iters):
+        mid = 0.5 * (lo + hi)
+        done = ~((mid > lo) & (mid < hi))                                            # adjacent doubles
+        if done.all():
+            break
+        tail = special.ndtr(sign * (mid[:, :, None] - mu[:, None, :]) / sd[:, None, :]).mean(axis=2)
+        below = np.where(upper[None, :], tail > target, tail < target)               # F(mid) < tau
+        lo = np.where(below & ~done, mid, lo)
+        hi = np.where(~below & ~done, mid, hi)
+    return 0.5 * (lo + hi)
 
 
 def abs_moment(m, var):

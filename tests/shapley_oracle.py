@@ -27,10 +27,8 @@ def coalition_copy(x, col_group, rank, k, donor):
     """Copy (m, k) of x [N,T,F] or [N,T*F]: the columns whose group ranks >= k (rank [G]) from window donor[i]."""
     N = x.shape[0]
     flat = x.reshape(N, -1)
-    out = flat.copy()
     take = np.asarray(rank)[np.asarray(col_group)] >= k
-    out[:, take] = flat[donor][:, take]
-    return out.reshape(x.shape)
+    return np.where(take[None, :], flat[donor], flat).reshape(x.shape)
 
 
 def shapley(x, col_group, G, samples, seed, outputs):
