@@ -412,6 +412,46 @@ int32_t lfmq_chain_ale_work_bytes(const lfmq_handle* stages, int32_t n_stages, i
 int32_t lfmq_chain_ale(const lfmq_handle* stages, int32_t n_stages, const float* x, int32_t N, const int32_t* cols,
                        int32_t G, int32_t K, int64_t step, int32_t* n_bins, float* edges, int32_t* counts, float* ale,
                        float* local_mean, float* local_sd, void* work, uint64_t work_bytes, void* stream);
+/* ---- training-window attributions -----------------------------------------------------------------------------------
+ * Which training windows taught the model each forecast: TracIn (Pruthi et al. 2020) at the trained checkpoint,
+ * restricted to the output head theta (OUTPUT_1, or OUTPUT_TARGET_1 and OUTPUT_VARIANCE_1), with every dropout off.
+ * The influence of training window t on output j of query window q is I_j(t, q) = -grad_theta l_t . grad_theta f^j_q,
+ * the first-order change of the forecast from one unit-rate gradient step on t alone: positive pushes it up.  l_t is
+ * the training loss of a batch holding t alone (B = 1, the window's own mask counts as denominators, no row weights;
+ * masked all-zero-target elements contribute exactly 0).  The J outputs are pred[T-1, target_idx] (J = 1) and on a uq
+ * handle also the variance (J = 2).  With a_tau the head input at step tau (the last layer's output after
+ * BatchNormalization, D = num_hidden; on a dense handle the flattened window, D = T * F, one step) and ~a = (a; 1):
+ *   I_j(t, q) = -s_jq (~a_{q,T-1} . u_jt),  u_jt = sum_tau G_j[t, tau] ~a_{t,tau}  (length D1 = D + 1)
+ * where G_j = dl_t / d(head output j at [tau, target_idx]) (the variance head's pre-softplus activation), s_0q = 1 and
+ * s_1q = sigmoid(pre_q), 0 where the 1e-6 variance floor binds.
+ * lfmq_influence_train_features: u [J][B][D1] of B training windows x, y.
+ * lfmq_influence_query_features: ~a [B][D1] and s [J][B] of B query windows.
+ * Both run a forward with every dropout off (also on a uq handle) in launches of at most max_batch rows (B is not
+ * bounded by it), with the training loss's device expressions.  Accepted: recurrent handles of precision LFMQ_PREC_FP32
+ * or LFMQ_PREC_TF32 (either cell, point or uq, forward_only or not) and dense handles; one handle, so a forecast chain
+ * is not accepted.  LFMQ_PREC_BF16 / LFMQ_PREC_BF16X3 handles, B < 1 and null pointers: LFMQ_ERR_ARG (explain a
+ * LFMQ_PREC_FP32 handle with the same parameters).  Parameters, gradients and optimizer slots are left untouched.
+ * `work`: caller-owned device scratch, 256-byte aligned, of the size lfmq_influence_features_work_bytes gives. */
+int32_t lfmq_influence_features_work_bytes(lfmq_handle h, uint64_t* bytes);
+int32_t lfmq_influence_train_features(lfmq_handle h, const float* x, const float* y, int32_t B, float* u, void* work,
+                                      uint64_t work_bytes, void* stream);
+int32_t lfmq_influence_query_features(lfmq_handle h, const float* x, int32_t B, float* a, float* s, void* work,
+                                      uint64_t work_bytes, void* stream);
+/* Per query q and output j, from a [Nq][D1], u [J][Nt][D1] and s [J][Nq] (device fp32; no handle):
+ *   pos_idx / pos_score [Nq][J][K]  the K largest positive influences, largest first
+ *   neg_idx / neg_score [Nq][J][K]  the K most negative, most negative first
+ *   total [Nq][J]                   sum_t I_j(t, q) over the whole pool
+ * Ties go to the lower training index; fewer than K influences of a sign pad the list with index -1 and score 0 (a zero
+ * influence has no sign).  The scores a . u run on sm_90a wgmma with every operand split into tf32 high and low parts
+ * (hi*hi + hi*lo + lo*hi, fp32 accumulation: about 1e-6 |a| |u| of fp64), each over its k range in a fixed order, and
+ * the top K is kept exactly inside the GEMM's epilogue, per pool slice, then merged.  total is -s (a . sum_t u_t) with
+ * the sum and the product in fp64 in a fixed order.  Two calls give the same bits, and a query's results do not depend
+ * on Nq, on the other queries or on the pool split.  1 <= K <= 64, J in {1, 2}, Nq, Nt, D1 >= 1, else LFMQ_ERR_ARG, as
+ * for null pointers.  `work`: device scratch, 256-byte aligned, of the size lfmq_influence_topk_work_bytes gives. */
+int32_t lfmq_influence_topk_work_bytes(int32_t Nq, int32_t Nt, int32_t D1, int32_t J, int32_t K, uint64_t* bytes);
+int32_t lfmq_influence_topk(const float* a, const float* u, const float* s, int32_t Nq, int32_t Nt, int32_t D1,
+                            int32_t J, int32_t K, int32_t* pos_idx, float* pos_score, int32_t* neg_idx,
+                            float* neg_score, float* total, void* work, uint64_t work_bytes, void* stream);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

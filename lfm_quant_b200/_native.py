@@ -108,6 +108,13 @@ SYMBOLS = {
     'lfmq_chain_ale_work_bytes': (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
     'lfmq_chain_ale': (C.c_int32, [_P, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P, _P,
                                     _P, _P, _P, C.c_uint64, _P]),
+    'lfmq_influence_features_work_bytes': (C.c_int32, [_P, C.POINTER(C.c_uint64)]),
+    'lfmq_influence_train_features': (C.c_int32, [_P, _P, _P, C.c_int32, _P, _P, C.c_uint64, _P]),
+    'lfmq_influence_query_features': (C.c_int32, [_P, _P, C.c_int32, _P, _P, _P, C.c_uint64, _P]),
+    'lfmq_influence_topk_work_bytes': (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                   C.POINTER(C.c_uint64)]),
+    'lfmq_influence_topk': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P,
+                                         _P, _P, _P, C.c_uint64, _P]),
     'lfmq_chain_loss': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_loss_uq': (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_backward': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),

@@ -133,6 +133,24 @@ int ale_pick(cudaStream_t s, const ShapleySrc& src, int J, long stride, long off
 // sums of the means; mean [K][J] is fp64 scratch.
 int ale_fold(cudaStream_t s, const AleSort& w, const int32_t* n_bins, int g, int N, int K, int J, const float* d,
              double* mean, float* ale, float* local_mean, float* local_sd);
+// Training-window attributions (influence.cu, lfmq_influence_*).  influence_grad: u [J][ldu][D + 1] rows [r0, r0 + n)
+// from the head inputs a [n][Ta][D] and the launch's pred / var / pre / y [n][Ta][O] (mode 0 point, 1 uq, 2 dense with
+// Ta = 1).  influence_query: aout [..][D + 1] and s [J][lds] rows from r0.
+int influence_grad(cudaStream_t s, int n, int mode, int Ta, int D, int O, int tidx, float p1, float p2, int huber,
+                   float delta, const float* a, const float* pred, const float* var, const float* pre, const float* y,
+                   long r0, long ldu, float* u);
+int influence_query(cudaStream_t s, int n, int Ta, int D, int O, int tidx, int uq, const float* a, const float* pre,
+                    long r0, long lds, float* aout, float* sout);
+// The pool split of one influence_topk call (a function of the shapes alone) and the sizes of its scratch.
+struct InfluencePlan {
+  int P, tiles_per_slice, n_sum;
+  size_t list_elems, part_elems, usum_elems;
+};
+constexpr int LFMQ_INFLUENCE_MAX_K = 64;
+InfluencePlan influence_plan(int Nq, int Nt, int D1, int J, int K);
+int influence_topk(cudaStream_t s, const InfluencePlan& pl, const float* a, const float* u, const float* sc, int Nq,
+                   int Nt, int D1, int J, int K, float* lscore, int* lidx, double* part, double* usum, int* pos_idx,
+                   float* pos_score, int* neg_idx, float* neg_score, float* total);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

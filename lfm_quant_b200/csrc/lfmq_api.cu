@@ -338,8 +338,10 @@ int gemm(lfmq_handle h, cudaStream_t s, int M, int N, int K, const float* A, lon
 
 // fp32 SIMT (or tf32 GEMM) forward of all layers; fills layers[l].{h,c,y,(gates)} and `preds`.
 // uq handles also fill `var` [B,T,O] (and keep the variance head's pre-activation when a backward pass can follow).
+// dropout_off: every dropout off, also on a uq handle (training-window attributions only; no entry point of the
+// model's own forward sets it).
 int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t step, float* preds, float* var,
-                 cudaStream_t s) {
+                 cudaStream_t s, bool dropout_off = false) {
   const lfmq_config& c = h->cfg;
   const int H = c.num_hidden, T = c.seq_len, O = c.n_outputs, L = c.num_layers;
   const float* P = h->params;
@@ -350,7 +352,7 @@ int forward_fp32(lfmq_handle h, const float* x, int B, int64_t row0, int64_t ste
     const float* in = (l == 0) ? x : h->layers[l - 1].y;
     const int I = o.I;
     const float* rmask = nullptr;
-    const bool stochastic = c.train || c.uq;       // rnn_uq_range_estimate.py:86,88: training=True is a literal there
+    const bool stochastic = (c.train || c.uq) && !dropout_off;   // rnn_uq_range_estimate.py:86,88: training=True
     if (stochastic && c.recurrent_dropout > 0.f) {
       RUN(gen_row_mask(s, B, H, dropout_key(c.seed, h->tc.stream_base + 2 * l + 1, step, c.recurrent_dropout), row0,
                        lb.rmask));
@@ -1850,6 +1852,149 @@ int32_t lfmq_chain_ale(const lfmq_handle* stages, int32_t n_stages, const float*
     RUN(ale_fold(s, w.sort, n_bins, g, N, K, J, w.d, w.mean, ale, local_mean, local_sd));
   }
   return LFMQ_OK;
+}
+
+// ---- training-window attributions (lfmq_influence_*) ----------------------------------------------------------------
+namespace {
+// Recurrent handles on the fp32 step (LFMQ_PREC_FP32 / LFMQ_PREC_TF32, any cell, point or uq) and dense handles.
+int influence_check(lfmq_handle h, int32_t B, const char* fn) {
+  if (!h || B < 1) {
+    LFMQ_SET_ERR("%s: need a handle and B >= 1 (got B = %d)", fn, B);
+    return LFMQ_ERR_ARG;
+  }
+  if (h->path != Path::Fp32 && h->path != Path::Dense) {
+    LFMQ_SET_ERR("%s: precision %d is not explained directly; explain a LFMQ_PREC_FP32 handle with the same parameters",
+                 fn, h->cfg.precision);
+    return LFMQ_ERR_ARG;
+  }
+  return 0;
+}
+
+// Caller scratch of the feature passes: a dense launch's predictions [rows][O], a uq launch's variance-head
+// pre-activations [rows][T][O].
+struct InfluenceWork {
+  float *pred, *pre;
+};
+InfluenceWork influence_layout(lfmq_handle h, Carver& cv) {
+  const lfmq_config& c = h->cfg;
+  const size_t rows = (size_t)c.max_batch;
+  InfluenceWork w{};
+  if (h->path == Path::Dense) w.pred = cv.take<float>(rows * c.n_outputs);
+  if (c.uq) w.pre = cv.take<float>(rows * c.seq_len * c.n_outputs);
+  return w;
+}
+
+// u != nullptr: the training features u [J][B][D+1]; else the query features aout [B][D+1] and sout [J][B].  Launches of
+// at most max_batch rows, each a forward with every dropout off.
+int influence_features(lfmq_handle h, const float* x, const float* y, int B, float* u, float* aout, float* sout,
+                       const InfluenceWork& w, cudaStream_t s) {
+  const lfmq_config& c = h->cfg;
+  const int T = c.seq_len, F = c.n_inputs, O = c.n_outputs, H = c.num_hidden;
+  const float* P = h->params;
+  for (int r0 = 0; r0 < B; r0 += c.max_batch) {
+    const int n = std::min(c.max_batch, B - r0);
+    const float* xr = x + (size_t)r0 * T * F;
+    if (h->path == Path::Dense) {
+      RUN(dense_forward(s, xr, n, T * F, O, P + h->pl.oWo, P + h->pl.obo, w.pred));
+      if (u)
+        RUN(influence_grad(s, n, 2, 1, T * F, O, c.target_idx, c.target_lambda, 0.f, h->huber, h->huber_delta, xr,
+                           w.pred, nullptr, nullptr, y + (size_t)r0 * O, r0, B, u));
+      else
+        RUN(influence_query(s, n, 1, T * F, O, c.target_idx, 0, xr, nullptr, r0, B, aout, sout));
+      continue;
+    }
+    RUN(forward_fp32(h, xr, n, 0, 0, h->preds, h->var, s, /*dropout_off=*/true));
+    const float* a = h->layers[c.num_layers - 1].y;
+    if (c.uq) {      // the variance head's pre-activation, by the forward's own product
+      RUN(gemm(h, s, n * T, O, H, a, H, 1, P + h->pl.oWv, O, 1, w.pre, O, 0.f, nullptr, 0));
+      RUN(add_bias_rows(s, (long)n * T, O, w.pre, P + h->pl.obv));
+    }
+    if (u)
+      RUN(influence_grad(s, n, c.uq ? 1 : 0, T, H, O, c.target_idx, c.target_lambda, c.rnn_lambda, 0, 1.f, a, h->preds,
+                         h->var, w.pre, y + (size_t)r0 * T * O, r0, B, u));
+    else
+      RUN(influence_query(s, n, T, H, O, c.target_idx, c.uq, a, w.pre, r0, B, aout, sout));
+  }
+  return 0;
+}
+
+struct TopkWork {
+  float* lscore;
+  int32_t* lidx;
+  double *part, *usum;
+};
+TopkWork topk_layout(const lfmq::InfluencePlan& pl, Carver& cv) {
+  TopkWork w{};
+  w.lscore = cv.take<float>(pl.list_elems);
+  w.lidx = cv.take<int32_t>(pl.list_elems);
+  w.part = cv.take<double>(pl.part_elems);
+  w.usum = cv.take<double>(pl.usum_elems);
+  return w;
+}
+
+int topk_check(int32_t Nq, int32_t Nt, int32_t D1, int32_t J, int32_t K, const char* fn) {
+  if (Nq < 1 || Nt < 1 || D1 < 1 || J < 1 || J > 2 || K < 1 || K > lfmq::LFMQ_INFLUENCE_MAX_K) {
+    LFMQ_SET_ERR("%s: need Nq, Nt, D1 >= 1, J in {1, 2} and 1 <= K <= %d (got %d, %d, %d, %d, %d)", fn,
+                 lfmq::LFMQ_INFLUENCE_MAX_K, Nq, Nt, D1, J, K);
+    return LFMQ_ERR_ARG;
+  }
+  return 0;
+}
+}  // namespace
+
+int32_t lfmq_influence_features_work_bytes(lfmq_handle h, uint64_t* bytes) {
+  const char* fn = "lfmq_influence_features_work_bytes";
+  RUN(influence_check(h, 1, fn));
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return influence_layout(h, cv); });
+}
+
+int32_t lfmq_influence_train_features(lfmq_handle h, const float* x, const float* y, int32_t B, float* u, void* work,
+                                      uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_influence_train_features";
+  RUN(influence_check(h, B, fn));
+  if (!x || !y || !u) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  InfluenceWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return influence_layout(h, cv); }, &w));
+  return influence_features(h, x, y, B, u, nullptr, nullptr, w, (cudaStream_t)stream);
+}
+
+int32_t lfmq_influence_query_features(lfmq_handle h, const float* x, int32_t B, float* a, float* s, void* work,
+                                      uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_influence_query_features";
+  RUN(influence_check(h, B, fn));
+  if (!x || !a || !s) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  InfluenceWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return influence_layout(h, cv); }, &w));
+  return influence_features(h, x, nullptr, B, nullptr, a, s, w, (cudaStream_t)stream);
+}
+
+int32_t lfmq_influence_topk_work_bytes(int32_t Nq, int32_t Nt, int32_t D1, int32_t J, int32_t K, uint64_t* bytes) {
+  const char* fn = "lfmq_influence_topk_work_bytes";
+  RUN(topk_check(Nq, Nt, D1, J, K, fn));
+  const lfmq::InfluencePlan pl = lfmq::influence_plan(Nq, Nt, D1, J, K);
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return topk_layout(pl, cv); });
+}
+
+int32_t lfmq_influence_topk(const float* a, const float* u, const float* s, int32_t Nq, int32_t Nt, int32_t D1,
+                            int32_t J, int32_t K, int32_t* pos_idx, float* pos_score, int32_t* neg_idx,
+                            float* neg_score, float* total, void* work, uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_influence_topk";
+  RUN(topk_check(Nq, Nt, D1, J, K, fn));
+  if (!a || !u || !s || !pos_idx || !pos_score || !neg_idx || !neg_score || !total) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  const lfmq::InfluencePlan pl = lfmq::influence_plan(Nq, Nt, D1, J, K);
+  TopkWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return topk_layout(pl, cv); }, &w));
+  return lfmq::influence_topk((cudaStream_t)stream, pl, a, u, s, Nq, Nt, D1, J, K, w.lscore, w.lidx, w.part, w.usum,
+                              pos_idx, pos_score, neg_idx, neg_score, total);
 }
 
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,

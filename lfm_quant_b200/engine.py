@@ -37,6 +37,35 @@ def _scratch(owner, key, work_bytes, *args):
     return bufs[key]
 
 
+class _TopkScratch(object):
+    """Keeps influence_topk's scratch between calls without an engine."""
+
+    def __init__(self, device):
+        self.device = device
+
+
+def influence_topk(a, u, s, k, owner=None):
+    """lfmq_influence_topk: for the query features a [Nq,D1], s [J,Nq] and the pool's training features u [J,Nt,D1] (all
+    device fp32), the device tensors (pos_idx, pos_score, neg_idx, neg_score) [Nq,J,K] -- the K training windows with the
+    largest positive and the most negative influences, index -1 and score 0 where fewer have that sign -- and total
+    [Nq,J], the summed influence of the whole pool.  `owner` (an engine) keeps the scratch between calls."""
+    a, u, s = a.contiguous(), u.contiguous(), s.contiguous()
+    J, Nt, D1 = u.shape
+    Nq, K = a.shape[0], int(k)
+    assert a.shape == (Nq, D1) and s.shape == (J, Nq), (tuple(a.shape), tuple(u.shape), tuple(s.shape))
+    lib = N.load()
+    work = _scratch(owner if owner is not None else _TopkScratch(a.device), 'influence_topk',
+                    lib.lfmq_influence_topk_work_bytes, Nq, Nt, D1, J, K)
+    pos_idx = torch.empty(Nq, J, K, dtype=torch.int32, device=a.device)
+    neg_idx = torch.empty_like(pos_idx)
+    pos_score = torch.empty(Nq, J, K, dtype=torch.float32, device=a.device)
+    neg_score = torch.empty_like(pos_score)
+    total = torch.empty(Nq, J, dtype=torch.float32, device=a.device)
+    N.check(lib.lfmq_influence_topk(_ptr(a), _ptr(u), _ptr(s), Nq, Nt, D1, J, K, _ptr(pos_idx), _ptr(pos_score),
+                                    _ptr(neg_idx), _ptr(neg_score), _ptr(total), _ptr(work), work.numel(), _stream()))
+    return pos_idx, pos_score, neg_idx, neg_score, total
+
+
 class _HandleEngine(object):
     """What every native handle offers whatever its model: parameter specs and views, weights in Keras order, the
     device share, the optimizer apply, the mask count, un-scaling and profiling."""
@@ -128,6 +157,39 @@ class _HandleEngine(object):
         assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous(), 'x must be a contiguous CUDA fp32 tensor'
         assert x.dim() == 3 and x.shape[1] == self.T and x.shape[2] == self.F, tuple(x.shape)
         return x.shape[0]
+
+    def _influence_dims(self):
+        """(D, J) of the training-window attributions: the head input's width (num_hidden, or T * F on a dense handle)
+        and the explained outputs (2 on a uq handle)."""
+        return (self.T * self.F if isinstance(self, DenseEngine) else self.H), (2 if self.uq else 1)
+
+    def influence_features(self, x, y=None):
+        """The features of the training-window attributions (lfmq_influence_*_features, DESIGN.md section 5i), with every
+        dropout off: with targets y, the training features u [J,B,D+1]; without, the query features (a [B,D+1],
+        s [J,B]).  fp32 / tf32 and dense engines; B is not bounded by max_batch."""
+        B = self._check_x(x)
+        D, J = self._influence_dims()
+        work = _scratch(self, 'influence', self.lib.lfmq_influence_features_work_bytes, self.handle)
+        if y is not None:
+            y = y.contiguous()
+            assert y.is_cuda and y.dtype == torch.float32 and y.shape[0] == B
+            u = torch.empty(J, B, D + 1, dtype=torch.float32, device=x.device)
+            N.check(self.lib.lfmq_influence_train_features(self.handle, _ptr(x), _ptr(y), B, _ptr(u), _ptr(work),
+                                                           work.numel(), _stream()))
+            return u
+        a = torch.empty(B, D + 1, dtype=torch.float32, device=x.device)
+        s = torch.empty(J, B, dtype=torch.float32, device=x.device)
+        N.check(self.lib.lfmq_influence_query_features(self.handle, _ptr(x), B, _ptr(a), _ptr(s), _ptr(work),
+                                                       work.numel(), _stream()))
+        return a, s
+
+    def influence(self, pool, queries, k):
+        """Training-window attributions of the query windows: pool = [(x, y)] device batches of training windows, whose
+        rows are numbered on in order; queries [N,T,F].  Returns influence_topk's tensors for the K = `k` windows that
+        push each forecast up and down the most."""
+        u = torch.cat([self.influence_features(x, y) for x, y in pool], dim=1)
+        a, s = self.influence_features(queries)
+        return influence_topk(a, u, s, k, owner=self)
 
     def unscale(self, arr, scale, center, log_squasher):
         """Train._unscale_preds (train.py:420-432) on the device: arr [..., O] fp32, scale / center fp64 CUDA tensors."""

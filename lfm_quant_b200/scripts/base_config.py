@@ -121,6 +121,10 @@ SCHEMA = [
     ('ale_bins', _INT, 0, 'Quantile bins per input field for accumulated local effects at prediction; more than 0 '
                           'also writes pred/ale.dat: in which direction and with what shape the forecast (and a UQ '
                           'model\'s variance) responds to each input field\'s latest value'),
+    ('influence_top_k', _INT, 0, 'Training windows listed per forecast at prediction (1 to 64); more than 0 also '
+                                 'writes pred/influence.npz: for every predicted window the K windows of the training '
+                                 'split whose gradient step pushes its forecast (and a UQ model\'s variance) up the most '
+                                 'and the K that push it down the most, with the summed influence of the whole split'),
     ('pred_quantiles', _STRING, None, "'-'-separated levels in (0, 1), e.g. 0.05-0.25-0.5-0.75-0.95, at UQ prediction; "
                                       'writes pred/quantiles.dat (the quantiles of each window\'s Monte-Carlo dropout '
                                       'mixture, with its CRPS, log score and PIT) and pred/calibration.dat; unset = off'),

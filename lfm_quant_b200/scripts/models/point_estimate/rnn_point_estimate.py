@@ -254,6 +254,27 @@ class NativeForecaster(object):
             raise ValueError('attribute: steps must be >= 1 (got %r)' % (steps,))
         return self._ig_rows_engine(int(steps)).integrated_gradients(_to_device(self.engine, inp), int(steps))
 
+    def influence(self, pool_batches, query_windows, k):
+        """Training-window attributions (_HandleEngine.influence, DESIGN.md section 5i): for every query window the K =
+        `k` training windows of pool_batches ([(inp, targets)] device batches, numbered on in order) that push its
+        norm_preds_1 (and a UQ model's norm_variance_1) up and down the most, and the summed influence of the whole
+        pool, as the device tensors (pos_idx, pos_score, neg_idx, neg_score) [N,J,K] and total [N,J].  forecast_steps = 1
+        only.  fp32, tf32 and linear models are explained through their own handle; bf16 and bf16x3 models through an
+        fp32 handle with the same parameters (their forecasts may differ from it by that precision's rounding)."""
+        if self.config.forecast_steps != 1:
+            raise ValueError('influence explains models with forecast_steps = 1 (got %d)' % self.config.forecast_steps)
+        eng = self.engine.stages[0]
+        if getattr(eng, 'precision', 'fp32') not in ('fp32', 'tf32'):
+            eng = self._side_engine('influence', self.config.batch_size, self._new_influence_engine).stages[0]
+        return eng.influence([(_to_device(eng, x), y.contiguous()) for x, y in pool_batches],
+                             _to_device(eng, query_windows), int(k))
+
+    def _new_influence_engine(self, rows):
+        from ....engine import ForecastChainEngine, ForecasterEngine
+        kw = {k: v for k, v in self._engine_kw.items() if k not in ('forecast_steps', 'weights')}
+        kw.update(max_batch=rows, train=False, forward_only=True, device=self.engine.device, precision='fp32')
+        return ForecastChainEngine(stages=[ForecasterEngine(**kw)])
+
     def _ig_rows_engine(self, steps):
         """The engine attribute runs on: a trainable-mode handle with train = 0 (dropout off) of the model's stage,
         tf32 for a tf32 model and fp32 otherwise, with max_batch = min(steps * batch_size, IG_ROWS).  Created at the first

@@ -91,7 +91,7 @@ class Predict(object):
                     ig[key].append(t.cpu().numpy())
             if self.config.perm_importance > 0:
                 held_out.append((inp_dev, target_dev))
-            if self.config.shapley_samples > 0 or self.config.ale_bins > 0:
+            if self.config.shapley_samples > 0 or self.config.ale_bins > 0 or self._influence_k() > 0:
                 windows.append(inp_dev)
         if self.config.ig_steps > 0:
             self._write_attributions(outputs, ig)
@@ -101,6 +101,8 @@ class Predict(object):
             self._write_shapley(outputs, windows)
         if self.config.ale_bins > 0:
             self._write_ale(windows)
+        if self._influence_k() > 0:
+            self._write_influence(outputs, windows)
 
         single_outputs = ['date', 'gvkey', 'seq_norm'] + [x for x in outputs.keys() if 'inp_t' in x]
         for key in single_outputs:
@@ -219,6 +221,31 @@ class Predict(object):
                   shapley_output_names(self.config.forecast_steps, self.config.UQ), *out).to_csv(
             os.path.join(self.pred_dir, 'ale.dat'), sep=' ', index=False)
 
+    def _influence_k(self):
+        return int(getattr(self.config, 'influence_top_k', 0))
+
+    def _write_influence(self, outputs, windows):
+        """<model_dir>/pred/influence.npz (--influence_top_k K): for every predicted window, known targets or not, the K
+        windows of the training split that push its forecast up and down the most (NativeForecaster.influence).  The
+        pool is the training split a --train=True run with this run's flags draws, with this model's scales.dat; in a
+        walk-forward run the origin's own (pool_dates).  write_influence gives the layout."""
+        import copy
+        import torch
+        cfg = copy.deepcopy(self.config)
+        cfg.train = True
+        if getattr(self.config, 'pool_dates', None):
+            cfg.start_date, cfg.end_date = self.config.pool_dates
+        pool = type(self.dataset)(cfg)
+        pool.generate_dataset()
+        batches = [pool.get_batch(*items) for items in pool.train_set.batch(batch_size=self.config.batch_size)]
+        meta = np.concatenate([m for _, _, m in batches])
+        tgt = torch.cat([(y if y.dim() == 2 else y[:, -1]) for _, y, _ in batches])[:, self.target_index]
+        res = self.model.influence([(x, y) for x, y, _ in batches], torch.cat(windows), self._influence_k())
+        write_influence(os.path.join(self.pred_dir, 'influence.npz'), np.vstack(outputs['date']).flatten(),
+                        np.vstack(outputs['gvkey']).flatten(),
+                        shapley_output_names(1, self.config.UQ), meta[:, 0].astype('int32'), meta[:, 1],
+                        tgt.cpu().numpy(), *[t.cpu().numpy() for t in res])
+
     def _flat(self):
         """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""
         return 'MLP' in self.config.nn_type or 'Naive' in self.config.nn_type
@@ -277,6 +304,20 @@ def write_shapley(path, date, gvkey, field_names, outputs, phi_field, phi_quarte
              outputs=np.array(list(outputs)), phi_field=np.asarray(phi_field, dtype=np.float32),
              phi_quarter=np.asarray(phi_quarter, dtype=np.float32), f_x=np.asarray(f_x, dtype=np.float32),
              f_bg=np.asarray(f_bg, dtype=np.float32))
+
+
+def write_influence(path, date, gvkey, outputs, train_date, train_gvkey, train_target, pos_idx, pos_score, neg_idx,
+                    neg_score, total):
+    """influence.npz: date [N], gvkey [N] (preds.dat row order), outputs [J] (shapley_output_names), train_date [Nt]
+    (the last input date of each training window), train_gvkey [Nt], train_target [Nt] (its normalised target of the
+    target field at the last step), pos_idx / pos_score / neg_idx / neg_score [N,J,K] (indices into the train_* arrays,
+    -1 with score 0 where fewer windows have that sign) and total [N,J], the summed influence of the whole pool."""
+    np.savez(path, date=np.asarray(date, dtype=np.int32), gvkey=np.asarray(gvkey, dtype=str),
+             outputs=np.asarray(outputs, dtype=str), train_date=np.asarray(train_date, dtype=np.int32),
+             train_gvkey=np.asarray(train_gvkey, dtype=str), train_target=np.asarray(train_target, dtype=np.float32),
+             pos_idx=np.asarray(pos_idx, dtype=np.int32), pos_score=np.asarray(pos_score, dtype=np.float32),
+             neg_idx=np.asarray(neg_idx, dtype=np.int32), neg_score=np.asarray(neg_score, dtype=np.float32),
+             total=np.asarray(total, dtype=np.float32))
 
 
 def ale_table(field_names, outputs, n_bins, edges, counts, ale, local_mean, local_sd):

@@ -115,6 +115,8 @@ def origin_configs(config):
         pred.train = False
         pred.start_date = add_months(origin, 1)
         pred.end_date = min(add_months(origin, config.stride), config.end_date)
+        if getattr(config, 'influence_top_k', 0) > 0:     # the origin's own training split is the attribution pool
+            pred.pool_dates = (train.start_date, train.end_date)
         out.append((origin, train, pred))
     return experiment_dir, out
 
@@ -360,6 +362,17 @@ class ModelExecution(object):
             raise ValueError('--ale_bins %d: accumulated local effects explain the forecasts of a trained model, at '
                              'prediction (--train=False), with ale_bins >= 1 quantile bins per field (0 = off); '
                              'NaivePointEstimate has no model to explain' % c.ale_bins)
+        if getattr(c, 'influence_top_k', 0) != 0:
+            bad = ['influence_top_k must be in [1, 64]' if not 0 < c.influence_top_k <= 64 else None,
+                   'it explains a trained model at prediction (--train=False)' if c.train else None,
+                   'NaivePointEstimate has no model to explain' if 'Naive' in c.nn_type else None,
+                   'it needs forecast_steps = 1' if c.forecast_steps != 1 else None,
+                   'it explains one model, not an ensemble (num_procs = 1)' if getattr(c, 'num_procs', 1) > 1 else None]
+            bad = [b for b in bad if b]
+            if bad:
+                raise ValueError('--influence_top_k %d: training-window attributions list, for every forecast, the '
+                                 'training windows that push it up and down the most; %s' % (c.influence_top_k,
+                                                                                              '; '.join(bad)))
         if getattr(c, 'pred_quantiles', None) is not None:
             if not c.UQ or c.train:
                 raise ValueError('--pred_quantiles %s: predictive quantiles are those of a UQ model\'s Monte-Carlo '
