@@ -452,6 +452,54 @@ int32_t lfmq_influence_topk_work_bytes(int32_t Nq, int32_t Nt, int32_t D1, int32
 int32_t lfmq_influence_topk(const float* a, const float* u, const float* s, int32_t Nq, int32_t Nt, int32_t D1,
                             int32_t J, int32_t K, int32_t* pos_idx, float* pos_score, int32_t* neg_idx,
                             float* neg_score, float* total, void* work, uint64_t work_bytes, void* stream);
+/* ---- nearest pool rows ----------------------------------------------------------------------------------------------
+ * The K rows of the pool b [Nt][D1] nearest to each query a [Nq][D1] in Euclidean distance (device fp32; no handle):
+ *   idx [Nq][K]  pool rows, nearest first, ties to the lower index; -1 past Nt
+ *   d2 [Nq][K]   |a - b|^2, summed from the difference in fp64 and rounded to fp32; +inf past Nt
+ *   mean [Nq]    with value [Nt]: the mean of value over the listed rows, summed in rank order in fp64
+ * It is lfmq_influence_topk's kernel in a second mode: the same 3xTF32 wgmma product a.b, scored 2 a.b - |b|^2 (|b|^2
+ * summed in fp64 in a fixed order and rounded to fp32), with one list of the largest scores kept in the epilogue.  That
+ * score shortlists K + 16 rows per query; their exact fp64 distances then pick and order the K (the score alone
+ * cannot resolve a small distance next to large norms: its fp32 accumulation errs by about 1e-5 (|a|^2 + |b|^2) at
+ * D1 ~ 1500).  A row missing from the result is at most the score's error nearer than the K-th listed one; two calls
+ * give the same bits, and a query's results do not depend on Nq, on the other queries or on the pool split.
+ * 1 <= K <= 64, Nq, Nt, D1 >= 1, else LFMQ_ERR_ARG, as for null pointers (value and mean are both given or both null).
+ * `work`: device scratch, 256-byte aligned, of the size lfmq_nearest_topk_work_bytes gives. */
+int32_t lfmq_nearest_topk_work_bytes(int32_t Nq, int32_t Nt, int32_t D1, int32_t K, uint64_t* bytes);
+int32_t lfmq_nearest_topk(const float* a, const float* b, const float* value, int32_t Nq, int32_t Nt, int32_t D1,
+                          int32_t K, int32_t* idx, float* d2, float* mean, void* work, uint64_t work_bytes,
+                          void* stream);
+/* ---- split-conformal prediction intervals ---------------------------------------------------------------------------
+ * DESIGN.md section 5j.  Arrays are device fp32 [S][N] (S forecast steps, N windows; no handle), so any model, the
+ * naive forecast included, uses the same calls.  The nonconformity score of a window with a finite target y is
+ *   r = |y - pred| / scale        (scale optional: 1 when null; it must be > 0)
+ * in IEEE single precision, subtraction and division each rounded once: the bits NumPy's float32 arithmetic gives.
+ * r is NaN where y is not finite.  scale is sigma for a UQ forecast, d(x) + beta for the normalised kNN score, or null.
+ * lfmq_conformal_scores: r [S][N].
+ * lfmq_conformal_calibrate: of the calibration windows [S][Nc] and the host fp64 levels l_1 < .. < l_Q in (0, 1),
+ * Q <= 32:
+ *   n_valid [S]       the windows of step s with a score (finite target)
+ *   sorted [S][Nc]    step s's scores ascending, NaN after the n_valid[s] scores (one radix sort of every step)
+ *   qhat [S][Q]       the ceil((n + 1) l)-th smallest score (rank in fp64), +inf when that rank exceeds n = n_valid[s]
+ * lfmq_conformal_apply: of the query windows [S][N] (y optional), with calibrate's outputs:
+ *   lower / upper [S][N][Q]  pred -/+ qhat * scale (product and sum each rounded once; +-inf where qhat is +inf)
+ *   pvalue [S][N]            (1 + #{i : r_i >= r}) / (n + 1) by binary search in sorted; NaN where y is null or not
+ *                            finite
+ * S, N, Nc >= 1 with S * N and S * Nc below 2^31, levels as above, and null pointers (other than y and scale):
+ * LFMQ_ERR_ARG.  The results do not depend on the order of the windows.  `work`: device scratch, 256-byte aligned, of
+ * the size the call's *_work_bytes gives (0 bytes for scores and apply). */
+int32_t lfmq_conformal_scores_work_bytes(int32_t S, int32_t N, uint64_t* bytes);
+int32_t lfmq_conformal_scores(const float* pred, const float* y, const float* scale, int32_t S, int32_t N, float* r,
+                              void* work, uint64_t work_bytes, void* stream);
+int32_t lfmq_conformal_calibrate_work_bytes(int32_t S, int32_t Nc, uint64_t* bytes);
+int32_t lfmq_conformal_calibrate(const float* pred, const float* y, const float* scale, int32_t S, int32_t Nc,
+                                 const double* levels, int32_t Q, int32_t* n_valid, float* sorted, float* qhat,
+                                 void* work, uint64_t work_bytes, void* stream);
+int32_t lfmq_conformal_apply_work_bytes(int32_t S, int32_t N, int32_t Nc, int32_t Q, uint64_t* bytes);
+int32_t lfmq_conformal_apply(const float* pred, const float* y, const float* scale, int32_t S, int32_t N,
+                             const float* sorted, const int32_t* n_valid, const float* qhat, int32_t Nc, int32_t Q,
+                             float* lower, float* upper, float* pvalue, void* work, uint64_t work_bytes,
+                             void* stream);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

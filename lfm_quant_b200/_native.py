@@ -115,7 +115,19 @@ SYMBOLS = {
                                                    C.POINTER(C.c_uint64)]),
     'lfmq_influence_topk': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P,
                                          _P, _P, _P, C.c_uint64, _P]),
-    'lfmq_chain_loss': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P]),
+    'lfmq_nearest_topk_work_bytes': (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
+    'lfmq_nearest_topk': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P,
+                                       C.c_uint64, _P]),
+    'lfmq_conformal_scores_work_bytes': (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
+    'lfmq_conformal_scores': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P, C.c_uint64, _P]),
+    'lfmq_conformal_calibrate_work_bytes': (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
+    'lfmq_conformal_calibrate': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P,
+                                              C.c_uint64, _P]),
+    'lfmq_conformal_apply_work_bytes': (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                    C.POINTER(C.c_uint64)]),
+    'lfmq_conformal_apply': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, C.c_int32, _P, _P,
+                                          _P, _P, C.c_uint64, _P]),
+    'lfmq_chain_loss':(C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_loss_uq': (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_backward': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),
     'lfmq_chain_apply': (C.c_int32, [_P, C.c_int32, C.c_float, C.c_int64, _P]),

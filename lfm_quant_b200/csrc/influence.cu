@@ -19,6 +19,14 @@
 // appends.  influence_merge merges the slices' lists in slice order.
 //
 // total = -s_jq (a_q . sum_t u_jt): fixed blocks of pool rows summed in fp64, the blocks in order, one warp per query.
+//
+// lfmq_nearest_topk is the same kernel in its second mode (kNearest): the pool is b [Nt][D1], J = 1, and the score of
+// pool row t is 2 (a . b_t) - |b_t|^2, with |b_t|^2 an fp64 sum in a fixed order rounded to fp32 and passed in S.  It
+// keeps one list, of the largest scores whatever their sign (the nearest rows), in the sign-0 slot; its threshold is
+// -inf until the list is full.  The score only shortlists: for a query near a pool row it is |a|^2 - d^2, a difference
+// of large numbers, and the fp32 accumulation of the product errs by about 1e-5 of |a|^2 + |b|^2 at D1 ~ 1500, far
+// more than a small d^2.  So the GEMM keeps Kc = nearest_candidates(K) = K + 16 candidates, and nearest_finish merges the
+// slices, recomputes each candidate's distance exactly from the difference a - b_t in fp64, and keeps the K nearest.
 #include <algorithm>
 #include <atomic>
 
@@ -188,7 +196,11 @@ __device__ float merge_list(float* __restrict__ ls, int* __restrict__ li, int* l
   return L == K ? ls[K - 1] : 0.f;
 }
 
-// grid (query tiles, slices, J).  lists: score [J][P][Nq][2][K] and index alike, the slice's running lists.
+constexpr int kDot = 0, kNearest = 1;
+
+// grid (query tiles, slices, J).  lists: score [J][P][Nq][2][K] and index alike, the slice's running lists.  MODE kDot:
+// S [J][Nq] the s_jq; kNearest: S [Nt] the pool rows' squared norms.
+template <int MODE>
 __global__ void __launch_bounds__(NT, 1) influence_topk_kernel(const float* __restrict__ A, const float* __restrict__ U,
                                                                const float* __restrict__ S, int Nq, int Nt, int D1,
                                                                int K, int tiles_per_slice, float* __restrict__ lscore,
@@ -216,17 +228,18 @@ __global__ void __launch_bounds__(NT, 1) influence_topk_kernel(const float* __re
   const long oq = q0 + orow;
   float* my_ls = lscore + ((((long)j * P + p) * Nq + oq) * 2 + osgn) * K;
   int* my_li = lidx + ((((long)j * P + p) * Nq + oq) * 2 + osgn) * K;
-  thr[orow * 2 + osgn] = 0.f;
+  thr[orow * 2 + osgn] = MODE == kNearest ? -INFINITY : 0.f;
   ccnt[orow * 2 + osgn] = 0;
   lcnt[orow * 2 + osgn] = 0;
 
   const int w = (tid >> 5) & 3, l = tid & 31;
   const int rl0 = 64 * wg + 16 * w + (l >> 2);      // rows rl0 and rl0 + 8 of the CTA tile
-  float srow[2];
-  for (int h = 0; h < 2; ++h) {
-    const long q = q0 + rl0 + 8 * h;
-    srow[h] = q < Nq ? S[(long)j * Nq + q] : 0.f;
-  }
+  float srow[2] = {0.f, 0.f};
+  if constexpr (MODE == kDot)
+    for (int h = 0; h < 2; ++h) {
+      const long q = q0 + rl0 + 8 * h;
+      srow[h] = q < Nq ? S[(long)j * Nq + q] : 0.f;
+    }
 
   float acc[64];
   float va[PER_T], vb[PER_T];
@@ -286,6 +299,17 @@ __global__ void __launch_bounds__(NT, 1) influence_topk_kernel(const float* __re
           const int h = (i >> 1) & 1;
           const int row = rl0 + 8 * h;
           const long t = n0 + 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+          if constexpr (MODE == kNearest) {
+            if (t < Nt) {
+              const float sc = 2.f * acc[i] - __ldg(S + t);
+              if (sc >= thr[row * 2]) {
+                const int slot = atomicAdd(&ccnt[row * 2], 1);
+                cs[(row * 2) * CAP + slot] = sc;
+                ci[(row * 2) * CAP + slot] = (int)t;
+              }
+            }
+            continue;
+          }
           const float sc = -(srow[h] * acc[i]);
           if (t < Nt) {
             if (sc > 0.f && sc >= thr[row * 2]) {
@@ -305,6 +329,7 @@ __global__ void __launch_bounds__(NT, 1) influence_topk_kernel(const float* __re
         if (ccnt[o] > CAP - 8 * CG || (flush && ccnt[o] > 0)) {
           int len = lcnt[o];
           if (oq < Nq) thr[o] = merge_list(my_ls, my_li, &len, K, cs + o * CAP, ci + o * CAP, ccnt[o], osgn == 1);
+          if (MODE == kNearest && len < K) thr[o] = -INFINITY;
           lcnt[o] = len;
           ccnt[o] = 0;
         }
@@ -344,6 +369,106 @@ __global__ void influence_merge_kernel(int Nq, int J, int P, int K, const float*
     oi[k] = -1;
     os[k] = 0.f;
   }
+}
+
+constexpr int kFinishWarps = 4;
+
+// One warp per query.  Lane 0 merges the P slices' sign-0 lists of Kc candidates in slice order (by the GEMM's score);
+// the warp then forms every candidate's exact squared distance |a - b_t|^2 from the difference in fp64 (lanes strided
+// over the columns, then a fixed butterfly), and lane 0 sorts the candidates by (distance, index) and writes the first
+// K: idx and d2, padded with -1 / +inf past the pool, and mean = their values summed in rank order in fp64 over their
+// count.
+__global__ void __launch_bounds__(32 * kFinishWarps) nearest_finish_kernel(int Nq, int P, int Kc, int K,
+                                                                           const float* __restrict__ lscore,
+                                                                           const int* __restrict__ lidx,
+                                                                           const float* __restrict__ a,
+                                                                           const float* __restrict__ b, int D1,
+                                                                           const float* __restrict__ value,
+                                                                           int32_t* __restrict__ idx,
+                                                                           float* __restrict__ d2,
+                                                                           float* __restrict__ mean) {
+  __shared__ float cs[kFinishWarps][LFMQ_NEAREST_MAX_CAND];
+  __shared__ int ci[kFinishWarps][LFMQ_NEAREST_MAX_CAND];
+  __shared__ double cd[kFinishWarps][LFMQ_NEAREST_MAX_CAND];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long q = (long)blockIdx.x * kFinishWarps + w;
+  if (q >= Nq) return;                       // the whole warp
+  int len = 0;
+  if (lane == 0)
+    for (int p = 0; p < P; ++p) {
+      const long e = (((long)p * Nq + q) * 2) * Kc;
+      int n = 0;
+      while (n < Kc && lidx[e + n] >= 0) ++n;
+      merge_list(cs[w], ci[w], &len, Kc, lscore + e, lidx + e, n, false);
+    }
+  len = __shfl_sync(0xffffffffu, len, 0);
+  __syncwarp();
+  const float* aq = a + q * D1;
+  for (int c = 0; c < len; ++c) {
+    const float* bt = b + (long)ci[w][c] * D1;
+    double acc = 0.0;
+    for (int d = lane; d < D1; d += 32) {
+      const double v = (double)aq[d] - (double)bt[d];
+      acc += v * v;
+    }
+    acc = warp_sum(acc);
+    if (lane == 0) cd[w][c] = acc;
+  }
+  __syncwarp();
+  if (lane != 0) return;
+  for (int c = 1; c < len; ++c) {            // insertion sort by (distance, lower index)
+    const double dv = cd[w][c];
+    const int iv = ci[w][c];
+    int p = c;
+    while (p > 0 && (cd[w][p - 1] > dv || (cd[w][p - 1] == dv && ci[w][p - 1] > iv))) {
+      cd[w][p] = cd[w][p - 1];
+      ci[w][p] = ci[w][p - 1];
+      --p;
+    }
+    cd[w][p] = dv;
+    ci[w][p] = iv;
+  }
+  const int n = len < K ? len : K;
+  double acc = 0.0;
+  for (int k = 0; k < K; ++k) {
+    if (k < n) {
+      idx[q * K + k] = ci[w][k];
+      d2[q * K + k] = (float)cd[w][k];
+      if (value) acc += (double)value[ci[w][k]];
+    } else {
+      idx[q * K + k] = -1;
+      d2[q * K + k] = INFINITY;
+    }
+  }
+  if (value) mean[q] = (float)(acc / n);
+}
+
+// One warp per row of p [R][D1]: the squared norm, lanes strided over the columns in fp64, then a fixed butterfly,
+// rounded to fp32.
+__global__ void nearest_norm_kernel(const float* __restrict__ p, int R, int D1, float* __restrict__ nf) {
+  const long r = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (r >= R) return;
+  double acc = 0.0;
+  for (int d = threadIdx.x & 31; d < D1; d += 32) {
+    const double v = (double)p[r * D1 + d];
+    acc += v * v;
+  }
+  acc = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) nf[r] = (float)acc;
+}
+
+template <int MODE>
+int configure_topk() {
+  static std::atomic<uint64_t> configured{0};
+  int dev = 0;
+  LFMQ_CUDA_CHECK(cudaGetDevice(&dev));
+  const uint64_t bit = 1ull << (dev & 63);
+  if (!(configured.load() & bit)) {
+    LFMQ_CUDA_CHECK(cudaFuncSetAttribute(influence_topk_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)TOPK_SMEM));
+    configured.fetch_or(bit);
+  }
+  return 0;
 }
 
 constexpr int kSumRows = 2048;     // pool rows per partial sum of sum_t u_t
@@ -425,17 +550,9 @@ InfluencePlan influence_plan(int Nq, int Nt, int D1, int J, int K) {
 int influence_topk(cudaStream_t s, const InfluencePlan& pl, const float* a, const float* u, const float* sc, int Nq,
                    int Nt, int D1, int J, int K, float* lscore, int* lidx, double* part, double* usum, int* pos_idx,
                    float* pos_score, int* neg_idx, float* neg_score, float* total) {
-  static std::atomic<uint64_t> configured{0};
-  int dev = 0;
-  LFMQ_CUDA_CHECK(cudaGetDevice(&dev));
-  const uint64_t bit = 1ull << (dev & 63);
-  if (!(configured.load() & bit)) {
-    LFMQ_CUDA_CHECK(cudaFuncSetAttribute(influence_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)TOPK_SMEM));
-    configured.fetch_or(bit);
-  }
+  if (int e = configure_topk<kDot>()) return e;
   const dim3 grid((unsigned)cdivl(Nq, TM), (unsigned)pl.P, (unsigned)J);
-  influence_topk_kernel<<<grid, NT, TOPK_SMEM, s>>>(a, u, sc, Nq, Nt, D1, K, pl.tiles_per_slice, lscore, lidx);
+  influence_topk_kernel<kDot><<<grid, NT, TOPK_SMEM, s>>>(a, u, sc, Nq, Nt, D1, K, pl.tiles_per_slice, lscore, lidx);
   LFMQ_LAUNCH_CHECK();
   const long nm = (long)J * Nq * 2;
   influence_merge_kernel<<<(int)cdivl(nm, 128), 128, 0, s>>>(Nq, J, pl.P, K, lscore, lidx, pos_idx, pos_score, neg_idx,
@@ -447,6 +564,27 @@ int influence_topk(cudaStream_t s, const InfluencePlan& pl, const float* a, cons
   influence_usum_final_kernel<<<(int)cdivl((long)J * D1, 128), 128, 0, s>>>(part, pl.n_sum, D1, J, usum);
   LFMQ_LAUNCH_CHECK();
   influence_total_kernel<<<(int)cdivl((long)Nq * J * 32, 256), 256, 0, s>>>(a, sc, usum, Nq, D1, J, total);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+int nearest_norms(cudaStream_t s, const float* p, int R, int D1, float* nf) {
+  nearest_norm_kernel<<<(int)cdivl((long)R * 32, 256), 256, 0, s>>>(p, R, D1, nf);
+  LFMQ_LAUNCH_CHECK();
+  return 0;
+}
+
+int nearest_topk(cudaStream_t s, const InfluencePlan& pl, const float* a, const float* b, const float* bn,
+                 const float* value, int Nq, int Nt, int D1, int K, float* lscore, int* lidx, int32_t* idx, float* d2,
+                 float* mean) {
+  const int Kc = nearest_candidates(K);
+  if (int e = configure_topk<kNearest>()) return e;
+  const dim3 grid((unsigned)cdivl(Nq, TM), (unsigned)pl.P, 1u);
+  influence_topk_kernel<kNearest><<<grid, NT, TOPK_SMEM, s>>>(a, b, bn, Nq, Nt, D1, Kc, pl.tiles_per_slice, lscore,
+                                                              lidx);
+  LFMQ_LAUNCH_CHECK();
+  nearest_finish_kernel<<<(int)cdivl(Nq, kFinishWarps), 32 * kFinishWarps, 0, s>>>(Nq, pl.P, Kc, K, lscore, lidx, a, b,
+                                                                                 D1, value, idx, d2, mean);
   LFMQ_LAUNCH_CHECK();
   return 0;
 }

@@ -151,6 +151,29 @@ InfluencePlan influence_plan(int Nq, int Nt, int D1, int J, int K);
 int influence_topk(cudaStream_t s, const InfluencePlan& pl, const float* a, const float* u, const float* sc, int Nq,
                    int Nt, int D1, int J, int K, float* lscore, int* lidx, double* part, double* usum, int* pos_idx,
                    float* pos_score, int* neg_idx, float* neg_score, float* total);
+// influence_topk's second mode (lfmq_nearest_topk): the K pool rows b [Nt][D1] nearest to each query a [Nq][D1].
+// nearest_norms: the rows' squared norms nf [R] (fp64 sums in a fixed order, rounded to fp32).  The GEMM shortlists
+// nearest_candidates(K) rows per query by the score 2 a.b - |b|^2 (bn [Nt] the pool's norms; pl planned for that many
+// candidates); their exact fp64 distances pick idx / d2 [Nq][K] and, with value [Nt], mean [Nq].
+constexpr int LFMQ_NEAREST_MAX_CAND = 80;
+__host__ __device__ constexpr int nearest_candidates(int K) { return K + 16; }
+int nearest_norms(cudaStream_t s, const float* p, int R, int D1, float* nf);
+int nearest_topk(cudaStream_t s, const InfluencePlan& pl, const float* a, const float* b, const float* bn,
+                 const float* value, int Nq, int Nt, int D1, int K, float* lscore, int* lidx, int32_t* idx, float* d2,
+                 float* mean);
+// Split-conformal intervals (conformal.cu, lfmq_conformal_*).  conformal_sort_bytes: the temp storage of the radix sort
+// of S * Nc 64-bit (step, score) keys.  conformal_scores: r [n] of pred / y / scale [n] (scale nullable).
+// conformal_calibrate: key / skey [S * Nc] scratch; n_valid [S], sorted [S][Nc], qhat [S][Q] of the host levels [Q].
+// conformal_apply: lower / upper [S][N][Q] and pvalue [S][N] (y nullable: NaN p-values).
+constexpr int LFMQ_CONFORMAL_MAX_LEVELS = 32;
+int conformal_sort_bytes(int S, int Nc, size_t* bytes);
+int conformal_scores(cudaStream_t s, long n, const float* pred, const float* y, const float* scale, float* r);
+int conformal_calibrate(cudaStream_t s, int S, int Nc, const float* pred, const float* y, const float* scale,
+                        const double* levels, int Q, void* temp, size_t temp_bytes, uint64_t* key, uint64_t* skey,
+                        int32_t* n_valid, float* sorted, float* qhat);
+int conformal_apply(cudaStream_t s, int S, int N, int Nc, int Q, const float* pred, const float* y, const float* scale,
+                    const float* sorted, const int32_t* n_valid, const float* qhat, float* lower, float* upper,
+                    float* pvalue);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

@@ -1307,7 +1307,7 @@ int dist_levels_check(const float* levels, int32_t n_levels, const char* fn) {
     return LFMQ_ERR_ARG;
   }
   for (int k = 0; k < n_levels; ++k)
-    if (!(levels[k] > 0.f && levels[k] < 1.f) || (k > 0 && !(levels[k] > levels[k - 1]))) {
+    if (!(levels[k] > 0.0 && levels[k] < 1.0) || (k > 0 && !(levels[k] > levels[k - 1]))) {
       LFMQ_SET_ERR("%s: levels must be strictly increasing inside (0, 1) (level %d is %g)", fn, k, levels[k]);
       return LFMQ_ERR_ARG;
     }
@@ -1995,6 +1995,160 @@ int32_t lfmq_influence_topk(const float* a, const float* u, const float* s, int3
   RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return topk_layout(pl, cv); }, &w));
   return lfmq::influence_topk((cudaStream_t)stream, pl, a, u, s, Nq, Nt, D1, J, K, w.lscore, w.lidx, w.part, w.usum,
                               pos_idx, pos_score, neg_idx, neg_score, total);
+}
+
+// ---- nearest pool rows (lfmq_nearest_topk) ------------------------------------------------------------------------
+namespace {
+struct NearestWork {
+  float* lscore;
+  int32_t* lidx;
+  float* bn;
+};
+NearestWork nearest_layout(const lfmq::InfluencePlan& pl, int32_t Nt, Carver& cv) {
+  NearestWork w{};
+  w.lscore = cv.take<float>(pl.list_elems);
+  w.lidx = cv.take<int32_t>(pl.list_elems);
+  w.bn = cv.take<float>((size_t)Nt);
+  return w;
+}
+
+// the pool split of the shortlisting GEMM, which keeps nearest_candidates(K) rows per query
+lfmq::InfluencePlan nearest_plan(int32_t Nq, int32_t Nt, int32_t D1, int32_t K) {
+  return lfmq::influence_plan(Nq, Nt, D1, 1, lfmq::nearest_candidates(K));
+}
+}  // namespace
+
+int32_t lfmq_nearest_topk_work_bytes(int32_t Nq, int32_t Nt, int32_t D1, int32_t K, uint64_t* bytes) {
+  const char* fn = "lfmq_nearest_topk_work_bytes";
+  RUN(topk_check(Nq, Nt, D1, 1, K, fn));
+  const lfmq::InfluencePlan pl = nearest_plan(Nq, Nt, D1, K);
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return nearest_layout(pl, Nt, cv); });
+}
+
+int32_t lfmq_nearest_topk(const float* a, const float* b, const float* value, int32_t Nq, int32_t Nt, int32_t D1,
+                          int32_t K, int32_t* idx, float* d2, float* mean, void* work, uint64_t work_bytes,
+                          void* stream) {
+  const char* fn = "lfmq_nearest_topk";
+  RUN(topk_check(Nq, Nt, D1, 1, K, fn));
+  if (!a || !b || !idx || !d2 || (!value) != (!mean)) {
+    LFMQ_SET_ERR("%s: null pointer (value and mean go together)", fn);
+    return LFMQ_ERR_ARG;
+  }
+  const lfmq::InfluencePlan pl = nearest_plan(Nq, Nt, D1, K);
+  NearestWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return nearest_layout(pl, Nt, cv); }, &w));
+  const cudaStream_t s = (cudaStream_t)stream;
+  RUN(lfmq::nearest_norms(s, b, Nt, D1, w.bn));
+  return lfmq::nearest_topk(s, pl, a, b, w.bn, value, Nq, Nt, D1, K, w.lscore, w.lidx, idx, d2, mean);
+}
+
+// ---- split-conformal intervals (lfmq_conformal_*) -----------------------------------------------------------------
+namespace {
+int conformal_shape_check(int32_t S, int32_t N, const char* fn) {
+  if (S < 1 || N < 1 || (int64_t)S * N > INT32_MAX) {
+    LFMQ_SET_ERR("%s: need S, N >= 1 with S * N < 2^31 (got %d, %d)", fn, S, N);
+    return LFMQ_ERR_ARG;
+  }
+  return 0;
+}
+
+int conformal_levels_check(const double* levels, int32_t Q, const char* fn) {
+  if (!levels || Q < 1 || Q > lfmq::LFMQ_CONFORMAL_MAX_LEVELS) {
+    LFMQ_SET_ERR("%s: need 1 <= Q <= %d host levels (got %d)", fn, lfmq::LFMQ_CONFORMAL_MAX_LEVELS, Q);
+    return LFMQ_ERR_ARG;
+  }
+  for (int k = 0; k < Q; ++k)
+    if (!(levels[k] > 0.0 && levels[k] < 1.0) || (k > 0 && !(levels[k] > levels[k - 1]))) {
+      LFMQ_SET_ERR("%s: the levels must be strictly increasing inside (0, 1)", fn);
+      return LFMQ_ERR_ARG;
+    }
+  return 0;
+}
+
+struct ConformalWork {
+  uint64_t *key, *skey;
+  char* temp;
+};
+ConformalWork conformal_layout(int32_t S, int32_t Nc, size_t temp_bytes, Carver& cv) {
+  ConformalWork w{};
+  w.key = cv.take<uint64_t>((size_t)S * Nc);
+  w.skey = cv.take<uint64_t>((size_t)S * Nc);
+  w.temp = cv.take<char>(temp_bytes);
+  return w;
+}
+}  // namespace
+
+int32_t lfmq_conformal_scores_work_bytes(int32_t S, int32_t N, uint64_t* bytes) {
+  const char* fn = "lfmq_conformal_scores_work_bytes";
+  RUN(conformal_shape_check(S, N, fn));
+  return report_work_bytes(bytes, fn, [](Carver&) { return 0; });
+}
+
+int32_t lfmq_conformal_scores(const float* pred, const float* y, const float* scale, int32_t S, int32_t N, float* r,
+                              void* work, uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_conformal_scores";
+  RUN(conformal_shape_check(S, N, fn));
+  if (!pred || !y || !r) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  (void)work;
+  (void)work_bytes;
+  return lfmq::conformal_scores((cudaStream_t)stream, (long)S * N, pred, y, scale, r);
+}
+
+int32_t lfmq_conformal_calibrate_work_bytes(int32_t S, int32_t Nc, uint64_t* bytes) {
+  const char* fn = "lfmq_conformal_calibrate_work_bytes";
+  RUN(conformal_shape_check(S, Nc, fn));
+  size_t temp = 0;
+  RUN(lfmq::conformal_sort_bytes(S, Nc, &temp));
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return conformal_layout(S, Nc, temp, cv); });
+}
+
+int32_t lfmq_conformal_calibrate(const float* pred, const float* y, const float* scale, int32_t S, int32_t Nc,
+                                 const double* levels, int32_t Q, int32_t* n_valid, float* sorted, float* qhat,
+                                 void* work, uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_conformal_calibrate";
+  RUN(conformal_shape_check(S, Nc, fn));
+  RUN(conformal_levels_check(levels, Q, fn));
+  if (!pred || !y || !n_valid || !sorted || !qhat) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  size_t temp = 0;
+  RUN(lfmq::conformal_sort_bytes(S, Nc, &temp));
+  ConformalWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return conformal_layout(S, Nc, temp, cv); }, &w));
+  return lfmq::conformal_calibrate((cudaStream_t)stream, S, Nc, pred, y, scale, levels, Q, w.temp, temp, w.key, w.skey,
+                                   n_valid, sorted, qhat);
+}
+
+int32_t lfmq_conformal_apply_work_bytes(int32_t S, int32_t N, int32_t Nc, int32_t Q, uint64_t* bytes) {
+  const char* fn = "lfmq_conformal_apply_work_bytes";
+  RUN(conformal_shape_check(S, N, fn));
+  RUN(conformal_shape_check(S, Nc, fn));
+  if (Q < 1 || Q > lfmq::LFMQ_CONFORMAL_MAX_LEVELS) {
+    LFMQ_SET_ERR("%s: need 1 <= Q <= %d (got %d)", fn, lfmq::LFMQ_CONFORMAL_MAX_LEVELS, Q);
+    return LFMQ_ERR_ARG;
+  }
+  return report_work_bytes(bytes, fn, [](Carver&) { return 0; });
+}
+
+int32_t lfmq_conformal_apply(const float* pred, const float* y, const float* scale, int32_t S, int32_t N,
+                             const float* sorted, const int32_t* n_valid, const float* qhat, int32_t Nc, int32_t Q,
+                             float* lower, float* upper, float* pvalue, void* work, uint64_t work_bytes,
+                             void* stream) {
+  const char* fn = "lfmq_conformal_apply";
+  uint64_t need = 0;
+  RUN(lfmq_conformal_apply_work_bytes(S, N, Nc, Q, &need));
+  if (!pred || !sorted || !n_valid || !qhat || !lower || !upper || !pvalue) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  (void)work;
+  (void)work_bytes;
+  return lfmq::conformal_apply((cudaStream_t)stream, S, N, Nc, Q, pred, y, scale, sorted, n_valid, qhat, lower, upper,
+                               pvalue);
 }
 
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,

@@ -38,7 +38,7 @@ def _scratch(owner, key, work_bytes, *args):
 
 
 class _TopkScratch(object):
-    """Keeps influence_topk's scratch between calls without an engine."""
+    """Keeps the scratch of influence_topk, nearest_topk and conformal_calibrate between calls without an engine."""
 
     def __init__(self, device):
         self.device = device
@@ -64,6 +64,91 @@ def influence_topk(a, u, s, k, owner=None):
     N.check(lib.lfmq_influence_topk(_ptr(a), _ptr(u), _ptr(s), Nq, Nt, D1, J, K, _ptr(pos_idx), _ptr(pos_score),
                                     _ptr(neg_idx), _ptr(neg_score), _ptr(total), _ptr(work), work.numel(), _stream()))
     return pos_idx, pos_score, neg_idx, neg_score, total
+
+
+def nearest_topk(a, b, k, value=None, owner=None):
+    """lfmq_nearest_topk: for the queries a [Nq,D1] and the pool b [Nt,D1] (device fp32), the device tensors idx
+    [Nq,K] (int32, nearest first, ties to the lower row, -1 past Nt) and d2 [Nq,K] (squared distances, +inf past Nt),
+    and with value [Nt] also mean [Nq], the mean value of the listed rows (else None).  `owner` keeps the scratch."""
+    a, b = a.contiguous(), b.contiguous()
+    Nq, D1 = a.shape
+    Nt, K = b.shape[0], int(k)
+    assert b.shape == (Nt, D1), (tuple(a.shape), tuple(b.shape))
+    if value is not None:
+        value = value.contiguous()
+        assert value.shape == (Nt,) and value.dtype == torch.float32, tuple(value.shape)
+    lib = N.load()
+    work = _scratch(owner if owner is not None else _TopkScratch(a.device), 'nearest_topk',
+                    lib.lfmq_nearest_topk_work_bytes, Nq, Nt, D1, K)
+    idx = torch.empty(Nq, K, dtype=torch.int32, device=a.device)
+    d2 = torch.empty(Nq, K, dtype=torch.float32, device=a.device)
+    mean = torch.empty(Nq, dtype=torch.float32, device=a.device) if value is not None else None
+    N.check(lib.lfmq_nearest_topk(_ptr(a), _ptr(b), _ptr(value), Nq, Nt, D1, K, _ptr(idx), _ptr(d2), _ptr(mean),
+                                  _ptr(work), work.numel(), _stream()))
+    return idx, d2, mean
+
+
+def _conformal_args(pred, y, scale):
+    """pred, y and scale as contiguous device fp32 [S,N] (y, scale may be None)."""
+    pred = pred.contiguous()
+    assert pred.dim() == 2 and pred.is_cuda and pred.dtype == torch.float32, (tuple(pred.shape), pred.dtype)
+    out = [pred]
+    for t in (y, scale):
+        if t is not None:
+            t = t.contiguous()
+            assert t.shape == pred.shape and t.dtype == torch.float32, (tuple(t.shape), t.dtype)
+        out.append(t)
+    return out
+
+
+def conformal_scores(pred, y, scale=None):
+    """lfmq_conformal_scores: the nonconformity scores r = |y - pred| (/ scale) [S,N] of device fp32 [S,N] arrays, NaN
+    where y is not finite."""
+    pred, y, scale = _conformal_args(pred, y, scale)
+    S, n = pred.shape
+    lib = N.load()
+    r = torch.empty_like(pred)
+    N.check(lib.lfmq_conformal_scores(_ptr(pred), _ptr(y), _ptr(scale), S, n, _ptr(r), None, 0, _stream()))
+    return r
+
+
+def conformal_calibrate(pred, y, levels, scale=None, owner=None):
+    """lfmq_conformal_calibrate: of the calibration windows' pred, y (and scale) [S,Nc] and the host `levels`, the device
+    tensors n_valid [S] (int32), sorted [S,Nc] (each step's scores ascending, NaN last) and qhat [S,Q] (+inf where the
+    rank exceeds n_valid).  `owner` keeps the scratch."""
+    pred, y, scale = _conformal_args(pred, y, scale)
+    S, nc = pred.shape
+    lv = np.ascontiguousarray(levels, dtype=np.float64)
+    Q = int(lv.size)
+    lib = N.load()
+    work = _scratch(owner if owner is not None else _TopkScratch(pred.device), 'conformal',
+                    lib.lfmq_conformal_calibrate_work_bytes, S, nc)
+    n_valid = torch.empty(S, dtype=torch.int32, device=pred.device)
+    sorted_ = torch.empty_like(pred)
+    qhat = torch.empty(S, max(Q, 1), dtype=torch.float32, device=pred.device)
+    N.check(lib.lfmq_conformal_calibrate(_ptr(pred), _ptr(y), _ptr(scale), S, nc,
+                                         lv.ctypes.data_as(C.c_void_p), Q, _ptr(n_valid), _ptr(sorted_), _ptr(qhat),
+                                         _ptr(work), work.numel(), _stream()))
+    return n_valid, sorted_, qhat
+
+
+def conformal_apply(pred, calibration, y=None, scale=None):
+    """lfmq_conformal_apply: the intervals of the query windows pred (y, scale) [S,N] from conformal_calibrate's
+    (n_valid, sorted, qhat): the device tensors lower, upper [S,N,Q] and pvalue [S,N] (NaN where y is None or not
+    finite)."""
+    pred, y, scale = _conformal_args(pred, y, scale)
+    n_valid, sorted_, qhat = calibration
+    S, n = pred.shape
+    nc, Q = sorted_.shape[1], qhat.shape[1]
+    assert sorted_.shape[0] == S and qhat.shape[0] == S and n_valid.shape == (S,)
+    lib = N.load()
+    lower = torch.empty(S, n, Q, dtype=torch.float32, device=pred.device)
+    upper = torch.empty_like(lower)
+    pvalue = torch.empty_like(pred)
+    N.check(lib.lfmq_conformal_apply(_ptr(pred), _ptr(y), _ptr(scale), S, n, _ptr(sorted_.contiguous()),
+                                     _ptr(n_valid.contiguous()), _ptr(qhat.contiguous()), nc, Q, _ptr(lower),
+                                     _ptr(upper), _ptr(pvalue), None, 0, _stream()))
+    return lower, upper, pvalue
 
 
 class _HandleEngine(object):

@@ -128,6 +128,12 @@ SCHEMA = [
     ('pred_quantiles', _STRING, None, "'-'-separated levels in (0, 1), e.g. 0.05-0.25-0.5-0.75-0.95, at UQ prediction; "
                                       'writes pred/quantiles.dat (the quantiles of each window\'s Monte-Carlo dropout '
                                       'mixture, with its CRPS, log score and PIT) and pred/calibration.dat; unset = off'),
+    ('conformal_levels', _STRING, None, "'-'-separated coverage levels in (0, 1), e.g. 0.5-0.8-0.9, at prediction; "
+                                        'writes pred/intervals.dat (every forecast\'s split-conformal interval, '
+                                        'calibrated on the held-out validation companies, with its conformal p-value) '
+                                        'and pred/coverage.dat; unset = off'),
+    ('conformal_knn', _INT, 0, 'Training windows whose mean absolute error scales each conformal interval (1 to 64) '
+                               'of a point or linear model with forecast_steps = 1: the normalised score; 0 = off'),
     ('sample_weight_field', _STRING, None, 'Datafile column that weighs each training window in the training loss, read '
                                          'raw at the window\'s last input row (NaN counts as 0; negative or infinite '
                                          'values are refused); unset = off.  Ignored with --train=False'),
@@ -173,19 +179,32 @@ def get_configs(argv=None, list_sep='-'):
 MAX_PRED_QUANTILES = 32      # lfmq_chain_forward_uq_dist's cap on the levels
 
 
+MAX_CONFORMAL_LEVELS = 32    # lfmq_conformal_calibrate's cap on the levels
+
+
 def pred_quantile_levels(spec):
     """The levels of --pred_quantiles: None when unset, else the '-'-separated floats, which must be strictly
     increasing inside (0, 1), at most MAX_PRED_QUANTILES of them.  A malformed value raises ValueError."""
+    return _levels(spec, 'pred_quantiles', MAX_PRED_QUANTILES)
+
+
+def conformal_levels(spec):
+    """The coverage levels of --conformal_levels, parsed and checked as pred_quantile_levels parses its levels, at most
+    MAX_CONFORMAL_LEVELS of them."""
+    return _levels(spec, 'conformal_levels', MAX_CONFORMAL_LEVELS)
+
+
+def _levels(spec, flag, cap):
     if spec is None or str(spec).strip() == '':
         return None
     try:
         levels = [float(v) for v in str(spec).split('-')]
     except ValueError:
-        raise ValueError("--pred_quantiles %s: expected '-'-separated levels such as 0.05-0.5-0.95" % spec)
-    if not 1 <= len(levels) <= MAX_PRED_QUANTILES:
-        raise ValueError('--pred_quantiles %s: between 1 and %d levels' % (spec, MAX_PRED_QUANTILES))
+        raise ValueError("--%s %s: expected '-'-separated levels such as 0.05-0.5-0.95" % (flag, spec))
+    if not 1 <= len(levels) <= cap:
+        raise ValueError('--%s %s: between 1 and %d levels' % (flag, spec, cap))
     if any(not 0.0 < v < 1.0 for v in levels) or any(b <= a for a, b in zip(levels, levels[1:])):
-        raise ValueError('--pred_quantiles %s: the levels must be strictly increasing inside (0, 1)' % spec)
+        raise ValueError('--%s %s: the levels must be strictly increasing inside (0, 1)' % (flag, spec))
     if any(not 0.0 < v < 1.0 for v in np.float32(levels)) or any(np.diff(np.float32(levels)) <= 0):
-        raise ValueError('--pred_quantiles %s: the levels must stay distinct inside (0, 1) in single precision' % spec)
+        raise ValueError('--%s %s: the levels must stay distinct inside (0, 1) in single precision' % (flag, spec))
     return levels

@@ -18,6 +18,7 @@ class NativeDenseForecaster(NativeForecaster):
     ``layer_with_weights-0``."""
 
     title = 'MLPLinearPointEstimate'
+    _flat_outputs = True          # model.predict returns [B, n_outputs]
 
     def _build_engine(self, config, seq_len, n_inputs, n_outputs, target_idx):
         from ....engine import DenseEngine, ForecastChainEngine

@@ -19,8 +19,9 @@ class NaiveForecaster(object):
     engine = None
     trainable_variables = []
 
-    def __init__(self, seq_len, n_inputs, n_outputs):
+    def __init__(self, seq_len, n_inputs, n_outputs, target_idx=0):
         self.T, self.F, self.O = seq_len, n_inputs, n_outputs
+        self.target_idx = target_idx
 
     def predict_device(self, inp):
         import torch
@@ -32,6 +33,22 @@ class NaiveForecaster(object):
 
     def predict(self, inp, batch_size=None):
         return self.predict_device(inp).cpu().numpy()
+
+    def conformal_forecast(self, inp):
+        """(pred [1,B], None): the forecast of the target field, whose score is |y - pred| (DESIGN.md section 5j)."""
+        return self.predict_device(inp)[:, self.target_idx].unsqueeze(0).contiguous(), None
+
+    def conformal(self, cal_batches, query_windows, levels, knn=0, query_forecast=None, query_targets=None,
+                  pool_batches=None):
+        """Split-conformal intervals of the naive forecast, as NativeForecaster.conformal (no kNN score: the naive
+        forecast has no features)."""
+        from .rnn_point_estimate import conformal_intervals
+        if int(knn) > 0:
+            raise ValueError('conformal: NaivePointEstimate has no head-input features for the kNN score')
+        if query_forecast is None:
+            query_forecast = self.conformal_forecast(query_windows)
+        return conformal_intervals(self.conformal_forecast, cal_batches, query_windows, query_forecast, query_targets,
+                                   levels)
 
     def load_weights(self, prefix):
         return None
@@ -65,4 +82,5 @@ class NaivePointEstimate(BaseModelClass):
             raise NotImplementedError('NaivePointEstimate has one output (naive_point_estimate.py:45-58); '
                                       'forecast_steps = %d' % config.forecast_steps)
         super(NaivePointEstimate, self).__init__(self.seq_len, self.n_inputs, self.n_outputs)
-        self.model = NaiveForecaster(self.seq_len, self.n_inputs, self.n_outputs)
+        # the target field's index, which the conformal intervals read
+        self.model = NaiveForecaster(self.seq_len, self.n_inputs, self.n_outputs, getattr(dataset, 'target_index', 0))

@@ -47,6 +47,50 @@ def _keras(outputs):
     return outputs[0] if len(outputs) == 1 else outputs
 
 
+def conformal_intervals(forecast, cal_batches, query_windows, query_forecast, query_targets, levels, knn=0,
+                        knn_features=None, pool_batches=None):
+    """Split-conformal intervals (DESIGN.md section 5j) of any model: forecast(inp) -> (pred [S,B], scale [S,B] or
+    None), device fp32, gives the calibration windows' forecasts, query_forecast the query windows'.  The scores are
+    those of engine.conformal_scores; the calibration set is cal_batches ([(inp, target)] with target [B] the normalised
+    target field at the window's last step, which is norm_targets_s of every step s).  With knn = K > 0 the scale of a window x is d(x) + beta: d(x) the mean |y_t - pred_t| of
+    the K windows of pool_batches nearest to x in knn_features(x) (engine.nearest_topk), beta 0.1 x the mean of
+    |y_t - pred_t| over the pool (windows with a finite target only).  Returns the device tensors (n_cal [S], qhat
+    [S,Q], lower, upper [S,N,Q], pvalue [S,N], scale [S,N]; scale 1 without one)."""
+    import torch
+    from ....engine import conformal_apply, conformal_calibrate, conformal_scores, nearest_topk
+    pred_c, scale_c, y_c = [], [], []
+    for x, y in cal_batches:
+        p, sc = forecast(x)
+        pred_c.append(p)
+        scale_c.append(sc)
+        y_c.append(y.to(torch.float32).unsqueeze(0).expand(p.shape[0], -1))
+    pred_c, y_c = torch.cat(pred_c, dim=1), torch.cat(y_c, dim=1)
+    scale_c = torch.cat(scale_c, dim=1) if scale_c[0] is not None else None
+    pred_q, scale_q = query_forecast
+    if knn > 0:
+        feats, resid = [], []
+        for x, y in pool_batches:
+            p, _ = forecast(x)
+            feats.append(knn_features(x))
+            resid.append(conformal_scores(p, y.to(torch.float32).unsqueeze(0))[0])
+        feats, resid = torch.cat(feats), torch.cat(resid)
+        known = torch.isfinite(resid)
+        feats, resid = feats[known].contiguous(), resid[known].contiguous()
+        if resid.numel() == 0:
+            raise ValueError('conformal: the kNN score needs training windows with known targets')
+        beta = torch.tensor(0.1 * float(resid.double().mean()), dtype=torch.float32, device=resid.device)
+        k = min(knn, resid.numel())
+
+        def knn_scale(windows):
+            return (nearest_topk(knn_features(windows), feats, k, value=resid)[2] + beta).unsqueeze(0).contiguous()
+        scale_c = torch.cat([knn_scale(x) for x, _ in cal_batches], dim=1)
+        scale_q = knn_scale(query_windows)
+    cal = conformal_calibrate(pred_c, y_c, levels, scale=scale_c)
+    lower, upper, pvalue = conformal_apply(pred_q, cal, y=query_targets, scale=scale_q)
+    scale = scale_q if scale_q is not None else torch.ones_like(pred_q)
+    return cal[0], cal[2], lower, upper, pvalue, scale
+
+
 class NativeForecaster(object):
     """Keras-subset model object (SURVEY 8b) of every trained model kind: __call__, predict, trainable_variables,
     save/load_weights, reset_states, summary -- plus ``train_step`` / ``train_step_dp``, the fused native training step,
@@ -263,11 +307,57 @@ class NativeForecaster(object):
         fp32 handle with the same parameters (their forecasts may differ from it by that precision's rounding)."""
         if self.config.forecast_steps != 1:
             raise ValueError('influence explains models with forecast_steps = 1 (got %d)' % self.config.forecast_steps)
+        eng = self._feature_engine()
+        return eng.influence([(_to_device(eng, x), y.contiguous()) for x, y in pool_batches],
+                             _to_device(eng, query_windows), int(k))
+
+    def _feature_engine(self):
+        """The handle engine of the head-input features (influence, the conformal kNN score): the model's own stage at
+        fp32 and tf32 and on the linear model, else an fp32 handle with the same parameters."""
         eng = self.engine.stages[0]
         if getattr(eng, 'precision', 'fp32') not in ('fp32', 'tf32'):
             eng = self._side_engine('influence', self.config.batch_size, self._new_influence_engine).stages[0]
-        return eng.influence([(_to_device(eng, x), y.contiguous()) for x, y in pool_batches],
-                             _to_device(eng, query_windows), int(k))
+        return eng
+
+    _flat_outputs = False         # model.predict returns [B,T,O] per output
+
+    def conformal_forecast(self, inp):
+        """The forecast and its conformal scale (DESIGN.md section 5j) of windows inp, as predict.py writes the
+        forecast: (pred [S,B], scale [S,B] or None) device fp32, pred = norm_preds_s.  A point model's scale is None
+        (the score is |y - pred|).  A uq model's is sigma: the one sample's at mc_samples = 1 (config.mc_samples),
+        else sqrt(mean_var + var_pred) of predict_mc's moments, the mixture's total variance, with pred = mean_pred."""
+        import torch
+        tidx = self._engine_kw['target_idx']
+        pick = (lambda t: t[:, tidx]) if self._flat_outputs else (lambda t: t[:, -1, tidx])      # noqa: E731
+        if self.uq and self.config.mc_samples > 1:
+            moments = self.predict_mc(inp, self.config.mc_samples)
+            pred = [pick(m[0]) for m in moments]
+            var = [pick(m[1] + m[2]) for m in moments]
+        else:
+            outs = self.predict_device(inp)
+            pred = [pick(t) for t in (outs[0::2] if self.uq else outs)]
+            var = [pick(t) for t in outs[1::2]] if self.uq else None
+        pred = torch.stack(pred).contiguous()
+        return pred, (torch.sqrt(torch.stack(var)).contiguous() if var is not None else None)
+
+    def conformal(self, cal_batches, query_windows, levels, knn=0, query_forecast=None, query_targets=None,
+                  pool_batches=None):
+        """Split-conformal intervals (conformal_intervals, DESIGN.md section 5j) of the query windows, calibrated on
+        cal_batches ([(inp, targets)] device batches).  query_forecast: the (pred, scale) conformal_forecast gave the
+        query windows, when they are already predicted (a uq model draws new dropout masks at every call); else they
+        are forecast here.  query_targets [S,N]: the normalised targets, for the p-values.  knn = K > 0 (point and
+        linear models with forecast_steps = 1): the normalised score, with neighbours from pool_batches ([(inp, target)],
+        the training split), in the head-input features of _feature_engine.  bf16 and bf16x3 models forecast at their own precision."""
+        knn_features = None
+        if int(knn) > 0:
+            if self.uq or self.config.forecast_steps != 1:
+                raise ValueError('conformal: the kNN score is for point and linear models with forecast_steps = 1')
+            eng = self._feature_engine()
+            knn_features = lambda x: eng.influence_features(_to_device(eng, x))[0]     # noqa: E731
+        if query_forecast is None:
+            query_forecast = self.conformal_forecast(query_windows)
+        return conformal_intervals(self.conformal_forecast, cal_batches, query_windows, query_forecast, query_targets,
+                                   levels, int(knn), knn_features, pool_batches)
 
     def _new_influence_engine(self, rows):
         from ....engine import ForecastChainEngine, ForecasterEngine

@@ -10,7 +10,7 @@ from collections import defaultdict
 import numpy as np
 import pandas as pd
 
-from .base_config import pred_quantile_levels
+from .base_config import conformal_levels, pred_quantile_levels
 from .model_utils.model import Model
 
 
@@ -48,6 +48,8 @@ class Predict(object):
         windows = []
         levels = pred_quantile_levels(getattr(self.config, 'pred_quantiles', None))
         dist = defaultdict(list)
+        conf_levels = conformal_levels(getattr(self.config, 'conformal_levels', None))
+        conf = defaultdict(list)          # the forecast and its variance that preds.dat holds, per step [B]
         for (inp_dev, target_dev, metadata) in self._batches:
             # one target window per input window: every forecast step is compared with it (Train._step_targets)
             inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()] * self.config.forecast_steps
@@ -73,6 +75,7 @@ class Predict(object):
                     dist['scores'].append(scores.cpu().numpy())
                 moments = [[t.cpu().numpy() for t in m] for m in moments]
                 preds = [m[0] for m in moments]
+                conf_var = [m[1] + m[2] for m in moments]      # the mixture's total variance (DESIGN.md 5j)
                 if self.config.mc_samples > 1:
                     # the reference's UQ ensemble in one prediction: the mean of the samples, and mean of the
                     # variances + variance of the variances (utils/post_processing.py:52-55); var_pred, the spread of
@@ -80,18 +83,24 @@ class Predict(object):
                     variance = [m[1] + m[3] for m in moments]
                     outputs['norm_preds_var'].append(self._extract_preds([m[2] for m in moments]))
                 else:           # one sample: its prediction and variance, the bits model.predict returns
-                    variance = [m[1] for m in moments]
+                    variance = conf_var = [m[1] for m in moments]
             else:                       # predict.py:135-138: [tar_1, var_1, .., tar_S, var_S]
                 model_preds = self.model.predict(inp_dev)
                 preds, variance = model_preds[0::2], model_preds[1::2]
+                conf_var = variance
             outputs['norm_preds'].append(self._extract_preds(preds))
+            if conf_levels is not None:
+                conf['pred'].append(np.concatenate(self._extract_preds(preds), axis=1).T)
+                if self.config.UQ:
+                    conf['var'].append(np.concatenate(self._extract_preds(conf_var), axis=1).T)
             outputs['norm_variance'].append(self._extract_preds(variance))
             if self.config.ig_steps > 0:
                 for key, t in zip(('attr', 'f_x', 'f_base'), self.model.attribute(inp_dev, self.config.ig_steps)):
                     ig[key].append(t.cpu().numpy())
             if self.config.perm_importance > 0:
                 held_out.append((inp_dev, target_dev))
-            if self.config.shapley_samples > 0 or self.config.ale_bins > 0 or self._influence_k() > 0:
+            if (self.config.shapley_samples > 0 or self.config.ale_bins > 0 or self._influence_k() > 0
+                    or (conf_levels is not None and getattr(self.config, 'conformal_knn', 0) > 0)):
                 windows.append(inp_dev)
         if self.config.ig_steps > 0:
             self._write_attributions(outputs, ig)
@@ -154,6 +163,8 @@ class Predict(object):
         if levels is not None:
             self._write_quantiles(df, levels, np.concatenate(dist['quantiles'], axis=1),
                                   np.concatenate(dist['scores'], axis=1), unscale)
+        if conf_levels is not None:
+            self._write_conformal(df, conf_levels, conf, windows, unscale)
         print("Unscaled MSE normalized by Seq_Norm (%s)" % self.config.model_dir.split('/')[-1])
         print(df[[x for x in df.columns if 'unscaled' in x]].mean())
         for i in range(self.config.forecast_steps):
@@ -229,14 +240,8 @@ class Predict(object):
         windows of the training split that push its forecast up and down the most (NativeForecaster.influence).  The
         pool is the training split a --train=True run with this run's flags draws, with this model's scales.dat; in a
         walk-forward run the origin's own (pool_dates).  write_influence gives the layout."""
-        import copy
         import torch
-        cfg = copy.deepcopy(self.config)
-        cfg.train = True
-        if getattr(self.config, 'pool_dates', None):
-            cfg.start_date, cfg.end_date = self.config.pool_dates
-        pool = type(self.dataset)(cfg)
-        pool.generate_dataset()
+        pool = self._training_draw()
         batches = [pool.get_batch(*items) for items in pool.train_set.batch(batch_size=self.config.batch_size)]
         meta = np.concatenate([m for _, _, m in batches])
         tgt = torch.cat([(y if y.dim() == 2 else y[:, -1]) for _, y, _ in batches])[:, self.target_index]
@@ -245,6 +250,58 @@ class Predict(object):
                         np.vstack(outputs['gvkey']).flatten(),
                         shapley_output_names(1, self.config.UQ), meta[:, 0].astype('int32'), meta[:, 1],
                         tgt.cpu().numpy(), *[t.cpu().numpy() for t in res])
+
+    def _training_draw(self):
+        """The Dataset a --train=True run with this run's flags draws (its training and validation splits), with this
+        model's scales.dat; in a walk-forward run the origin's own (pool_dates)."""
+        import copy
+        cfg = copy.deepcopy(self.config)
+        cfg.train = True
+        if getattr(self.config, 'pool_dates', None):
+            cfg.start_date, cfg.end_date = self.config.pool_dates
+        pool = type(self.dataset)(cfg)
+        pool.generate_dataset()
+        return pool
+
+    def _target_batches(self, index_set, pool):
+        """[(inp, target [B])] device batches of an IndexSet of `pool`, with each window's normalised target field at
+        its last step (norm_targets_s), and the windows' metadata."""
+        batches = [pool.get_batch(*items) for items in index_set.batch(batch_size=self.config.batch_size)]
+        pairs = [(x, (y if y.dim() == 2 else y[:, -1])[:, self.target_index].contiguous()) for x, y, _ in batches]
+        meta = np.concatenate([m for _, _, m in batches]) if batches else np.zeros((0, 3), dtype=object)
+        return pairs, meta
+
+    def _write_conformal(self, df, levels, conf, windows, unscale):
+        """<model_dir>/pred/intervals.dat and coverage.dat (--conformal_levels): split-conformal intervals of every
+        row of preds.dat (`df`), calibrated on the validation split of _training_draw (NativeForecaster.conformal,
+        DESIGN.md section 5j); interval_table and coverage_table give the layouts."""
+        import torch
+        pool = self._training_draw()
+        cal, cal_meta = self._target_batches(pool.valid_set, pool)
+        if not cal:
+            raise ValueError('--conformal_levels: the validation split of the training draw has no windows to '
+                             'calibrate on (validation_size = %s)' % self.config.validation_size)
+        knn = int(getattr(self.config, 'conformal_knn', 0))
+        train = self._target_batches(pool.train_set, pool)[0] if knn > 0 else None
+        dev = cal[0][0].device
+        pred = torch.from_numpy(np.concatenate(conf['pred'], axis=1)).to(dev)
+        scale = (torch.sqrt(torch.from_numpy(np.concatenate(conf['var'], axis=1)).to(dev))
+                 if self.config.UQ else None)
+        S = pred.shape[0]
+        targets = np.stack([df['norm_targets_%d' % (s + 1)].to_numpy(dtype=np.float32) for s in range(S)])
+        n_cal, qhat, lower, upper, pvalue, scale = (t.cpu().numpy() for t in self.model.conformal(
+            cal, torch.cat(windows) if knn > 0 else None, levels, knn=knn, query_forecast=(pred, scale),
+            query_targets=torch.from_numpy(targets).to(dev), pool_batches=train))
+        seq_norm = df['seq_norm'].to_numpy(dtype=np.float64)
+        interval_table(df[['date', 'gvkey']], levels, lower, upper, scale, pvalue, seq_norm, unscale).to_csv(
+            os.path.join(self.pred_dir, 'intervals.dat'), sep=' ', index=False, date_format="%Y%m%d")
+        date = np.asarray([int(d.strftime('%Y%m%d')) for d in df['date']], dtype=np.int64)
+        gvkey = df['gvkey'].astype(str).to_numpy()
+        subset = conformal_subsets(date, gvkey, cal_meta[:, 0].astype(np.int64),
+                                   [g.decode('utf-8') if isinstance(g, bytes) else str(g) for g in cal_meta[:, 1]],
+                                   set(str(g) for g in pool._train_gvkeys), int(pool.config.end_date))
+        coverage_table(levels, subset, n_cal, qhat, pred.cpu().numpy(), targets, scale, lower, upper, seq_norm,
+                       unscale).to_csv(os.path.join(self.pred_dir, 'coverage.dat'), sep=' ', index=False)
 
     def _flat(self):
         """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""
@@ -395,3 +452,77 @@ def calibration_table(levels, quantiles, scores, targets):
             rows.append({'step': s + 1, 'level': level, 'frac_below': below, 'n_known': n, 'mean_crps': mean_crps,
                          'mean_nll': mean_nll, 'pit_ks': ks})
     return pd.DataFrame(rows, columns=['step', 'level', 'frac_below', 'n_known', 'mean_crps', 'mean_nll', 'pit_ks'])
+
+
+def conformal_level_name(level):
+    """A coverage level as intervals.dat names it: quantile_name without its q (0.9 -> 90, 0.125 -> 12.5)."""
+    return quantile_name(level)[1:]
+
+
+def _unscaled_bounds(lo, hi, seq_norm, unscale):
+    """The fundamentals-unit bounds of normalised bounds: unscale of each, swapped where seq_norm < 0 (where unscale
+    reverses the order), so that lower <= upper."""
+    a, b = unscale(lo), unscale(hi)
+    flip = np.asarray(seq_norm) < 0
+    return np.where(flip, b, a), np.where(flip, a, b)
+
+
+def interval_table(keys, levels, lower, upper, scale, pvalue, seq_norm, unscale):
+    """The rows of intervals.dat: `keys` (date, gvkey of preds.dat), then per forecast step s and level l (named by
+    conformal_level_name, e.g. 90) norm_lo90_s and norm_hi90_s (normalised units), lo90_s and hi90_s (the fundamentals'
+    units: unscale of the bounds, as preds_s, swapped where seq_norm < 0), then scale_s (the window's scale: 1, sigma
+    or d(x) + beta) and pvalue_s (its conformal p-value, NaN where the target is unknown).  lower / upper [S,N,Q],
+    scale and pvalue [S,N] as NativeForecaster.conformal returns them."""
+    df = keys.reset_index(drop=True).copy()
+    cols = {}
+    for s in range(len(lower)):
+        for k, level in enumerate(levels):
+            name = '%s_%d' % (conformal_level_name(level), s + 1)
+            cols['norm_lo' + name] = lower[s][:, k]
+            cols['norm_hi' + name] = upper[s][:, k]
+            cols['lo' + name], cols['hi' + name] = _unscaled_bounds(lower[s][:, k], upper[s][:, k], seq_norm, unscale)
+        cols['scale_%d' % (s + 1)] = scale[s]
+        cols['pvalue_%d' % (s + 1)] = pvalue[s]
+    return pd.concat([df, pd.DataFrame(cols)], axis=1)
+
+
+def conformal_subsets(date, gvkey, cal_date, cal_gvkey, train_gvkeys, end_date):
+    """The coverage.dat subset of every window (date yyyymmdd, gvkey): 'calibration' when (date, gvkey) is a
+    calibration window, 'training' when its company is in the training split and its date is in or before end_date
+    (YYYYMM) of the training draw, else 'out_of_sample'."""
+    cal = set(zip((int(d) for d in cal_date), (str(g) for g in cal_gvkey)))
+    out = []
+    for d, g in zip(date, gvkey):
+        if (int(d), str(g)) in cal:
+            out.append('calibration')
+        elif str(g) in train_gvkeys and int(d) // 100 <= end_date:
+            out.append('training')
+        else:
+            out.append('out_of_sample')
+    return np.asarray(out)
+
+
+def coverage_table(levels, subset, n_cal, qhat, pred, targets, scale, lower, upper, seq_norm, unscale):
+    """The rows of coverage.dat, one per forecast step, level and subset (calibration, training, out_of_sample, all):
+    n_cal and qhat of the step and level, n (the subset's windows with a known target), coverage (the share of them
+    whose score |y - pred| / scale, in float32 as the library forms it, is at most qhat: whose target lies in the
+    interval) and the mean normalised and fundamentals-unit interval widths over those n windows."""
+    rows = []
+    for s in range(len(lower)):
+        y = np.asarray(targets[s], dtype=np.float32)
+        r = np.abs(y - np.asarray(pred[s], dtype=np.float32)) / np.asarray(scale[s], dtype=np.float32)
+        known = np.isfinite(y)
+        for k, level in enumerate(levels):
+            lo, hi = np.asarray(lower[s][:, k], dtype=np.float64), np.asarray(upper[s][:, k], dtype=np.float64)
+            ulo, uhi = _unscaled_bounds(lo, hi, seq_norm, unscale)
+            for name in ('calibration', 'training', 'out_of_sample', 'all'):
+                m = known & ((subset == name) if name != 'all' else True)
+                n = int(m.sum())
+                with np.errstate(invalid='ignore'):
+                    rows.append({'step': s + 1, 'level': level, 'subset': name, 'n_cal': int(n_cal[s]),
+                                 'qhat': float(qhat[s][k]), 'n': n,
+                                 'coverage': float(np.mean(r[m] <= qhat[s][k])) if n else np.nan,
+                                 'mean_norm_width': float(np.mean(hi[m] - lo[m])) if n else np.nan,
+                                 'mean_width': float(np.mean(uhi[m] - ulo[m])) if n else np.nan})
+    return pd.DataFrame(rows, columns=['step', 'level', 'subset', 'n_cal', 'qhat', 'n', 'coverage', 'mean_norm_width',
+                                       'mean_width'])

@@ -115,7 +115,8 @@ def origin_configs(config):
         pred.train = False
         pred.start_date = add_months(origin, 1)
         pred.end_date = min(add_months(origin, config.stride), config.end_date)
-        if getattr(config, 'influence_top_k', 0) > 0:     # the origin's own training split is the attribution pool
+        if getattr(config, 'influence_top_k', 0) > 0 or getattr(config, 'conformal_levels', None) is not None:
+            # the origin's own training draw: the attribution pool, the conformal calibration set
             pred.pool_dates = (train.start_date, train.end_date)
         out.append((origin, train, pred))
     return experiment_dir, out
@@ -324,6 +325,31 @@ def run_candidates(conf_paths, npe):
     return errors
 
 
+def check_conformal(c):
+    """Refuses --conformal_levels / --conformal_knn where they cannot run, before any work."""
+    levels, knn = getattr(c, 'conformal_levels', None), getattr(c, 'conformal_knn', 0)
+    if knn != 0:
+        bad = ['conformal_knn must be in [1, 64] (0 = off)' if not 0 < knn <= 64 else None,
+               'it scales conformal intervals: set --conformal_levels' if levels is None else None,
+               'a UQ model is scaled by its own sigma' if c.UQ else None,
+               'NaivePointEstimate has no features to find neighbours in' if 'Naive' in c.nn_type else None,
+               'it needs forecast_steps = 1' if c.forecast_steps != 1 else None]
+        bad = [b for b in bad if b]
+        if bad:
+            raise ValueError('--conformal_knn %d: the normalised conformal score divides each error by the mean error '
+                             'of the K nearest training windows; %s' % (knn, '; '.join(bad)))
+    if levels is None:
+        return
+    bad = ['they are calibrated at prediction (--train=False)' if c.train else None,
+           'they calibrate one model, not an ensemble (num_procs = 1)' if getattr(c, 'num_procs', 1) > 1 else None,
+           'the calibration set is the validation split: validation_size must be > 0'
+           if not c.validation_size > 0 else None]
+    bad = [b for b in bad if b]
+    if bad:
+        raise ValueError('--conformal_levels %s: split-conformal intervals; %s' % (levels, '; '.join(bad)))
+    base_config.conformal_levels(levels)
+
+
 def check_row_weights(c):
     """The refusals of --sample_weight_field / --recency_halflife that need no data (DESIGN.md section 6d); the field's
     values are checked when the dataset loads."""
@@ -378,6 +404,7 @@ class ModelExecution(object):
                 raise ValueError('--pred_quantiles %s: predictive quantiles are those of a UQ model\'s Monte-Carlo '
                                  'dropout mixture, at prediction (--UQ=True --train=False)' % c.pred_quantiles)
             base_config.pred_quantile_levels(c.pred_quantiles)
+        check_conformal(c)
         check_row_weights(c)
         if c.training_type == 'iterative':
             check_walk_forward(c)
@@ -509,6 +536,12 @@ class ModelExecution(object):
                                              dtype={'gvkey': str}, float_precision='round_trip')
                                  for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
                 os.path.join(experiment_dir, 'walk_forward_quantiles.dat'), sep=' ', index=False)
+        if getattr(cfg, 'conformal_levels', None) is not None:      # each origin calibrated on its own draw
+            for name, key in (('intervals', 'gvkey'), ('coverage', 'subset')):
+                stitch_walk_forward([pd.read_csv(os.path.join(pred.model_dir, 'pred', name + '.dat'), sep=' ',
+                                                 dtype={key: str}, float_precision='round_trip')
+                                     for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
+                    os.path.join(experiment_dir, 'walk_forward_%s.dat' % name), sep=' ', index=False)
         _print_scaled_mse(df, cfg.forecast_steps)
         return df
 
