@@ -500,6 +500,30 @@ int32_t lfmq_conformal_apply(const float* pred, const float* y, const float* sca
                              const float* sorted, const int32_t* n_valid, const float* qhat, int32_t Nc, int32_t Q,
                              float* lower, float* upper, float* pvalue, void* work, uint64_t work_bytes,
                              void* stream);
+/* ---- lookahead factor backtests -------------------------------------------------------------------------------------
+ * DESIGN.md section 5k.  N rows, each with a date index date_idx [N] in [0, D) and a company code company [N] (device
+ * int32; no two rows share a (date, company) pair), G factor scores score [G][N] and M outcome measures measure [M][N]
+ * (device fp64; no handle, so every model, the naive forecast included, uses the one call).  For factor g and date d
+ * the universe is the rows of d with a finite score; each gets its average rank r among them (ties share the mean
+ * rank; -0 ties +0) and the bucket floor((r - 1/2) Q / n) + 1 in [1, Q], bucket Q the highest scores.  Outputs:
+ *   n [G][D]                the universe's size
+ *   bucket_n [G][D][Q]      the rows of each bucket
+ *   n_pair [G][M][D]        the rows of d where score and measure are both finite
+ *   ic [G][M][D]            Spearman's rank correlation over those rows (both re-ranked over them; NaN when
+ *                           n_pair < 3 or either rank variance is 0), from exact integer rank moments
+ *   bucket_mean [G][M][D][Q] the mean measure of each bucket's rows with a finite measure (NaN when none)
+ *   spread [G][M][D]        bucket_mean of bucket Q - bucket_mean of bucket 1
+ *   turnover [G][D]         the share of bucket Q's companies at d that were not in bucket Q at date index d - 1;
+ *                           NaN at d = 0 or when bucket Q is empty
+ * Every fp64 sum runs over a date in (score, company) order, with no atomics: permuting the rows, or calling twice,
+ * gives the same bits.  N, D >= 1, 1 <= G <= 8, 1 <= M <= 4, 2 <= Q <= 100 and null pointers: LFMQ_ERR_ARG.  The call
+ * does not synchronise with the host.  `work`: device scratch, 256-byte aligned, of the size
+ * lfmq_factor_eval_work_bytes gives. */
+int32_t lfmq_factor_eval_work_bytes(int32_t N, int32_t D, int32_t G, int32_t M, int32_t Q, uint64_t* bytes);
+int32_t lfmq_factor_eval(const int32_t* date_idx, const int32_t* company, int32_t N, int32_t D, const double* score,
+                         int32_t G, const double* measure, int32_t M, int32_t Q, int32_t* n, int32_t* bucket_n,
+                         int32_t* n_pair, double* ic, double* bucket_mean, double* spread, double* turnover, void* work,
+                         uint64_t work_bytes, void* stream);
 /* uq chain: Losses.weight_adjusted_uq_loss(y_true list, y_pred list, y_var list) (losses.py:137-178): out_dev =
  * {sum_s w_s uq_loss_s, sum_s w_s uq_loss_last_tar_s, sum_s w_s mse_s}, each stage with its own mask counts.  A
  * zero-padded step makes the uq loss NaN, as for lfmq_loss_uq.  B may exceed max_batch (validation). */

@@ -127,6 +127,10 @@ SYMBOLS = {
                                                     C.POINTER(C.c_uint64)]),
     'lfmq_conformal_apply': (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, C.c_int32, _P, _P,
                                           _P, _P, C.c_uint64, _P]),
+    'lfmq_factor_eval_work_bytes': (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                C.POINTER(C.c_uint64)]),
+    'lfmq_factor_eval': (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P, _P,
+                                      _P, _P, _P, _P, _P, C.c_uint64, _P]),
     'lfmq_chain_loss':(C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_loss_uq': (C.c_int32, [_P, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P]),
     'lfmq_chain_backward': (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P]),

@@ -174,6 +174,28 @@ int conformal_calibrate(cudaStream_t s, int S, int Nc, const float* pred, const 
 int conformal_apply(cudaStream_t s, int S, int N, int Nc, int Q, const float* pred, const float* y, const float* scale,
                     const float* sorted, const int32_t* n_valid, const float* qhat, float* lower, float* upper,
                     float* pvalue);
+// Lookahead factor backtests (factor.cu, lfmq_factor_eval).  FactorWork: the scratch the call carves (k0 / k1 / v0 / v1
+// / d0 / d1 / pos [N] sort buffers; base_row [N] the (date, company) order; seg_off [D + 1] the date segments; pred [N] each row's
+// predecessor at date index d - 1; mkey / mrow [M][N] the measures sorted within the dates; gkey / grow [N] one factor
+// sorted; bq [N] its buckets; flag [N], pcg [M][N + 1] and pcm [N + 1] pair-row counts; yr [M][N] doubled measure
+// ranks; temp of factor_temp_bytes).  FactorOut: the caller's outputs, as lfmq.h lays them out.
+constexpr int LFMQ_FACTOR_MAX_G = 8;
+constexpr int LFMQ_FACTOR_MAX_M = 4;
+constexpr int LFMQ_FACTOR_MAX_Q = 100;
+struct FactorWork {
+  uint64_t *k0, *k1, *mkey, *gkey;
+  int32_t *v0, *v1, *pos, *base_row, *seg_off, *pred, *mrow, *grow, *flag, *pcg, *pcm;
+  uint32_t *d0, *d1, *yr;
+  uint8_t* bq;
+  char* temp;
+};
+struct FactorOut {
+  int32_t *n, *bucket_n, *n_pair;
+  double *ic, *bucket_mean, *spread, *turnover;
+};
+int factor_temp_bytes(int N, int D, size_t* bytes);
+int factor_eval(cudaStream_t s, const int32_t* date, const int32_t* company, int N, int D, const double* score, int G,
+                const double* measure, int M, int Q, const FactorWork& w, size_t temp_bytes, FactorOut o);
 // The uq loss of RNNUqRangeEstimate, one stage (S = 1, w = 1) or a forecast chain: every stage's loss rows in one launch,
 // then one reduction launch.
 // pred.p[s] == nullptr: counts only, into counts.p[s].  Otherwise per stage {loss, uq0, mse0}.p[s] (each nullable) and

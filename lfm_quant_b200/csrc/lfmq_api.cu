@@ -2151,6 +2151,76 @@ int32_t lfmq_conformal_apply(const float* pred, const float* y, const float* sca
                                pvalue);
 }
 
+// ---- lookahead factor backtests (lfmq_factor_eval) ----------------------------------------------------------------
+namespace {
+int factor_check(int32_t N, int32_t D, int32_t G, int32_t M, int32_t Q, const char* fn) {
+  if (N < 1 || D < 1 || G < 1 || G > lfmq::LFMQ_FACTOR_MAX_G || M < 1 || M > lfmq::LFMQ_FACTOR_MAX_M || Q < 2 ||
+      Q > lfmq::LFMQ_FACTOR_MAX_Q) {
+    LFMQ_SET_ERR("%s: need N, D >= 1, 1 <= G <= %d, 1 <= M <= %d and 2 <= Q <= %d (got N %d, D %d, G %d, M %d, Q %d)",
+                 fn, lfmq::LFMQ_FACTOR_MAX_G, lfmq::LFMQ_FACTOR_MAX_M, lfmq::LFMQ_FACTOR_MAX_Q, N, D, G, M, Q);
+    return LFMQ_ERR_ARG;
+  }
+  return 0;
+}
+
+lfmq::FactorWork factor_layout(int32_t N, int32_t D, int32_t M, size_t temp_bytes, Carver& cv) {
+  const size_t n = (size_t)N;
+  lfmq::FactorWork w{};
+  w.k0 = cv.take<uint64_t>(n);
+  w.k1 = cv.take<uint64_t>(n);
+  w.gkey = cv.take<uint64_t>(n);
+  w.mkey = cv.take<uint64_t>(M * n);
+  w.v0 = cv.take<int32_t>(n);
+  w.v1 = cv.take<int32_t>(n);
+  w.pos = cv.take<int32_t>(n);
+  w.d0 = cv.take<uint32_t>(n);
+  w.d1 = cv.take<uint32_t>(n);
+  w.base_row = cv.take<int32_t>(n);
+  w.seg_off = cv.take<int32_t>((size_t)D + 1);
+  w.pred = cv.take<int32_t>(n);
+  w.mrow = cv.take<int32_t>(M * n);
+  w.grow = cv.take<int32_t>(n);
+  w.flag = cv.take<int32_t>(n);
+  w.pcg = cv.take<int32_t>(M * (n + 1));
+  w.pcm = cv.take<int32_t>(n + 1);
+  w.yr = cv.take<uint32_t>(M * n);
+  w.bq = cv.take<uint8_t>(n);
+  w.temp = cv.take<char>(temp_bytes);
+  return w;
+}
+}  // namespace
+
+int32_t lfmq_factor_eval_work_bytes(int32_t N, int32_t D, int32_t G, int32_t M, int32_t Q, uint64_t* bytes) {
+  const char* fn = "lfmq_factor_eval_work_bytes";
+  RUN(factor_check(N, D, G, M, Q, fn));
+  if (!bytes) {
+    LFMQ_SET_ERR("%s: bytes == NULL", fn);
+    return LFMQ_ERR_ARG;
+  }
+  size_t temp = 0;
+  RUN(lfmq::factor_temp_bytes(N, D, &temp));
+  return report_work_bytes(bytes, fn, [&](Carver& cv) { return factor_layout(N, D, M, temp, cv); });
+}
+
+int32_t lfmq_factor_eval(const int32_t* date_idx, const int32_t* company, int32_t N, int32_t D, const double* score,
+                         int32_t G, const double* measure, int32_t M, int32_t Q, int32_t* n, int32_t* bucket_n,
+                         int32_t* n_pair, double* ic, double* bucket_mean, double* spread, double* turnover, void* work,
+                         uint64_t work_bytes, void* stream) {
+  const char* fn = "lfmq_factor_eval";
+  RUN(factor_check(N, D, G, M, Q, fn));
+  if (!date_idx || !company || !score || !measure || !n || !bucket_n || !n_pair || !ic || !bucket_mean || !spread ||
+      !turnover) {
+    LFMQ_SET_ERR("%s: null pointer", fn);
+    return LFMQ_ERR_ARG;
+  }
+  size_t temp = 0;
+  RUN(lfmq::factor_temp_bytes(N, D, &temp));
+  lfmq::FactorWork w;
+  RUN(carve_work(work, work_bytes, fn, [&](Carver& cv) { return factor_layout(N, D, M, temp, cv); }, &w));
+  const lfmq::FactorOut o{n, bucket_n, n_pair, ic, bucket_mean, spread, turnover};
+  return lfmq::factor_eval((cudaStream_t)stream, date_idx, company, N, D, score, G, measure, M, Q, w, temp, o);
+}
+
 int32_t lfmq_chain_loss(const lfmq_handle* stages, int32_t n_stages, const float* const* preds, const float* const* y,
                         const float* weights, int32_t B, float* out_dev, void* stream) {
   if (!stages || n_stages < 1 || n_stages > lfmq::LFMQ_MAX_STAGES || !preds || !y || !weights || !out_dev || B <= 0) {

@@ -151,6 +151,35 @@ def conformal_apply(pred, calibration, y=None, scale=None):
     return lower, upper, pvalue
 
 
+def factor_eval(date_idx, company, score, measure, Q, owner=None):
+    """lfmq_factor_eval: the per-date quantile backtest of the factor scores score [G,N] against the measures measure
+    [M,N] (device fp64), with date_idx [N] in [0, D) and company [N] (device int32; D = date_idx.max() + 1).  Returns a
+    dict of device tensors: n [G,D], bucket_n [G,D,Q] (int32), n_pair [G,M,D] (int32), ic [G,M,D], bucket_mean
+    [G,M,D,Q], spread [G,M,D] and turnover [G,D] (fp64).  `owner` keeps the scratch."""
+    date_idx, company = date_idx.contiguous(), company.contiguous()
+    score, measure = score.contiguous(), measure.contiguous()
+    n = date_idx.shape[0]
+    G, M, Q = score.shape[0], measure.shape[0], int(Q)
+    assert score.shape == (G, n) and measure.shape == (M, n) and company.shape == (n,), (
+        tuple(score.shape), tuple(measure.shape), tuple(company.shape))
+    assert score.dtype == measure.dtype == torch.float64 and date_idx.dtype == company.dtype == torch.int32
+    D = int(date_idx.max().item()) + 1 if n else 0
+    lib = N.load()
+    dev = score.device
+    work = _scratch(owner if owner is not None else _TopkScratch(dev), 'factor', lib.lfmq_factor_eval_work_bytes,
+                    n, D, G, M, Q)
+    i32 = dict(dtype=torch.int32, device=dev)
+    f64 = dict(dtype=torch.float64, device=dev)
+    out = dict(n=torch.empty(G, D, **i32), bucket_n=torch.empty(G, D, Q, **i32), n_pair=torch.empty(G, M, D, **i32),
+               ic=torch.empty(G, M, D, **f64), bucket_mean=torch.empty(G, M, D, Q, **f64),
+               spread=torch.empty(G, M, D, **f64), turnover=torch.empty(G, D, **f64))
+    N.check(lib.lfmq_factor_eval(_ptr(date_idx), _ptr(company), n, D, _ptr(score), G, _ptr(measure), M, Q,
+                                 _ptr(out['n']), _ptr(out['bucket_n']), _ptr(out['n_pair']), _ptr(out['ic']),
+                                 _ptr(out['bucket_mean']), _ptr(out['spread']), _ptr(out['turnover']), _ptr(work),
+                                 work.numel(), _stream()))
+    return out
+
+
 class _HandleEngine(object):
     """What every native handle offers whatever its model: parameter specs and views, weights in Keras order, the
     device share, the optimizer apply, the mask count, un-scaling and profiling."""

@@ -134,6 +134,14 @@ SCHEMA = [
                                         'and pred/coverage.dat; unset = off'),
     ('conformal_knn', _INT, 0, 'Training windows whose mean absolute error scales each conformal interval (1 to 64) '
                                'of a point or linear model with forecast_steps = 1: the normalised score; 0 = off'),
+    ('factor_quantiles', _INT, 0, 'Quantile buckets (2 to 100) of a lookahead factor backtest at prediction: each '
+                                  'date\'s companies ranked by forecast yield (preds / seq_norm) and by current yield '
+                                  '(inp_t0 / seq_norm), scored against the realised yield; writes pred/factor_dates.dat '
+                                  'and pred/factor.dat (walk_forward_factor*.dat in a walk-forward run); 0 = off'),
+    ('factor_return_field', _STRING, None, 'Datafile column of each row\'s simple return over the month that ends at '
+                                           'its date: adds the measure ret, the compounded return over the '
+                                           'factor_horizon months after each forecast date; unset = off'),
+    ('factor_horizon', _INT, 1, 'Months compounded into the factor backtest\'s ret measure (>= 1)'),
     ('sample_weight_field', _STRING, None, 'Datafile column that weighs each training window in the training loss, read '
                                          'raw at the window\'s last input row (NaN counts as 0; negative or infinite '
                                          'values are refused); unset = off.  Ignored with --train=False'),

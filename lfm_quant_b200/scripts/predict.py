@@ -3,6 +3,7 @@
 column order (predict.py:113-126,148-157,174-182,214-259; SURVEY section 8b "Files")."""
 from __future__ import absolute_import, division, print_function
 
+import io
 import os
 import pathlib
 from collections import defaultdict
@@ -50,6 +51,7 @@ class Predict(object):
         dist = defaultdict(list)
         conf_levels = conformal_levels(getattr(self.config, 'conformal_levels', None))
         conf = defaultdict(list)          # the forecast and its variance that preds.dat holds, per step [B]
+        factor_inp = []                   # the normalised inp_t0 of each window when preds.dat does not hold it
         for (inp_dev, target_dev, metadata) in self._batches:
             # one target window per input window: every forecast step is compared with it (Train._step_targets)
             inp, targets = inp_dev.cpu().numpy(), [target_dev.cpu().numpy()] * self.config.forecast_steps
@@ -59,6 +61,8 @@ class Predict(object):
             if self.config.write_inp_to_out_file:
                 for i, t_step in enumerate(range(1 - self.seq_len, 1)):
                     outputs['inp_t' + str(t_step)].append(self._extract_inputs(inp, i))
+            elif self._factor_q() > 0:      # qfm's current value, not written to preds.dat
+                factor_inp.append(self._extract_inputs(inp, self.seq_len - 1))
             outputs['targets'].append(self._extract_targets(targets))
             if not self.config.UQ:      # predict.py:128-133: model.predict returns a list when forecast_steps > 1
                 preds = self.model.predict(inp_dev)
@@ -165,6 +169,8 @@ class Predict(object):
                                   np.concatenate(dist['scores'], axis=1), unscale)
         if conf_levels is not None:
             self._write_conformal(df, conf_levels, conf, windows, unscale)
+        if self._factor_q() > 0:
+            self._write_factor(df, unscale(np.vstack(factor_inp).flatten()) if factor_inp else None)
         print("Unscaled MSE normalized by Seq_Norm (%s)" % self.config.model_dir.split('/')[-1])
         print(df[[x for x in df.columns if 'unscaled' in x]].mean())
         for i in range(self.config.forecast_steps):
@@ -302,6 +308,17 @@ class Predict(object):
                                    set(str(g) for g in pool._train_gvkeys), int(pool.config.end_date))
         coverage_table(levels, subset, n_cal, qhat, pred.cpu().numpy(), targets, scale, lower, upper, seq_norm,
                        unscale).to_csv(os.path.join(self.pred_dir, 'coverage.dat'), sep=' ', index=False)
+
+    def _factor_q(self):
+        return int(getattr(self.config, 'factor_quantiles', 0))
+
+    def _write_factor(self, df, inp_t0):
+        """<model_dir>/pred/factor_dates.dat and factor.dat (--factor_quantiles Q): the lookahead factor backtest of
+        the rows of preds.dat (`df`; inp_t0 the fundamentals-unit inp_t0 when df does not hold it); factor_tables,
+        factor_dates_table and factor_summary give the layouts."""
+        per_date, summary = factor_tables(df, self.config, inp_t0)
+        per_date.to_csv(os.path.join(self.pred_dir, 'factor_dates.dat'), sep=' ', index=False)
+        summary.to_csv(os.path.join(self.pred_dir, 'factor.dat'), sep=' ', index=False)
 
     def _flat(self):
         """MLP* / Naive* batches are 2-D: targets [B, O], inputs [B, T*F] (predict.py:275-300)."""
@@ -526,3 +543,183 @@ def coverage_table(levels, subset, n_cal, qhat, pred, targets, scale, lower, upp
                                  'mean_width': float(np.mean(uhi[m] - ulo[m])) if n else np.nan})
     return pd.DataFrame(rows, columns=['step', 'level', 'subset', 'n_cal', 'qhat', 'n', 'coverage', 'mean_norm_width',
                                        'mean_width'])
+
+
+# ---- lookahead factor backtests (--factor_quantiles, DESIGN.md section 5k) ---------------------------------------------
+FACTOR_MAX_SCORES = 8       # lfmq_factor_eval's caps on the factors and the measures
+FACTOR_MAX_MEASURES = 4
+
+
+def factor_names(forecast_steps, uq):
+    """The factors of a run: lfm_s (forecast yield) per step, qfm (current yield), and on a UQ model lfm_risk_s."""
+    return (['lfm_%d' % s for s in range(1, forecast_steps + 1)] + ['qfm']
+            + (['lfm_risk_%d' % s for s in range(1, forecast_steps + 1)] if uq else []))
+
+
+def factor_scores(df, forecast_steps, uq, inp_t0=None):
+    """(names, scores [G,N] fp64) of the rows of a preds.dat frame: lfm_s = preds_s / seq_norm, qfm = inp_t0 / seq_norm
+    (inp_t0 the frame's column unless given) and, on a UQ model, lfm_risk_s = pred_var_s / seq_norm with pred_var_s =
+    preds_s / sqrt(variance_s) as ensemble_uq_estimate forms it; NaN where variance_s is not finite or not > 0."""
+    seq_norm = df['seq_norm'].to_numpy(dtype=np.float64)
+    col = lambda c: df[c].to_numpy(dtype=np.float64)        # noqa: E731
+    inp = col('inp_t0') if inp_t0 is None else np.asarray(inp_t0, dtype=np.float64)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        scores = [col('preds_%d' % s) / seq_norm for s in range(1, forecast_steps + 1)] + [inp / seq_norm]
+        if uq:
+            for s in range(1, forecast_steps + 1):
+                v = col('variance_%d' % s)
+                ok = np.isfinite(v) & (v > 0)
+                scores.append(np.where(ok, col('preds_%d' % s) / np.sqrt(np.where(ok, v, 1.0)), np.nan) / seq_norm)
+    return factor_names(forecast_steps, uq), np.stack(scores)
+
+
+def _yyyymmdd(dates):
+    """The dates of a frame column (datetime or yyyymmdd / yyyymm integers) as int64."""
+    d = pd.Series(dates)
+    if np.issubdtype(d.dtype, np.datetime64):
+        return (d.dt.year * 10000 + d.dt.month * 100 + d.dt.day).to_numpy(dtype=np.int64)
+    return d.astype(np.int64).to_numpy()
+
+
+def month_index(dates):
+    """The calendar month (12 * year + month - 1) of yyyymmdd or yyyymm integer dates."""
+    d = np.asarray(dates, dtype=np.int64)
+    ym = np.where(d >= 10 ** 7, d // 100, d)
+    return (ym // 100) * 12 + ym % 100 - 1
+
+
+def forward_returns(data, field, date, gvkey, horizon):
+    """ret of rows (date, gvkey): prod_{k=1..H} (1 + r_{c, t+k}) - 1, with r the raw column `field` of the datafile
+    frame `data` (date, gvkey, field) and t+k the company's row exactly k calendar months after the row's date; NaN
+    when any of those rows is missing or its r is not finite."""
+    months = month_index(_yyyymmdd(data['date']))
+    r = pd.Series(data[field].to_numpy(dtype=np.float64),
+                  index=pd.MultiIndex.from_arrays([data['gvkey'].astype(str).to_numpy(), months]))
+    if not r.index.is_unique:
+        raise ValueError('--factor_return_field %s: the datafile has two rows for one company in one month' % field)
+    g, t = np.asarray(gvkey).astype(str), month_index(date)
+    prod, ok = np.ones(len(g)), np.ones(len(g), dtype=bool)
+    for k in range(1, int(horizon) + 1):
+        rk = r.reindex(pd.MultiIndex.from_arrays([g, t + k])).to_numpy(dtype=np.float64)
+        ok &= np.isfinite(rk)
+        prod *= np.where(np.isfinite(rk), 1.0 + rk, 1.0)
+    return np.where(ok, prod - 1.0, np.nan)
+
+
+def factor_codes(date, gvkey):
+    """(dates [D] ascending, date_idx [N], company [N]) int codes of the rows; two rows of one (date, gvkey) raise."""
+    dates, date_idx = np.unique(np.asarray(date, dtype=np.int64), return_inverse=True)
+    _, company = np.unique(np.asarray(gvkey).astype(str), return_inverse=True)
+    pairs = date_idx.astype(np.int64) * (int(company.max()) + 1 if len(company) else 1) + company
+    if len(np.unique(pairs)) != len(pairs):
+        raise ValueError('--factor_quantiles: the frame has two rows for one (date, gvkey); a factor ranks each '
+                         'company once per date')
+    return dates, date_idx.astype(np.int32), company.astype(np.int32)
+
+
+def factor_dates_table(dates, factors, measures, out, Q):
+    """The rows of factor_dates.dat, one per (date, factor, measure) in that order: date factor measure n n_pair ic
+    q1..qQ (the bucket means, bucket Q the highest scores) spread turnover, from lfmq_factor_eval's outputs `out`
+    (NumPy arrays as engine.factor_eval names them)."""
+    D, G, M = len(dates), len(factors), len(measures)
+    d, g, m = (a.ravel() for a in np.meshgrid(np.arange(D), np.arange(G), np.arange(M), indexing='ij'))
+    cols = {'date': np.asarray(dates)[d], 'factor': np.asarray(factors)[g], 'measure': np.asarray(measures)[m],
+            'n': out['n'][g, d], 'n_pair': out['n_pair'][g, m, d], 'ic': out['ic'][g, m, d]}
+    for q in range(Q):
+        cols['q%d' % (q + 1)] = out['bucket_mean'][g, m, d, q]
+    cols['spread'] = out['spread'][g, m, d]
+    cols['turnover'] = out['turnover'][g, d]
+    return pd.DataFrame(cols)
+
+
+def newey_west_t(x, lag):
+    """x̄ / sqrt(var / n) of the finite entries of x (consecutive ones adjacent), var = γ0 + 2 Σ_{k=1..L} (1 - k/(L+1))
+    γk with Bartlett weights; NaN when n < 2 or var <= 0."""
+    x = np.asarray(x, dtype=np.float64)
+    x = x[np.isfinite(x)]
+    n = len(x)
+    if n < 2:
+        return np.nan
+    xc = x - x.mean()
+    var = xc @ xc / n
+    for k in range(1, min(int(lag), n - 1) + 1):
+        var += 2.0 * (1.0 - k / (lag + 1.0)) * (xc[k:] @ xc[:-k]) / n
+    return float(x.mean() / np.sqrt(var / n)) if var > 0 else np.nan
+
+
+def newey_west_lag(dates, horizon):
+    """L = max(0, ceil(h / spacing) - 1), spacing the smallest gap in months between consecutive dates (0 for one
+    date): overlapping h-month outcomes are correlated over L dates."""
+    months = np.unique(month_index(dates))
+    if len(months) < 2:
+        return 0
+    return max(0, int(np.ceil(horizon / float(np.diff(months).min()))) - 1)
+
+
+def _finite_stats(x):
+    """(n, mean, sd with ddof 1) of the finite entries of x (NaN where undefined)."""
+    x = np.asarray(x, dtype=np.float64)
+    x = x[np.isfinite(x)]
+    return len(x), (float(x.mean()) if len(x) else np.nan), (float(x.std(ddof=1)) if len(x) > 1 else np.nan)
+
+
+def factor_summary(dates, factors, measures, out, Q, horizons):
+    """The rows of factor.dat, one per (factor, measure): n_dates (dates with a finite ic), mean_ic, sd_ic, ir =
+    mean_ic / sd_ic, hit (share of those dates with ic > 0), t_ic, mean_q1..mean_qQ (means over dates of each bucket's
+    mean), mean_spread, sd_spread, t_spread, mean_turnover and nw_lag, the Newey-West lag of the t-statistics for the
+    measure's horizon in months (horizons [M])."""
+    rows = []
+    for g, f in enumerate(factors):
+        for m, meas in enumerate(measures):
+            lag = newey_west_lag(dates, horizons[m])
+            ic = out['ic'][g, m]
+            n, mean_ic, sd_ic = _finite_stats(ic)
+            _, mean_sp, sd_sp = _finite_stats(out['spread'][g, m])
+            row = {'factor': f, 'measure': meas, 'n_dates': n, 'mean_ic': mean_ic, 'sd_ic': sd_ic,
+                   'ir': mean_ic / sd_ic if sd_ic > 0 else np.nan,
+                   'hit': float(np.mean(ic[np.isfinite(ic)] > 0)) if n else np.nan,
+                   't_ic': newey_west_t(ic, lag)}
+            for q in range(Q):
+                row['mean_q%d' % (q + 1)] = _finite_stats(out['bucket_mean'][g, m, :, q])[1]
+            row.update({'mean_spread': mean_sp, 'sd_spread': sd_sp, 't_spread': newey_west_t(out['spread'][g, m], lag),
+                        'mean_turnover': _finite_stats(out['turnover'][g])[1], 'nw_lag': lag})
+            rows.append(row)
+    return pd.DataFrame(rows)
+
+
+def factor_measures(df, forecast_n, returns=None, horizon=1):
+    """(names, measures [M,N], horizons [M] in months): yield = targets_1 / seq_norm over forecast_n months, and with
+    `returns` (forward_returns of the rows) ret over `horizon` months."""
+    with np.errstate(divide='ignore', invalid='ignore'):
+        y = df['targets_1'].to_numpy(dtype=np.float64) / df['seq_norm'].to_numpy(dtype=np.float64)
+    if returns is None:
+        return ['yield'], y[None, :], [int(forecast_n)]
+    return ['yield', 'ret'], np.stack([y, np.asarray(returns, dtype=np.float64)]), [int(forecast_n), int(horizon)]
+
+
+def factor_tables(df, config, inp_t0=None):
+    """(factor_dates.dat, factor.dat) frames of a preds.dat frame `df` (or walk_forward_preds.dat's) for the run's
+    --factor_quantiles Q: the factors (factor_scores), the measures (factor_measures, ret read from the datafile with
+    --factor_return_field), one lfmq_factor_eval call on the GPU, and the summary on the host."""
+    import torch
+    from ..engine import factor_eval
+    Q = int(config.factor_quantiles)
+    date = _yyyymmdd(df['date'])
+    gvkey = df['gvkey'].astype(str).to_numpy()
+    # the values as preds.dat holds them: a float32 column (seq_norm) is written in its shortest decimal form, so a
+    # fixed_dates run and a walk-forward run, which reads its frame back from the files, rank the same numbers
+    cols = [c for c in df.columns if c in ('seq_norm', 'inp_t0') or c.startswith(('preds_', 'targets_', 'variance_'))]
+    df = pd.read_csv(io.StringIO(df[cols].to_csv(sep=' ', index=False)), sep=' ', float_precision='round_trip')
+    factors, score = factor_scores(df, config.forecast_steps, config.UQ, inp_t0)
+    field = getattr(config, 'factor_return_field', None)
+    returns = None
+    if field:
+        data = pd.read_csv(os.path.join(config.data_dir, config.datafile), sep=' ', usecols=['date', 'gvkey', field],
+                           dtype={'gvkey': str})
+        returns = forward_returns(data, field, date, gvkey, config.factor_horizon)
+    measures, measure, horizons = factor_measures(df, config.forecast_n, returns, config.factor_horizon)
+    dates, date_idx, company = factor_codes(date, gvkey)
+    cu = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()      # noqa: E731
+    out = {k: v.cpu().numpy() for k, v in factor_eval(cu(date_idx), cu(company), cu(score), cu(measure), Q).items()}
+    return (factor_dates_table(dates, factors, measures, out, Q),
+            factor_summary(dates, factors, measures, out, Q, horizons))

@@ -23,6 +23,7 @@ import scipy.optimize
 import scipy.stats
 
 from .. import base_config
+from ..predict import FACTOR_MAX_SCORES, factor_names, factor_tables
 
 
 def member_configs(config):
@@ -118,6 +119,9 @@ def origin_configs(config):
         if getattr(config, 'influence_top_k', 0) > 0 or getattr(config, 'conformal_levels', None) is not None:
             # the origin's own training draw: the attribution pool, the conformal calibration set
             pred.pool_dates = (train.start_date, train.end_date)
+        # an origin predicts only its stride's months: the factor backtest runs once, over the stitched frame
+        pred.factor_quantiles = 0
+        pred.factor_return_field, pred.factor_horizon = None, 1
         out.append((origin, train, pred))
     return experiment_dir, out
 
@@ -350,6 +354,44 @@ def check_conformal(c):
     base_config.conformal_levels(levels)
 
 
+def check_factor(c):
+    """Refuses --factor_quantiles / --factor_return_field / --factor_horizon where they cannot run, before any work;
+    the return field is checked against the datafile's header and values."""
+    q, field, horizon = (getattr(c, 'factor_quantiles', 0), getattr(c, 'factor_return_field', None),
+                         getattr(c, 'factor_horizon', 1))
+    if q == 0:
+        if field or horizon != 1:
+            raise ValueError('--factor_return_field / --factor_horizon: they add the ret measure to a factor '
+                             'backtest; set --factor_quantiles')
+        return
+    G = len(factor_names(c.forecast_steps, c.UQ))
+    bad = ['factor_quantiles must be in [2, 100] (0 = off)' if not 2 <= q <= 100 else None,
+           'it ranks forecasts at prediction (--train=False)' if c.train else None,
+           'it ranks the forecasts of one model, not an ensemble (num_procs = 1)'
+           if getattr(c, 'num_procs', 1) > 1 else None,
+           'forecast_steps %d gives %d factors, more than %d' % (c.forecast_steps, G, FACTOR_MAX_SCORES)
+           if G > FACTOR_MAX_SCORES else None,
+           'a walk-forward backtest reads the current yield from walk_forward_preds.dat: '
+           'set --write_inp_to_out_file=True'
+           if c.training_type == 'iterative' and not c.write_inp_to_out_file else None]
+    bad = [b for b in bad if b]
+    if bad:
+        raise ValueError('--factor_quantiles %d: a lookahead factor backtest; %s' % (q, '; '.join(bad)))
+    if horizon < 1:
+        raise ValueError('--factor_horizon %d: ret compounds the returns of the H >= 1 months after each date' % horizon)
+    if field:
+        path = os.path.join(c.data_dir, c.datafile)
+        header = pd.read_csv(path, sep=' ', nrows=0).columns
+        numeric = field in header and field not in ('date', 'gvkey')
+        if numeric:
+            try:
+                pd.to_numeric(pd.read_csv(path, sep=' ', usecols=[field])[field], errors='raise')
+            except (ValueError, TypeError):
+                numeric = False
+        if not numeric:
+            raise ValueError('--factor_return_field %s: not a numeric column of %s' % (field, c.datafile))
+
+
 def check_row_weights(c):
     """The refusals of --sample_weight_field / --recency_halflife that need no data (DESIGN.md section 6d); the field's
     values are checked when the dataset loads."""
@@ -405,6 +447,7 @@ class ModelExecution(object):
                                  'dropout mixture, at prediction (--UQ=True --train=False)' % c.pred_quantiles)
             base_config.pred_quantile_levels(c.pred_quantiles)
         check_conformal(c)
+        check_factor(c)
         check_row_weights(c)
         if c.training_type == 'iterative':
             check_walk_forward(c)
@@ -542,6 +585,10 @@ class ModelExecution(object):
                                                  dtype={key: str}, float_precision='round_trip')
                                      for _, _, pred in origins], [origin for origin, _, _ in origins]).to_csv(
                     os.path.join(experiment_dir, 'walk_forward_%s.dat' % name), sep=' ', index=False)
+        if getattr(cfg, 'factor_quantiles', 0) > 0:       # the out-of-sample backtest over every origin's months
+            per_date, summary = factor_tables(df, cfg)
+            per_date.to_csv(os.path.join(experiment_dir, 'walk_forward_factor_dates.dat'), sep=' ', index=False)
+            summary.to_csv(os.path.join(experiment_dir, 'walk_forward_factor.dat'), sep=' ', index=False)
         _print_scaled_mse(df, cfg.forecast_steps)
         return df
 
